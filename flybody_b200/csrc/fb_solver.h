@@ -28,7 +28,6 @@ enum { W_LAM = 0, W_JAR, W_F, W_R, W_U, W_DL, W_ADL, W_P, X_E0, X_E1, X_XQ, X_OU
        S_D, S_B, S_R, S_TYPE /* 0 plain, 1 elliptic head, 2 elliptic tail */, S_MU, S_F1, S_F2, S_LA, S_LB,
        S_STATE, S_COLIDX, S_ECROW, S_ECKIND, S_NSLOT };
 #define TRI(r, c) ((r) * ((r) + 1) / 2 + (c))
-#define FB_SOLVE_WARP_FLOATS (S_NSLOT * FB_SOLVE_NCAP + 2 * TRI(FB_SOLVE_NCAP, 0) + 4 * 32)
 
 // memory of one env's problem: base pointers + element strides (1 in shared memory, Np in global memory)
 struct SolveMem { float* v; float* A; float* G; float* red; int cap; };

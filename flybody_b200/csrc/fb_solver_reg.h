@@ -4,8 +4,9 @@
 // force gather); what changes is where the data lives.  Lane r owns row r: its constants (D, b, R, friction), its
 // work values (lam, jar, f, residual, search direction ...) are registers; vectors are "read" with warp shuffles.
 // Shared memory only holds what is indexed irregularly: the Delassus matrix A as a full 32 x 33 array (row stride 33:
-// lane r reading A[r][j] for a common j is bank-conflict free), the small Hessian block G with its right-hand sides,
-// and mirrors of E / u for the Hessian assembly.  Matrix-vector products cost one shuffle, one shared load and one FMA
+// lane r reading A[r][j] for a common j is bank-conflict free), the Hessian block G (up to FB_CHOL_REG columns: larger
+// blocks are rare and are assembled and factorised in the env's record, efc_G) with its right-hand sides, and mirrors of
+// E / u for the Hessian assembly.  Matrix-vector products cost one shuffle, one shared load and one FMA
 // per element instead of a packed-index computation and two shared loads.
 //
 // Host emulation (-DFB_EMU): a lane register is an array over the 32 lanes and a shuffle is an indexed read.  WPAR
@@ -19,6 +20,9 @@
 #ifndef FB_CHOL_REG
 #define FB_CHOL_REG 24                           // Hessian blocks up to this size are factorised in registers (steady-state walk: 8 - 23 columns)
 #endif
+// one warp's slice: A, G of up to FB_CHOL_REG columns, P XQ XO E0s E1s Us ECR ECK.  6448 bytes: 4 warps + the 1 KB the system
+// reserves per CTA fit 8 CTAs on an sm_90 SM (228 KB; tests/test_smem_budget.py)
+#define FB_SOLVE_WARP_FLOATS (32 * 33 + TRI(FB_CHOL_REG, 0) + 8 * 32)
 #ifdef __CUDACC__
 #define FB_RSQRT(x) rsqrtf(x)
 #else
@@ -71,6 +75,27 @@ FB_DEV void reg_head_ls(int kind, float alpha, float jar, float jv, float ja1, f
   }
 }
 
+// p = E^T u ; G = I + E^T A E (packed lower triangle, nc columns) -- one lane's share
+FB_DEV void reg_assemble(const float* A, const float* E0s, const float* E1s, const float* Us, const int* ECR, const int* ECK,
+                         float* P, float* G, int nc, int lane) {
+  NOUNROLL for (int p = lane; p < nc; p += 32) {
+    int rp = ECR[p], kd = ECK[p], np = kd == 0 ? 1 : 3; const float* Ep = kd == 2 ? E1s : E0s;
+    float pv = 0; NOUNROLL for (int a = 0; a < np; a++) pv += Ep[rp + a] * Us[rp + a];
+    P[p] = pv;
+  }
+  const int npairs = nc * (nc + 1) / 2;
+  NOUNROLL for (int t = lane; t < npairs; t += 32) {
+    int p = (int)((sqrtf(8.0f * t + 1.0f) - 1.0f) * 0.5f);
+    while ((p + 1) * (p + 2) / 2 <= t) p++;
+    while (p * (p + 1) / 2 > t) p--;
+    int q = t - p * (p + 1) / 2;
+    int rp = ECR[p], np = ECK[p] == 0 ? 1 : 3, rq = ECR[q], nq = ECK[q] == 0 ? 1 : 3;
+    const float* Ep = ECK[p] == 2 ? E1s : E0s; const float* Eq = ECK[q] == 2 ? E1s : E0s;
+    float s = (p == q) ? 1.0f : 0.0f;
+    NOUNROLL for (int a = 0; a < np; a++) { float va = Ep[rp + a]; if (va == 0.0f) continue; NOUNROLL for (int bb = 0; bb < nq; bb++) s += va * A_(rp + a, rq + bb) * Eq[rq + bb]; }
+    GP(p, q) = s;
+  }
+}
 // out = sum_j A[lane][j] * x[j]   (x: lane register written in an earlier section)
 #define REG_MATVEC(out, xname) { float s_ = 0; _Pragma("unroll 4") for (int j = 0; j < n; j++) s_ += A_(lane, j) * SHF(xname, j); out = lane < n ? s_ : 0.0f; }
 // evaluate the rows headed by this lane from the current jar; tails take their values from the head (lanes -1 / -2)
@@ -89,10 +114,13 @@ FB_DEV void reg_head_ls(int kind, float alpha, float jar, float jv, float ja1, f
 
 FB_WARPFN void ksolve_reg(const DevModel& m, const DevData& d, float* wsm, int e, int n) {
   const float scale = 1.0f / (m.meaninertia * (m.nv > 1 ? m.nv : 1));
-  float* A = wsm; float* G = A + 32 * 33; float* P = G + TRI(32, 0); float* XQ = P + 32; float* XO = XQ + 32;
+  float* A = wsm; float* G = A + 32 * 33; float* P = G + TRI(FB_CHOL_REG, 0); float* XQ = P + 32; float* XO = XQ + 32;
   float* E0s = XO + 32; float* E1s = E0s + 32; float* Us = E1s + 32;
   int* ECR = reinterpret_cast<int*>(Us + 32); int* ECK = ECR + 32;
-  [[maybe_unused]] SolveMem sm; sm.v = nullptr; sm.A = nullptr; sm.G = nullptr; sm.cap = 32; sm.red = reinterpret_cast<float*>(ECK + 32);     // WSUM staging (host emulation)
+  [[maybe_unused]] SolveMem sm; sm.v = nullptr; sm.A = nullptr; sm.G = nullptr; sm.cap = 32; sm.red = nullptr;
+#ifndef __CUDACC__
+  float red_[4 * 32]; sm.red = red_;                // WSUM staging of the host emulation (warp shuffles on the GPU)
+#endif
   float tot[4] = {0, 0, 0, 0}; (void)tot;
   LREG(float, D); LREG(float, D1); LREG(float, D2); LREG(float, b); LREG(float, Rr); LREG(float, mu); LREG(float, c1); LREG(float, c2);
   LREG(float, lam); LREG(float, jar); LREG(float, f); LREG(float, res); LREG(float, dl); LREG(float, adl); LREG(float, e0); LREG(float, e1);
@@ -157,29 +185,11 @@ FB_WARPFN void ksolve_reg(const DevModel& m, const DevData& d, float* wsm, int e
           if (L(state) == 1) { ECR[c0] = lane; ECK[c0] = 0; }
           else if (L(state) == 2) { ECR[c0] = lane; ECK[c0] = 1; ECR[c0 + 1] = lane; ECK[c0 + 1] = 2; } } WPAR_END
       WPAR_BEGIN { int c1_ = SHF(colx, lane - 1), c2_ = SHF(colx, lane - 2); if (L(state) == 3) L(colx) = (L(kind) == 2) ? c1_ : c2_; } WPAR_END
-      // u = A r ; p = E^T u ; G = I + E^T A E (packed lower triangle)
+      // u = A r, then p and G (reg_assemble)
       WPAR_BEGIN { float s; REG_MATVEC(s, res) Us[lane] = s; } WPAR_END
-      WPAR_BEGIN
-        NOUNROLL for (int p = lane; p < nc; p += 32) {
-          int rp = ECR[p], kd = ECK[p], np = kd == 0 ? 1 : 3; const float* Ep = kd == 2 ? E1s : E0s;
-          float pv = 0; NOUNROLL for (int a = 0; a < np; a++) pv += Ep[rp + a] * Us[rp + a];
-          P[p] = pv;
-        }
-        const int npairs = nc * (nc + 1) / 2;
-        NOUNROLL for (int t = lane; t < npairs; t += 32) {
-          int p = (int)((sqrtf(8.0f * t + 1.0f) - 1.0f) * 0.5f);
-          while ((p + 1) * (p + 2) / 2 <= t) p++;
-          while (p * (p + 1) / 2 > t) p--;
-          int q = t - p * (p + 1) / 2;
-          int rp = ECR[p], np = ECK[p] == 0 ? 1 : 3, rq = ECR[q], nq = ECK[q] == 0 ? 1 : 3;
-          const float* Ep = ECK[p] == 2 ? E1s : E0s; const float* Eq = ECK[q] == 2 ? E1s : E0s;
-          float s = (p == q) ? 1.0f : 0.0f;
-          NOUNROLL for (int a = 0; a < np; a++) { float va = Ep[rp + a]; if (va == 0.0f) continue; NOUNROLL for (int bb = 0; bb < nq; bb++) s += va * A_(rp + a, rq + bb) * Eq[rq + bb]; }
-          GP(p, q) = s;
-        }
-      WPAR_END
 #if FB_CHOL_REG > 0
       if (nc <= FB_CHOL_REG) {
+        WPAR_BEGIN reg_assemble(A, E0s, E1s, Us, ECR, ECK, P, G, nc, lane); WPAR_END
         // Cholesky G = L L^T with ROW i OF G / L IN THE REGISTERS OF LANE i (right-looking: after step j every lane has subtracted
         // column j's outer product from its row; L[k][j] travels by shuffle).  Register indices must be static, so the row lives
         // in slots that shift by one per step (below).  The forward substitution L y = p rides along (y in a lane register); L is
@@ -224,21 +234,23 @@ FB_WARPFN void ksolve_reg(const DevModel& m, const DevData& d, float* wsm, int e
       } else
 #endif
       {
-        // larger blocks: column by column in shared memory (two warp barriers per column); the forward substitution L y = p
-        // rides along on lane 0
+        // larger blocks (rare, see FB_CHOL_REG) in the env's record, which keeps the shared slice at the size of the register
+        // form's G: column by column (two warp barriers per column); the forward substitution L y = p rides along on lane 0
+        float* Gr = &AT(d.efc_G, 0);
+        WPAR_BEGIN reg_assemble(A, E0s, E1s, Us, ECR, ECK, P, Gr, nc, lane); WPAR_END
         NOUNROLL for (int j = 0; j < nc; j++) {
           WPAR_BEGIN NOUNROLL for (int i = j + lane; i < nc; i += 32) {
-              float t = GP(i, j); NOUNROLL for (int k = 0; k < j; k++) t -= GP(i, k) * GP(j, k);
-              GP(i, j) = (i == j) ? sqrtf(fmaxf(t, 1e-12f)) : t; }
+              float t = Gr[TRI(i, j)]; NOUNROLL for (int k = 0; k < j; k++) t -= Gr[TRI(i, k)] * Gr[TRI(j, k)];
+              Gr[TRI(i, j)] = (i == j) ? sqrtf(fmaxf(t, 1e-12f)) : t; }
           WPAR_END
-          WPAR_BEGIN const float dg = GP(j, j);
-            NOUNROLL for (int i = j + 1 + lane; i < nc; i += 32) GP(i, j) = GP(i, j) / dg;
-            if (lane == 0) { float yv = P[j]; NOUNROLL for (int k = 0; k < j; k++) yv -= GP(j, k) * XQ[k]; XQ[j] = yv / dg; }
+          WPAR_BEGIN const float dg = Gr[TRI(j, j)];
+            NOUNROLL for (int i = j + 1 + lane; i < nc; i += 32) Gr[TRI(i, j)] = Gr[TRI(i, j)] / dg;
+            if (lane == 0) { float yv = P[j]; NOUNROLL for (int k = 0; k < j; k++) yv -= Gr[TRI(j, k)] * XQ[k]; XQ[j] = yv / dg; }
           WPAR_END
         }
         NOUNROLL for (int j = nc - 1; j >= 0; j--) {     // backward: L^T out = y
-          WPAR_BEGIN float xj = XQ[j] / GP(j, j);
-            NOUNROLL for (int i = lane; i < j; i += 32) XQ[i] -= GP(j, i) * xj;
+          WPAR_BEGIN float xj = XQ[j] / Gr[TRI(j, j)];
+            NOUNROLL for (int i = lane; i < j; i += 32) XQ[i] -= Gr[TRI(j, i)] * xj;
             if (lane == 0) XO[j] = xj;
           WPAR_END
         }

@@ -11,13 +11,17 @@
 
 // Shared memory of one warp (= one env) in the tree kernels.  Fixed part: one float per lane for small reductions.
 // Dynamic part (sized per launch), in this order where present:
-//   PART  [FB_NY][FB_PARTK]  per-list partial sums towards the root (crb: 10, factor: 21, rne: 12)   -- pos, vel
+//   PART  [FB_PARTR][FB_PARTK]  partial sums towards the root: per branch list (crb: 10, rne: 12, packed), or the
+//                            factorisation's root-block partials (21) of FB_PARTR lanes at a time              -- pos, vel
 //   LS    [nM]               the joint-space inertia / its factor                                     -- pos
 //   XS    [nv + FB_ROOTD*nlist], LDS [nM]   right-hand side and staged factor of the triangular solves -- smooth, finish
 struct ShTree { float red[FB_NY][FB_LANES]; const unsigned* prog; const unsigned* pad_; };   // prog: the CTA's copy of the sweep program (smooth / finish kernels)
 #define FB_PARTK 21
-#define FB_PARTF (FB_NY * FB_PARTK * FB_LANES)
+#define FB_PARTR 8             // 8 rows instead of one per lane: the position kernel's CTA then fits 8 per SM (and the larger L1 carveout)
+#define FB_PARTF (FB_PARTR * FB_PARTK * FB_LANES)
 #define PART(yy, k) part_[((yy) * FB_PARTK + (k)) * FB_LANES + lane]
+#define PARTL(l, k, K) part_[((l) * (K) + (k)) * FB_LANES + lane]     // K entries per branch list l
+static_assert(FB_NLMAX * 12 <= FB_PARTR * FB_PARTK, "the per-list partial sums must fit PART");
 
 // dynamic shared memory that follows the fixed struct (per-kernel scratch: the L^T D L rows during the
 // factorisation, the right-hand side during tree solves), laid out [entry][lane]
@@ -161,14 +165,14 @@ FB_DEV void kpos_p2(FB_PHASE_ARGS) {
     else { for (int k = 0; k < 10; k++) carry[k] = cur[k]; carry_to = p; }
   }
   if (carry_to >= 0) for (int k = 0; k < 10; k++) CRBS(carry_to, k) += carry[k];
-  for (int k = 0; k < 10; k++) PART(y, k) = acc[k];
+  for (int k = 0; k < 10; k++) PARTL(y, k, 10) = acc[k];
 }
 FB_DEV void kpos_p3(FB_PHASE_ARGS) {       // composite inertia of the root bodies: lanes over (root, component)
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF;
   for (int t = y; t < 10 * m.nroot; t += FB_NY) {
     int r = t / 10, k = t - 10 * r, b = m.root_body[r];
     float s = CRBS(b, k);
-    for (int l = 0; l < m.nlist; l++) if (m.list_root[l] == r) s += PART(l, k);
+    for (int l = 0; l < m.nlist; l++) if (m.list_root[l] == r) s += PARTL(l, k, 10);
     CRBS(b, k) = s;
   }
 }
@@ -261,9 +265,8 @@ FB_DEV void factor_step_sched(const DevModel& m, const DevData& d, ShTree& sh, i
 // Root blocks.  Once the lists are eliminated, row k of a non-root dof holds its final (unscaled) coupling r_k to the
 // root's dofs and D_k; the Schur update of the root block is sum_k r_k r_k^T / D_k.  32 lanes split the dofs, each
 // accumulates the 21 packed lower-triangle entries in registers ...
-FB_DEV void factor_root_accum(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, int r) {
-  float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF;
-  float acc[21];
+FB_DEV void factor_root_accum(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, int r, float acc[21]) {
+  float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF; (void)part_;
 #pragma unroll
   for (int j = 0; j < 21; j++) acc[j] = 0;
   for (int k = y; k < m.nv; k += FB_NY) {
@@ -279,19 +282,28 @@ FB_DEV void factor_root_accum(const DevModel& m, const DevData& d, ShTree& sh, i
       for (int j = 0; j <= i; j++) acc[i * (i + 1) / 2 + (i - j)] += a * rr[j];                   // row i, (i-j)-th ancestor
     }
   }
-#pragma unroll
-  for (int j = 0; j < 21; j++) PART(y, j) = acc[j];
 }
-// ... 21 lanes add the partials up (one packed entry each) ...
-FB_DEV void factor_root_gather(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, int r) {
+// ... 21 lanes add the partials up (one packed entry each), in lane order: lanes y0 .. y0 + FB_PARTR - 1 put theirs into PART,
+// then the summing lanes add them on; a sum over all 32 lanes takes FB_NY / FB_PARTR such rounds ...
+FB_DEV void factor_root_put(ShTree& sh, int lane, int y, int y0, const float acc[21]) {
+  float* part_ = sh_dyn(sh);
+  if (y < y0 || y >= y0 + FB_PARTR) return;
+#pragma unroll
+  for (int j = 0; j < 21; j++) PART(y - y0, j) = acc[j];
+}
+FB_DEV void factor_root_sum(ShTree& sh, int lane, int y, float& acc) {
+  float* part_ = sh_dyn(sh);
+  if (y >= 21) return;
+#pragma unroll
+  for (int l = 0; l < FB_PARTR; l++) acc += PART(l, y);
+}
+FB_DEV void factor_root_gather(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, int r, float acc) {
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF;
   if (y >= 21) return;
   int il = 0; while ((il + 1) * (il + 2) / 2 <= y) il++;
   int s = y - il * (il + 1) / 2;
   int b = m.root_body[r], nd = m.body_dofnum[b], d0 = m.body_dofadr[b];
   if (il >= nd) return;
-  float acc = 0;
-  for (int l = 0; l < FB_NY; l++) acc += PART(l, y);
   LS(m.dof_Madr[d0 + il] + s) -= acc;
 }
 // ... then one lane per root body factors its dense (<= 6x6) block
@@ -328,8 +340,19 @@ FB_WARPFN void kpos_factor(const DevModel& m, const DevData& d, ShTree& sh, int 
 #endif
   for (int r = 0; r < m.nroot; r++) {
     if (!m.root_haslists[r]) continue;
-    WPAR_BEGIN factor_root_accum(m, d, sh, e, 0, lane, r); WPAR_END
-    WPAR_BEGIN factor_root_gather(m, d, sh, e, 0, lane, r); WPAR_END
+    LREGA(float, acc, 21); LREG(float, tot);
+    WPAR_BEGIN { float a[21]; factor_root_accum(m, d, sh, e, 0, lane, r, a);
+#pragma unroll
+      for (int j = 0; j < 21; j++) LA(acc, j) = a[j];
+      L(tot) = 0.0f; } WPAR_END
+    for (int y0 = 0; y0 < FB_NY; y0 += FB_PARTR) {
+      WPAR_BEGIN { float a[21];
+#pragma unroll
+        for (int j = 0; j < 21; j++) a[j] = LA(acc, j);
+        factor_root_put(sh, 0, lane, y0, a); } WPAR_END
+      WPAR_BEGIN factor_root_sum(sh, 0, lane, L(tot)); WPAR_END
+    }
+    WPAR_BEGIN factor_root_gather(m, d, sh, e, 0, lane, r, L(tot)); WPAR_END
   }
   WPAR_BEGIN factor_root(m, d, sh, e, 0, lane); WPAR_END
 }
@@ -708,7 +731,7 @@ FB_DEV void kvel_p2(FB_PHASE_ARGS) {
     else { for (int k = 0; k < 12; k++) carry[k] = cur[k]; carry_to = p; }
   }
   if (carry_to >= 0) { add6v(d.bfrc, carry_to, d, e, carry); add6v(d.bfl, carry_to, d, e, carry + 6); }
-  for (int k = 0; k < 12; k++) PART(y, k) = acc[k];
+  for (int k = 0; k < 12; k++) PARTL(y, k, 12) = acc[k];
 }
 FB_DEV void sensors_vel(const DevModel& m, const DevData& d, int e, int y);
 FB_DEV void kvel_p3(FB_PHASE_ARGS) {
@@ -716,7 +739,7 @@ FB_DEV void kvel_p3(FB_PHASE_ARGS) {
   for (int t = y; t < 12 * m.nroot; t += FB_NY) {      // lanes over (root, component): the lists' partial sums onto the root bodies
     const int r = t / 12, k = t - 12 * r, b = m.root_body[r];
     float a = 0;
-    for (int l = 0; l < m.nlist; l++) if (m.list_root[l] == r) a += PART(l, k);
+    for (int l = 0; l < m.nlist; l++) if (m.list_root[l] == r) a += PARTL(l, k, 12);
     if (k < 6) AT(d.bfrc, S6I(b, k)) += a; else AT(d.bfl, S6I(b, k - 6)) += a;
   }
   sensors_vel(m, d, e, y);

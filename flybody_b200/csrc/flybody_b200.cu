@@ -235,9 +235,11 @@ static void fb_launch(FbSim* s, int kind, size_t dyn_floats = 0, int nwarps = -1
   s->launches++;
 }
 static void fb_launch_warp(FbSim* s, int kind) {
-  (void)kind;
-  static std::vector<float> buf(FB_SOLVE_WARP_FLOATS);
-  for (int e = s->cur_e0; e < s->cur_e0 + s->cur_n; e++) ksolve_warp(s->m, s->d, buf.data(), e);
+  const size_t used = sizeof(float) * FB_SOLVE_WARP_FLOATS;      // as fb_launch: the slice as the GPU launch sizes it, then a canary
+  std::vector<unsigned char> buf(used + 256, 0);
+  memset(buf.data() + used, 0xAB, 256);
+  for (int e = s->cur_e0; e < s->cur_e0 + s->cur_n; e++) ksolve_warp(s->m, s->d, reinterpret_cast<float*>(buf.data()), e);
+  for (size_t i = 0; i < 256; i++) if (buf[used + i] != 0xAB) { fprintf(stderr, "fb_emu: shared-memory slice overrun in a kernel of kind %d (slice %zu bytes)\n", kind, used); abort(); }
   s->launches++;
 }
 #endif
@@ -1220,6 +1222,47 @@ int fb_profile_read(FbHandle s, double* ms, long long* counts, int n) {
   return K_NKIND;
 }
 const char* fb_profile_name(int kind) { return (kind >= 0 && kind < K_NKIND) ? kKindNames[kind] : ""; }
+
+// dynamic shared memory per CTA of the step kernel `kind` exactly as launch_step1 / launch_step2 request it (0: not a step kernel)
+static size_t step_kernel_bytes(const FbSim* s, int kind) {
+  const size_t blob = s->blob_in_smem ? (size_t)s->m.ts_blob_words * 4 : 0;
+  switch (kind) {
+    case K_SMOOTH: case K_FINISH: return slice_bytes(sizeof(ShTree), dyn_tsolve(s->m)) * FB_WPB + blob;
+    case K_SOLVE: return sizeof(float) * FB_SOLVE_WARP_FLOATS * FB_SOLVE_WPB;
+    case K_POS: return slice_bytes(sizeof(ShTree), dyn_pos(s->m)) * FB_WPB;
+    case K_COL: return slice_bytes(sizeof(ShCol), dyn_col(s->m)) * FB_WPB;
+    case K_PROJ: return slice_bytes(sizeof(ShCon), dyn_proj(s->m)) * FB_WPB;
+    case K_VEL: return slice_bytes(sizeof(ShTree), dyn_vel(s->m)) * FB_WPB;
+    default: return 0;
+  }
+}
+#ifndef FB_EMU
+static const void* step_kernel_fn(int kind) {
+  switch (kind) {
+    case K_SMOOTH: return (const void*)fb_run<ShTree, FB_ST_SMOOTH>;
+    case K_SOLVE: return (const void*)fb_run_solve;
+    case K_FINISH: return (const void*)fb_run<ShTree, FB_ST_FINISH>;
+    case K_POS: return (const void*)fb_run<ShTree, FB_ST_POS>;
+    case K_COL: return (const void*)fb_run<ShCol, FB_ST_COL>;
+    case K_PROJ: return (const void*)fb_run<ShCon, FB_ST_PROJ>;
+    case K_VEL: return (const void*)fb_run<ShTree, FB_ST_VEL>;
+    default: return nullptr;
+  }
+}
+#endif
+int fb_step_kernel_smem(FbHandle s, int kind, int* bytes_per_cta, int* blocks_per_sm) {
+  if (!s || !bytes_per_cta || !blocks_per_sm) return -1;
+  const size_t bytes = (kind >= 0 && kind < K_NKIND) ? step_kernel_bytes(s, kind) : 0;
+  if (bytes == 0) return -1;
+  *bytes_per_cta = (int)bytes; *blocks_per_sm = 0;
+#ifndef FB_EMU
+  int nb = 0;
+  FB_CUDA_OK(cudaSetDevice(s->device));
+  FB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, step_kernel_fn(kind), 32 * FB_WPB, bytes));
+  *blocks_per_sm = nb;
+#endif
+  return 0;
+}
 
 int fb_obs_program(FbHandle s, const FbObsProgram* p) {
   if (!s || !p || p->n_items <= 0) return -1;

@@ -22,7 +22,7 @@ MAXCON, MAXEFC = 64, 160
 
 EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_step', 'fb_forward',
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
-           'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version']
+           'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version']
 
 
 # enum FbObsItem
@@ -116,6 +116,7 @@ def load_library(path=None):
     lib.fb_profile_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     lib.fb_profile_name.argtypes = [C.c_int]
     lib.fb_profile_name.restype = C.c_char_p
+    lib.fb_step_kernel_smem.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.fb_n_envs.argtypes = [C.c_void_p]
     lib.fb_n_envs_padded.argtypes = [C.c_void_p]
     lib.fb_stream.argtypes = [C.c_void_p]
@@ -409,6 +410,18 @@ class BatchedStepper:
         cnt = np.zeros(16, np.int64)
         n = self._lib.fb_profile_read(self._h, ms.ctypes.data, cnt.ctypes.data, 16)
         return {self._lib.fb_profile_name(k).decode(): (float(ms[k]), int(cnt[k])) for k in range(n)}
+
+    def step_kernel_smem(self):
+        """{stage name: (dynamic shared bytes per CTA as launched, resident CTAs per SM at that size)} of the seven step
+        kernels (fb_step_kernel_smem; the CTA count is 0 in a build without a device)."""
+        out, nb, blocks = {}, C.c_int(), C.c_int()
+        for k in range(16):
+            rc = self._lib.fb_step_kernel_smem(self._h, k, C.byref(nb), C.byref(blocks))
+            if rc == 0:
+                out[self._lib.fb_profile_name(k).decode()] = (nb.value, blocks.value)
+            elif rc != -1:
+                self._check(rc, 'fb_step_kernel_smem')
+        return out
 
     def set_control_device(self, dev_ptr):
         """ctrl already resident on the device as contiguous rows [n_envs][nu] fp32."""

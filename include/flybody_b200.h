@@ -386,6 +386,12 @@ float fb_last_step_ms(FbHandle h);
 int fb_profile(FbHandle h, int enable);
 int fb_profile_read(FbHandle h, double* ms, long long* counts, int n);
 const char* fb_profile_name(int kind);
+/* Shared-memory budget of the seven step kernels (kinds smooth, solve, finish, pos, col, proj, vel of fb_profile_name): the
+ * dynamic shared memory one CTA of 4 warps requests when this handle launches it, and the CTAs of that kernel that fit on one
+ * SM of the handle's device at that size (cudaOccupancyMaxActiveBlocksPerMultiprocessor; 0 in a build without a device).
+ * The kernels are compiled for 8 resident CTAs per SM, which puts 4096 envs in one wave on an H100.
+ * Returns -1 for a kind that is not a step kernel.                                                                      */
+int fb_step_kernel_smem(FbHandle h, int kind, int* bytes_per_cta, int* blocks_per_sm);
 int fb_set_solver(FbHandle h, float tolerance, int max_iter);
 const char* fb_last_error(FbHandle h);
 const char* fb_version(void);
