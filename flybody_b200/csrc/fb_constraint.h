@@ -1181,7 +1181,8 @@ FB_DEV void ktaskobs(const DevModel& m, const DevData& d, int e, int y) {
 //   ktask_reset  : composer auto-reset of envs whose last step was LAST -> initialize_episode (walk_imitation.py:112-136,
 //                  flight_imitation.py:113-144): template state, root / ghost on the first reference row, wings on the beat
 //                  pattern at a random phase (flight), optional U(-a, a) noise on listed joints; the env is held (not
-//                  integrated) through the coming step, exactly as fb_reset_hold does for the host-side task code
+//                  integrated) through the coming step, exactly as fb_reset_hold does for the host-side task code; flight with
+//                  a dataset (ref_bank): the env's own reference cut from the trajectory bank first (ktask_reset_ref)
 //   ktask_before : before_step (walk_imitation.py:138-150, flight_imitation.py:146-168): ghost root pose / velocity from
 //                  the reference row of the current step; flight: one step of the wing-beat pattern generator at the requested
 //                  frequency, wing force commands += pattern angle - wing angle (pattern_generators.py:131-203)
@@ -1238,6 +1239,45 @@ FB_DEV void ktask_reset_vision(const DevModel& m, const DevData& d, const DevTas
   AT(d.time, 0) = 0; AT(d.flags, 0) = 0; AT(d.hold, 0) = 1; AT(d.prev_n, 0) = 0;
   t.step[e] = 0;          // (has_uniform is read by every lane above: ktask_commit clears it)
 }
+// kind 1 with ref_bank (flight_imitation with a dataset, flight_imitation.py:88-111, trajectory_loaders.py:109-121): the episode's
+// trajectory and start step -- the pin of fb_task_ref_pick, else the counter hash (draw indices 256, 257: past the wing-beat phase's 0
+// and the noise joints' 1 + i).  Every lane computes the same pick.
+FB_DEV void tk_ref_pick(const DevTask& t, int e, int episode, int& traj, int& start) {
+  const int* pin = t.pin + 3 * (size_t)e;
+  if (pin[0]) { traj = pin[1]; start = pin[2]; return; }
+  int k = (int)floorf(tk_u01(t, e, episode, 256) * (float)t.n_pick); k = k > t.n_pick - 1 ? t.n_pick - 1 : k;
+  traj = t.pick_traj[k];
+  const int span = t.traj_len[traj] - t.start_margin;
+  start = 0;
+  if (t.randomize_start) { start = (int)floorf(tk_u01(t, e, episode, 257) * (float)span); start = start > span - 1 ? span - 1 : start; }
+}
+// the env's reference of the new episode: rows start .. start + n of its trajectory into its slot, root x, y relative to the CoM x, y of
+// row `start`, the rest of the slot padded with the last row (as the host-side code fills a slot); root and ghost on row `start`, read
+// from the bank because the other lanes are still writing the slot
+FB_DEV void ktask_reset_ref(const DevModel& m, const DevData& d, const DevTask& t, int e, int y, int episode) {
+  int traj, start; tk_ref_pick(t, e, episode, traj, start);
+  const int len = t.traj_len[traj], row0 = t.traj_off[traj] + start;
+  const int n = len - start < t.slot_len ? len - start : t.slot_len;
+  const float* b0 = t.rbank + (size_t)FB_RBANK_W * row0;
+  const float cx = b0[13], cy = b0[14];
+  float* slot = t.slots + (size_t)e * 7 * t.slot_len;
+  for (int i = y; i < t.slot_len; i += FB_NY) {
+    const float* r = t.rbank + (size_t)FB_RBANK_W * (row0 + (i < n ? i : n - 1));
+    float* o = slot + 7 * (size_t)i;
+    o[0] = r[0] - cx; o[1] = r[1] - cy;
+    for (int c = 2; c < 7; c++) o[c] = r[c];
+  }
+  if (y < 7) {
+    const float r = y == 0 ? b0[0] - cx : (y == 1 ? b0[1] - cy : b0[y]);
+    AT(d.qpos, t.root_qadr + y) = r;
+    if (t.ghost_qadr >= 0) AT(d.qpos, t.ghost_qadr + y) = r + (y < 3 ? t.ghost_offset[y] : 0.0f);
+  }
+  if (y == 0) {
+    for (int i = 0; i < 3; i++) AT(d.qvel, t.root_vadr + i) = b0[7 + i];
+    const int rows = n < t.max_episode_rows ? n : t.max_episode_rows;
+    t.ep_traj[e] = traj; t.ep_start[e] = start; t.ep_row0[e] = row0; t.ep_n[e] = n; t.ep_steps[e] = rows - (t.future_steps + 1);
+  }
+}
 FB_DEV void ktask_reset(const DevModel& m, const DevData& d, int e, int y) {
   if (!d.task || e >= d.N) return;
   const DevTask& t = *d.task;
@@ -1253,7 +1293,8 @@ FB_DEV void ktask_reset2(const DevModel& m, const DevData& d, int e, int y) {   
   if (!t.needs_reset[e]) return;
   const int episode = t.episode[e];
   if (t.kind == 2) { ktask_reset_vision(m, d, t, e, y, episode); return; }
-  if (y < 7) { float r = t.ref_qpos[y]; AT(d.qpos, t.root_qadr + y) = r; if (t.ghost_qadr >= 0) AT(d.qpos, t.ghost_qadr + y) = r + (y < 3 ? t.ghost_offset[y] : 0.0f); }
+  if (t.ref_bank) ktask_reset_ref(m, d, t, e, y, episode);
+  else if (y < 7) { float r = t.ref_qpos[y]; AT(d.qpos, t.root_qadr + y) = r; if (t.ghost_qadr >= 0) AT(d.qpos, t.ghost_qadr + y) = r + (y < 3 ? t.ghost_offset[y] : 0.0f); }
   for (int i = y; i < t.n_noise; i += FB_NY) AT(d.qpos, t.noise_qadr[i]) += t.noise_amp * (2.0f * tk_u01(t, e, episode, 1 + i) - 1.0f);
   if (y == 0) {
     if (t.kind == 1) {          // wings on the beat pattern of the base frequency at a random phase, root at the reference speed
@@ -1263,7 +1304,7 @@ FB_DEV void ktask_reset2(const DevModel& m, const DevData& d, int e, int y) {   
       int nxt = pos + 1 < len ? pos + 1 : len - 1;
       const float* q0 = t.wb_traj + ((size_t)idx * t.tab_len + pos) * t.n_wing; const float* q1 = t.wb_traj + ((size_t)idx * t.tab_len + nxt) * t.n_wing;
       for (int i = 0; i < t.n_wing; i++) { AT(d.qpos, t.wing_qadr[i]) = q0[i]; AT(d.qvel, t.wing_vadr[i]) = (q1[i] - q0[i]) / t.dt; }
-      for (int i = 0; i < 3; i++) AT(d.qvel, t.root_vadr + i) = t.ref_qvel[i];
+      if (!t.ref_bank) for (int i = 0; i < 3; i++) AT(d.qvel, t.root_vadr + i) = t.ref_qvel[i];
       t.wb_freq[e] = t.wb_base_freq; t.wb_idx[e] = idx; t.wb_pos[e] = pos;
     }
     AT(d.time, 0) = 0; AT(d.flags, 0) = 0; AT(d.hold, 0) = 1; AT(d.prev_n, 0) = 0;
@@ -1275,10 +1316,14 @@ FB_DEV void ktask_before(const DevModel& m, const DevData& d, int e, int y) {
   const DevTask& t = *d.task;
   const int resetting = t.needs_reset[e];
   int step = resetting ? 0 : t.step[e];
-  if (step > t.ref_len - 1) step = t.ref_len - 1;
+  // the shared reference, or (ref_bank) the env's own: pose from its slot, velocity from the bank, step clamped by its rows in use
+  const int last = t.ref_bank ? t.ep_n[e] - 1 : t.ref_len - 1;
+  if (step > last) step = last;
   if (t.ghost_qadr >= 0) {
-    if (y < 7) AT(d.qpos, t.ghost_qadr + y) = t.ref_qpos[7 * step + y] + (y < 3 ? t.ghost_offset[y] : 0.0f);
-    else if (y < 13) AT(d.qvel, t.ghost_vadr + y - 7) = resetting ? 0.0f : t.ref_qvel[6 * step + y - 7];
+    const float* rq = t.ref_bank ? t.slots + ((size_t)e * t.slot_len + step) * 7 : t.ref_qpos + 7 * step;
+    const float* rv = t.ref_bank ? t.rbank + (size_t)FB_RBANK_W * (t.ep_row0[e] + step) + 7 : t.ref_qvel + 6 * step;
+    if (y < 7) AT(d.qpos, t.ghost_qadr + y) = rq[y] + (y < 3 ? t.ghost_offset[y] : 0.0f);
+    else if (y < 13) AT(d.qvel, t.ghost_vadr + y - 7) = resetting ? 0.0f : rv[y - 7];
   }
   if (y == 0) {
     if (t.kind >= 1 && !resetting) {
@@ -1305,7 +1350,7 @@ FB_DEV void ktask_commit(const DevModel& m, const DevData& d, int e, int y) {
   const DevTask& t = *d.task;
   const int resetting = t.needs_reset[e];
   t.resetting[e] = resetting;
-  if (resetting) { t.episode[e] = t.episode[e] + 1; t.has_uniform[e] = 0; } else t.step[e] = t.step[e] + 1;
+  if (resetting) { t.episode[e] = t.episode[e] + 1; t.has_uniform[e] = 0; if (t.ref_bank) t.pin[3 * (size_t)e] = 0; } else t.step[e] = t.step[e] + 1;
   t.op_step[e] = t.step[e]; t.op_first[e] = (unsigned char)resetting;
 }
 FB_DEV float tk_lin_tol(float x, float margin) { float v = 1.0f - fabsf(x) / margin; return v < 0.0f ? 0.0f : (v > 1.0f ? 1.0f : v); }
@@ -1316,7 +1361,7 @@ FB_DEV void ktask_after(const DevModel& m, const DevData& d, int e, int y) {
   const int resetting = t.resetting[e], step_now = t.step[e];
   const float* rd = o + t.obs_refdisp_off;
   const float com_dist = sqrtf(rd[0] * rd[0] + rd[1] * rd[1] + rd[2] * rd[2]);
-  const bool reached_end = step_now == t.episode_steps;
+  const bool reached_end = step_now == t.ep_steps[e];
   float s2 = 0; for (int i = 0; i < m.nv; i++) { float x = AT(d.qacc, i); s2 += x * x; }
   const bool bad = (AT(d.flags, 0) & 1) != 0 || !(sqrtf(s2) <= t.term_qacc);      // bits 1, 2 are capacity overflows, not bad physics
   bool terminate; float reward;

@@ -79,6 +79,7 @@ struct FbSim {
   int blob_in_smem;            // copy the sweep program of the triangular solves into shared memory per CTA (default: for batches <= 1024 envs; FB_BLOB=0/1 overrides)
   int* op_step_dev; unsigned char* op_first_dev;
   float* ref_slots; int ref_slot_len;      // per-env reference tables (fb_ref_slots)
+  float* rbank_dev; int *rbank_off_dev, *rbank_len_dev; std::vector<int> rbank_len; std::vector<void*> rbank_scope;   // flight trajectory bank (fb_ref_bank)
   DevHf hf; bool hf_on; int hf_nrow, hf_ncol;      // heightfield collision (fb_hfield_collision)
   float *bank_dev, *bank_hmax_dev, *bank_cmax_dev; int bank_n;      // terrain bank of the device-side vision task (fb_hfield_bank)
   DevEye eye; float* hfield_dev; float* hmax_dev; float* cmax_dev; int hf_nbr, hf_nbc; unsigned char* eye_out; size_t eye_bytes;   // eye cameras (fb_eye_program)
@@ -799,6 +800,7 @@ int fb_create(const FbModel* hm, int n_envs, int device, FbHandle* out) {
   s->device = device; s->launches = 0; s->last_ms = 0; s->hm = *hm; s->first_substep = 1; s->hold_pending = 0; s->prof_on = 0; memset(s->prof_ms, 0, sizeof(s->prof_ms)); memset(s->prof_n, 0, sizeof(s->prof_n));
   s->fuse = getenv("FB_FUSE") ? atoi(getenv("FB_FUSE")) : FB_FUSE_DEFAULT; if (s->fuse < 0 || s->fuse > 6 || s->fuse == 5) s->fuse = FB_FUSE_DEFAULT;
   s->ref_slots = nullptr; s->ref_slot_len = 0; s->eye_out = nullptr; s->hfield_dev = nullptr; s->hmax_dev = nullptr; s->cmax_dev = nullptr; s->hf_nbr = s->hf_nbc = 0; s->bank_dev = s->bank_hmax_dev = s->bank_cmax_dev = nullptr; s->bank_n = 0; s->eye_bytes = 0; s->hf_on = false; s->hf_nrow = s->hf_ncol = 0;
+  s->rbank_dev = nullptr; s->rbank_off_dev = s->rbank_len_dev = nullptr;
   s->op_step_dev = nullptr; s->op_first_dev = nullptr; s->stage_cap = 0; s->stage_icap = 0; s->stage = nullptr; s->stage_i = nullptr;
 #ifndef FB_EMU
   if (cudaSetDevice(device) != cudaSuccess) { delete s; return -2; }
@@ -1319,6 +1321,7 @@ int fb_ref_slots(FbHandle s, int slot_len) {
     if (s->ref_slots) {
       for (auto& a : s->allocs) if (a == s->ref_slots) { a = nullptr; break; }
       dev_free(s->ref_slots);
+      if (s->d.task && s->task_host.ref_bank) { scope_free(s, s->task_scope); s->d.task = nullptr; }      // it wrote into the old slots
     }
     s->ref_slots = dalloc<float>(s, (size_t)s->d.Np * 7 * slot_len); s->ref_slot_len = slot_len;
   }
@@ -1337,8 +1340,22 @@ int fb_ref_slot_write(FbHandle s, const int32_t* env_ids, int n, const float* ro
 int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   if (!s || !p) return -1;
   if (!s->d.tobs || !s->act_map_dev) { s->err = "fb_task_program: call fb_set_action_map and fb_obs_program first"; return -1; }
-  if (s->d.op_ref_slot) { s->err = "fb_task_program: per-env reference slots keep the host-side task code"; return -1; }
-  if (p->ref_len <= 0 || !p->ref_qpos || !p->ref_qvel || !p->reset_qpos) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
+  const bool bank = p->kind == 1 && p->ref_bank;
+  if (p->ref_bank && p->kind != 1) { s->err = "fb_task_program: ref_bank is for kind 1 (flight_imitation)"; return -1; }
+  if (s->d.op_ref_slot && !bank) { s->err = "fb_task_program: per-env reference slots keep the host-side task code"; return -1; }
+  if (bank) {
+    if (!s->d.op_ref_slot || !s->ref_slots || s->ref_slot_len < 1) { s->err = "fb_task_program: ref_bank needs the per-env reference slots (fb_ref_slots) first"; return -1; }
+    if (!s->rbank_dev) { s->err = "fb_task_program: ref_bank needs a trajectory bank (fb_ref_bank) first"; return -1; }
+    if (p->n_pick <= 0 || !p->pick_traj) { s->err = "fb_task_program: ref_bank needs the trajectory indices to draw from (n_pick, pick_traj)"; return -1; }
+    if (p->start_margin < 0 || p->max_episode_rows < 1 || p->future_steps < 0) { s->err = "fb_task_program: bad start_margin / max_episode_rows / future_steps"; return -1; }
+    for (int k = 0; k < p->n_pick; k++) {
+      const int j = p->pick_traj[k];
+      if (j < 0 || j >= (int)s->rbank_len.size()) { s->err = "fb_task_program: trajectory index of pick_traj out of range of the bank"; return -1; }
+      if (p->randomize_start && s->rbank_len[j] <= p->start_margin) {
+        s->err = "fb_task_program: with randomize_start every trajectory to draw from must be longer than start_margin rows"; return -1; }
+    }
+  } else if (p->ref_len <= 0 || !p->ref_qpos || !p->ref_qvel) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
+  if (!p->reset_qpos) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
   if (p->kind == 2 && (!s->bank_dev || !s->hfield_dev || s->bank_n <= 0)) { s->err = "fb_task_program: kind 2 needs fb_hfield_collision / fb_eye_program and fb_hfield_bank first"; return -1; }
   if (p->kind >= 1 && (p->n_wing <= 0 || p->n_freq <= 0 || p->tab_len <= 0 || !p->wb_traj || !p->wb_phase || !p->wb_phase_mod || !p->wb_freqs || !p->wb_len)) { s->err = "fb_task_program: wing-beat tables missing"; return -1; }
   if (sync_stream(s) != 0) return -2;
@@ -1355,7 +1372,9 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   t.ref_len = p->ref_len; t.obs_refdisp_off = p->obs_refdisp_off; t.obs_refquat_off = p->obs_refquat_off;
   auto upf32 = [&](const float* src, size_t n) { std::vector<float> v(src, src + n); return up(s, v); };
   auto upi32 = [&](const int32_t* src, size_t n) { std::vector<int> v(src, src + n); return up(s, v); };
-  t.reset_qpos = upf32(p->reset_qpos, m.nq); t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len);
+  t.reset_qpos = upf32(p->reset_qpos, m.nq);
+  if (!bank) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
+  else t.ref_len = 0;
   t.n_noise = p->noise_qadr ? p->n_noise : 0; t.noise_qadr = t.n_noise ? upi32(p->noise_qadr, t.n_noise) : nullptr; t.noise_amp = p->noise_amp; t.seed = p->seed;
   if (p->kind >= 1) {
     t.n_wing = p->n_wing; t.wing_qadr = upi32(p->wing_qadr, p->n_wing); t.wing_vadr = upi32(p->wing_vadr, p->n_wing); t.wing_ctrl = upi32(p->wing_ctrl, p->n_wing);
@@ -1367,6 +1386,16 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   t.step = dalloc<int>(s, Np); t.needs_reset = dalloc<int>(s, Np); t.resetting = dalloc<int>(s, Np); t.episode = dalloc<int>(s, Np);
   t.wb_idx = dalloc<int>(s, Np); t.wb_pos = dalloc<int>(s, Np); t.has_uniform = dalloc<int>(s, Np);
   t.uniform = dalloc<float>(s, (size_t)8 * Np); t.wb_freq = dalloc<float>(s, Np); t.out = dalloc<float>(s, (size_t)4 * Np);
+  t.ep_steps = dalloc<int>(s, Np);
+  if (bank) {          // episode lengths are set per env by each reset
+    t.ref_bank = 1; t.n_traj = (int)s->rbank_len.size(); t.rbank = s->rbank_dev; t.traj_off = s->rbank_off_dev; t.traj_len = s->rbank_len_dev;
+    t.n_pick = p->n_pick; t.pick_traj = upi32(p->pick_traj, p->n_pick); t.randomize_start = p->randomize_start ? 1 : 0; t.start_margin = p->start_margin;
+    t.max_episode_rows = p->max_episode_rows; t.future_steps = p->future_steps; t.slots = s->ref_slots; t.slot_len = s->ref_slot_len;
+    t.ep_traj = dalloc<int>(s, Np); t.ep_start = dalloc<int>(s, Np); t.ep_row0 = dalloc<int>(s, Np); t.ep_n = dalloc<int>(s, Np); t.pin = dalloc<int>(s, (size_t)3 * Np);
+  } else {
+    std::vector<int> steps((size_t)Np, p->episode_steps);
+    h2d(t.ep_steps, steps.data(), sizeof(int) * steps.size());
+  }
   if (p->kind == 2) {
     for (int i = 0; i < 2; i++) { t.th_rng[i] = p->target_height_range[i]; t.ts_rng[i] = p->target_speed_range[i]; t.x_rng[i] = p->init_x_range[i]; t.y_rng[i] = p->init_y_range[i]; }
     for (int i = 0; i < 4; i++) t.hover_quat[i] = p->hover_quat[i];
@@ -1468,6 +1497,51 @@ int fb_hfield_bank(FbHandle s, int n_terrain, const float* heights) {
   if (!s->bank_dev) { s->err = "out of device memory (terrain bank)"; return -4; }
   h2d(s->bank_dev, heights, sizeof(float) * cells * n_terrain); h2d(s->bank_hmax_dev, hmax.data(), sizeof(float) * n_terrain); h2d(s->bank_cmax_dev, cm.data(), sizeof(float) * cm.size());
   s->bank_n = n_terrain;
+  return 0;
+}
+int fb_ref_bank(FbHandle s, int n_traj, const int32_t* traj_len, const float* rows) {
+  if (!s) return -1;
+  if (n_traj <= 0 || !traj_len || !rows) { s->err = "fb_ref_bank: no trajectories"; return -1; }
+  std::vector<int> off(n_traj), len(traj_len, traj_len + n_traj);
+  size_t total = 0;
+  for (int k = 0; k < n_traj; k++) {
+    if (len[k] < 1) { s->err = "fb_ref_bank: empty trajectory"; return -1; }
+    off[k] = (int)total; total += (size_t)len[k];
+  }
+  if (total > (size_t)INT32_MAX / FB_RBANK_W) { s->err = "fb_ref_bank: bank too large"; return -1; }
+  if (sync_stream(s) != 0) return -2;
+  if (s->rbank_dev) {      // a replaced bank is freed; a flight program drawing from it has to be uploaded again
+    scope_free(s, s->rbank_scope);
+    if (s->d.task && s->task_host.ref_bank) { scope_free(s, s->task_scope); s->d.task = nullptr; }
+  }
+  const size_t mark = s->allocs.size();
+  s->rbank_dev = dalloc<float>(s, total * FB_RBANK_W); s->rbank_off_dev = dalloc<int>(s, n_traj); s->rbank_len_dev = dalloc<int>(s, n_traj);
+  s->rbank_scope.assign(s->allocs.begin() + mark, s->allocs.end());
+  if (!s->rbank_dev || !s->rbank_off_dev || !s->rbank_len_dev) { scope_free(s, s->rbank_scope); s->rbank_dev = nullptr; s->rbank_len.clear(); s->err = "out of device memory (trajectory bank)"; return -4; }
+  h2d(s->rbank_dev, rows, sizeof(float) * total * FB_RBANK_W); h2d(s->rbank_off_dev, off.data(), sizeof(int) * n_traj); h2d(s->rbank_len_dev, len.data(), sizeof(int) * n_traj);
+  s->rbank_len = len;
+  return 0;
+}
+int fb_task_ref_pick(FbHandle s, const int32_t* env_ids, int n, const int32_t* traj, const int32_t* start) {
+  if (!s || n < 0 || (n > 0 && (!env_ids || !traj || !start))) return -1;
+  if (!s->d.task || !s->task_host.ref_bank) { s->err = "fb_task_ref_pick: needs a kind 1 task program with ref_bank"; return -1; }
+  std::vector<int> pins((size_t)3 * n);
+  for (int k = 0; k < n; k++) {
+    if (env_ids[k] < 0 || env_ids[k] >= s->d.N) { s->err = "fb_task_ref_pick: env id out of range"; return -1; }
+    if (traj[k] < 0 || traj[k] >= (int)s->rbank_len.size()) { s->err = "fb_task_ref_pick: trajectory index out of range of the bank"; return -1; }
+    if (start[k] < 0 || start[k] >= s->rbank_len[traj[k]]) { s->err = "fb_task_ref_pick: start step outside the trajectory"; return -1; }
+    pins[3 * k] = 1; pins[3 * k + 1] = traj[k]; pins[3 * k + 2] = start[k];
+  }
+  if (sync_stream(s) != 0) return -2;
+  for (int k = 0; k < n; k++) upload_async(s, s->task_host.pin + (size_t)3 * env_ids[k], pins.data() + 3 * k, 3 * sizeof(int));
+  return sync_stream(s);                                        // `pins` goes out of scope
+}
+int fb_task_ref_state(FbHandle s, int32_t* traj, int32_t* start) {
+  if (!s || !traj || !start) return -1;
+  if (!s->d.task || !s->task_host.ref_bank) { s->err = "fb_task_ref_state: needs a kind 1 task program with ref_bank"; return -1; }
+  if (sync_stream(s) != 0) return -2;
+  d2h(traj, s->task_host.ep_traj, sizeof(int) * (size_t)s->d.N);
+  d2h(start, s->task_host.ep_start, sizeof(int) * (size_t)s->d.N);
   return 0;
 }
 int fb_task_step(FbHandle s, const float* action, int is_device, int n_substeps) {

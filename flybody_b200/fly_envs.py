@@ -298,11 +298,20 @@ class BatchedFlyEnv:
         self._ref_rows = None                       # per-env mode: [N, slot_len, 13] fp32 (root qpos 7, root qvel 6), padded with the last row
         self._ref_len = np.zeros(N, np.int64)
         self._episode_steps = np.zeros(N, np.int64)
+        self._ref_pick = np.zeros((N, 2), np.int64)      # flight dataset on the device: (trajectory, start step) the host pinned last
+        self._bank_rows = None                           # ... and the dataset as uploaded by fb_ref_bank (_bank_tables)
         # full-body imitation reward (reference walk_imitation.py:152-177): mocap joints / sites named by the dataset
         self._inference_mode = bool(inference_mode) or variant != 'walk'
-        if self._device_task and (self._per_env_ref or not self._inference_mode):
-            raise NotImplementedError('device_task covers the shared-reference (inference-mode) tasks; dataset mode keeps the '
-                                      'host-side task code')
+        # flight with a trajectory dataset on the device: the whole dataset in a device bank, every reset cuts its own reference from it
+        self._device_bank = self._device_task and self._per_env_ref and isinstance(tg, HDF5FlightTrajectoryLoader)
+        if self._device_task and not self._device_bank and (self._per_env_ref or not self._inference_mode):
+            raise NotImplementedError('device_task covers the shared-reference (inference-mode) tasks and flight_imitation with a '
+                                      'trajectory dataset; dataset-mode walk_imitation keeps the host-side task code')
+        if self._device_bank and tg.randomize_start_step:
+            short = [int(j) for j in np.unique(tg.traj_indices) if tg.trajectory_len(j) <= tg.START_MARGIN]
+            if short:
+                raise ValueError(f'randomize_start_step needs trajectories longer than {tg.START_MARGIN} rows; trajectories {short} have '
+                                 f'{[tg.trajectory_len(j) for j in short]}')
         self._seed = seed
         if not self._inference_mode:
             jnames, snames = tg.get_joint_names(), tg.get_site_names()
@@ -424,11 +433,19 @@ class BatchedFlyEnv:
                   control_timestep=self._control_timestep, time_limit=self._time_limit, terminal_com_dist=min(t._terminal_com_dist, 3e38),
                   terminal_linvel=_TERMINAL_LINVEL, terminal_angvel=_TERMINAL_ANGVEL, terminal_qacc=_TERMINAL_QACC, terminal_height=_TERMINAL_HEIGHT,
                   velocimeter_adr=int(self._sd['velocimeter'][0]), gyro_adr=int(self._sd['gyro'][0]), com_body=m.body_id('walker/thorax'),
-                  episode_steps=int(self._steps_of(self._ref_qpos.shape[0])), ref_len=self._ref_qpos.shape[0], ref_qpos=self._ref_qpos[:, :7],
-                  ref_qvel=self._ref_qvel[:, :6], obs_refdisp_off=sl['walker/ref_displacement'].start, obs_refquat_off=sl['walker/ref_root_quat'].start,
+                  obs_refdisp_off=sl['walker/ref_displacement'].start, obs_refquat_off=sl['walker/ref_root_quat'].start,
                   reset_qpos=q0, n_noise=len(self._leg_act_qadr) if (self._variant == 'walk' and self._reset_noise > 0) else 0,
                   noise_qadr=self._leg_act_qadr if (self._variant == 'walk' and self._reset_noise > 0) else None,
                   noise_amp=self._reset_noise, seed=int(self._seed) & 0xffffffff, com_offset=_COM_OFFSET)
+        if self._device_bank:                    # the draws of _load_snippet / HDF5FlightTrajectoryLoader.get_trajectory, on the device
+            tg = t._traj_generator
+            self._sim.ref_bank(*self._bank_tables())
+            kw.update(ref_bank=1, n_pick=len(tg.traj_indices), pick_traj=np.asarray(tg.traj_indices, np.int64),
+                      randomize_start=int(bool(tg.randomize_start_step)), start_margin=tg.START_MARGIN,
+                      max_episode_rows=round(self._time_limit / self._control_timestep), future_steps=t._future_steps)
+        else:
+            kw.update(episode_steps=int(self._steps_of(self._ref_qpos.shape[0])), ref_len=self._ref_qpos.shape[0], ref_qpos=self._ref_qpos[:, :7],
+                      ref_qvel=self._ref_qvel[:, :6])
         if self._variant == 'flight':
             wb = self._wbpg
             kw.update(n_wing=6, wing_qadr=self._wing_qadr, wing_vadr=self._wing_vadr, wing_ctrl=self._ctrl_of_action[self._action_indices['wings']],
@@ -458,7 +475,8 @@ class BatchedFlyEnv:
         values (content digest, so in-place edits count).  The switch is global: envs in mid-episode follow the new trajectory from
         their current step on, and with the task hooks on the device the re-upload restarts every env (`_program_switched`) -- a
         batch whose envs need independent references uses the per-env mode (`ref_path=` datasets), where each env of `ids` draws
-        its own snippet and only its device slot is rewritten."""
+        its own snippet and only its device slot is rewritten (flight with the task on the device: the device cuts the snippet from
+        its trajectory bank, `_pick_references`)."""
         t = self.task
         tg = t._traj_generator
         if not self._per_env_ref:
@@ -475,13 +493,10 @@ class BatchedFlyEnv:
             self._ref_len[:] = self._ref_qpos.shape[0]
             self._episode_steps[:] = self._steps_of(self._ref_qpos.shape[0])
             return
-        if self._ref_rows is None:                   # slot length: the longest reference an episode can consume
-            cap = self._max_reference_steps or (t._max_episode_steps + t._future_steps + 1)
-            if hasattr(tg, 'trajectory_len') and hasattr(tg, 'num_trajectories'):
-                cap = min(cap, max(int(tg.trajectory_len(i)) for i in range(tg.num_trajectories)))
-            self._slot_len = int(cap)
-            self._ref_rows = np.zeros((self.n_envs, self._slot_len, 13), np.float32)
-            self._upload_program()
+        self._ensure_slots()
+        if self._device_bank:
+            self._pick_references(ids)
+            return
         L = self._slot_len
         for e in ids:
             idx = t._next_traj_idx
@@ -498,6 +513,71 @@ class BatchedFlyEnv:
                 self._env_bank_off[e] = self._bank.offset_of(idx, snip)
         t._next_traj_idx = None
         self._sim.ref_slot_write(ids, self._ref_rows[ids, :, :7])
+
+    def _ensure_slots(self):
+        """per-env mode: the slot length (the longest reference an episode can consume), the host mirror and the programs, once"""
+        if self._ref_rows is not None:
+            return
+        t, tg = self.task, self.task._traj_generator
+        cap = self._max_reference_steps or (t._max_episode_steps + t._future_steps + 1)
+        if hasattr(tg, 'trajectory_len') and hasattr(tg, 'num_trajectories'):
+            cap = min(cap, max(int(tg.trajectory_len(i)) for i in range(tg.num_trajectories)))
+        self._slot_len = int(cap)
+        self._ref_rows = np.zeros((self.n_envs, self._slot_len, 13), np.float32)
+        self._upload_program()
+
+    def _bank_tables(self):
+        """(rows per trajectory, rows [sum][15]) of every trajectory of the flight dataset for fb_ref_bank -- all of them, because
+        set_next_trajectory_index may name any: root qpos (com2root in fp64), CoM qvel, CoM x, y.  Kept as the host mirror's source."""
+        if self._bank_rows is None:
+            tg = self.task._traj_generator
+            rows, lens = [], []
+            for j in range(tg.num_trajectories):
+                cq, cv = tg.full_trajectory(j)
+                cq, cv = np.asarray(cq, np.float64), np.asarray(cv, np.float64)
+                rows.append(np.concatenate([com2root(cq[:, :3], cq[:, 3:7]), cq[:, 3:7], cv[:, :6], cq[:, :2]], 1))
+                lens.append(cq.shape[0])
+            self._bank_len = np.asarray(lens, np.int64)
+            self._bank_off = np.concatenate([[0], np.cumsum(self._bank_len)[:-1]]).astype(np.int64)
+            self._bank_rows = np.concatenate(rows, 0).astype(np.float32)
+        return self._bank_len, self._bank_rows
+
+    def _pick_references(self, ids):
+        """flight dataset with the task on the device: the draws the host-side code makes at these resets (ascending env id; from the
+        loader's RandomState `choice`, then `randint`; a pending set_next_trajectory_index goes to every env of `ids` and is then
+        cleared), pinned for the device's reset (fb_task_ref_pick).  The host mirror (_ref_rows, _ref_len, _episode_steps) is cut
+        from the bank as ktask_reset_ref cuts it: fp32 rows start .. start + n, root x, y relative to the CoM x, y of row `start`,
+        padded with the last row."""
+        t, tg = self.task, self.task._traj_generator
+        ids = np.sort(np.asarray(ids, np.int64))
+        traj, start = np.zeros(len(ids), np.int64), np.zeros(len(ids), np.int64)
+        for k in range(len(ids)):
+            idx = t._next_traj_idx
+            if idx is None:
+                idx = tg._random_state.choice(tg.traj_indices)
+            traj[k] = idx
+            start[k] = tg._random_state.randint(tg.trajectory_len(idx) - tg.START_MARGIN) if tg.randomize_start_step else 0
+        t._next_traj_idx = None
+        self._sim.task_ref_pick(ids, traj, start)
+        self._ref_pick[ids, 0], self._ref_pick[ids, 1] = traj, start
+        for e, j, s0 in zip(ids, traj, start):
+            rows = self._bank_rows[self._bank_off[j] + s0:self._bank_off[j] + self._bank_len[j]]
+            n = min(rows.shape[0], self._slot_len)
+            r = rows[:n, :13].copy()
+            r[:, :2] -= rows[0, 13:15]
+            self._ref_rows[e, :n], self._ref_rows[e, n:] = r, r[n - 1]
+            self._ref_len[e] = n
+            self._episode_steps[e] = self._steps_of(n)
+
+    def reference_picks(self):
+        """(trajectory index, start step) of the reference every env tracks in its running episode, int32 [n_envs] each, read from
+        the device (flight_imitation with a dataset and device_task=True) -- e.g. to log which trajectory each env follows."""
+        if not self._device_bank:
+            raise RuntimeError('reference_picks needs flight_imitation(ref_path=..., device_task=True)')
+        if self._rec is None:
+            raise RuntimeError('no episode has started yet: call reset() or step_device() first')
+        traj, start = self._sim.task_ref_state()
+        return (traj, start) if self._batched else (int(traj[0]), int(start[0]))
 
     def _ref_at(self, step, ids=None):
         """[n, 13] root reference (qpos 7, qvel 6) of the listed envs at their own steps."""
@@ -597,16 +677,12 @@ class BatchedFlyEnv:
         (observation rows [n_envs, obs_dim], out [n_envs, 4] = reward, discount, step_type, 0) of the library's buffers, valid
         until the next step.  Nothing is copied to the host and the call does not synchronise: work is ordered on
         `env.physics.stepper.stream` (wrap it in `torch.cuda.ExternalStream` to order a policy after it).  Requires
-        `device_task=True`; `observation_layout()` names the columns."""
+        `device_task=True`; `observation_layout()` names the columns.  With a flight dataset the envs that reset draw their
+        trajectory and start step on the device (counter hash of seed, env, episode), so no trajectory index may be pending."""
         if not self._device_task:
             raise RuntimeError('step_device needs device_task=True (task hooks on the device)')
         import torch
-        if self._rec is None:
-            self._load_snippet(np.arange(self.n_envs))
-        cai = action.__cuda_array_interface__
-        assert tuple(cai['shape']) == (self.n_envs, self._action_spec.shape[0]) and cai['typestr'] == '<f4', cai
-        self._sim.task_step(cai['data'][0], self._n_sub, is_device=True)
-        self._needs_reset[:] = False            # (host mirror of the device's reset flags: not read back on this path)
+        self._launch_step_device(action)
         if getattr(self, '_dev_views', None) is None:
             obs_ptr, dim, out_ptr = self._sim.task_ptrs()
 
@@ -617,6 +693,21 @@ class BatchedFlyEnv:
             self._dev_views = (torch.as_tensor(_View(obs_ptr, (self.n_envs, dim)), device=dev),
                                torch.as_tensor(_View(out_ptr, (self.n_envs, 4)), device=dev))
         return self._dev_views
+
+    def _launch_step_device(self, action):
+        """the work of step_device up to its result views: the control step on the device, for actions already there"""
+        if self._device_bank and self.task._next_traj_idx is not None:
+            raise RuntimeError('set_next_trajectory_index is pending: which envs reset next is only known on the device, so apply it '
+                               'with step() (every env resetting in that step gets the index)')
+        if self._rec is None:
+            if self._device_bank:
+                self._ensure_slots()
+            else:
+                self._load_snippet(np.arange(self.n_envs))
+        cai = action.__cuda_array_interface__
+        assert tuple(cai['shape']) == (self.n_envs, self._action_spec.shape[0]) and cai['typestr'] == '<f4', cai
+        self._sim.task_step(cai['data'][0], self._n_sub, is_device=True)
+        self._needs_reset[:] = False            # (host mirror of the device's reset flags: not read back on this path)
 
     # ---------------------------------------------------------------------------------- eyes
     # cameras `eye_right` / `eye_left` on the head (reference fruitfly.xml:335-336; the head body keeps its XML frame)
@@ -652,7 +743,10 @@ class BatchedFlyEnv:
 
     def reset(self):
         if self._device_task:
-            self._load_snippet(np.arange(self.n_envs))
+            if self._device_bank:                # (the references are drawn once, by the step below)
+                self._ensure_slots()
+            else:
+                self._load_snippet(np.arange(self.n_envs))
             self._sim.task_reset_all()
             self._needs_reset[:] = True
             ts = self._device_step(np.zeros((self.n_envs, self._action_spec.shape[0]), np.float32))    # every env held: FIRST
@@ -823,7 +917,8 @@ def flight_imitation(ref_path=None, wpg_pattern_path=None, force_actuators=False
                      n_envs=None, device=0, lib_path=None, seed=0, device_task=False):
     """Batched `flybody.fly_envs.flight_imitation` (reference `fly_envs.py:30-97`): wing-beat-pattern-generator flight
     tracking, 4 substeps of 5e-5 s per control step, 12 actions (head 3, wings 6, abdomen 2, beat frequency 1).  With
-    `ref_path` every env tracks its own (randomly cut) CoM trajectory of the flight dataset."""
+    `ref_path` every env tracks its own (randomly cut) CoM trajectory of the flight dataset; with `device_task=True` as well, the
+    whole dataset is uploaded once as a device bank and every reset cuts its reference there (`reference_picks()` reads which)."""
     model = None
     if force_actuators or not disable_legs or joint_filter != 0.0:      # a non-default FruitFly: compiled on first use (flymodel.model_for)
         from .flymodel import model_for

@@ -22,7 +22,7 @@ MAXCON, MAXEFC = 64, 160
 
 EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_step', 'fb_forward',
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
-           'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version']
+           'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version']
 
 
 # enum FbObsItem
@@ -52,7 +52,9 @@ class FbTaskProgram(C.Structure):
                 ('wb_base_freq', C.c_float), ('wb_rel_range', C.c_float), ('wb_rate', C.c_float), ('com_offset', C.c_float * 3),
                 ('target_height_range', C.c_float * 2), ('target_speed_range', C.c_float * 2), ('init_x_range', C.c_float * 2), ('init_y_range', C.c_float * 2),
                 ('hover_quat', C.c_float * 4), ('target_zaxis', C.c_float * 3), ('floor_contacts_fatal', C.c_int32),
-                ('trench_cap', C.c_int32), ('trench_x', C.POINTER(C.c_float)), ('trench_len', C.POINTER(C.c_int32)), ('trench_y', C.POINTER(C.c_float))]
+                ('trench_cap', C.c_int32), ('trench_x', C.POINTER(C.c_float)), ('trench_len', C.POINTER(C.c_int32)), ('trench_y', C.POINTER(C.c_float)),
+                ('ref_bank', C.c_int32), ('n_pick', C.c_int32), ('pick_traj', C.POINTER(C.c_int32)), ('randomize_start', C.c_int32),
+                ('start_margin', C.c_int32), ('max_episode_rows', C.c_int32), ('future_steps', C.c_int32)]
 
 
 class FbEyeProgram(C.Structure):
@@ -100,6 +102,9 @@ def load_library(path=None):
     lib.fb_task_set_reset_noise.argtypes = [C.c_void_p, C.c_float]
     lib.fb_task_uniform_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.fb_hfield_bank.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    lib.fb_ref_bank.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.fb_task_ref_pick.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.fb_task_ref_state.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.fb_task_ptrs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p)]
     lib.fb_task_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.fb_eye_program.argtypes = [C.c_void_p, C.c_void_p]
@@ -319,6 +324,26 @@ class BatchedStepper:
         h = np.ascontiguousarray(heights, np.float32).reshape(len(heights), -1)
         assert h.shape[1] == self._hfield_cells, (h.shape, self._hfield_cells)
         self._check(self._lib.fb_hfield_bank(self._h, h.shape[0], h.ctypes.data), 'fb_hfield_bank')
+
+    def ref_bank(self, traj_len, rows):
+        """fb_ref_bank: flight trajectories as rows [sum(traj_len)][15] (root qpos 7, CoM qvel 6, CoM x, y 2), one after the other."""
+        ln = np.ascontiguousarray(traj_len, np.int32)
+        r = np.ascontiguousarray(rows, np.float32)
+        assert r.shape == (int(ln.sum()), 15), (r.shape, int(ln.sum()))
+        self._check(self._lib.fb_ref_bank(self._h, len(ln), ln.ctypes.data, r.ctypes.data), 'fb_ref_bank')
+
+    def task_ref_pick(self, env_ids, traj, start):
+        """pin the trajectory and start step of the listed envs' next reset (fb_task_ref_pick)"""
+        ids = np.ascontiguousarray(env_ids, np.int32)
+        tr, s0 = np.ascontiguousarray(traj, np.int32), np.ascontiguousarray(start, np.int32)
+        assert tr.shape == s0.shape == ids.shape, (ids.shape, tr.shape, s0.shape)
+        self._check(self._lib.fb_task_ref_pick(self._h, ids.ctypes.data, len(ids), tr.ctypes.data, s0.ctypes.data), 'fb_task_ref_pick')
+
+    def task_ref_state(self):
+        """-> (trajectory, start step) int32 [n_envs] of every env's running episode (fb_task_ref_state)"""
+        traj, start = np.zeros(self.n_envs, np.int32), np.zeros(self.n_envs, np.int32)
+        self._check(self._lib.fb_task_ref_state(self._h, traj.ctypes.data, start.ctypes.data), 'fb_task_ref_state')
+        return traj, start
 
     def task_set_reset_noise(self, amp):
         self._check(self._lib.fb_task_set_reset_noise(self._h, float(amp)), 'fb_task_set_reset_noise')

@@ -103,15 +103,27 @@ class HDF5FlightTrajectoryLoader(HDF5TrajectoryLoader):
             self._com_qvel.append(np.asarray(self._store.get(g + 'com_qvel')))
             assert self._com_qpos[-1].shape[0] == self._com_qvel[-1].shape[0]
 
+    START_MARGIN = 50                                          # a random start leaves at least this many rows
+
     def trajectory_len(self, traj_idx):
         return len(self._com_qpos[traj_idx])
+
+    @property
+    def randomize_start_step(self):
+        return self._randomize_start_step
+
+    def full_trajectory(self, traj_idx):
+        """(com_qpos [T,7], com_qvel [T,6]) of one whole trajectory as stored: no start cut, no shift to the origin (read-only)."""
+        q, v = self._com_qpos[traj_idx].view(), self._com_qvel[traj_idx].view()
+        q.flags.writeable = v.flags.writeable = False
+        return q, v
 
     def get_trajectory(self, traj_idx=None, start_step=None, end_step=None):
         if traj_idx is None:
             traj_idx = self._random_state.choice(self._traj_indices)
         traj_len = len(self._com_qpos[traj_idx])
         if self._randomize_start_step:
-            start_step, end_step = self._random_state.randint(traj_len - 50), traj_len
+            start_step, end_step = self._random_state.randint(traj_len - self.START_MARGIN), traj_len
         else:
             start_step = 0 if start_step is None else start_step
             end_step = traj_len if end_step is None else end_step

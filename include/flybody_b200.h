@@ -288,7 +288,9 @@ int fb_read_obs(FbHandle h, float* host_dst);
  * check_termination / get_reward / get_discount (tasks/base.py:203-225, walk_imitation.py:179-203,
  * flight_imitation.py:170-226) -- evaluated on the device, so that a control step needs no host round trip: actions in
  * (host or device pointer), observation rows + (reward, discount, step_type) out.  Covers the shared-reference (inference-mode)
- * tasks; dataset mode keeps the host-side task code.  Requires fb_set_action_map and fb_obs_program first.          */
+ * tasks and flight_imitation with a trajectory dataset (kind 1 with ref_bank = 1: fb_ref_slots, then fb_ref_bank, then this
+ * program; every env draws its own trajectory and start step of the bank at each reset).  Dataset-mode walk_imitation keeps
+ * the host-side task code.  Requires fb_set_action_map and fb_obs_program first.                                      */
 typedef struct FbTaskProgram {
   int32_t kind;                        /* 0 walk_imitation, 1 flight_imitation, 2 vision_guided_flight (fields at the end of the struct) */
   int32_t root_qadr, root_vadr, ghost_qadr, ghost_vadr;   /* free-joint slots of the walker root and of the ghost */
@@ -319,8 +321,29 @@ typedef struct FbTaskProgram {
   int32_t floor_contacts_fatal;
   int32_t trench_cap;                  /* 0: no centre-line factor; else the row stride of trench_y */
   const float* trench_x /* [n_terrain][2] first / last x */; const int32_t* trench_len /* [n_terrain] samples */; const float* trench_y /* [n_terrain][trench_cap] */;
+  /* kind 1 with a trajectory dataset (tasks/flight_imitation.py:88-111, trajectory_loaders.py:67-141).  ref_bank = 1: per-env
+   * references from the bank of fb_ref_bank, written into the env's fb_ref_slots table at each reset (ref_qpos / ref_qvel /
+   * episode_steps are then unused).  A reset takes the pick pinned by fb_task_ref_pick, else draws from the counter hash: the
+   * trajectory uniformly over pick_traj (repeats allowed), the start step uniformly in [0, len - start_margin) if
+   * randomize_start, else 0.  Rows in use n = min(len - start, slot_len); the episode ends at step
+   * min(n, max_episode_rows) - (future_steps + 1).  Zero (the default of a zeroed struct): shared reference.           */
+  int32_t ref_bank;
+  int32_t n_pick; const int32_t* pick_traj /* [n_pick] trajectory indices of the bank */;
+  int32_t randomize_start, start_margin;
+  int32_t max_episode_rows;            /* round(time_limit / control_timestep) */
+  int32_t future_steps;
 } FbTaskProgram;
 int fb_task_program(FbHandle h, const FbTaskProgram* p);
+/* Flight trajectory bank for kind 1 with ref_bank: n_traj trajectories, rows [sum(traj_len)][15] fp32, trajectory k after
+ * trajectory k - 1: root qpos (7; the dataset's CoM pose through com2root), CoM qvel (6), CoM x, y (2).  A reset at start step s
+ * shifts the root x, y of its rows by the CoM x, y of row s (every episode starts above the origin, trajectory_loaders.py:120).
+ * Uploaded once; calling it again replaces the bank and drops a task program that points at it.                       */
+int fb_ref_bank(FbHandle h, int n_traj, const int32_t* traj_len, const float* rows);
+/* Pin the trajectory and start step of the listed envs' next reset (consumed and cleared by that reset) -- the draws of a host
+ * RandomState, where the counter hash would draw otherwise.  Needs a kind 1 program with ref_bank.                    */
+int fb_task_ref_pick(FbHandle h, const int32_t* env_ids, int n, const int32_t* traj, const int32_t* start);
+/* Trajectory and start step of every env's running episode, int32 [n_envs] each, to the host (synchronises).          */
+int fb_task_ref_state(FbHandle h, int32_t* traj, int32_t* start);
 /* One control step with the task logic on the device: [auto-reset] -> action -> ctrl -> before_step -> n_substeps x physics ->
  * observation program -> termination / reward.  `action` rows [n_envs][n_action] (fb_set_action_map), host or device.  */
 int fb_task_step(FbHandle h, const float* action, int is_device, int n_substeps);
