@@ -812,7 +812,6 @@ FB_DEV void kref(FB_PHASE_ARGS) {
 // ---------------------------------------------------------------------------------------------
 // K3 + K8 transmission and actuation (MuJoCo mj_transmission, mj_fwdActuation), lane = env
 FB_DEV void kact_p0(FB_PHASE_ARGS) {
-  if (e == 0 && y == 0 && d.heavy_count) *d.heavy_count = 0;       // the heavy-env queue of this substep's solve (filled by the next kernel)
   tsolve_stage_issue(m, d, sh, e, lane, y, d.qLD); for (int k = y; k < m.nv; k += FB_NY) AT(d.qfrc_actuator, k) = 0; }
 FB_DEV void kact_p1(FB_PHASE_ARGS) {
   for (int i = y; i < m.nu; i += FB_NY) {

@@ -4,9 +4,10 @@
 // rows of that env's dual problem (rows of the Delassus matrix-vector products, columns of the Hessian
 // factor, line-search partial sums).  Every env therefore runs exactly its own number of Newton
 // iterations on its own problem size -- no divergence between envs -- and synchronisation is
-// __syncwarp only.  The working set of an env (row constants, 12 work vectors, the packed Delassus
-// matrix A and the packed Hessian factor G) lives in the warp's slice of shared memory when
-// nefc <= FB_SOLVE_NCAP (the common case); larger problems run the same code on the global arrays.
+// __syncwarp only.  This generic form solves the problems the register path (fb_solver_reg.h) does not
+// hold (nefc > solve_ncap): the working set of an env (row constants, 12 work vectors, the packed Delassus
+// matrix A and the packed Hessian factor G) stays in the env's record; only the warp-sum staging RED
+// uses the warp's shared-memory slice.
 //
 // Math (see DESIGN.md "Solver"): with a = qacc_smooth + M^-1 J^T lam the primal cost of MuJoCo's Newton
 // solver becomes  c(lam) = 1/2 lam^T A lam + s(b + A lam),  A = J M^-1 J^T,  b = J qacc_smooth - aref,
@@ -29,14 +30,12 @@ enum { W_LAM = 0, W_JAR, W_F, W_R, W_U, W_DL, W_ADL, W_P, X_E0, X_E1, X_XQ, X_OU
        S_STATE, S_COLIDX, S_ECROW, S_ECKIND, S_NSLOT };
 #define TRI(r, c) ((r) * ((r) + 1) / 2 + (c))
 
-// memory of one env's problem: base pointers + element strides (1 in shared memory, Np in global memory)
+// memory of one env's problem: work vectors v [S_NSLOT][cap], packed Delassus matrix A and packed Hessian factor G in the env's
+// record (efc_w, efc_A, efc_G; cap = FB_MAXEFC), warp-sum staging red [4][32] in the warp's shared-memory slice
 struct SolveMem { float* v; float* A; float* G; float* red; int cap; };
-// Work vectors v [S_NSLOT][cap], packed Delassus matrix A and packed Hessian factor G.  SM == true: all three in shared memory (A is
-// copied in from the record): the heavy-env kernel fb_run_solve_big, cap = FB_MAXEFC; false: in the env's global record.
 #define SV(slot, r) sm.v[(slot) * sm.cap + (r)]
 #define AM(r, c) sm.A[(r) >= (c) ? TRI(r, c) : TRI(c, r)]
 #define GM(p, q) sm.G[TRI(p, q)]        // p >= q
-#define FB_SOLVE_BIG_FLOATS (S_NSLOT * FB_MAXEFC + 2 * TRI(FB_MAXEFC, 0) + 4 * 32)
 #define RED(k, l) sm.red[(k) * 32 + (l)]
 
 #define NOUNROLL _Pragma("unroll 1")
@@ -55,7 +54,7 @@ FB_DEV float wsum(float v) { for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sy
 #define IS_HEAD(r) (SV(S_TYPE, r) < 1.5f)
 
 // forces / cost of the rows headed at r (a plain row, or the first row of an elliptic contact)
-template <bool SM> FB_DEVN float head_update(const SolveMem sm, int r, bool build) {
+FB_DEVN float head_update(const SolveMem sm, int r, bool build) {
   int tp = (int)SV(S_TYPE, r);
   float jar = SV(W_JAR, r), D = SV(S_D, r), cost = 0;
   if (tp == 0) {
@@ -89,7 +88,7 @@ template <bool SM> FB_DEVN float head_update(const SolveMem sm, int r, bool buil
   return cost;
 }
 // line-search contribution (value, 1st, 2nd derivative) of the rows headed at r
-template <bool SM> FB_DEVN void head_ls(const SolveMem sm, int r, float alpha, float& c, float& g, float& h) {
+FB_DEVN void head_ls(const SolveMem sm, int r, float alpha, float& c, float& g, float& h) {
   int tp = (int)SV(S_TYPE, r);
   float jv = SV(W_ADL, r), x = SV(W_JAR, r) + alpha * jv, D = SV(S_D, r);
   if (tp == 0) { if (x < 0) { c += 0.5f * D * x * x; g += D * x * jv; h += D * jv * jv; } return; }
@@ -110,14 +109,14 @@ template <bool SM> FB_DEVN void head_ls(const SolveMem sm, int r, float alpha, f
     c += 0.5f * Dm * f * f; g += Dm * f * fp; h += Dm * (fp * fp + f * fpp);
   }
 }
-template <bool SM> FB_DEV float ecol_val(const SolveMem& sm, int p, int a) {   // a-th entry of column p of E
+FB_DEV float ecol_val(const SolveMem& sm, int p, int a) {   // a-th entry of column p of E
   int kind = (int)SV(S_ECKIND, p), r = (int)SV(S_ECROW, p);
   return kind == 2 ? SV(X_E1, r + a) : SV(X_E0, r + a);
 }
 
 // dst[r] = (addb ? b[r] : 0) + sum_j A[r][j] src[j] for this lane's rows; returns sum_r src[r]*(dst[r]-b[r]) partial
 // (one loop over j with a select for the packed index: splitting it at the diagonal makes the lanes diverge)
-template <bool SM> FB_DEVN float matvec_rows(const SolveMem sm, int n, int lane, int src, int dst, bool addb) {
+FB_DEVN float matvec_rows(const SolveMem sm, int n, int lane, int src, int dst, bool addb) {
   float acc = 0;
   NOUNROLL for (int r = lane; r < n; r += 32) {
     float s = 0;
@@ -130,7 +129,6 @@ template <bool SM> FB_DEVN float matvec_rows(const SolveMem sm, int n, int lane,
 }
 
 
-template <bool SM>
 FB_WARPFN void ksolve_impl(const DevModel& m, const DevData& d, const SolveMem& sm, int e, int n) {
   const float scale = 1.0f / (m.meaninertia * (m.nv > 1 ? m.nv : 1));
   float tot[4] = {0, 0, 0, 0}; (void)tot;
@@ -148,25 +146,24 @@ FB_WARPFN void ksolve_impl(const DevModel& m, const DevData& d, const SolveMem& 
         NOUNROLL for (int q = 0; q < pn; q++) if (AT(d.prev_key, q) == key) { l0 = AT(d.prev_lam, q); break; }
         SV(W_LAM, r) = l0; }
     }
-    if (SM) { int nt = TRI(n, 0); NOUNROLL for (int k = lane; k < nt; k += 32) sm.A[k] = AT(d.efc_A, k); }
     WPAR_END
     // ---- warm start: the previous solve's forces (matched by row identity), kept if cheaper than lam = 0.
     // jar = b + A lam and quad = 1/2 lam^T A lam are carried along the iterations: a step lam += alpha dlam changes them by
     // alpha * (A dlam) and alpha q1 + alpha^2 q2, both already known from the line search (the forces at the solution are
     // recomputed from scratch after the loop)
     WPAR_BEGIN WROWS SV(W_JAR, r) = SV(S_B, r); WPAR_END
-    WPAR_BEGIN float c = 0; WROWS if (IS_HEAD(r)) c += head_update<SM>(sm, r, false); WSUM_PUT(0, c); WPAR_END
+    WPAR_BEGIN float c = 0; WROWS if (IS_HEAD(r)) c += head_update(sm, r, false); WSUM_PUT(0, c); WPAR_END
     const float cost0 = WSUM_GET(0);
     WPAR_BEGIN WPAR_END
-    WPAR_BEGIN float q = 0.5f * matvec_rows<SM>(sm, n, lane, W_LAM, W_JAR, true); WSUM_PUT(0, q); WPAR_END
-    WPAR_BEGIN float c = 0; WROWS if (IS_HEAD(r)) c += head_update<SM>(sm, r, false); WSUM_PUT(1, c); WPAR_END
+    WPAR_BEGIN float q = 0.5f * matvec_rows(sm, n, lane, W_LAM, W_JAR, true); WSUM_PUT(0, q); WPAR_END
+    WPAR_BEGIN float c = 0; WROWS if (IS_HEAD(r)) c += head_update(sm, r, false); WSUM_PUT(1, c); WPAR_END
     float quad = WSUM_GET(0);
     const float cost_ws = quad + WSUM_GET(1);
     WPAR_BEGIN WPAR_END
     if (!(cost_ws < cost0)) { WPAR_BEGIN WROWS { SV(W_LAM, r) = 0; SV(W_JAR, r) = SV(S_B, r); } WPAR_END quad = 0; }
     // ---- Newton iterations
     NOUNROLL for (int iter = 0; iter < m.max_iter; iter++) {
-      WPAR_BEGIN float c = 0; WROWS if (IS_HEAD(r)) c += head_update<SM>(sm, r, true); WSUM_PUT(1, c); WPAR_END
+      WPAR_BEGIN float c = 0; WROWS if (IS_HEAD(r)) c += head_update(sm, r, true); WSUM_PUT(1, c); WPAR_END
       WPAR_BEGIN float rr = 0, ll = 0; WROWS { float f = SV(W_F, r), rv = SV(W_LAM, r) - f; SV(W_R, r) = rv; rr += rv * rv; ll += f * f; } WSUM_PUT(2, rr); WSUM_PUT(3, ll); WPAR_END
       float cost = quad + WSUM_GET(1);
       float rr = WSUM_GET(2), ll = WSUM_GET(3);
@@ -182,12 +179,12 @@ FB_WARPFN void ksolve_impl(const DevModel& m, const DevData& d, const SolveMem& 
       WPAR_END
       const int nc = (int)RED(0, 0);
       // u = A r
-      WPAR_BEGIN matvec_rows<SM>(sm, n, lane, W_R, W_U, false); WPAR_END
+      WPAR_BEGIN matvec_rows(sm, n, lane, W_R, W_U, false); WPAR_END
       // p = E^T u ; G = I + E^T A E (packed lower triangle)
       WPAR_BEGIN
         NOUNROLL for (int p = lane; p < nc; p += 32) {
           int rp = (int)SV(S_ECROW, p), np = SV(S_ECKIND, p) == 0 ? 1 : 3;
-          float pv = 0; NOUNROLL for (int a = 0; a < np; a++) pv += ecol_val<SM>(sm, p, a) * SV(W_U, rp + a);
+          float pv = 0; NOUNROLL for (int a = 0; a < np; a++) pv += ecol_val(sm, p, a) * SV(W_U, rp + a);
           SV(W_P, p) = pv;
         }
         const int npairs = nc * (nc + 1) / 2;                 // lanes over the entries (p >= q) of the packed triangle
@@ -199,7 +196,7 @@ FB_WARPFN void ksolve_impl(const DevModel& m, const DevData& d, const SolveMem& 
           int rp = (int)SV(S_ECROW, p), np = SV(S_ECKIND, p) == 0 ? 1 : 3;
           int rq = (int)SV(S_ECROW, q), nq = SV(S_ECKIND, q) == 0 ? 1 : 3;
           float s = (p == q) ? 1.0f : 0.0f;
-          NOUNROLL for (int a = 0; a < np; a++) { float va = ecol_val<SM>(sm, p, a); if (va == 0.0f) continue; NOUNROLL for (int bb = 0; bb < nq; bb++) s += va * AM(rp + a, rq + bb) * ecol_val<SM>(sm, q, bb); }
+          NOUNROLL for (int a = 0; a < np; a++) { float va = ecol_val(sm, p, a); if (va == 0.0f) continue; NOUNROLL for (int bb = 0; bb < nq; bb++) s += va * AM(rp + a, rq + bb) * ecol_val(sm, q, bb); }
           GM(p, q) = s;
         }
       WPAR_END
@@ -226,14 +223,14 @@ FB_WARPFN void ksolve_impl(const DevModel& m, const DevData& d, const SolveMem& 
           else if (stt >= 2) v += SV(X_E0, r) * SV(X_OUT, c0) + SV(X_E1, r) * SV(X_OUT, c0 + 1);
           SV(W_DL, r) = v; }
       WPAR_END
-      WPAR_BEGIN float q2 = 0.5f * matvec_rows<SM>(sm, n, lane, W_DL, W_ADL, false), q1 = 0;
+      WPAR_BEGIN float q2 = 0.5f * matvec_rows(sm, n, lane, W_DL, W_ADL, false), q1 = 0;
           WROWS q1 += SV(W_DL, r) * (SV(W_JAR, r) - SV(S_B, r)); WSUM_PUT(0, q1); WSUM_PUT(1, q2); WPAR_END
       const float q1 = WSUM_GET(0), q2 = WSUM_GET(1);
       WPAR_BEGIN WPAR_END
       // exact line search: safeguarded Newton on the derivative of the 1-D cost
       float alpha = 0, lo = 0, hi = -1, g0 = 0, cbest = cost; bool stop = false, nodescent = false;
       NOUNROLL for (int ls = 0; ls <= m.ls_iter && !stop; ls++) {
-        WPAR_BEGIN float c = 0, g = 0, h = 0; WROWS if (IS_HEAD(r)) head_ls<SM>(sm, r, alpha, c, g, h); WSUM_PUT(0, c); WSUM_PUT(1, g); WSUM_PUT(2, h); WPAR_END
+        WPAR_BEGIN float c = 0, g = 0, h = 0; WROWS if (IS_HEAD(r)) head_ls(sm, r, alpha, c, g, h); WSUM_PUT(0, c); WSUM_PUT(1, g); WSUM_PUT(2, h); WPAR_END
         float c = quad + alpha * q1 + alpha * alpha * q2 + WSUM_GET(0), g = q1 + 2 * alpha * q2 + WSUM_GET(1), h = 2 * q2 + WSUM_GET(2);
         WPAR_BEGIN WPAR_END          // keep RED reads of all lanes ahead of the next section's writes
         if (ls == 0) {
@@ -262,13 +259,13 @@ FB_WARPFN void ksolve_impl(const DevModel& m, const DevData& d, const SolveMem& 
       if (scale * (cost - cbest) < m.tolerance || (cost - cbest) < m.solve_rtol * fabsf(cost)) break;
     }
     // ---- forces at the solution: lam = f(b + A lam)
-    WPAR_BEGIN matvec_rows<SM>(sm, n, lane, W_LAM, W_JAR, true); WPAR_END
-    WPAR_BEGIN WROWS if (IS_HEAD(r)) head_update<SM>(sm, r, false); WPAR_END
+    WPAR_BEGIN matvec_rows(sm, n, lane, W_LAM, W_JAR, true); WPAR_END
+    WPAR_BEGIN WROWS if (IS_HEAD(r)) head_update(sm, r, false); WPAR_END
     // ---- noslip (MuJoCo mj_solNoSlip): sequential Gauss-Seidel over the friction rows with the unregularised A
     if (m.noslip_iterations > 0) {
       // residual res = b + A f of every row, kept current in W_U: the contact being updated reads its two friction
       // entries, then all lanes apply the rank-2 change -- no O(n) dot products on a single lane
-      WPAR_BEGIN matvec_rows<SM>(sm, n, lane, W_F, W_U, true); WPAR_END
+      WPAR_BEGIN matvec_rows(sm, n, lane, W_F, W_U, true); WPAR_END
       WPAR_BEGIN if (lane == 0) { float imp = 0; NOUNROLL for (int i = 0; i < n; i++) imp += 0.5f * SV(W_F, i) * SV(W_F, i) * SV(S_R, i); RED(1, 0) = imp; } WPAR_END
       NOUNROLL for (int it = 0; it < m.noslip_iterations; it++) {
         bool any = false;

@@ -383,31 +383,13 @@ FB_WARPFN void ksolve_reg(const DevModel& m, const DevData& d, float* wsm, int e
   WPAR_END
 }
 
-// Envs with more rows than the register path holds (nefc > 32: freshly reset flies, flies pressed against their joint limits --
-// 0.05 - 1 % of a batch) run the generic code on their record in global memory, inline in this kernel (default), or -- FB_HEAVY_KERNEL=1,
-// measured slower, see alloc_data -- are queued (d.heavy_list) and solved by fb_run_solve_big right behind this kernel: one warp per
-// heavy env with the whole problem (work vectors, A, G for up to FB_MAXEFC rows, 117 KB) in shared memory.  The host emulation always
-// takes the shared-memory form, so that both instantiations of ksolve_impl are exercised by the CPU tests.
-FB_WARPFN void ksolve_big(const DevModel& m, const DevData& d, float* smem, int e) {
-  const int n = AT(d.nefc, 0);
-  SolveMem sm;
-  sm.v = smem; sm.A = sm.v + S_NSLOT * FB_MAXEFC; sm.G = sm.A + TRI(FB_MAXEFC, 0); sm.red = sm.G + TRI(FB_MAXEFC, 0); sm.cap = FB_MAXEFC;
-  ksolve_impl<true>(m, d, sm, e, n);
-}
-// one env; `wsm` = this warp's shared-memory slice (FB_SOLVE_WARP_FLOATS floats)
+// one env; `wsm` = this warp's shared-memory slice (FB_SOLVE_WARP_FLOATS floats).  Envs with more rows than the register path
+// holds (nefc > 32: freshly reset flies, flies pressed against their joint limits -- 0.05 - 1 % of a batch) run the generic code
+// on their record in global memory, inline in this kernel: there their solve overlaps with the other envs' solves.
 FB_WARPFN void ksolve_warp(const DevModel& m, const DevData& d, float* wsm, int e) {
   const int n = AT(d.nefc, 0);
   if (n <= m.solve_ncap) { ksolve_reg(m, d, wsm, e, n); return; }
-#ifdef __CUDACC__
-  if (d.heavy_list) {                      // queue it for fb_run_solve_big
-    if (threadIdx.x == 0) { int slot = atomicAdd(d.heavy_count, 1); d.heavy_list[slot] = e; }
-    return;
-  }
-  { SolveMem sm;                           // fused launch groupings (FB_FUSE): no second kernel, the generic code on the env's global record
-    sm.red = wsm; sm.v = &AT(d.efc_w, 0); sm.A = &AT(d.efc_A, 0); sm.G = &AT(d.efc_G, 0); sm.cap = FB_MAXEFC;
-    ksolve_impl<false>(m, d, sm, e, n); }
-#else
-  { static float* big = nullptr; if (!big) big = (float*)malloc(sizeof(float) * FB_SOLVE_BIG_FLOATS);      // host emulation: the heavy-env kernel's code path, inline
-    ksolve_big(m, d, big, e); }
-#endif
+  SolveMem sm;
+  sm.red = wsm; sm.v = &AT(d.efc_w, 0); sm.A = &AT(d.efc_A, 0); sm.G = &AT(d.efc_G, 0); sm.cap = FB_MAXEFC;
+  ksolve_impl(m, d, sm, e, n);
 }

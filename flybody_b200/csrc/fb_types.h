@@ -149,7 +149,6 @@ struct DevData {
   // sensors / outputs
   float *sensordata, *sensor_sum;
   int clk_launch; long long* clk;              // -DFB_CLK builds only: clock64() of warp 0 after every stage of every launch (latency profile)
-  int *heavy_count, *heavy_list;   // envs with more rows than the register solver holds, queued for fb_run_solve_big (global, not per env)
   int *flags, *niter, *hold;   // hold != 0: env is not integrated by the next fb_step (pending reset)
   const int* rst_ids; const float* rst_qpos; const float* rst_qvel; int rst_n, rst_has_qvel, rst_hold;   // staged partial reset
   float* sc_field; const int* sc_idx; const float* sc_vals; int sc_k, sc_nan0;                                 // staged column scatter

@@ -45,17 +45,8 @@ static void h2d(void* dst, const void* src, size_t n) { memcpy(dst, src, n); }
 static void d2h(void* dst, const void* src, size_t n) { memcpy(dst, src, n); }
 #endif
 
-#ifndef FB_SPLIT_DEFAULT
-#define FB_SPLIT_DEFAULT 1
-#endif
-#ifndef FB_FUSE_DEFAULT
-#define FB_FUSE_DEFAULT 0
-#endif
-#ifndef FB_OVERLAP_VEL_DEFAULT
-#define FB_OVERLAP_VEL_DEFAULT 0
-#endif
-enum { K_ACT = 0, K_SMOOTH, K_REF, K_SOLVE, K_FINISH, K_POS, K_COL, K_CON, K_PROJ, K_VEL, K_SENS, K_PACK, K_MISC, K_STEP2, K_STEP1, K_STEP, K_NKIND };
-static const char* const kKindNames[K_NKIND] = {"act", "smooth", "ref", "solve", "finish", "pos", "col", "con", "proj", "vel", "sens", "pack", "misc", "step2", "step1", "step"};
+enum { K_ACT = 0, K_SMOOTH, K_REF, K_SOLVE, K_FINISH, K_POS, K_COL, K_CON, K_PROJ, K_VEL, K_SENS, K_PACK, K_MISC, K_NKIND };
+static const char* const kKindNames[K_NKIND] = {"act", "smooth", "ref", "solve", "finish", "pos", "col", "con", "proj", "vel", "sens", "pack", "misc"};
 #ifndef FB_EMU
 struct ProfEvent { int kind; cudaEvent_t a, b; };
 #endif
@@ -70,12 +61,10 @@ struct FbSim {
   std::vector<void*> obs_scope, task_scope;   // device buffers of the current observation / task program: freed when the program is replaced
   std::vector<int> h_dof_parent, h_dof_Madr, h_body_lastdof, h_geom_bodyid;
   std::vector<double> h_qpos0;
-  int device, n_sm; long long launches; float last_ms; std::string err;
+  int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
   const int* act_map_dev; int n_action;
-  int cur_e0, cur_n;           // env range of the step kernels being issued (whole batch unless FB_SPLIT)
-  int fuse;                    // FB_FUSE: how the stage kernels of a step are grouped into launches (see fb_launch_fused)
   int blob_in_smem;            // copy the sweep program of the triangular solves into shared memory per CTA (default: for batches <= 1024 envs; FB_BLOB=0/1 overrides)
   int* op_step_dev; unsigned char* op_first_dev;
   float* ref_slots; int ref_slot_len;      // per-env reference tables (fb_ref_slots)
@@ -87,23 +76,12 @@ struct FbSim {
   float* stage; int* stage_i; size_t stage_cap, stage_icap; unsigned ws_slot;
 #ifndef FB_EMU
   cudaStream_t stream; cudaEvent_t ev0, ev1;
-  // FB_SPLIT: the batch is stepped as `split` env ranges ("chains") on their own streams, each chain started a few kernels
-  // after the previous one, so that different stage kernels share the SMs and one chain's stragglers overlap the other's work
-  int split, chain_stagger, chain_count, chain_idx; cudaStream_t cur_stream, aux[3]; cudaEvent_t chain_ev[4], join_ev[4];
-  int overlap_vel; cudaEvent_t fork_ev, vel_ev;       // FB_OVERLAP_VEL: velocity stage as a parallel branch of the step (launch_step1)
   struct StepGraph { cudaGraphExec_t exec; bool seen, failed; int n_sub; long long launches; DevData d; DevModel m; };
   StepGraph graph[2];          // [hold pending?]
   bool graphs_on;
 #endif
 };
 
-#ifndef FB_EMU
-// FB_SPLIT chains (step_sequence): after the `chain_stagger`-th step kernel of a chain an event lets the next chain start
-static void chain_mark(FbSim* s) {
-  if (s->chain_count < 0) return;
-  if (++s->chain_count == s->chain_stagger) cudaEventRecord(s->chain_ev[s->chain_idx], s->cur_stream);
-}
-#endif
 static size_t slice_bytes(size_t fixed, size_t dyn_floats) { return ((((fixed + 15) & ~(size_t)15) + dyn_floats * sizeof(float)) + 15) & ~(size_t)15; }
 // kernel = sequence of stages for one env.  Ph<f>: per-lane phase f(m, d, sh, e, 0, y), a warp barrier follows;
 // Wf<f>: warp function f(m, d, sh, e) written with WPAR sections (its own barriers inside).
@@ -125,6 +103,9 @@ template <typename Sh> __device__ __forceinline__ void set_prog(Sh&, const unsig
 __device__ __forceinline__ void set_prog(ShTree& sh, const unsigned* p) { sh.prog = p; }
 template <typename Sh> __device__ __forceinline__ void set_slice(Sh&, int) {}
 __device__ __forceinline__ void set_slice(ShCol& sh, int slice) { sh.slice = slice; }
+// e0 (the first env of the launch) is always 0.  It stays a run-time kernel parameter because ptxas (CUDA 12.9) schedules
+// the step kernels differently without it: the velocity kernel grew by 104 SASS instructions and ran 3 % slower on an
+// H100 SXM at 700 W.
 template <typename Sh, typename... St>
 __global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_run(DevModel m, DevData d, int slice, int e0, int nwarps, int blob_words) {
   extern __shared__ __align__(16) unsigned char fb_smem[];
@@ -151,9 +132,7 @@ __global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_run(DevModel m, DevDa
 }
 template <typename Sh, typename... St>
 static void fb_launch(FbSim* s, int kind, size_t dyn_floats = 0, int nwarps = -1, int blob_words = 0) {
-  // step kernels (nwarps < 0) cover the env range of the chain being issued (all envs unless FB_SPLIT, see step_sequence)
-  int e0 = 0;
-  if (nwarps < 0) { e0 = s->cur_e0; nwarps = s->cur_n; }
+  if (nwarps < 0) nwarps = s->d.Np;          // step kernels cover the padded batch
 #ifdef FB_CLK
   s->d.clk_launch = (int)(s->launches % 4096);
 #endif
@@ -161,23 +140,22 @@ static void fb_launch(FbSim* s, int kind, size_t dyn_floats = 0, int nwarps = -1
   size_t slice = slice_bytes(sizeof(Sh), dyn_floats), bytes = slice * FB_WPB + (size_t)blob_words * 4;
   static size_t configured = 0;
   if (bytes > configured) { cudaFuncSetAttribute(fb_run<Sh, St...>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); configured = bytes; }
-  cudaStream_t st = s->cur_stream;
+  cudaStream_t st = s->stream;
   if (s->prof_on) {
     cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
     cudaEventRecord(a, st);
-    fb_run<Sh, St...><<<grid, block, bytes, st>>>(s->m, s->d, (int)slice, e0, nwarps, blob_words);
+    fb_run<Sh, St...><<<grid, block, bytes, st>>>(s->m, s->d, (int)slice, 0, nwarps, blob_words);
     cudaEventRecord(b, st);
     s->prof_events.push_back({kind, a, b});
   } else {
-    fb_run<Sh, St...><<<grid, block, bytes, st>>>(s->m, s->d, (int)slice, e0, nwarps, blob_words);
+    fb_run<Sh, St...><<<grid, block, bytes, st>>>(s->m, s->d, (int)slice, 0, nwarps, blob_words);
   }
   s->launches++;
-  chain_mark(s);
 }
-__global__ void __launch_bounds__(32 * FB_SOLVE_WPB, FB_MINB) fb_run_solve(DevModel m, DevData d, int e0, int nwarps) {
+__global__ void __launch_bounds__(32 * FB_SOLVE_WPB, FB_MINB) fb_run_solve(DevModel m, DevData d, int nwarps) {
   extern __shared__ __align__(16) float fb_smem_w[];
-  int e = e0 + blockIdx.x * FB_SOLVE_WPB + threadIdx.y;
-  if (e >= e0 + nwarps) return;
+  int e = blockIdx.x * FB_SOLVE_WPB + threadIdx.y;
+  if (e >= nwarps) return;
 #ifdef FB_CLK
   if (e == 0 && threadIdx.x == 0) d.clk[32 * d.clk_launch] = clock64();
 #endif
@@ -186,35 +164,25 @@ __global__ void __launch_bounds__(32 * FB_SOLVE_WPB, FB_MINB) fb_run_solve(DevMo
   if (e == 0 && threadIdx.x == 0) d.clk[32 * d.clk_launch + 1] = clock64();
 #endif
 }
-// heavy envs (nefc > 32) queued by fb_run_solve: one warp per env, the whole problem in shared memory; the blocks stride over the queue
-__global__ void __launch_bounds__(32, 1) fb_run_solve_big(DevModel m, DevData d) {
-  extern __shared__ __align__(16) float fb_smem_big[];
-  const int count = *d.heavy_count;
-  for (int i = blockIdx.x; i < count; i += gridDim.x) { ksolve_big(m, d, fb_smem_big, d.heavy_list[i]); __syncwarp(); }
-}
 static void fb_launch_warp(FbSim* s, int kind) {
 #ifdef FB_CLK
   s->d.clk_launch = (int)(s->launches % 4096);
 #endif
-  dim3 block(32, FB_SOLVE_WPB), grid((s->cur_n + FB_SOLVE_WPB - 1) / FB_SOLVE_WPB);
+  dim3 block(32, FB_SOLVE_WPB), grid((s->d.Np + FB_SOLVE_WPB - 1) / FB_SOLVE_WPB);
   size_t bytes = sizeof(float) * FB_SOLVE_WARP_FLOATS * FB_SOLVE_WPB;
   static bool configured = false;
-  if (!configured) { cudaFuncSetAttribute(fb_run_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    cudaFuncSetAttribute(fb_run_solve_big, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * FB_SOLVE_BIG_FLOATS)); configured = true; }
-  cudaStream_t st = s->cur_stream;
+  if (!configured) { cudaFuncSetAttribute(fb_run_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); configured = true; }
+  cudaStream_t st = s->stream;
   if (s->prof_on) {
     cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
     cudaEventRecord(a, st);
-    fb_run_solve<<<grid, block, bytes, st>>>(s->m, s->d, s->cur_e0, s->cur_n);
-    if (s->d.heavy_list) fb_run_solve_big<<<s->n_sm, 32, sizeof(float) * FB_SOLVE_BIG_FLOATS, st>>>(s->m, s->d);
+    fb_run_solve<<<grid, block, bytes, st>>>(s->m, s->d, s->d.Np);
     cudaEventRecord(b, st);
     s->prof_events.push_back({kind, a, b});
   } else {
-    fb_run_solve<<<grid, block, bytes, st>>>(s->m, s->d, s->cur_e0, s->cur_n);
-    if (s->d.heavy_list) fb_run_solve_big<<<s->n_sm, 32, sizeof(float) * FB_SOLVE_BIG_FLOATS, st>>>(s->m, s->d);
+    fb_run_solve<<<grid, block, bytes, st>>>(s->m, s->d, s->d.Np);
   }
-  s->launches += s->d.heavy_list ? 2 : 1;
-  chain_mark(s);
+  s->launches++;
 }
 #else
 template <typename Sh> static void set_prog(Sh&, const unsigned*) {}
@@ -222,8 +190,7 @@ static void set_prog(ShTree& sh, const unsigned* p) { sh.prog = p; }
 template <typename Sh, typename... St>
 static void fb_launch(FbSim* s, int kind, size_t dyn_floats = 0, int nwarps = -1, int blob_words = 0) {
   (void)kind;
-  int e0 = 0;
-  if (nwarps < 0) { e0 = s->cur_e0; nwarps = s->cur_n; }
+  if (nwarps < 0) nwarps = s->d.Np;
   // the slice is exactly as large as the GPU launch makes it, followed by a canary: a phase that writes past its shared-memory
   // slice (on the GPU: into the next warp's slice or out of the block's allocation) aborts the CPU tests instead of passing
   const size_t used = slice_bytes(sizeof(Sh), dyn_floats);
@@ -231,7 +198,7 @@ static void fb_launch(FbSim* s, int kind, size_t dyn_floats = 0, int nwarps = -1
   memset(buf.data() + used, 0xAB, 256);
   Sh& sh = *reinterpret_cast<Sh*>(buf.data());
   (void)blob_words; set_prog(sh, s->m.tsolve_blob);        // host emulation: the program is read in place
-  for (int e = e0; e < e0 + nwarps; e++) (St::emu(s->m, s->d, sh, e), ...);
+  for (int e = 0; e < nwarps; e++) (St::emu(s->m, s->d, sh, e), ...);
   for (size_t i = 0; i < 256; i++) if (buf[used + i] != 0xAB) { fprintf(stderr, "fb_emu: shared-memory slice overrun in a kernel of kind %d (slice %zu bytes)\n", kind, used); abort(); }
   s->launches++;
 }
@@ -239,7 +206,7 @@ static void fb_launch_warp(FbSim* s, int kind) {
   const size_t used = sizeof(float) * FB_SOLVE_WARP_FLOATS;      // as fb_launch: the slice as the GPU launch sizes it, then a canary
   std::vector<unsigned char> buf(used + 256, 0);
   memset(buf.data() + used, 0xAB, 256);
-  for (int e = s->cur_e0; e < s->cur_e0 + s->cur_n; e++) ksolve_warp(s->m, s->d, reinterpret_cast<float*>(buf.data()), e);
+  for (int e = 0; e < s->d.Np; e++) ksolve_warp(s->m, s->d, reinterpret_cast<float*>(buf.data()), e);
   for (size_t i = 0; i < 256; i++) if (buf[used + i] != 0xAB) { fprintf(stderr, "fb_emu: shared-memory slice overrun in a kernel of kind %d (slice %zu bytes)\n", kind, used); abort(); }
   s->launches++;
 }
@@ -262,7 +229,7 @@ __global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_hf_kernel(DevModel m,
 static void launch_hfield(FbSim* s) {
 #ifndef FB_EMU
   dim3 block(32, FB_WPB), grid((s->d.N + FB_WPB - 1) / FB_WPB);
-  fb_hf_kernel<<<grid, block, 0, s->cur_stream>>>(s->m, s->d, s->hf, s->d.N);
+  fb_hf_kernel<<<grid, block, 0, s->stream>>>(s->m, s->d, s->hf, s->d.N);
 #else
   for (int e = 0; e < s->d.N; e++) { for (int y = 0; y < FB_NY; y++) khf_narrow(s->m, s->d, s->hf, e, y); for (int y = 0; y < FB_NY; y++) khf_append(s->m, s->d, s->hf, e, y); }
 #endif
@@ -288,7 +255,7 @@ FB_DEV void ph_smooth_out(FB_PHASE_ARGS) {
   }
 }
 
-// the stage lists of the seven step kernels (shared by the one-kernel-per-stage launches and the fused launches below)
+// the stage lists of the seven step kernels (also named by step_kernel_fn for the occupancy query)
 #define FB_ST_POS Ph<kpos_p0>, Ph<kpos_p1>, Ph<kpos_p1b>, Ph<kpos_p2>, Ph<kpos_p3>, Ph<kpos_p3b>, Ph<kpos_p4>, Wf<kpos_factor>, Ph<kpos_p6w>, Ph<kpos_p6d>, Wf<kpos_factor>, Ph<kpos_p9>
 #define FB_ST_COL Ph<kcol_stage>, Wf<kcol_broad>, Ph<kcol_narrow>, Wf<kcol_mpr>, Ph<kcol_compact>
 #define FB_ST_PROJ Ph<kcon_p0>, Ph<kcon_p1>, Ph<kcon_p2>, Ph<kcon_p3>, Ph<kproj_p0>, Ph<kproj_p1>
@@ -303,25 +270,6 @@ static size_t dyn_tsolve(const DevModel& m) { return (size_t)(FB_NXS(m) + ((m.nM
 
 static void launch_step1(FbSim* s) {
   fb_launch<ShTree, FB_ST_POS>(s, K_POS, dyn_pos(s->m));
-#ifndef FB_EMU
-  // The velocity stage (comVel, RNE bias, passive forces, velocity sensors) needs the position stage only; collision and the
-  // constraint rows need it too but not each other's outputs: vel runs as a parallel branch next to col -> proj (second stream,
-  // captured into the step graph as a fork / join).  Every kernel is a single wave that fills the register file, so the branch's
-  // blocks start as the collision kernel's blocks drain -- they fill its barrier / MPR tail instead of waiting behind proj.
-  if (s->overlap_vel && s->split == 1 && !s->prof_on) {
-    cudaStream_t main_st = s->cur_stream, side = s->aux[2];
-    cudaEventRecord(s->fork_ev, main_st); cudaStreamWaitEvent(side, s->fork_ev, 0);
-    s->cur_stream = side;
-    fb_launch<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m));
-    cudaEventRecord(s->vel_ev, side);
-    s->cur_stream = main_st;
-    fb_launch<ShCol, FB_ST_COL>(s, K_COL, dyn_col(s->m));
-    if (s->hf_on) launch_hfield(s);
-    fb_launch<ShCon, FB_ST_PROJ>(s, K_PROJ, dyn_proj(s->m));
-    cudaStreamWaitEvent(main_st, s->vel_ev, 0);
-    return;
-  }
-#endif
   fb_launch<ShCol, FB_ST_COL>(s, K_COL, dyn_col(s->m));
   if (s->hf_on) launch_hfield(s);              // heightfield contacts join the contact list before the constraint rows are built
   fb_launch<ShCon, FB_ST_PROJ>(s, K_PROJ, dyn_proj(s->m));
@@ -332,98 +280,6 @@ static void launch_step2(FbSim* s, bool integrate) {
   fb_launch<ShTree, FB_ST_SMOOTH>(s, K_SMOOTH, dyn_tsolve(s->m), -1, s->blob_in_smem ? s->m.ts_blob_words : 0);
   fb_launch_warp(s, K_SOLVE);
   fb_launch<ShTree, FB_ST_FINISH>(s, K_FINISH, dyn_tsolve(s->m), -1, s->blob_in_smem ? s->m.ts_blob_words : 0);
-}
-
-// -------------------------------------------------------------------------------------------
-// Fused launches.  An env is owned by one warp from the first to the last stage of a step and no stage looks at another
-// env, so consecutive stage kernels can run back to back inside one launch: a *group* is one of the kernels above (its
-// shared-memory struct re-interpreted on the warp's slice, sized for the largest group), a fused kernel is a list of groups,
-// optionally looped over the substeps of a control step.  What it buys: no grid-wide drain between stages (the envs of a
-// batch differ in contact count and Newton iterations, so every stage boundary otherwise waits for its slowest warp), the
-// warps of an SM drift apart and stop competing for the same unit at the same time, and an env's intermediates are re-read
-// from the L1/L2 of the SM that wrote them.  FB_FUSE selects: 0 one kernel per stage (7 per substep), 1 two kernels per
-// substep ([smooth solve finish] [pos col proj vel]), 2 one kernel per substep, 3 one kernel per control step.
-template <typename Sh, typename... St> struct Grp {
-#ifdef __CUDACC__
-  static __device__ __forceinline__ void run(const DevModel& m, const DevData& d, unsigned char* slice, int stride, const unsigned* prog, int e, int y) {
-    Sh& sh = *reinterpret_cast<Sh*>(slice);
-    set_slice(sh, stride); set_prog(sh, prog); __syncwarp();
-    ((St::run(m, d, sh, e, y), __syncwarp()), ...);
-  }
-#endif
-  static void emu(const DevModel& m, const DevData& d, unsigned char* slice, int e) {
-    Sh& sh = *reinterpret_cast<Sh*>(slice);
-    set_prog(sh, m.tsolve_blob);
-    (St::emu(m, d, sh, e), ...);
-  }
-};
-struct GrpSolve {
-#ifdef __CUDACC__
-  static __device__ __forceinline__ void run(const DevModel& m, const DevData& d, unsigned char* slice, int, const unsigned*, int e, int) {
-    ksolve_warp(m, d, reinterpret_cast<float*>(slice), e); __syncwarp();
-  }
-#else
-  static void emu(const DevModel& m, const DevData& d, unsigned char* slice, int e) { ksolve_warp(m, d, reinterpret_cast<float*>(slice), e); }
-#endif
-};
-using GSmooth = Grp<ShTree, FB_ST_SMOOTH>; using GFinish = Grp<ShTree, FB_ST_FINISH>; using GPos = Grp<ShTree, FB_ST_POS>;
-using GCol = Grp<ShCol, FB_ST_COL>; using GProj = Grp<ShCon, FB_ST_PROJ>; using GVel = Grp<ShTree, FB_ST_VEL>;
-FB_DEV void fused_sens_accum(const DevModel& m, const DevData& d, int e, int y, int first) {
-  for (int i = y; i < m.nsensordata; i += FB_NY) AT(d.sensor_sum, i) = (first ? 0.0f : AT(d.sensor_sum, i)) + AT(d.sensordata, i);
-}
-static size_t fused_slice_bytes(const DevModel& m) {
-  size_t b = slice_bytes(sizeof(ShTree), std::max(std::max(dyn_pos(m), dyn_tsolve(m)), dyn_vel(m)));
-  b = std::max(b, slice_bytes(sizeof(ShCol), dyn_col(m)));
-  b = std::max(b, slice_bytes(sizeof(ShCon), dyn_proj(m)));
-  b = std::max(b, slice_bytes(0, (size_t)FB_SOLVE_WARP_FLOATS));
-  return b;
-}
-#ifndef FB_EMU
-// loop_sens: the kernel runs n_sub whole substeps and restarts / continues the sensor sums itself (d.sens_mode is -1 then)
-template <typename... G>
-__global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_run_fused(DevModel m, DevData d, int slice, int nwarps, int blob_words, int n_sub, int loop_sens) {
-  extern __shared__ __align__(16) unsigned char fb_smem[];
-  unsigned* blob = reinterpret_cast<unsigned*>(fb_smem);
-  if (blob_words) {
-    for (int i = threadIdx.y * 32 + threadIdx.x; i < blob_words; i += 32 * FB_WPB) blob[i] = m.tsolve_blob[i];
-    __syncthreads();
-  }
-  int e = blockIdx.x * FB_WPB + threadIdx.y;
-  if (e >= nwarps) return;
-  unsigned char* sl = fb_smem + (size_t)blob_words * 4 + (size_t)threadIdx.y * slice;
-  const unsigned* prog = blob_words ? blob : m.tsolve_blob;
-  const int y = threadIdx.x;
-  for (int k = 0; k < n_sub; k++) {
-    (G::run(m, d, sl, slice, prog, e, y), ...);
-    if (loop_sens) { fused_sens_accum(m, d, e, y, k == 0); __syncwarp(); }
-  }
-}
-#endif
-template <typename... G>
-static void fb_launch_fused(FbSim* s, int kind, int n_sub, int loop_sens) {
-  const int nwarps = s->d.Np;
-  size_t slice = fused_slice_bytes(s->m);
-#ifndef FB_EMU
-  const int blob_words = s->blob_in_smem ? s->m.ts_blob_words : 0;
-  dim3 block(32, FB_WPB), grid((nwarps + FB_WPB - 1) / FB_WPB);
-  size_t bytes = slice * FB_WPB + (size_t)blob_words * 4;
-  static size_t configured = 0;
-  if (bytes > configured) { cudaFuncSetAttribute(fb_run_fused<G...>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); configured = bytes; }
-  cudaEvent_t a = nullptr, b = nullptr;
-  if (s->prof_on) { cudaEventCreate(&a); cudaEventCreate(&b); cudaEventRecord(a, s->cur_stream); }
-  fb_run_fused<G...><<<grid, block, bytes, s->cur_stream>>>(s->m, s->d, (int)slice, nwarps, blob_words, n_sub, loop_sens);
-  if (s->prof_on) { cudaEventRecord(b, s->cur_stream); s->prof_events.push_back({kind, a, b}); }
-#else
-  (void)kind;
-  static std::vector<unsigned char> buf;
-  if (buf.size() < slice + 64) buf.resize(slice + 64);
-  for (int e = 0; e < nwarps; e++)
-    for (int k = 0; k < n_sub; k++) {
-      (G::emu(s->m, s->d, buf.data(), e), ...);
-      if (loop_sens) for (int y = 0; y < FB_NY; y++) fused_sens_accum(s->m, s->d, e, y, k == 0);
-    }
-#endif
-  s->launches++;
 }
 
 // -------------------------------------------------------------------------------------------
@@ -728,12 +584,6 @@ static int alloc_data(FbSim* s, int N) {
 #ifdef FB_CLK
   d.clk = (long long*)dalloc<long long>(s, 32 * 4096);
 #endif
-#ifndef FB_EMU
-  // FB_HEAVY_KERNEL=1: queue of envs for the heavy-env solve kernel (fb_run_solve_big).  Off by default: a single warp needs a long time
-  // for a 48-row problem even from shared memory, and behind the main kernel that time is serial, whereas inline (generic code on the
-  // env's global record) it overlaps with the other envs' solves.
-  if (s->fuse == 0 && s->split == 1 && getenv("FB_HEAVY_KERNEL") && atoi(getenv("FB_HEAVY_KERNEL"))) { d.heavy_count = dalloc<int>(s, 4); d.heavy_list = dalloc<int>(s, d.Np); }
-#endif
   d.obs_dim = m.nq + m.nv + m.na + 2 * m.nsensordata + 12 + 3 * m.nsite + 3;
   d.obs = dalloc<float>(s, (size_t)d.obs_dim * d.Np);
   s->stage_cap = 0; s->stage = nullptr; s->stage_i = nullptr;
@@ -807,30 +657,20 @@ int fb_create(const FbModel* hm, int n_envs, int device, FbHandle* out) {
   if (!hm || !out || n_envs <= 0) return -1;
   FbSim* s = new FbSim();
   s->device = device; s->launches = 0; s->last_ms = 0; s->hm = *hm; s->first_substep = 1; s->hold_pending = 0; s->prof_on = 0; memset(s->prof_ms, 0, sizeof(s->prof_ms)); memset(s->prof_n, 0, sizeof(s->prof_n));
-  s->fuse = getenv("FB_FUSE") ? atoi(getenv("FB_FUSE")) : FB_FUSE_DEFAULT; if (s->fuse < 0 || s->fuse > 6 || s->fuse == 5) s->fuse = FB_FUSE_DEFAULT;
   s->ref_slots = nullptr; s->ref_slot_len = 0; s->eye_out = nullptr; s->hfield_dev = nullptr; s->hmax_dev = nullptr; s->cmax_dev = nullptr; s->hf_nbr = s->hf_nbc = 0; s->bank_dev = s->bank_hmax_dev = s->bank_cmax_dev = nullptr; s->bank_n = 0; s->eye_bytes = 0; s->hf_on = false; s->hf_nrow = s->hf_ncol = 0;
   s->rbank_dev = nullptr; s->rbank_off_dev = s->rbank_len_dev = nullptr;
   s->op_step_dev = nullptr; s->op_first_dev = nullptr; s->stage_cap = 0; s->stage_icap = 0; s->stage = nullptr; s->stage_i = nullptr;
 #ifndef FB_EMU
   if (cudaSetDevice(device) != cudaSuccess) { delete s; return -2; }
   cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-  { int n_sm = 0; cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device); s->n_sm = n_sm > 0 ? n_sm : 132; }
   cudaEventCreate(&s->ev0); cudaEventCreate(&s->ev1);
   s->graphs_on = getenv("FB_NO_GRAPH") == nullptr;
-  s->split = getenv("FB_SPLIT") ? atoi(getenv("FB_SPLIT")) : FB_SPLIT_DEFAULT; if (s->split < 1 || s->split > 4) s->split = 1;
-  s->chain_stagger = getenv("FB_STAGGER") ? atoi(getenv("FB_STAGGER")) : (s->split == 2 ? 3 : 2);
-  s->chain_count = -1; s->chain_idx = 0; s->cur_stream = s->stream;
-  for (int i = 0; i < 3; i++) cudaStreamCreateWithFlags(&s->aux[i], cudaStreamNonBlocking);
-  for (int i = 0; i < 4; i++) { cudaEventCreateWithFlags(&s->chain_ev[i], cudaEventDisableTiming); cudaEventCreateWithFlags(&s->join_ev[i], cudaEventDisableTiming); }
-  cudaEventCreateWithFlags(&s->fork_ev, cudaEventDisableTiming); cudaEventCreateWithFlags(&s->vel_ev, cudaEventDisableTiming);
-  s->overlap_vel = getenv("FB_OVERLAP_VEL") ? atoi(getenv("FB_OVERLAP_VEL")) : FB_OVERLAP_VEL_DEFAULT;
   // small batches are latency-bound (a per-CTA copy of the sweep program in shared memory halves the sweeps' latency);
   // at full occupancy the copy costs more than it saves and the compact program is read in place.  FB_BLOB=0/1 overrides.
   s->blob_in_smem = getenv("FB_BLOB") ? atoi(getenv("FB_BLOB")) : (n_envs <= 1024);
 #endif
   int rc = build_model(s, hm);
   if (rc == 0) rc = alloc_data(s, n_envs);
-  s->cur_e0 = 0; s->cur_n = s->d.Np;
   *out = s;
   if (rc != 0) return rc;
 #ifndef FB_EMU
@@ -915,57 +755,10 @@ int fb_forward(FbHandle s) {
 
 // the launch sequence of one control step: n x [ step2 ; step1 ], sensor accumulation restarted at the first substep
 static void step_sequence(FbSim* s, int n_substeps) {
-  if (s->fuse == 3) {                       // the whole control step in one launch
-    s->d.do_integrate = 1; s->d.sens_mode = -1;
-    fb_launch_fused<GSmooth, GrpSolve, GFinish, GPos, GCol, GProj, GVel>(s, K_STEP, n_substeps, 1);
-  }
-#ifndef FB_EMU
-  else if (s->fuse == 0 && s->split > 1) {
-    // env ranges as staggered chains on their own streams (captured into the step graph as parallel branches)
-    const int S = s->split, per = ((s->d.Np / FB_WPB + S - 1) / S) * FB_WPB;
-    for (int h = 0; h < S; h++) {
-      s->cur_stream = h == 0 ? s->stream : s->aux[h - 1];
-      s->cur_e0 = h * per; s->cur_n = std::min(per, s->d.Np - h * per);
-      if (s->cur_n <= 0) { s->cur_n = 0; continue; }
-      if (h > 0) cudaStreamWaitEvent(s->cur_stream, s->chain_ev[h - 1], 0);
-      s->chain_idx = h; s->chain_count = 0;
-      for (int k = 0; k < n_substeps; k++) {
-        launch_step2(s, true);
-        s->d.sens_mode = (k == 0) ? 1 : 0;
-        launch_step1(s);
-        s->d.sens_mode = -1;
-      }
-      s->chain_count = -1;
-      if (h > 0) { cudaEventRecord(s->join_ev[h], s->cur_stream); cudaStreamWaitEvent(s->stream, s->join_ev[h], 0); }
-    }
-    s->cur_stream = s->stream; s->cur_e0 = 0; s->cur_n = s->d.Np;
-  }
-#endif
-  else for (int k = 0; k < n_substeps; k++) {
-    if (s->fuse == 0) {
-      launch_step2(s, true);
-      s->d.sens_mode = (k == 0) ? 1 : 0;
-      launch_step1(s);
-    } else if (s->fuse == 4 || s->fuse == 6) {
-      // only the straggler-prone stage pairs share a launch: the Newton solve (1-7 iterations per env) with the finish stage,
-      // and (6) collision (MPR tail on one warp per block) with the constraint rows
-      s->d.do_integrate = 1;
-      fb_launch<ShTree, FB_ST_SMOOTH>(s, K_SMOOTH, dyn_tsolve(s->m), -1, s->blob_in_smem ? s->m.ts_blob_words : 0);
-      fb_launch_fused<GrpSolve, GFinish>(s, K_STEP2, 1, 0);
-      s->d.sens_mode = (k == 0) ? 1 : 0;
-      fb_launch<ShTree, FB_ST_POS>(s, K_POS, dyn_pos(s->m));
-      if (s->fuse == 6) fb_launch_fused<GCol, GProj>(s, K_STEP1, 1, 0);
-      else { fb_launch<ShCol, FB_ST_COL>(s, K_COL, dyn_col(s->m)); fb_launch<ShCon, FB_ST_PROJ>(s, K_PROJ, dyn_proj(s->m)); }
-      fb_launch<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m));
-    } else if (s->fuse == 1) {
-      s->d.do_integrate = 1;
-      fb_launch_fused<GSmooth, GrpSolve, GFinish>(s, K_STEP2, 1, 0);
-      s->d.sens_mode = (k == 0) ? 1 : 0;
-      fb_launch_fused<GPos, GCol, GProj, GVel>(s, K_STEP1, 1, 0);
-    } else {
-      s->d.do_integrate = 1; s->d.sens_mode = (k == 0) ? 1 : 0;       // only the last group (vel) reads sens_mode
-      fb_launch_fused<GSmooth, GrpSolve, GFinish, GPos, GCol, GProj, GVel>(s, K_STEP, 1, 0);
-    }
+  for (int k = 0; k < n_substeps; k++) {
+    launch_step2(s, true);
+    s->d.sens_mode = (k == 0) ? 1 : 0;
+    launch_step1(s);
     s->d.sens_mode = -1;
   }
   s->d.nsub_done = n_substeps;
@@ -1610,10 +1403,6 @@ int fb_hfield_collision(FbHandle s, int geom, const float* size, int nrow, int n
   if (!s || !size || !pair_geom || npair <= 0 || npair > FB_MAXCAND || nrow < 2 || ncol < 2) return -1;
   if (geom < 0 || geom >= s->m.ngeom) { s->err = "fb_hfield_collision: geom id out of range"; return -1; }
   for (int k = 0; k < npair; k++) if (pair_geom[k] < 0 || pair_geom[k] >= s->m.ngeom) { s->err = "fb_hfield_collision: pair geom out of range"; return -1; }
-  if (s->fuse != 0) { s->err = "fb_hfield_collision: needs the one-kernel-per-stage launch sequence (FB_FUSE=0, FB_SPLIT=1)"; return -1; }
-#ifndef FB_EMU
-  if (s->split > 1) { s->err = "fb_hfield_collision: needs the one-kernel-per-stage launch sequence (FB_FUSE=0, FB_SPLIT=1)"; return -1; }
-#endif
   if (sync_stream(s) != 0) return -2;
   if (ensure_hfield(s, nrow, ncol) != 0) return -1;
   DevHf& h = s->hf; h.geom = geom; h.nrow = nrow; h.ncol = ncol; h.npair = npair;

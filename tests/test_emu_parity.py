@@ -107,24 +107,3 @@ def test_generic_convex_narrowphase_matches_the_oracle_on_shallow_contacts():
         ok += int(nd == 1 and abs(dd - dist) < 2e-5 and np.abs(nn - nrm).max() < 5e-2)
     assert tot > 150 and ok >= 0.95 * tot, (ok, tot)
 
-
-def test_fused_launch_groupings_are_bit_identical(emu, monkeypatch):
-    """FB_FUSE regroups the same stage functions into fewer launches (2 per substep, 1 per substep, 1 per control step);
-    an env never looks at another env, so every grouping must reproduce the 7-launch sequence bit for bit, sensor sums
-    included."""
-    m = load_model('walk')
-    out = {}
-    for mode in ('0', '1', '2', '3', '4', '6'):
-        monkeypatch.setenv('FB_FUSE', mode)
-        sim = st.BatchedStepper(m, 2, lib_path=emu)
-        rs = np.random.RandomState(5)
-        l0 = sim.launch_count
-        for _ in range(2):
-            sim.set_control(rs.uniform(-0.5, 0.5, (2, m.nu)).astype(np.float32))
-            sim.step(10)
-        out[mode] = (sim.get(st.QPOS).copy(), sim.get(st.QVEL).copy(), sim.get(st.SENSOR_MEAN).copy(), sim.launch_count - l0)
-        sim.close()
-    assert out['0'][3] > out['4'][3] > out['6'][3] > out['1'][3] > out['2'][3] > out['3'][3]
-    for mode in ('1', '2', '3', '4', '6'):
-        for a, b in zip(out['0'][:3], out[mode][:3]):
-            assert np.array_equal(a, b)
