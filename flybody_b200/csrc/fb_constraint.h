@@ -1180,13 +1180,15 @@ FB_DEV void ktaskobs(const DevModel& m, const DevData& d, int e, int y) {
 //   ktask_reset  : composer auto-reset of envs whose last step was LAST -> initialize_episode (walk_imitation.py:112-136,
 //                  flight_imitation.py:113-144): template state, root / ghost on the first reference row, wings on the beat
 //                  pattern at a random phase (flight), optional U(-a, a) noise on listed joints; the env is held (not
-//                  integrated) through the coming step, exactly as fb_reset_hold does for the host-side task code; flight with
-//                  a dataset (ref_bank): the env's own reference cut from the trajectory bank first (ktask_reset_ref)
+//                  integrated) through the coming step, exactly as fb_reset_hold does for the host-side task code; with a
+//                  dataset (ref_bank): the env's own reference cut from the trajectory bank first (ktask_reset_ref), walking:
+//                  then the full-body start pose of the snippet and the wings back at their springs (ktask_reset3, ktask_reset4)
 //   ktask_before : before_step (walk_imitation.py:138-150, flight_imitation.py:146-168): ghost root pose / velocity from
 //                  the reference row of the current step; flight: one step of the wing-beat pattern generator at the requested
 //                  frequency, wing force commands += pattern angle - wing angle (pattern_generators.py:131-203)
 //   ktask_after  : check_termination, get_reward, get_discount (base.py:203-225, walk_imitation.py:179-203,
-//                  flight_imitation.py:170-226) -> out[e] = reward, discount, step_type
+//                  flight_imitation.py:170-226) -> out[e] = reward, discount, step_type; walking with a dataset: the DeepMimic
+//                  reward, its joint / site sums spread over the lanes first (ktask_reward)
 // Scalar work runs on lane 0 (table scans of <= ~500 entries a few times per episode), array copies over the lanes.
 FB_DEV unsigned tk_mix(unsigned x) { x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16; return x; }
 FB_DEV float tk_u01(const DevTask& t, int e, int episode, int k) {
@@ -1238,9 +1240,10 @@ FB_DEV void ktask_reset_vision(const DevModel& m, const DevData& d, const DevTas
   AT(d.time, 0) = 0; AT(d.flags, 0) = 0; AT(d.hold, 0) = 1; AT(d.prev_n, 0) = 0;
   t.step[e] = 0;          // (has_uniform is read by every lane above: ktask_commit clears it)
 }
-// kind 1 with ref_bank (flight_imitation with a dataset, flight_imitation.py:88-111, trajectory_loaders.py:109-121): the episode's
-// trajectory and start step -- the pin of fb_task_ref_pick, else the counter hash (draw indices 256, 257: past the wing-beat phase's 0
-// and the noise joints' 1 + i).  Every lane computes the same pick.
+// ref_bank (flight_imitation with a dataset, flight_imitation.py:88-111, trajectory_loaders.py:109-121; walk_imitation with a dataset,
+// walk_imitation.py:93-110, trajectory_loaders.py:146-156, start always 0): the episode's trajectory and start step -- the pin of
+// fb_task_ref_pick, else the counter hash (draw indices 256, 257: past the wing-beat phase's 0 and the noise joints' 1 + i).  Every lane
+// computes the same pick.
 FB_DEV void tk_ref_pick(const DevTask& t, int e, int episode, int& traj, int& start) {
   const int* pin = t.pin + 3 * (size_t)e;
   if (pin[0]) { traj = pin[1]; start = pin[2]; return; }
@@ -1250,18 +1253,18 @@ FB_DEV void tk_ref_pick(const DevTask& t, int e, int episode, int& traj, int& st
   start = 0;
   if (t.randomize_start) { start = (int)floorf(tk_u01(t, e, episode, 257) * (float)span); start = start > span - 1 ? span - 1 : start; }
 }
-// the env's reference of the new episode: rows start .. start + n of its trajectory into its slot, root x, y relative to the CoM x, y of
-// row `start`, the rest of the slot padded with the last row (as the host-side code fills a slot); root and ghost on row `start`, read
-// from the bank because the other lanes are still writing the slot
+// the env's reference of the new episode: rows start .. start + n of its trajectory into its slot, root x, y relative to the x, y in
+// columns 13, 14 of row `start` (flight: the CoM's, walking: the root's), the rest of the slot padded with the last row (as the host-side
+// code fills a slot); root and ghost on row `start`, read from the bank because the other lanes are still writing the slot
 FB_DEV void ktask_reset_ref(const DevModel& m, const DevData& d, const DevTask& t, int e, int y, int episode) {
   int traj, start; tk_ref_pick(t, e, episode, traj, start);
   const int len = t.traj_len[traj], row0 = t.traj_off[traj] + start;
   const int n = len - start < t.slot_len ? len - start : t.slot_len;
-  const float* b0 = t.rbank + (size_t)FB_RBANK_W * row0;
+  const float* b0 = t.rbank + (size_t)t.rbank_w * row0;
   const float cx = b0[13], cy = b0[14];
   float* slot = t.slots + (size_t)e * 7 * t.slot_len;
   for (int i = y; i < t.slot_len; i += FB_NY) {
-    const float* r = t.rbank + (size_t)FB_RBANK_W * (row0 + (i < n ? i : n - 1));
+    const float* r = t.rbank + (size_t)t.rbank_w * (row0 + (i < n ? i : n - 1));
     float* o = slot + 7 * (size_t)i;
     o[0] = r[0] - cx; o[1] = r[1] - cy;
     for (int c = 2; c < 7; c++) o[c] = r[c];
@@ -1272,7 +1275,7 @@ FB_DEV void ktask_reset_ref(const DevModel& m, const DevData& d, const DevTask& 
     if (t.ghost_qadr >= 0) AT(d.qpos, t.ghost_qadr + y) = r + (y < 3 ? t.ghost_offset[y] : 0.0f);
   }
   if (y == 0) {
-    for (int i = 0; i < 3; i++) AT(d.qvel, t.root_vadr + i) = b0[7 + i];
+    if (t.kind == 1) for (int i = 0; i < 3; i++) AT(d.qvel, t.root_vadr + i) = b0[7 + i];      // (walking starts at rest)
     const int rows = n < t.max_episode_rows ? n : t.max_episode_rows;
     t.ep_traj[e] = traj; t.ep_start[e] = start; t.ep_row0[e] = row0; t.ep_n[e] = n; t.ep_steps[e] = rows - (t.future_steps + 1);
   }
@@ -1294,7 +1297,6 @@ FB_DEV void ktask_reset2(const DevModel& m, const DevData& d, int e, int y) {   
   if (t.kind == 2) { ktask_reset_vision(m, d, t, e, y, episode); return; }
   if (t.ref_bank) ktask_reset_ref(m, d, t, e, y, episode);
   else if (y < 7) { float r = t.ref_qpos[y]; AT(d.qpos, t.root_qadr + y) = r; if (t.ghost_qadr >= 0) AT(d.qpos, t.ghost_qadr + y) = r + (y < 3 ? t.ghost_offset[y] : 0.0f); }
-  for (int i = y; i < t.n_noise; i += FB_NY) AT(d.qpos, t.noise_qadr[i]) += t.noise_amp * (2.0f * tk_u01(t, e, episode, 1 + i) - 1.0f);
   if (y == 0) {
     if (t.kind == 1) {          // wings on the beat pattern of the base frequency at a random phase, root at the reference speed
       float phase = t.has_uniform[e] ? t.uniform[8 * e] : tk_u01(t, e, episode, 0);
@@ -1310,6 +1312,31 @@ FB_DEV void ktask_reset2(const DevModel& m, const DevData& d, int e, int y) {   
     t.step[e] = 0; t.has_uniform[e] = 0;          // (the episode counter, read by every lane above, advances in ktask_before)
   }
 }
+// The later writes of a reset each take a phase of their own, after the write they build on: the dataset's joint list may include the
+// wings, and the noise joints are among its joints, so different lanes write and add to the same qpos entries (walk_imitation.py:112-136).
+// walking with a dataset: the mocap joints at row `start` of the snippet (the full-body start pose, walk_imitation.py:117-118)
+FB_DEV void ktask_reset3(const DevModel& m, const DevData& d, int e, int y) {
+  if (!d.task || e >= d.N) return;
+  const DevTask& t = *d.task;
+  if (t.kind != 0 || !t.ref_bank || !t.needs_reset[e]) return;
+  const float* b0 = t.rbank + (size_t)t.rbank_w * t.ep_row0[e] + 15;
+  for (int i = y; i < t.n_mjnt; i += FB_NY) AT(d.qpos, t.mocap_qadr[i]) = b0[i];
+}
+// ... then the wings back at their spring references (walk_imitation.py:119-121)
+FB_DEV void ktask_reset4(const DevModel& m, const DevData& d, int e, int y) {
+  if (!d.task || e >= d.N) return;
+  const DevTask& t = *d.task;
+  if (t.kind != 0 || !t.ref_bank || !t.needs_reset[e]) return;
+  for (int i = y; i < t.n_wing; i += FB_NY) AT(d.qpos, t.wing_qadr[i]) = t.wing_spring[i];
+}
+// ... then the optional U(-a, a) noise on the listed joints
+FB_DEV void ktask_reset5(const DevModel& m, const DevData& d, int e, int y) {
+  if (!d.task || e >= d.N) return;
+  const DevTask& t = *d.task;
+  if (t.kind == 2 || !t.needs_reset[e]) return;
+  const int episode = t.episode[e];
+  for (int i = y; i < t.n_noise; i += FB_NY) AT(d.qpos, t.noise_qadr[i]) += t.noise_amp * (2.0f * tk_u01(t, e, episode, 1 + i) - 1.0f);
+}
 FB_DEV void ktask_before(const DevModel& m, const DevData& d, int e, int y) {
   if (!d.task || e >= d.N) return;
   const DevTask& t = *d.task;
@@ -1320,7 +1347,7 @@ FB_DEV void ktask_before(const DevModel& m, const DevData& d, int e, int y) {
   if (step > last) step = last;
   if (t.ghost_qadr >= 0) {
     const float* rq = t.ref_bank ? t.slots + ((size_t)e * t.slot_len + step) * 7 : t.ref_qpos + 7 * step;
-    const float* rv = t.ref_bank ? t.rbank + (size_t)FB_RBANK_W * (t.ep_row0[e] + step) + 7 : t.ref_qvel + 6 * step;
+    const float* rv = t.ref_bank ? t.rbank + (size_t)t.rbank_w * (t.ep_row0[e] + step) + 7 : t.ref_qvel + 6 * step;
     if (y < 7) AT(d.qpos, t.ghost_qadr + y) = rq[y] + (y < 3 ? t.ghost_offset[y] : 0.0f);
     else if (y < 13) AT(d.qvel, t.ghost_vadr + y - 7) = resetting ? 0.0f : rv[y - 7];
   }
@@ -1353,6 +1380,73 @@ FB_DEV void ktask_commit(const DevModel& m, const DevData& d, int e, int y) {
   t.op_step[e] = t.step[e]; t.op_first[e] = (unsigned char)resetting;
 }
 FB_DEV float tk_lin_tol(float x, float margin) { float v = 1.0f - fabsf(x) / margin; return v < 0.0f ? 0.0f : (v > 1.0f ? 1.0f : v); }
+// quaternions.py:215-333 restated in fp32: quat_z2vec with its exact-zero edge cases (vec = (0, 0, z): identity, or the half turn about x
+// for z < 0), axis_angle_to_quat, joint_orientation_quat and the short-arc distance acos(min(1, 2 (p.q)^2 - 1)) of normalised quaternions
+FB_DEV Q4 tk_quat_z2vec(V3 v) {
+  if (v.x == 0.0f && v.y == 0.0f) return v.z < 0.0f ? q4(0.0f, 1.0f, 0.0f, 0.0f) : q4(1.0f, 0.0f, 0.0f, 0.0f);
+  const float n = sqrtf(v.x * v.x + v.y * v.y + v.z * v.z);
+  const float ux = v.x / n, uy = v.y / n, uz = v.z / n, an = sqrtf(uy * uy + ux * ux);
+  const float h = 0.5f * acosf(uz > 1.0f ? 1.0f : (uz < -1.0f ? -1.0f : uz)), s = sinf(h);      // (|uz| > 1 only by rounding)
+  return q4(cosf(h), s * (-uy / an), s * (ux / an), 0.0f);
+}
+FB_DEV Q4 tk_axis_angle_quat(V3 a, float angle) {
+  const float n = sqrtf(a.x * a.x + a.y * a.y + a.z * a.z), h = 0.5f * angle, s = sinf(h);
+  return q4(cosf(h), s * (a.x / n), s * (a.y / n), s * (a.z / n));
+}
+FB_DEV Q4 tk_joint_quat(V3 axis, float qpos) { return qmul(tk_axis_angle_quat(axis, qpos), tk_quat_z2vec(axis)); }
+FB_DEV float tk_quat_dist(Q4 p, Q4 q) {
+  const float np_ = sqrtf(p.w * p.w + p.x * p.x + p.y * p.y + p.z * p.z), nq = sqrtf(q.w * q.w + q.x * q.x + q.y * q.y + q.z * q.z);
+  const float c = (p.w / np_) * (q.w / nq) + (p.x / np_) * (q.x / nq) + (p.y / np_) * (q.y / nq) + (p.z / np_) * (q.z / nq);
+  const float x = 2.0f * c * c - 1.0f;
+  return acosf(x < 1.0f ? x : 1.0f);
+}
+// walking with a dataset: the bank row of the reference features at the env's step (rewards.py:66-83: the row of step min(step, n - 1))
+FB_DEV const float* tk_walk_ref_row(const DevTask& t, int e) {
+  const int s = t.step[e], last = t.ep_n[e] - 1;
+  return t.rbank + (size_t)t.rbank_w * (t.ep_row0[e] + (s < last ? s : last));
+}
+// ... the DeepMimic terms over the dataset's joints and sites, lanes over joints / sites (rewards.py:10-63): squared mocap qvel errors,
+// squared end-effector (root2site) errors, squared short-arc angles between the joint orientations; per-lane sums to rw_part
+FB_DEV void ktask_reward(const DevModel& m, const DevData& d, int e, int y) {
+  if (!d.task || !d.tobs || e >= d.N) return;
+  const DevTask& t = *d.task;
+  if (t.kind != 0 || !t.ref_bank) return;
+  const float* o = d.tobs + (size_t)e * d.tobs_dim;
+  const int nj = t.n_mjnt, ns = t.n_msite;
+  const float* rqv = tk_walk_ref_row(t, e) + 15 + nj;
+  const float* rsite = rqv + nj;
+  const float* rjq = rsite + 3 * ns;
+  float sv = 0.0f, ss = 0.0f, sq = 0.0f;
+  for (int i = y; i < nj; i += FB_NY) {
+    const float dv = o[t.obs_mocap_qvel_off + i] - rqv[i];
+    sv += dv * dv;
+    const float* a = o + t.obs_mocap_axes_off + 3 * i;
+    const float ang = tk_quat_dist(tk_joint_quat(v3(a[0], a[1], a[2]), o[t.obs_mocap_qpos_off + i]), q4(rjq[4 * i], rjq[4 * i + 1], rjq[4 * i + 2], rjq[4 * i + 3]));
+    sq += ang * ang;
+  }
+  for (int i = y; i < 3 * ns; i += FB_NY) { const float ds = o[t.obs_mocap_sites_off + i] - rsite[i]; ss += ds * ds; }
+  float* p = t.rw_part + ((size_t)e * FB_NY + y) * 3;
+  p[0] = sv; p[1] = ss; p[2] = sq;
+}
+// ... and on lane 0: the root terms, the lanes' sums in lane order, the product of the four DeepMimic factors (weights 20, 1, 1, 1) and the
+// six wing-retraction factors (walk_imitation.py:152-177).  The CoM feature is the snippet's root position shifted as the loader shifts it.
+FB_DEV float tk_walk_reward(const DevTask& t, int e, const float* o) {
+  const float* r = tk_walk_ref_row(t, e);
+  const float* b0 = t.rbank + (size_t)t.rbank_w * t.ep_row0[e];
+  const float* rp = o + t.obs_root_pose_off;
+  const float* rv = o + t.obs_root_qvel_off;
+  const float c0 = rp[0] - (r[0] - b0[13]), c1 = rp[1] - (r[1] - b0[14]), c2 = rp[2] - r[2];
+  const float d_com = c0 * c0 + c1 * c1 + c2 * c2;
+  float d_qvel = 0.0f, d_site = 0.0f;
+  for (int k = 0; k < 6; k++) { const float dv = rv[k] - r[7 + k]; d_qvel += dv * dv; }
+  const float a = tk_quat_dist(q4(rp[3], rp[4], rp[5], rp[6]), q4(r[3], r[4], r[5], r[6]));
+  float d_quat = a * a;
+  for (int l = 0; l < FB_NY; l++) { const float* p = t.rw_part + ((size_t)e * FB_NY + l) * 3; d_qvel += p[0]; d_site += p[1]; d_quat += p[2]; }
+  auto factor = [&](int k, float diff) { return expf(-0.5f / (t.dm_std[k] * t.dm_std[k]) * diff) * t.dm_weight[k]; };
+  float reward = factor(0, d_com) * factor(1, d_qvel) * factor(2, d_site) * factor(3, d_quat);
+  for (int i = 0; i < t.n_wing; i++) reward *= tk_lin_tol(o[t.obs_wing_qpos_off + i] - t.wing_spring[i], t.retract_margin);
+  return reward;
+}
 FB_DEV void ktask_after(const DevModel& m, const DevData& d, int e, int y) {
   if (!d.task || !d.tobs || e >= d.N || y != 0) return;
   const DevTask& t = *d.task;
@@ -1400,7 +1494,7 @@ FB_DEV void ktask_after(const DevModel& m, const DevData& d, int e, int y) {
     const float* lv = &AT(d.sensordata, t.velocimeter_adr); const float* av = &AT(d.sensordata, t.gyro_adr);
     float linvel = sqrtf(lv[0] * lv[0] + lv[1] * lv[1] + lv[2] * lv[2]), angvel = sqrtf(av[0] * av[0] + av[1] * av[1] + av[2] * av[2]);
     terminate = linvel > t.term_linvel || angvel > t.term_angvel || reached_end || com_dist > t.term_com || bad;
-    reward = 1.0f;                                   // inference mode: reward factors == (1,)
+    reward = t.ref_bank ? tk_walk_reward(t, e, o) : 1.0f;      // inference mode: reward factors == (1,)
   } else {
     const float height = AT(d.qpos, t.root_qadr + 2);
     terminate = height < t.term_height || com_dist > t.term_com || reached_end || bad;

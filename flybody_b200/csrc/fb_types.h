@@ -162,9 +162,9 @@ struct DevData {
 
 // Device-side task logic (fb_task_program): what the reference's task hooks do around the physics step -- auto-reset,
 // ghost placement, wing-beat pattern generator, termination, reward, discount -- for the shared-reference (inference)
-// form of walk_imitation / flight_imitation, and for flight_imitation with a trajectory dataset (ref_bank).  Lives in device
-// memory; DevData::task points at it.
-#define FB_RBANK_W 15                      // bank row: root qpos 7, CoM qvel 6, CoM x, y 2
+// form of walk_imitation / flight_imitation, and for both with a trajectory dataset (ref_bank).  Lives in device memory;
+// DevData::task points at it.
+#define FB_RBANK_W 15                      // flight bank row: root qpos 7, CoM qvel 6, CoM x, y 2 (the first 15 columns of every bank row)
 struct DevTask {
   int kind;                                // 0 walk_imitation, 1 flight_imitation, 2 vision_guided_flight
   int root_qadr, root_vadr, ghost_qadr, ghost_vadr, root_body, user_col /* action column of the beat-frequency action, -1: none */;
@@ -181,11 +181,17 @@ struct DevTask {
   const float *bank, *bank_hmax, *bank_cmax; float *hf_data, *hf_hmax, *hf_cmax;
   float* target;                           // [N][2] target height, target speed of the running episode
   int trench_cap; const float *trench_x, *trench_y; const int* trench_len; int* pick;   // 'trench' arenas: centre line per bank terrain; the env's terrain
-  // kind 1 with ref_bank (flight dataset): trajectory bank [rows][FB_RBANK_W] (fb_ref_bank), picks, the env's reference slot
-  int ref_bank, n_traj, n_pick, randomize_start, start_margin, max_episode_rows, future_steps, slot_len;
+  // kind 0 / 1 with ref_bank (dataset): trajectory bank [rows][rbank_w] (fb_ref_bank / fb_ref_bank_wide), picks, the env's reference slot
+  int ref_bank, n_traj, n_pick, randomize_start, start_margin, max_episode_rows, future_steps, slot_len, rbank_w;
   const float* rbank; const int *traj_off, *traj_len, *pick_traj; float* slots /* [N][slot_len][7] */;
   int *ep_traj, *ep_start, *ep_row0, *ep_n;   // the running episode: trajectory, start step, bank row of its row 0, rows in use
   int* pin;                                // [N][3] has pin, trajectory, start step of the next reset (fb_task_ref_pick)
+  // kind 0 with ref_bank (walking dataset): the dataset's joints / sites, the observation columns of the walker features, the DeepMimic
+  // reward's constants; bank row after the 15 root columns: mocap qpos [nj], mocap qvel [nj], root2site [ns][3], joint_quat [nj][4]
+  int n_mjnt, n_msite; const int* mocap_qadr; const float* wing_spring;
+  int obs_root_pose_off, obs_root_qvel_off, obs_mocap_qpos_off, obs_mocap_qvel_off, obs_mocap_axes_off, obs_mocap_sites_off, obs_wing_qpos_off;
+  float dm_std[4], dm_weight[4], retract_margin;
+  float* rw_part;                          // [N][FB_NY][3] per-lane partial sums of the joint / site terms of the reward (ktask_reward)
   // per-env state
   int *step, *needs_reset, *resetting, *episode, *ep_steps /* step index that ends the episode */, *wb_idx, *wb_pos, *has_uniform;
   float *uniform /* [N][8] */, *wb_freq;

@@ -68,7 +68,7 @@ struct FbSim {
   int blob_in_smem;            // copy the sweep program of the triangular solves into shared memory per CTA (default: for batches <= 1024 envs; FB_BLOB=0/1 overrides)
   int* op_step_dev; unsigned char* op_first_dev;
   float* ref_slots; int ref_slot_len;      // per-env reference tables (fb_ref_slots)
-  float* rbank_dev; int *rbank_off_dev, *rbank_len_dev; std::vector<int> rbank_len; std::vector<void*> rbank_scope;   // flight trajectory bank (fb_ref_bank)
+  float* rbank_dev; int *rbank_off_dev, *rbank_len_dev, rbank_w; std::vector<int> rbank_len; std::vector<void*> rbank_scope;   // trajectory bank (fb_ref_bank_wide)
   DevHf hf; bool hf_on; int hf_nrow, hf_ncol;      // heightfield collision (fb_hfield_collision)
   float *bank_dev, *bank_hmax_dev, *bank_cmax_dev; int bank_n;      // terrain bank of the device-side vision task (fb_hfield_bank)
   DevEye eye; float* hfield_dev; float* hmax_dev; float* cmax_dev; int hf_nbr, hf_nbc; unsigned char* eye_out; size_t eye_bytes;   // eye cameras (fb_eye_program)
@@ -237,6 +237,10 @@ static void launch_hfield(FbSim* s) {
 }
 FB_DEV void ph_task_reset(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset(m, d, e, y); }
 FB_DEV void ph_task_reset2(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset2(m, d, e, y); }
+FB_DEV void ph_task_reset3(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset3(m, d, e, y); }
+FB_DEV void ph_task_reset4(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset4(m, d, e, y); }
+FB_DEV void ph_task_reset5(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset5(m, d, e, y); }
+FB_DEV void ph_task_reward(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reward(m, d, e, y); }
 FB_DEV void ph_task_before(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_before(m, d, e, y); }
 FB_DEV void ph_task_commit(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_commit(m, d, e, y); }
 FB_DEV void ph_task_after(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_after(m, d, e, y); }
@@ -658,7 +662,7 @@ int fb_create(const FbModel* hm, int n_envs, int device, FbHandle* out) {
   FbSim* s = new FbSim();
   s->device = device; s->launches = 0; s->last_ms = 0; s->hm = *hm; s->first_substep = 1; s->hold_pending = 0; s->prof_on = 0; memset(s->prof_ms, 0, sizeof(s->prof_ms)); memset(s->prof_n, 0, sizeof(s->prof_n));
   s->ref_slots = nullptr; s->ref_slot_len = 0; s->eye_out = nullptr; s->hfield_dev = nullptr; s->hmax_dev = nullptr; s->cmax_dev = nullptr; s->hf_nbr = s->hf_nbc = 0; s->bank_dev = s->bank_hmax_dev = s->bank_cmax_dev = nullptr; s->bank_n = 0; s->eye_bytes = 0; s->hf_on = false; s->hf_nrow = s->hf_ncol = 0;
-  s->rbank_dev = nullptr; s->rbank_off_dev = s->rbank_len_dev = nullptr;
+  s->rbank_dev = nullptr; s->rbank_off_dev = s->rbank_len_dev = nullptr; s->rbank_w = 0;
   s->op_step_dev = nullptr; s->op_first_dev = nullptr; s->stage_cap = 0; s->stage_icap = 0; s->stage = nullptr; s->stage_i = nullptr;
 #ifndef FB_EMU
   if (cudaSetDevice(device) != cudaSuccess) { delete s; return -2; }
@@ -1142,19 +1146,37 @@ int fb_ref_slot_write(FbHandle s, const int32_t* env_ids, int n, const float* ro
 int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   if (!s || !p) return -1;
   if (!s->d.tobs || !s->act_map_dev) { s->err = "fb_task_program: call fb_set_action_map and fb_obs_program first"; return -1; }
-  const bool bank = p->kind == 1 && p->ref_bank;
-  if (p->ref_bank && p->kind != 1) { s->err = "fb_task_program: ref_bank is for kind 1 (flight_imitation)"; return -1; }
+  const bool bank = (p->kind == 0 || p->kind == 1) && p->ref_bank;
+  if (p->ref_bank && !bank) { s->err = "fb_task_program: ref_bank is for kind 0 / 1 (walk_imitation / flight_imitation)"; return -1; }
   if (s->d.op_ref_slot && !bank) { s->err = "fb_task_program: per-env reference slots keep the host-side task code"; return -1; }
   if (bank) {
     if (!s->d.op_ref_slot || !s->ref_slots || s->ref_slot_len < 1) { s->err = "fb_task_program: ref_bank needs the per-env reference slots (fb_ref_slots) first"; return -1; }
-    if (!s->rbank_dev) { s->err = "fb_task_program: ref_bank needs a trajectory bank (fb_ref_bank) first"; return -1; }
+    if (!s->rbank_dev) { s->err = "fb_task_program: ref_bank needs a trajectory bank (fb_ref_bank / fb_ref_bank_wide) first"; return -1; }
     if (p->n_pick <= 0 || !p->pick_traj) { s->err = "fb_task_program: ref_bank needs the trajectory indices to draw from (n_pick, pick_traj)"; return -1; }
     if (p->start_margin < 0 || p->max_episode_rows < 1 || p->future_steps < 0) { s->err = "fb_task_program: bad start_margin / max_episode_rows / future_steps"; return -1; }
+    if (p->kind == 0 && p->randomize_start) { s->err = "fb_task_program: walking starts every snippet at row 0 (randomize_start must be 0)"; return -1; }
     for (int k = 0; k < p->n_pick; k++) {
       const int j = p->pick_traj[k];
       if (j < 0 || j >= (int)s->rbank_len.size()) { s->err = "fb_task_program: trajectory index of pick_traj out of range of the bank"; return -1; }
       if (p->randomize_start && s->rbank_len[j] <= p->start_margin) {
         s->err = "fb_task_program: with randomize_start every trajectory to draw from must be longer than start_margin rows"; return -1; }
+      if (p->kind == 0 && s->rbank_len[j] <= p->future_steps + 1) {
+        s->err = "fb_task_program: every walking trajectory to draw from must be longer than future_steps + 1 rows"; return -1; }
+    }
+    if (p->kind == 0) {          // the walking reward: the dataset's joints / sites in the bank rows and the walker's in the observation row
+      const int nj = p->n_mocap_joints, ns = p->n_mocap_sites, dim = s->d.tobs_dim;
+      if (nj <= 0 || ns < 0 || !p->mocap_qadr) { s->err = "fb_task_program: a kind 0 ref_bank program needs the dataset's joints (n_mocap_joints, mocap_qadr)"; return -1; }
+      for (int i = 0; i < nj; i++) if (p->mocap_qadr[i] < 0 || p->mocap_qadr[i] >= s->m.nq) { s->err = "fb_task_program: mocap_qadr entry out of range"; return -1; }
+      if ((size_t)s->rbank_w != (size_t)FB_RBANK_W + 6 * (size_t)nj + 3 * (size_t)ns) {
+        s->err = "fb_task_program: the bank rows are not 15 + 6 n_mocap_joints + 3 n_mocap_sites wide (fb_ref_bank_wide)"; return -1; }
+      const int off[7] = {p->obs_root_pose_off, p->obs_root_qvel_off, p->obs_mocap_qpos_off, p->obs_mocap_qvel_off, p->obs_mocap_axes_off, p->obs_mocap_sites_off, p->obs_wing_qpos_off};
+      const int wid[7] = {7, 6, nj, nj, 3 * nj, 3 * ns, p->n_wing};
+      for (int k = 0; k < 7; k++) if (off[k] < 1 || off[k] + wid[k] > dim) {
+        s->err = "fb_task_program: a kind 0 ref_bank program needs the observation columns of the walker features (obs_*_off)"; return -1; }
+      if (p->n_wing <= 0 || !p->wing_qadr || !p->wing_spring) { s->err = "fb_task_program: a kind 0 ref_bank program needs the wing joints and their springs"; return -1; }
+      for (int i = 0; i < p->n_wing; i++) if (p->wing_qadr[i] < 0 || p->wing_qadr[i] >= s->m.nq) { s->err = "fb_task_program: wing_qadr entry out of range"; return -1; }
+      for (int k = 0; k < 4; k++) if (!(p->deep_mimic_std[k] > 0)) { s->err = "fb_task_program: deep_mimic_std must be positive"; return -1; }
+      if (!(p->retract_margin > 0)) { s->err = "fb_task_program: retract_margin must be positive"; return -1; }
     }
   } else if (p->ref_len <= 0 || !p->ref_qpos || !p->ref_qvel) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
   if (!p->reset_qpos) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
@@ -1190,10 +1212,20 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   t.uniform = dalloc<float>(s, (size_t)8 * Np); t.wb_freq = dalloc<float>(s, Np); t.out = dalloc<float>(s, (size_t)4 * Np);
   t.ep_steps = dalloc<int>(s, Np);
   if (bank) {          // episode lengths are set per env by each reset
-    t.ref_bank = 1; t.n_traj = (int)s->rbank_len.size(); t.rbank = s->rbank_dev; t.traj_off = s->rbank_off_dev; t.traj_len = s->rbank_len_dev;
+    t.ref_bank = 1; t.n_traj = (int)s->rbank_len.size(); t.rbank = s->rbank_dev; t.traj_off = s->rbank_off_dev; t.traj_len = s->rbank_len_dev; t.rbank_w = s->rbank_w;
     t.n_pick = p->n_pick; t.pick_traj = upi32(p->pick_traj, p->n_pick); t.randomize_start = p->randomize_start ? 1 : 0; t.start_margin = p->start_margin;
     t.max_episode_rows = p->max_episode_rows; t.future_steps = p->future_steps; t.slots = s->ref_slots; t.slot_len = s->ref_slot_len;
     t.ep_traj = dalloc<int>(s, Np); t.ep_start = dalloc<int>(s, Np); t.ep_row0 = dalloc<int>(s, Np); t.ep_n = dalloc<int>(s, Np); t.pin = dalloc<int>(s, (size_t)3 * Np);
+    if (p->kind == 0) {
+      t.n_mjnt = p->n_mocap_joints; t.n_msite = p->n_mocap_sites; t.mocap_qadr = upi32(p->mocap_qadr, p->n_mocap_joints);
+      t.n_wing = p->n_wing; t.wing_qadr = upi32(p->wing_qadr, p->n_wing); t.wing_spring = upf32(p->wing_spring, p->n_wing);
+      t.obs_root_pose_off = p->obs_root_pose_off; t.obs_root_qvel_off = p->obs_root_qvel_off; t.obs_mocap_qpos_off = p->obs_mocap_qpos_off;
+      t.obs_mocap_qvel_off = p->obs_mocap_qvel_off; t.obs_mocap_axes_off = p->obs_mocap_axes_off; t.obs_mocap_sites_off = p->obs_mocap_sites_off;
+      t.obs_wing_qpos_off = p->obs_wing_qpos_off;
+      for (int k = 0; k < 4; k++) { t.dm_std[k] = p->deep_mimic_std[k]; t.dm_weight[k] = p->deep_mimic_weight[k]; }
+      t.retract_margin = p->retract_margin;
+      t.rw_part = dalloc<float>(s, (size_t)Np * FB_NY * 3);
+    }
   } else {
     std::vector<int> steps((size_t)Np, p->episode_steps);
     h2d(t.ep_steps, steps.data(), sizeof(int) * steps.size());
@@ -1301,32 +1333,41 @@ int fb_hfield_bank(FbHandle s, int n_terrain, const float* heights) {
   s->bank_n = n_terrain;
   return 0;
 }
-int fb_ref_bank(FbHandle s, int n_traj, const int32_t* traj_len, const float* rows) {
+int fb_ref_bank(FbHandle s, int n_traj, const int32_t* traj_len, const float* rows) { return fb_ref_bank_wide(s, n_traj, traj_len, FB_RBANK_W, rows); }
+int fb_ref_bank_wide(FbHandle s, int n_traj, const int32_t* traj_len, int row_width, const float* rows) {
   if (!s) return -1;
   if (n_traj <= 0 || !traj_len || !rows) { s->err = "fb_ref_bank: no trajectories"; return -1; }
+  if (row_width < FB_RBANK_W) { s->err = "fb_ref_bank_wide: rows narrower than the 15 root columns"; return -1; }
   std::vector<int> off(n_traj), len(traj_len, traj_len + n_traj);
   size_t total = 0;
   for (int k = 0; k < n_traj; k++) {
     if (len[k] < 1) { s->err = "fb_ref_bank: empty trajectory"; return -1; }
+    if (total > (size_t)INT32_MAX - (size_t)len[k]) { s->err = "fb_ref_bank: bank too large: more than 2^31 - 1 rows (int32 row index)"; return -1; }
     off[k] = (int)total; total += (size_t)len[k];
   }
-  if (total > (size_t)INT32_MAX / FB_RBANK_W) { s->err = "fb_ref_bank: bank too large"; return -1; }
+  const size_t bytes = sizeof(float) * total * (size_t)row_width;      // (rows < 2^31, width < 2^31: no size_t overflow)
+#ifndef FB_EMU
+  size_t free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && bytes > free_b) {
+    s->err = "fb_ref_bank: bank too large for the device's free memory"; return -4; }
+#endif
   if (sync_stream(s) != 0) return -2;
-  if (s->rbank_dev) {      // a replaced bank is freed; a flight program drawing from it has to be uploaded again
+  if (s->rbank_dev) {      // a replaced bank is freed; a dataset program drawing from it has to be uploaded again
     scope_free(s, s->rbank_scope);
     if (s->d.task && s->task_host.ref_bank) { scope_free(s, s->task_scope); s->d.task = nullptr; }
   }
   const size_t mark = s->allocs.size();
-  s->rbank_dev = dalloc<float>(s, total * FB_RBANK_W); s->rbank_off_dev = dalloc<int>(s, n_traj); s->rbank_len_dev = dalloc<int>(s, n_traj);
+  s->rbank_dev = dalloc<float>(s, total * (size_t)row_width); s->rbank_off_dev = dalloc<int>(s, n_traj); s->rbank_len_dev = dalloc<int>(s, n_traj);
   s->rbank_scope.assign(s->allocs.begin() + mark, s->allocs.end());
-  if (!s->rbank_dev || !s->rbank_off_dev || !s->rbank_len_dev) { scope_free(s, s->rbank_scope); s->rbank_dev = nullptr; s->rbank_len.clear(); s->err = "out of device memory (trajectory bank)"; return -4; }
-  h2d(s->rbank_dev, rows, sizeof(float) * total * FB_RBANK_W); h2d(s->rbank_off_dev, off.data(), sizeof(int) * n_traj); h2d(s->rbank_len_dev, len.data(), sizeof(int) * n_traj);
-  s->rbank_len = len;
+  if (!s->rbank_dev || !s->rbank_off_dev || !s->rbank_len_dev) {
+    scope_free(s, s->rbank_scope); s->rbank_dev = nullptr; s->rbank_len.clear(); s->rbank_w = 0; s->err = "out of device memory (trajectory bank)"; return -4; }
+  h2d(s->rbank_dev, rows, bytes); h2d(s->rbank_off_dev, off.data(), sizeof(int) * n_traj); h2d(s->rbank_len_dev, len.data(), sizeof(int) * n_traj);
+  s->rbank_len = len; s->rbank_w = row_width;
   return 0;
 }
 int fb_task_ref_pick(FbHandle s, const int32_t* env_ids, int n, const int32_t* traj, const int32_t* start) {
   if (!s || n < 0 || (n > 0 && (!env_ids || !traj || !start))) return -1;
-  if (!s->d.task || !s->task_host.ref_bank) { s->err = "fb_task_ref_pick: needs a kind 1 task program with ref_bank"; return -1; }
+  if (!s->d.task || !s->task_host.ref_bank) { s->err = "fb_task_ref_pick: needs a task program with ref_bank"; return -1; }
   std::vector<int> pins((size_t)3 * n);
   for (int k = 0; k < n; k++) {
     if (env_ids[k] < 0 || env_ids[k] >= s->d.N) { s->err = "fb_task_ref_pick: env id out of range"; return -1; }
@@ -1340,7 +1381,7 @@ int fb_task_ref_pick(FbHandle s, const int32_t* env_ids, int n, const int32_t* t
 }
 int fb_task_ref_state(FbHandle s, int32_t* traj, int32_t* start) {
   if (!s || !traj || !start) return -1;
-  if (!s->d.task || !s->task_host.ref_bank) { s->err = "fb_task_ref_state: needs a kind 1 task program with ref_bank"; return -1; }
+  if (!s->d.task || !s->task_host.ref_bank) { s->err = "fb_task_ref_state: needs a task program with ref_bank"; return -1; }
   if (sync_stream(s) != 0) return -2;
   d2h(traj, s->task_host.ep_traj, sizeof(int) * (size_t)s->d.N);
   d2h(start, s->task_host.ep_start, sizeof(int) * (size_t)s->d.N);
@@ -1351,14 +1392,14 @@ int fb_task_step(FbHandle s, const float* action, int is_device, int n_substeps)
 #ifndef FB_EMU
   cudaSetDevice(s->device);
 #endif
-  fb_launch<ShNone, Ph<ph_task_reset>, Ph<ph_task_reset2>>(s, K_MISC, 0, s->d.N);      // envs whose last step was LAST
+  fb_launch<ShNone, Ph<ph_task_reset>, Ph<ph_task_reset2>, Ph<ph_task_reset3>, Ph<ph_task_reset4>, Ph<ph_task_reset5>>(s, K_MISC, 0, s->d.N);      // envs whose last step was LAST
   int rc = fb_set_ctrl(s, action, is_device);                                           // action -> ctrl (NaN -> 0), staged rows stay readable
   if (rc != 0) return rc;
   fb_launch<ShNone, Ph<ph_task_before>, Ph<ph_task_commit>>(s, K_MISC, 0, s->d.N);
   s->hold_pending = 1;                                                                  // freshly reset envs are held through this step
   rc = fb_step(s, n_substeps);
   if (rc != 0) return rc;
-  fb_launch<ShNone, Ph<ph_pack>, Ph<ph_task_after>>(s, K_PACK, 0, s->d.N);
+  fb_launch<ShNone, Ph<ph_pack>, Ph<ph_task_reward>, Ph<ph_task_after>>(s, K_PACK, 0, s->d.N);
   return 0;
 }
 int fb_task_ptrs(FbHandle s, void** obs_dev, int* obs_dim, void** out_dev) {

@@ -104,6 +104,10 @@ class BatchedWingBeatPatternGenerator:
 
 
 
+_WALK_REWARD_WEIGHTS = (20, 1, 1, 1)            # DeepMimic factor weights of walk_imitation (walk_imitation.py:152-177)
+_WING_RETRACT_MARGIN = 3.0                      # ... and the margin of its wing-retraction factors
+
+
 class _FeatureBank:
     """Full-body reference features of the walking snippets in use, concatenated row-wise (append-only, cached by
     trajectory index) so that the per-env reward gathers are single fancy-index reads."""
@@ -302,12 +306,22 @@ class BatchedFlyEnv:
         self._bank_rows = None                           # ... and the dataset as uploaded by fb_ref_bank (_bank_tables)
         # full-body imitation reward (reference walk_imitation.py:152-177): mocap joints / sites named by the dataset
         self._inference_mode = bool(inference_mode) or variant != 'walk'
-        # flight with a trajectory dataset on the device: the whole dataset in a device bank, every reset cuts its own reference from it
-        self._device_bank = self._device_task and self._per_env_ref and isinstance(tg, HDF5FlightTrajectoryLoader)
+        # a trajectory dataset on the device: the whole dataset in a device bank, every reset cuts its own reference from it
+        self._device_bank = self._device_task and self._per_env_ref and isinstance(tg, (HDF5FlightTrajectoryLoader, HDF5WalkingTrajectoryLoader))
         if self._device_task and not self._device_bank and (self._per_env_ref or not self._inference_mode):
-            raise NotImplementedError('device_task covers the shared-reference (inference-mode) tasks and flight_imitation with a '
-                                      'trajectory dataset; dataset-mode walk_imitation keeps the host-side task code')
-        if self._device_bank and tg.randomize_start_step:
+            raise NotImplementedError('device_task covers the shared-reference (inference-mode) tasks and the HDF5 trajectory datasets of '
+                                      'walk_imitation / flight_imitation')
+        if self._device_bank and variant == 'walk':
+            if not tg.get_joint_names():
+                raise NotImplementedError('walk_imitation(device_task=True) needs a dataset that lists its mocap joints: the DeepMimic '
+                                          'reward on the device compares them')
+            short = [int(j) for j in np.unique(tg.traj_indices) if tg.trajectory_len(j) <= future_steps + 1]
+            if short:
+                raise NotImplementedError(f'trajectories {short} have at most future_steps + 1 = {future_steps + 1} rows '
+                                          f'({[tg.trajectory_len(j) for j in short]}): such snippets, which the host-side task code pads '
+                                          'with their last row and the reference cannot index past, are not run on the device; use '
+                                          'device_task=False or leave them out of traj_indices')
+        if self._device_bank and variant == 'flight' and tg.randomize_start_step:
             short = [int(j) for j in np.unique(tg.traj_indices) if tg.trajectory_len(j) <= tg.START_MARGIN]
             if short:
                 raise ValueError(f'randomize_start_step needs trajectories longer than {tg.START_MARGIN} rows; trajectories {short} have '
@@ -437,12 +451,24 @@ class BatchedFlyEnv:
                   reset_qpos=q0, n_noise=len(self._leg_act_qadr) if (self._variant == 'walk' and self._reset_noise > 0) else 0,
                   noise_qadr=self._leg_act_qadr if (self._variant == 'walk' and self._reset_noise > 0) else None,
                   noise_amp=self._reset_noise, seed=int(self._seed) & 0xffffffff, com_offset=_COM_OFFSET)
-        if self._device_bank:                    # the draws of _load_snippet / HDF5FlightTrajectoryLoader.get_trajectory, on the device
+        if self._device_bank and self._variant == 'flight':      # the draws of _load_snippet / HDF5FlightTrajectoryLoader.get_trajectory
             tg = t._traj_generator
             self._sim.ref_bank(*self._bank_tables())
             kw.update(ref_bank=1, n_pick=len(tg.traj_indices), pick_traj=np.asarray(tg.traj_indices, np.int64),
                       randomize_start=int(bool(tg.randomize_start_step)), start_margin=tg.START_MARGIN,
                       max_episode_rows=round(self._time_limit / self._control_timestep), future_steps=t._future_steps)
+        elif self._device_bank:                  # walking: the draws of _load_snippet, the full-body start pose and the DeepMimic reward
+            tg = t._traj_generator
+            self._sim.ref_bank_wide(*self._bank_tables())
+            kw.update(ref_bank=1, n_pick=len(tg.traj_indices), pick_traj=np.asarray(tg.traj_indices, np.int64), randomize_start=0,
+                      start_margin=0, max_episode_rows=t._max_episode_steps + t._future_steps + 1, future_steps=t._future_steps,
+                      n_mocap_joints=len(self._mocap_qadr), mocap_qadr=self._mocap_qadr, n_mocap_sites=len(self._mocap_sites),
+                      obs_root_pose_off=sl['_root_pose'].start, obs_root_qvel_off=sl['_root_qvel'].start,
+                      obs_mocap_qpos_off=sl['_mocap_qpos'].start, obs_mocap_qvel_off=sl['_mocap_qvel'].start,
+                      obs_mocap_axes_off=sl['_mocap_axes'].start, obs_mocap_sites_off=sl['_mocap_sites'].start,
+                      obs_wing_qpos_off=sl['_wing_qpos'].start, n_wing=len(self._wing_qadr), wing_qadr=self._wing_qadr,
+                      wing_spring=self._wing_spring, deep_mimic_std=[rw.DEEP_MIMIC_STD[k] for k in ('com', 'qvel', 'root2site', 'joint_quat')],
+                      deep_mimic_weight=_WALK_REWARD_WEIGHTS, retract_margin=_WING_RETRACT_MARGIN)
         else:
             kw.update(episode_steps=int(self._steps_of(self._ref_qpos.shape[0])), ref_len=self._ref_qpos.shape[0], ref_qpos=self._ref_qpos[:, :7],
                       ref_qvel=self._ref_qvel[:, :6])
@@ -528,7 +554,10 @@ class BatchedFlyEnv:
 
     def _bank_tables(self):
         """(rows per trajectory, rows [sum][15]) of every trajectory of the flight dataset for fb_ref_bank -- all of them, because
-        set_next_trajectory_index may name any: root qpos (com2root in fp64), CoM qvel, CoM x, y.  Kept as the host mirror's source."""
+        set_next_trajectory_index may name any: root qpos (com2root in fp64), CoM qvel, CoM x, y.  Kept as the host mirror's source.
+        Walking: rows [sum][15 + 6 nj + 3 ns] for fb_ref_bank_wide (_walk_bank_tables)."""
+        if self._variant == 'walk':
+            return self._walk_bank_tables()
         if self._bank_rows is None:
             tg = self.task._traj_generator
             rows, lens = [], []
@@ -542,21 +571,51 @@ class BatchedFlyEnv:
             self._bank_rows = np.concatenate(rows, 0).astype(np.float32)
         return self._bank_len, self._bank_rows
 
+    def _walk_bank_tables(self):
+        """walking dataset: (rows per trajectory, rows [sum][15 + 6 nj + 3 ns]) of every trajectory for fb_ref_bank_wide: root qpos,
+        root qvel, root x, y (what a reset at the row shifts the root x, y by), mocap qpos, mocap qvel, root2site, joint_quat, as stored.
+        The host mirror of the reward features (`_bank`, read by _walk_reward_factors) is cut from the same fp32 rows as the device
+        reads them: one block per trajectory at the trajectory's bank offset, root x, y shifted by row 0's in fp32."""
+        if self._bank_rows is None:
+            tg = self.task._traj_generator
+            rows, lens = [], []
+            for j in range(tg.num_trajectories):
+                T = tg.trajectory_len(j)
+                f = {k: np.asarray(v[:T], np.float64) for k, v in tg.full_trajectory(j).items()}
+                rows.append(np.concatenate([f['root_qpos'], f['root_qvel'], f['root_qpos'][:, :2], f['qpos'], f['qvel'],
+                                            f['root2site'].reshape(T, -1), f['joint_quat'].reshape(T, -1)], 1))
+                lens.append(T)
+            self._bank_len = np.asarray(lens, np.int64)
+            self._bank_off = np.concatenate([[0], np.cumsum(self._bank_len)[:-1]]).astype(np.int64)
+            self._bank_rows = r = np.concatenate(rows, 0).astype(np.float32)
+            nj, ns = len(self._mocap_qadr), len(self._mocap_sites)
+            root = r[:, :7].copy()
+            root[:, :2] -= np.repeat(r[self._bank_off, 13:15], self._bank_len, 0)
+            b = _FeatureBank()
+            b.qpos = np.concatenate([root, r[:, 15:15 + nj]], 1).astype(np.float64)
+            b.qvel = np.concatenate([r[:, 7:13], r[:, 15 + nj:15 + 2 * nj]], 1).astype(np.float64)
+            b.root2site = r[:, 15 + 2 * nj:15 + 2 * nj + 3 * ns].reshape(-1, ns, 3).astype(np.float64)
+            b.joint_quat = r[:, 15 + 2 * nj + 3 * ns:].reshape(-1, nj, 4).astype(np.float64)
+            b._off, b._n = {j: int(o) for j, o in enumerate(self._bank_off)}, r.shape[0]
+            self._bank = b
+        return self._bank_len, self._bank_rows
+
     def _pick_references(self, ids):
-        """flight dataset with the task on the device: the draws the host-side code makes at these resets (ascending env id; from the
-        loader's RandomState `choice`, then `randint`; a pending set_next_trajectory_index goes to every env of `ids` and is then
-        cleared), pinned for the device's reset (fb_task_ref_pick).  The host mirror (_ref_rows, _ref_len, _episode_steps) is cut
-        from the bank as ktask_reset_ref cuts it: fp32 rows start .. start + n, root x, y relative to the CoM x, y of row `start`,
-        padded with the last row."""
+        """dataset with the task on the device: the draws the host-side code makes at these resets (ascending env id; from the
+        loader's RandomState `choice`, then, flight, `randint`; a pending set_next_trajectory_index goes to every env of `ids` and is
+        then cleared), pinned for the device's reset (fb_task_ref_pick).  The host mirror (_ref_rows, _ref_len, _episode_steps;
+        walking: _env_bank_off into the feature mirror) is cut from the bank as ktask_reset_ref cuts it: fp32 rows start .. start + n,
+        root x, y relative to the x, y in columns 13, 14 of row `start` (flight: the CoM's, walking: the root's), padded with the last row."""
         t, tg = self.task, self.task._traj_generator
         ids = np.sort(np.asarray(ids, np.int64))
         traj, start = np.zeros(len(ids), np.int64), np.zeros(len(ids), np.int64)
+        random_start = self._variant == 'flight' and tg.randomize_start_step      # walking snippets always start at row 0
         for k in range(len(ids)):
             idx = t._next_traj_idx
             if idx is None:
                 idx = tg._random_state.choice(tg.traj_indices)
             traj[k] = idx
-            start[k] = tg._random_state.randint(tg.trajectory_len(idx) - tg.START_MARGIN) if tg.randomize_start_step else 0
+            start[k] = tg._random_state.randint(tg.trajectory_len(idx) - tg.START_MARGIN) if random_start else 0
         t._next_traj_idx = None
         self._sim.task_ref_pick(ids, traj, start)
         self._ref_pick[ids, 0], self._ref_pick[ids, 1] = traj, start
@@ -568,12 +627,15 @@ class BatchedFlyEnv:
             self._ref_rows[e, :n], self._ref_rows[e, n:] = r, r[n - 1]
             self._ref_len[e] = n
             self._episode_steps[e] = self._steps_of(n)
+        if self._variant == 'walk':
+            self._env_bank_off[ids] = self._bank_off[traj]
 
     def reference_picks(self):
         """(trajectory index, start step) of the reference every env tracks in its running episode, int32 [n_envs] each, read from
-        the device (flight_imitation with a dataset and device_task=True) -- e.g. to log which trajectory each env follows."""
+        the device (walk_imitation / flight_imitation with a dataset and device_task=True; walking starts at 0) -- e.g. to log which
+        trajectory each env follows."""
         if not self._device_bank:
-            raise RuntimeError('reference_picks needs flight_imitation(ref_path=..., device_task=True)')
+            raise RuntimeError('reference_picks needs walk_imitation / flight_imitation(ref_path=..., device_task=True)')
         if self._rec is None:
             raise RuntimeError('no episode has started yet: call reset() or step_device() first')
         traj, start = self._sim.task_ref_state()
@@ -677,8 +739,8 @@ class BatchedFlyEnv:
         (observation rows [n_envs, obs_dim], out [n_envs, 4] = reward, discount, step_type, 0) of the library's buffers, valid
         until the next step.  Nothing is copied to the host and the call does not synchronise: work is ordered on
         `env.physics.stepper.stream` (wrap it in `torch.cuda.ExternalStream` to order a policy after it).  Requires
-        `device_task=True`; `observation_layout()` names the columns.  With a flight dataset the envs that reset draw their
-        trajectory and start step on the device (counter hash of seed, env, episode), so no trajectory index may be pending."""
+        `device_task=True`; `observation_layout()` names the columns.  With a dataset the envs that reset draw their trajectory (and,
+        flight, start step) on the device (counter hash of seed, env, episode), so no trajectory index may be pending."""
         if not self._device_task:
             raise RuntimeError('step_device needs device_task=True (task hooks on the device)')
         import torch
@@ -866,8 +928,8 @@ class BatchedFlyEnv:
         b = self._bank
         rf = {'com': b.qpos[rows, :3], 'qvel': b.qvel[rows], 'root2site': b.root2site[rows],
               'joint_quat': np.concatenate([b.qpos[rows, None, 3:7], b.joint_quat[rows]], 1)}
-        factors = rw.reward_factors_deep_mimic(wf, rf, weights=(20, 1, 1, 1))
-        retract = linear_tolerance(f64('_wing_qpos') - self._wing_spring, 3.0)
+        factors = rw.reward_factors_deep_mimic(wf, rf, weights=_WALK_REWARD_WEIGHTS)
+        retract = linear_tolerance(f64('_wing_qpos') - self._wing_spring, _WING_RETRACT_MARGIN)
         return np.concatenate([factors, retract], 1)
 
     # ---------------------------------------------------------------------------- observations
@@ -898,7 +960,9 @@ def walk_imitation(ref_path=None, force_actuators=False, disable_wings=True, tra
     """Batched `flybody.fly_envs.walk_imitation` (reference `fly_envs.py:100-155`).  With `ref_path` (an HDF5 walking
     dataset, or its `.npz` conversion, see `trajectory_loaders`) every env tracks its own snippet, starts from the
     snippet's full-body pose and is rewarded with the DeepMimic factors; without it the task runs in inference mode on
-    the synthetic straight walk, reward 1 (`fly_envs.py:127-135`).  `force_actuators`, `disable_wings=False` and `joint_filter` select
+    the synthetic straight walk, reward 1 (`fly_envs.py:127-135`).  With `ref_path` and `device_task=True` the whole dataset is
+    uploaded once as a device bank with the reward features, and every reset, the full-body start pose and the DeepMimic reward run on
+    the device (`reference_picks()` reads which trajectory each env tracks).  `force_actuators`, `disable_wings=False` and `joint_filter` select
     a model variant (`flymodel.model_for`); each is tested against the oracle in tests/test_model_variants.py."""
     model = None
     if force_actuators or not disable_wings or joint_filter != 0.01:

@@ -22,7 +22,7 @@ MAXCON, MAXEFC = 64, 160
 
 EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_step', 'fb_forward',
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
-           'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version']
+           'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version']
 
 
 # enum FbObsItem
@@ -54,7 +54,12 @@ class FbTaskProgram(C.Structure):
                 ('hover_quat', C.c_float * 4), ('target_zaxis', C.c_float * 3), ('floor_contacts_fatal', C.c_int32),
                 ('trench_cap', C.c_int32), ('trench_x', C.POINTER(C.c_float)), ('trench_len', C.POINTER(C.c_int32)), ('trench_y', C.POINTER(C.c_float)),
                 ('ref_bank', C.c_int32), ('n_pick', C.c_int32), ('pick_traj', C.POINTER(C.c_int32)), ('randomize_start', C.c_int32),
-                ('start_margin', C.c_int32), ('max_episode_rows', C.c_int32), ('future_steps', C.c_int32)]
+                ('start_margin', C.c_int32), ('max_episode_rows', C.c_int32), ('future_steps', C.c_int32),
+                ('n_mocap_joints', C.c_int32), ('mocap_qadr', C.POINTER(C.c_int32)), ('n_mocap_sites', C.c_int32),
+                ('obs_root_pose_off', C.c_int32), ('obs_root_qvel_off', C.c_int32), ('obs_mocap_qpos_off', C.c_int32),
+                ('obs_mocap_qvel_off', C.c_int32), ('obs_mocap_axes_off', C.c_int32), ('obs_mocap_sites_off', C.c_int32),
+                ('obs_wing_qpos_off', C.c_int32), ('wing_spring', C.POINTER(C.c_float)), ('deep_mimic_std', C.c_float * 4),
+                ('deep_mimic_weight', C.c_float * 4), ('retract_margin', C.c_float)]
 
 
 class FbEyeProgram(C.Structure):
@@ -103,6 +108,7 @@ def load_library(path=None):
     lib.fb_task_uniform_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.fb_hfield_bank.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     lib.fb_ref_bank.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.fb_ref_bank_wide.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
     lib.fb_task_ref_pick.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     lib.fb_task_ref_state.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.fb_task_ptrs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p)]
@@ -331,6 +337,14 @@ class BatchedStepper:
         r = np.ascontiguousarray(rows, np.float32)
         assert r.shape == (int(ln.sum()), 15), (r.shape, int(ln.sum()))
         self._check(self._lib.fb_ref_bank(self._h, len(ln), ln.ctypes.data, r.ctypes.data), 'fb_ref_bank')
+
+    def ref_bank_wide(self, traj_len, rows):
+        """fb_ref_bank_wide: trajectories as rows [sum(traj_len)][w >= 15], one after the other; the first 15 columns as for ref_bank
+        (walking: root qpos 7, root qvel 6, root x, y 2), then the task's own columns (walking: the reward features)."""
+        ln = np.ascontiguousarray(traj_len, np.int32)
+        r = np.ascontiguousarray(rows, np.float32)
+        assert r.ndim == 2 and r.shape[0] == int(ln.sum()) and r.shape[1] >= 15, (r.shape, int(ln.sum()))
+        self._check(self._lib.fb_ref_bank_wide(self._h, len(ln), ln.ctypes.data, r.shape[1], r.ctypes.data), 'fb_ref_bank_wide')
 
     def task_ref_pick(self, env_ids, traj, start):
         """pin the trajectory and start step of the listed envs' next reset (fb_task_ref_pick)"""

@@ -143,6 +143,18 @@ class HDF5WalkingTrajectoryLoader(HDF5TrajectoryLoader):
     def trajectory_len(self, traj_idx):
         return int(self._traj_lens[traj_idx])
 
+    _FIELDS = ('root_qpos', 'qpos', 'root_qvel', 'qvel', 'root2site', 'joint_quat')
+
+    def full_trajectory(self, traj_idx):
+        """{root_qpos, qpos, root_qvel, qvel, root2site, joint_quat} of one whole trajectory as stored: no shift of the root x, y to
+        the origin, no draw from the loader's RandomState (read-only)."""
+        g = f'trajectories/{self._key(traj_idx)}/'
+        out = {}
+        for k in self._FIELDS:
+            out[k] = np.array(self._store.get(g + k))
+            out[k].flags.writeable = False
+        return out
+
     def get_trajectory(self, traj_idx=None, start_step=None, end_step=None):
         if traj_idx is None:
             traj_idx = self._random_state.choice(self._traj_indices)

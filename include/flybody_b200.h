@@ -288,9 +288,9 @@ int fb_read_obs(FbHandle h, float* host_dst);
  * check_termination / get_reward / get_discount (tasks/base.py:203-225, walk_imitation.py:179-203,
  * flight_imitation.py:170-226) -- evaluated on the device, so that a control step needs no host round trip: actions in
  * (host or device pointer), observation rows + (reward, discount, step_type) out.  Covers the shared-reference (inference-mode)
- * tasks and flight_imitation with a trajectory dataset (kind 1 with ref_bank = 1: fb_ref_slots, then fb_ref_bank, then this
- * program; every env draws its own trajectory and start step of the bank at each reset).  Dataset-mode walk_imitation keeps
- * the host-side task code.  Requires fb_set_action_map and fb_obs_program first.                                      */
+ * tasks and walk_imitation / flight_imitation with a trajectory dataset (kind 0 / 1 with ref_bank = 1: fb_ref_slots, then
+ * fb_ref_bank_wide / fb_ref_bank, then this program; every env draws its own trajectory (and, flight, start step) of the bank at
+ * each reset).  Requires fb_set_action_map and fb_obs_program first.                                                 */
 typedef struct FbTaskProgram {
   int32_t kind;                        /* 0 walk_imitation, 1 flight_imitation, 2 vision_guided_flight (fields at the end of the struct) */
   int32_t root_qadr, root_vadr, ghost_qadr, ghost_vadr;   /* free-joint slots of the walker root and of the ghost */
@@ -330,17 +330,34 @@ typedef struct FbTaskProgram {
   int32_t ref_bank;
   int32_t n_pick; const int32_t* pick_traj /* [n_pick] trajectory indices of the bank */;
   int32_t randomize_start, start_margin;
-  int32_t max_episode_rows;            /* round(time_limit / control_timestep) */
+  int32_t max_episode_rows;            /* flight: round(time_limit / control_timestep); walking: max_episode_steps + future_steps + 1 */
   int32_t future_steps;
+  /* kind 0 with a trajectory dataset (tasks/walk_imitation.py:93-177): ref_bank = 1 with a bank of fb_ref_bank_wide whose rows are
+   * 15 + 6 n_mocap_joints + 3 n_mocap_sites wide; randomize_start = 0 (every snippet starts at row 0).  A reset puts the root and
+   * ghost on row 0 (root x, y shifted to the origin), the mocap joints at the snippet's row-0 qpos, the wings back at wing_spring,
+   * then adds the noise.  The reward is the product of the four DeepMimic factors
+   * deep_mimic_weight[k] * exp(-0.5 / deep_mimic_std[k]^2 * diff_k) (com, qvel, root2site, joint_quat; tasks/rewards.py:86-116) and
+   * the n_wing factors max(0, 1 - |wing qpos - wing_spring| / retract_margin), from the walker features in the observation
+   * row (obs_*_off: root pose 7, root qvel 6, mocap qpos nj, mocap qvel nj, mocap joint axes nj x 3, mocap sites ns x 3, wing qpos
+   * n_wing) and the bank row of step min(step, n - 1).  wing_qadr / n_wing name the wing joints.  Zero: no such fields.  */
+  int32_t n_mocap_joints; const int32_t* mocap_qadr /* [n_mocap_joints] */; int32_t n_mocap_sites;
+  int32_t obs_root_pose_off, obs_root_qvel_off, obs_mocap_qpos_off, obs_mocap_qvel_off, obs_mocap_axes_off, obs_mocap_sites_off, obs_wing_qpos_off;
+  const float* wing_spring;            /* [n_wing] */
+  float deep_mimic_std[4], deep_mimic_weight[4], retract_margin;
 } FbTaskProgram;
 int fb_task_program(FbHandle h, const FbTaskProgram* p);
 /* Flight trajectory bank for kind 1 with ref_bank: n_traj trajectories, rows [sum(traj_len)][15] fp32, trajectory k after
  * trajectory k - 1: root qpos (7; the dataset's CoM pose through com2root), CoM qvel (6), CoM x, y (2).  A reset at start step s
  * shifts the root x, y of its rows by the CoM x, y of row s (every episode starts above the origin, trajectory_loaders.py:120).
- * Uploaded once; calling it again replaces the bank and drops a task program that points at it.                       */
+ * Uploaded once; calling it again replaces the bank and drops a task program that points at it.  = fb_ref_bank_wide(.., 15, ..) */
 int fb_ref_bank(FbHandle h, int n_traj, const int32_t* traj_len, const float* rows);
+/* Trajectory bank with rows of row_width >= 15 floats; the first 15 columns keep their flight meaning (columns 13, 14: the x, y a
+ * reset at that row shifts the root x, y by).  Walking (kind 0): root qpos 7, root qvel 6, root x, y 2, then mocap qpos [nj],
+ * mocap qvel [nj], root2site [ns][3], joint_quat [nj][4] of the dataset (trajectory_loaders.py:146-156).  At most 2^31 - 1 rows in
+ * all; a bank larger than the device's free memory is refused (-4) with an fb_last_error message.                      */
+int fb_ref_bank_wide(FbHandle h, int n_traj, const int32_t* traj_len, int row_width, const float* rows);
 /* Pin the trajectory and start step of the listed envs' next reset (consumed and cleared by that reset) -- the draws of a host
- * RandomState, where the counter hash would draw otherwise.  Needs a kind 1 program with ref_bank.                    */
+ * RandomState, where the counter hash would draw otherwise.  Needs a program with ref_bank.                           */
 int fb_task_ref_pick(FbHandle h, const int32_t* env_ids, int n, const int32_t* traj, const int32_t* start);
 /* Trajectory and start step of every env's running episode, int32 [n_envs] each, to the host (synchronises).          */
 int fb_task_ref_state(FbHandle h, int32_t* traj, int32_t* start);
