@@ -341,14 +341,16 @@ def compile_variant(variant='walk', assets_dir=None, inertia_mode='legacy2', mes
                            force_actuators=force_actuators, dyntype_filterexact=dyntype_filterexact)
         timestep = float(fx.root.find('option').get('timestep'))
         spawn, prefix = np.zeros(3), ''
-    elif variant == 'walk':
+    elif variant in ('walk', 'template'):
+        # template: template_task (reference fly_envs.py:249-300, tasks/template_task.py:35-43), the same Walking surgery
+        # without the ghost (add_ghost=False), with the factory's adhesion filter
         jf = 0.01 if joint_filter is None else joint_filter
         fx = build_fly_xml(xml_path, name='walker', use_legs=True if use_legs is None else use_legs,
                            use_wings=False if use_wings is None else use_wings, use_mouth=False,
-                           use_antennae=False, joint_filter=jf, adhesion_filter=0.007, force_actuators=force_actuators,
+                           use_antennae=False, joint_filter=jf, adhesion_filter=adhesion_filter, force_actuators=force_actuators,
                            dyntype_filterexact=dyntype_filterexact)
         timestep = 2e-4                                  # reference tasks/constants.py:11
-        spawn, prefix, ghost = _SPAWN_POS, 'walker/', True
+        spawn, prefix, ghost = _SPAWN_POS, 'walker/', variant == 'walk'
         # Walking.__init__: floor params (base.py:398-401)
         floor = dict(friction=np.array([0.5, 0.005, 0.0001]), solref=np.array([0.001, 1.0]),
                      solimp=np.array([0.95, 0.99, 0.01, 0.5, 2.0]), contype=1, conaffinity=1)

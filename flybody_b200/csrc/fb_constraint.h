@@ -871,10 +871,29 @@ FB_DEV void kact_p2b(FB_PHASE_ARGS) {
     if (s != 0.0f) AT(d.qfrc_actuator, k) += s;
   }
 }
+// qfrc_applied[k] + the dof-k row of J^T xfrc_applied (MuJoCo mj_xfrcAccumulate / mj_applyFT): a body's wrench, force at its CoM
+// xipos, reaches the dofs of its ancestor chain, the dofs k with k <= body_lastdof[b] <= dof_subend[k].  Inlined: an out-of-line call
+// would take DevModel / DevData by address and copy the kernel parameters to the stack on every launch, null path included.
+FB_DEV float applied_force(const DevModel& m, const DevData& d, int e, int k) {
+  float s = d.qfrc_applied[(size_t)e * m.nv + k];
+  const float* xf = d.xfrc_applied + (size_t)e * m.nbody * 6;
+  const int se = m.dof_subend[k];
+  const V3 sa = ld3(d.Sang, k, d, e), sl = ld3(d.Slin, k, d, e);
+  for (int b = 1; b < m.nbody; b++) {
+    const int l = m.body_lastdof[b];
+    if (l < k || l > se) continue;
+    const float* w = xf + 6 * b;
+    if (w[0] == 0.0f && w[1] == 0.0f && w[2] == 0.0f && w[3] == 0.0f && w[4] == 0.0f && w[5] == 0.0f) continue;
+    const V3 f = v3(w[0], w[1], w[2]), t = v3(w[3], w[4], w[5]);
+    s += dot(f, sl + cross(sa, ld3(d.xipos, b, d, e))) + dot(t, sa);
+  }
+  return s;
+}
 FB_DEV void kact_p3(FB_PHASE_ARGS) {
   float* xs = sh_dyn(sh);
   for (int k = y; k < m.nv; k += FB_NY) {
     float s = AT(d.qfrc_passive, k) - AT(d.qfrc_bias, k) + AT(d.qfrc_actuator, k);
+    if (d.qfrc_applied) s += applied_force(m, d, e, k);      // uniform over the launch: null unless the handle has applied forces
     AT(d.qfrc_smooth, k) = s; XS(k) = s;
   }
 }
@@ -1280,6 +1299,12 @@ FB_DEV void ktask_reset_ref(const DevModel& m, const DevData& d, const DevTask& 
     t.ep_traj[e] = traj; t.ep_start[e] = start; t.ep_row0[e] = row0; t.ep_n[e] = n; t.ep_steps[e] = rows - (t.future_steps + 1);
   }
 }
+// mj_resetData zeroes qfrc_applied and xfrc_applied: the rows of a resetting env (no-op while the handle has none)
+FB_DEV void zero_applied(const DevModel& m, const DevData& d, int e, int y) {
+  if (!d.qfrc_applied) return;
+  for (int i = y; i < m.nv; i += FB_NY) d.qfrc_applied[(size_t)e * m.nv + i] = 0.0f;
+  for (int i = y; i < 6 * m.nbody; i += FB_NY) d.xfrc_applied[(size_t)e * 6 * m.nbody + i] = 0.0f;
+}
 FB_DEV void ktask_reset(const DevModel& m, const DevData& d, int e, int y) {
   if (!d.task || e >= d.N) return;
   const DevTask& t = *d.task;
@@ -1288,6 +1313,7 @@ FB_DEV void ktask_reset(const DevModel& m, const DevData& d, int e, int y) {
   for (int i = y; i < m.nv; i += FB_NY) { AT(d.qvel, i) = 0.0f; AT(d.qacc, i) = 0.0f; }
   for (int i = y; i < m.na; i += FB_NY) AT(d.act, i) = 0.0f;
   for (int i = y; i < m.nu; i += FB_NY) AT(d.ctrl, i) = 0.0f;      // physics.reset() = mj_resetData: the FIRST observation does not see the old controls
+  zero_applied(m, d, e, y);
 }
 FB_DEV void ktask_reset2(const DevModel& m, const DevData& d, int e, int y) {      // after the template copy (other lanes wrote it)
   if (!d.task || e >= d.N) return;
@@ -1295,6 +1321,10 @@ FB_DEV void ktask_reset2(const DevModel& m, const DevData& d, int e, int y) {   
   if (!t.needs_reset[e]) return;
   const int episode = t.episode[e];
   if (t.kind == 2) { ktask_reset_vision(m, d, t, e, y, episode); return; }
+  if (t.kind == 3) {          // template_task: the template pose as copied, at rest (no reference, no ghost)
+    if (y == 0) { AT(d.time, 0) = 0; AT(d.flags, 0) = 0; AT(d.hold, 0) = 1; AT(d.prev_n, 0) = 0; t.step[e] = 0; t.has_uniform[e] = 0; }
+    return;
+  }
   if (t.ref_bank) ktask_reset_ref(m, d, t, e, y, episode);
   else if (y < 7) { float r = t.ref_qpos[y]; AT(d.qpos, t.root_qadr + y) = r; if (t.ghost_qadr >= 0) AT(d.qpos, t.ghost_qadr + y) = r + (y < 3 ? t.ghost_offset[y] : 0.0f); }
   if (y == 0) {
@@ -1352,7 +1382,7 @@ FB_DEV void ktask_before(const DevModel& m, const DevData& d, int e, int y) {
     else if (y < 13) AT(d.qvel, t.ghost_vadr + y - 7) = resetting ? 0.0f : rv[y - 7];
   }
   if (y == 0) {
-    if (t.kind >= 1 && !resetting) {
+    if ((t.kind == 1 || t.kind == 2) && !resetting) {
       float a = t.user_col >= 0 ? d.sc_vals[(size_t)e * d.sc_k + t.user_col] : 0.0f;
       if (!(a == a)) a = 0.0f;
       float ctrl_freq = t.wb_base_freq * (1.0f + t.wb_rel_range * a);
@@ -1458,6 +1488,13 @@ FB_DEV void ktask_after(const DevModel& m, const DevData& d, int e, int y) {
   float s2 = 0; for (int i = 0; i < m.nv; i++) { float x = AT(d.qacc, i); s2 += x * x; }
   const bool bad = (AT(d.flags, 0) & 1) != 0 || !(sqrtf(s2) <= t.term_qacc);      // bits 1, 2 are capacity overflows, not bad physics
   bool terminate; float reward;
+  if (t.kind == 3) {      // template_task (tasks/template_task.py): reward 1; only a bad state ends an episode early, with discount 0
+    const bool last = bad || (double)step_now * (double)t.dt >= (double)t.time_limit - 1e-9;
+    float* out = t.out + 4 * (size_t)e;
+    out[0] = resetting ? 0.0f : 1.0f; out[1] = resetting ? 1.0f : (bad ? 0.0f : 1.0f); out[2] = resetting ? 0.0f : (last ? 2.0f : 1.0f); out[3] = 0.0f;
+    t.needs_reset[e] = (last && !resetting) ? 1 : 0;
+    return;
+  }
   if (t.kind == 2) {      // vision_flight.py:157-254: reward factors, fatal contacts with world geoms
     const float th = t.target[2 * e], ts = t.target[2 * e + 1];
     const float x = AT(d.qpos, t.root_qadr), yy = AT(d.qpos, t.root_qadr + 1), z = AT(d.qpos, t.root_qadr + 2);
@@ -1527,6 +1564,7 @@ FB_DEV void kreset_scatter(const DevModel& m, const DevData& d, int w, int y) {
   for (int i = y; i < m.nv; i += FB_NY) { AT(d.qvel, i) = d.rst_has_qvel ? d.rst_qvel[(size_t)w * m.nv + i] : 0.0f; AT(d.qacc, i) = 0; }
   for (int i = y; i < m.na; i += FB_NY) AT(d.act, i) = 0;
   for (int i = y; i < m.nu; i += FB_NY) AT(d.ctrl, i) = 0;         // mj_resetData zeroes ctrl (reference: physics.reset() before initialize_episode)
+  zero_applied(m, d, e, y);
   if (y == 0) { AT(d.time, 0) = 0; AT(d.flags, 0) = 0; AT(d.hold, 0) = d.rst_hold; AT(d.prev_n, 0) = 0; }
 }
 FB_DEV void kclear_hold(const DevModel& m, const DevData& d, int e, int y) { if (y == 0) AT(d.hold, 0) = 0; }
@@ -1542,6 +1580,7 @@ FB_DEV void kscatter(const DevModel& m, const DevData& d, int e, int y) {
     if (t < 0) continue;                                 // column without a target (e.g. a user action)
     float v = d.sc_vals[(size_t)src * d.sc_k + c];
     if (d.sc_nan0 && !(v == v)) v = 0.0f;                // NaN actions act as 0 (reference tasks/base.py:199)
-    AT(d.sc_field, t) = drop ? 0.0f : v;
+    if (d.sc_stride) d.sc_field[(size_t)e * d.sc_stride + t] = v;      // compact per-env array (applied forces)
+    else AT(d.sc_field, t) = drop ? 0.0f : v;
   }
 }

@@ -152,12 +152,17 @@ struct DevData {
   int *flags, *niter, *hold;   // hold != 0: env is not integrated by the next fb_step (pending reset)
   const int* rst_ids; const float* rst_qpos; const float* rst_qvel; int rst_n, rst_has_qvel, rst_hold;   // staged partial reset
   float* sc_field; const int* sc_idx; const float* sc_vals; int sc_k, sc_nan0;                                 // staged column scatter
+  unsigned sc_stride;          // slots between the scatter target's env rows: 0 = a record field, else a compact [Np][sc_stride] array
   float *obs;                  // packed AoS observation [N][obs_dim]
   int obs_dim;
   // task observation program (fb_obs_program): final observation rows [N][tobs_dim]
   float *tobs; int tobs_dim, op_n, op_root_body, op_ref_len, op_nsub, op_ref_slot /* 1: op_ref is [N][op_ref_len][7], one table per env */;
   const int *op_kind, *op_a, *op_b, *op_off, *op_list; const float* op_ref; const int* op_step; const unsigned char* op_first;
   const struct DevTask* task;  // device-side task logic, or nullptr
+  // applied forces (mjData.qfrc_applied, mjData.xfrc_applied): compact [Np][nv] and [Np][nbody][6] (world force, then torque, at the
+  // body's CoM), allocated together on first use (fb_applied_ptrs / fb_set / fb_write_state); nullptr until then and after
+  // fb_clear_applied, so a step that never set them runs without the term
+  float *qfrc_applied, *xfrc_applied;
 };
 
 // Device-side task logic (fb_task_program): what the reference's task hooks do around the physics step -- auto-reset,

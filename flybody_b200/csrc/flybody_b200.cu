@@ -59,6 +59,7 @@ struct FbSim {
   FbModel hm;                       // host copy of scalar fields (pointers invalid after create)
   std::vector<void*> allocs;
   std::vector<void*> obs_scope, task_scope;   // device buffers of the current observation / task program: freed when the program is replaced
+  std::vector<void*> applied_scope;           // qfrc_applied / xfrc_applied: freed by fb_clear_applied
   std::vector<int> h_dof_parent, h_dof_Madr, h_body_lastdof, h_geom_bodyid;
   std::vector<double> h_qpos0;
   int device; long long launches; float last_ms; std::string err;
@@ -647,6 +648,22 @@ static int sync_stream(FbSim* s) {
   return 0;
 }
 
+// applied forces (FB_QFRC_APPLIED, FB_XFRC_APPLIED): compact device arrays [Np][n], both allocated zeroed on first use
+static float* applied_ptr(FbSim* s, int field, int* n) {
+  *n = field == FB_QFRC_APPLIED ? s->m.nv : 6 * s->m.nbody;
+  return field == FB_QFRC_APPLIED ? s->d.qfrc_applied : s->d.xfrc_applied;
+}
+static int ensure_applied(FbSim* s) {
+  if (s->d.qfrc_applied) return 0;
+  if (sync_stream(s) != 0) return -2;
+  const size_t mark = s->allocs.size();
+  float* q = dalloc<float>(s, (size_t)s->d.Np * s->m.nv); float* x = dalloc<float>(s, (size_t)s->d.Np * 6 * s->m.nbody);
+  s->applied_scope.assign(s->allocs.begin() + mark, s->allocs.end());
+  if (!q || !x) { scope_free(s, s->applied_scope); s->err = "out of device memory (applied forces)"; return -4; }
+  s->d.qfrc_applied = q; s->d.xfrc_applied = x;      // the step graph is captured again: DevData changed
+  return 0;
+}
+
 extern "C" {
 
 const char* fb_version(void) {
@@ -774,7 +791,7 @@ static void step_sequence(FbSim* s, int n_substeps) {
 // read by them and are masked out of the comparison.
 static DevData canonical(const DevData& d) {
   DevData c = d;
-  c.sc_field = nullptr; c.sc_idx = nullptr; c.sc_vals = nullptr; c.sc_k = 0; c.sc_nan0 = 0;
+  c.sc_field = nullptr; c.sc_idx = nullptr; c.sc_vals = nullptr; c.sc_k = 0; c.sc_nan0 = 0; c.sc_stride = 0;
   c.rst_ids = nullptr; c.rst_qpos = nullptr; c.rst_qvel = nullptr; c.rst_n = 0; c.rst_has_qvel = 0; c.rst_hold = 0;
   return c;
 }
@@ -851,6 +868,8 @@ int fb_field_size(FbHandle s, int field) {
   if (!s) return -1;
   int n; if (field_ptr(s, field, &n)) return n;
   switch (field) {
+    case FB_QFRC_APPLIED: return s->m.nv;
+    case FB_XFRC_APPLIED: return 6 * s->m.nbody;
     case FB_SUBTREE_COM: return 3 * s->m.nbody;
     case FB_NCON: case FB_NEFC: case FB_SOLVER_NITER: case FB_FLAGS: return 1;
     case FB_QM_DENSE: return s->m.nv * s->m.nv;
@@ -864,6 +883,12 @@ int fb_get(FbHandle s, int field, void* dst, int is_device) {
   if (sync_stream(s) != 0) return -2;
   int n; void* p = field_ptr(s, field, &n);
   const DevModel& m = s->m; int N = s->d.N;
+  if (field == FB_QFRC_APPLIED || field == FB_XFRC_APPLIED) {
+    if (is_device) { s->err = "applied forces are compact [n_envs][n] arrays, not record fields: use fb_applied_ptrs"; return -1; }
+    const float* a = applied_ptr(s, field, &n);
+    if (a) d2h(dst, a, sizeof(float) * (size_t)N * n); else memset(dst, 0, sizeof(float) * (size_t)N * n);      // unset = zero
+    return 0;
+  }
   if (is_device) { if (!p) { s->err = "field has no device array"; return -1; } *(void**)dst = p; return 0; }
   float* out = (float*)dst;
   if (p) {
@@ -920,16 +945,25 @@ int fb_get(FbHandle s, int field, void* dst, int is_device) {
 int fb_set(FbHandle s, int field, const float* src) {
   if (!s || !src) return -1;
   if (sync_stream(s) != 0) return -2;
-  int n; void* p = field_ptr(s, field, &n);
+  int n;
+  if (field == FB_QFRC_APPLIED || field == FB_XFRC_APPLIED) {
+    int rc = ensure_applied(s);
+    if (rc != 0) return rc;
+    float* a = applied_ptr(s, field, &n);
+    h2d(a, src, sizeof(float) * (size_t)s->d.N * n);      // (pad envs keep zero applied forces)
+    return 0;
+  }
+  void* p = field_ptr(s, field, &n);
   if (!p || !(field == FB_QPOS || field == FB_QVEL || field == FB_ACT || field == FB_CTRL || field == FB_QACC_WARMSTART || field == FB_QACC || field == FB_TIME)) { s->err = "field is not writable"; return -1; }
   if (n > 0) field_from_host(s, p, n, src);
   return 0;
 }
 
 // scatter vals[N][k] (already on the device, row-major) into columns idx[k] (device ints, or NULL = 0..k-1) of `field`
-static void launch_scatter(FbSim* s, float* field, const int* idx_dev, const float* vals_dev, int k, int nan_to_zero = 0) {
-  s->d.sc_field = field; s->d.sc_idx = idx_dev; s->d.sc_vals = vals_dev; s->d.sc_k = k; s->d.sc_nan0 = nan_to_zero;
+static void launch_scatter(FbSim* s, float* field, const int* idx_dev, const float* vals_dev, int k, int nan_to_zero = 0, unsigned stride = 0) {
+  s->d.sc_field = field; s->d.sc_idx = idx_dev; s->d.sc_vals = vals_dev; s->d.sc_k = k; s->d.sc_nan0 = nan_to_zero; s->d.sc_stride = stride;
   fb_launch<ShNone, Ph<ph_scatter>>(s, K_MISC);
+  s->d.sc_stride = 0;
 }
 
 int fb_set_ctrl(FbHandle s, const float* ctrl, int is_device) {
@@ -956,8 +990,11 @@ int fb_set_action_map(FbHandle s, const int32_t* ctrl_index, int n_action) {
 
 int fb_write_state(FbHandle s, int field, const int32_t* idx, int k, const float* vals) {
   if (!s || !idx || !vals || k <= 0) return -1;
-  int n; float* p = (float*)field_ptr(s, field, &n);
-  if (!p || !(field == FB_QPOS || field == FB_QVEL || field == FB_ACT)) { s->err = "fb_write_state: field must be qpos, qvel or act"; return -1; }
+  const bool applied = field == FB_QFRC_APPLIED || field == FB_XFRC_APPLIED;
+  if (applied) { int rc = ensure_applied(s); if (rc != 0) return rc; }
+  int n; float* p = applied ? applied_ptr(s, field, &n) : (float*)field_ptr(s, field, &n);
+  if (!p || !(field == FB_QPOS || field == FB_QVEL || field == FB_ACT || applied)) {
+    s->err = "fb_write_state: field must be qpos, qvel, act, qfrc_applied or xfrc_applied"; return -1; }
   for (int c = 0; c < k; c++) if (idx[c] < 0 || idx[c] >= n) { s->err = "fb_write_state: index out of range"; return -1; }
   // separate staging regions so that several writes can be in flight before the next sync
   size_t need = (size_t)s->d.N * s->m.nu + (size_t)4 * s->d.N * 16;
@@ -968,7 +1005,23 @@ int fb_write_state(FbHandle s, int field, const int32_t* idx, int k, const float
   int* idev = s->stage_i + slot * 16;
   upload_async(s, idev, idx, sizeof(int) * k);
   upload_async(s, vdev, vals, sizeof(float) * (size_t)s->d.N * k);
-  launch_scatter(s, p, idev, vdev, k);
+  launch_scatter(s, p, idev, vdev, k, 0, applied ? (unsigned)n : 0u);
+  return 0;
+}
+int fb_applied_ptrs(FbHandle s, void** qfrc_dev, void** xfrc_dev) {
+  if (!s) return -1;
+  int rc = ensure_applied(s);
+  if (rc != 0) return rc;
+  if (qfrc_dev) *qfrc_dev = s->d.qfrc_applied;
+  if (xfrc_dev) *xfrc_dev = s->d.xfrc_applied;
+  return 0;
+}
+int fb_clear_applied(FbHandle s) {
+  if (!s) return -1;
+  if (!s->d.qfrc_applied) return 0;
+  if (sync_stream(s) != 0) return -2;
+  scope_free(s, s->applied_scope);
+  s->d.qfrc_applied = nullptr; s->d.xfrc_applied = nullptr;
   return 0;
 }
 
@@ -1178,10 +1231,13 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
       for (int k = 0; k < 4; k++) if (!(p->deep_mimic_std[k] > 0)) { s->err = "fb_task_program: deep_mimic_std must be positive"; return -1; }
       if (!(p->retract_margin > 0)) { s->err = "fb_task_program: retract_margin must be positive"; return -1; }
     }
+  } else if (p->kind == 3) {
+    if (p->ghost_qadr >= 0 || p->user_col >= 0 || p->n_noise > 0) { s->err = "fb_task_program: kind 3 (template_task) has no ghost, user action or reset noise"; return -1; }
+  } else if (p->kind < 0 || p->kind > 3) { s->err = "fb_task_program: unknown kind"; return -1;
   } else if (p->ref_len <= 0 || !p->ref_qpos || !p->ref_qvel) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
   if (!p->reset_qpos) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
   if (p->kind == 2 && (!s->bank_dev || !s->hfield_dev || s->bank_n <= 0)) { s->err = "fb_task_program: kind 2 needs fb_hfield_collision / fb_eye_program and fb_hfield_bank first"; return -1; }
-  if (p->kind >= 1 && (p->n_wing <= 0 || p->n_freq <= 0 || p->tab_len <= 0 || !p->wb_traj || !p->wb_phase || !p->wb_phase_mod || !p->wb_freqs || !p->wb_len)) { s->err = "fb_task_program: wing-beat tables missing"; return -1; }
+  if ((p->kind == 1 || p->kind == 2) && (p->n_wing <= 0 || p->n_freq <= 0 || p->tab_len <= 0 || !p->wb_traj || !p->wb_phase || !p->wb_phase_mod || !p->wb_freqs || !p->wb_len)) { s->err = "fb_task_program: wing-beat tables missing"; return -1; }
   if (sync_stream(s) != 0) return -2;
   const DevModel& m = s->m; const int Np = s->d.Np;
   scope_free(s, s->task_scope); s->d.task = nullptr;
@@ -1197,10 +1253,10 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   auto upf32 = [&](const float* src, size_t n) { std::vector<float> v(src, src + n); return up(s, v); };
   auto upi32 = [&](const int32_t* src, size_t n) { std::vector<int> v(src, src + n); return up(s, v); };
   t.reset_qpos = upf32(p->reset_qpos, m.nq);
-  if (!bank) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
+  if (!bank && p->kind != 3) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
   else t.ref_len = 0;
   t.n_noise = p->noise_qadr ? p->n_noise : 0; t.noise_qadr = t.n_noise ? upi32(p->noise_qadr, t.n_noise) : nullptr; t.noise_amp = p->noise_amp; t.seed = p->seed;
-  if (p->kind >= 1) {
+  if (p->kind == 1 || p->kind == 2) {
     t.n_wing = p->n_wing; t.wing_qadr = upi32(p->wing_qadr, p->n_wing); t.wing_vadr = upi32(p->wing_vadr, p->n_wing); t.wing_ctrl = upi32(p->wing_ctrl, p->n_wing);
     t.n_freq = p->n_freq; t.tab_len = p->tab_len; const size_t nt = (size_t)p->n_freq * p->tab_len;
     t.wb_traj = upf32(p->wb_traj, nt * p->n_wing); t.wb_phase = upf32(p->wb_phase, nt); t.wb_phase_mod = upf32(p->wb_phase_mod, nt);

@@ -181,6 +181,20 @@ class WalkImitationTask(_ImitationTask):
     """Batched `WalkImitation` (reference `tasks/walk_imitation.py:19-203`, `tasks/base.py:367-428`)."""
 
 
+class TemplateTask:
+    """What the reference's callers reach through `env.task` of `template_task` (`tasks/template_task.py`)."""
+    name = 'FruitFlyTask'
+
+    def __init__(self, env, time_limit, control_timestep):
+        self._env = env
+        self._traj_generator = None
+        self._time_limit = time_limit
+        self._future_steps = 0
+        self._ghost_offset = np.zeros(3)
+        self._terminal_com_dist = np.inf
+        self._max_episode_steps = round(time_limit / control_timestep)
+
+
 class FlightImitationTask(_ImitationTask):
     """Batched `FlightImitationWBPG` (reference `tasks/flight_imitation.py:16-212`, `tasks/base.py:271-364`)."""
 
@@ -196,6 +210,9 @@ _VARIANTS = {
                                                  'ref_displacement', 'ref_root_quat')),
     'flight': dict(dt=_FLY_CONTROL_TIMESTEP, obs=('accelerometer', 'actuator_activation', 'gyro', 'joints_pos', 'joints_vel',
                                                   'velocimeter', 'world_zaxis', 'ref_displacement', 'ref_root_quat')),
+    # template_task: the walker's observables only (reference tests/test_core.py:9-20)
+    'template': dict(dt=_WALK_CONTROL_TIMESTEP, obs=('accelerometer', 'actuator_activation', 'appendages_pos', 'force', 'gyro',
+                                                     'joints_pos', 'joints_vel', 'touch', 'velocimeter', 'world_zaxis')),
 }
 
 
@@ -222,6 +239,9 @@ class BatchedFlyEnv:
             self.task = WalkImitationTask(self, traj_generator or InferenceWalkingTrajectoryLoader(), terminal_com_dist,
                                           future_steps, time_limit, self._control_timestep)
             self._n_user = 0
+        elif variant == 'template':
+            self.task = TemplateTask(self, time_limit, self._control_timestep)
+            self._n_user = 0
         else:
             self._wbpg = BatchedWingBeatPatternGenerator(self.n_envs, base_pattern_path=wpg_pattern_path)
             self.task = FlightImitationTask(self, self._wbpg, traj_generator or InferenceFlightTrajectoryLoader(),
@@ -241,7 +261,7 @@ class BatchedFlyEnv:
         # walking: actions go to the device as they are, the action -> ctrl permutation and NaN -> 0 run in the scatter
         # kernel (fb_set_action_map); flight keeps the host path because the wing actions are modified by the WBPG first
         self._device_task = bool(device_task)       # task hooks evaluated on the device (fb_task_*): no host logic in step()
-        self._device_action_map = variant == 'walk' or self._device_task
+        self._device_action_map = variant in ('walk', 'template') or self._device_task
         if self._device_action_map:
             # user actions (flight: the beat frequency) have no ctrl slot: column -> -1, read by the device-side task code
             self._sim.set_action_map(np.concatenate([self._ctrl_of_action, -np.ones(self._n_user, np.int64)]) if self._device_task
@@ -255,8 +275,8 @@ class BatchedFlyEnv:
         jn = m.meta['jnt_names']
         self._root_q = m.jnt_qposadr_of('walker/')
         self._root_v = m.jnt_dofadr_of('walker/')
-        self._ghost_q = m.jnt_qposadr_of('ghost/')
-        self._ghost_v = m.jnt_dofadr_of('ghost/')
+        self._ghost_q = m.jnt_qposadr_of('ghost/') if 'ghost/' in jn else -1      # (template_task: no ghost)
+        self._ghost_v = m.jnt_dofadr_of('ghost/') if 'ghost/' in jn else -1
         obsj = [jn.index(n) for n in m.meta['observable_joints']]
         self._obs_qadr = m.jnt_qposadr[obsj]
         self._obs_vadr = m.jnt_dofadr[obsj]
@@ -282,7 +302,7 @@ class BatchedFlyEnv:
             self._app_sites = np.array([sn.index(n) for n in app])
         else:
             self._app_sites = np.zeros(0, np.int64)
-        if variant != 'walk':
+        if variant == 'flight':
             # position of the wing joints inside the joints_pos observable (the host reads wing angles from there)
             self._wing_in_obs = np.array([m.meta['observable_joints'].index(n) for n in wing_names])
             self._wing_qpos_host = np.zeros((N, 6))
@@ -297,7 +317,7 @@ class BatchedFlyEnv:
         # One reference per env (dataset loaders hand out a different snippet per episode) or one shared by all envs (the
         # Inference* loaders hold a single trajectory): the shared case keeps one device table, the per-env case one slot per env.
         tg = self.task._traj_generator
-        self._per_env_ref = not isinstance(tg, (InferenceWalkingTrajectoryLoader, InferenceFlightTrajectoryLoader))
+        self._per_env_ref = tg is not None and not isinstance(tg, (InferenceWalkingTrajectoryLoader, InferenceFlightTrajectoryLoader))
         self._max_reference_steps = max_reference_steps
         self._ref_rows = None                       # per-env mode: [N, slot_len, 13] fp32 (root qpos 7, root qvel 6), padded with the last row
         self._ref_len = np.zeros(N, np.int64)
@@ -416,7 +436,7 @@ class BatchedFlyEnv:
         if not self._inference_mode:
             lists += list(range(self._root_v, self._root_v + 6)) + list(self._mocap_qadr) + list(self._mocap_vadr) \
                 + list(self._mocap_sites) + list(self._wing_qadr)
-        shared = self._ref_qpos[:, :7] if not self._per_env_ref else np.zeros((self._future, 7))
+        shared = None if self._variant == 'template' else self._ref_qpos[:, :7] if not self._per_env_ref else np.zeros((self._future, 7))
         dim = self._sim.obs_program([r[3] for r in rows], lists, m.body_id('walker/thorax'), self._n_sub, shared)
         if self._per_env_ref:
             self._sim.ref_slots(self._slot_len)
@@ -707,6 +727,17 @@ class BatchedFlyEnv:
         self._needs_reset = step_type == int(StepType.LAST)
         return TimeStep(step_type,
                         self._out4[:, 0].astype(np.float64), self._out4[:, 1].astype(np.float64), self._observation(self._rec))
+
+    def set_applied_forces(self, qfrc=None, xfrc=None, env_ids=None):
+        """MuJoCo's `physics.data.qfrc_applied` ([nv] per env) and `xfrc_applied` ([nbody, 6] per env: world-frame force, then torque,
+        at each body's CoM) for every env (`env_ids` None; a single row broadcasts) or the listed envs.  They act in every physics
+        substep until overwritten or cleared, and a reset of an env zeroes its own (mj_resetData).  None leaves a field as it is.
+        The batched counterpart of writing them from a per-substep `mjcb_control` callback."""
+        self._sim.set_applied(qfrc, xfrc, env_ids)
+
+    def clear_applied_forces(self):
+        """zero every env's applied forces (the step goes back to the path without the applied-force term)"""
+        self._sim.clear_applied()
 
     def request_reset(self, env_ids):
         """Restart the listed envs at the next step (their action of that step is dropped and they report FIRST), whatever their
@@ -1018,6 +1049,119 @@ def walk_on_ball(*args, **kwargs):
     raise NotImplementedError(walk_on_ball.__doc__)
 
 
-def template_task(*args, **kwargs):
-    """`flybody.fly_envs.template_task` (reference `fly_envs.py:249-310`): outside the hot-path scope (SURVEY.md section 8)."""
-    raise NotImplementedError(template_task.__doc__)
+class TemplateTaskEnv(BatchedFlyEnv):
+    """Batched `TemplateTask` (reference `tasks/template_task.py`): the walker on the flat Walking floor without a ghost or a
+    reference.  Every episode starts from the template pose at rest (`qpos0`, the upright spawn); the reward is 1; an episode ends
+    early only on a bad state (non-finite, or |qacc| > _TERMINAL_QACC: base.py:222-225, discount 0), else at the time limit (discount 1).
+    An optional `action_corruptor(action, random_state)` rewrites the actions on the host before they are applied; `prev_action`
+    returns what was applied (the reference walker's `prev_action`)."""
+
+    def __init__(self, n_envs, time_limit=1.0, action_corruptor=None, random_state=None, **kw):
+        super().__init__('template', n_envs, time_limit=time_limit, **kw)
+        self._corruptor = action_corruptor
+        if random_state is not None:
+            self._rs = random_state if isinstance(random_state, np.random.RandomState) else np.random.RandomState(random_state)
+        self._prev_action = np.zeros((self.n_envs, self._action_spec.shape[0]))
+
+    @property
+    def prev_action(self):
+        """the actions applied by the last step (after the corruptor; zero for an env that started an episode in it)"""
+        return self._prev_action.copy() if self._batched else self._prev_action[0].copy()
+
+    def _load_snippet(self, ids):
+        if self._rec is None:                   # no reference: the programs are uploaded once
+            self._upload_program()
+
+    def _upload_task_program(self):
+        m = self.model
+        self._sim.task_program(kind=3, root_qadr=self._root_q, root_vadr=self._root_v, ghost_qadr=-1, ghost_vadr=-1, user_col=-1,
+                               control_timestep=self._control_timestep, time_limit=self._time_limit, terminal_com_dist=3e38,
+                               terminal_linvel=3e38, terminal_angvel=3e38, terminal_qacc=_TERMINAL_QACC, terminal_height=-3e38,
+                               velocimeter_adr=int(self._sd['velocimeter'][0]), gyro_adr=int(self._sd['gyro'][0]),
+                               com_body=m.body_id('walker/thorax'), reset_qpos=m.qpos0, n_noise=0, seed=int(self._seed) & 0xffffffff)
+        self._out4 = np.zeros((self.n_envs, 4), np.float32)
+
+    def _reset_envs(self, ids, hold=False):
+        """physics.reset() (mj_resetData: qpos0 at rest, controls and applied forces zeroed) + initialize_episode"""
+        ids = np.asarray(ids)
+        self._load_snippet(ids)
+        qpos = np.tile(self.model.qpos0, (len(ids), 1))
+        if hold:
+            self._sim.reset_hold(ids, qpos)
+        else:
+            self._sim.reset(qpos=qpos, env_ids=None if len(ids) == self.n_envs else ids)
+        self._step_counter[ids] = 0
+        self._time[ids] = 0.0
+        self._needs_reset[ids] = False
+        self._prev_action[ids] = 0.0
+        self.n_resets += len(ids)
+
+    def reset(self):
+        self._prev_action[:] = 0.0
+        return super().reset()
+
+    def step(self, action):
+        N = self.n_envs
+        action = np.array(action, np.float64, copy=True).reshape(N, -1)
+        assert action.shape[1] == self._action_spec.shape[0], f'action must have {self._action_spec.shape[0]} entries'
+        if self._corruptor is not None:                 # before_step (template_task.py): on the host, before the action map
+            action = np.array(self._corruptor(action, self._rs), np.float64).reshape(N, -1)
+        resetting = self._needs_reset.copy()
+        self._prev_action = np.where(resetting[:, None], 0.0, action)      # a resetting env drops its action (composer auto-reset)
+        if self._device_task:
+            return self._unbatch(self._device_step(action.astype(np.float32)))
+        if resetting.any():
+            self._reset_envs(np.nonzero(resetting)[0], hold=True)
+        self._step_counter += np.where(resetting, 0, 1)
+        a32 = action.astype(np.float32)
+        self._sim.set_control(a32)                      # action -> ctrl permutation and NaN -> 0 on the device
+        self.h2d_bytes_per_step = a32.nbytes
+        self._sim.task_inputs(self._step_counter, resetting)
+        self._sim.step(self._n_sub)
+        rec = self._sim.read_task_obs(self._rec)
+        self.d2h_bytes_per_step = rec.nbytes
+        self._time = np.where(resetting, 0.0, self._time + self._control_timestep)
+        obs = self._observation(rec)
+        step_type, reward, discount, self._needs_reset = self._task_after(rec, obs, resetting, self._time, None)
+        return self._unbatch(TimeStep(step_type, reward, discount, obs))
+
+    def _task_after(self, rec, obs, resetting, time, ghost):
+        """get_reward (factors (1,)), check_termination (base.py:222-225), get_discount; the device task kind 3 is the same logic"""
+        flags = rec[:, self._obs_slices['_scalars']][:, 0].astype(np.int64)
+        self.n_capacity_overflows += int(((flags & 6) != 0).sum())
+        bad = ((flags & 1) != 0) | ~(np.sqrt(rec[:, self._obs_slices['_scalars']][:, 1].astype(np.float64)) <= _TERMINAL_QACC)
+        last = bad | (time >= self._time_limit - 1e-9)
+        step_type = np.where(resetting, StepType.FIRST, np.where(last, StepType.LAST, StepType.MID))
+        reward = np.where(resetting, 0.0, 1.0)
+        discount = np.where(resetting | ~bad, 1.0, 0.0)
+        return step_type, reward, discount, last & ~resetting
+
+    def step_device(self, action):
+        if self._corruptor is not None:
+            raise RuntimeError('step_device does not run an action_corruptor (a host callable): corrupt the actions on the device, '
+                               'or use step()')
+        return super().step_device(action)
+
+
+def template_task(random_state=None, force_actuators=False, disable_wings=True, joint_filter=0.01, adhesion_filter=0.007,
+                  time_limit=1.0, mjcb_control=None, observables_options=None, action_corruptor=None, n_envs=None, device=0,
+                  lib_path=None, seed=0, device_task=False):
+    """Batched `flybody.fly_envs.template_task` (reference `fly_envs.py:249-300`, `tasks/template_task.py`): the walking fly
+    without a ghost on flat ground, reward 1, the reference's installation test (`tests/test_core.py`) and the class to start a
+    walking task from.  `force_actuators`, `disable_wings=False`, `joint_filter` and `adhesion_filter` select a model variant
+    (`flymodel.model_for('template', ...)`).  `device_task=True` runs the task hooks on the device (kind 3), which `step_device` needs.
+    `mjcb_control` (a per-substep Python callback) and `observables_options` are not supported."""
+    if mjcb_control is not None:
+        raise NotImplementedError('mjcb_control: a per-substep Python callback cannot run at batch speed (DESIGN.md section 8). Perturbation '
+                                  'forces go through env.set_applied_forces(qfrc=..., xfrc=...), the batched physics.data.qfrc_applied / '
+                                  'xfrc_applied, which act in every substep until overwritten')
+    if observables_options is not None:
+        raise NotImplementedError('observables_options (observable noise, delay, buffering) are not supported')
+    model = None
+    if force_actuators or not disable_wings or joint_filter != 0.01 or adhesion_filter != 0.007:
+        from .flymodel import model_for
+        model = model_for('template', force_actuators=force_actuators, use_wings=True if not disable_wings else None,
+                          joint_filter=None if joint_filter == 0.01 else joint_filter,
+                          adhesion_filter=None if adhesion_filter == 0.007 else adhesion_filter)
+    return TemplateTaskEnv(n_envs, time_limit=time_limit, action_corruptor=action_corruptor, random_state=random_state, device=device,
+                           lib_path=lib_path, seed=seed, device_task=device_task, model=model)

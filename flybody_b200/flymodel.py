@@ -150,11 +150,59 @@ class FlyModel:
 
 
 def load_model(variant='walk', path=None):
+    if path is None and variant == 'template':
+        return template_from_walk(load_model('walk'))
     path = path or os.path.join(ASSETS, f'fly_{variant}.npz')
     d = np.load(path)
     meta = json.loads(bytes(d['__meta__']).decode())
     arrays = {k: d[k] for k in d.files if k != '__meta__'}
     return FlyModel(arrays, meta)
+
+
+_TRAILING = (('body_', 'nbody', 'body_names'), ('jnt_', 'njnt', 'jnt_names'), ('site_', 'nsite', 'site_names'))
+
+
+def template_from_walk(walk):
+    """The model of `template_task` (reference tasks/template_task.py:35: the Walking task with add_ghost=False) cut from the walk model:
+    the compiler appends the ghost after the walker (its body, free joint, 7 qpos, 6 dofs and site come last, its geoms do not collide),
+    so the walker's arrays are the leading parts of the walk model's.  Recomputed: the sizes, the world's subtree mass and the mean
+    inertia at qpos0 (mj_setConst; the ghost's armature dominated it).  The invweights and the stiffness / damping the compiler derives
+    from them are kept: the ghost is a tree of its own, so they differ from a compile without it by rounding only
+    (`compile_variant('template')` compiles it, and tests/test_template_task.py holds the two together where the reference's XML is
+    reachable)."""
+    a, meta = dict(walk.a), json.loads(json.dumps(walk.meta))
+    cut = {}
+    for prefix, size, names in _TRAILING:
+        keep = [n for n in meta[names] if not n.startswith('ghost/')]
+        assert meta[names][:len(keep)] == keep, f'the ghost is not at the end of {names}'
+        cut[prefix] = len(keep)
+        meta[names], meta[size] = keep, len(keep)
+    nv = int((a['dof_bodyid'] < cut['body_']).sum())
+    assert np.all(a['dof_bodyid'][:nv] < cut['body_']), 'the ghost dofs are not at the end'
+    last = cut['jnt_'] - 1                 # free (type 0): 7 qpos; hinge: 1
+    nq = int(a['jnt_qposadr'][last] + (7 if a['jnt_type'][last] == 0 else 1))
+    cut['dof_'] = nv
+    out = {}
+    for k, v in a.items():
+        if not isinstance(v, np.ndarray) or k in meta:
+            continue
+        n = nq if k in ('qpos0', 'qpos_spring') else next((cut[p] for p in cut if k.startswith(p)), None)
+        out[k] = v[:n].copy() if n is not None else v.copy()
+    for k in ('geom_bodyid', 'site_bodyid', 'fluid_bodyid'):
+        assert not len(out[k]) or out[k].max() < meta['nbody'], k
+    chain = np.zeros(nv, np.int64)
+    for d in range(nv):
+        p = out['dof_parentid'][d]
+        chain[d] = 1 + (chain[p] if p >= 0 else 0)
+    meta['nv'], meta['nq'], meta['nM'] = nv, nq, int(chain.sum())
+    assert np.array_equal(out['dof_Madr'], np.concatenate([[0], np.cumsum(chain)[:-1]]))
+    children = out['body_parentid'][1:] == 0
+    out['body_subtreemass'][0] = out['body_mass'][0] + out['body_subtreemass'][1:][children].sum()
+    meta.pop('ngeom_all', None)           # (the count of every geom of the compiled MJCF, visual ones included, is not recoverable here)
+    from .compiler.compile_model import dense_mass_matrix
+    M, _ = dense_mass_matrix({**out, **meta})
+    meta['stat_meaninertia'] = float(np.mean(np.diag(M)))
+    return FlyModel(out, meta)
 
 
 def from_compiled(m):
@@ -181,7 +229,7 @@ def reference_assets_dir():
     return None
 
 
-def variant_name(variant, force_actuators=False, use_wings=None, use_legs=None, joint_filter=None):
+def variant_name(variant, force_actuators=False, use_wings=None, use_legs=None, joint_filter=None, adhesion_filter=None):
     name = f'fly_{variant}'
     if force_actuators:
         name += '_force'
@@ -191,17 +239,20 @@ def variant_name(variant, force_actuators=False, use_wings=None, use_legs=None, 
         name += '_legs' if use_legs else '_nolegs'
     if joint_filter is not None:
         name += f'_jf{joint_filter:g}'
+    if adhesion_filter is not None:
+        name += f'_af{adhesion_filter:g}'
     return name
 
 
-def model_for(variant, force_actuators=False, use_wings=None, use_legs=None, joint_filter=None, cache_dir=None):
-    """The compiled model of a task (`variant` = walk / flight / vision) with the `FruitFly` switches the reference's env factories
-    expose (reference fly_envs.py:100-246: force_actuators, disable_wings, disable_legs, joint_filter; None = the task's default).
+def model_for(variant, force_actuators=False, use_wings=None, use_legs=None, joint_filter=None, cache_dir=None, adhesion_filter=None):
+    """The compiled model of a task (`variant` = walk / flight / vision / template) with the `FruitFly` switches the reference's env
+    factories expose (reference fly_envs.py:100-300: force_actuators, disable_wings, disable_legs, joint_filter, adhesion_filter;
+    None = the task's default).
     The default models ship pre-compiled (`assets/fly_*.npz`); any other combination is compiled from the reference's
     `fruitfly.xml` on first use (`flybody_b200.compiler`, ~2 s) and cached."""
-    if not force_actuators and use_wings is None and use_legs is None and joint_filter is None:
+    if not force_actuators and use_wings is None and use_legs is None and joint_filter is None and adhesion_filter is None:
         return load_model(variant)
-    name = variant_name(variant, force_actuators, use_wings, use_legs, joint_filter)
+    name = variant_name(variant, force_actuators, use_wings, use_legs, joint_filter, adhesion_filter)
     cache_dir = cache_dir or os.environ.get('FLYBODY_B200_CACHE') or os.path.join(os.path.expanduser('~'), '.cache', 'flybody_b200')
     for d in (ASSETS, cache_dir):
         p = os.path.join(d, name + '.npz')
@@ -214,7 +265,7 @@ def model_for(variant, force_actuators=False, use_wings=None, use_legs=None, joi
             "reference's fruitfly.xml was not found to compile it: install flybody or set FLYBODY_ASSETS to its fruitfly/assets directory")
     from .compiler import compile_model as cm
     m = cm.compile_variant(variant, assets_dir=src, mesh_cache=cm.load_mesh_cache(src), force_actuators=force_actuators, use_wings=use_wings,
-                           use_legs=use_legs, joint_filter=joint_filter)
+                           use_legs=use_legs, joint_filter=joint_filter, **({} if adhesion_filter is None else dict(adhesion_filter=adhesion_filter)))
     os.makedirs(cache_dir, exist_ok=True)
     p = os.path.join(cache_dir, name + '.npz')
     cm.save_model(m, p)

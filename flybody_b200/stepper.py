@@ -17,10 +17,10 @@ LIB_PATH = os.path.join(_HERE, 'lib', 'libflybody_b200.so')
 # enum FbField
 (QPOS, QVEL, ACT, CTRL, QACC, QACC_WARMSTART, SENSORDATA, SENSOR_MEAN, XPOS, XMAT, SITE_XPOS, SITE_XMAT,
  SUBTREE_COM, NCON, NEFC, TIME, QFRC_SMOOTH, QM_DENSE, QFRC_CONSTRAINT, SOLVER_NITER, QFRC_PASSIVE,
- QFRC_BIAS, QFRC_ACTUATOR, CONTACT, EFC_FORCE, FLAGS) = range(26)
+ QFRC_BIAS, QFRC_ACTUATOR, CONTACT, EFC_FORCE, FLAGS, QFRC_APPLIED, XFRC_APPLIED) = range(28)
 MAXCON, MAXEFC = 64, 160
 
-EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_step', 'fb_forward',
+EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_applied_ptrs', 'fb_clear_applied', 'fb_step', 'fb_forward',
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
            'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version']
 
@@ -88,6 +88,8 @@ def load_library(path=None):
     lib.fb_set_ctrl.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     lib.fb_set_action_map.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     lib.fb_write_state.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
+    lib.fb_applied_ptrs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    lib.fb_clear_applied.argtypes = [C.c_void_p]
     lib.fb_step.argtypes = [C.c_void_p, C.c_int]
     lib.fb_forward.argtypes = [C.c_void_p]
     lib.fb_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
@@ -197,6 +199,36 @@ class BatchedStepper:
         idx = np.ascontiguousarray(idx, np.int32)
         v = np.ascontiguousarray(np.broadcast_to(np.asarray(vals, np.float32), (self.n_envs, len(idx))))
         self._check(self._lib.fb_write_state(self._h, field, idx.ctypes.data, len(idx), v.ctypes.data), 'fb_write_state')
+
+    # ---- applied forces (mjData.qfrc_applied / xfrc_applied; persist until overwritten, zeroed by a reset of the env)
+    def set_applied(self, qfrc=None, xfrc=None, env_ids=None):
+        """qfrc [N or n, nv] generalized forces and / or xfrc [N or n, nbody, 6] world-frame force, then torque, at each body's CoM,
+        for every env (env_ids None; rows broadcast) or only the listed envs (the others keep theirs).  None leaves a field as is."""
+        for field, v, shape in ((QFRC_APPLIED, qfrc, (self.model.nv,)), (XFRC_APPLIED, xfrc, (self.model.nbody, 6))):
+            if v is None:
+                continue
+            v = np.asarray(v, np.float32)
+            if env_ids is None:
+                full = np.broadcast_to(v.reshape((-1,) + shape), (self.n_envs,) + shape)
+            else:
+                ids = np.asarray(env_ids, np.int64).reshape(-1)
+                full = self.get(field).reshape((self.n_envs,) + shape)
+                full[ids] = np.broadcast_to(v.reshape((-1,) + shape), (len(ids),) + shape)
+            self.set(field, np.ascontiguousarray(full).reshape(self.n_envs, -1))
+
+    def applied(self):
+        """-> (qfrc_applied [N, nv], xfrc_applied [N, nbody, 6]); zero while unset."""
+        return self.get(QFRC_APPLIED), self.get(XFRC_APPLIED).reshape(self.n_envs, self.model.nbody, 6)
+
+    def applied_ptrs(self):
+        """(qfrc_applied, xfrc_applied) device pointers of contiguous fp32 rows [N, nv], [N, nbody, 6] to write in place."""
+        q, x = C.c_void_p(), C.c_void_p()
+        self._check(self._lib.fb_applied_ptrs(self._h, C.byref(q), C.byref(x)), 'fb_applied_ptrs')
+        return q.value, x.value
+
+    def clear_applied(self):
+        """drop every env's applied forces: the step goes back to the path without them"""
+        self._check(self._lib.fb_clear_applied(self._h), 'fb_clear_applied')
 
     def reset(self, qpos=None, qvel=None, env_ids=None):
         n = self.n_envs if env_ids is None else len(env_ids)

@@ -177,7 +177,13 @@ enum FbField {
   FB_CONTACT = 23,    /* FB_MAXCON * 16: per contact [dist, pos3, normal3, geom1, geom2, dim, incl, mu, efc_adr, pad3] */
   FB_EFC_FORCE = 24,  /* FB_MAXEFC                                                  */
   FB_FLAGS = 25,      /* 1 (as float): bit0 bad state (nan/inf or |qacc|>1e14), bit1 contact overflow, bit2 efc overflow */
-  FB_NFIELDS = 26
+  FB_QFRC_APPLIED = 26, /* nv : physics.data.qfrc_applied, generalized forces added to qfrc_smooth every substep           */
+  FB_XFRC_APPLIED = 27, /* nbody*6 : physics.data.xfrc_applied, per body a world-frame force, then torque, applied at the
+                           body's CoM (mj_xfrcAccumulate: qfrc_smooth += J^T wrench over the body's ancestor dofs).
+                           Both (fb_set, fb_write_state, fb_get with is_device = 0) persist across substeps and steps until
+                           overwritten, are zeroed for the envs of fb_reset / fb_reset_hold / a device-task reset
+                           (mj_resetData), and read as zero while unset                                                  */
+  FB_NFIELDS = 28
 };
 
 #define FB_MAXCON 64     /* contact slots per env   */
@@ -210,9 +216,16 @@ int fb_set_ctrl(FbHandle h, const float* ctrl, int is_device);
 int fb_set_action_map(FbHandle h, const int32_t* ctrl_index, int n_action);
 
 /* walker.set_pose / set_velocity on a subset of coordinates (walk_imitation.py:141-145):
- * field in {FB_QPOS, FB_QVEL, FB_ACT}; vals is [N][k] AoS host, written to coordinates idx[k]
- * of every env.  No forward pass is run (dm_control does not run one either).               */
+ * field in {FB_QPOS, FB_QVEL, FB_ACT, FB_QFRC_APPLIED, FB_XFRC_APPLIED}; vals is [N][k] AoS host (k <= 16), written to
+ * coordinates idx[k] of every env.  No forward pass is run (dm_control does not run one either).                        */
 int fb_write_state(FbHandle h, int field, const int32_t* idx, int k, const float* vals);
+/* physics.data.qfrc_applied / physics.data.xfrc_applied in place, for a policy on the GPU: borrowed device pointers of the
+ * compact rows [n_envs][nv] and [n_envs][nbody][6] (fp32, contiguous; allocated zeroed on first use, which any applied-force
+ * call does).  Writes on another stream must be ordered before the next fb_step / fb_task_step on fb_stream.           */
+int fb_applied_ptrs(FbHandle h, void** qfrc_applied_dev, void** xfrc_applied_dev);
+/* Drop qfrc_applied and xfrc_applied of every env (mjData's are zero-filled; here the buffers are freed and the step goes
+ * back to the path without the applied-force term).  Pointers of fb_applied_ptrs become invalid.                      */
+int fb_clear_applied(FbHandle h);
 
 /* n_substeps x physics.step() with legacy_step=True, i.e. (mj_step2; mj_step1) per substep
  * (SURVEY.md App. A), accumulating the per-substep sensor mean.  Asynchronous on the handle's
@@ -292,7 +305,10 @@ int fb_read_obs(FbHandle h, float* host_dst);
  * fb_ref_bank_wide / fb_ref_bank, then this program; every env draws its own trajectory (and, flight, start step) of the bank at
  * each reset).  Requires fb_set_action_map and fb_obs_program first.                                                 */
 typedef struct FbTaskProgram {
-  int32_t kind;                        /* 0 walk_imitation, 1 flight_imitation, 2 vision_guided_flight (fields at the end of the struct) */
+  int32_t kind;                        /* 0 walk_imitation, 1 flight_imitation, 2 vision_guided_flight (fields at the end of the struct),
+                                          3 template_task (tasks/template_task.py): reset to reset_qpos at rest, no ghost / reference /
+                                          before_step hook; reward 1, LAST with discount 0 on a bad state or |qacc| > terminal_qacc,
+                                          LAST with discount 1 at time_limit (ghost_qadr = user_col = -1, no noise) */
   int32_t root_qadr, root_vadr, ghost_qadr, ghost_vadr;   /* free-joint slots of the walker root and of the ghost */
   int32_t user_col;                    /* column of the beat-frequency action in the action row, -1 if none */
   float ghost_offset[3];
