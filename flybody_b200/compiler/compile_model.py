@@ -9,6 +9,8 @@ Variants
   walk   : `walk_imitation()` model  (reference `fly_envs.py:100-155`, `tasks/base.py:367-428`,
            `tasks/walk_imitation.py:22-85`) : walker (nq 109, nv 108, nu 59) + ghost free body
   flight : `flight_imitation()` model (reference `fly_envs.py:30-97`, `tasks/base.py:271-364`)
+  ball   : `walk_on_ball()` model (reference `fly_envs.py:158-191`, `tasks/walk_on_ball.py`, `tasks/arenas/ball.py`): the BallFloor
+           arena's ball (ball joint: nq 4, nv 3) first, then the walker with its thorax welded to the world
 """
 import json
 import os
@@ -29,7 +31,7 @@ _SPAWN_POS = np.array((0, 0, 0.1278))    # reference fruitfly.py:23
 GEOM_PLANE, GEOM_SPHERE, GEOM_CAPSULE, GEOM_ELLIPSOID, GEOM_CYLINDER, GEOM_BOX = 0, 2, 3, 4, 5, 6
 GEOM_HFIELD = 1
 GEOM_TYPES = {'plane': 0, 'sphere': 2, 'capsule': 3, 'ellipsoid': 4, 'cylinder': 5, 'box': 6, 'mesh': 7}
-JNT_FREE, JNT_HINGE = 0, 3
+JNT_FREE, JNT_BALL, JNT_HINGE = 0, 1, 3
 TRN_JOINT, TRN_TENDON, TRN_BODY = 0, 1, 2
 DYN_NONE, DYN_FILTER, DYN_FILTEREXACT = 0, 2, 3
 SENS_TOUCH, SENS_ACC, SENS_VEL, SENS_GYRO, SENS_FORCE = 0, 1, 2, 3, 4
@@ -341,6 +343,20 @@ def compile_variant(variant='walk', assets_dir=None, inertia_mode='legacy2', mes
                            force_actuators=force_actuators, dyntype_filterexact=dyntype_filterexact)
         timestep = float(fx.root.find('option').get('timestep'))
         spawn, prefix = np.zeros(3), ''
+    elif variant == 'ball':
+        # walk_on_ball (reference fly_envs.py:158-191, tasks/walk_on_ball.py:18-43): the Walking surgery without the ghost, the walker's
+        # free joint removed (its thorax welded to the world at the spawn pose), one exclude between the thorax and each of its child
+        # bodies, and the BallFloor arena (tasks/arenas/ball.py) instead of the floor plane
+        fx = build_fly_xml(xml_path, name='walker', use_legs=True if use_legs is None else use_legs,
+                           use_wings=False if use_wings is None else use_wings, use_mouth=False, use_antennae=False,
+                           joint_filter=0.01 if joint_filter is None else joint_filter, adhesion_filter=adhesion_filter,
+                           force_actuators=force_actuators, dyntype_filterexact=dyntype_filterexact)
+        timestep = 2e-4                                  # reference tasks/constants.py:11
+        spawn, prefix = _SPAWN_POS, 'walker/'
+        _add_wing_leg_excludes(fx)                        # base.py:404-411
+        _add_thorax_excludes(fx)                          # walk_on_ball.py:30-38
+        if claw_friction is not None:                     # walk_on_ball.py:40-44
+            fx.class_child('adhesion-collision', 'geom').set('friction', repr(float(claw_friction)))
     elif variant in ('walk', 'template'):
         # template: template_task (reference fly_envs.py:249-300, tasks/template_task.py:35-43), the same Walking surgery
         # without the ghost (add_ghost=False), with the factory's adhesion filter
@@ -407,8 +423,10 @@ def compile_variant(variant='walk', assets_dir=None, inertia_mode='legacy2', mes
 
     classes = parse_defaults(fx.root)
     bodies = [Body('world', -1, np.zeros(3), np.array([1.0, 0, 0, 0]))]
+    if variant == 'ball':             # the arena is built before the walker is attached: its body, joint, qpos and dofs come first
+        bodies.append(_ball_body())
     _extract_bodies(fx, classes, prefix, mesh_cache, inertia_mode, bodies, 0, spawn,
-                    root_free=(variant not in ('bare', 'walker')))
+                    root_free=(variant not in ('bare', 'walker', 'ball')))
     n_walker_bodies = len(bodies)
 
     # excludes -> body-name pairs
@@ -459,6 +477,32 @@ def _bare_xml(xml_path):
     return fx
 
 
+def _ball_body(pos=(-0.05, 0, -0.419), radius=0.454, density=0.0025):
+    """BallFloor's ball as walk_on_ball builds it (reference fly_envs.py:174-177, tasks/arenas/ball.py:60-67): a sphere on a ball
+    joint, with Walking's ground-geom contact parameters (base.py:398-401)"""
+    b = Body('ball', 0, np.array(pos, float), np.array([1.0, 0, 0, 0]))
+    b.joints.append(dict(name='ball', type=JNT_BALL, axis=np.array([0.0, 0, 1]), pos=np.zeros(3), range=np.zeros(2), limited=0,
+                         stiffness=0.0, damping=0.0, armature=0.0, springref=0.0, ref=0.0, solref=np.array([0.02, 1.0]),
+                         solimp=np.array([0.9, 0.95, 0.001, 0.5, 2.0]), margin=0.0, springdamper=np.zeros(2)))
+    size = np.array([radius, 0.0, 0.0])
+    V, Id = primitive_props(GEOM_SPHERE, size)
+    b.geoms.append(dict(name='', type=GEOM_SPHERE, pos=np.zeros(3), quat=np.array([1.0, 0, 0, 0]), size=size, contype=1,
+                        conaffinity=1, condim=3, priority=0, friction=np.array([0.5, 0.005, 0.0001]), solmix=1.0,
+                        solref=np.array([0.001, 1.0]), solimp=np.array([0.95, 0.99, 0.01, 0.5, 2.0]), margin=0.0, gap=0.0,
+                        fluidshape='none', fluidcoef=np.array([0.5, 0.25, 1.5, 1.0, 1.0]), mass=density * V, com=np.zeros(3),
+                        inertia=density * np.diag(Id)))
+    return b
+
+
+def _add_thorax_excludes(fx):
+    contact = fx.root.find('contact')
+    thorax = next(b for b in fx.all('body') if b.get('name') == 'thorax')
+    for child in thorax:
+        if child.tag == 'body':
+            ET.SubElement(contact, 'exclude', name=f"thorax_{child.get('name')}", body1='thorax', body2=child.get('name'))
+    fx._reindex()
+
+
 def _add_wing_leg_excludes(fx):
     contact = fx.root.find('contact')
     for body in fx.all('body'):
@@ -500,6 +544,11 @@ def _flatten(bodies, classes, fx, prefix, actuators, tendons, sensors, excludes,
                 qspring += list(b.pos) + list(b.quat)
                 nq += 7
                 nd = 6
+            elif j['type'] == JNT_BALL:
+                qpos0 += [1.0, 0.0, 0.0, 0.0]
+                qspring += [1.0, 0.0, 0.0, 0.0]
+                nq += 4
+                nd = 3
             else:
                 qpos0.append(j['ref'])
                 qspring.append(j['springref'])
@@ -834,6 +883,15 @@ def kinematics0(m, qpos=None):
                     dof_istrans[da + i] = True
                     dof_axis[da + 3 + i] = R[:, i]
                     dof_anchor[da + 3 + i] = pos
+            elif m['jnt_type'][j] == JNT_BALL:
+                # rotation about the anchor (MuJoCo mj_kinematics); the dof axes are the body frame's columns (mj_comPos)
+                anchor = pos + qrot(quat, m['jnt_pos'][j])
+                quat = qmul(quat, qnorm(qpos[qa:qa + 4]))
+                pos = anchor - qrot(quat, m['jnt_pos'][j])
+                R = q2mat(quat)
+                for i in range(3):
+                    dof_axis[da + i] = R[:, i]
+                    dof_anchor[da + i] = anchor
             else:
                 anchor = pos + qrot(quat, m['jnt_pos'][j])
                 axis = qrot(quat, m['jnt_axis'][j])
@@ -907,6 +965,8 @@ def _set0(m):
             d = np.diag(Minv)[da:da + 6]
             diw[da:da + 3] = d[:3].mean()
             diw[da + 3:da + 6] = d[3:].mean()
+        elif m['jnt_type'][j] == JNT_BALL:
+            diw[da:da + 3] = np.diag(Minv)[da:da + 3].mean()
         else:
             diw[da] = Minv[da, da]
     m['dof_invweight0'] = diw

@@ -1020,7 +1020,7 @@ FB_DEV void kfin_f8(FB_PHASE_ARGS) {
   const float h = m.timestep;
   for (int k = y; k < m.nv; k += FB_NY) {
     const int j = m.dof_jntid[k];
-    if (m.jnt_type[j] == FB_JNT_FREE) continue;
+    if (m.jnt_type[j] != FB_JNT_HINGE) continue;          // free and ball joints: integrate_body
     const float v = AT(d.qvel, k) + h * XS(k);
     AT(d.qvel, k) = v; AT(d.qpos, m.jnt_qposadr[j]) += h * v;
   }
@@ -1091,6 +1091,17 @@ FB_DEV void kfin_f10(FB_PHASE_ARGS) {
   float s2 = 0; for (int l = 0; l < FB_NY; l++) s2 += sh.red[l][lane];
   if (!(s2 < 1e28f)) FB_FLAG_OR(1);
 }
+// a ball joint: qvel += h qacc, then the quaternion qpos[qa .. qa + 3] turned by the body-frame angular velocity over one step (MuJoCo
+// mju_quatIntegrate; the free joint's branch restates it)
+FB_DEV void integrate_ball(const DevData& d, int e, int lane, const float* xs, int qa, int da, float h) {
+  for (int i = 0; i < 3; i++) { AT(d.qvel, da + i) += h * XS(da + i); }
+  V3 w = v3(AT(d.qvel, da), AT(d.qvel, da + 1), AT(d.qvel, da + 2));
+  float ang = norm(w) * h;
+  Q4 q = q4(AT(d.qpos, qa), AT(d.qpos, qa + 1), AT(d.qpos, qa + 2), AT(d.qpos, qa + 3));
+  if (ang > 0) q = qmul(q, axisangle(normalized(w), ang));
+  q = qnormalize(q);
+  AT(d.qpos, qa) = q.w; AT(d.qpos, qa + 1) = q.x; AT(d.qpos, qa + 2) = q.y; AT(d.qpos, qa + 3) = q.z;
+}
 FB_DEV void integrate_body(const DevModel& m, const DevData& d, int e, int lane, const float* xs, int b) {
   float h = m.timestep;
   for (int k = 0; k < m.body_jntnum[b]; k++) {
@@ -1104,6 +1115,8 @@ FB_DEV void integrate_body(const DevModel& m, const DevData& d, int e, int lane,
       if (ang > 0) q = qmul(q, axisangle(normalized(w), ang));
       q = qnormalize(q);
       AT(d.qpos, qa + 3) = q.w; AT(d.qpos, qa + 4) = q.x; AT(d.qpos, qa + 5) = q.y; AT(d.qpos, qa + 6) = q.z;
+    } else if (m.jnt_type[j] == FB_JNT_BALL) {
+      FB_NO_MERGE(); integrate_ball(d, e, lane, xs, qa, da, h); FB_NO_MERGE();
     } else {
       AT(d.qvel, da) += h * XS(da);
       AT(d.qpos, qa) += h * AT(d.qvel, da);
@@ -1321,7 +1334,7 @@ FB_DEV void ktask_reset2(const DevModel& m, const DevData& d, int e, int y) {   
   if (!t.needs_reset[e]) return;
   const int episode = t.episode[e];
   if (t.kind == 2) { ktask_reset_vision(m, d, t, e, y, episode); return; }
-  if (t.kind == 3) {          // template_task: the template pose as copied, at rest (no reference, no ghost)
+  if (t.kind == 3 || t.kind == 4) {          // template_task, walk_on_ball: the template pose as copied, at rest (no reference, no ghost)
     if (y == 0) { AT(d.time, 0) = 0; AT(d.flags, 0) = 0; AT(d.hold, 0) = 1; AT(d.prev_n, 0) = 0; t.step[e] = 0; t.has_uniform[e] = 0; }
     return;
   }
@@ -1492,6 +1505,18 @@ FB_DEV void ktask_after(const DevModel& m, const DevData& d, int e, int y) {
     const bool last = bad || (double)step_now * (double)t.dt >= (double)t.time_limit - 1e-9;
     float* out = t.out + 4 * (size_t)e;
     out[0] = resetting ? 0.0f : 1.0f; out[1] = resetting ? 1.0f : (bad ? 0.0f : 1.0f); out[2] = resetting ? 0.0f : (last ? 2.0f : 1.0f); out[3] = 0.0f;
+    t.needs_reset[e] = (last && !resetting) ? 1 : 0;
+    return;
+  }
+  if (t.kind == 4) {      // walk_on_ball (tasks/walk_on_ball.py:55-81): ball-velocity reward; velocimeter / gyro / bad state end an episode, discount 0
+    const float* lv = &AT(d.sensordata, t.velocimeter_adr); const float* av = &AT(d.sensordata, t.gyro_adr);
+    const float linvel = sqrtf(lv[0] * lv[0] + lv[1] * lv[1] + lv[2] * lv[2]), angvel = sqrtf(av[0] * av[0] + av[1] * av[1] + av[2] * av[2]);
+    terminate = linvel > t.term_linvel || angvel > t.term_angvel || bad;
+    reward = 1.0f;
+    for (int i = 0; i < 3; i++) reward *= tk_lin_tol(AT(d.qvel, t.ball_vadr + i) - t.ball_target[i], t.ball_margin);
+    const bool last = terminate || (double)step_now * (double)t.dt >= (double)t.time_limit - 1e-9;
+    float* out = t.out + 4 * (size_t)e;
+    out[0] = resetting ? 0.0f : reward; out[1] = resetting ? 1.0f : (terminate ? 0.0f : 1.0f); out[2] = resetting ? 0.0f : (last ? 2.0f : 1.0f); out[3] = 0.0f;
     t.needs_reset[e] = (last && !resetting) ? 1 : 0;
     return;
   }

@@ -35,6 +35,21 @@ template <typename Sh> FB_DEV float* sh_dyn(Sh& sh) { return reinterpret_cast<fl
 
 // ---------------------------------------------------------------------------------------------
 // K1 kinematics (MuJoCo mj_kinematics + mj_comPos; reference model fruitfly.xml:307-731)
+// Ball joints (MuJoCo's BALL cases; the free joint's branches restate them for its rotational half), called between FB_NO_MERGE barriers.
+// Pose: the normalised quaternion from qpos turns the body about the anchor (mj_kinematics); the dof axes are the columns of the
+// body frame (mj_comPos)
+FB_DEV void ball_pose(const DevModel& m, const DevData& d, int e, int j, int qa, int da, V3& pos, Q4& quat) {
+  V3 jp = mld3(m.jnt_pos, j);
+  V3 anchor = pos + mul(q2m(quat), jp);
+  quat = qmul(quat, qnormalize(q4(AT(d.qpos, qa), AT(d.qpos, qa + 1), AT(d.qpos, qa + 2), AT(d.qpos, qa + 3))));
+  M3 R = q2m(quat);
+  pos = anchor - mul(R, jp);
+  for (int i = 0; i < 3; i++) {
+    V3 ax = col(R, i);
+    st3(d.Sang, da + i, d, e, ax);
+    st3(d.Slin, da + i, d, e, cross(anchor, ax));
+  }
+}
 // chain part: pose of body b from its parent's pose (pp, pq) and the joint coordinates; writes xpos, xquat
 // and the motion subspaces of the body's dofs.  Returns the body's pose for the next link of the chain.
 FB_DEV void body_pose(const DevModel& m, const DevData& d, int e, int b, V3 ppos, Q4 pq, V3 ref, V3& pos, Q4& quat) {
@@ -44,7 +59,8 @@ FB_DEV void body_pose(const DevModel& m, const DevData& d, int e, int b, V3 ppos
   int jn = MLD(m.body_jntnum[b]);
   for (int k = 0; k < jn; k++) {
     int j = MLD(m.body_jntadr[b]) + k, qa = MLD(m.jnt_qposadr[j]), da = MLD(m.jnt_dofadr[j]);
-    if (MLD(m.jnt_type[j]) == FB_JNT_FREE) {
+    const int jt = MLD(m.jnt_type[j]);
+    if (jt == FB_JNT_FREE) {
       pos = v3(AT(d.qpos, qa), AT(d.qpos, qa + 1), AT(d.qpos, qa + 2)) - ref;
       quat = qnormalize(q4(AT(d.qpos, qa + 3), AT(d.qpos, qa + 4), AT(d.qpos, qa + 5), AT(d.qpos, qa + 6)));
       M3 R = q2m(quat);
@@ -56,6 +72,8 @@ FB_DEV void body_pose(const DevModel& m, const DevData& d, int e, int b, V3 ppos
         st3(d.Sang, da + 3 + i, d, e, ax);
         st3(d.Slin, da + 3 + i, d, e, cross(pos, ax));
       }
+    } else if (jt == FB_JNT_BALL) {
+      FB_NO_MERGE(); ball_pose(m, d, e, j, qa, da, pos, quat); FB_NO_MERGE();
     } else {
       M3 R = q2m(quat);
       V3 jp = mld3(m.jnt_pos, j), ja = mld3(m.jnt_axis, j);
@@ -525,6 +543,20 @@ FB_WARPFN void tri_solve(const DevModel& m, const DevData& d, ShTree& sh, int e)
 // K4 velocities + RNE bias, K5-K7 passive forces (MuJoCo mj_comVel, mj_rne, mj_passive)
 FB_DEV S6 motion_cross(const S6& v, V3 Sa, V3 Sl) { S6 r; r.a = cross(v.a, Sa); r.l = cross(v.a, Sl) + cross(v.l, Sa); return r; }
 
+// The three dofs da .. da + 2 of a ball joint (MuJoCo mj_comVel's BALL case, which FREE falls through to):
+// v += S qd (qacc != nullptr: a += S qacc) and the cdof_dot term.  Ball joints sit on root bodies (fb_create), so the velocity before
+// them is (0, vlin) and sum_i cdof_dot_i qd_i = (0, vlin x w).
+FB_DEV void rot3_vel_acc(const DevData& d, int e, int da, V3 vlin, const float* qacc, S6& v, S6& a) {
+  V3 w = v3(0, 0, 0);
+  for (int i = 0; i < 3; i++) {
+    float qd = AT(d.qvel, da + i);
+    V3 Sa = ld3(d.Sang, da + i, d, e), Sl = ld3(d.Slin, da + i, d, e);
+    v.a = v.a + Sa * qd; v.l = v.l + Sl * qd;
+    w = w + Sa * qd;
+    if (qacc) { float qa = AT(qacc, da + i); a.a = a.a + Sa * qa; a.l = a.l + Sl * qa; }
+  }
+  a.l = a.l + cross(vlin, w);
+}
 // forward recursion for one body; qacc == nullptr -> bias acceleration only
 FB_DEV void body_vel_acc(const DevModel& m, const DevData& d, int e, int b, const float* qacc, float* bvel, float* bacc) {
   int p = m.body_parentid[b];
@@ -542,7 +574,8 @@ FB_DEV void body_vel_acc(const DevModel& m, const DevData& d, int e, int b, cons
         if (qacc) { float qa = AT(qacc, da + i); a.a = a.a + Sa * qa; a.l = a.l + Sl * qa; }
       }
       a.l = a.l + cross(vlin, w);
-    } else {
+    } else if (m.jnt_type[j] == FB_JNT_BALL) { FB_NO_MERGE(); rot3_vel_acc(d, e, da, v.l, qacc, v, a); FB_NO_MERGE(); }
+    else {
       float qd = AT(d.qvel, da);
       V3 Sa = ld3(d.Sang, da, d, e), Sl = ld3(d.Slin, da, d, e);
       S6 r = motion_cross(v, Sa, Sl);
@@ -667,7 +700,8 @@ FB_DEV void vel_acc_from_parent(const DevModel& m, const DevData& d, int e, int 
         if (i >= 3) w = w + Sa * qd;
       }
       a.l = a.l + cross(vlin, w);
-    } else {
+    } else if (m.jnt_type[j] == FB_JNT_BALL) { FB_NO_MERGE(); rot3_vel_acc(d, e, da, v.l, nullptr, v, a); FB_NO_MERGE(); }
+    else {
       float qd = AT(d.qvel, da);
       V3 Sa = ld3(d.Sang, da, d, e), Sl = ld3(d.Slin, da, d, e);
       S6 r = motion_cross(v, Sa, Sl);

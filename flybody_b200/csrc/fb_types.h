@@ -202,8 +202,14 @@ struct DevTask {
   float *uniform /* [N][8] */, *wb_freq;
   int* op_step; unsigned char* op_first;   // the observation program's per-env inputs, maintained here instead of by fb_task_inputs
   float* out;                              // [N][4] reward, discount, step_type (0 FIRST, 1 MID, 2 LAST), 0
+  // kind 4 (walk_on_ball): the ball joint's first dof, the target ball velocity and the reward's margin
+  int ball_vadr; float ball_target[3], ball_margin;
 };
 
+// A compiler barrier at both ends of a branch that only some models take (ball joints).  Without it the optimiser may hoist
+// or sink arithmetic that branch shares with its neighbours (free and hinge joints) across the branch, so that a multiply and its add
+// end up in different blocks and are no longer fused: the other models' results would change in the last bits.
+#define FB_NO_MERGE() asm volatile("" ::: "memory")
 #ifdef __CUDACC__
 #define FB_FLAG_OR(bit) atomicOr(&AT(d.flags, 0), (bit))
 #else

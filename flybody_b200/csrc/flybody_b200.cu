@@ -341,8 +341,17 @@ static int build_model(FbSim* s, const FbModel* h) {
   for (int b = 1; b < nb; b++) if (h->body_parentid[b] == 0) { roots.push_back(b); isroot[b] = 1; }
   isroot[0] = 1;   // the world behaves like a root for "parent is root" tests (never accumulated into)
   for (int r : roots) {
-    if (!(h->body_jntnum[r] == 0 || (h->body_jntnum[r] == 1 && h->jnt_type[h->body_jntadr[r]] == FB_JNT_FREE))) { s->err = "root bodies must carry a single free joint or none"; return -3; }
+    const int jt = h->body_jntnum[r] == 1 ? h->jnt_type[h->body_jntadr[r]] : -1;
+    if (!(h->body_jntnum[r] == 0 || jt == FB_JNT_FREE || jt == FB_JNT_BALL)) { s->err = "root bodies must carry a single free or ball joint or none"; return -3; }
   }
+  for (int j = 0; j < h->njnt; j++) {
+    if (h->jnt_type[j] != FB_JNT_BALL) continue;
+    // ball joints are stepped as the rotational half of a free joint: no quaternion spring, no cone limit (neither is implemented)
+    if (h->body_parentid[h->jnt_bodyid[j]] != 0) { s->err = "ball joints are implemented on root bodies only"; return -3; }
+    if (h->jnt_stiffness[j] != 0 || h->jnt_limited[j]) { s->err = "ball joints with stiffness or limits are not implemented"; return -3; }
+  }
+  for (int j = 0; j < h->njnt; j++)
+    if (h->jnt_type[j] != FB_JNT_FREE && h->jnt_type[j] != FB_JNT_BALL && h->jnt_type[j] != FB_JNT_HINGE) { s->err = "joint type not implemented (free, ball and hinge are)"; return -3; }
   std::vector<std::vector<int>> subtrees; std::vector<int> sub_root;
   for (size_t ri = 0; ri < roots.size(); ri++) {
     for (int b = 1; b < nb; b++) if (h->body_parentid[b] == roots[ri]) {
@@ -1231,9 +1240,10 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
       for (int k = 0; k < 4; k++) if (!(p->deep_mimic_std[k] > 0)) { s->err = "fb_task_program: deep_mimic_std must be positive"; return -1; }
       if (!(p->retract_margin > 0)) { s->err = "fb_task_program: retract_margin must be positive"; return -1; }
     }
-  } else if (p->kind == 3) {
-    if (p->ghost_qadr >= 0 || p->user_col >= 0 || p->n_noise > 0) { s->err = "fb_task_program: kind 3 (template_task) has no ghost, user action or reset noise"; return -1; }
-  } else if (p->kind < 0 || p->kind > 3) { s->err = "fb_task_program: unknown kind"; return -1;
+  } else if (p->kind == 3 || p->kind == 4) {
+    if (p->ghost_qadr >= 0 || p->user_col >= 0 || p->n_noise > 0) { s->err = "fb_task_program: kinds 3 and 4 (template_task, walk_on_ball) have no ghost, user action or reset noise"; return -1; }
+    if (p->kind == 4 && (p->ball_vadr < 0 || p->ball_vadr + 3 > s->m.nv || !(p->ball_margin > 0))) { s->err = "fb_task_program: kind 4 needs the ball's dofs (ball_vadr) and a positive ball_margin"; return -1; }
+  } else if (p->kind < 0 || p->kind > 4) { s->err = "fb_task_program: unknown kind"; return -1;
   } else if (p->ref_len <= 0 || !p->ref_qpos || !p->ref_qvel) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
   if (!p->reset_qpos) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
   if (p->kind == 2 && (!s->bank_dev || !s->hfield_dev || s->bank_n <= 0)) { s->err = "fb_task_program: kind 2 needs fb_hfield_collision / fb_eye_program and fb_hfield_bank first"; return -1; }
@@ -1253,7 +1263,8 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   auto upf32 = [&](const float* src, size_t n) { std::vector<float> v(src, src + n); return up(s, v); };
   auto upi32 = [&](const int32_t* src, size_t n) { std::vector<int> v(src, src + n); return up(s, v); };
   t.reset_qpos = upf32(p->reset_qpos, m.nq);
-  if (!bank && p->kind != 3) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
+  if (p->kind == 4) { t.ball_vadr = p->ball_vadr; for (int i = 0; i < 3; i++) t.ball_target[i] = p->ball_target[i]; t.ball_margin = p->ball_margin; }
+  if (!bank && p->kind != 3 && p->kind != 4) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
   else t.ref_len = 0;
   t.n_noise = p->noise_qadr ? p->n_noise : 0; t.noise_qadr = t.n_noise ? upi32(p->noise_qadr, t.n_noise) : nullptr; t.noise_amp = p->noise_amp; t.seed = p->seed;
   if (p->kind == 1 || p->kind == 2) {

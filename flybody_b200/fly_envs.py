@@ -195,6 +195,10 @@ class TemplateTask:
         self._max_episode_steps = round(time_limit / control_timestep)
 
 
+class WalkOnBallTask(TemplateTask):
+    """What the reference's callers reach through `env.task` of `walk_on_ball` (`tasks/walk_on_ball.py`)."""
+
+
 class FlightImitationTask(_ImitationTask):
     """Batched `FlightImitationWBPG` (reference `tasks/flight_imitation.py:16-212`, `tasks/base.py:271-364`)."""
 
@@ -213,6 +217,9 @@ _VARIANTS = {
     # template_task: the walker's observables only (reference tests/test_core.py:9-20)
     'template': dict(dt=_WALK_CONTROL_TIMESTEP, obs=('accelerometer', 'actuator_activation', 'appendages_pos', 'force', 'gyro',
                                                      'joints_pos', 'joints_vel', 'touch', 'velocimeter', 'world_zaxis')),
+    # walk_on_ball: the walker's observables, then the task's ball_qvel (reference tasks/walk_on_ball.py:46)
+    'ball': dict(dt=_WALK_CONTROL_TIMESTEP, obs=('accelerometer', 'actuator_activation', 'appendages_pos', 'force', 'gyro',
+                                                 'joints_pos', 'joints_vel', 'touch', 'velocimeter', 'world_zaxis', 'ball_qvel')),
 }
 
 
@@ -242,6 +249,9 @@ class BatchedFlyEnv:
         elif variant == 'template':
             self.task = TemplateTask(self, time_limit, self._control_timestep)
             self._n_user = 0
+        elif variant == 'ball':
+            self.task = WalkOnBallTask(self, time_limit, self._control_timestep)
+            self._n_user = 0
         else:
             self._wbpg = BatchedWingBeatPatternGenerator(self.n_envs, base_pattern_path=wpg_pattern_path)
             self.task = FlightImitationTask(self, self._wbpg, traj_generator or InferenceFlightTrajectoryLoader(),
@@ -261,7 +271,7 @@ class BatchedFlyEnv:
         # walking: actions go to the device as they are, the action -> ctrl permutation and NaN -> 0 run in the scatter
         # kernel (fb_set_action_map); flight keeps the host path because the wing actions are modified by the WBPG first
         self._device_task = bool(device_task)       # task hooks evaluated on the device (fb_task_*): no host logic in step()
-        self._device_action_map = variant in ('walk', 'template') or self._device_task
+        self._device_action_map = variant in ('walk', 'template', 'ball') or self._device_task
         if self._device_action_map:
             # user actions (flight: the beat frequency) have no ctrl slot: column -> -1, read by the device-side task code
             self._sim.set_action_map(np.concatenate([self._ctrl_of_action, -np.ones(self._n_user, np.int64)]) if self._device_task
@@ -273,8 +283,10 @@ class BatchedFlyEnv:
         self._action_spec = BoundedArray((len(names),), np.float64, lo, hi, name='\t'.join(names))
         # --- index tables
         jn = m.meta['jnt_names']
-        self._root_q = m.jnt_qposadr_of('walker/')
-        self._root_v = m.jnt_dofadr_of('walker/')
+        # the walker's free joint (-1: none, walk_on_ball's thorax is welded to the world)
+        self._root_q = m.jnt_qposadr_of('walker/') if 'walker/' in jn else -1
+        self._root_v = m.jnt_dofadr_of('walker/') if 'walker/' in jn else -1
+        self._ball_v = m.jnt_dofadr_of('ball') if 'ball' in jn else -1
         self._ghost_q = m.jnt_qposadr_of('ghost/') if 'ghost/' in jn else -1      # (template_task: no ghost)
         self._ghost_v = m.jnt_dofadr_of('ghost/') if 'ghost/' in jn else -1
         obsj = [jn.index(n) for n in m.meta['observable_joints']]
@@ -383,6 +395,7 @@ class BatchedFlyEnv:
             'world_zaxis': (3, (3,), (st.OBS_ROOT_ZAXIS, 0, 3)),
             'ref_displacement': (3 * f, (f, 3), (st.OBS_REF_DISP, 0, f)),
             'ref_root_quat': (4 * f, (f, 4), (st.OBS_REF_QUAT, 0, f)),
+            'ball_qvel': (3, (3,), (st.OBS_QVEL, o_v + nq, 3)),        # qvel of the ball joint after the last substep
         }
         if 'force' in sd:
             full['force'] = (len(sd['force']), (len(sd['force']),), (st.OBS_SENSOR_MEAN, sd['force'][0], len(sd['force'])))
@@ -433,10 +446,12 @@ class BatchedFlyEnv:
         lists = list(self._app_sites) + list(self._obs_qadr) + list(self._obs_vadr)
         if self._variant == 'flight':
             lists += list(range(self._ghost_q, self._ghost_q + 7))
+        if self._variant == 'ball':
+            lists += list(range(self._ball_v, self._ball_v + 3))
         if not self._inference_mode:
             lists += list(range(self._root_v, self._root_v + 6)) + list(self._mocap_qadr) + list(self._mocap_vadr) \
                 + list(self._mocap_sites) + list(self._wing_qadr)
-        shared = None if self._variant == 'template' else self._ref_qpos[:, :7] if not self._per_env_ref else np.zeros((self._future, 7))
+        shared = None if self._variant in ('template', 'ball') else self._ref_qpos[:, :7] if not self._per_env_ref else np.zeros((self._future, 7))
         dim = self._sim.obs_program([r[3] for r in rows], lists, m.body_id('walker/thorax'), self._n_sub, shared)
         if self._per_env_ref:
             self._sim.ref_slots(self._slot_len)
@@ -1044,11 +1059,6 @@ def vision_guided_flight(wpg_pattern_path=None, bumps_or_trench='bumps', force_a
                                   seed=seed, **kwargs_arena)
 
 
-def walk_on_ball(*args, **kwargs):
-    """`flybody.fly_envs.walk_on_ball` (reference `fly_envs.py:158-191`): outside the hot-path scope (SURVEY.md section 8)."""
-    raise NotImplementedError(walk_on_ball.__doc__)
-
-
 class TemplateTaskEnv(BatchedFlyEnv):
     """Batched `TemplateTask` (reference `tasks/template_task.py`): the walker on the flat Walking floor without a ghost or a
     reference.  Every episode starts from the template pose at rest (`qpos0`, the upright spawn); the reward is 1; an episode ends
@@ -1165,3 +1175,64 @@ def template_task(random_state=None, force_actuators=False, disable_wings=True, 
                           adhesion_filter=None if adhesion_filter == 0.007 else adhesion_filter)
     return TemplateTaskEnv(n_envs, time_limit=time_limit, action_corruptor=action_corruptor, random_state=random_state, device=device,
                            lib_path=lib_path, seed=seed, device_task=device_task, model=model)
+
+
+_BALL_TARGET_QVEL = (0.0, -5.0, 0.0)            # target ball angular velocity of walk_on_ball (tasks/walk_on_ball.py:67)
+_BALL_MARGIN = 6.0                              # ... and the margin of its linear tolerance
+
+
+class WalkOnBallEnv(TemplateTaskEnv):
+    """Batched `WalkOnBall` (reference `tasks/walk_on_ball.py`, `tasks/arenas/ball.py`): the fly tethered at its spawn pose (thorax
+    welded to the world) walks on a floating ball.  Every episode starts from `qpos0` at rest (mj_resetData: the ball's quaternion is
+    the identity).  The reward is the product over the ball's three angular velocities of max(0, 1 - |ball_qvel - (0, -5, 0)| / 6);
+    an episode ends with discount 0 when |velocimeter| > 50, |gyro| > 200 or the state is bad (non-finite, |qacc| > 1e14), and with
+    discount 1 at the 2 s time limit.  `before_step` applies the action only."""
+
+    def __init__(self, n_envs, time_limit=2.0, random_state=None, **kw):
+        BatchedFlyEnv.__init__(self, 'ball', n_envs, time_limit=time_limit, **kw)
+        self._corruptor = None
+        if random_state is not None:
+            self._rs = random_state if isinstance(random_state, np.random.RandomState) else np.random.RandomState(random_state)
+        self._prev_action = np.zeros((self.n_envs, self._action_spec.shape[0]))
+
+    def _upload_task_program(self):
+        m = self.model
+        self._sim.task_program(kind=4, root_qadr=-1, root_vadr=-1, ghost_qadr=-1, ghost_vadr=-1, user_col=-1,
+                               control_timestep=self._control_timestep, time_limit=self._time_limit, terminal_com_dist=3e38,
+                               terminal_linvel=_TERMINAL_LINVEL, terminal_angvel=_TERMINAL_ANGVEL, terminal_qacc=_TERMINAL_QACC,
+                               terminal_height=-3e38, velocimeter_adr=int(self._sd['velocimeter'][0]), gyro_adr=int(self._sd['gyro'][0]),
+                               com_body=m.body_id('walker/thorax'), reset_qpos=m.qpos0, n_noise=0, seed=int(self._seed) & 0xffffffff,
+                               ball_vadr=self._ball_v, ball_target=_BALL_TARGET_QVEL, ball_margin=_BALL_MARGIN)
+        self._out4 = np.zeros((self.n_envs, 4), np.float32)
+
+    def _task_after(self, rec, obs, resetting, time, ghost):
+        """get_reward_factors, check_termination (walk_on_ball.py:55-81, base.py:222-225), get_discount; the device task kind 4 is the
+        same logic"""
+        sl = self._obs_slices
+        flags = rec[:, sl['_scalars']][:, 0].astype(np.int64)
+        self.n_capacity_overflows += int(((flags & 6) != 0).sum())
+        bad = ((flags & 1) != 0) | ~(np.sqrt(rec[:, sl['_scalars']][:, 1].astype(np.float64)) <= _TERMINAL_QACC)
+        linvel = np.linalg.norm(rec[:, sl['_velocimeter_now']], axis=1)
+        angvel = np.linalg.norm(rec[:, sl['_gyro_now']], axis=1)
+        terminate = (linvel > _TERMINAL_LINVEL) | (angvel > _TERMINAL_ANGVEL) | bad
+        ball_qvel = obs['walker/ball_qvel'].astype(np.float64)
+        reward = np.prod(linear_tolerance(ball_qvel - np.asarray(_BALL_TARGET_QVEL), _BALL_MARGIN), axis=1)
+        last = terminate | (time >= self._time_limit - 1e-9)
+        step_type = np.where(resetting, StepType.FIRST, np.where(last, StepType.LAST, StepType.MID))
+        reward = np.where(resetting, 0.0, reward)
+        discount = np.where(resetting | ~terminate, 1.0, 0.0)
+        return step_type, reward, discount, last & ~resetting
+
+
+def walk_on_ball(force_actuators=False, disable_wings=True, random_state=None, n_envs=None, device=0, lib_path=None, seed=0,
+                 device_task=False):
+    """Batched `flybody.fly_envs.walk_on_ball` (reference `fly_envs.py:158-191`, `tasks/walk_on_ball.py`): the tethered fly walking on
+    a floating ball, 10 substeps of 2e-4 s per control step, a 2 s time limit, 59 actions and the ten walker observables plus
+    `walker/ball_qvel`.  `force_actuators` and `disable_wings=False` select a model variant (`flymodel.model_for('ball', ...)`).
+    `device_task=True` runs the task hooks on the device (kind 4), which `step_device` needs."""
+    model = None
+    if force_actuators or not disable_wings:
+        from .flymodel import model_for
+        model = model_for('ball', force_actuators=force_actuators, use_wings=True if not disable_wings else None)
+    return WalkOnBallEnv(n_envs, random_state=random_state, device=device, lib_path=lib_path, seed=seed, device_task=device_task,
+                         model=model)

@@ -152,6 +152,8 @@ class FlyModel:
 def load_model(variant='walk', path=None):
     if path is None and variant == 'template':
         return template_from_walk(load_model('walk'))
+    if path is None and variant == 'ball':
+        return ball_from_template(load_model('template'))
     path = path or os.path.join(ASSETS, f'fly_{variant}.npz')
     d = np.load(path)
     meta = json.loads(bytes(d['__meta__']).decode())
@@ -205,6 +207,118 @@ def template_from_walk(walk):
     return FlyModel(out, meta)
 
 
+def ball_from_template(template):
+    """The model of `walk_on_ball` (reference fly_envs.py:158-191, tasks/walk_on_ball.py) built from the template model: the same Walking
+    surgery without the ghost, with the walker's free joint removed (its thorax becomes a jointless root at the spawn pose) and BallFloor's
+    ball (`compiler.compile_model._ball_body`: a sphere on a ball joint, 4 qpos, 3 dofs) as the first body, joint, qpos and dofs, its
+    geom in place of the floor plane.  The collision pairs are the template's with the ball in the floor's place: the floor's pairs become
+    the ball's, and the thorax excludes of walk_on_ball.py:30-38 remove the thorax-child pairs that the template's parent-child filter
+    removed.  The world's subtree mass, the invweights, the mean inertia and the halteres' springdamper stiffness and damping are
+    recomputed at qpos0 (mj_setConst: welding the thorax changes the halteres' effective inertia).  `compile_variant('ball')` compiles it
+    from the reference's XML, and tests/test_walk_on_ball.py holds the two together where that file is reachable."""
+    from .compiler import compile_model as cm
+    t, meta = template.a, json.loads(json.dumps(template.meta))
+    jn = meta['jnt_names']
+    assert jn[0] == 'walker/' and t['jnt_type'][0] == cm.JNT_FREE and t['jnt_qposadr'][1] == 7 and t['jnt_dofadr'][1] == 6, \
+        'the template model does not start with the walker\'s free joint'
+    assert t['geom_type'][0] == cm.GEOM_PLANE and t['geom_bodyid'][0] == 0, 'the template model has no floor plane first'
+    assert t['body_parentid'][1] == 0 and t['body_jntadr'][1] == 0 and t['body_jntnum'][1] == 1
+    ball = cm._ball_body()
+    cm._body_inertial(ball)
+    bj, bg = ball.joints[0], ball.geoms[0]
+    nb, nv = int(meta['nbody']) + 1, int(meta['nv']) - 3
+    a = {}
+
+    def ins(k, row):                       # insert the ball's row at body index 1
+        return np.insert(np.asarray(t[k]), 1, row, axis=0)
+    bshift = lambda v: np.where(np.asarray(v) > 0, np.asarray(v) + 1, np.asarray(v))      # body ids after the inserted ball
+    a['body_parentid'] = ins('body_parentid', 0)
+    a['body_parentid'][2:] = bshift(t['body_parentid'][1:])
+    a['body_rootid'] = ins('body_rootid', 1)
+    a['body_rootid'][2:] = bshift(t['body_rootid'][1:])
+    a['body_weldid'] = np.zeros(nb, np.int32)
+    a['body_jntadr'] = ins('body_jntadr', 0)
+    a['body_jntadr'][2] = -1
+    a['body_jntnum'] = ins('body_jntnum', 1)
+    a['body_jntnum'][2] = 0
+    a['body_dofadr'] = ins('body_dofadr', 0)
+    a['body_dofadr'][2:] = np.where(t['body_dofadr'][1:] >= 6, t['body_dofadr'][1:] - 3, -1)
+    a['body_dofnum'] = ins('body_dofnum', 3)
+    a['body_dofnum'][2] = 0
+    for k, row in (('body_pos', ball.pos), ('body_quat', ball.quat), ('body_ipos', ball.ipos), ('body_iquat', ball.iquat),
+                   ('body_mass', ball.mass), ('body_inertia', ball.inertia), ('body_fluid_ellipsoid', 0), ('body_invweight0', (0.0, 0.0)),
+                   ('body_subtreemass', ball.mass)):
+        a[k] = ins(k, row)
+    for b in range(1, nb):
+        a['body_weldid'][b] = b if a['body_jntnum'][b] > 0 else a['body_weldid'][a['body_parentid'][b]]
+    lastdof = np.full(nb, -1, np.int32)
+    for b in range(1, nb):
+        lastdof[b] = a['body_dofadr'][b] + a['body_dofnum'][b] - 1 if a['body_dofnum'][b] > 0 else lastdof[a['body_parentid'][b]]
+    a['body_lastdof'] = lastdof
+    a['body_subtreemass'][0] = a['body_mass'][0] + a['body_subtreemass'][1:][a['body_parentid'][1:] == 0].sum()
+    # joints: the walker's free joint (joint 0) becomes the ball joint; qpos 7 -> 4, dofs 6 -> 3
+    for k in [k for k in t if k.startswith('jnt_') and isinstance(t[k], np.ndarray)]:
+        a[k] = np.array(t[k], copy=True)
+    a['jnt_type'][0], a['jnt_bodyid'][0] = cm.JNT_BALL, 1
+    a['jnt_bodyid'][1:] = t['jnt_bodyid'][1:] + 1
+    a['jnt_qposadr'][1:] -= 3
+    a['jnt_dofadr'][1:] -= 3
+    for k, v in (('jnt_pos', bj['pos']), ('jnt_axis', bj['axis']), ('jnt_stiffness', bj['stiffness']), ('jnt_range', bj['range']),
+                 ('jnt_limited', bj['limited']), ('jnt_solref', bj['solref']), ('jnt_solimp', bj['solimp']), ('jnt_margin', bj['margin'])):
+        a[k][0] = v
+    a['qpos0'] = np.concatenate([[1.0, 0, 0, 0], t['qpos0'][7:]])
+    a['qpos_spring'] = np.concatenate([[1.0, 0, 0, 0], t['qpos_spring'][7:]])
+    a['dof_bodyid'] = np.concatenate([[1, 1, 1], t['dof_bodyid'][6:] + 1]).astype(np.int32)
+    a['dof_jntid'] = np.concatenate([[0, 0, 0], t['dof_jntid'][6:]]).astype(np.int32)
+    a['dof_armature'] = np.concatenate([[bj['armature']] * 3, t['dof_armature'][6:]])
+    a['dof_damping'] = np.concatenate([[bj['damping']] * 3, t['dof_damping'][6:]])
+    par = np.full(nv, -1, np.int32)
+    for d in range(nv):
+        b = a['dof_bodyid'][d]
+        par[d] = d - 1 if d > a['body_dofadr'][b] else lastdof[a['body_parentid'][b]]
+    a['dof_parentid'] = par
+    chain = np.zeros(nv, np.int64)
+    for d in range(nv):
+        chain[d] = 1 + (chain[par[d]] if par[d] >= 0 else 0)
+    a['dof_Madr'] = np.concatenate([[0], np.cumsum(chain)[:-1]]).astype(np.int32)
+    # geoms: the ball's sphere in the floor's slot (both come first: the world's, then body 1's)
+    for k in [k for k in t if k.startswith('geom_') and isinstance(t[k], np.ndarray)]:
+        a[k] = np.array(t[k], copy=True)
+    a['geom_bodyid'][1:] += 1
+    for k, v in (('geom_type', bg['type']), ('geom_bodyid', 1), ('geom_size', bg['size']), ('geom_pos', bg['pos']), ('geom_quat', bg['quat']),
+                 ('geom_rbound', cm.rbound(bg['type'], bg['size'])), ('geom_condim', bg['condim']), ('geom_priority', bg['priority']),
+                 ('geom_friction', bg['friction']), ('geom_solmix', bg['solmix']), ('geom_solref', bg['solref']), ('geom_solimp', bg['solimp']),
+                 ('geom_margin', bg['margin']), ('geom_gap', bg['gap'])):
+        a[k][0] = v
+    meta['geom_names'][0] = bg['name']
+    for k in ('site_bodyid', 'fluid_bodyid'):
+        a[k] = t[k] + 1
+    a['wrap_dofid'], a['wrap_qposadr'] = t['wrap_dofid'] - 3, t['wrap_qposadr'] - 3
+    a['actuator_trnid'] = np.where(t['actuator_trntype'] == cm.TRN_BODY, t['actuator_trnid'] + 1, t['actuator_trnid'])
+    for k, v in t.items():
+        if isinstance(v, np.ndarray) and k not in a:
+            a[k] = np.array(v, copy=True)
+    meta['jnt_names'][0] = bj['name']
+    meta['body_names'].insert(1, ball.name)
+    meta.update(nbody=nb, nq=int(meta['nq']) - 3, nv=nv, nM=int(chain.sum()))
+    # mj_setConst at qpos0: the invweights, the mean inertia and the springdamper joints (class `haltere`, fruitfly.xml:89-91), whose
+    # (timeconst, dampratio) are recovered from the template's values
+    m = {**a, **meta}
+    sd = [np.zeros(2)] * len(jn)
+    for j, name in enumerate(jn):
+        if 'haltere' in name:
+            da = t['jnt_dofadr'][j]
+            inertia = 1.0 / t['dof_invweight0'][da]
+            tc = 2 * inertia / t['dof_damping'][da]
+            sd[j] = np.array([tc, np.sqrt(inertia / (t['jnt_stiffness'][j] * tc * tc))])
+    m['_jnt_springdamper'] = sd
+    cm._set0(m)
+    for k in ('body_invweight0', 'dof_invweight0', 'jnt_stiffness', 'dof_damping'):
+        a[k] = m[k]
+    meta['stat_meaninertia'] = m['stat_meaninertia']
+    return FlyModel(a, meta)
+
+
 def from_compiled(m):
     arrays = {k: v for k, v in m.items() if isinstance(v, np.ndarray)}
     meta = {k: v for k, v in m.items() if not isinstance(v, np.ndarray) and not k.startswith('_')}
@@ -252,6 +366,8 @@ def model_for(variant, force_actuators=False, use_wings=None, use_legs=None, joi
     `fruitfly.xml` on first use (`flybody_b200.compiler`, ~2 s) and cached."""
     if not force_actuators and use_wings is None and use_legs is None and joint_filter is None and adhesion_filter is None:
         return load_model(variant)
+    if variant == 'ball':               # walk_on_ball's model is cut from the template model with the same switches
+        return ball_from_template(model_for('template', force_actuators, use_wings, use_legs, joint_filter, cache_dir, adhesion_filter))
     name = variant_name(variant, force_actuators, use_wings, use_legs, joint_filter, adhesion_filter)
     cache_dir = cache_dir or os.environ.get('FLYBODY_B200_CACHE') or os.path.join(os.path.expanduser('~'), '.cache', 'flybody_b200')
     for d in (ASSETS, cache_dir):

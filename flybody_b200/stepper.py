@@ -59,7 +59,8 @@ class FbTaskProgram(C.Structure):
                 ('obs_root_pose_off', C.c_int32), ('obs_root_qvel_off', C.c_int32), ('obs_mocap_qpos_off', C.c_int32),
                 ('obs_mocap_qvel_off', C.c_int32), ('obs_mocap_axes_off', C.c_int32), ('obs_mocap_sites_off', C.c_int32),
                 ('obs_wing_qpos_off', C.c_int32), ('wing_spring', C.POINTER(C.c_float)), ('deep_mimic_std', C.c_float * 4),
-                ('deep_mimic_weight', C.c_float * 4), ('retract_margin', C.c_float)]
+                ('deep_mimic_weight', C.c_float * 4), ('retract_margin', C.c_float),
+                ('ball_vadr', C.c_int32), ('ball_target', C.c_float * 3), ('ball_margin', C.c_float)]
 
 
 class FbEyeProgram(C.Structure):

@@ -22,7 +22,7 @@ extern "C" {
 /* enums shared by compiler (Python), oracle (C) and kernels (CUDA) */
 enum { FB_GEOM_PLANE = 0, FB_GEOM_SPHERE = 2, FB_GEOM_CAPSULE = 3, FB_GEOM_ELLIPSOID = 4,
        FB_GEOM_CYLINDER = 5, FB_GEOM_BOX = 6 };
-enum { FB_JNT_FREE = 0, FB_JNT_HINGE = 3 };
+enum { FB_JNT_FREE = 0, FB_JNT_BALL = 1, FB_JNT_HINGE = 3 };
 enum { FB_TRN_JOINT = 0, FB_TRN_TENDON = 1, FB_TRN_BODY = 2 };
 enum { FB_DYN_NONE = 0, FB_DYN_FILTER = 2, FB_DYN_FILTEREXACT = 3 };
 enum { FB_SENS_TOUCH = 0, FB_SENS_ACCELEROMETER = 1, FB_SENS_VELOCIMETER = 2, FB_SENS_GYRO = 3,
@@ -308,8 +308,9 @@ typedef struct FbTaskProgram {
   int32_t kind;                        /* 0 walk_imitation, 1 flight_imitation, 2 vision_guided_flight (fields at the end of the struct),
                                           3 template_task (tasks/template_task.py): reset to reset_qpos at rest, no ghost / reference /
                                           before_step hook; reward 1, LAST with discount 0 on a bad state or |qacc| > terminal_qacc,
-                                          LAST with discount 1 at time_limit (ghost_qadr = user_col = -1, no noise) */
-  int32_t root_qadr, root_vadr, ghost_qadr, ghost_vadr;   /* free-joint slots of the walker root and of the ghost */
+                                          LAST with discount 1 at time_limit (ghost_qadr = user_col = -1, no noise),
+                                          4 walk_on_ball (fields at the end of the struct; kind 3's reset and hooks, its own reward) */
+  int32_t root_qadr, root_vadr, ghost_qadr, ghost_vadr;   /* free-joint slots of the walker root and of the ghost (-1: none) */
   int32_t user_col;                    /* column of the beat-frequency action in the action row, -1 if none */
   float ghost_offset[3];
   float control_timestep, time_limit;
@@ -360,6 +361,10 @@ typedef struct FbTaskProgram {
   int32_t obs_root_pose_off, obs_root_qvel_off, obs_mocap_qpos_off, obs_mocap_qvel_off, obs_mocap_axes_off, obs_mocap_sites_off, obs_wing_qpos_off;
   const float* wing_spring;            /* [n_wing] */
   float deep_mimic_std[4], deep_mimic_weight[4], retract_margin;
+  /* kind 4, walk_on_ball (tasks/walk_on_ball.py:55-81): the reset is kind 3's (reset_qpos at rest); the reward is the product over
+   * i < 3 of max(0, 1 - |qvel[ball_vadr + i] - ball_target[i]| / ball_margin); an episode ends with discount 0 when |velocimeter| >
+   * terminal_linvel, |gyro| > terminal_angvel or the state is bad, and with discount 1 at the time limit.  */
+  int32_t ball_vadr; float ball_target[3], ball_margin;
 } FbTaskProgram;
 int fb_task_program(FbHandle h, const FbTaskProgram* p);
 /* Flight trajectory bank for kind 1 with ref_bank: n_traj trajectories, rows [sum(traj_len)][15] fp32, trajectory k after
