@@ -171,7 +171,7 @@ struct DevData {
 // DevData::task points at it.
 #define FB_RBANK_W 15                      // flight bank row: root qpos 7, CoM qvel 6, CoM x, y 2 (the first 15 columns of every bank row)
 struct DevTask {
-  int kind;                                // 0 walk_imitation, 1 flight_imitation, 2 vision_guided_flight
+  int kind;                                // enum FbTaskKind (include/flybody_b200.h)
   int root_qadr, root_vadr, ghost_qadr, ghost_vadr, root_body, user_col /* action column of the beat-frequency action, -1: none */;
   float ghost_offset[3], dt, time_limit, term_com, term_linvel, term_angvel, term_qacc, term_height;
   int velocimeter_adr, gyro_adr, com_body, episode_steps, ref_len, obs_refdisp_off, obs_refquat_off;
@@ -180,18 +180,18 @@ struct DevTask {
   int n_wing; const int *wing_qadr, *wing_vadr, *wing_ctrl;
   int n_freq, tab_len; const float *wb_traj /*[n_freq][tab_len][n_wing]*/, *wb_phase, *wb_phase_mod /*[n_freq][tab_len], +inf padded*/, *wb_freqs; const int* wb_len;
   float wb_base_freq, wb_rel_range, wb_rate, com_offset[3];
-  // kind 2 (vision_guided_flight): ranges of the per-episode draws, hover pose, terrain bank and the env's own heightfield buffers
+  // FB_TASK_VISION (vision_guided_flight): ranges of the per-episode draws, hover pose, terrain bank and the env's own heightfield buffers
   float th_rng[2], ts_rng[2], x_rng[2], y_rng[2], hover_quat[4], target_zaxis[3]; int fatal;
   int n_bank, hf_nrow, hf_ncol, hf_ncm; float hf_half, hf_zoff;
   const float *bank, *bank_hmax, *bank_cmax; float *hf_data, *hf_hmax, *hf_cmax;
   float* target;                           // [N][2] target height, target speed of the running episode
   int trench_cap; const float *trench_x, *trench_y; const int* trench_len; int* pick;   // 'trench' arenas: centre line per bank terrain; the env's terrain
-  // kind 0 / 1 with ref_bank (dataset): trajectory bank [rows][rbank_w] (fb_ref_bank / fb_ref_bank_wide), picks, the env's reference slot
+  // FB_TASK_WALK / FB_TASK_FLIGHT with ref_bank (dataset): trajectory bank [rows][rbank_w] (fb_ref_bank / fb_ref_bank_wide), picks, the env's reference slot
   int ref_bank, n_traj, n_pick, randomize_start, start_margin, max_episode_rows, future_steps, slot_len, rbank_w;
   const float* rbank; const int *traj_off, *traj_len, *pick_traj; float* slots /* [N][slot_len][7] */;
   int *ep_traj, *ep_start, *ep_row0, *ep_n;   // the running episode: trajectory, start step, bank row of its row 0, rows in use
   int* pin;                                // [N][3] has pin, trajectory, start step of the next reset (fb_task_ref_pick)
-  // kind 0 with ref_bank (walking dataset): the dataset's joints / sites, the observation columns of the walker features, the DeepMimic
+  // FB_TASK_WALK with ref_bank (walking dataset): the dataset's joints / sites, the observation columns of the walker features, the DeepMimic
   // reward's constants; bank row after the 15 root columns: mocap qpos [nj], mocap qvel [nj], root2site [ns][3], joint_quat [nj][4]
   int n_mjnt, n_msite; const int* mocap_qadr; const float* wing_spring;
   int obs_root_pose_off, obs_root_qvel_off, obs_mocap_qpos_off, obs_mocap_qvel_off, obs_mocap_axes_off, obs_mocap_sites_off, obs_wing_qpos_off;
@@ -202,7 +202,7 @@ struct DevTask {
   float *uniform /* [N][8] */, *wb_freq;
   int* op_step; unsigned char* op_first;   // the observation program's per-env inputs, maintained here instead of by fb_task_inputs
   float* out;                              // [N][4] reward, discount, step_type (0 FIRST, 1 MID, 2 LAST), 0
-  // kind 4 (walk_on_ball): the ball joint's first dof, the target ball velocity and the reward's margin
+  // FB_TASK_BALL (walk_on_ball): the ball joint's first dof, the target ball velocity and the reward's margin
   int ball_vadr; float ball_target[3], ball_margin;
 };
 

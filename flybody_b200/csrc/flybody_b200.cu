@@ -23,6 +23,7 @@
 #include "fb_solver_reg.h"
 #include "fb_render.h"
 #include "fb_hfield.h"
+#include "fb_task.h"
 
 #ifdef FB_EMU
 typedef int cudaStream_t_;
@@ -1208,46 +1209,46 @@ int fb_ref_slot_write(FbHandle s, const int32_t* env_ids, int n, const float* ro
 int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   if (!s || !p) return -1;
   if (!s->d.tobs || !s->act_map_dev) { s->err = "fb_task_program: call fb_set_action_map and fb_obs_program first"; return -1; }
-  const bool bank = (p->kind == 0 || p->kind == 1) && p->ref_bank;
-  if (p->ref_bank && !bank) { s->err = "fb_task_program: ref_bank is for kind 0 / 1 (walk_imitation / flight_imitation)"; return -1; }
+  const bool bank = (p->kind == FB_TASK_WALK || p->kind == FB_TASK_FLIGHT) && p->ref_bank;
+  if (p->ref_bank && !bank) { s->err = "fb_task_program: ref_bank is for FB_TASK_WALK / FB_TASK_FLIGHT (walk_imitation / flight_imitation)"; return -1; }
   if (s->d.op_ref_slot && !bank) { s->err = "fb_task_program: per-env reference slots keep the host-side task code"; return -1; }
   if (bank) {
     if (!s->d.op_ref_slot || !s->ref_slots || s->ref_slot_len < 1) { s->err = "fb_task_program: ref_bank needs the per-env reference slots (fb_ref_slots) first"; return -1; }
     if (!s->rbank_dev) { s->err = "fb_task_program: ref_bank needs a trajectory bank (fb_ref_bank / fb_ref_bank_wide) first"; return -1; }
     if (p->n_pick <= 0 || !p->pick_traj) { s->err = "fb_task_program: ref_bank needs the trajectory indices to draw from (n_pick, pick_traj)"; return -1; }
     if (p->start_margin < 0 || p->max_episode_rows < 1 || p->future_steps < 0) { s->err = "fb_task_program: bad start_margin / max_episode_rows / future_steps"; return -1; }
-    if (p->kind == 0 && p->randomize_start) { s->err = "fb_task_program: walking starts every snippet at row 0 (randomize_start must be 0)"; return -1; }
+    if (p->kind == FB_TASK_WALK && p->randomize_start) { s->err = "fb_task_program: walking starts every snippet at row 0 (randomize_start must be 0)"; return -1; }
     for (int k = 0; k < p->n_pick; k++) {
       const int j = p->pick_traj[k];
       if (j < 0 || j >= (int)s->rbank_len.size()) { s->err = "fb_task_program: trajectory index of pick_traj out of range of the bank"; return -1; }
       if (p->randomize_start && s->rbank_len[j] <= p->start_margin) {
         s->err = "fb_task_program: with randomize_start every trajectory to draw from must be longer than start_margin rows"; return -1; }
-      if (p->kind == 0 && s->rbank_len[j] <= p->future_steps + 1) {
+      if (p->kind == FB_TASK_WALK && s->rbank_len[j] <= p->future_steps + 1) {
         s->err = "fb_task_program: every walking trajectory to draw from must be longer than future_steps + 1 rows"; return -1; }
     }
-    if (p->kind == 0) {          // the walking reward: the dataset's joints / sites in the bank rows and the walker's in the observation row
+    if (p->kind == FB_TASK_WALK) {          // the walking reward: the dataset's joints / sites in the bank rows and the walker's in the observation row
       const int nj = p->n_mocap_joints, ns = p->n_mocap_sites, dim = s->d.tobs_dim;
-      if (nj <= 0 || ns < 0 || !p->mocap_qadr) { s->err = "fb_task_program: a kind 0 ref_bank program needs the dataset's joints (n_mocap_joints, mocap_qadr)"; return -1; }
+      if (nj <= 0 || ns < 0 || !p->mocap_qadr) { s->err = "fb_task_program: an FB_TASK_WALK ref_bank program needs the dataset's joints (n_mocap_joints, mocap_qadr)"; return -1; }
       for (int i = 0; i < nj; i++) if (p->mocap_qadr[i] < 0 || p->mocap_qadr[i] >= s->m.nq) { s->err = "fb_task_program: mocap_qadr entry out of range"; return -1; }
       if ((size_t)s->rbank_w != (size_t)FB_RBANK_W + 6 * (size_t)nj + 3 * (size_t)ns) {
         s->err = "fb_task_program: the bank rows are not 15 + 6 n_mocap_joints + 3 n_mocap_sites wide (fb_ref_bank_wide)"; return -1; }
       const int off[7] = {p->obs_root_pose_off, p->obs_root_qvel_off, p->obs_mocap_qpos_off, p->obs_mocap_qvel_off, p->obs_mocap_axes_off, p->obs_mocap_sites_off, p->obs_wing_qpos_off};
       const int wid[7] = {7, 6, nj, nj, 3 * nj, 3 * ns, p->n_wing};
       for (int k = 0; k < 7; k++) if (off[k] < 1 || off[k] + wid[k] > dim) {
-        s->err = "fb_task_program: a kind 0 ref_bank program needs the observation columns of the walker features (obs_*_off)"; return -1; }
-      if (p->n_wing <= 0 || !p->wing_qadr || !p->wing_spring) { s->err = "fb_task_program: a kind 0 ref_bank program needs the wing joints and their springs"; return -1; }
+        s->err = "fb_task_program: an FB_TASK_WALK ref_bank program needs the observation columns of the walker features (obs_*_off)"; return -1; }
+      if (p->n_wing <= 0 || !p->wing_qadr || !p->wing_spring) { s->err = "fb_task_program: an FB_TASK_WALK ref_bank program needs the wing joints and their springs"; return -1; }
       for (int i = 0; i < p->n_wing; i++) if (p->wing_qadr[i] < 0 || p->wing_qadr[i] >= s->m.nq) { s->err = "fb_task_program: wing_qadr entry out of range"; return -1; }
       for (int k = 0; k < 4; k++) if (!(p->deep_mimic_std[k] > 0)) { s->err = "fb_task_program: deep_mimic_std must be positive"; return -1; }
       if (!(p->retract_margin > 0)) { s->err = "fb_task_program: retract_margin must be positive"; return -1; }
     }
-  } else if (p->kind == 3 || p->kind == 4) {
-    if (p->ghost_qadr >= 0 || p->user_col >= 0 || p->n_noise > 0) { s->err = "fb_task_program: kinds 3 and 4 (template_task, walk_on_ball) have no ghost, user action or reset noise"; return -1; }
-    if (p->kind == 4 && (p->ball_vadr < 0 || p->ball_vadr + 3 > s->m.nv || !(p->ball_margin > 0))) { s->err = "fb_task_program: kind 4 needs the ball's dofs (ball_vadr) and a positive ball_margin"; return -1; }
-  } else if (p->kind < 0 || p->kind > 4) { s->err = "fb_task_program: unknown kind"; return -1;
+  } else if (p->kind == FB_TASK_TEMPLATE || p->kind == FB_TASK_BALL) {
+    if (p->ghost_qadr >= 0 || p->user_col >= 0 || p->n_noise > 0) { s->err = "fb_task_program: FB_TASK_TEMPLATE and FB_TASK_BALL (template_task, walk_on_ball) have no ghost, user action or reset noise"; return -1; }
+    if (p->kind == FB_TASK_BALL && (p->ball_vadr < 0 || p->ball_vadr + 3 > s->m.nv || !(p->ball_margin > 0))) { s->err = "fb_task_program: FB_TASK_BALL needs the ball's dofs (ball_vadr) and a positive ball_margin"; return -1; }
+  } else if (p->kind < FB_TASK_WALK || p->kind > FB_TASK_BALL) { s->err = "fb_task_program: unknown kind"; return -1;
   } else if (p->ref_len <= 0 || !p->ref_qpos || !p->ref_qvel) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
   if (!p->reset_qpos) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
-  if (p->kind == 2 && (!s->bank_dev || !s->hfield_dev || s->bank_n <= 0)) { s->err = "fb_task_program: kind 2 needs fb_hfield_collision / fb_eye_program and fb_hfield_bank first"; return -1; }
-  if ((p->kind == 1 || p->kind == 2) && (p->n_wing <= 0 || p->n_freq <= 0 || p->tab_len <= 0 || !p->wb_traj || !p->wb_phase || !p->wb_phase_mod || !p->wb_freqs || !p->wb_len)) { s->err = "fb_task_program: wing-beat tables missing"; return -1; }
+  if (p->kind == FB_TASK_VISION && (!s->bank_dev || !s->hfield_dev || s->bank_n <= 0)) { s->err = "fb_task_program: FB_TASK_VISION needs fb_hfield_collision / fb_eye_program and fb_hfield_bank first"; return -1; }
+  if ((p->kind == FB_TASK_FLIGHT || p->kind == FB_TASK_VISION) && (p->n_wing <= 0 || p->n_freq <= 0 || p->tab_len <= 0 || !p->wb_traj || !p->wb_phase || !p->wb_phase_mod || !p->wb_freqs || !p->wb_len)) { s->err = "fb_task_program: wing-beat tables missing"; return -1; }
   if (sync_stream(s) != 0) return -2;
   const DevModel& m = s->m; const int Np = s->d.Np;
   scope_free(s, s->task_scope); s->d.task = nullptr;
@@ -1263,11 +1264,11 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   auto upf32 = [&](const float* src, size_t n) { std::vector<float> v(src, src + n); return up(s, v); };
   auto upi32 = [&](const int32_t* src, size_t n) { std::vector<int> v(src, src + n); return up(s, v); };
   t.reset_qpos = upf32(p->reset_qpos, m.nq);
-  if (p->kind == 4) { t.ball_vadr = p->ball_vadr; for (int i = 0; i < 3; i++) t.ball_target[i] = p->ball_target[i]; t.ball_margin = p->ball_margin; }
-  if (!bank && p->kind != 3 && p->kind != 4) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
+  if (p->kind == FB_TASK_BALL) { t.ball_vadr = p->ball_vadr; for (int i = 0; i < 3; i++) t.ball_target[i] = p->ball_target[i]; t.ball_margin = p->ball_margin; }
+  if (!bank && p->kind != FB_TASK_TEMPLATE && p->kind != FB_TASK_BALL) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
   else t.ref_len = 0;
   t.n_noise = p->noise_qadr ? p->n_noise : 0; t.noise_qadr = t.n_noise ? upi32(p->noise_qadr, t.n_noise) : nullptr; t.noise_amp = p->noise_amp; t.seed = p->seed;
-  if (p->kind == 1 || p->kind == 2) {
+  if (p->kind == FB_TASK_FLIGHT || p->kind == FB_TASK_VISION) {
     t.n_wing = p->n_wing; t.wing_qadr = upi32(p->wing_qadr, p->n_wing); t.wing_vadr = upi32(p->wing_vadr, p->n_wing); t.wing_ctrl = upi32(p->wing_ctrl, p->n_wing);
     t.n_freq = p->n_freq; t.tab_len = p->tab_len; const size_t nt = (size_t)p->n_freq * p->tab_len;
     t.wb_traj = upf32(p->wb_traj, nt * p->n_wing); t.wb_phase = upf32(p->wb_phase, nt); t.wb_phase_mod = upf32(p->wb_phase_mod, nt);
@@ -1283,7 +1284,7 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
     t.n_pick = p->n_pick; t.pick_traj = upi32(p->pick_traj, p->n_pick); t.randomize_start = p->randomize_start ? 1 : 0; t.start_margin = p->start_margin;
     t.max_episode_rows = p->max_episode_rows; t.future_steps = p->future_steps; t.slots = s->ref_slots; t.slot_len = s->ref_slot_len;
     t.ep_traj = dalloc<int>(s, Np); t.ep_start = dalloc<int>(s, Np); t.ep_row0 = dalloc<int>(s, Np); t.ep_n = dalloc<int>(s, Np); t.pin = dalloc<int>(s, (size_t)3 * Np);
-    if (p->kind == 0) {
+    if (p->kind == FB_TASK_WALK) {
       t.n_mjnt = p->n_mocap_joints; t.n_msite = p->n_mocap_sites; t.mocap_qadr = upi32(p->mocap_qadr, p->n_mocap_joints);
       t.n_wing = p->n_wing; t.wing_qadr = upi32(p->wing_qadr, p->n_wing); t.wing_spring = upf32(p->wing_spring, p->n_wing);
       t.obs_root_pose_off = p->obs_root_pose_off; t.obs_root_qvel_off = p->obs_root_qvel_off; t.obs_mocap_qpos_off = p->obs_mocap_qpos_off;
@@ -1297,7 +1298,7 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
     std::vector<int> steps((size_t)Np, p->episode_steps);
     h2d(t.ep_steps, steps.data(), sizeof(int) * steps.size());
   }
-  if (p->kind == 2) {
+  if (p->kind == FB_TASK_VISION) {
     for (int i = 0; i < 2; i++) { t.th_rng[i] = p->target_height_range[i]; t.ts_rng[i] = p->target_speed_range[i]; t.x_rng[i] = p->init_x_range[i]; t.y_rng[i] = p->init_y_range[i]; }
     for (int i = 0; i < 4; i++) t.hover_quat[i] = p->hover_quat[i];
     for (int i = 0; i < 3; i++) t.target_zaxis[i] = p->target_zaxis[i];
@@ -1392,7 +1393,7 @@ int fb_hfield_bank(FbHandle s, int n_terrain, const float* heights) {
   if (s->bank_dev) {      // a replaced bank is freed; a vision task program pointing at it has to be uploaded again
     std::vector<void*> old = {s->bank_dev, s->bank_hmax_dev, s->bank_cmax_dev};
     scope_free(s, old);
-    if (s->d.task && s->task_host.kind == 2) { scope_free(s, s->task_scope); s->d.task = nullptr; }
+    if (s->d.task && s->task_host.kind == FB_TASK_VISION) { scope_free(s, s->task_scope); s->d.task = nullptr; }
   }
   s->bank_dev = dalloc<float>(s, cells * n_terrain); s->bank_hmax_dev = dalloc<float>(s, n_terrain); s->bank_cmax_dev = dalloc<float>(s, ncm * n_terrain);
   if (!s->bank_dev) { s->err = "out of device memory (terrain bank)"; return -4; }

@@ -10,6 +10,7 @@ logic mirrors `flybody/tasks/walk_imitation.py` / `tasks/base.py` in vectorised 
 """
 import collections
 import hashlib
+import types
 
 import numpy as np
 
@@ -208,22 +209,183 @@ class FlightImitationTask(_ImitationTask):
 
 
 _VARIANTS = {
-    # control dt, time limit, observation names in spec order (hidden '_' entries feed termination / reward)
-    'walk': dict(dt=_WALK_CONTROL_TIMESTEP, obs=('accelerometer', 'actuator_activation', 'appendages_pos', 'force', 'gyro',
-                                                 'joints_pos', 'joints_vel', 'touch', 'velocimeter', 'world_zaxis',
-                                                 'ref_displacement', 'ref_root_quat')),
-    'flight': dict(dt=_FLY_CONTROL_TIMESTEP, obs=('accelerometer', 'actuator_activation', 'gyro', 'joints_pos', 'joints_vel',
-                                                  'velocimeter', 'world_zaxis', 'ref_displacement', 'ref_root_quat')),
+    # control dt, device task kind, observation names in spec order (hidden '_' entries feed termination / reward)
+    'walk': dict(dt=_WALK_CONTROL_TIMESTEP, kind=st.TASK_WALK, obs=('accelerometer', 'actuator_activation', 'appendages_pos', 'force',
+                                                                    'gyro', 'joints_pos', 'joints_vel', 'touch', 'velocimeter',
+                                                                    'world_zaxis', 'ref_displacement', 'ref_root_quat')),
+    'flight': dict(dt=_FLY_CONTROL_TIMESTEP, kind=st.TASK_FLIGHT, obs=('accelerometer', 'actuator_activation', 'gyro', 'joints_pos',
+                                                                       'joints_vel', 'velocimeter', 'world_zaxis', 'ref_displacement',
+                                                                       'ref_root_quat')),
     # template_task: the walker's observables only (reference tests/test_core.py:9-20)
-    'template': dict(dt=_WALK_CONTROL_TIMESTEP, obs=('accelerometer', 'actuator_activation', 'appendages_pos', 'force', 'gyro',
-                                                     'joints_pos', 'joints_vel', 'touch', 'velocimeter', 'world_zaxis')),
+    'template': dict(dt=_WALK_CONTROL_TIMESTEP, kind=st.TASK_TEMPLATE, obs=('accelerometer', 'actuator_activation', 'appendages_pos',
+                                                                            'force', 'gyro', 'joints_pos', 'joints_vel', 'touch',
+                                                                            'velocimeter', 'world_zaxis')),
     # walk_on_ball: the walker's observables, then the task's ball_qvel (reference tasks/walk_on_ball.py:46)
-    'ball': dict(dt=_WALK_CONTROL_TIMESTEP, obs=('accelerometer', 'actuator_activation', 'appendages_pos', 'force', 'gyro',
-                                                 'joints_pos', 'joints_vel', 'touch', 'velocimeter', 'world_zaxis', 'ball_qvel')),
+    'ball': dict(dt=_WALK_CONTROL_TIMESTEP, kind=st.TASK_BALL, obs=('accelerometer', 'actuator_activation', 'appendages_pos', 'force',
+                                                                    'gyro', 'joints_pos', 'joints_vel', 'touch', 'velocimeter',
+                                                                    'world_zaxis', 'ball_qvel')),
 }
 
 
-class BatchedFlyEnv:
+def _pinned(shape, dtype):
+    """page-locked host buffer where torch + CUDA are present (device -> host copies at full PCIe rate), plain numpy otherwise"""
+    try:
+        import torch
+        if torch.cuda.is_available():
+            return torch.empty(shape, dtype=getattr(torch, np.dtype(dtype).name)).pin_memory().numpy()
+    except Exception:
+        pass
+    return np.empty(shape, dtype)
+
+
+def _device_tensor(ptr, shape, typestr, device):
+    """zero-copy torch tensor over a buffer the library owns on `device` (typestr '<f4': fp32, '|u1': uint8)"""
+    import torch
+    view = types.SimpleNamespace(__cuda_array_interface__={'shape': shape, 'typestr': typestr, 'data': (int(ptr), False), 'version': 2})
+    return torch.as_tensor(view, device=f'cuda:{device}')
+
+
+class _TaskEnv:
+    """The episode shell of every task env: N lock-stepped flies of one model on one stepper, the action layout and the dm_env specs,
+    auto-reset bookkeeping, and the end of a control step -- on the host (`_bad_state`, `_end_step`) and with the task hooks on the device
+    (`_device_step`, `step_device`'s launch and views).  A task adds its observation program, its `_task_after` (termination and
+    reward) and its `_before_device_step` / `_after_device_step` extras."""
+
+    def __init__(self, model, n_envs, device, lib_path, control_timestep, time_limit, n_user, seed, kind, device_task):
+        self._batched = n_envs is not None
+        self.n_envs = N = int(n_envs) if self._batched else 1
+        self.model = m = model
+        self._sim = st.BatchedStepper(m, N, device=device, lib_path=lib_path)
+        self._control_timestep, self._physics_timestep = control_timestep, float(m.opt_timestep)
+        self._n_sub = int(round(self._control_timestep / self._physics_timestep))
+        self._time_limit = time_limit
+        self._rs = np.random.RandomState(seed)
+        self._seed, self._task_kind = seed, kind
+        self._device_task = bool(device_task)       # task hooks evaluated on the device (fb_task_*): no host logic in step()
+        # actions (reference fruitfly.py:342-379, 532-579): the actuator classes in a fixed order, then the task's user actions in
+        # [-1, 1], which have no ctrl slot (flight: the beat frequency)
+        ci, idx, self._action_indices = m.meta['ctrl_indices'], [], {}
+        for key in _ACTION_CLASS_ORDER:
+            if ci.get(key):
+                self._action_indices[key] = np.arange(len(idx), len(idx) + len(ci[key]))
+                idx.extend(ci[key])
+        self._ctrl_of_action, self._n_user = np.asarray(idx, np.int64), n_user
+        names = [m.meta['actuator_names'][i].split('/')[-1] for i in idx] + [f'user_{i}' for i in range(n_user)]
+        rng = m.actuator_ctrlrange[idx]
+        self._action_spec = BoundedArray((len(names),), np.float64, np.concatenate([rng[:, 0], -np.ones(n_user)]),
+                                         np.concatenate([rng[:, 1], np.ones(n_user)]), name='\t'.join(names))
+        # per-env episode state
+        self._time = np.zeros(N)
+        self._needs_reset = np.ones(N, bool)
+        self._dev_views = None
+        self.n_resets = 0
+        self.n_capacity_overflows = 0            # env-steps whose contact / constraint-row lists hit their capacity (FB_FLAGS bits 1, 2)
+
+    # ---------------------------------------------------------------------------------- specs
+    def action_spec(self):
+        return self._action_spec
+
+    def reward_spec(self):
+        return Array((self.n_envs,) if self._batched else (), np.float64, name='reward')
+
+    def discount_spec(self):
+        return BoundedArray((self.n_envs,) if self._batched else (), np.float64, 0.0, 1.0, name='discount')
+
+    def control_timestep(self):
+        return self._control_timestep
+
+    # -------------------------------------------------------------------------------- episode
+    def request_reset(self, env_ids):
+        """Restart the listed envs at the next step (their action of that step is dropped and they report FIRST), whatever their
+        episode state -- an actor restarting single environments."""
+        ids = np.asarray(env_ids, np.int64).reshape(-1)
+        if len(ids) == 0:
+            return
+        if self._device_task:
+            self._sim.task_request_reset(ids)
+        self._needs_reset[ids] = True
+
+    def _count_overflows(self, rec):
+        """count the envs whose step hit a contact / constraint-row capacity (FB_FLAGS bits 1, 2: counted, not a termination)
+        -> the record's _scalars columns (flags, |qacc|^2, time)"""
+        scal = rec[:, self._obs_slices['_scalars']]
+        self.n_capacity_overflows += int(((scal[:, 0].astype(np.int64) & 6) != 0).sum())
+        return scal
+
+    def _bad_state(self, rec):
+        """non-finite / diverged state (FB_FLAGS bit 0) or |qacc| > _TERMINAL_QACC: the reference terminates on it (base.py:222-225)"""
+        scal = self._count_overflows(rec)
+        return ((scal[:, 0].astype(np.int64) & 1) != 0) | ~(np.sqrt(scal[:, 1].astype(np.float64)) <= _TERMINAL_QACC)
+
+    def _end_step(self, resetting, terminate, reward, time, end_ok=None):
+        """get_discount and the step type (base.py:203-225) -> step_type, reward, discount, needs_reset.  A termination costs the
+        discount except where `end_ok` (walking / flight at the end of the reference); the time limit ends an episode with discount 1.
+        Rows that were reset this call report FIRST (their action was ignored).  The device's tk_end_step is the same logic."""
+        last = terminate | (time >= self._time_limit - 1e-9)
+        discount = np.where(terminate if end_ok is None else terminate & ~end_ok, 0.0, 1.0)
+        step_type = np.where(resetting, StepType.FIRST, np.where(last, StepType.LAST, StepType.MID))
+        return step_type, np.where(resetting, 0.0, reward), np.where(resetting, 1.0, discount), last & ~resetting
+
+    def _task_program_base(self):
+        """the fb_task_program fields every task sets; a task updates its own (ghost, thresholds, reference, wing-beat tables ...).
+        Thresholds are off (+-3e38) but the bad-state |qacc|."""
+        m = self.model
+        sens = m.meta['sensor_names']
+        return dict(kind=self._task_kind, root_qadr=self._root_q, root_vadr=self._root_v, ghost_qadr=-1, ghost_vadr=-1,
+                    user_col=len(self._ctrl_of_action) if self._n_user else -1, control_timestep=self._control_timestep,
+                    time_limit=self._time_limit, terminal_com_dist=3e38, terminal_linvel=3e38, terminal_angvel=3e38,
+                    terminal_qacc=_TERMINAL_QACC, terminal_height=-3e38, velocimeter_adr=int(m.sensor_adr[sens.index('walker/velocimeter')]),
+                    gyro_adr=int(m.sensor_adr[sens.index('walker/gyro')]), com_body=m.body_id('walker/thorax'), reset_qpos=m.qpos0,
+                    n_noise=0, seed=int(self._seed) & 0xffffffff)
+
+    def _device_step(self, action):
+        """one control step with the task hooks on the device: actions in, observation rows + (reward, discount, step_type) out"""
+        resetting = self._needs_reset.copy()
+        self._before_device_step(resetting)
+        self._sim.task_step(action, self._n_sub)
+        self._sim.task_read(self._rec, self._out4)
+        self._count_overflows(self._rec)
+        self._time = np.where(resetting, 0.0, self._time + self._control_timestep)
+        self.n_resets += int(resetting.sum())
+        self._after_device_step(action, resetting)
+        step_type = self._out4[:, 2].astype(np.int64)
+        self._needs_reset = step_type == int(StepType.LAST)
+        return TimeStep(step_type, self._out4[:, 0].astype(np.float64), self._out4[:, 1].astype(np.float64), self._observation(self._rec))
+
+    def _device_reset(self):
+        """reset() with the task hooks on the device: every env starts an episode in one held step (FIRST)"""
+        self._sim.task_reset_all()
+        self._needs_reset[:] = True
+        return self._unbatch(self._device_step(np.zeros((self.n_envs, self._action_spec.shape[0]), np.float32)), first=True)
+
+    def _task_step_device(self, action):
+        """step_device's control step for actions already on the device (nothing read back)"""
+        cai = action.__cuda_array_interface__
+        assert tuple(cai['shape']) == (self.n_envs, self._action_spec.shape[0]) and cai['typestr'] == '<f4', cai
+        self._sim.task_step(cai['data'][0], self._n_sub, is_device=True)
+        self._needs_reset[:] = False            # (host mirror of the device's reset flags: not read back on this path)
+
+    def _device_views(self):
+        """zero-copy torch views (observation rows [n_envs, obs_dim], out [n_envs, 4]) of the library's task buffers"""
+        if self._dev_views is None:
+            obs_ptr, dim, out_ptr = self._sim.task_ptrs()
+            self._dev_views = (_device_tensor(obs_ptr, (self.n_envs, dim), '<f4', self._sim.device),
+                               _device_tensor(out_ptr, (self.n_envs, 4), '<f4', self._sim.device))
+        return self._dev_views
+
+    def _unbatch(self, ts, first=False):
+        if self._batched:
+            return ts
+        obs = collections.OrderedDict((k, v[0]) for k, v in ts.observation.items())
+        if first or ts.step_type[0] == StepType.FIRST:
+            return TimeStep(StepType.FIRST, None, None, obs)
+        return TimeStep(StepType(int(ts.step_type[0])), float(ts.reward[0]), float(ts.discount[0]), obs)
+
+    def close(self):
+        self._sim.close()
+
+
+class BatchedFlyEnv(_TaskEnv):
     """dm_env-shaped environment over N lock-stepped flies (composer.Environment stand-in)."""
 
     def __init__(self, variant, n_envs, device=0, terminal_com_dist=0.3, time_limit=10.0, future_steps=64,
@@ -231,56 +393,33 @@ class BatchedFlyEnv:
                  max_reference_steps=None, device_task=False, model=None):
         assert variant in _VARIANTS
         self._variant = variant
-        self._batched = n_envs is not None
-        self.n_envs = int(n_envs) if self._batched else 1
-        self.model = model if model is not None else load_model(variant)      # `model`: a variant from flymodel.model_for
+        v = _VARIANTS[variant]
+        # `model`: a variant from flymodel.model_for; flight has one user action, the beat frequency (flight_imitation.py:38)
+        super().__init__(model if model is not None else load_model(variant), n_envs, device, lib_path, v['dt'], time_limit,
+                         n_user=1 if variant == 'flight' else 0, seed=seed, kind=v['kind'], device_task=device_task)
         m = self.model
         self._device = int(device)
-        self._sim = st.BatchedStepper(m, self.n_envs, device=device, lib_path=lib_path)
-        self._control_timestep = _VARIANTS[variant]['dt']
-        self._physics_timestep = float(m.opt_timestep)
-        self._n_sub = int(round(self._control_timestep / self._physics_timestep))
-        self._time_limit = time_limit
         self.physics = _PhysicsFacade(self)
         if variant == 'walk':
             self.task = WalkImitationTask(self, traj_generator or InferenceWalkingTrajectoryLoader(), terminal_com_dist,
                                           future_steps, time_limit, self._control_timestep)
-            self._n_user = 0
         elif variant == 'template':
             self.task = TemplateTask(self, time_limit, self._control_timestep)
-            self._n_user = 0
         elif variant == 'ball':
             self.task = WalkOnBallTask(self, time_limit, self._control_timestep)
-            self._n_user = 0
         else:
             self._wbpg = BatchedWingBeatPatternGenerator(self.n_envs, base_pattern_path=wpg_pattern_path)
             self.task = FlightImitationTask(self, self._wbpg, traj_generator or InferenceFlightTrajectoryLoader(),
                                             terminal_com_dist, future_steps, time_limit, self._control_timestep)
-            self._n_user = 1                                          # flight_imitation.py:38 num_user_actions=1
-        self._rs = np.random.RandomState(seed)
         self._reset_noise = reset_noise
         N = self.n_envs
-        # --- action <-> ctrl maps (reference fruitfly.py:342-379, 532-579): actuator classes in fixed order, then user
-        ci = m.meta['ctrl_indices']
-        idx, self._action_indices = [], {}
-        for key in _ACTION_CLASS_ORDER:
-            if ci.get(key):
-                self._action_indices[key] = np.arange(len(idx), len(idx) + len(ci[key]))
-                idx.extend(ci[key])
-        self._ctrl_of_action = np.asarray(idx, np.int64)
         # walking: actions go to the device as they are, the action -> ctrl permutation and NaN -> 0 run in the scatter
         # kernel (fb_set_action_map); flight keeps the host path because the wing actions are modified by the WBPG first
-        self._device_task = bool(device_task)       # task hooks evaluated on the device (fb_task_*): no host logic in step()
         self._device_action_map = variant in ('walk', 'template', 'ball') or self._device_task
         if self._device_action_map:
             # user actions (flight: the beat frequency) have no ctrl slot: column -> -1, read by the device-side task code
             self._sim.set_action_map(np.concatenate([self._ctrl_of_action, -np.ones(self._n_user, np.int64)]) if self._device_task
                                      else self._ctrl_of_action)
-        names = [m.meta['actuator_names'][i].split('/')[-1] for i in idx] + [f'user_{i}' for i in range(self._n_user)]
-        rng = m.actuator_ctrlrange[idx]
-        lo = np.concatenate([rng[:, 0], -np.ones(self._n_user)])
-        hi = np.concatenate([rng[:, 1], np.ones(self._n_user)])
-        self._action_spec = BoundedArray((len(names),), np.float64, lo, hi, name='\t'.join(names))
         # --- index tables
         jn = m.meta['jnt_names']
         # the walker's free joint (-1: none, walk_on_ball's thorax is welded to the world)
@@ -325,7 +464,6 @@ class BatchedFlyEnv:
         self._rec = None
         self._program_ref_id = None
         self._program_switched = False
-        self.n_capacity_overflows = 0            # env-steps whose contact / constraint-row lists hit their capacity (FB_FLAGS bits 1, 2)
         # One reference per env (dataset loaders hand out a different snippet per episode) or one shared by all envs (the
         # Inference* loaders hold a single trajectory): the shared case keeps one device table, the per-env case one slot per env.
         tg = self.task._traj_generator
@@ -358,7 +496,6 @@ class BatchedFlyEnv:
             if short:
                 raise ValueError(f'randomize_start_step needs trajectories longer than {tg.START_MARGIN} rows; trajectories {short} have '
                                  f'{[tg.trajectory_len(j) for j in short]}')
-        self._seed = seed
         if not self._inference_mode:
             jnames, snames = tg.get_joint_names(), tg.get_site_names()
             mj = [jn.index('walker/' + n) for n in jnames]
@@ -366,19 +503,12 @@ class BatchedFlyEnv:
             self._mocap_sites = np.array([sn.index('walker/' + n) for n in snames], np.int64)
             self._bank = _FeatureBank()
             self._env_bank_off = np.zeros(N, np.int64)
-        # --- per-env episode state
         self._step_counter = np.zeros(N, np.int64)
-        self._time = np.zeros(N)
-        self._needs_reset = np.ones(N, bool)
         self._ref_qpos = None
         self.h2d_bytes_per_step = 0
         self.d2h_bytes_per_step = 0
-        self.n_resets = 0
 
     # ---------------------------------------------------------------------------------- specs
-    def action_spec(self):
-        return self._action_spec
-
     def _obs_table(self):
         """(name, width, shape, program item) per observable, in spec order; hidden entries last."""
         m, sd, f = self.model, self._sd, self._future
@@ -429,15 +559,6 @@ class BatchedFlyEnv:
         return collections.OrderedDict((n, Array(lead + shp, np.float32, name=n)) for n, _, shp, _ in self._obs_table()
                                        if not n.startswith('_'))
 
-    def reward_spec(self):
-        return Array((self.n_envs,) if self._batched else (), np.float64, name='reward')
-
-    def discount_spec(self):
-        return BoundedArray((self.n_envs,) if self._batched else (), np.float64, 0.0, 1.0, name='discount')
-
-    def control_timestep(self):
-        return self._control_timestep
-
     # -------------------------------------------------------------------------------- episode
     def _upload_program(self):
         """Observation program = the task's observables in spec order, evaluated on the device (fb_obs_program)."""
@@ -460,14 +581,9 @@ class BatchedFlyEnv:
         off = np.concatenate([[0], np.cumsum(widths)])
         self._obs_slices = {r[0]: slice(int(off[i]), int(off[i + 1])) for i, r in enumerate(rows)}
         self._obs_shapes = {r[0]: r[2] for r in rows}
-        N = self.n_envs
-        try:
-            import torch
-            self._rec = torch.empty((N, dim), dtype=torch.float32).pin_memory().numpy() if torch.cuda.is_available() \
-                else np.empty((N, dim), np.float32)
-        except Exception:
-            self._rec = np.empty((N, dim), np.float32)
+        self._rec = _pinned((self.n_envs, dim), np.float32)
         if self._device_task:
+            self._out4 = _pinned((self.n_envs, 4), np.float32)
             self._upload_task_program()
             self._dev_views = None
 
@@ -477,15 +593,13 @@ class BatchedFlyEnv:
         q0 = m.qpos0.copy()
         if self._variant == 'walk':
             q0[self._wing_qadr] = self._wing_spring
-        kw = dict(kind=0 if self._variant == 'walk' else 1, root_qadr=self._root_q, root_vadr=self._root_v, ghost_qadr=self._ghost_q,
-                  ghost_vadr=self._ghost_v, user_col=len(self._ctrl_of_action) if self._n_user else -1, ghost_offset=t._ghost_offset,
-                  control_timestep=self._control_timestep, time_limit=self._time_limit, terminal_com_dist=min(t._terminal_com_dist, 3e38),
-                  terminal_linvel=_TERMINAL_LINVEL, terminal_angvel=_TERMINAL_ANGVEL, terminal_qacc=_TERMINAL_QACC, terminal_height=_TERMINAL_HEIGHT,
-                  velocimeter_adr=int(self._sd['velocimeter'][0]), gyro_adr=int(self._sd['gyro'][0]), com_body=m.body_id('walker/thorax'),
-                  obs_refdisp_off=sl['walker/ref_displacement'].start, obs_refquat_off=sl['walker/ref_root_quat'].start,
-                  reset_qpos=q0, n_noise=len(self._leg_act_qadr) if (self._variant == 'walk' and self._reset_noise > 0) else 0,
-                  noise_qadr=self._leg_act_qadr if (self._variant == 'walk' and self._reset_noise > 0) else None,
-                  noise_amp=self._reset_noise, seed=int(self._seed) & 0xffffffff, com_offset=_COM_OFFSET)
+        noise = self._variant == 'walk' and self._reset_noise > 0
+        kw = self._task_program_base() | dict(
+            ghost_qadr=self._ghost_q, ghost_vadr=self._ghost_v, ghost_offset=t._ghost_offset, terminal_com_dist=min(t._terminal_com_dist, 3e38),
+            terminal_linvel=_TERMINAL_LINVEL, terminal_angvel=_TERMINAL_ANGVEL, terminal_height=_TERMINAL_HEIGHT,
+            obs_refdisp_off=sl['walker/ref_displacement'].start, obs_refquat_off=sl['walker/ref_root_quat'].start, reset_qpos=q0,
+            n_noise=len(self._leg_act_qadr) if noise else 0, noise_qadr=self._leg_act_qadr if noise else None, noise_amp=self._reset_noise,
+            com_offset=_COM_OFFSET)
         if self._device_bank and self._variant == 'flight':      # the draws of _load_snippet / HDF5FlightTrajectoryLoader.get_trajectory
             tg = t._traj_generator
             self._sim.ref_bank(*self._bank_tables())
@@ -514,7 +628,6 @@ class BatchedFlyEnv:
                       wb_phase_mod=np.where(np.isfinite(wb.phase_mod), wb.phase_mod, 3e38), wb_freqs=wb.beat_freqs, wb_len=wb.lengths,
                       wb_base_freq=wb.base_beat_freq, wb_rel_range=wb.rel_freq_range, wb_rate=wb._rate)
         self._sim.task_program(**kw)
-        self._out4 = np.zeros((self.n_envs, 4), np.float32)
 
     def _snippet_root(self, snip):
         """root-joint reference (qpos [T,7], qvel [T,6]) of one loader snippet."""
@@ -718,30 +831,20 @@ class BatchedFlyEnv:
         self._needs_reset[ids] = False
         self.n_resets += n
 
-    def _device_step(self, action):
-        """one control step with the task hooks on the device: actions in, observation rows + (reward, discount, step_type) out."""
-        resetting = self._needs_reset.copy()
+    def _before_device_step(self, resetting):
         if resetting.any():
             self._load_snippet(np.nonzero(resetting)[0])            # a trajectory set since the last reset re-uploads the programs
             if self._program_switched:                              # ... which restarts every env on the device (fb_task_reset_all)
                 resetting[:] = True
                 self._program_switched = False
-        if self._variant == 'flight' and resetting.any():           # the wing-beat phases the host path would draw at these resets
-            ids = np.nonzero(resetting)[0]
-            self._sim.task_uniforms(ids, self._rs.uniform(size=len(ids)))
-        self._sim.task_step(action, self._n_sub)
-        self._sim.task_read(self._rec, self._out4)
-        flags = self._rec[:, self._obs_slices['_scalars']][:, 0].astype(np.int64)      # bits 1, 2: capacity overflows (counted, not a termination)
-        self.n_capacity_overflows += int(((flags & 6) != 0).sum())
+            if self._variant == 'flight':                           # the wing-beat phases the host path would draw at these resets
+                ids = np.nonzero(resetting)[0]
+                self._sim.task_uniforms(ids, self._rs.uniform(size=len(ids)))
+
+    def _after_device_step(self, action, resetting):
         self.h2d_bytes_per_step = action.nbytes
         self.d2h_bytes_per_step = self._rec.nbytes + self._out4.nbytes
         self._step_counter = np.where(resetting, 0, self._step_counter + 1)
-        self._time = np.where(resetting, 0.0, self._time + self._control_timestep)
-        self.n_resets += int(resetting.sum())
-        step_type = self._out4[:, 2].astype(np.int64)
-        self._needs_reset = step_type == int(StepType.LAST)
-        return TimeStep(step_type,
-                        self._out4[:, 0].astype(np.float64), self._out4[:, 1].astype(np.float64), self._observation(self._rec))
 
     def set_applied_forces(self, qfrc=None, xfrc=None, env_ids=None):
         """MuJoCo's `physics.data.qfrc_applied` ([nv] per env) and `xfrc_applied` ([nbody, 6] per env: world-frame force, then torque,
@@ -753,16 +856,6 @@ class BatchedFlyEnv:
     def clear_applied_forces(self):
         """zero every env's applied forces (the step goes back to the path without the applied-force term)"""
         self._sim.clear_applied()
-
-    def request_reset(self, env_ids):
-        """Restart the listed envs at the next step (their action of that step is dropped and they report FIRST), whatever their
-        episode state -- an actor restarting single environments."""
-        ids = np.asarray(env_ids, np.int64).reshape(-1)
-        if len(ids) == 0:
-            return
-        if self._device_task:
-            self._sim.task_request_reset(ids)
-        self._needs_reset[ids] = True
 
     def set_reset_noise(self, amp):
         """U(-amp, amp) rad added to the actuated leg joints of the start pose at the resets from now on (0: the reference's exact
@@ -789,18 +882,8 @@ class BatchedFlyEnv:
         flight, start step) on the device (counter hash of seed, env, episode), so no trajectory index may be pending."""
         if not self._device_task:
             raise RuntimeError('step_device needs device_task=True (task hooks on the device)')
-        import torch
         self._launch_step_device(action)
-        if getattr(self, '_dev_views', None) is None:
-            obs_ptr, dim, out_ptr = self._sim.task_ptrs()
-
-            class _View:
-                def __init__(self, ptr, shape):
-                    self.__cuda_array_interface__ = {'shape': shape, 'typestr': '<f4', 'data': (int(ptr), False), 'version': 2}
-            dev = f'cuda:{self._device}'
-            self._dev_views = (torch.as_tensor(_View(obs_ptr, (self.n_envs, dim)), device=dev),
-                               torch.as_tensor(_View(out_ptr, (self.n_envs, 4)), device=dev))
-        return self._dev_views
+        return self._device_views()
 
     def _launch_step_device(self, action):
         """the work of step_device up to its result views: the control step on the device, for actions already there"""
@@ -812,10 +895,7 @@ class BatchedFlyEnv:
                 self._ensure_slots()
             else:
                 self._load_snippet(np.arange(self.n_envs))
-        cai = action.__cuda_array_interface__
-        assert tuple(cai['shape']) == (self.n_envs, self._action_spec.shape[0]) and cai['typestr'] == '<f4', cai
-        self._sim.task_step(cai['data'][0], self._n_sub, is_device=True)
-        self._needs_reset[:] = False            # (host mirror of the device's reset flags: not read back on this path)
+        self._task_step_device(action)
 
     # ---------------------------------------------------------------------------------- eyes
     # cameras `eye_right` / `eye_left` on the head (reference fruitfly.xml:335-336; the head body keeps its XML frame)
@@ -855,10 +935,7 @@ class BatchedFlyEnv:
                 self._ensure_slots()
             else:
                 self._load_snippet(np.arange(self.n_envs))
-            self._sim.task_reset_all()
-            self._needs_reset[:] = True
-            ts = self._device_step(np.zeros((self.n_envs, self._action_spec.shape[0]), np.float32))    # every env held: FIRST
-            return self._unbatch(ts, first=True)
+            return self._device_reset()
         self._reset_envs(np.arange(self.n_envs))
         self._sim.task_inputs(self._step_counter, np.ones(self.n_envs, np.uint8))
         rec = self._sim.read_task_obs(self._rec)
@@ -927,12 +1004,7 @@ class BatchedFlyEnv:
         step_now = np.round(time / self._control_timestep).astype(np.int64)
         com_dist = np.linalg.norm(obs['walker/ref_displacement'][:, 0], axis=1)
         reached_end = step_now == self._episode_steps
-        scal = rec[:, sl['_scalars']]
-        # FB_FLAGS bit 0 = non-finite / diverged state (reference base.py:222-225 terminates on it); bits 1, 2 = contact /
-        # constraint-row capacity overflows, which are counted, not treated as bad physics
-        flags = scal[:, 0].astype(np.int64)
-        self.n_capacity_overflows += int(((flags & 6) != 0).sum())
-        bad = ((flags & 1) != 0) | ~(np.sqrt(scal[:, 1].astype(np.float64)) <= _TERMINAL_QACC)
+        bad = self._bad_state(rec)
         if self._variant == 'walk':
             linvel = np.linalg.norm(rec[:, sl['_velocimeter_now']], axis=1)
             angvel = np.linalg.norm(rec[:, sl['_gyro_now']], axis=1)
@@ -953,14 +1025,7 @@ class BatchedFlyEnv:
             disp = np.linalg.norm(ghost_com - rec[:, sl['_subtree_com']], axis=1)
             qd = quat_dist_short_arc(np.array([1.0, 0, 0, 0]), obs['walker/ref_root_quat'][:, 0].astype(np.float64))
             reward = linear_tolerance(disp, 0.4) * linear_tolerance(qd, np.pi)
-        discount = np.where(terminate & ~reached_end, 0.0, 1.0)
-        last = terminate | (time >= self._time_limit - 1e-9)
-        step_type = np.where(last, StepType.LAST, StepType.MID)
-        # rows that were reset this call report FIRST (their action was ignored)
-        step_type = np.where(resetting, StepType.FIRST, step_type)
-        reward = np.where(resetting, 0.0, reward)
-        discount = np.where(resetting, 1.0, discount)
-        return step_type, reward, discount, last & ~resetting
+        return self._end_step(resetting, terminate, reward, time, end_ok=reached_end)
 
     def _walk_reward_factors(self, rec, step):
         """[N, 4 + 6]: DeepMimic factors (weights 20, 1, 1, 1) and one wing-retraction factor per wing joint
@@ -988,16 +1053,6 @@ class BatchedFlyEnv:
                 obs[k] = rec[:, sl].reshape((N,) + self._obs_shapes[k])
         return obs
 
-    def _unbatch(self, ts, first=False):
-        if self._batched:
-            return ts
-        obs = collections.OrderedDict((k, v[0]) for k, v in ts.observation.items())
-        if first or ts.step_type[0] == StepType.FIRST:
-            return TimeStep(StepType.FIRST, None, None, obs)
-        return TimeStep(StepType(int(ts.step_type[0])), float(ts.reward[0]), float(ts.discount[0]), obs)
-
-    def close(self):
-        self._sim.close()
 
 
 def walk_imitation(ref_path=None, force_actuators=False, disable_wings=True, traj_indices=None, random_state=None,
@@ -1051,7 +1106,7 @@ def vision_guided_flight(wpg_pattern_path=None, bumps_or_trench='bumps', force_a
     """Batched `flybody.fly_envs.vision_guided_flight` (reference `fly_envs.py:194-246`): 'bumps' or 'trench' terrain, eye
     cameras, wing-beat pattern generator, fatal ground contacts -- `flybody_b200.vision_env.BatchedVisionFlightEnv` (SURVEY.md
     8(f).1; terrain contacts against the fp64 oracle and eyes against the camera model in tests/test_hfield.py, test_eyes.py and on the
-    GPU in tests/test_gpu_parity.py).  `terrain_bank=K, device_task=True` run the task's hooks on the device (fb_task_* kind 2)."""
+    GPU in tests/test_gpu_parity.py).  `terrain_bank=K, device_task=True` run the task's hooks on the device (FB_TASK_VISION)."""
     if force_actuators or not disable_legs or joint_filter != 0.0:
         raise NotImplementedError('only the default vision_guided_flight model variant is compiled (flybody_b200/assets/fly_vision.npz)')
     from .vision_env import BatchedVisionFlightEnv
@@ -1066,8 +1121,8 @@ class TemplateTaskEnv(BatchedFlyEnv):
     An optional `action_corruptor(action, random_state)` rewrites the actions on the host before they are applied; `prev_action`
     returns what was applied (the reference walker's `prev_action`)."""
 
-    def __init__(self, n_envs, time_limit=1.0, action_corruptor=None, random_state=None, **kw):
-        super().__init__('template', n_envs, time_limit=time_limit, **kw)
+    def __init__(self, n_envs, time_limit=1.0, action_corruptor=None, random_state=None, variant='template', **kw):
+        super().__init__(variant, n_envs, time_limit=time_limit, **kw)
         self._corruptor = action_corruptor
         if random_state is not None:
             self._rs = random_state if isinstance(random_state, np.random.RandomState) else np.random.RandomState(random_state)
@@ -1083,13 +1138,7 @@ class TemplateTaskEnv(BatchedFlyEnv):
             self._upload_program()
 
     def _upload_task_program(self):
-        m = self.model
-        self._sim.task_program(kind=3, root_qadr=self._root_q, root_vadr=self._root_v, ghost_qadr=-1, ghost_vadr=-1, user_col=-1,
-                               control_timestep=self._control_timestep, time_limit=self._time_limit, terminal_com_dist=3e38,
-                               terminal_linvel=3e38, terminal_angvel=3e38, terminal_qacc=_TERMINAL_QACC, terminal_height=-3e38,
-                               velocimeter_adr=int(self._sd['velocimeter'][0]), gyro_adr=int(self._sd['gyro'][0]),
-                               com_body=m.body_id('walker/thorax'), reset_qpos=m.qpos0, n_noise=0, seed=int(self._seed) & 0xffffffff)
-        self._out4 = np.zeros((self.n_envs, 4), np.float32)
+        self._sim.task_program(**self._task_program_base())
 
     def _reset_envs(self, ids, hold=False):
         """physics.reset() (mj_resetData: qpos0 at rest, controls and applied forces zeroed) + initialize_episode"""
@@ -1136,15 +1185,9 @@ class TemplateTaskEnv(BatchedFlyEnv):
         return self._unbatch(TimeStep(step_type, reward, discount, obs))
 
     def _task_after(self, rec, obs, resetting, time, ghost):
-        """get_reward (factors (1,)), check_termination (base.py:222-225), get_discount; the device task kind 3 is the same logic"""
-        flags = rec[:, self._obs_slices['_scalars']][:, 0].astype(np.int64)
-        self.n_capacity_overflows += int(((flags & 6) != 0).sum())
-        bad = ((flags & 1) != 0) | ~(np.sqrt(rec[:, self._obs_slices['_scalars']][:, 1].astype(np.float64)) <= _TERMINAL_QACC)
-        last = bad | (time >= self._time_limit - 1e-9)
-        step_type = np.where(resetting, StepType.FIRST, np.where(last, StepType.LAST, StepType.MID))
-        reward = np.where(resetting, 0.0, 1.0)
-        discount = np.where(resetting | ~bad, 1.0, 0.0)
-        return step_type, reward, discount, last & ~resetting
+        """get_reward (factors (1,)), check_termination (base.py:222-225), get_discount; the device task FB_TASK_TEMPLATE is the same
+        logic"""
+        return self._end_step(resetting, self._bad_state(rec), 1.0, time)
 
     def step_device(self, action):
         if self._corruptor is not None:
@@ -1159,7 +1202,7 @@ def template_task(random_state=None, force_actuators=False, disable_wings=True, 
     """Batched `flybody.fly_envs.template_task` (reference `fly_envs.py:249-300`, `tasks/template_task.py`): the walking fly
     without a ghost on flat ground, reward 1, the reference's installation test (`tests/test_core.py`) and the class to start a
     walking task from.  `force_actuators`, `disable_wings=False`, `joint_filter` and `adhesion_filter` select a model variant
-    (`flymodel.model_for('template', ...)`).  `device_task=True` runs the task hooks on the device (kind 3), which `step_device` needs.
+    (`flymodel.model_for('template', ...)`).  `device_task=True` runs the task hooks on the device (FB_TASK_TEMPLATE), which `step_device` needs.
     `mjcb_control` (a per-substep Python callback) and `observables_options` are not supported."""
     if mjcb_control is not None:
         raise NotImplementedError('mjcb_control: a per-substep Python callback cannot run at batch speed (DESIGN.md section 8). Perturbation '
@@ -1189,39 +1232,22 @@ class WalkOnBallEnv(TemplateTaskEnv):
     discount 1 at the 2 s time limit.  `before_step` applies the action only."""
 
     def __init__(self, n_envs, time_limit=2.0, random_state=None, **kw):
-        BatchedFlyEnv.__init__(self, 'ball', n_envs, time_limit=time_limit, **kw)
-        self._corruptor = None
-        if random_state is not None:
-            self._rs = random_state if isinstance(random_state, np.random.RandomState) else np.random.RandomState(random_state)
-        self._prev_action = np.zeros((self.n_envs, self._action_spec.shape[0]))
+        super().__init__(n_envs, time_limit=time_limit, random_state=random_state, variant='ball', **kw)
 
     def _upload_task_program(self):
-        m = self.model
-        self._sim.task_program(kind=4, root_qadr=-1, root_vadr=-1, ghost_qadr=-1, ghost_vadr=-1, user_col=-1,
-                               control_timestep=self._control_timestep, time_limit=self._time_limit, terminal_com_dist=3e38,
-                               terminal_linvel=_TERMINAL_LINVEL, terminal_angvel=_TERMINAL_ANGVEL, terminal_qacc=_TERMINAL_QACC,
-                               terminal_height=-3e38, velocimeter_adr=int(self._sd['velocimeter'][0]), gyro_adr=int(self._sd['gyro'][0]),
-                               com_body=m.body_id('walker/thorax'), reset_qpos=m.qpos0, n_noise=0, seed=int(self._seed) & 0xffffffff,
-                               ball_vadr=self._ball_v, ball_target=_BALL_TARGET_QVEL, ball_margin=_BALL_MARGIN)
-        self._out4 = np.zeros((self.n_envs, 4), np.float32)
+        self._sim.task_program(**self._task_program_base() | dict(terminal_linvel=_TERMINAL_LINVEL, terminal_angvel=_TERMINAL_ANGVEL,
+                                                                  ball_vadr=self._ball_v, ball_target=_BALL_TARGET_QVEL, ball_margin=_BALL_MARGIN))
 
     def _task_after(self, rec, obs, resetting, time, ghost):
-        """get_reward_factors, check_termination (walk_on_ball.py:55-81, base.py:222-225), get_discount; the device task kind 4 is the
-        same logic"""
+        """get_reward_factors, check_termination (walk_on_ball.py:55-81, base.py:222-225), get_discount; the device task FB_TASK_BALL is
+        the same logic"""
         sl = self._obs_slices
-        flags = rec[:, sl['_scalars']][:, 0].astype(np.int64)
-        self.n_capacity_overflows += int(((flags & 6) != 0).sum())
-        bad = ((flags & 1) != 0) | ~(np.sqrt(rec[:, sl['_scalars']][:, 1].astype(np.float64)) <= _TERMINAL_QACC)
         linvel = np.linalg.norm(rec[:, sl['_velocimeter_now']], axis=1)
         angvel = np.linalg.norm(rec[:, sl['_gyro_now']], axis=1)
-        terminate = (linvel > _TERMINAL_LINVEL) | (angvel > _TERMINAL_ANGVEL) | bad
+        terminate = (linvel > _TERMINAL_LINVEL) | (angvel > _TERMINAL_ANGVEL) | self._bad_state(rec)
         ball_qvel = obs['walker/ball_qvel'].astype(np.float64)
         reward = np.prod(linear_tolerance(ball_qvel - np.asarray(_BALL_TARGET_QVEL), _BALL_MARGIN), axis=1)
-        last = terminate | (time >= self._time_limit - 1e-9)
-        step_type = np.where(resetting, StepType.FIRST, np.where(last, StepType.LAST, StepType.MID))
-        reward = np.where(resetting, 0.0, reward)
-        discount = np.where(resetting | ~terminate, 1.0, 0.0)
-        return step_type, reward, discount, last & ~resetting
+        return self._end_step(resetting, terminate, reward, time)
 
 
 def walk_on_ball(force_actuators=False, disable_wings=True, random_state=None, n_envs=None, device=0, lib_path=None, seed=0,
@@ -1229,7 +1255,7 @@ def walk_on_ball(force_actuators=False, disable_wings=True, random_state=None, n
     """Batched `flybody.fly_envs.walk_on_ball` (reference `fly_envs.py:158-191`, `tasks/walk_on_ball.py`): the tethered fly walking on
     a floating ball, 10 substeps of 2e-4 s per control step, a 2 s time limit, 59 actions and the ten walker observables plus
     `walker/ball_qvel`.  `force_actuators` and `disable_wings=False` select a model variant (`flymodel.model_for('ball', ...)`).
-    `device_task=True` runs the task hooks on the device (kind 4), which `step_device` needs."""
+    `device_task=True` runs the task hooks on the device (FB_TASK_BALL), which `step_device` needs."""
     model = None
     if force_actuators or not disable_wings:
         from .flymodel import model_for

@@ -25,6 +25,9 @@ EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl'
            'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version']
 
 
+# enum FbTaskKind (FbTaskProgram.kind)
+TASK_WALK, TASK_FLIGHT, TASK_VISION, TASK_TEMPLATE, TASK_BALL = range(5)
+
 # enum FbObsItem
 (OBS_SENSOR_MEAN, OBS_SENSOR_NOW, OBS_ACT, OBS_QPOS, OBS_QVEL, OBS_SITES_EGO, OBS_ROOT_ZAXIS, OBS_REF_DISP,
  OBS_REF_QUAT, OBS_SCALARS, OBS_ROOT_POSE, OBS_SUBTREE_COM, OBS_DOF_AXIS_EGO, OBS_WORLD_CONTACT, OBS_TASK_TARGET) = range(15)

@@ -15,10 +15,10 @@ import numpy as np
 
 from . import arenas
 from . import stepper as st
-from .dm_env_shim import Array, BoundedArray, StepType, TimeStep
-from .fly_envs import BatchedFlyEnv, BatchedWingBeatPatternGenerator
+from .dm_env_shim import Array, StepType, TimeStep
+from .fly_envs import BatchedFlyEnv, BatchedWingBeatPatternGenerator, _TaskEnv, _device_tensor, _pinned
 from .flymodel import load_model
-from .synthetic import _ACTION_CLASS_ORDER, _FLY_CONTROL_TIMESTEP, _TERMINAL_QACC
+from .synthetic import _FLY_CONTROL_TIMESTEP
 
 _BODY_PITCH_ANGLE = 47.5          # reference tasks/constants.py: body pitch of the hover pose, degrees
 
@@ -30,7 +30,7 @@ def _tolerance_linear(x, lo, hi, margin):
     return np.where(d <= 0, 1.0, np.clip(1.0 - d, 0.0, 1.0))
 
 
-class BatchedVisionFlightEnv:
+class BatchedVisionFlightEnv(_TaskEnv):
     """dm_env-shaped environment over N lock-stepped flies on their own terrains."""
 
     _OBS = ('accelerometer', 'actuator_activation', 'gyro', 'joints_pos', 'joints_vel', 'left_eye', 'right_eye', 'velocimeter', 'world_zaxis',
@@ -41,14 +41,11 @@ class BatchedVisionFlightEnv:
                  init_pos_y_range=(0, 0), time_limit=0.4, floor_contacts_fatal=True, terrain_bank=None, device_task=False, **kwargs_arena):
         if bumps_or_trench not in ('bumps', 'trench'):
             raise ValueError("Only 'bumps' and 'trench' terrains are supported.")
-        self._batched = n_envs is not None
-        self.n_envs = N = int(n_envs) if self._batched else 1
-        self.model = m = load_model('vision')
-        self._sim = st.BatchedStepper(m, N, device=device, lib_path=lib_path)
-        self._control_timestep, self._physics_timestep = _FLY_CONTROL_TIMESTEP, float(m.opt_timestep)
-        self._n_sub = int(round(self._control_timestep / self._physics_timestep))
-        self._time_limit, self._fatal = time_limit, floor_contacts_fatal
-        self._rs = np.random.RandomState(seed)
+        # head 3, wings 6, abdomen 2 actions + 1 user action (beat frequency)
+        super().__init__(load_model('vision'), n_envs, device, lib_path, _FLY_CONTROL_TIMESTEP, time_limit, n_user=1, seed=seed,
+                         kind=st.TASK_VISION, device_task=device_task)
+        m, N = self.model, self.n_envs
+        self._fatal = floor_contacts_fatal
         self._wbpg = BatchedWingBeatPatternGenerator(N, base_pattern_path=wpg_pattern_path)
         cls = arenas.SineBumps if bumps_or_trench == 'bumps' else arenas.SineTrench
         self._arenas = [cls(**kwargs_arena) for _ in range(N)]
@@ -66,17 +63,6 @@ class BatchedVisionFlightEnv:
                 self._bank.append((t.astype(np.float32), a0.trench_specs))
         self._sim.hfield_collision(m.meta['hf_geom'], m.hf_size, a0.nrow, a0.ncol, m.hf_pair_geom)
         self._ranges = dict(h=target_height_range, v=target_speed_range, x=init_pos_x_range, y=init_pos_y_range)
-        # action <-> ctrl (reference fruitfly.py:342-379): head 3, wings 6, abdomen 2, + 1 user action (beat frequency)
-        ci, idx, self._action_indices = m.meta['ctrl_indices'], [], {}
-        for key in _ACTION_CLASS_ORDER:
-            if ci.get(key):
-                self._action_indices[key] = np.arange(len(idx), len(idx) + len(ci[key]))
-                idx.extend(ci[key])
-        self._ctrl_of_action = np.asarray(idx, np.int64)
-        names = [m.meta['actuator_names'][i].split('/')[-1] for i in idx] + ['user_0']
-        rng = m.actuator_ctrlrange[idx]
-        self._action_spec = BoundedArray((len(names),), np.float64, np.concatenate([rng[:, 0], [-1.0]]), np.concatenate([rng[:, 1], [1.0]]),
-                                         name='\t'.join(names))
         # index tables
         jn, sens = m.meta['jnt_names'], m.meta['sensor_names']
         self._root_q, self._root_v = m.jnt_qposadr_of('walker/'), m.jnt_dofadr_of('walker/')
@@ -84,6 +70,7 @@ class BatchedVisionFlightEnv:
         self._obs_qadr, self._obs_vadr = m.jnt_qposadr[obsj], m.jnt_dofadr[obsj]
         wing = [f'walker/wing_{a}_{s}' for s in ('left', 'right') for a in ('yaw', 'roll', 'pitch')]
         self._wing_qadr = np.array([m.jnt_qposadr_of(n) for n in wing])
+        self._wing_vadr = np.array([m.jnt_dofadr_of(n) for n in wing])
         self._wing_in_obs = np.array([m.meta['observable_joints'].index(n) for n in wing])
         sd = lambda n: int(m.sensor_adr[sens.index('walker/' + n)])
         up = m.site_quat[m.meta['site_names'].index('walker/hover_up_dir')].copy()
@@ -103,75 +90,44 @@ class BatchedVisionFlightEnv:
         dim = self._sim.obs_program([r[2] for r in rows], lists, m.body_id('walker/thorax'), self._n_sub, None)
         off = np.concatenate([[0], np.cumsum([r[1] for r in rows])])
         assert off[-1] == dim
-        self._sl = {r[0]: slice(int(off[i]), int(off[i + 1])) for i, r in enumerate(rows)}
-        self._rec = self._pinned((N, dim), np.float32)
+        # column slices of the rows (`_obs_slices`: the name the shared shell reads)
+        self._sl = self._obs_slices = {r[0]: slice(int(off[i]), int(off[i + 1])) for i, r in enumerate(rows)}
+        self._rec = _pinned((N, dim), np.float32)
+        self._out4 = _pinned((N, 4), np.float32)
         # eyes
         quats = [np.asarray(q, np.float64) / np.linalg.norm(q) for _, _, q in BatchedFlyEnv._EYE_CAMERAS]
         head = m.body_id('walker/head')
         self._sim.eye_program([head, head], [p for _, p, _ in BatchedFlyEnv._EYE_CAMERAS], quats, fovy_deg=eye_camera_fovy, size=eye_camera_size,
                               nrow=a0.nrow, ncol=a0.ncol, half_size=self._half, z_offset=float(m.geom_pos[m.meta['hf_geom']][2]))
         self._eye_size = eye_camera_size
-        self._eyes_host = self._pinned((N, 2, eye_camera_size, eye_camera_size, 3), np.uint8)      # D2H target of every step's render
+        self._eyes_host = _pinned((N, 2, eye_camera_size, eye_camera_size, 3), np.uint8)      # D2H target of every step's render
         self._eyes_dev = None
         # per-env episode state
         self._target_height, self._target_speed = np.zeros(N), np.zeros(N)
-        self._time = np.zeros(N)
-        self._needs_reset = np.ones(N, bool)
         self._wing_qpos = np.zeros((N, 6))
         self._has_trench = np.zeros(N, bool)
         self._last_draws = np.zeros((N, 8), np.float32)
-        self.n_resets = 0
-        self.n_capacity_overflows = 0            # env-steps whose contact / constraint-row lists hit their capacity (FB_FLAGS bits 1, 2)
-        # task hooks on the device (fb_task_*, kind 2): needs the terrain bank (a resetting env copies one of its terrains on the device)
-        self._device_task = bool(device_task)
+        # task hooks on the device (fb_task_*, FB_TASK_VISION): needs the terrain bank (a resetting env copies one of its terrains on the device)
         if self._device_task:
             if self._bank is None:
                 raise NotImplementedError('device_task=True needs terrain_bank=K (a resetting env copies one of the K terrains on the device)')
             self._upload_task_program(seed)
 
-    @staticmethod
-    def _pinned(shape, dtype):
-        """page-locked host buffer where torch + CUDA are present (device -> host copies at full PCIe rate), plain numpy otherwise"""
-        try:
-            import torch
-            if torch.cuda.is_available():
-                return torch.empty(shape, dtype=getattr(torch, np.dtype(dtype).name)).pin_memory().numpy()
-        except Exception:
-            pass
-        return np.empty(shape, dtype)
-
     def eyes_device(self):
         """zero-copy torch view [n_envs, 2, size, size, 3] uint8 (index 0 right eye, 1 left eye) of the images the last step rendered,
         on this env's device -- for a policy that lives on the GPU (the numpy observation holds the same images on the host)."""
-        import torch
         if self._eyes_dev is None:
             ptr, nbytes = self._sim.eyes_ptr()
-
-            class _View:
-                def __init__(self, ptr, shape):
-                    self.__cuda_array_interface__ = {'shape': shape, 'typestr': '|u1', 'data': (int(ptr), False), 'version': 2}
-            self._eyes_dev = torch.as_tensor(_View(ptr, (self.n_envs, 2, self._eye_size, self._eye_size, 3)), device=f'cuda:{self._sim.device}')
+            self._eyes_dev = _device_tensor(ptr, (self.n_envs, 2, self._eye_size, self._eye_size, 3), '|u1', self._sim.device)
         return self._eyes_dev
 
     # ---------------------------------------------------------------------------------- specs
-    def action_spec(self):
-        return self._action_spec
-
     def observation_spec(self):
         lead = (self.n_envs,) if self._batched else ()
         nq, s = len(self._obs_qadr), self._eye_size
         shapes = {'accelerometer': (3,), 'actuator_activation': (0,), 'gyro': (3,), 'joints_pos': (nq,), 'joints_vel': (nq,), 'left_eye': (s, s, 3),
                   'right_eye': (s, s, 3), 'velocimeter': (3,), 'world_zaxis': (3,), 'task_input': (2,)}
         return collections.OrderedDict(('walker/' + k, Array(lead + shapes[k], np.uint8 if 'eye' in k else np.float32, name='walker/' + k)) for k in self._OBS)
-
-    def reward_spec(self):
-        return Array((self.n_envs,) if self._batched else (), np.float64, name='reward')
-
-    def discount_spec(self):
-        return BoundedArray((self.n_envs,) if self._batched else (), np.float64, 0.0, 1.0, name='discount')
-
-    def control_timestep(self):
-        return self._control_timestep
 
     @property
     def target_height(self):
@@ -182,8 +138,10 @@ class BatchedVisionFlightEnv:
         return self._target_speed.copy()
 
     def _upload_task_program(self, seed):
-        """fb_task_program kind 2: the hooks of this env as a device-side program (same constants as the host path)."""
-        m, wb, r = self.model, self._wbpg, self._ranges
+        """fb_task_program FB_TASK_VISION: the hooks of this env as a device-side program (same constants as the host path); `seed`
+        seeds the device's counter-hash draws."""
+        self._seed = seed
+        wb, r = self._wbpg, self._ranges
         self._sim.set_action_map(np.concatenate([self._ctrl_of_action, [-1]]))      # the user action (beat frequency) has no ctrl slot
         self._sim.hfield_bank(np.stack([t for t, _ in self._bank]))
         dummy = np.zeros((1, 7), np.float32); dummy[0, 3] = 1.0
@@ -195,40 +153,25 @@ class BatchedVisionFlightEnv:
                 ty[k, :len(sp['y_coords'])] = sp['y_coords']
             trench = dict(trench_cap=cap, trench_y=ty, trench_len=np.array([len(sp['y_coords']) for _, sp in self._bank], np.int32),
                           trench_x=np.array([[sp['x_coords'][0], sp['x_coords'][-1]] for _, sp in self._bank], np.float32))
-        self._sim.task_program(
-            kind=2, root_qadr=self._root_q, root_vadr=self._root_v, ghost_qadr=-1, ghost_vadr=-1, user_col=len(self._ctrl_of_action),
-            ghost_offset=(0, 0, 0), control_timestep=self._control_timestep, time_limit=self._time_limit, terminal_com_dist=3e38, terminal_linvel=3e38,
-            terminal_angvel=3e38, terminal_qacc=_TERMINAL_QACC, terminal_height=-3e38,
-            velocimeter_adr=int(m.sensor_adr[m.meta['sensor_names'].index('walker/velocimeter')]),
-            gyro_adr=int(m.sensor_adr[m.meta['sensor_names'].index('walker/gyro')]), com_body=m.body_id('walker/thorax'), episode_steps=1 << 30, ref_len=1,
-            ref_qpos=dummy, ref_qvel=np.zeros((1, 6), np.float32), obs_refdisp_off=0, obs_refquat_off=0, reset_qpos=m.qpos0, n_noise=0, noise_qadr=None,
-            noise_amp=0.0, seed=int(seed) & 0xffffffff, n_wing=6, wing_qadr=self._wing_qadr,
-            wing_vadr=np.array([m.jnt_dofadr_of(n) for n in [f'walker/wing_{a}_{s_}' for s_ in ('left', 'right') for a in ('yaw', 'roll', 'pitch')]]),
-            wing_ctrl=self._ctrl_of_action[self._action_indices['wings']], n_freq=wb.traj.shape[0], tab_len=wb.traj.shape[1], wb_traj=wb.traj,
-            wb_phase=np.where(np.isfinite(wb.phase), wb.phase, 3e38), wb_phase_mod=np.where(np.isfinite(wb.phase_mod), wb.phase_mod, 3e38),
-            wb_freqs=wb.beat_freqs, wb_len=wb.lengths, wb_base_freq=wb.base_beat_freq, wb_rel_range=wb.rel_freq_range, wb_rate=wb._rate,
-            com_offset=(0, 0, 0), target_height_range=r['h'], target_speed_range=r['v'], init_x_range=r['x'], init_y_range=r['y'],
-            hover_quat=self._hover_quat, target_zaxis=self._target_zaxis, floor_contacts_fatal=1 if self._fatal else 0, **trench)
-        self._out4 = self._pinned((self.n_envs, 4), np.float32)
+        self._sim.task_program(**self._task_program_base() | dict(
+            episode_steps=1 << 30, ref_len=1, ref_qpos=dummy, ref_qvel=np.zeros((1, 6), np.float32), n_wing=6, wing_qadr=self._wing_qadr,
+            wing_vadr=self._wing_vadr, wing_ctrl=self._ctrl_of_action[self._action_indices['wings']], n_freq=wb.traj.shape[0],
+            tab_len=wb.traj.shape[1], wb_traj=wb.traj, wb_phase=np.where(np.isfinite(wb.phase), wb.phase, 3e38),
+            wb_phase_mod=np.where(np.isfinite(wb.phase_mod), wb.phase_mod, 3e38), wb_freqs=wb.beat_freqs, wb_len=wb.lengths,
+            wb_base_freq=wb.base_beat_freq, wb_rel_range=wb.rel_freq_range, wb_rate=wb._rate, target_height_range=r['h'],
+            target_speed_range=r['v'], init_x_range=r['x'], init_y_range=r['y'], hover_quat=self._hover_quat, target_zaxis=self._target_zaxis,
+            floor_contacts_fatal=1 if self._fatal else 0, **trench))
         self._dev_views = None
 
-    def _device_step(self, action, draws=None):
-        """one control step with the task hooks on the device: actions in, observation rows + (reward, discount, step_type) + eyes out"""
-        resetting = self._needs_reset.copy()
-        if draws is not None and resetting.any():               # (tests: the draws the host-side code would make at these resets)
+    def _before_device_step(self, resetting):
+        draws = getattr(self, '_forced_draws', None)               # (tests: the draws the host-side code would make at these resets)
+        if draws is not None and resetting.any():
             ids = np.nonzero(resetting)[0]
             self._sim.task_uniform_rows(ids, draws[ids])
-        self._sim.task_step(action, self._n_sub)
-        self._sim.task_read(self._rec, self._out4)
-        flags = self._rec[:, self._sl['_scalars']][:, 0].astype(np.int64)        # bits 1, 2: capacity overflows (counted, not a termination)
-        self.n_capacity_overflows += int(((flags & 6) != 0).sum())
-        self._time = np.where(resetting, 0.0, self._time + self._control_timestep)
-        self.n_resets += int(resetting.sum())
+
+    def _after_device_step(self, action, resetting):
         tgt = self._rec[:, self._sl['_task_target']]
         self._target_height, self._target_speed = tgt[:, 0].astype(np.float64), tgt[:, 1].astype(np.float64)
-        step_type = self._out4[:, 2].astype(np.int64)
-        self._needs_reset = step_type == int(StepType.LAST)
-        return TimeStep(step_type, self._out4[:, 0].astype(np.float64), self._out4[:, 1].astype(np.float64), self._observation())
 
     def step_device(self, action):
         """Device-resident control step (see `BatchedFlyEnv.step_device`): `action` a CUDA tensor [n_envs, 12]; returns zero-copy torch
@@ -236,31 +179,14 @@ class BatchedVisionFlightEnv:
         the host and the call does not synchronise.  Column slices of the rows: `observation_layout()`."""
         if not self._device_task:
             raise RuntimeError('step_device needs device_task=True')
-        import torch
-        cai = action.__cuda_array_interface__
-        assert tuple(cai['shape']) == (self.n_envs, self._action_spec.shape[0]) and cai['typestr'] == '<f4', cai
-        self._sim.task_step(cai['data'][0], self._n_sub, is_device=True)
+        self._task_step_device(action)
         self._sim.render_eyes_async()
-        self._needs_reset[:] = False
-        if self._dev_views is None:
-            obs_ptr, dim, out_ptr = self._sim.task_ptrs()
-
-            class _View:
-                def __init__(self, ptr, shape):
-                    self.__cuda_array_interface__ = {'shape': shape, 'typestr': '<f4', 'data': (int(ptr), False), 'version': 2}
-            dev = f'cuda:{self._sim.device}'
-            self._dev_views = (torch.as_tensor(_View(obs_ptr, (self.n_envs, dim)), device=dev), torch.as_tensor(_View(out_ptr, (self.n_envs, 4)), device=dev))
-        return self._dev_views + (self.eyes_device(),)
+        return self._device_views() + (self.eyes_device(),)
 
     def observation_layout(self):
         """{observable name: column slice} of the observation rows `step_device` returns (eyes come as their own tensor)"""
-        return {k: sl for k, sl in self._sl.items() if not k.startswith('_')} | {'walker/task_input': self._sl['_task_target']}
-
-    def request_reset(self, env_ids):
-        ids = np.asarray(env_ids, np.int64).reshape(-1)
-        if len(ids) and self._device_task:
-            self._sim.task_request_reset(ids)
-        self._needs_reset[ids] = True
+        sl = self._sl
+        return {k: v for k, v in sl.items() if not k.startswith('_')} | {'walker/task_input': sl['_task_target']}
 
     def hfield_height(self, x, y):
         """`VisionFlightImitationWBPG.get_hfield_height` per env: height at the grid point nearest to (x, y)."""
@@ -302,8 +228,8 @@ class BatchedVisionFlightEnv:
         self._needs_reset[ids] = False
         self.n_resets += n
 
-    def _observation(self):
-        rec, sl, N = self._rec, self._sl, self.n_envs
+    def _observation(self, rec):
+        sl, N = self._sl, self.n_envs
         eyes = self._sim.render_eyes(self._eyes_host)
         obs = collections.OrderedDict()
         for k in self._OBS:
@@ -323,21 +249,18 @@ class BatchedVisionFlightEnv:
     def reset(self):
         N = self.n_envs
         if self._device_task:
-            self._sim.task_reset_all()
-            self._needs_reset[:] = True
-            ts = self._device_step(np.zeros((N, self._action_spec.shape[0]), np.float32), draws=getattr(self, '_forced_draws', None))
-            return self._unbatch(ts, first=True)
+            return self._device_reset()
         self._reset_envs(np.arange(N), hold=False)
         self._sim.task_inputs(np.zeros(N, np.int32), np.ones(N, np.uint8))
-        self._sim.read_task_obs(self._rec)
-        return self._unbatch(TimeStep(np.full(N, StepType.FIRST), np.zeros(N), np.ones(N), self._observation()), first=True)
+        obs = self._observation(self._sim.read_task_obs(self._rec))
+        return self._unbatch(TimeStep(np.full(N, StepType.FIRST), np.zeros(N), np.ones(N), obs), first=True)
 
     def step(self, action):
         m, N = self.model, self.n_envs
         if self._device_task:
             a = np.asarray(action, np.float32).reshape(N, -1)
             assert a.shape[1] == self._action_spec.shape[0], f'action must have {self._action_spec.shape[0]} entries'
-            return self._unbatch(self._device_step(a, draws=getattr(self, '_forced_draws', None)))
+            return self._unbatch(self._device_step(a))
         action = np.array(action, np.float64, copy=True).reshape(N, -1)
         assert action.shape[1] == self._action_spec.shape[0], f'action must have {self._action_spec.shape[0]} entries'
         resetting = self._needs_reset.copy()
@@ -356,20 +279,16 @@ class BatchedVisionFlightEnv:
         rec = self._sim.read_task_obs(self._rec)
         self._time = np.where(resetting, 0.0, self._time + self._control_timestep)
         self._wing_qpos = rec[:, self._sl['walker/joints_pos']][:, self._wing_in_obs].astype(np.float64)
-        obs = self._observation()
+        obs = self._observation(rec)
+        step_type, reward, discount, self._needs_reset = self._task_after(rec, obs, resetting, self._time, None)
+        return self._unbatch(TimeStep(step_type, reward, discount, obs))
+
+    def _task_after(self, rec, obs, resetting, time, ghost):
+        """get_reward (vision_flight.py:157-233), check_termination (a bad state, base.py:222-225, or a fatal floor contact), get_discount;
+        the device task FB_TASK_VISION is the same logic"""
         reward = np.prod(self.reward_factors(rec), axis=1)
-        scal = rec[:, self._sl['_scalars']]
-        # FB_FLAGS bit 0 = non-finite / diverged state (reference base.py:222-225 terminates on it); bits 1, 2 = contact /
-        # constraint-row capacity overflows, which are counted, not treated as bad physics
-        flags = scal[:, 0].astype(np.int64)
-        self.n_capacity_overflows += int(((flags & 6) != 0).sum())
-        bad = ((flags & 1) != 0) | ~(np.sqrt(scal[:, 1].astype(np.float64)) <= _TERMINAL_QACC)
-        terminate = bad | (self.floor_contact() if self._fatal else False)
-        discount = np.where(terminate, 0.0, 1.0)                      # base.py:208-212
-        last = terminate | (self._time >= self._time_limit - 1e-9)
-        step_type = np.where(resetting, StepType.FIRST, np.where(last, StepType.LAST, StepType.MID))
-        self._needs_reset = last & ~resetting
-        return self._unbatch(TimeStep(step_type, np.where(resetting, 0.0, reward), np.where(resetting, 1.0, discount), obs))
+        terminate = self._bad_state(rec) | (self.floor_contact() if self._fatal else False)
+        return self._end_step(resetting, terminate, reward, time)
 
     # -------------------------------------------------------------------------- task quantities
     def floor_contact(self):
@@ -397,14 +316,3 @@ class BatchedVisionFlightEnv:
                 yc = spec['y_coords'][np.abs(spec['x_coords'] - pose[e, 0]).argmin()]
                 centre[e] = _tolerance_linear(pose[e, 1], yc, yc, 0.15)
         return np.stack([height, x_speed, speed, side, world_zaxis, centre], 1)
-
-    def _unbatch(self, ts, first=False):
-        if self._batched:
-            return ts
-        obs = collections.OrderedDict((k, v[0]) for k, v in ts.observation.items())
-        if first or ts.step_type[0] == StepType.FIRST:
-            return TimeStep(StepType.FIRST, None, None, obs)
-        return TimeStep(StepType(int(ts.step_type[0])), float(ts.reward[0]), float(ts.discount[0]), obs)
-
-    def close(self):
-        self._sim.close()

@@ -265,7 +265,7 @@ enum FbObsItem {
   FB_OBS_SUBTREE_COM = 11,/* a = body id : physics.data.subtree_com[body]                                    */
   FB_OBS_DOF_AXIS_EGO = 12,/* a = offset into list (dof ids), b = count : world joint axis (physics.bind(joints).xaxis,
                               tasks/rewards.py:48-50) rotated into the root frame                                */
-  FB_OBS_TASK_TARGET = 14,   /* b floats of the device task's per-episode targets (kind 2: target height, target speed = the reference's
+  FB_OBS_TASK_TARGET = 14,   /* b floats of the device task's per-episode targets (FB_TASK_VISION: target height, target speed = the reference's
                                `task_input` observable, tasks/vision_flight.py:56-76)                                     */
   FB_OBS_WORLD_CONTACT = 13 /* 1 float: 1 if an active contact (efc_address >= 0) involves a geom of the world body (ground plane, terrain):
                                the reference's check_floor_contact (tasks/vision_flight.py:235-247)                        */
@@ -301,15 +301,20 @@ int fb_read_obs(FbHandle h, float* host_dst);
  * check_termination / get_reward / get_discount (tasks/base.py:203-225, walk_imitation.py:179-203,
  * flight_imitation.py:170-226) -- evaluated on the device, so that a control step needs no host round trip: actions in
  * (host or device pointer), observation rows + (reward, discount, step_type) out.  Covers the shared-reference (inference-mode)
- * tasks and walk_imitation / flight_imitation with a trajectory dataset (kind 0 / 1 with ref_bank = 1: fb_ref_slots, then
+ * tasks and walk_imitation / flight_imitation with a trajectory dataset (FB_TASK_WALK / FB_TASK_FLIGHT with ref_bank = 1: fb_ref_slots, then
  * fb_ref_bank_wide / fb_ref_bank, then this program; every env draws its own trajectory (and, flight, start step) of the bank at
  * each reset).  Requires fb_set_action_map and fb_obs_program first.                                                 */
+enum FbTaskKind {
+  FB_TASK_WALK = 0,       /* walk_imitation */
+  FB_TASK_FLIGHT = 1,     /* flight_imitation */
+  FB_TASK_VISION = 2,     /* vision_guided_flight (fields at the end of FbTaskProgram) */
+  FB_TASK_TEMPLATE = 3,   /* template_task (tasks/template_task.py): reset to reset_qpos at rest, no ghost / reference / before_step
+                             hook; reward 1, LAST with discount 0 on a bad state or |qacc| > terminal_qacc, LAST with discount 1 at
+                             time_limit (ghost_qadr = user_col = -1, no noise) */
+  FB_TASK_BALL = 4        /* walk_on_ball (fields at the end of FbTaskProgram; FB_TASK_TEMPLATE's reset and hooks, its own reward) */
+};
 typedef struct FbTaskProgram {
-  int32_t kind;                        /* 0 walk_imitation, 1 flight_imitation, 2 vision_guided_flight (fields at the end of the struct),
-                                          3 template_task (tasks/template_task.py): reset to reset_qpos at rest, no ghost / reference /
-                                          before_step hook; reward 1, LAST with discount 0 on a bad state or |qacc| > terminal_qacc,
-                                          LAST with discount 1 at time_limit (ghost_qadr = user_col = -1, no noise),
-                                          4 walk_on_ball (fields at the end of the struct; kind 3's reset and hooks, its own reward) */
+  int32_t kind;                        /* enum FbTaskKind */
   int32_t root_qadr, root_vadr, ghost_qadr, ghost_vadr;   /* free-joint slots of the walker root and of the ghost (-1: none) */
   int32_t user_col;                    /* column of the beat-frequency action in the action row, -1 if none */
   float ghost_offset[3];
@@ -328,7 +333,7 @@ typedef struct FbTaskProgram {
   const float* wb_freqs /* [n_freq] */; const int32_t* wb_len /* [n_freq] */;
   float wb_base_freq, wb_rel_range, wb_rate;
   float com_offset[3];                 /* root -> CoM offset in the root frame (tasks/task_utils.py:237) */
-  /* kind 2, vision_guided_flight (tasks/vision_flight.py:97-254): no ghost / reference; per episode a target height and speed, a start
+  /* FB_TASK_VISION, vision_guided_flight (tasks/vision_flight.py:97-254): no ghost / reference; per episode a target height and speed, a start
    * point, a wing-beat phase and a terrain of the device bank (fb_hfield_bank) are drawn; reward = product of the height / forward speed /
    * speed / side speed / body axis factors and, for 'trench' arenas, the distance to the corridor's centre line (vision_flight.py:214-226:
    * y of the centre line at trench_len[k] equally spaced x in [trench_x[k][0], trench_x[k][1]] for bank terrain k);
@@ -338,7 +343,7 @@ typedef struct FbTaskProgram {
   int32_t floor_contacts_fatal;
   int32_t trench_cap;                  /* 0: no centre-line factor; else the row stride of trench_y */
   const float* trench_x /* [n_terrain][2] first / last x */; const int32_t* trench_len /* [n_terrain] samples */; const float* trench_y /* [n_terrain][trench_cap] */;
-  /* kind 1 with a trajectory dataset (tasks/flight_imitation.py:88-111, trajectory_loaders.py:67-141).  ref_bank = 1: per-env
+  /* FB_TASK_FLIGHT with a trajectory dataset (tasks/flight_imitation.py:88-111, trajectory_loaders.py:67-141).  ref_bank = 1: per-env
    * references from the bank of fb_ref_bank, written into the env's fb_ref_slots table at each reset (ref_qpos / ref_qvel /
    * episode_steps are then unused).  A reset takes the pick pinned by fb_task_ref_pick, else draws from the counter hash: the
    * trajectory uniformly over pick_traj (repeats allowed), the start step uniformly in [0, len - start_margin) if
@@ -349,7 +354,7 @@ typedef struct FbTaskProgram {
   int32_t randomize_start, start_margin;
   int32_t max_episode_rows;            /* flight: round(time_limit / control_timestep); walking: max_episode_steps + future_steps + 1 */
   int32_t future_steps;
-  /* kind 0 with a trajectory dataset (tasks/walk_imitation.py:93-177): ref_bank = 1 with a bank of fb_ref_bank_wide whose rows are
+  /* FB_TASK_WALK with a trajectory dataset (tasks/walk_imitation.py:93-177): ref_bank = 1 with a bank of fb_ref_bank_wide whose rows are
    * 15 + 6 n_mocap_joints + 3 n_mocap_sites wide; randomize_start = 0 (every snippet starts at row 0).  A reset puts the root and
    * ghost on row 0 (root x, y shifted to the origin), the mocap joints at the snippet's row-0 qpos, the wings back at wing_spring,
    * then adds the noise.  The reward is the product of the four DeepMimic factors
@@ -361,19 +366,19 @@ typedef struct FbTaskProgram {
   int32_t obs_root_pose_off, obs_root_qvel_off, obs_mocap_qpos_off, obs_mocap_qvel_off, obs_mocap_axes_off, obs_mocap_sites_off, obs_wing_qpos_off;
   const float* wing_spring;            /* [n_wing] */
   float deep_mimic_std[4], deep_mimic_weight[4], retract_margin;
-  /* kind 4, walk_on_ball (tasks/walk_on_ball.py:55-81): the reset is kind 3's (reset_qpos at rest); the reward is the product over
+  /* FB_TASK_BALL, walk_on_ball (tasks/walk_on_ball.py:55-81): the reset is FB_TASK_TEMPLATE's (reset_qpos at rest); the reward is the product over
    * i < 3 of max(0, 1 - |qvel[ball_vadr + i] - ball_target[i]| / ball_margin); an episode ends with discount 0 when |velocimeter| >
    * terminal_linvel, |gyro| > terminal_angvel or the state is bad, and with discount 1 at the time limit.  */
   int32_t ball_vadr; float ball_target[3], ball_margin;
 } FbTaskProgram;
 int fb_task_program(FbHandle h, const FbTaskProgram* p);
-/* Flight trajectory bank for kind 1 with ref_bank: n_traj trajectories, rows [sum(traj_len)][15] fp32, trajectory k after
+/* Flight trajectory bank for FB_TASK_FLIGHT with ref_bank: n_traj trajectories, rows [sum(traj_len)][15] fp32, trajectory k after
  * trajectory k - 1: root qpos (7; the dataset's CoM pose through com2root), CoM qvel (6), CoM x, y (2).  A reset at start step s
  * shifts the root x, y of its rows by the CoM x, y of row s (every episode starts above the origin, trajectory_loaders.py:120).
  * Uploaded once; calling it again replaces the bank and drops a task program that points at it.  = fb_ref_bank_wide(.., 15, ..) */
 int fb_ref_bank(FbHandle h, int n_traj, const int32_t* traj_len, const float* rows);
 /* Trajectory bank with rows of row_width >= 15 floats; the first 15 columns keep their flight meaning (columns 13, 14: the x, y a
- * reset at that row shifts the root x, y by).  Walking (kind 0): root qpos 7, root qvel 6, root x, y 2, then mocap qpos [nj],
+ * reset at that row shifts the root x, y by).  Walking (FB_TASK_WALK): root qpos 7, root qvel 6, root x, y 2, then mocap qpos [nj],
  * mocap qvel [nj], root2site [ns][3], joint_quat [nj][4] of the dataset (trajectory_loaders.py:146-156).  At most 2^31 - 1 rows in
  * all; a bank larger than the device's free memory is refused (-4) with an fb_last_error message.                      */
 int fb_ref_bank_wide(FbHandle h, int n_traj, const int32_t* traj_len, int row_width, const float* rows);
@@ -399,8 +404,8 @@ int fb_task_episodes(FbHandle h, int32_t* dst);
 /* Terrain bank for the device-side vision task: K heightfields [K][nrow * ncol] (world units, the grid of fb_hfield_collision /
  * fb_eye_program); a resetting env copies one of them into its own heightfield (collision + eyes).                      */
 int fb_hfield_bank(FbHandle h, int n_terrain, const float* heights);
-/* Rows of 8 uniform numbers in [0,1) consumed by the listed envs' next reset instead of the device's counter hash (kind 2: target
- * height, target speed, start x, start y, wing-beat phase, terrain pick; kind 1: wing-beat phase) -- lets a test feed the device the
+/* Rows of 8 uniform numbers in [0,1) consumed by the listed envs' next reset instead of the device's counter hash (FB_TASK_VISION:
+ * target height, target speed, start x, start y, wing-beat phase, terrain pick; FB_TASK_FLIGHT: wing-beat phase) -- lets a test feed the device the
  * draws of the host-side task code.                                                                                    */
 int fb_task_uniform_rows(FbHandle h, const int32_t* env_ids, int n, const float* u);
 /* Uniform numbers in [0,1) consumed by the listed envs' next reset (flight: wing-beat phase); without them the device
