@@ -13,15 +13,12 @@
 #define FB_ZCAP 24      // longest dof chain a row may have (fly: 20)
 #define FB_JROW (2 * FB_ZCAP)
 #define EJC(arr, r, slot) AT(arr, (r) * FB_JROW + (slot))
-#define EA(arr, r, c) AT(arr, (r) * FB_MAXEFC + (c))
-#define EW(slot, r) AT(d.efc_w, (slot) * FB_MAXEFC + (r))
 
 // ---------------------------------------------------------------------------------------------
-// K9 collision: blockDim = (32 envs, nchunk).  Each thread scans a contiguous chunk of the
-// candidate pair list (bounding-sphere broadphase, then the analytic narrowphase) into a private
-// staging area; a prefix sum over the chunk counts makes the final contact order deterministic
-// (pair-list order), which the Gauss-Seidel noslip sweeps depend on.
-struct ShCol { int cnt[FB_MAXCHUNK][FB_LANES]; int njobs, slice; /* MPR jobs of this env; byte stride between the warps' slices (GPU) */ };
+// K9 collision: one warp per env.  A bounding-sphere broadphase over the static pair list, then the analytic narrowphase
+// one candidate per lane (kcol_broad .. kcol_compact below); the contacts come out in pair-list order, which the Gauss-Seidel
+// noslip sweeps depend on.
+struct ShCol { int cnt; int njobs, slice; /* candidates of this env; MPR jobs of this env; byte stride between the warps' slices (GPU) */ };
 struct RawCon { float dist; V3 pos, n, t; };
 
 FB_DEV int raw_sphere_sphere(RawCon* c, float margin, V3 p1, float r1, V3 p2, float r2) {
@@ -123,89 +120,74 @@ static long g_convex_stats[4];     // host emulation only: generic candidates, p
 #else
 #define CONVEX_STAT(i)
 #endif
-// Scalar type of MPR.  libccd's zero tests compare against an ABSOLUTE machine epsilon, which in double (1e-16) is far below
+// MPR runs in single precision.  libccd's zero tests compare against an ABSOLUTE machine epsilon, which in double (1e-16) is far below
 // any geometric quantity but in single precision (1e-7) is not: with centimetre-scale geometry |v0 x v1|^2 ~ 1e-7 sin^2 and
 // the portal discovery mis-classifies ordinary configurations as degenerate (6 % of shallow contacts came out 10x too deep).
-// The fp32 variant therefore keeps the RELATIVE comparisons at FLT_EPSILON and makes the absolute zero test scale-free
+// The fp32 code therefore keeps the RELATIVE comparisons at FLT_EPSILON and makes the absolute zero test scale-free
 // (1e-30); with that it agrees with the fp64 oracle as often as a double-precision copy fed with the same fp32 inputs does
-// (tests/test_emu_parity.py).  -DFB_MPR_DOUBLE selects double (3x slower: the FP64 pipe is narrow).
-#ifndef FB_MPR_DOUBLE
-typedef float mreal;
+// (tests/test_emu_parity.py).  MPR in double was 3x slower on the GPU (the FP64 pipe is narrow).
 #define MPR_EPS 1.1920929e-7f
 #define MPR_ZERO 1e-30f
-#define MSQRT(x) sqrtf(x)
-#define MFABS(x) fabsf(x)
-#define MFMIN(a, b) fminf(a, b)
-#else
-typedef double mreal;
-#define MPR_EPS 2.220446049250313e-16
-#define MPR_ZERO 2.220446049250313e-16
-#define MSQRT(x) sqrt(x)
-#define MFABS(x) fabs(x)
-#define MFMIN(a, b) fmin(a, b)
-#endif
-struct D3 { mreal x, y, z; };
-FB_DEV D3 d3(mreal x, mreal y, mreal z) { D3 r; r.x = x; r.y = y; r.z = z; return r; }
+struct D3 { float x, y, z; };
+FB_DEV D3 d3(float x, float y, float z) { D3 r; r.x = x; r.y = y; r.z = z; return r; }
 FB_DEV D3 operator+(D3 a, D3 b) { return d3(a.x + b.x, a.y + b.y, a.z + b.z); }
 FB_DEV D3 operator-(D3 a, D3 b) { return d3(a.x - b.x, a.y - b.y, a.z - b.z); }
-FB_DEV D3 operator*(D3 a, mreal s) { return d3(a.x * s, a.y * s, a.z * s); }
-FB_DEV mreal ddot(D3 a, D3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+FB_DEV D3 operator*(D3 a, float s) { return d3(a.x * s, a.y * s, a.z * s); }
+FB_DEV float ddot(D3 a, D3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 FB_DEV D3 dcross(D3 a, D3 b) { return d3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x); }
-FB_DEV mreal dnorm(D3 a) { return MSQRT(ddot(a, a)); }
-// 1/MSQRT(x) and 1/x to ~1e-15: single-precision seed + two Newton steps in mreal (the mreal-precision sqrt / divide of the
-// GPU are long software sequences; these sit in the inner loop of MPR)
-#if defined(__CUDACC__) && !defined(FB_MPR_DOUBLE)
-// fp32: hardware reciprocal square root + two Newton steps (full single precision without the IEEE sqrt and divide sequences)
-FB_DEV mreal fast_rsqrt(mreal x) { float y = rsqrtf(x); y = y * (1.5f - 0.5f * x * y * y); return y * (1.5f - 0.5f * x * y * y); }
+FB_DEV float dnorm(D3 a) { return sqrtf(ddot(a, a)); }
+// 1/sqrtf(x): a single-precision seed + two Newton steps (full single precision without the IEEE sqrt and divide sequences; this
+// sits in the inner loop of MPR).  GPU: the hardware reciprocal square root as the seed
+#ifdef __CUDACC__
+FB_DEV float fast_rsqrt(float x) { float y = rsqrtf(x); y = y * (1.5f - 0.5f * x * y * y); return y * (1.5f - 0.5f * x * y * y); }
 #else
-FB_DEV mreal fast_rsqrt(mreal x) { mreal y = (mreal)(1.0f / sqrtf((float)x)); y = y * ((mreal)1.5 - (mreal)0.5 * x * y * y); return y * ((mreal)1.5 - (mreal)0.5 * x * y * y); }
+FB_DEV float fast_rsqrt(float x) { float y = (float)(1.0f / sqrtf((float)x)); y = y * ((float)1.5 - (float)0.5 * x * y * y); return y * ((float)1.5 - (float)0.5 * x * y * y); }
 #endif
-FB_DEV mreal fast_rcp(mreal x) { mreal y = (mreal)(1.0f / (float)x); y = y * ((mreal)2.0 - x * y); return y * ((mreal)2.0 - x * y); }
-FB_DEV D3 dnormalized(D3 a) { mreal n2 = ddot(a, a); if (n2 < 1e-36) { mreal n = MSQRT(n2); if (n < 1e-300) return d3(1, 0, 0); return a * (1.0 / n); } return a * fast_rsqrt(n2); }
+FB_DEV D3 dnormalized(D3 a) { float n2 = ddot(a, a); if (n2 < 1e-36) { float n = sqrtf(n2); if (n < 1e-300) return d3(1, 0, 0); return a * (1.0 / n); } return a * fast_rsqrt(n2); }
 FB_DEV D3 dsel(bool c, D3 a, D3 b) { return d3(c ? a.x : b.x, c ? a.y : b.y, c ? a.z : b.z); }
 struct MprPt { D3 v, v1, v2; };
 // e / zoff: per-type coefficients of the branch-free support function below (set by mpr_obj_coefs)
-struct MprObj { D3 pos; mreal mat[9]; D3 size; int type; mreal margin; D3 e; mreal zoff; bool round; };
+struct MprObj { D3 pos; float mat[9]; D3 size; int type; float margin; D3 e; float zoff; bool round; };
 FB_DEV void mpr_obj_coefs(MprObj& o) {
   const bool round = o.type == FB_GEOM_SPHERE || o.type == FB_GEOM_CAPSULE, cyl = o.type == FB_GEOM_CYLINDER;
   o.round = round;
   o.e = (round || cyl) ? d3(o.size.x, o.size.x, cyl ? 0 : o.size.x) : o.size;
   o.zoff = (o.type == FB_GEOM_CAPSULE || cyl) ? o.size.y : 0;
 }
-FB_DEV bool mpr_zero(mreal x) { return MFABS(x) < MPR_ZERO; }
-FB_DEV bool mpr_eq(mreal a, mreal b) { mreal ab = MFABS(a - b); if (ab < MPR_ZERO) return true; a = MFABS(a); b = MFABS(b); return (b > a) ? ab < MPR_EPS * b : ab < MPR_EPS * a; }
-FB_DEV mreal mpr_sgn(mreal x) { return x > 0 ? 1.0 : (x < 0 ? -1.0 : 0.0); }
+FB_DEV bool mpr_zero(float x) { return fabsf(x) < MPR_ZERO; }
+FB_DEV bool mpr_eq(float a, float b) { float ab = fabsf(a - b); if (ab < MPR_ZERO) return true; a = fabsf(a); b = fabsf(b); return (b > a) ? ab < MPR_EPS * b : ab < MPR_EPS * a; }
+FB_DEV float mpr_sgn(float x) { return x > 0 ? 1.0 : (x < 0 ? -1.0 : 0.0); }
 // mjccd_support for sphere / capsule / ellipsoid / cylinder as ONE expression: in the geom frame the support point is
 //   e (.) normalize(e (.) d) + sgn(d_z) zoff e_z        e = (r, r, r) sphere, capsule; semi-axes ellipsoid; (r, r, 0) cylinder
 // (a sphere is an ellipsoid with equal axes, a capsule a sphere swept by +-zoff, a cylinder a disc swept by +-zoff).  The MPR
 // jobs of a warp's lanes are different geom pairs: with a switch over the type every lane pays for every type present.
 FB_DEV D3 mpr_support1(const MprObj& o, D3 dir) {
-  const mreal* R = o.mat;
+  const float* R = o.mat;
   D3 ld = d3(R[0] * dir.x + R[3] * dir.y + R[6] * dir.z, R[1] * dir.x + R[4] * dir.y + R[7] * dir.z, R[2] * dir.x + R[5] * dir.y + R[8] * dir.z);
   D3 t = d3(ld.x * o.e.x, ld.y * o.e.y, ld.z * o.e.z);
-  mreal n2 = ddot(t, t), in = n2 >= (mreal)1e-30 ? fast_rsqrt(n2) : (mreal)0;
+  float n2 = ddot(t, t), in = n2 >= (float)1e-30 ? fast_rsqrt(n2) : (float)0;
   D3 r = d3(t.x * in * o.e.x, t.y * in * o.e.y, t.z * in * o.e.z);
   r = dsel(o.round, ld * o.e.x, r);                 // spheres / capsule caps: radius * d exactly (no normalisation of the unit d)
   r.z += mpr_sgn(ld.z) * o.zoff;
-  r = r + ld * ((mreal)0.5 * o.margin);
+  r = r + ld * ((float)0.5 * o.margin);
   return d3(R[0] * r.x + R[1] * r.y + R[2] * r.z, R[3] * r.x + R[4] * r.y + R[5] * r.z, R[6] * r.x + R[7] * r.y + R[8] * r.z) + o.pos;
 }
 FB_DEV MprPt mpr_support(const MprObj& a, const MprObj& b, D3 dir) { MprPt p;
   CONVEX_STAT(3);
  p.v1 = mpr_support1(a, dir); p.v2 = mpr_support1(b, d3(0, 0, 0) - dir); p.v = p.v1 - p.v2; return p; }
-FB_DEV mreal mpr_seg_dist2(D3 P, D3 x0, D3 b, D3& w) {
-  D3 dd = b - x0, a = x0 - P; mreal t = -ddot(a, dd) / ddot(dd, dd);
+FB_DEV float mpr_seg_dist2(D3 P, D3 x0, D3 b, D3& w) {
+  D3 dd = b - x0, a = x0 - P; float t = -ddot(a, dd) / ddot(dd, dd);
   if (t < 0 || mpr_zero(t)) w = x0; else if (t > 1 || mpr_eq(t, 1)) w = b; else w = x0 + dd * t;
   D3 ee = w - P; return ddot(ee, ee);
 }
-FB_DEV mreal mpr_tri_dist2(D3 P, D3 x0, D3 B, D3 C, D3& w) {
+FB_DEV float mpr_tri_dist2(D3 P, D3 x0, D3 B, D3 C, D3& w) {
   D3 d1 = B - x0, d2 = C - x0, a = x0 - P;
-  mreal v = ddot(d1, d1), ww = ddot(d2, d2), pp = ddot(a, d1), q = ddot(a, d2), r = ddot(d1, d2);
-  mreal s = (q * r - ww * pp) / (ww * v - r * r), t = (-s * r - q) / ww;
+  float v = ddot(d1, d1), ww = ddot(d2, d2), pp = ddot(a, d1), q = ddot(a, d2), r = ddot(d1, d2);
+  float s = (q * r - ww * pp) / (ww * v - r * r), t = (-s * r - q) / ww;
   if ((mpr_zero(s) || s > 0) && (mpr_eq(s, 1) || s < 1) && (mpr_zero(t) || t > 0) && (mpr_eq(t, 1) || t < 1) && (mpr_eq(t + s, 1) || t + s < 1)) {
     w = x0 + d1 * s + d2 * t; D3 ee = w - P; return ddot(ee, ee);
   }
-  D3 w2; mreal dist = mpr_seg_dist2(P, x0, B, w), dd = mpr_seg_dist2(P, x0, C, w2);
+  D3 w2; float dist = mpr_seg_dist2(P, x0, B, w), dd = mpr_seg_dist2(P, x0, C, w2);
   if (dd < dist) { dist = dd; w = w2; }
   dd = mpr_seg_dist2(P, B, C, w2);
   if (dd < dist) { dist = dd; w = w2; }
@@ -215,15 +197,15 @@ FB_DEV mreal mpr_tri_dist2(D3 P, D3 x0, D3 B, D3 C, D3& w) {
 // vertex i (the second's is p1[i] - v_i; only read for the contact position at the very end, so it may sit in local memory).
 // Vertex replacement is a chain of selects, not a branch per case: the lanes of a warp refine different pairs.
 FB_DEV D3 mpr_portal_dir3(D3 v1, D3 v2, D3 v3) { return dnormalized(dcross(v2 - v1, v3 - v1)); }
-FB_DEV bool mpr_reach_tol3(D3 v1, D3 v2, D3 v3, D3 v4, D3 dir, mreal tol) {
-  mreal dv4 = ddot(v4, dir), dmin = MFMIN(dv4 - ddot(v1, dir), MFMIN(dv4 - ddot(v2, dir), dv4 - ddot(v3, dir)));
+FB_DEV bool mpr_reach_tol3(D3 v1, D3 v2, D3 v3, D3 v4, D3 dir, float tol) {
+  float dv4 = ddot(v4, dir), dmin = fminf(dv4 - ddot(v1, dir), fminf(dv4 - ddot(v2, dir), dv4 - ddot(v3, dir)));
   return mpr_eq(dmin, tol) || dmin < tol;
 }
 #define MPR_EXPAND() { D3 v4v0 = dcross(n.v, v0); const bool c1 = ddot(v1, v4v0) > 0, c2 = ddot(v2, v4v0) > 0, c3 = ddot(v3, v4v0) > 0; \
     const int k = c1 ? (c2 ? 1 : 3) : (c3 ? 2 : 1); v1 = dsel(k == 1, n.v, v1); v2 = dsel(k == 2, n.v, v2); v3 = dsel(k == 3, n.v, v3); p1[k] = n.v1; }
 // 0 and depth / dir / pos when the inflated shapes intersect, -1 otherwise
-FB_DEVN int mpr_penetration(const MprObj& o1, const MprObj& o2, mreal tol, int max_iter, mreal& depth, D3& pdir, D3& pos) {
-  D3 p1[4], v0, v1, v2, v3, dir; mreal dt; MprPt n;
+FB_DEVN int mpr_penetration(const MprObj& o1, const MprObj& o2, float tol, int max_iter, float& depth, D3& pdir, D3& pos) {
+  D3 p1[4], v0, v1, v2, v3, dir; float dt; MprPt n;
   v2 = v3 = d3(0, 0, 0); p1[2] = p1[3] = d3(0, 0, 0);
   p1[0] = o1.pos; v0 = o1.pos - o2.pos;
   if (mpr_eq(v0.x, 0) && mpr_eq(v0.y, 0) && mpr_eq(v0.z, 0)) v0 = d3(MPR_EPS * 10, 0, 0);
@@ -268,17 +250,17 @@ FB_DEVN int mpr_penetration(const MprObj& o1, const MprObj& o2, mreal tol, int m
     dir = mpr_portal_dir3(v1, v2, v3);
     n = mpr_support(o1, o2, dir);
     if (mpr_reach_tol3(v1, v2, v3, n.v, dir, tol) || it > max_iter) {
-      depth = MSQRT(mpr_tri_dist2(d3(0, 0, 0), v1, v2, v3, pdir));
+      depth = sqrtf(mpr_tri_dist2(d3(0, 0, 0), v1, v2, v3, pdir));
       if (mpr_zero(pdir.x) && mpr_zero(pdir.y) && mpr_zero(pdir.z)) pdir = dir;
       pdir = dnormalized(pdir);
-      mreal b0 = ddot(dcross(v1, v2), v3), b1 = ddot(dcross(v3, v2), v0);
-      mreal b2 = ddot(dcross(v0, v1), v3), b3 = ddot(dcross(v2, v1), v0);
-      mreal sum = b0 + b1 + b2 + b3;
+      float b0 = ddot(dcross(v1, v2), v3), b1 = ddot(dcross(v3, v2), v0);
+      float b2 = ddot(dcross(v0, v1), v3), b3 = ddot(dcross(v2, v1), v0);
+      float sum = b0 + b1 + b2 + b3;
       if (mpr_zero(sum) || sum < 0) {
         b0 = 0; b1 = ddot(dcross(v2, v3), dir); b2 = ddot(dcross(v3, v1), dir); b3 = ddot(dcross(v1, v2), dir);
         sum = b1 + b2 + b3;
       }
-      mreal inv = 0.5 / sum;
+      float inv = 0.5 / sum;
       // sum_i b_i (first_i + second_i): vertex 0 = the two centres, vertices 1..3 second_i = first_i - v_i
       pos = ((o1.pos + o2.pos) * b0 + (p1[1] + p1[1] - v1) * b1 + (p1[2] + p1[2] - v2) * b2 + (p1[3] + p1[3] - v3) * b3) * inv;
       return 0;
@@ -360,8 +342,8 @@ FB_DEV int convex_mpr(RawCon* c, float margin, int t1, V3 p1, const M3& m1, V3 s
   b.pos = d3(p2.x - mid.x, p2.y - mid.y, p2.z - mid.z); b.size = d3(s2.x, s2.y, s2.z); b.type = t2; b.margin = margin;
   for (int k = 0; k < 9; k++) { a.mat[k] = m1.m[k]; b.mat[k] = m2.m[k]; }
   mpr_obj_coefs(a); mpr_obj_coefs(b);
-  mreal depth; D3 dir, pos;
-  if (mpr_penetration(a, b, (mreal)1e-6, 50, depth, dir, pos) != 0) return 0;
+  float depth; D3 dir, pos;
+  if (mpr_penetration(a, b, (float)1e-6, 50, depth, dir, pos) != 0) return 0;
   if (mpr_eq(dir.x, 0) && mpr_eq(dir.y, 0) && mpr_eq(dir.z, 0)) return 0;
   CONVEX_STAT(2);
   c->dist = (float)(margin - depth); c->pos = v3((float)pos.x, (float)pos.y, (float)pos.z) + mid; c->n = v3((float)dir.x, (float)dir.y, (float)dir.z); c->t = v3(0, 0, 0);
@@ -379,24 +361,22 @@ FB_DEV void make_frame(V3 n, V3 t, V3& f1, V3& f2) {   // mju_makeFrame
   f1 = t; f2 = cross(n, t);
 }
 
-#define FB_COL_ARGS const DevModel& m, const DevData& d, ShCol& sh, int e, int lane, int y
+#define FB_COL_ARGS const DevModel& m, const DevData& d, ShCol& sh, int e, int y
 // geom positions of this env into shared memory (coalesced), so that the pair loop does not touch the record
 FB_DEV void kcol_stage(FB_COL_ARGS) {
-  float* gx = sh_dyn(sh); float* gn = gx + 3 * m.ngeom * FB_LANES;      // positions; normals (z axes) of the plane geoms
+  float* gx = sh_dyn(sh); float* gn = gx + 3 * m.ngeom;      // positions; normals (z axes) of the plane geoms
   for (int g = y; g < m.ngeom; g += FB_NY) {
-    V3 p = ld3(d.geom_xpos, g, d, e); gx[(3 * g) * FB_LANES + lane] = p.x; gx[(3 * g + 1) * FB_LANES + lane] = p.y; gx[(3 * g + 2) * FB_LANES + lane] = p.z;
-    if (m.geom_type[g] == FB_GEOM_PLANE) for (int c = 0; c < 3; c++) gn[(3 * g + c) * FB_LANES + lane] = AT(d.geom_xmat, FB_M3S * g + 3 * c + 2);
+    V3 p = ld3(d.geom_xpos, g, d, e); gx[3 * g] = p.x; gx[3 * g + 1] = p.y; gx[3 * g + 2] = p.z;
+    if (m.geom_type[g] == FB_GEOM_PLANE) for (int c = 0; c < 3; c++) gn[3 * g + c] = AT(d.geom_xmat, FB_M3S * g + 3 * c + 2);
   }
 }
 // Collision in three converged phases.  Broadphase and narrowphase are separated on purpose: in a fused pair loop the
 // whole warp pays for the narrowphase whenever ANY lane has a candidate in that iteration (68 iterations x ~1300 cycles);
 // here the lanes first only filter their pairs, and the candidates are then narrow-phased one per lane.
 #define FB_MAXCAND 192                 // candidates per env (4 contact slots each in tmp_con)
-#define COL_FLAT(j) flat[(j) * FB_LANES + lane]
-#define COL_NCON(j) ccnt[(j) * FB_LANES + lane]
 #define FB_COL_DYN(m) (6 * (m).ngeom + 3 * FB_MAXCAND)
-#define FB_COL_PTRS float* gx = sh_dyn(sh); float* gn = gx + 3 * m.ngeom * FB_LANES; int* flat = reinterpret_cast<int*>(gn + 3 * m.ngeom * FB_LANES); \
-  int* ccnt = flat + FB_MAXCAND * FB_LANES; [[maybe_unused]] int* jobs = ccnt + FB_MAXCAND * FB_LANES; (void)gx; (void)gn; (void)flat; (void)ccnt;
+#define FB_COL_PTRS float* gx = sh_dyn(sh); float* gn = gx + 3 * m.ngeom; int* flat = reinterpret_cast<int*>(gn + 3 * m.ngeom); \
+  int* ccnt = flat + FB_MAXCAND; [[maybe_unused]] int* jobs = ccnt + FB_MAXCAND; (void)gx; (void)gn; (void)flat; (void)ccnt;
 // 1. broadphase: lane l tests the pairs l, l + 32, ... of the static pair list (packed record: geoms, plane flag; margin +
 // bounding radii -- one coalesced line per step), four steps loaded ahead of the tests.  The hits are ranked with ballots,
 // so the candidate list comes out in pair order without per-lane lists.
@@ -432,7 +412,7 @@ FB_WARPFN void kcol_broad(const DevModel& m, const DevData& d, ShCol& sh, int e)
     } WPAR_END
     base += POPC(m0) + POPC(m1) + POPC(m2) + POPC(m3);
   }
-  WPAR_BEGIN { if (lane == 0) { sh.cnt[0][0] = base > FB_MAXCAND ? FB_MAXCAND : base; if (base > FB_MAXCAND) FB_FLAG_OR(2); } } WPAR_END
+  WPAR_BEGIN { if (lane == 0) { sh.cnt = base > FB_MAXCAND ? FB_MAXCAND : base; if (base > FB_MAXCAND) FB_FLAG_OR(2); } } WPAR_END
 }
 FB_DEV void col_store(const DevModel& m, const DevData& d, int e, int j, const RawCon* rc, int n, int g1, int g2) {
   for (int i = 0; i < n; i++) {
@@ -449,17 +429,16 @@ FB_DEV void col_store(const DevModel& m, const DevData& d, int e, int j, const R
 // 2. narrowphase: one candidate per lane, up to 4 contacts each into tmp_con[4 j + i]
 FB_DEV void kcol_narrow(FB_COL_ARGS) {
   FB_COL_PTRS
-  const int T = sh.cnt[0][lane];
+  const int T = sh.cnt;
   for (int j = y; j < T; j += FB_NY) {
-    const int k = COL_FLAT(j), pw = m.pair_info[k];
+    const int k = flat[j], pw = m.pair_info[k];
     const int g1 = pw & 0x7fff, g2 = (pw >> 15) & 0x7fff; const bool plane = (pw >> 30) & 1;
-    V3 x1 = v3(gx[(3 * g1) * FB_LANES + lane], gx[(3 * g1 + 1) * FB_LANES + lane], gx[(3 * g1 + 2) * FB_LANES + lane]);
-    V3 x2 = v3(gx[(3 * g2) * FB_LANES + lane], gx[(3 * g2 + 1) * FB_LANES + lane], gx[(3 * g2 + 2) * FB_LANES + lane]);
+    V3 x1 = v3(gx[3 * g1], gx[3 * g1 + 1], gx[3 * g1 + 2]), x2 = v3(gx[3 * g2], gx[3 * g2 + 1], gx[3 * g2 + 2]);
     const int t1 = m.geom_type[g1], t2 = m.geom_type[g2];
     const float margin = fmaxf(m.geom_margin[g1], m.geom_margin[g2]);
     RawCon rc[4]; int n = 0;
     if (plane) {
-      V3 pn = v3(gn[(3 * g1) * FB_LANES + lane], gn[(3 * g1 + 1) * FB_LANES + lane], gn[(3 * g1 + 2) * FB_LANES + lane]);
+      V3 pn = v3(gn[3 * g1], gn[3 * g1 + 1], gn[3 * g1 + 2]);
       V3 s2 = mld3(m.geom_size, g2);
       if (t2 == FB_GEOM_SPHERE) n = raw_plane_sphere(rc, margin, x1, pn, x2, s2.x);
       else { M3 R2 = ld9(d.geom_xmat, g2, d, e);
@@ -475,14 +454,14 @@ FB_DEV void kcol_narrow(FB_COL_ARGS) {
         n = convex_prefilter(margin, t1, x1, R1, s1, t2, x2, R2, s2) ? -1 : 0; }
     }
     col_store(m, d, e, j, rc, n, g1, g2);
-    COL_NCON(j) = n;
+    ccnt[j] = n;
   }
 }
 // 2b. the generic pairs that survived the cheap tests, compacted with ballots and run through MPR one per lane: in the
 // candidate loop above a single such pair would stall the other 31 lanes of its round
-FB_WARPFN void kcol_mpr(const DevModel& m, const DevData& d, ShCol& sh, int e) {      // (`lane` is the real lane here: index the lists directly, not through the per-phase macros)
+FB_WARPFN void kcol_mpr(const DevModel& m, const DevData& d, ShCol& sh, int e) {
   LREG(int, pend);
-  const int T = sh.cnt[0][0];
+  const int T = sh.cnt;
   int njobs = 0;
   for (int base = 0; base < T; base += 32) {
     WPAR_BEGIN { FB_COL_PTRS L(pend) = (base + lane < T && ccnt[base + lane] < 0) ? 1 : 0; } WPAR_END
@@ -490,7 +469,7 @@ FB_WARPFN void kcol_mpr(const DevModel& m, const DevData& d, ShCol& sh, int e) {
     WPAR_BEGIN { FB_COL_PTRS if (L(pend)) jobs[njobs + POPC(mk & ((1u << lane) - 1u))] = base + lane; } WPAR_END
     njobs += POPC(mk);
   }
-#if defined(__CUDACC__) && !defined(FB_MPR_PER_WARP)
+#ifdef __CUDACC__
   // The block's envs pool their jobs: an env has ~3 of them, so a warp working on its own list keeps 3 of 32 lanes busy
   // through the longest MPR of the three.  Warp 0 takes the jobs of all FB_WPB envs of the block (one per lane, reading the
   // other warps' lists and geom positions in their shared slices) while the other warps wait at the barrier and leave
@@ -522,8 +501,8 @@ FB_WARPFN void kcol_mpr(const DevModel& m, const DevData& d, ShCol& sh, int e) {
     }
   }
   __syncthreads();
-  return;
-#endif
+#else
+  // host emulation: each env runs its own jobs
   WPAR_BEGIN { FB_COL_PTRS
     for (int q = lane; q < njobs; q += 32) {
       const int j = jobs[q], k = flat[j], pw = m.pair_info[k];
@@ -535,15 +514,16 @@ FB_WARPFN void kcol_mpr(const DevModel& m, const DevData& d, ShCol& sh, int e) {
       col_store(m, d, e, j, rc, n, g1, g2);
       ccnt[j] = n;
     } } WPAR_END
+#endif
 }
 // 3. compaction into the contact list, in candidate order
 FB_DEV void kcol_compact(FB_COL_ARGS) {
   FB_COL_PTRS
-  const int T = sh.cnt[0][lane];
+  const int T = sh.cnt;
   int off = 0, jj = 0;
   for (int j = y; j < T; j += FB_NY) {
-    for (; jj < j; jj++) off += COL_NCON(jj);
-    int cnt = COL_NCON(j);
+    for (; jj < j; jj++) off += ccnt[jj];
+    int cnt = ccnt[j];
     for (int i = 0; i < cnt; i++) {
       int dst = off + i, src = 4 * j + i;
       if (dst >= FB_MAXCON) { FB_FLAG_OR(2); break; }
@@ -553,11 +533,11 @@ FB_DEV void kcol_compact(FB_COL_ARGS) {
       AT(d.con_geom1, dst) = AT(d.tmp_geom, 2 * src); AT(d.con_geom2, dst) = AT(d.tmp_geom, 2 * src + 1);
     }
   }
-  if (y == 0) { int tot = 0; for (int j = 0; j < T; j++) tot += COL_NCON(j); AT(d.ncon, 0) = tot > FB_MAXCON ? FB_MAXCON : tot; }
+  if (y == 0) { int tot = 0; for (int j = 0; j < T; j++) tot += ccnt[j]; AT(d.ncon, 0) = tot > FB_MAXCON ? FB_MAXCON : tot; }
 }
 
 // ---------------------------------------------------------------------------------------------
-// K10 constraint rows (MuJoCo mj_makeConstraint + mj_makeImpedance), lane = env
+// K10 constraint rows (MuJoCo mj_makeConstraint + mj_makeImpedance)
 FB_DEV float impedance(const float* si, float pos, float margin) {
   if (si[0] == si[1] || si[2] <= FB_MINVAL) return 0.5f * (si[0] + si[1]);
   float x = fabsf((pos - margin) / si[2]);
@@ -580,8 +560,8 @@ FB_DEV void row_params(const DevModel& m, const DevData& d, int e, int r, const 
   if (isfric) K = 0;
   EFC(d.efc_R, r) = R; EFC(d.efc_D, r) = 1.0f / R; EFC(d.efc_K, r) = K; EFC(d.efc_B, r) = B; EFC(d.efc_imp, r) = imp;
 }
-struct ShCon { int cnt[FB_ROWPAR][FB_LANES]; int base[FB_LANES]; };
-#define FB_CON_ARGS const DevModel& m, const DevData& d, ShCon& sh, int e, int lane, int y
+struct ShCon { int cnt[FB_ROWPAR]; int base; };
+#define FB_CON_ARGS const DevModel& m, const DevData& d, ShCon& sh, int e, int y
 FB_DEV bool limit_active(const DevModel& m, const DevData& d, int e, int j, int side, float& dist) {
   float value = AT(d.qpos, m.jnt_qposadr[j]);
   dist = side * (m.jnt_range[2 * j + (side + 1) / 2] - value);
@@ -593,11 +573,11 @@ FB_DEV void kcon_p0(FB_CON_ARGS) {
   if (y >= FB_ROWPAR) return;
   int j0 = (int)((long)y * m.njnt / FB_ROWPAR), j1 = (int)((long)(y + 1) * m.njnt / FB_ROWPAR), c = 0; float dist;
   for (int j = j0; j < j1; j++) { if (!m.jnt_limited[j] || m.jnt_type[j] != FB_JNT_HINGE) continue; for (int side = -1; side <= 1; side += 2) c += limit_active(m, d, e, j, side, dist) ? 1 : 0; }
-  sh.cnt[y][lane] = c;
+  sh.cnt[y] = c;
 }
 FB_DEV void kcon_p1(FB_CON_ARGS) {
   if (y >= FB_ROWPAR) return;
-  int n = 0; for (int yy = 0; yy < y; yy++) n += sh.cnt[yy][lane];
+  int n = 0; for (int yy = 0; yy < y; yy++) n += sh.cnt[yy];
   int j0 = (int)((long)y * m.njnt / FB_ROWPAR), j1 = (int)((long)(y + 1) * m.njnt / FB_ROWPAR); float dist;
   for (int j = j0; j < j1; j++) {
     if (!m.jnt_limited[j] || m.jnt_type[j] != FB_JNT_HINGE) continue;
@@ -610,7 +590,7 @@ FB_DEV void kcon_p1(FB_CON_ARGS) {
       }
     }
   }
-  if (y == FB_ROWPAR - 1) sh.base[lane] = n < FB_MAXEFC ? n : FB_MAXEFC;
+  if (y == FB_ROWPAR - 1) sh.base = n < FB_MAXEFC ? n : FB_MAXEFC;
 }
 // contact -> (dim, included)
 FB_DEV int contact_dim(const DevModel& m, const DevData& d, int e, int ci, float& includemargin, bool& incl) {
@@ -626,12 +606,12 @@ FB_DEV void kcon_p2(FB_CON_ARGS) {
   int ncon = AT(d.ncon, 0);
   int c0 = y * ncon / FB_ROWPAR, c1 = (y + 1) * ncon / FB_ROWPAR, rows = 0;
   for (int ci = c0; ci < c1; ci++) { float im; bool incl; int dim = contact_dim(m, d, e, ci, im, incl); if (incl) rows += dim; }
-  sh.cnt[y][lane] = rows;
+  sh.cnt[y] = rows;
 }
 FB_DEV void kcon_p3(FB_CON_ARGS) {
   if (y >= FB_ROWPAR) return;
   int ncon = AT(d.ncon, 0);
-  int n = sh.base[lane]; for (int yy = 0; yy < y; yy++) n += sh.cnt[yy][lane];
+  int n = sh.base; for (int yy = 0; yy < y; yy++) n += sh.cnt[yy];
   int c0 = y * ncon / FB_ROWPAR, c1 = (y + 1) * ncon / FB_ROWPAR;
   for (int ci = c0; ci < c1; ci++) {
     float includemargin; bool incl; int dim = contact_dim(m, d, e, ci, includemargin, incl);
@@ -667,7 +647,7 @@ FB_DEV void kcon_p3(FB_CON_ARGS) {
   if (y == FB_ROWPAR - 1) {
     // rows are contiguous up to the first overflowing contact; later ones were all dropped
     int tot = n;
-    if (tot > FB_MAXEFC) { tot = sh.base[lane]; for (int ci = 0; ci < ncon; ci++) { int a = AT(d.con_efcadr, ci); if (a >= 0 && a + AT(d.con_dim, ci) > tot) tot = a + AT(d.con_dim, ci); } }
+    if (tot > FB_MAXEFC) { tot = sh.base; for (int ci = 0; ci < ncon; ci++) { int a = AT(d.con_efcadr, ci); if (a >= 0 && a + AT(d.con_dim, ci) > tot) tot = a + AT(d.con_dim, ci); } }
     AT(d.nefc, 0) = tot;
   }
 }
@@ -689,7 +669,6 @@ FB_DEV RowChains row_chains(const DevModel& m, const DevData& d, int e, int r, i
   }
   return rc;
 }
-FB_DEV bool in_chain(const DevModel& m, int dof, int last) { return last >= 0 && dof <= last && last <= m.dof_subend[dof]; }
 
 // Jacobian entry of contact `ci`, frame row `frow`, on dof k of chain side s (+1 body2, -1 body1)
 FB_DEV float contact_J(const DevModel& m, const DevData& d, int e, V3 f, V3 pos, int k) {
@@ -697,11 +676,11 @@ FB_DEV float contact_J(const DevModel& m, const DevData& d, int e, V3 f, V3 pos,
   return dot(f, t);
 }
 
-// K10b projection: blockDim = (32, FB_ROWPAR): rows are distributed over threadIdx.y.
+// K10b projection: one warp per env, rows dealt to the lanes.
 //   phase 0: J (dense-by-dof storage), Z = D^-1/2 L^-T J^T restricted to the row's dof set
 //   phase 1: A = Z Z^T  (= J M^-1 J^T, the unregularised Delassus matrix)
 struct ShNone { int dummy; };
-#define FB_ROW_ARGS const DevModel& m, const DevData& d, ShCon& sh, int e, int lane, int y
+#define FB_ROW_ARGS const DevModel& m, const DevData& d, ShCon& sh, int e, int y
 // one dof chain of a row: Jacobian entries along the chain, then z = D^-1/2 L^-T j by a dense back-sweep over the
 // chain (the ancestors of the p-th chain element are the elements p+1.. and L[k_p][k_q] sits at qLD[Madr[k_p] + q - p])
 FB_DEV void proj_chain(const DevModel& m, const DevData& d, int e, int r, int last, float sgn, bool contact, V3 f, V3 pos, float* zc,
@@ -810,9 +789,9 @@ FB_DEV void kref(FB_PHASE_ARGS) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// K3 + K8 transmission and actuation (MuJoCo mj_transmission, mj_fwdActuation), lane = env
+// K3 + K8 transmission and actuation (MuJoCo mj_transmission, mj_fwdActuation)
 FB_DEV void kact_p0(FB_PHASE_ARGS) {
-  tsolve_stage_issue(m, d, sh, e, lane, y, d.qLD); for (int k = y; k < m.nv; k += FB_NY) AT(d.qfrc_actuator, k) = 0; }
+  tsolve_stage_issue(m, d, sh, e, y, d.qLD); for (int k = y; k < m.nv; k += FB_NY) AT(d.qfrc_actuator, k) = 0; }
 FB_DEV void kact_p1(FB_PHASE_ARGS) {
   for (int i = y; i < m.nu; i += FB_NY) {
     float ctrl = AT(d.ctrl, i);
@@ -898,7 +877,7 @@ FB_DEV void kact_p3(FB_PHASE_ARGS) {
   }
 }
 // ---------------------------------------------------------------------------------------------
-// K11 constraint solve in the dual (force) space, lane = env.
+// K11 constraint solve in the dual (force) space.
 //
 // With a = qacc_smooth + M^-1 J^T lam the primal cost of MuJoCo's Newton solver becomes
 //   c(lam) = 1/2 lam^T A lam + s(b + A lam),   A = J M^-1 J^T, b = J qacc_smooth - aref,
@@ -940,21 +919,21 @@ FB_DEV int qcqp2(float* res, const float* A, const float* b, float d0, float d1,
 // delta_b = delta_parent + sum_d S_d qacc_d (MuJoCo mj_rnePostConstraint restated).
 FB_DEV void kfin_f1(FB_PHASE_ARGS) {
   float* xs = sh_dyn(sh);
-  tsolve_stage_issue(m, d, sh, e, lane, y, d.qLD);
+  tsolve_stage_issue(m, d, sh, e, y, d.qLD);
   prefetch_rec(d.Sang, FB_V3S * m.nv, d, e, y); prefetch_rec(d.Slin, FB_V3S * m.nv, d, e, y); prefetch_rec(d.inert10, FB_I10S * m.nbody, d, e, y); prefetch_rec(d.bfrc0, FB_S6S * m.nbody, d, e, y);
   if (d.do_integrate) prefetch_rec(d.qLDe, m.nM, d, e, y);   // second factor, staged after the first solve
   for (int i = y; i < m.nv; i += FB_NY) XS(i) = AT(d.qtmp, i) + AT(d.dof_isd, i) * AT(d.qfrc_zf, i);      // D^-1 u + D^-1/2 Z^T f
   for (int k = y; k < FB_S6S * m.nbody; k += FB_NY) AT(d.bfl, k) = 0;
 }
 FB_WARPFN void kfin_solve(const DevModel& m, const DevData& d, ShTree& sh, int e) {      // qacc = L^-1 (...)
-  WPAR_BEGIN tsolve_stage_wait(m, d, sh, e, 0, lane); WPAR_END
+  WPAR_BEGIN tsolve_stage_wait(m, d, sh, e, lane); WPAR_END
   tsolve_c(m, d, sh, e);
 }
 // Euler with implicit joint damping: qacc' = (M + h D)^-1 (qfrc_smooth + qfrc_constraint), second factor qLDe
 FB_WARPFN void kfin_solve_euler(const DevModel& m, const DevData& d, ShTree& sh, int e) { if (d.do_integrate) tri_solve(m, d, sh, e); }
 FB_DEV void kfin_f5(FB_PHASE_ARGS) {
   float* xs = sh_dyn(sh);
-  if (d.do_integrate) tsolve_stage_issue(m, d, sh, e, lane, y, d.qLDe);      // overlaps the sensor sweeps below
+  if (d.do_integrate) tsolve_stage_issue(m, d, sh, e, y, d.qLDe);      // overlaps the sensor sweeps below
   for (int i = y; i < m.nv; i += FB_NY) { AT(d.qacc, i) = XS(i); XS(i) = AT(d.qfrc_smooth, i) + AT(d.qfrc_constraint, i); }
   if (y != 0) return;
   // external (contact) wrench per body into bfl (about ref)
@@ -999,7 +978,7 @@ FB_DEV void kfin_f7(FB_PHASE_ARGS) {
     }
   }
 }
-FB_DEV void integrate_body(const DevModel& m, const DevData& d, int e, int lane, const float* xs, int b);
+FB_DEV void integrate_body(const DevModel& m, const DevData& d, int e, const float* xs, int b);
 FB_DEV void kfin_f8(FB_PHASE_ARGS) {
   float* xs = sh_dyn(sh);
   if (y < m.nlist) {
@@ -1015,7 +994,7 @@ FB_DEV void kfin_f8(FB_PHASE_ARGS) {
   if (AT(d.hold, 0)) return;          // env staged for reset: recompute (forward) but do not integrate
   // semi-implicit Euler: the free joints one lane per root (quaternion update), every other dof on its own lane -- walking the lists
   // body by body put a chain of dependent read-modify-writes of qvel / qpos on one lane per list
-  if (y < m.nroot) integrate_body(m, d, e, lane, xs, m.root_body[y]);
+  if (y < m.nroot) integrate_body(m, d, e, xs, m.root_body[y]);
   if (y == 0) AT(d.time, 0) += m.timestep;
   const float h = m.timestep;
   for (int k = y; k < m.nv; k += FB_NY) {
@@ -1083,17 +1062,17 @@ FB_DEV void kfin_f9(FB_PHASE_ARGS) {
   // state check (|qacc| > 1e14 or non-finite: reference tasks/base.py:222-225): each lane sums its dofs, kfin_f10 adds the lanes up
   float s2 = 0; bool bad = false;
   for (int k = y; k < m.nv; k += FB_NY) { float a = AT(d.qacc, k); s2 += a * a; if (!isfinite(a) || !isfinite(AT(d.qvel, k))) bad = true; }
-  sh.red[y][lane] = bad ? INFINITY : s2;
+  sh.red[y] = bad ? INFINITY : s2;
   if (d.do_integrate && !AT(d.hold, 0)) for (int i = y; i < m.na; i += FB_NY) AT(d.act, i) += m.timestep * AT(d.act_dot, i);
 }
 FB_DEV void kfin_f10(FB_PHASE_ARGS) {
   if (y != 0) return;
-  float s2 = 0; for (int l = 0; l < FB_NY; l++) s2 += sh.red[l][lane];
+  float s2 = 0; for (int l = 0; l < FB_NY; l++) s2 += sh.red[l];
   if (!(s2 < 1e28f)) FB_FLAG_OR(1);
 }
 // a ball joint: qvel += h qacc, then the quaternion qpos[qa .. qa + 3] turned by the body-frame angular velocity over one step (MuJoCo
 // mju_quatIntegrate; the free joint's branch restates it)
-FB_DEV void integrate_ball(const DevData& d, int e, int lane, const float* xs, int qa, int da, float h) {
+FB_DEV void integrate_ball(const DevData& d, int e, const float* xs, int qa, int da, float h) {
   for (int i = 0; i < 3; i++) { AT(d.qvel, da + i) += h * XS(da + i); }
   V3 w = v3(AT(d.qvel, da), AT(d.qvel, da + 1), AT(d.qvel, da + 2));
   float ang = norm(w) * h;
@@ -1102,7 +1081,7 @@ FB_DEV void integrate_ball(const DevData& d, int e, int lane, const float* xs, i
   q = qnormalize(q);
   AT(d.qpos, qa) = q.w; AT(d.qpos, qa + 1) = q.x; AT(d.qpos, qa + 2) = q.y; AT(d.qpos, qa + 3) = q.z;
 }
-FB_DEV void integrate_body(const DevModel& m, const DevData& d, int e, int lane, const float* xs, int b) {
+FB_DEV void integrate_body(const DevModel& m, const DevData& d, int e, const float* xs, int b) {
   float h = m.timestep;
   for (int k = 0; k < m.body_jntnum[b]; k++) {
     int j = m.body_jntadr[b] + k, qa = m.jnt_qposadr[j], da = m.jnt_dofadr[j];
@@ -1116,16 +1095,12 @@ FB_DEV void integrate_body(const DevModel& m, const DevData& d, int e, int lane,
       q = qnormalize(q);
       AT(d.qpos, qa + 3) = q.w; AT(d.qpos, qa + 4) = q.x; AT(d.qpos, qa + 5) = q.y; AT(d.qpos, qa + 6) = q.z;
     } else if (m.jnt_type[j] == FB_JNT_BALL) {
-      FB_NO_MERGE(); integrate_ball(d, e, lane, xs, qa, da, h); FB_NO_MERGE();
+      FB_NO_MERGE(); integrate_ball(d, e, xs, qa, da, h); FB_NO_MERGE();
     } else {
       AT(d.qvel, da) += h * XS(da);
       AT(d.qpos, qa) += h * AT(d.qvel, da);
     }
   }
-}
-// accumulate sensor sums (after step1 of the substep: vel sensors are from the new state)
-FB_DEV void ksens_accum(const DevModel& m, const DevData& d, int e, int first) {
-  for (int i = 0; i < m.nsensordata; i++) AT(d.sensor_sum, i) = (first ? 0.0f : AT(d.sensor_sum, i)) + AT(d.sensordata, i);
 }
 // last phase of the velocity kernel: per-substep sensor accumulation (d.sens_mode: 1 first substep, 0 next, -1 off)
 FB_DEV void kvel_p4(FB_PHASE_ARGS) {

@@ -13,13 +13,13 @@
 
 struct HfPrism { D3 v[6]; };
 FB_DEV MprPt hf_support(const HfPrism& pr, const MprObj& g, D3 dir) {
-  MprPt p; int best = 0; mreal bd = ddot(pr.v[0], dir);
+  MprPt p; int best = 0; float bd = ddot(pr.v[0], dir);
 #pragma unroll
-  for (int k = 1; k < 6; k++) { mreal dd = ddot(pr.v[k], dir); if (dd > bd) { bd = dd; best = k; } }
+  for (int k = 1; k < 6; k++) { float dd = ddot(pr.v[k], dir); if (dd > bd) { bd = dd; best = k; } }
   p.v1 = pr.v[best]; p.v2 = mpr_support1(g, d3(0, 0, 0) - dir); p.v = p.v1 - p.v2; return p;
 }
-FB_DEVN int hf_mpr_penetration(const HfPrism& o1, D3 c1, const MprObj& o2, mreal tol, int max_iter, mreal& depth, D3& pdir, D3& pos) {
-  D3 p1[4], v0, v1, v2, v3, dir; mreal dt; MprPt n;
+FB_DEVN int hf_mpr_penetration(const HfPrism& o1, D3 c1, const MprObj& o2, float tol, int max_iter, float& depth, D3& pdir, D3& pos) {
+  D3 p1[4], v0, v1, v2, v3, dir; float dt; MprPt n;
   v2 = v3 = d3(0, 0, 0); p1[2] = p1[3] = d3(0, 0, 0);
   p1[0] = c1; v0 = c1 - o2.pos;
   if (mpr_eq(v0.x, 0) && mpr_eq(v0.y, 0) && mpr_eq(v0.z, 0)) v0 = d3(MPR_EPS * 10, 0, 0);
@@ -64,17 +64,17 @@ FB_DEVN int hf_mpr_penetration(const HfPrism& o1, D3 c1, const MprObj& o2, mreal
     dir = mpr_portal_dir3(v1, v2, v3);
     n = hf_support(o1, o2, dir);
     if (mpr_reach_tol3(v1, v2, v3, n.v, dir, tol) || it > max_iter) {
-      depth = MSQRT(mpr_tri_dist2(d3(0, 0, 0), v1, v2, v3, pdir));
+      depth = sqrtf(mpr_tri_dist2(d3(0, 0, 0), v1, v2, v3, pdir));
       if (mpr_zero(pdir.x) && mpr_zero(pdir.y) && mpr_zero(pdir.z)) pdir = dir;
       pdir = dnormalized(pdir);
-      mreal b0 = ddot(dcross(v1, v2), v3), b1 = ddot(dcross(v3, v2), v0);
-      mreal b2 = ddot(dcross(v0, v1), v3), b3 = ddot(dcross(v2, v1), v0);
-      mreal sum = b0 + b1 + b2 + b3;
+      float b0 = ddot(dcross(v1, v2), v3), b1 = ddot(dcross(v3, v2), v0);
+      float b2 = ddot(dcross(v0, v1), v3), b3 = ddot(dcross(v2, v1), v0);
+      float sum = b0 + b1 + b2 + b3;
       if (mpr_zero(sum) || sum < 0) {
         b0 = 0; b1 = ddot(dcross(v2, v3), dir); b2 = ddot(dcross(v3, v1), dir); b3 = ddot(dcross(v1, v2), dir);
         sum = b1 + b2 + b3;
       }
-      mreal inv = 0.5 / sum;
+      float inv = 0.5 / sum;
       pos = ((c1 + o2.pos) * b0 + (p1[1] + p1[1] - v1) * b1 + (p1[2] + p1[2] - v2) * b2 + (p1[3] + p1[3] - v3) * b3) * inv;
       return 0;
     }
@@ -112,9 +112,9 @@ FB_DEV int col_convex_hfield(HfCon* out, int max, float margin, int type, V3 gp,
       pr.v[5] = d3(x, y, data[(size_t)(r + i) * ncol + c] * hf_size[2] + margin - rel.z);
       if (++nvert < 3) continue;
       if (pr.v[3].z < lo.z && pr.v[4].z < lo.z && pr.v[5].z < lo.z) continue;        // the geom is above this prism
-      D3 ctr = (pr.v[0] + pr.v[1] + pr.v[2] + pr.v[3] + pr.v[4] + pr.v[5]) * (mreal)(1.0 / 6.0);
-      mreal depth; D3 dir, cp;
-      if (hf_mpr_penetration(pr, ctr, g, (mreal)1e-6, 50, depth, dir, cp) != 0) continue;
+      D3 ctr = (pr.v[0] + pr.v[1] + pr.v[2] + pr.v[3] + pr.v[4] + pr.v[5]) * (float)(1.0 / 6.0);
+      float depth; D3 dir, cp;
+      if (hf_mpr_penetration(pr, ctr, g, (float)1e-6, 50, depth, dir, cp) != 0) continue;
       if (mpr_eq(dir.x, 0) && mpr_eq(dir.y, 0) && mpr_eq(dir.z, 0)) continue;
       HfCon& o = out[cnt];
       o.dist = (float)(margin - depth);

@@ -5,7 +5,7 @@
 // kinematic tree (a leg, the abdomen chain, the head sub-tree ...) in topological order.  The root
 // bodies (free joints) are handled by y == 0; the lists exchange their contributions to the root through
 // the env's shared-memory slice.  Each kernel is a sequence of *phases* separated by warp barriers (see
-// fb_run in flybody_b200.cu).  (`lane` in the phase signatures indexes FB_LANES == 1 shared slices.)
+// fb_run in flybody_b200.cu).
 #pragma once
 #include "fb_math.h"
 
@@ -15,21 +15,21 @@
 //                            factorisation's root-block partials (21) of FB_PARTR lanes at a time              -- pos, vel
 //   LS    [nM]               the joint-space inertia / its factor                                     -- pos
 //   XS    [nv + FB_ROOTD*nlist], LDS [nM]   right-hand side and staged factor of the triangular solves -- smooth, finish
-struct ShTree { float red[FB_NY][FB_LANES]; const unsigned* prog; const unsigned* pad_; };   // prog: the CTA's copy of the sweep program (smooth / finish kernels)
+struct ShTree { float red[FB_NY]; const unsigned* prog; const unsigned* pad_; };   // prog: the CTA's copy of the sweep program (smooth / finish kernels)
 #define FB_PARTK 21
 #define FB_PARTR 8             // 8 rows instead of one per lane: the position kernel's CTA then fits 8 per SM (and the larger L1 carveout)
-#define FB_PARTF (FB_PARTR * FB_PARTK * FB_LANES)
-#define PART(yy, k) part_[((yy) * FB_PARTK + (k)) * FB_LANES + lane]
-#define PARTL(l, k, K) part_[((l) * (K) + (k)) * FB_LANES + lane]     // K entries per branch list l
+#define FB_PARTF (FB_PARTR * FB_PARTK)
+#define PART(yy, k) part_[(yy) * FB_PARTK + (k)]
+#define PARTL(l, k, K) part_[(l) * (K) + (k)]     // K entries per branch list l
 static_assert(FB_NLMAX * 12 <= FB_PARTR * FB_PARTK, "the per-list partial sums must fit PART");
 
 // dynamic shared memory that follows the fixed struct (per-kernel scratch: the L^T D L rows during the
-// factorisation, the right-hand side during tree solves), laid out [entry][lane]
+// factorisation, the right-hand side during tree solves)
 template <typename Sh> FB_DEV float* sh_dyn(Sh& sh) { return reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(&sh) + ((sizeof(Sh) + 15) & ~(size_t)15)); }
-#define LS(k) ldsh[(k) * FB_LANES + lane]
-#define XS(k) xs[(k) * FB_LANES + lane]
+#define LS(k) ldsh[k]
+#define XS(k) xs[k]
 
-#define FB_PHASE_ARGS const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y
+#define FB_PHASE_ARGS const DevModel& m, const DevData& d, ShTree& sh, int e, int y
 #define FB_LIST_LOOP_FWD for (int li_ = 0, b = 0; li_ < m.list_num[y] && ((b = m.list_body[m.list_adr[y] + li_]), true); li_++)
 #define FB_LIST_LOOP_REV for (int li_ = m.list_num[y] - 1, b = 0; li_ >= 0 && ((b = m.list_body[m.list_adr[y] + li_]), true); li_--)
 
@@ -93,8 +93,8 @@ FB_DEV void body_pose(const DevModel& m, const DevData& d, int e, int b, V3 ppos
 // CRBS(b, k): the composite inertias while they are being accumulated (kpos_p1b .. kpos_p3b) live in the shared-memory region that
 // later holds the inertia matrix rows (LS): the backward accumulation along the lists is a chain of read-modify-writes, which as
 // global-memory traffic costs an L2 round trip per body (12.8 % of the position kernel's stall samples, profiles/README.md)
-#define CRBS(b, k) ldsh[((b) * 10 + (k)) * FB_LANES + lane]
-FB_DEV void body_derived(const DevModel& m, const DevData& d, int e, int b, float* ldsh, int lane) {
+#define CRBS(b, k) ldsh[(b) * 10 + (k)]
+FB_DEV void body_derived(const DevModel& m, const DevData& d, int e, int b, float* ldsh) {
   V3 pos = ld3(d.xpos, b, d, e); Q4 quat = ld4(d.xquat, b, d, e);
   M3 R = q2m(quat);
   st9(d.xmat, b, d, e, R);
@@ -154,7 +154,7 @@ FB_DEV void kpos_p1b(FB_PHASE_ARGS) {
     if (b == 0) { M3 I; for (int k = 0; k < 9; k++) I.m[k] = (k % 4 == 0) ? 1.f : 0.f;
       st9(d.xmat, 0, d, e, I); st3(d.xipos, 0, d, e, ld3(d.xpos, 0, d, e)); st9(d.ximat, 0, d, e, I);
       { float z10[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0}; st10(d.inert10, 0, d, e, z10); for (int k = 0; k < 10; k++) CRBS(0, k) = 0; }
-    } else body_derived(m, d, e, b, ldsh, lane);
+    } else body_derived(m, d, e, b, ldsh);
   }
   for (int g = y; g < m.ngeom; g += FB_NY) {
     int b = m.geom_bodyid[g]; V3 pos = ld3(d.xpos, b, d, e); Q4 quat = ld4(d.xquat, b, d, e);
@@ -201,7 +201,7 @@ FB_DEV void kpos_p3b(FB_PHASE_ARGS) {
   for (int b = y; b < m.nbody; b += FB_NY) { float v[10]; for (int k = 0; k < 10; k++) v[k] = CRBS(b, k); st10(d.crb10, b, d, e, v); }
 }
 // joint-space inertia entries of dof i (row of the sparse lower triangle along the ancestor chain)
-FB_DEV void mass_row(const DevModel& m, const DevData& d, int e, int lane, float* ldsh, int i) {
+FB_DEV void mass_row(const DevModel& m, const DevData& d, int e, float* ldsh, int i) {
   int b = m.dof_bodyid[i];
   I10 I = ld10(d.crb10, b, d, e);
   V3 L, p;
@@ -227,17 +227,17 @@ FB_DEV void mass_row(const DevModel& m, const DevData& d, int e, int lane, float
 }
 FB_DEV void kpos_p4(FB_PHASE_ARGS) {      // all 32 lanes over the dofs
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF; (void)part_;
-  for (int i = y; i < m.nv; i += FB_NY) mass_row(m, d, e, lane, ldsh, i);
+  for (int i = y; i < m.nv; i += FB_NY) mass_row(m, d, e, ldsh, i);
 }
 // Copy the factor held in shared memory out to `dst`.  Convention of qLD / qLDe: the diagonal holds D[k], the off-diagonal
 // entries stay UNSCALED, M'[k][anc] = D[k] L[k][anc] -- every consumer multiplies a whole row by one 1/D[k] instead of
 // scaling each entry here.
-FB_DEV void ld_writeout(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, float* dst) {
+FB_DEV void ld_writeout(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, float* dst) {
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF; (void)part_;
   for (int k = y; k < m.nM; k += FB_NY) AT(dst, k) = LS(k);
 }
 // re-initialise the shared rows with M + h*diag(damping) for the second factorisation (Euler with implicit damping)
-FB_DEV void ld_reinit_damped(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y) {
+FB_DEV void ld_reinit_damped(const DevModel& m, const DevData& d, ShTree& sh, int e, int y) {
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF; (void)part_;
   for (int k = y; k < m.nM; k += FB_NY) LS(k) = AT(d.qM, k) + m.timestep * m.M_damp[k];
 }
@@ -247,20 +247,19 @@ FB_DEV void ld_reinit_damped(const DevModel& m, const DevData& d, ShTree& sh, in
 // ancestor rows of the step's dofs are dealt to all 32 lanes (factor_step_sched).  Updates that land in the root block are
 // summed into sh.part (21 entries per lane) and applied by the root lane afterwards.
 #define FB_FSUB 3
-// packed per-(step, lane) header of the lock-step sweeps: one coalesced load instead of the dependent chain
-// list_dofadr -> list_dof -> dof_Madr / dof_chainlen / dof_depth.  adr | len << 12 | depth << 18 | dof << 24, ~0 = idle
+// packed per-(step, lane) header of the lock-step sweeps (tsolve_blob), one word instead of the dependent chain list dof ->
+// dof_Madr / dof_chainlen / dof_depth.  adr | len << 12 | depth << 18 | dof << 24, ~0 = idle
 #define FB_HDR_IDLE 0xffffffffu
 #define HDR_ADR(h) ((int)((h) & 4095u))
 #define HDR_LEN(h) ((int)(((h) >> 12) & 63u))
-#define HDR_DEPTH(h) ((int)(((h) >> 18) & 63u))
 #define HDR_DOF(h) ((int)((h) >> 24))
 #define FB_ROOTD6 6            // dofs of a root body (free joint)
 // One step of the sweep: the dofs k of this step (one per list) subtract their rank-1 term from the rows of their non-root ancestors,
-// row(anc_t)[s] -= (r_k[t] / D_k) r_k[t + s]  (M_ancadr: row address of the t-th ancestor; the root's dofs are the tail of every chain
+// row(anc_t)[s] -= (r_k[t] / D_k) r_k[t + s]  (the item carries the row address of the t-th ancestor; the root's dofs are the tail of every chain
 // and are handled by factor_root_accum).  The (k, t) pairs of a step touch different rows, so they are independent work items; the
 // host deals them to the 32 lanes longest-first onto the least loaded lane (DevModel::fs_rng / fs_items, built in fb_create) --
 // round 1 gave every list 3 fixed lanes, which kept 12 of 32 busy.  The item after the current one is loaded while this one runs.
-FB_DEV void factor_step_sched(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, unsigned rng) {
+FB_DEV void factor_step_sched(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, unsigned rng) {
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF; (void)part_;
   const int cnt = (int)(rng >> 16);
   if (cnt == 0) return;
@@ -283,7 +282,7 @@ FB_DEV void factor_step_sched(const DevModel& m, const DevData& d, ShTree& sh, i
 // Root blocks.  Once the lists are eliminated, row k of a non-root dof holds its final (unscaled) coupling r_k to the
 // root's dofs and D_k; the Schur update of the root block is sum_k r_k r_k^T / D_k.  32 lanes split the dofs, each
 // accumulates the 21 packed lower-triangle entries in registers ...
-FB_DEV void factor_root_accum(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, int r, float acc[21]) {
+FB_DEV void factor_root_accum(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, int r, float acc[21]) {
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF; (void)part_;
 #pragma unroll
   for (int j = 0; j < 21; j++) acc[j] = 0;
@@ -303,19 +302,19 @@ FB_DEV void factor_root_accum(const DevModel& m, const DevData& d, ShTree& sh, i
 }
 // ... 21 lanes add the partials up (one packed entry each), in lane order: lanes y0 .. y0 + FB_PARTR - 1 put theirs into PART,
 // then the summing lanes add them on; a sum over all 32 lanes takes FB_NY / FB_PARTR such rounds ...
-FB_DEV void factor_root_put(ShTree& sh, int lane, int y, int y0, const float acc[21]) {
+FB_DEV void factor_root_put(ShTree& sh, int y, int y0, const float acc[21]) {
   float* part_ = sh_dyn(sh);
   if (y < y0 || y >= y0 + FB_PARTR) return;
 #pragma unroll
   for (int j = 0; j < 21; j++) PART(y - y0, j) = acc[j];
 }
-FB_DEV void factor_root_sum(ShTree& sh, int lane, int y, float& acc) {
+FB_DEV void factor_root_sum(ShTree& sh, int y, float& acc) {
   float* part_ = sh_dyn(sh);
   if (y >= 21) return;
 #pragma unroll
   for (int l = 0; l < FB_PARTR; l++) acc += PART(l, y);
 }
-FB_DEV void factor_root_gather(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, int r, float acc) {
+FB_DEV void factor_root_gather(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, int r, float acc) {
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF;
   if (y >= 21) return;
   int il = 0; while ((il + 1) * (il + 2) / 2 <= y) il++;
@@ -325,7 +324,7 @@ FB_DEV void factor_root_gather(const DevModel& m, const DevData& d, ShTree& sh, 
   LS(m.dof_Madr[d0 + il] + s) -= acc;
 }
 // ... then one lane per root body factors its dense (<= 6x6) block
-FB_DEV void factor_root(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y) {
+FB_DEV void factor_root(const DevModel& m, const DevData& d, ShTree& sh, int e, int y) {
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF; (void)part_;
   if (y >= m.nroot) return;
   int b = m.root_body[y], nd = m.body_dofnum[b], d0 = m.body_dofadr[b];
@@ -347,19 +346,19 @@ FB_WARPFN void kpos_factor(const DevModel& m, const DevData& d, ShTree& sh, int 
     unsigned hd = m.max_list_ndof > 0 ? hp[0] : 0u;
     for (int step = 0; step < m.max_list_ndof; step++) {
       const unsigned nxt = step + 1 < m.max_list_ndof ? hp[(step + 1) * FB_NY] : 0u;
-      factor_step_sched(m, d, sh, e, 0, lane, hd); __syncwarp();
+      factor_step_sched(m, d, sh, e, lane, hd); __syncwarp();
       hd = nxt;
     }
   }
 #else
   for (int step = 0; step < m.max_list_ndof; step++) {
-    WPAR_BEGIN factor_step_sched(m, d, sh, e, 0, lane, m.fs_rng[step * FB_NY + lane]); WPAR_END
+    WPAR_BEGIN factor_step_sched(m, d, sh, e, lane, m.fs_rng[step * FB_NY + lane]); WPAR_END
   }
 #endif
   for (int r = 0; r < m.nroot; r++) {
     if (!m.root_haslists[r]) continue;
     LREGA(float, acc, 21); LREG(float, tot);
-    WPAR_BEGIN { float a[21]; factor_root_accum(m, d, sh, e, 0, lane, r, a);
+    WPAR_BEGIN { float a[21]; factor_root_accum(m, d, sh, e, lane, r, a);
 #pragma unroll
       for (int j = 0; j < 21; j++) LA(acc, j) = a[j];
       L(tot) = 0.0f; } WPAR_END
@@ -367,21 +366,21 @@ FB_WARPFN void kpos_factor(const DevModel& m, const DevData& d, ShTree& sh, int 
       WPAR_BEGIN { float a[21];
 #pragma unroll
         for (int j = 0; j < 21; j++) a[j] = LA(acc, j);
-        factor_root_put(sh, 0, lane, y0, a); } WPAR_END
-      WPAR_BEGIN factor_root_sum(sh, 0, lane, L(tot)); WPAR_END
+        factor_root_put(sh, lane, y0, a); } WPAR_END
+      WPAR_BEGIN factor_root_sum(sh, lane, L(tot)); WPAR_END
     }
-    WPAR_BEGIN factor_root_gather(m, d, sh, e, 0, lane, r, L(tot)); WPAR_END
+    WPAR_BEGIN factor_root_gather(m, d, sh, e, lane, r, L(tot)); WPAR_END
   }
-  WPAR_BEGIN factor_root(m, d, sh, e, 0, lane); WPAR_END
+  WPAR_BEGIN factor_root(m, d, sh, e, lane); WPAR_END
 }
-FB_DEV void kpos_p6w(FB_PHASE_ARGS) { ld_writeout(m, d, sh, e, lane, y, d.qLD); }
-FB_DEV void kpos_p6d(FB_PHASE_ARGS) { ld_reinit_damped(m, d, sh, e, lane, y); }
-FB_DEV void kpos_p9(FB_PHASE_ARGS) { ld_writeout(m, d, sh, e, lane, y, d.qLDe); }
+FB_DEV void kpos_p6w(FB_PHASE_ARGS) { ld_writeout(m, d, sh, e, y, d.qLD); }
+FB_DEV void kpos_p6d(FB_PHASE_ARGS) { ld_reinit_damped(m, d, sh, e, y); }
+FB_DEV void kpos_p9(FB_PHASE_ARGS) { ld_writeout(m, d, sh, e, y, d.qLDe); }
 
 // ---------------------------------------------------------------------------------------------
 // x <- (L^T D L)^-1 x (MuJoCo mj_solveLD).  x lives in shared memory: XS(0..nv) plus FB_ROOTD private accumulators per
 // list at XS(nv + FB_ROOTD*l + il) for the updates that land on the root's dofs.  The lists advance in lock-step, one
-// dof per step; the FB_FSUB lanes of a list split that dof's ancestor chain (dof_ancslot / dof_anc give the shared slot
+// dof per step; the FB_FSUB lanes of a list split that dof's ancestor chain (the sweep program below gives the shared slot
 // of the t-th ancestor without pointer chasing).
 #define FB_ROOTD 6
 // Sweep program of the triangular solves, copied once per CTA into shared memory (DevModel::tsolve_blob): the packed step
@@ -392,11 +391,11 @@ FB_DEV void kpos_p9(FB_PHASE_ARGS) { ld_writeout(m, d, sh, e, lane, y, d.qLDe); 
 #define TS_SLOT8(sh, m) (reinterpret_cast<const unsigned char*>((sh).prog + 2 * (m).ts_hdr_words))
 #define TS_ANC8(sh, m) (TS_SLOT8(sh, m) + (m).ts_nm_pad)
 #define FB_NXS(m) (((m).nv + FB_ROOTD * (m).nlist + 3) & ~3)      // multiple of 4: the staged factor behind it stays 16-byte aligned
-#define LDS(k) lds[(k) * FB_LANES + lane]
+#define LDS(k) lds[k]
 // Stage a factor into the warp's shared slice with asynchronous 16-byte copies (cp.async): issued early (first phase
 // of the kernel / right after the previous solve), waited for at the start of tri_solve, so the DRAM latency overlaps
 // the phases in between and the sweeps only touch shared memory.  Record arrays start on 16-byte boundaries.
-FB_DEV void tsolve_stage_issue(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, const float* LD) {
+FB_DEV void tsolve_stage_issue(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, const float* LD) {
   float* xs = sh_dyn(sh); float* lds = xs + FB_NXS(m);
 #ifdef __CUDACC__
   unsigned sa = (unsigned)__cvta_generic_to_shared(lds);
@@ -414,7 +413,7 @@ FB_DEV void tsolve_stage_wait(FB_PHASE_ARGS) {
   for (int k = y; k < FB_ROOTD * m.nlist; k += FB_NY) XS(m.nv + k) = 0;      // the lists' private root accumulators
 }
 // x <- L^-T x restricted to the list dofs, deepest first: x[anc] -= L[k][anc] x[k]
-FB_DEV void tsolve_a_step_h(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, unsigned hd) {
+FB_DEV void tsolve_a_step_h(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, unsigned hd) {
   float* xs = sh_dyn(sh); const float* lds = xs + FB_NXS(m);
   if (hd == FB_HDR_IDLE) return;
   const int sub = y % FB_FSUB, k = HDR_DOF(hd), adrk = HDR_ADR(hd), len = HDR_LEN(hd);
@@ -422,8 +421,8 @@ FB_DEV void tsolve_a_step_h(const DevModel& m, const DevData& d, ShTree& sh, int
   float xk = XS(k) / LDS(adrk);                    // rows are stored unscaled: L[k][anc] x[k] = M'[k][anc] (x[k] / D[k])
   for (int t = 1 + sub; t < len; t += FB_FSUB) XS(slot8[adrk + t]) -= LDS(adrk + t) * xk;
 }
-FB_DEV void tsolve_a_step(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, int step) {
-  tsolve_a_step_h(m, d, sh, e, lane, y, TS_HDR_A(sh, m)[step * FB_NY + y]);
+FB_DEV void tsolve_a_step(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, int step) {
+  tsolve_a_step_h(m, d, sh, e, y, TS_HDR_A(sh, m)[step * FB_NY + y]);
 }
 // root blocks: collect the lists' contributions, then the dense (<= 6x6) back / scale / forward substitution
 FB_DEV void tsolve_b_gather(FB_PHASE_ARGS) {
@@ -461,7 +460,7 @@ FB_DEV void tsolve_scale(FB_PHASE_ARGS) {        // x <- D^-1 x
   for (int k = y; k < m.nv; k += FB_NY) XS(k) /= LDS(m.dof_Madr[k]);
 }
 // x <- L^-1 x on the list dofs, shallowest first: x[k] -= sum_t L[k][anc_t] x[anc_t]
-FB_DEV void tsolve_c_step(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, int step) {
+FB_DEV void tsolve_c_step(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, int step) {
   float* xs = sh_dyn(sh); const float* lds = xs + FB_NXS(m);
   const unsigned hd = TS_HDR_C(sh, m)[step * FB_NY + y];
   if (hd == FB_HDR_IDLE) return;
@@ -469,14 +468,14 @@ FB_DEV void tsolve_c_step(const DevModel& m, const DevData& d, ShTree& sh, int e
   const unsigned char* anc8 = TS_ANC8(sh, m);
   float p = 0;
   for (int t = 1 + sub; t < len; t += FB_FSUB) p += LDS(adrk + t) * XS(anc8[adrk + t]);
-  sh.red[y][lane] = p;
+  sh.red[y] = p;
 }
-FB_DEV void tsolve_c_fin(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, int step) {
+FB_DEV void tsolve_c_fin(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, int step) {
   float* xs = sh_dyn(sh); const float* lds = xs + FB_NXS(m);
   const unsigned hd = TS_HDR_C(sh, m)[step * FB_NY + y];
   if (hd == FB_HDR_IDLE || y % FB_FSUB != 0) return;
   float p = 0;
-  for (int u = 0; u < FB_FSUB; u++) p += sh.red[y + u][lane];
+  for (int u = 0; u < FB_FSUB; u++) p += sh.red[y + u];
   XS(HDR_DOF(hd)) -= p / LDS(HDR_ADR(hd));
 }
 // M^-1 = L^-1 D^-1 L^-T is applied in halves so that callers can work between them (the factor must have been issued
@@ -484,25 +483,25 @@ FB_DEV void tsolve_c_fin(const DevModel& m, const DevData& d, ShTree& sh, int e,
 //   tsolve_a : wait for the staged factor, x <- L^-T x
 //   tsolve_c : x <- L^-1 x
 FB_WARPFN void tsolve_a(const DevModel& m, const DevData& d, ShTree& sh, int e) {
-  WPAR_BEGIN tsolve_stage_wait(m, d, sh, e, 0, lane); WPAR_END
+  WPAR_BEGIN tsolve_stage_wait(m, d, sh, e, lane); WPAR_END
 #ifdef __CUDACC__
   { const int lane = threadIdx.x; const unsigned* hp = TS_HDR_A(sh, m) + lane;
     unsigned hd = m.max_list_ndof > 0 ? hp[0] : FB_HDR_IDLE;
     for (int step = 0; step < m.max_list_ndof; step++) {
       const unsigned nxt = step + 1 < m.max_list_ndof ? hp[(step + 1) * FB_NY] : FB_HDR_IDLE;      // next step's header in flight during this step
-      tsolve_a_step_h(m, d, sh, e, 0, lane, hd); __syncwarp();
+      tsolve_a_step_h(m, d, sh, e, lane, hd); __syncwarp();
       hd = nxt;
     } }
 #else
-  for (int step = 0; step < m.max_list_ndof; step++) { WPAR_BEGIN tsolve_a_step(m, d, sh, e, 0, lane, step); WPAR_END }
+  for (int step = 0; step < m.max_list_ndof; step++) { WPAR_BEGIN tsolve_a_step(m, d, sh, e, lane, step); WPAR_END }
 #endif
-  WPAR_BEGIN tsolve_b_gather(m, d, sh, e, 0, lane); WPAR_END
-  WPAR_BEGIN tsolve_root_a(m, d, sh, e, 0, lane); WPAR_END
+  WPAR_BEGIN tsolve_b_gather(m, d, sh, e, lane); WPAR_END
+  WPAR_BEGIN tsolve_root_a(m, d, sh, e, lane); WPAR_END
 }
 #ifdef __CUDACC__
 // GPU: the three partial dot products of a list are combined with two shuffles instead of a trip through shared memory
 // and a second barrier (the host emulation runs the lanes one after the other and keeps the two-section form)
-FB_DEV void tsolve_c_step_shfl(const DevModel& m, const DevData& d, ShTree& sh, int e, int lane, int y, unsigned hd) {
+FB_DEV void tsolve_c_step_shfl(const DevModel& m, const DevData& d, ShTree& sh, int e, int y, unsigned hd) {
   float* xs = sh_dyn(sh); const float* lds = xs + FB_NXS(m);
   const bool active = hd != FB_HDR_IDLE;
   const int sub = y % FB_FSUB, k = HDR_DOF(hd), adrk = HDR_ADR(hd);
@@ -517,25 +516,25 @@ FB_DEV void tsolve_c_step_shfl(const DevModel& m, const DevData& d, ShTree& sh, 
 }
 #endif
 FB_WARPFN void tsolve_c(const DevModel& m, const DevData& d, ShTree& sh, int e) {
-  WPAR_BEGIN tsolve_root_c(m, d, sh, e, 0, lane); WPAR_END
+  WPAR_BEGIN tsolve_root_c(m, d, sh, e, lane); WPAR_END
 #ifdef __CUDACC__
   { const int lane = threadIdx.x; const unsigned* hp = TS_HDR_C(sh, m) + lane;
     unsigned hd = m.max_list_ndof > 0 ? hp[0] : FB_HDR_IDLE;
     for (int step = 0; step < m.max_list_ndof; step++) {
       const unsigned nxt = step + 1 < m.max_list_ndof ? hp[(step + 1) * FB_NY] : FB_HDR_IDLE;
-      tsolve_c_step_shfl(m, d, sh, e, 0, lane, hd); __syncwarp();
+      tsolve_c_step_shfl(m, d, sh, e, lane, hd); __syncwarp();
       hd = nxt;
     } }
 #else
   for (int step = 0; step < m.max_list_ndof; step++) {
-    WPAR_BEGIN tsolve_c_step(m, d, sh, e, 0, lane, step); WPAR_END
-    WPAR_BEGIN tsolve_c_fin(m, d, sh, e, 0, lane, step); WPAR_END
+    WPAR_BEGIN tsolve_c_step(m, d, sh, e, lane, step); WPAR_END
+    WPAR_BEGIN tsolve_c_fin(m, d, sh, e, lane, step); WPAR_END
   }
 #endif
 }
 FB_WARPFN void tri_solve(const DevModel& m, const DevData& d, ShTree& sh, int e) {
   tsolve_a(m, d, sh, e);
-  WPAR_BEGIN tsolve_scale(m, d, sh, e, 0, lane); WPAR_END
+  WPAR_BEGIN tsolve_scale(m, d, sh, e, lane); WPAR_END
   tsolve_c(m, d, sh, e);
 }
 
@@ -556,35 +555,6 @@ FB_DEV void rot3_vel_acc(const DevData& d, int e, int da, V3 vlin, const float* 
     if (qacc) { float qa = AT(qacc, da + i); a.a = a.a + Sa * qa; a.l = a.l + Sl * qa; }
   }
   a.l = a.l + cross(vlin, w);
-}
-// forward recursion for one body; qacc == nullptr -> bias acceleration only
-FB_DEV void body_vel_acc(const DevModel& m, const DevData& d, int e, int b, const float* qacc, float* bvel, float* bacc) {
-  int p = m.body_parentid[b];
-  S6 v = ld6(bvel, p, d, e), a = ld6(bacc, p, d, e);
-  int jn = m.body_jntnum[b];
-  for (int k = 0; k < jn; k++) {
-    int j = m.body_jntadr[b] + k, da = m.jnt_dofadr[j];
-    if (m.jnt_type[j] == FB_JNT_FREE) {
-      V3 vlin = v3(AT(d.qvel, da), AT(d.qvel, da + 1), AT(d.qvel, da + 2)), w = v3(0, 0, 0);
-      for (int i = 0; i < 6; i++) {
-        float qd = AT(d.qvel, da + i);
-        V3 Sa = ld3(d.Sang, da + i, d, e), Sl = ld3(d.Slin, da + i, d, e);
-        v.a = v.a + Sa * qd; v.l = v.l + Sl * qd;
-        if (i >= 3) w = w + Sa * qd;
-        if (qacc) { float qa = AT(qacc, da + i); a.a = a.a + Sa * qa; a.l = a.l + Sl * qa; }
-      }
-      a.l = a.l + cross(vlin, w);
-    } else if (m.jnt_type[j] == FB_JNT_BALL) { FB_NO_MERGE(); rot3_vel_acc(d, e, da, v.l, qacc, v, a); FB_NO_MERGE(); }
-    else {
-      float qd = AT(d.qvel, da);
-      V3 Sa = ld3(d.Sang, da, d, e), Sl = ld3(d.Slin, da, d, e);
-      S6 r = motion_cross(v, Sa, Sl);
-      a.a = a.a + r.a * qd; a.l = a.l + r.l * qd;
-      v.a = v.a + Sa * qd; v.l = v.l + Sl * qd;
-      if (qacc) { float qa = AT(qacc, da); a.a = a.a + Sa * qa; a.l = a.l + Sl * qa; }
-    }
-  }
-  st6(bvel, b, d, e, v); st6(bacc, b, d, e, a);
 }
 // inertial force of body b: I a + v x* (I v), [torque about ref; force]
 FB_DEV S6 body_inertial_force(const DevModel& m, const DevData& d, int e, int b, const float* bvel, const float* bacc) {
@@ -738,7 +708,6 @@ FB_DEV void kvel_p1(FB_PHASE_ARGS) {
 }
 // (Subtree sums of the velocity stage stay in the record: moving them to shared memory as in the position kernel costs 3.3 KB more
 // shared memory per warp, which shrinks the L1 the scattered record loads live in.)
-// all lanes over bodies: bias force (kept un-accumulated in bfrc0 for the sensor pass) and fluid wrench
 // all lanes over bodies: bias force (kept un-accumulated in bfrc0 for the sensor pass) and fluid wrench
 FB_DEV void kvel_p1b(FB_PHASE_ARGS) {
   for (int b = y; b < m.nbody; b += FB_NY) {

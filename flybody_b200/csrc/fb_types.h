@@ -24,10 +24,7 @@
 #define FB_NY 32             // lanes per env (threadIdx.x); every kernel runs 32 lanes per env
 #define FB_MINB 8            // resident blocks per SM the kernels are compiled for: 8 x 4 warps >= 4096 envs / 132 SMs (H100), one wave
 #define FB_WPB 4             // envs (warps) per block
-#define FB_LANES 1           // shared-memory slices are per env
 #define FB_NLMAX 10          // branch lists of the tree kernels (lanes 0..nlist-1 active; 3 lanes per list in the factorisation)
-#define FB_MAXCHUNK 32       // collision chunks (one per lane)
-#define FB_CHUNKCAP 16       // contacts one chunk may emit
 #define FB_ROWPAR 8          // rows processed in parallel by the projection kernel
 #define FB_MINVAL 1e-15f
 
@@ -78,20 +75,18 @@ struct DevModel {
   int nroot, nlist;
   const int *root_body;                    // [nroot]
   const int *list_adr, *list_num, *list_body, *list_root;   // bodies of each branch list in topological order
-  const int *list_dofadr, *list_ndof, *list_dof; int max_list_ndof;   // dofs of each list, deepest first (factorisation order)
+  int max_list_ndof;                       // dofs of the longest list (steps of the lock-step sweeps)
   // bodies
-  const int *body_parentid, *body_rootid, *body_jntadr, *body_jntnum, *body_dofadr, *body_dofnum, *body_lastdof,
-      *body_fluid_ellipsoid, *body_isroot, *body_sensacc, *body_sensfrc, *body_geomadr, *body_geomnum, *body_siteadr, *body_sitenum;
+  const int *body_parentid, *body_jntadr, *body_jntnum, *body_dofadr, *body_dofnum, *body_lastdof,
+      *body_fluid_ellipsoid, *body_isroot, *body_sensacc, *body_sensfrc;
   const float *body_pos, *body_quat, *body_ipos, *body_iquat, *body_mass, *body_inertia, *body_invweight0;
   // joints / dofs
   const int *jnt_type, *jnt_qposadr, *jnt_dofadr, *jnt_bodyid, *jnt_limited;
   const float *jnt_pos, *jnt_axis, *jnt_stiffness, *jnt_range, *jnt_solref, *jnt_solimp, *jnt_margin, *qpos0, *qpos_spring;
-  const int *dof_bodyid, *dof_jntid, *dof_parentid, *dof_Madr, *dof_subend, *dof_depth /* #non-root ancestors; local index for root dofs */, *dof_isroot, *dof_chainlen, *dof_anc /* [nM] t-th ancestor of the row's dof */, *dof_ancslot /* same, as shared-memory slot of tri_solve */;
+  const int *dof_bodyid, *dof_jntid, *dof_parentid, *dof_Madr, *dof_subend, *dof_depth /* #non-root ancestors; local index for root dofs */, *dof_chainlen, *dof_anc /* [nM] t-th ancestor of the row's dof */;
   const unsigned char* dof_lca;   // [nv][nv] number of common ancestors-or-self of two dofs (= chain length of their lowest common ancestor, 0: none)
   const int *dof_rootidx /* root (index into root_body) a list dof hangs off, -1 for root dofs */, *root_haslists;
-  const unsigned *step_hdr_a, *step_hdr_c;   // [max_list_ndof][32] packed sweep headers, deepest-first / shallowest-first
   const unsigned* tsolve_blob; int ts_hdr_words, ts_nm_pad, ts_blob_words;    // sweep program copied per CTA into shared memory (fb_tree.h)
-  const int* M_ancadr;         // [nM] row address (dof_Madr) of the ancestor an entry belongs to
   const unsigned* fs_rng; const FsItem* fs_items;   // factorisation schedule: per (step, lane) first item | count << 16; item = (adr_k | t << 12 | update length << 18, adr of the ancestor row)
   const float* M_damp;         // per entry of the packed inertia: joint damping on the diagonals, 0 elsewhere
   const int* body_adhesion;    // adhesion actuator acting on the body, or -1
@@ -102,7 +97,6 @@ struct DevModel {
       *geom_margin, *geom_gap;
   const int *pair_geom1, *pair_geom2;
   const int* pair_info; const float* pair_rsum;   // packed broadphase record: g1 | g2 << 15 | plane << 30, margin + bounding radii
-  int nchunk; const int* chunk_start;   // [nchunk+1] pair ranges, balanced by expected contact count
   // fluid geoms, sites, tendons, actuators, sensors
   const int *fluid_bodyid; const float *fluid_pos, *fluid_quat, *fluid_size, *fluid_coef;
   const int *site_bodyid, *site_type; const float *site_pos, *site_quat, *site_size;
@@ -126,7 +120,7 @@ struct DevData {
   // position stage
   float *ref;                  // [3] reference point (root position) all spatial quantities are taken about
   float *xpos, *xquat, *xmat, *xipos, *ximat;          // body frames (positions relative to ref)
-  float *geom_xpos, *geom_xmat, *site_xpos, *site_xmat, *subtree_com;
+  float *geom_xpos, *geom_xmat, *site_xpos, *site_xmat;
   float *Sang, *Slin;          // [nv*3] motion subspaces about ref
   float *inert10, *crb10;      // [nbody*10]
   float *qM, *qLD, *qLDe;      // [nM] inertia, its L^T D L factor, factor of M + h*diag(damping)
@@ -137,15 +131,15 @@ struct DevData {
   // contacts
   int *ncon; float *con_dist, *con_pos, *con_frame; int *con_geom1, *con_geom2, *con_efcadr, *con_dim;
   float *con_mu, *con_fric;    // mu, friction[2]
-  float *tmp_con; int *tmp_geom;   // chunk staging
+  float *tmp_con; int *tmp_geom;   // collision candidates' contacts, before compaction
   // constraints
   int *nefc; int *efc_type, *efc_id;
-  float *efc_pos, *efc_margin, *efc_D, *efc_R, *efc_K, *efc_B, *efc_imp, *efc_aref, *efc_b, *efc_force, *efc_jarws;
+  float *efc_pos, *efc_margin, *efc_D, *efc_R, *efc_K, *efc_B, *efc_imp, *efc_aref, *efc_b, *efc_force;
   float *efc_J, *efc_Z;        // [MAXEFC][FB_JROW] chain-sparse rows (fb_constraint.h: EJC)
   float *efc_A, *efc_G;        // packed lower triangles
   int *efc_key, *prev_key, *prev_n; float *prev_lam;   // warm start: constraint forces of the previous solve, matched by row identity
   float *efc_w;                // [8*MAXEFC] solver work vectors
-  int *efc_ecol, *efc_ekind, *efc_state, *efc_colidx, *efc_la, *efc_lb;   // solver bookkeeping: E columns, row zones, row dof chains
+  int *efc_la, *efc_lb;       // row dof chains
   // sensors / outputs
   float *sensordata, *sensor_sum;
   int clk_launch; long long* clk;              // -DFB_CLK builds only: clock64() of warp 0 after every stage of every launch (latency profile)
@@ -174,7 +168,7 @@ struct DevTask {
   int kind;                                // enum FbTaskKind (include/flybody_b200.h)
   int root_qadr, root_vadr, ghost_qadr, ghost_vadr, root_body, user_col /* action column of the beat-frequency action, -1: none */;
   float ghost_offset[3], dt, time_limit, term_com, term_linvel, term_angvel, term_qacc, term_height;
-  int velocimeter_adr, gyro_adr, com_body, episode_steps, ref_len, obs_refdisp_off, obs_refquat_off;
+  int velocimeter_adr, gyro_adr, com_body, ref_len, obs_refdisp_off, obs_refquat_off;
   const float *reset_qpos, *ref_qpos /*[ref_len][7]*/, *ref_qvel /*[ref_len][6]*/;
   int n_noise; const int* noise_qadr; float noise_amp; unsigned seed;
   int n_wing; const int *wing_qadr, *wing_vadr, *wing_ctrl;
@@ -182,12 +176,12 @@ struct DevTask {
   float wb_base_freq, wb_rel_range, wb_rate, com_offset[3];
   // FB_TASK_VISION (vision_guided_flight): ranges of the per-episode draws, hover pose, terrain bank and the env's own heightfield buffers
   float th_rng[2], ts_rng[2], x_rng[2], y_rng[2], hover_quat[4], target_zaxis[3]; int fatal;
-  int n_bank, hf_nrow, hf_ncol, hf_ncm; float hf_half, hf_zoff;
+  int n_bank, hf_nrow, hf_ncol, hf_ncm; float hf_half;
   const float *bank, *bank_hmax, *bank_cmax; float *hf_data, *hf_hmax, *hf_cmax;
   float* target;                           // [N][2] target height, target speed of the running episode
   int trench_cap; const float *trench_x, *trench_y; const int* trench_len; int* pick;   // 'trench' arenas: centre line per bank terrain; the env's terrain
   // FB_TASK_WALK / FB_TASK_FLIGHT with ref_bank (dataset): trajectory bank [rows][rbank_w] (fb_ref_bank / fb_ref_bank_wide), picks, the env's reference slot
-  int ref_bank, n_traj, n_pick, randomize_start, start_margin, max_episode_rows, future_steps, slot_len, rbank_w;
+  int ref_bank, n_pick, randomize_start, start_margin, max_episode_rows, future_steps, slot_len, rbank_w;
   const float* rbank; const int *traj_off, *traj_len, *pick_traj; float* slots /* [N][slot_len][7] */;
   int *ep_traj, *ep_start, *ep_row0, *ep_n;   // the running episode: trajectory, start step, bank row of its row 0, rows in use
   int* pin;                                // [N][3] has pin, trajectory, start step of the next reset (fb_task_ref_pick)
@@ -215,4 +209,3 @@ struct DevTask {
 #else
 #define FB_FLAG_OR(bit) (AT(d.flags, 0) |= (bit))
 #endif
-static inline int fb_pad32(int n) { return (n + 31) & ~31; }

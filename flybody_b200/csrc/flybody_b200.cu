@@ -61,7 +61,7 @@ struct FbSim {
   std::vector<void*> allocs;
   std::vector<void*> obs_scope, task_scope;   // device buffers of the current observation / task program: freed when the program is replaced
   std::vector<void*> applied_scope;           // qfrc_applied / xfrc_applied: freed by fb_clear_applied
-  std::vector<int> h_dof_parent, h_dof_Madr, h_body_lastdof, h_geom_bodyid;
+  std::vector<int> h_dof_parent, h_dof_Madr;
   std::vector<double> h_qpos0;
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
@@ -85,13 +85,13 @@ struct FbSim {
 };
 
 static size_t slice_bytes(size_t fixed, size_t dyn_floats) { return ((((fixed + 15) & ~(size_t)15) + dyn_floats * sizeof(float)) + 15) & ~(size_t)15; }
-// kernel = sequence of stages for one env.  Ph<f>: per-lane phase f(m, d, sh, e, 0, y), a warp barrier follows;
+// kernel = sequence of stages for one env.  Ph<f>: per-lane phase f(m, d, sh, e, y), a warp barrier follows;
 // Wf<f>: warp function f(m, d, sh, e) written with WPAR sections (its own barriers inside).
 template <auto F> struct Ph {
 #ifdef __CUDACC__
-  template <typename Sh> static __device__ __forceinline__ void run(const DevModel& m, const DevData& d, Sh& sh, int e, int y) { F(m, d, sh, e, 0, y); }
+  template <typename Sh> static __device__ __forceinline__ void run(const DevModel& m, const DevData& d, Sh& sh, int e, int y) { F(m, d, sh, e, y); }
 #endif
-  template <typename Sh> static void emu(const DevModel& m, const DevData& d, Sh& sh, int e) { for (int y = 0; y < FB_NY; y++) F(m, d, sh, e, 0, y); }
+  template <typename Sh> static void emu(const DevModel& m, const DevData& d, Sh& sh, int e) { for (int y = 0; y < FB_NY; y++) F(m, d, sh, e, y); }
 };
 template <auto F> struct Wf {
 #ifdef __CUDACC__
@@ -214,10 +214,10 @@ static void fb_launch_warp(FbSim* s, int kind) {
 }
 #endif
 
-// lane == env kernels wrapped as single-phase functions
-FB_DEV void ph_reset_scatter(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { kreset_scatter(m, d, e, y); }
-FB_DEV void ph_scatter(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { kscatter(m, d, e, y); }
-FB_DEV void ph_clear_hold(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { kclear_hold(m, d, e, y); }
+// per-env kernels wrapped as single-phase functions
+FB_DEV void ph_reset_scatter(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kreset_scatter(m, d, e, y); }
+FB_DEV void ph_scatter(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kscatter(m, d, e, y); }
+FB_DEV void ph_clear_hold(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kclear_hold(m, d, e, y); }
 // heightfield contacts: DevHf travels in its own kernel (not in DevModel / DevData: the step kernels of models without a
 // heightfield keep their parameter layout)
 #ifndef FB_EMU
@@ -237,16 +237,16 @@ static void launch_hfield(FbSim* s) {
 #endif
   s->launches++;
 }
-FB_DEV void ph_task_reset(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset(m, d, e, y); }
-FB_DEV void ph_task_reset2(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset2(m, d, e, y); }
-FB_DEV void ph_task_reset3(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset3(m, d, e, y); }
-FB_DEV void ph_task_reset4(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset4(m, d, e, y); }
-FB_DEV void ph_task_reset5(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reset5(m, d, e, y); }
-FB_DEV void ph_task_reward(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_reward(m, d, e, y); }
-FB_DEV void ph_task_before(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_before(m, d, e, y); }
-FB_DEV void ph_task_commit(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_commit(m, d, e, y); }
-FB_DEV void ph_task_after(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { ktask_after(m, d, e, y); }
-FB_DEV void ph_pack(const DevModel& m, const DevData& d, ShNone&, int e, int, int y) { kpack(m, d, e, y, d.nsub_done > 0 ? 1.0f / d.nsub_done : 1.0f); ktaskobs(m, d, e, y); }
+FB_DEV void ph_task_reset(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reset(m, d, e, y); }
+FB_DEV void ph_task_reset2(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reset2(m, d, e, y); }
+FB_DEV void ph_task_reset3(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reset3(m, d, e, y); }
+FB_DEV void ph_task_reset4(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reset4(m, d, e, y); }
+FB_DEV void ph_task_reset5(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reset5(m, d, e, y); }
+FB_DEV void ph_task_reward(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reward(m, d, e, y); }
+FB_DEV void ph_task_before(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_before(m, d, e, y); }
+FB_DEV void ph_task_commit(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_commit(m, d, e, y); }
+FB_DEV void ph_task_after(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_after(m, d, e, y); }
+FB_DEV void ph_pack(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kpack(m, d, e, y, d.nsub_done > 0 ? 1.0f / d.nsub_done : 1.0f); ktaskobs(m, d, e, y); }
 // Smooth dynamics in half-solve form: with M = L^T D L and u = L^-T qfrc_smooth,
 //   J qacc_smooth = Z (D^-1/2 u)          (Z = D^-1/2 L^-T J^T, rows written by the projection kernel)
 //   qacc          = L^-1 (D^-1 u + D^-1/2 Z^T f)
@@ -376,13 +376,12 @@ static int build_model(FbSim* s, const FbModel* h) {
   std::vector<int> ladr, lnum, lbody, lr;
   for (int l = 0; l < nlist; l++) { ladr.push_back((int)lbody.size()); lnum.push_back((int)lists[l].size()); lbody.insert(lbody.end(), lists[l].begin(), lists[l].end()); lr.push_back(lroot[l] < 0 ? 0 : lroot[l]); }
   m.nroot = (int)roots.size(); m.nlist = nlist;
-  { // factorisation order of each list: bodies in reverse, dofs in reverse
-    std::vector<int> dadr, dnum, dl; int mx = 0;
-    for (int l = 0; l < nlist; l++) { dadr.push_back((int)dl.size()); int c = 0;
-      for (int bi = (int)lists[l].size() - 1; bi >= 0; bi--) { int bb = lists[l][bi]; for (int kk = h->body_dofnum[bb] - 1; kk >= 0; kk--) { dl.push_back(h->body_dofadr[bb] + kk); c++; } }
-      dnum.push_back(c); mx = std::max(mx, c); }
-    m.list_dofadr = up(s, dadr); m.list_ndof = up(s, dnum); m.list_dof = up(s, dl); m.max_list_ndof = mx;
-  }
+  // the dofs of each list in factorisation order (bodies in reverse, dofs in reverse): list l's are dl[dadr[l] .. dadr[l] + dnum[l]);
+  // dof_list: the list a dof belongs to, -1 for root dofs
+  std::vector<int> dadr, dnum, dl, dof_list(nv, -1);
+  for (int l = 0; l < nlist; l++) { dadr.push_back((int)dl.size()); int c = 0;
+    for (int bi = (int)lists[l].size() - 1; bi >= 0; bi--) { int bb = lists[l][bi]; for (int kk = h->body_dofnum[bb] - 1; kk >= 0; kk--) { dl.push_back(h->body_dofadr[bb] + kk); dof_list[h->body_dofadr[bb] + kk] = l; c++; } }
+    dnum.push_back(c); m.max_list_ndof = std::max(m.max_list_ndof, c); }
   m.root_body = up(s, roots); m.list_adr = up(s, ladr); m.list_num = up(s, lnum); m.list_body = up(s, lbody); m.list_root = up(s, lr);
   m.body_isroot = up(s, isroot);
   { // bodies the acceleration-stage sensors need: force sensors read the subtree sum at the site's body;
@@ -395,11 +394,9 @@ static int build_model(FbSim* s, const FbModel* h) {
     sacc[0] = 0;
     m.body_sensacc = up(s, sacc); m.body_sensfrc = up(s, sfrc);
   }
-  // geoms / sites per body (both are stored in body order by the compiler)
-  std::vector<int> gadr(nb, 0), gnum(nb, 0), sadr(nb, 0), snum(nb, 0);
-  for (int g = 0; g < m.ngeom; g++) { int b = h->geom_bodyid[g]; if (gnum[b] == 0) gadr[b] = g; gnum[b]++; if (g > 0 && h->geom_bodyid[g] < h->geom_bodyid[g - 1]) { s->err = "geoms not in body order"; return -3; } }
-  for (int t = 0; t < m.nsite; t++) { int b = h->site_bodyid[t]; if (snum[b] == 0) sadr[b] = t; snum[b]++; if (t > 0 && h->site_bodyid[t] < h->site_bodyid[t - 1]) { s->err = "sites not in body order"; return -3; } }
-  m.body_geomadr = up(s, gadr); m.body_geomnum = up(s, gnum); m.body_siteadr = up(s, sadr); m.body_sitenum = up(s, snum);
+  // geoms and sites come in body order (the compiler stores them so)
+  for (int g = 1; g < m.ngeom; g++) if (h->geom_bodyid[g] < h->geom_bodyid[g - 1]) { s->err = "geoms not in body order"; return -3; }
+  for (int t = 1; t < m.nsite; t++) if (h->site_bodyid[t] < h->site_bodyid[t - 1]) { s->err = "sites not in body order"; return -3; }
   // dof helpers
   std::vector<int> subend(nv), depth(nv), disroot(nv), chainlen(nv);
   for (int i = 0; i < nv; i++) subend[i] = i;
@@ -412,12 +409,7 @@ static int build_model(FbSim* s, const FbModel* h) {
     depth[i] = disroot[i] ? (i - h->body_dofadr[h->dof_bodyid[i]]) : nonroot;
   }
   { std::vector<int> anc(h->nM, -1); for (int i = 0; i < nv; i++) { int t = 0; for (int j = i; j >= 0; j = h->dof_parentid[j], t++) anc[h->dof_Madr[i] + t] = j; } m.dof_anc = up(s, anc); }
-  { // shared-memory slot of the t-th ancestor for the triangular solves: root dofs map to the list's private accumulators
-    std::vector<int> dof_list(nv, -1);
-    for (int l = 0; l < nlist; l++) for (int bb : lists[l]) for (int kk = 0; kk < h->body_dofnum[bb]; kk++) dof_list[h->body_dofadr[bb] + kk] = l;
-    std::vector<int> slot(h->nM, 0);
-    for (int i = 0; i < nv; i++) { int t = 0; for (int j = i; j >= 0; j = h->dof_parentid[j], t++) slot[h->dof_Madr[i] + t] = (disroot[j] && dof_list[i] >= 0) ? nv + FB_ROOTD * dof_list[i] + depth[j] : j; }
-    m.dof_ancslot = up(s, slot);
+  { // the root a list dof hangs off, and which roots have lists
     std::vector<int> rootidx(nv, -1), haslists(roots.size(), 0);
     for (int i = 0; i < nv; i++) if (dof_list[i] >= 0) { rootidx[i] = lr[dof_list[i]]; haslists[lr[dof_list[i]]] = 1; }
     m.dof_rootidx = up(s, rootidx); m.root_haslists = up(s, haslists);
@@ -433,37 +425,30 @@ static int build_model(FbSim* s, const FbModel* h) {
     m.dof_lca = up(s, lca);
   }
   { std::vector<int> adh(nb, -1); for (int i = 0; i < h->nu; i++) if (h->actuator_trntype[i] == FB_TRN_BODY) adh[h->actuator_trnid[i]] = i; m.body_adhesion = up(s, adh); }
-  { // packed headers of the lock-step sweeps (see fb_tree.h) and the row address of every ancestor entry
+  { // packed headers of the lock-step sweeps (see fb_tree.h), deepest-first (a) and shallowest-first (c)
     if (h->nM >= 4096 || nv >= 256) { s->err = "model too large for the packed sweep headers (nM < 4096, nv < 256)"; return -3; }
     std::vector<unsigned> ha((size_t)FB_NY * std::max(m.max_list_ndof, 1), 0xffffffffu), hc(ha);
-    std::vector<int> dadr_h, dnum_h, dl_h;      // rebuild the per-list dof order exactly as above
-    for (int l = 0; l < nlist; l++) { dadr_h.push_back((int)dl_h.size()); int c = 0;
-      for (int bi = (int)lists[l].size() - 1; bi >= 0; bi--) { int bb = lists[l][bi]; for (int kk = h->body_dofnum[bb] - 1; kk >= 0; kk--) { dl_h.push_back(h->body_dofadr[bb] + kk); c++; } }
-      dnum_h.push_back(c); }
     auto pack = [&](int k) -> unsigned {
       if (chainlen[k] >= 64 || depth[k] >= 64) return 0xfffffffeu;
       return (unsigned)h->dof_Madr[k] | ((unsigned)chainlen[k] << 12) | ((unsigned)depth[k] << 18) | ((unsigned)k << 24); };
-    for (int l = 0; l < nlist && FB_FSUB * l + FB_FSUB <= FB_NY; l++) for (int st = 0; st < dnum_h[l]; st++) for (int u = 0; u < FB_FSUB; u++) {
-      unsigned a = pack(dl_h[dadr_h[l] + st]), c = pack(dl_h[dadr_h[l] + dnum_h[l] - 1 - st]);
+    for (int l = 0; l < nlist && FB_FSUB * l + FB_FSUB <= FB_NY; l++) for (int st = 0; st < dnum[l]; st++) for (int u = 0; u < FB_FSUB; u++) {
+      unsigned a = pack(dl[dadr[l] + st]), c = pack(dl[dadr[l] + dnum[l] - 1 - st]);
       if (a == 0xfffffffeu || c == 0xfffffffeu) { s->err = "chain too long for the packed sweep headers"; return -3; }
       ha[(size_t)st * FB_NY + FB_FSUB * l + u] = a; hc[(size_t)st * FB_NY + FB_FSUB * l + u] = c; }
-    m.step_hdr_a = up(s, ha); m.step_hdr_c = up(s, hc);
-    { // the same headers + ancestor slots as bytes, in one blob that the smooth / finish kernels copy into shared memory
+    { // the headers + ancestor slots as bytes, in one blob that the smooth / finish kernels copy into shared memory
       if (nv + FB_ROOTD * nlist >= 256) { s->err = "too many dofs for byte-sized sweep slots"; return -3; }
       const int H = (int)ha.size(), nmp = (h->nM + 3) & ~3;
       std::vector<unsigned> blob((((size_t)2 * H + 2 * nmp / 4) + 3) & ~(size_t)3, 0u);       // whole 16-byte units: the warps' slices follow
       for (int i = 0; i < H; i++) { blob[i] = ha[i]; blob[H + i] = hc[i]; }
       unsigned char* b8 = reinterpret_cast<unsigned char*>(blob.data() + 2 * H);
-      std::vector<int> dof_list2(nv, -1);
-      for (int l = 0; l < nlist; l++) for (int bb : lists[l]) for (int kk = 0; kk < h->body_dofnum[bb]; kk++) dof_list2[h->body_dofadr[bb] + kk] = l;
       for (int i = 0; i < nv; i++) { int t = 0; for (int j = i; j >= 0; j = h->dof_parentid[j], t++) {
-          int slot = (disroot[j] && dof_list2[i] >= 0) ? nv + FB_ROOTD * dof_list2[i] + depth[j] : j;
+          // shared-memory slot of the t-th ancestor: root dofs map to the list's private accumulators
+          int slot = (disroot[j] && dof_list[i] >= 0) ? nv + FB_ROOTD * dof_list[i] + depth[j] : j;
           b8[h->dof_Madr[i] + t] = (unsigned char)slot; b8[nmp + h->dof_Madr[i] + t] = (unsigned char)j; } }
       m.tsolve_blob = up(s, blob); m.ts_hdr_words = H; m.ts_nm_pad = nmp; m.ts_blob_words = (int)blob.size();
     }
-    std::vector<int> ancadr(h->nM, 0);
+    std::vector<int> ancadr(h->nM, 0);      // row address (dof_Madr) of the ancestor an entry of the packed factor belongs to
     for (int i = 0; i < nv; i++) { int t = 0; for (int j = i; j >= 0; j = h->dof_parentid[j], t++) ancadr[h->dof_Madr[i] + t] = h->dof_Madr[j]; }
-    m.M_ancadr = up(s, ancadr);
     { // balanced schedule of the factorisation sweeps (fb_tree.h: factor_step_sched): the rank-1 update of one ancestor row by the
       // step's dof of one list is a work item (cost = its length + a constant); the items of a step touch different rows, so they
       // are dealt to the 32 lanes longest-first onto the least loaded lane instead of 3 fixed lanes per list
@@ -473,8 +458,8 @@ static int build_model(FbSim* s, const FbModel* h) {
         struct It { unsigned x, y; int cost; };
         std::vector<It> its;
         for (int l = 0; l < nlist; l++) {
-          if (st >= dnum_h[l]) continue;
-          const int k = dl_h[dadr_h[l] + st], adrk = h->dof_Madr[k], len = chainlen[k];
+          if (st >= dnum[l]) continue;
+          const int k = dl[dadr[l] + st], adrk = h->dof_Madr[k], len = chainlen[k];
           for (int t = 1; t < 1 + depth[k]; t++) its.push_back({(unsigned)adrk | ((unsigned)t << 12) | ((unsigned)(len - t) << 18), (unsigned)ancadr[adrk + t], len - t + 6});
         }
         std::stable_sort(its.begin(), its.end(), [](const It& a, const It& b) { return a.cost > b.cost; });
@@ -491,9 +476,9 @@ static int build_model(FbSim* s, const FbModel* h) {
     }
   }
   { std::vector<float> mdamp(h->nM, 0.0f); for (int i = 0; i < nv; i++) mdamp[h->dof_Madr[i]] = (float)h->dof_damping[i]; m.M_damp = up(s, mdamp); }
-  m.dof_subend = up(s, subend); m.dof_depth = up(s, depth); m.dof_isroot = up(s, disroot); m.dof_chainlen = up(s, chainlen);
+  m.dof_subend = up(s, subend); m.dof_depth = up(s, depth); m.dof_chainlen = up(s, chainlen);
   // plain copies
-  m.body_parentid = upi(s, h->body_parentid, nb); m.body_rootid = upi(s, h->body_rootid, nb);
+  m.body_parentid = upi(s, h->body_parentid, nb);
   m.body_jntadr = upi(s, h->body_jntadr, nb); m.body_jntnum = upi(s, h->body_jntnum, nb);
   m.body_dofadr = upi(s, h->body_dofadr, nb); m.body_dofnum = upi(s, h->body_dofnum, nb);
   m.body_lastdof = upi(s, h->body_lastdof, nb); m.body_fluid_ellipsoid = upi(s, h->body_fluid_ellipsoid, nb);
@@ -527,17 +512,6 @@ static int build_model(FbSim* s, const FbModel* h) {
     }
     m.pair_info = up(s, pi); m.pair_rsum = up(s, rs);
   }
-  {  // chunk boundaries: plane pairs produce most contacts (up to 4 each), weight them 16x
-    m.nchunk = FB_MAXCHUNK;
-    std::vector<int> w(m.npair); long tot = 0;
-    for (int k = 0; k < m.npair; k++) { w[k] = (h->geom_type[h->pair_geom1[k]] == FB_GEOM_PLANE) ? 16 : 1; tot += w[k]; }
-    std::vector<int> cs(m.nchunk + 1, m.npair); cs[0] = 0;
-    long acc = 0; int c = 1;
-    for (int k = 0; k < m.npair && c < m.nchunk; k++) { acc += w[k]; if (acc * m.nchunk >= tot * c) { cs[c++] = k + 1; } }
-    for (; c <= m.nchunk; c++) cs[c] = m.npair;
-    m.chunk_start = up(s, cs);
-
-  }
   m.fluid_bodyid = upi(s, h->fluid_bodyid, m.nfluid); m.fluid_pos = upf3(s, h->fluid_pos, m.nfluid);
   m.fluid_quat = upf(s, h->fluid_quat, 4 * m.nfluid); m.fluid_size = upf3(s, h->fluid_size, m.nfluid); m.fluid_coef = upf(s, h->fluid_coef, 12 * m.nfluid);
   m.site_bodyid = upi(s, h->site_bodyid, m.nsite); m.site_type = upi(s, h->site_type, m.nsite);
@@ -554,7 +528,6 @@ static int build_model(FbSim* s, const FbModel* h) {
   m.sensor_adr = upi(s, h->sensor_adr, m.nsensor); m.sensor_dim = upi(s, h->sensor_dim, m.nsensor);
   s->h_dof_parent.assign(h->dof_parentid, h->dof_parentid + nv); s->h_dof_Madr.assign(h->dof_Madr, h->dof_Madr + nv);
   s->h_qpos0.assign(h->qpos0, h->qpos0 + m.nq);
-  s->h_body_lastdof.assign(h->body_lastdof, h->body_lastdof + nb); s->h_geom_bodyid.assign(h->geom_bodyid, h->geom_bodyid + ng);
   return 0;
 }
 
@@ -581,7 +554,7 @@ static int alloc_data(FbSim* s, int N) {
   FA(tmp_con, 13 * 4 * FB_MAXCAND) IA(tmp_geom, 2 * 4 * FB_MAXCAND)
   IA(nefc, 1) IA(efc_type, FB_MAXEFC) IA(efc_id, FB_MAXEFC)
   FA(efc_pos, FB_MAXEFC) FA(efc_margin, FB_MAXEFC) FA(efc_D, FB_MAXEFC) FA(efc_R, FB_MAXEFC) FA(efc_K, FB_MAXEFC) FA(efc_B, FB_MAXEFC)
-  FA(efc_imp, FB_MAXEFC) FA(efc_aref, FB_MAXEFC) FA(efc_b, FB_MAXEFC) FA(efc_force, FB_MAXEFC) FA(efc_jarws, FB_MAXEFC)
+  FA(efc_imp, FB_MAXEFC) FA(efc_aref, FB_MAXEFC) FA(efc_b, FB_MAXEFC) FA(efc_force, FB_MAXEFC)
   IA(efc_la, FB_MAXEFC) IA(efc_lb, FB_MAXEFC) IA(efc_key, FB_MAXEFC) IA(prev_key, FB_MAXEFC) IA(prev_n, 1) FA(prev_lam, FB_MAXEFC)
   FA(sensordata, m.nsensordata + 1) FA(sensor_sum, m.nsensordata + 1) IA(flags, 1) IA(niter, 1) IA(hold, 1)
   // large, sparsely touched arrays last
@@ -1259,7 +1232,7 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   for (int i = 0; i < 3; i++) { t.ghost_offset[i] = p->ghost_offset[i]; t.com_offset[i] = p->com_offset[i]; }
   t.dt = p->control_timestep; t.time_limit = p->time_limit; t.term_com = p->terminal_com_dist; t.term_linvel = p->terminal_linvel;
   t.term_angvel = p->terminal_angvel; t.term_qacc = p->terminal_qacc; t.term_height = p->terminal_height;
-  t.velocimeter_adr = p->velocimeter_adr; t.gyro_adr = p->gyro_adr; t.com_body = p->com_body; t.episode_steps = p->episode_steps;
+  t.velocimeter_adr = p->velocimeter_adr; t.gyro_adr = p->gyro_adr; t.com_body = p->com_body;
   t.ref_len = p->ref_len; t.obs_refdisp_off = p->obs_refdisp_off; t.obs_refquat_off = p->obs_refquat_off;
   auto upf32 = [&](const float* src, size_t n) { std::vector<float> v(src, src + n); return up(s, v); };
   auto upi32 = [&](const int32_t* src, size_t n) { std::vector<int> v(src, src + n); return up(s, v); };
@@ -1280,7 +1253,7 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   t.uniform = dalloc<float>(s, (size_t)8 * Np); t.wb_freq = dalloc<float>(s, Np); t.out = dalloc<float>(s, (size_t)4 * Np);
   t.ep_steps = dalloc<int>(s, Np);
   if (bank) {          // episode lengths are set per env by each reset
-    t.ref_bank = 1; t.n_traj = (int)s->rbank_len.size(); t.rbank = s->rbank_dev; t.traj_off = s->rbank_off_dev; t.traj_len = s->rbank_len_dev; t.rbank_w = s->rbank_w;
+    t.ref_bank = 1; t.rbank = s->rbank_dev; t.traj_off = s->rbank_off_dev; t.traj_len = s->rbank_len_dev; t.rbank_w = s->rbank_w;
     t.n_pick = p->n_pick; t.pick_traj = upi32(p->pick_traj, p->n_pick); t.randomize_start = p->randomize_start ? 1 : 0; t.start_margin = p->start_margin;
     t.max_episode_rows = p->max_episode_rows; t.future_steps = p->future_steps; t.slots = s->ref_slots; t.slot_len = s->ref_slot_len;
     t.ep_traj = dalloc<int>(s, Np); t.ep_start = dalloc<int>(s, Np); t.ep_row0 = dalloc<int>(s, Np); t.ep_n = dalloc<int>(s, Np); t.pin = dalloc<int>(s, (size_t)3 * Np);
@@ -1303,7 +1276,7 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
     for (int i = 0; i < 4; i++) t.hover_quat[i] = p->hover_quat[i];
     for (int i = 0; i < 3; i++) t.target_zaxis[i] = p->target_zaxis[i];
     t.fatal = p->floor_contacts_fatal;
-    t.n_bank = s->bank_n; t.hf_nrow = s->hf_nrow; t.hf_ncol = s->hf_ncol; t.hf_ncm = s->hf_nbr * s->hf_nbc; t.hf_half = s->hf.size[0]; t.hf_zoff = 0.0f;
+    t.n_bank = s->bank_n; t.hf_nrow = s->hf_nrow; t.hf_ncol = s->hf_ncol; t.hf_ncm = s->hf_nbr * s->hf_nbc; t.hf_half = s->hf.size[0];
     t.bank = s->bank_dev; t.bank_hmax = s->bank_hmax_dev; t.bank_cmax = s->bank_cmax_dev; t.hf_data = s->hfield_dev; t.hf_hmax = s->hmax_dev; t.hf_cmax = s->cmax_dev;
     t.target = dalloc<float>(s, (size_t)2 * Np); t.pick = dalloc<int>(s, Np);
     t.trench_cap = 0; t.trench_x = t.trench_y = nullptr; t.trench_len = nullptr;
