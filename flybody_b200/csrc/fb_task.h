@@ -44,18 +44,24 @@ FB_DEV float tk_hf_nearest(const DevTask& t, const float* h, float x, float y) {
   return h[(size_t)yi * t.hf_ncol + xi];
 }
 FB_DEV float tk_draw(const DevTask& t, int e, int episode, int k) { return t.has_uniform[e] ? t.uniform[8 * e + k] : tk_u01(t, e, episode, 16 + k); }
-// initialize_episode_mjcf + initialize_episode of the vision task (vision_flight.py:97-139): targets, start point, wing-beat phase, a
-// terrain of the bank copied into the env's heightfield (all lanes), the fly in its hover pose `target_height` above the terrain at the
-// target speed.  Draw order: target height, target speed, x, y, wing-beat phase, terrain.
-FB_DEV void ktask_reset_vision(const DevModel& m, const DevData& d, const DevTask& t, int e, int y, int episode) {
-  int pick = (int)(tk_draw(t, e, episode, 5) * (float)t.n_bank); pick = pick < 0 ? 0 : (pick >= t.n_bank ? t.n_bank - 1 : pick);
+// terrain `pick` of the bank into the env's heightfield, block maxima and highest point (all lanes): a reset's, and a loaded state row's
+FB_DEV void tk_terrain_copy(const DevTask& t, int e, int y, int pick) {
   const size_t cells = (size_t)t.hf_nrow * t.hf_ncol;
   const float* src = t.bank + cells * pick;
   float* dst = t.hf_data + cells * e;
   for (size_t i = y; i < cells; i += FB_NY) dst[i] = src[i];
   for (int i = y; i < t.hf_ncm; i += FB_NY) t.hf_cmax[(size_t)t.hf_ncm * e + i] = t.bank_cmax[(size_t)t.hf_ncm * pick + i];
+  if (y == 0) t.hf_hmax[e] = t.bank_hmax[pick];
+}
+// initialize_episode_mjcf + initialize_episode of the vision task (vision_flight.py:97-139): targets, start point, wing-beat phase, a
+// terrain of the bank copied into the env's heightfield (all lanes), the fly in its hover pose `target_height` above the terrain at the
+// target speed.  Draw order: target height, target speed, x, y, wing-beat phase, terrain.
+FB_DEV void ktask_reset_vision(const DevModel& m, const DevData& d, const DevTask& t, int e, int y, int episode) {
+  int pick = (int)(tk_draw(t, e, episode, 5) * (float)t.n_bank); pick = pick < 0 ? 0 : (pick >= t.n_bank ? t.n_bank - 1 : pick);
+  const float* src = t.bank + (size_t)t.hf_nrow * t.hf_ncol * pick;
+  tk_terrain_copy(t, e, y, pick);
   if (y != 0) return;
-  t.hf_hmax[e] = t.bank_hmax[pick]; t.pick[e] = pick;
+  t.pick[e] = pick;
   const float th = t.th_rng[0] + (t.th_rng[1] - t.th_rng[0]) * tk_draw(t, e, episode, 0), ts = t.ts_rng[0] + (t.ts_rng[1] - t.ts_rng[0]) * tk_draw(t, e, episode, 1);
   const float x = t.x_rng[0] + (t.x_rng[1] - t.x_rng[0]) * tk_draw(t, e, episode, 2), yy = t.y_rng[0] + (t.y_rng[1] - t.y_rng[0]) * tk_draw(t, e, episode, 3);
   t.target[2 * e] = th; t.target[2 * e + 1] = ts;

@@ -24,6 +24,7 @@
 #include "fb_render.h"
 #include "fb_hfield.h"
 #include "fb_task.h"
+#include "fb_state.h"
 
 #ifdef FB_EMU
 typedef int cudaStream_t_;
@@ -76,6 +77,11 @@ struct FbSim {
   DevEye eye; float* hfield_dev; float* hmax_dev; float* cmax_dev; int hf_nbr, hf_nbc; unsigned char* eye_out; size_t eye_bytes;   // eye cameras (fb_eye_program)
   DevTask task_host;                       // host copy of the device-side task program (its pointers are device pointers)
   float* stage; int* stage_i; size_t stage_cap, stage_icap; unsigned ws_slot;
+  // state bank (fb_state_*): [st_slots][st_row] rows of the layout in st_segs; dropped (st_stale) when a program that shapes the layout is replaced
+  unsigned* st_bank = nullptr; int st_slots = 0; unsigned st_row = 0; bool st_stale = false; uint64_t st_sig = 0;
+  StSeg* st_segs_dev = nullptr; int st_nseg = 0, st_hold_off = 0; std::vector<void*> st_scope;
+  std::vector<char> st_written;            // per slot: 0 never written, 1 written, 2 written while an env may be held for its reset
+  int* st_ids_dev = nullptr; int st_ids_cap = 0;
 #ifndef FB_EMU
   cudaStream_t stream; cudaEvent_t ev0, ev1;
   struct StepGraph { cudaGraphExec_t exec; bool seen, failed; int n_sub; long long launches; DevData d; DevModel m; };
@@ -280,6 +286,57 @@ static void launch_step1(FbSim* s) {
   if (s->hf_on) launch_hfield(s);              // heightfield contacts join the contact list before the constraint rows are built
   fb_launch<ShCon, FB_ST_PROJ>(s, K_PROJ, dyn_proj(s->m));
   fb_launch<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m));
+}
+// The position / velocity stage for a list of envs (fb_state_load recomputes what a state row does not carry), through the stage
+// functions of the step kernels.  One env per block: the collision stage pools the jobs of a block's envs on warp 0 and takes them
+// to be consecutive envs, so a listed env runs as warp 0 of a block whose other slices report no jobs.
+#ifndef FB_EMU
+template <typename Sh, typename... St>
+__global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_run_ids(DevModel m, DevData d, int slice, const int* ids) {
+  extern __shared__ __align__(16) unsigned char fb_smem[];
+  for (int i = threadIdx.x; i < (FB_WPB - 1) * slice / 4; i += 32) reinterpret_cast<unsigned*>(fb_smem + slice)[i] = 0u;
+  const int e = ids[blockIdx.x], y = threadIdx.x;
+  Sh& sh = *reinterpret_cast<Sh*>(fb_smem);
+  set_slice(sh, slice); set_prog(sh, m.tsolve_blob); __syncwarp();
+  ((St::run(m, d, sh, e, y), __syncwarp()), ...);
+}
+__global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_hf_kernel_ids(      // (the bounds of fb_hf_kernel: the same code)
+DevModel m, DevData d, DevHf p, const int* ids) {
+  const int e = ids[blockIdx.x];
+  khf_narrow(m, d, p, e, threadIdx.x); __syncwarp();
+  khf_append(m, d, p, e, threadIdx.x);
+}
+#endif
+template <typename Sh, typename... St>
+static void fb_launch_ids(FbSim* s, size_t dyn_floats, const int* ids_dev, const int* ids_host, int n) {
+  const size_t slice = slice_bytes(sizeof(Sh), dyn_floats);
+#ifndef FB_EMU
+  const size_t bytes = slice * FB_WPB; (void)ids_host;
+  static size_t configured = 0;
+  if (bytes > configured) { cudaFuncSetAttribute(fb_run_ids<Sh, St...>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); configured = bytes; }
+  fb_run_ids<Sh, St...><<<n, dim3(32, 1), bytes, s->stream>>>(s->m, s->d, (int)slice, ids_dev);
+#else
+  (void)ids_dev;
+  std::vector<unsigned char> buf(slice, 0);
+  Sh& sh = *reinterpret_cast<Sh*>(buf.data());
+  set_prog(sh, s->m.tsolve_blob);
+  for (int k = 0; k < n; k++) (St::emu(s->m, s->d, sh, ids_host[k]), ...);
+#endif
+  s->launches++;
+}
+static void launch_step1_ids(FbSim* s, const int* ids_dev, const int* ids_host, int n) {
+  fb_launch_ids<ShTree, FB_ST_POS>(s, dyn_pos(s->m), ids_dev, ids_host, n);
+  fb_launch_ids<ShCol, FB_ST_COL>(s, dyn_col(s->m), ids_dev, ids_host, n);
+  if (s->hf_on) {
+#ifndef FB_EMU
+    fb_hf_kernel_ids<<<n, 32, 0, s->stream>>>(s->m, s->d, s->hf, ids_dev);
+#else
+    for (int k = 0; k < n; k++) { const int e = ids_host[k]; for (int y = 0; y < FB_NY; y++) khf_narrow(s->m, s->d, s->hf, e, y); for (int y = 0; y < FB_NY; y++) khf_append(s->m, s->d, s->hf, e, y); }
+#endif
+    s->launches++;
+  }
+  fb_launch_ids<ShCon, FB_ST_PROJ>(s, dyn_proj(s->m), ids_dev, ids_host, n);
+  fb_launch_ids<ShTree, FB_ST_VEL>(s, dyn_vel(s->m), ids_dev, ids_host, n);
 }
 static void launch_step2(FbSim* s, bool integrate) {
   s->d.do_integrate = integrate ? 1 : 0;     // read by the solve (warm-start bookkeeping) and the finish kernel
@@ -631,6 +688,13 @@ static int sync_stream(FbSim* s) {
   return 0;
 }
 
+// The state bank's rows follow the handle's arrays: whatever replaces an observation / task program, the reference slots or the
+// applied-force arrays drops the bank (the stream is idle: the callers synchronise first); fb_state_bank lays it out again.
+static void state_drop(FbSim* s) {
+  if (!s->st_bank) return;
+  scope_free(s, s->st_scope);
+  s->st_bank = nullptr; s->st_segs_dev = nullptr; s->st_slots = 0; s->st_written.clear(); s->st_stale = true;
+}
 // applied forces (FB_QFRC_APPLIED, FB_XFRC_APPLIED): compact device arrays [Np][n], both allocated zeroed on first use
 static float* applied_ptr(FbSim* s, int field, int* n) {
   *n = field == FB_QFRC_APPLIED ? s->m.nv : 6 * s->m.nbody;
@@ -639,6 +703,7 @@ static float* applied_ptr(FbSim* s, int field, int* n) {
 static int ensure_applied(FbSim* s) {
   if (s->d.qfrc_applied) return 0;
   if (sync_stream(s) != 0) return -2;
+  state_drop(s);
   const size_t mark = s->allocs.size();
   float* q = dalloc<float>(s, (size_t)s->d.Np * s->m.nv); float* x = dalloc<float>(s, (size_t)s->d.Np * 6 * s->m.nbody);
   s->applied_scope.assign(s->allocs.begin() + mark, s->allocs.end());
@@ -1003,6 +1068,7 @@ int fb_clear_applied(FbHandle s) {
   if (!s) return -1;
   if (!s->d.qfrc_applied) return 0;
   if (sync_stream(s) != 0) return -2;
+  state_drop(s);
   scope_free(s, s->applied_scope);
   s->d.qfrc_applied = nullptr; s->d.xfrc_applied = nullptr;
   return 0;
@@ -1140,6 +1206,7 @@ int fb_obs_program(FbHandle s, const FbObsProgram* p) {
   if (p->root_body <= 0 || p->root_body >= m.nbody) { s->err = "fb_obs_program: root body"; return -1; }
   // a replaced program's buffers are freed; the task program points into them (observation rows, per-env step inputs), so it goes too
   // and has to be uploaded again (fly_envs does: observation program, then task program)
+  state_drop(s);
   scope_free(s, s->task_scope); s->d.task = nullptr;
   scope_free(s, s->obs_scope);
   const size_t obs_mark = s->allocs.size();
@@ -1159,6 +1226,7 @@ int fb_obs_program(FbHandle s, const FbObsProgram* p) {
 int fb_ref_slots(FbHandle s, int slot_len) {
   if (!s || !s->d.tobs || slot_len <= 0) return -1;
   if (sync_stream(s) != 0) return -2;
+  if (!s->ref_slots || s->ref_slot_len != slot_len || !s->d.op_ref_slot) state_drop(s);
   if (!s->ref_slots || s->ref_slot_len != slot_len) {          // (re)allocate: one [slot_len][7] table per env
     if (s->ref_slots) {
       for (auto& a : s->allocs) if (a == s->ref_slots) { a = nullptr; break; }
@@ -1224,6 +1292,7 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   if ((p->kind == FB_TASK_FLIGHT || p->kind == FB_TASK_VISION) && (p->n_wing <= 0 || p->n_freq <= 0 || p->tab_len <= 0 || !p->wb_traj || !p->wb_phase || !p->wb_phase_mod || !p->wb_freqs || !p->wb_len)) { s->err = "fb_task_program: wing-beat tables missing"; return -1; }
   if (sync_stream(s) != 0) return -2;
   const DevModel& m = s->m; const int Np = s->d.Np;
+  state_drop(s);
   scope_free(s, s->task_scope); s->d.task = nullptr;
   const size_t task_mark = s->allocs.size();
   DevTask t; memset(&t, 0, sizeof(t));
@@ -1279,6 +1348,7 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
     t.n_bank = s->bank_n; t.hf_nrow = s->hf_nrow; t.hf_ncol = s->hf_ncol; t.hf_ncm = s->hf_nbr * s->hf_nbc; t.hf_half = s->hf.size[0];
     t.bank = s->bank_dev; t.bank_hmax = s->bank_hmax_dev; t.bank_cmax = s->bank_cmax_dev; t.hf_data = s->hfield_dev; t.hf_hmax = s->hmax_dev; t.hf_cmax = s->cmax_dev;
     t.target = dalloc<float>(s, (size_t)2 * Np); t.pick = dalloc<int>(s, Np);
+    { std::vector<int> none((size_t)Np, -1); h2d(t.pick, none.data(), sizeof(int) * none.size()); }      // no terrain yet (a reset, or a loaded state row, copies one)
     t.trench_cap = 0; t.trench_x = t.trench_y = nullptr; t.trench_len = nullptr;
     if (p->trench_cap > 0) {
       if (!p->trench_y || !p->trench_x || !p->trench_len) { s->err = "fb_task_program: trench centre lines missing"; return -1; }
@@ -1363,6 +1433,7 @@ int fb_hfield_bank(FbHandle s, int n_terrain, const float* heights) {
       cm[ncm * k + (size_t)br * s->hf_nbc + bc] = v;
     }
   }
+  if (s->bank_dev && s->d.task && s->task_host.kind == FB_TASK_VISION) state_drop(s);
   if (s->bank_dev) {      // a replaced bank is freed; a vision task program pointing at it has to be uploaded again
     std::vector<void*> old = {s->bank_dev, s->bank_hmax_dev, s->bank_cmax_dev};
     scope_free(s, old);
@@ -1393,6 +1464,7 @@ int fb_ref_bank_wide(FbHandle s, int n_traj, const int32_t* traj_len, int row_wi
     s->err = "fb_ref_bank: bank too large for the device's free memory"; return -4; }
 #endif
   if (sync_stream(s) != 0) return -2;
+  if (s->rbank_dev && s->d.task && s->task_host.ref_bank) state_drop(s);
   if (s->rbank_dev) {      // a replaced bank is freed; a dataset program drawing from it has to be uploaded again
     scope_free(s, s->rbank_scope);
     if (s->d.task && s->task_host.ref_bank) { scope_free(s, s->task_scope); s->d.task = nullptr; }
@@ -1602,6 +1674,202 @@ int fb_read_obs(FbHandle s, float* host_dst) {
 int fb_obs_ptr(FbHandle s, void** dev_ptr, int* floats_per_env) {
   if (!s || !dev_ptr || !floats_per_env) return -1;
   *dev_ptr = s->d.obs; *floats_per_env = s->d.obs_dim;
+  return 0;
+}
+
+}  // extern "C"
+
+// ---- state rows (fb_state_*): the batched stand-in for physics.get_state() / physics.set_state()
+// the row of the handle's current model, programs and applied-force arrays: segments in a fixed order, each on a 16-byte boundary
+static std::vector<StSeg> state_layout(FbSim* s, unsigned* row, uint64_t* sig, int* hold_off) {
+  const DevModel& m = s->m; const DevData& d = s->d;
+  std::vector<StSeg> v; int off = 0; uint64_t h = 1469598103934665603ull;
+  auto mix = [&](uint64_t x) { h = (h ^ x) * 1099511628211ull; };
+  auto add = [&](int id, const void* base, unsigned stride, int n, int bytes = 0) {
+    if (!base || n <= 0) return;
+    StSeg g; g.base = const_cast<void*>(base); g.stride = stride; g.n = n; g.off = off; g.bytes = bytes;
+    g.vec = (!bytes && stride % 4 == 0 && ((uintptr_t)base & 15) == 0) ? 1 : 0;
+    v.push_back(g); mix((uint64_t)id); mix((uint64_t)n);
+    off = (off + (bytes ? 1 : n) + 3) & ~3;
+  };
+  mix(1);                                    // layout version
+  add(1, d.qpos, d.rec, m.nq); add(2, d.qvel, d.rec, m.nv); add(3, d.act, d.rec, m.na); add(4, d.ctrl, d.rec, m.nu); add(5, d.qacc, d.rec, m.nv);
+  add(6, d.time, d.rec, 1); add(7, d.flags, d.rec, 1); add(8, d.niter, d.rec, 1);
+  *hold_off = off; add(9, d.hold, d.rec, 1);
+  add(10, d.prev_n, d.rec, 1); add(11, d.prev_key, d.rec, FB_MAXEFC); add(12, d.prev_lam, d.rec, FB_MAXEFC);
+  add(13, d.sensordata, d.rec, m.nsensordata); add(14, d.sensor_sum, d.rec, m.nsensordata);
+  add(15, d.obs, (unsigned)d.obs_dim, d.obs_dim);
+  if (d.tobs) { add(16, d.tobs, (unsigned)d.tobs_dim, d.tobs_dim); add(17, s->op_step_dev, 1, 1); add(18, s->op_first_dev, 1, 1, 1); }
+  if (d.op_ref_slot && s->ref_slots) add(19, s->ref_slots, (unsigned)(7 * s->ref_slot_len), 7 * s->ref_slot_len);
+  if (d.qfrc_applied) { add(20, d.qfrc_applied, (unsigned)m.nv, m.nv); add(21, d.xfrc_applied, (unsigned)(6 * m.nbody), 6 * m.nbody); }
+  mix(d.task ? (uint64_t)s->task_host.kind + 1 : 0); mix(d.task ? (uint64_t)s->task_host.ref_bank : 0);
+  if (d.task) {
+    const DevTask& t = s->task_host;
+    add(30, t.step, 1, 1); add(31, t.needs_reset, 1, 1); add(32, t.resetting, 1, 1); add(33, t.episode, 1, 1); add(34, t.ep_steps, 1, 1);
+    add(35, t.has_uniform, 1, 1); add(36, t.uniform, 8, 8); add(37, t.wb_idx, 1, 1); add(38, t.wb_pos, 1, 1); add(39, t.wb_freq, 1, 1);
+    add(40, t.out, 4, 4);
+    add(41, t.ep_traj, 1, 1); add(42, t.ep_start, 1, 1); add(43, t.ep_row0, 1, 1); add(44, t.ep_n, 1, 1); add(45, t.pin, 3, 3);
+    add(46, t.target, 2, 2); add(47, t.pick, 1, 1);
+  }
+  *row = (unsigned)off; *sig = h;
+  return v;
+}
+#ifndef FB_EMU
+template <bool LOAD> __global__ void __launch_bounds__(32 * FB_WPB) fb_state_kernel(StArgs a) {
+  const int w = blockIdx.x * FB_WPB + threadIdx.y;
+  if (w >= a.n) return;
+  const int old_pick = LOAD ? kstate_pick(a, w) : -1;
+  kstate_copy<LOAD>(a, w, threadIdx.x);
+  if (LOAD) { __syncwarp(); kstate_terrain(a, w, threadIdx.x, old_pick); }
+}
+#endif
+template <bool LOAD> static void launch_state(FbSim* s, const int* env_dev, const int* slot_dev, const int* env_host, const int* slot_host, int n) {
+#ifndef FB_EMU
+  StArgs a = {s->st_segs_dev, s->st_nseg, s->st_bank, s->st_row, env_dev, slot_dev, n, s->d.task};
+  (void)env_host; (void)slot_host;
+  fb_state_kernel<LOAD><<<(n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(a);
+#else
+  StArgs a = {s->st_segs_dev, s->st_nseg, s->st_bank, s->st_row, env_host, slot_host, n, s->d.task};
+  (void)env_dev; (void)slot_dev;
+  for (int w = 0; w < n; w++) {
+    const int old_pick = LOAD ? kstate_pick(a, w) : -1;
+    for (int y = 0; y < FB_NY; y++) kstate_copy<LOAD>(a, w, y);
+    if (LOAD) for (int y = 0; y < FB_NY; y++) kstate_terrain(a, w, y, old_pick);
+  }
+#endif
+  s->launches++;
+}
+static int state_ready(FbSim* s, const char* who) {
+  if (s->st_bank) return 0;
+  s->err = std::string(who) + (s->st_stale ? ": the state bank was dropped when the handle's programs, reference slots or applied-force arrays changed: call fb_state_bank again"
+                                           : ": no state bank (fb_state_bank)");
+  return -1;
+}
+// the (env, slot) lists of a save / load on the device: envs at [0, n), slots at [n, 2n); a NULL list stays NULL (the identity)
+static int state_ids(FbSim* s, const int32_t* env_ids, const int32_t* slots, int n, const int** env_dev, const int** slot_dev) {
+  *env_dev = *slot_dev = nullptr;
+  if (2 * n > s->st_ids_cap) {
+    if (sync_stream(s) != 0) return -2;
+    s->st_ids_cap = std::max(2 * n, 2 * s->d.Np); s->st_ids_dev = dalloc<int>(s, s->st_ids_cap);
+    if (!s->st_ids_dev) { s->st_ids_cap = 0; s->err = "out of device memory (state id lists)"; return -4; }
+  }
+  if (env_ids) { upload_async(s, s->st_ids_dev, env_ids, sizeof(int) * n); *env_dev = s->st_ids_dev; }
+  if (slots) { upload_async(s, s->st_ids_dev + n, slots, sizeof(int) * n); *slot_dev = s->st_ids_dev + n; }
+  return 0;
+}
+extern "C" {
+
+int fb_state_slots(FbHandle s) {
+  if (!s) return -1;
+  unsigned row; uint64_t sig; int ho; state_layout(s, &row, &sig, &ho);
+  return (int)row;
+}
+uint64_t fb_state_signature(FbHandle s) {
+  if (!s) return 0;
+  unsigned row; uint64_t sig; int ho; state_layout(s, &row, &sig, &ho);
+  return sig;
+}
+int fb_state_bank(FbHandle s, int n_slots) {
+  if (!s || n_slots < 0) return -1;
+  if (sync_stream(s) != 0) return -2;
+  state_drop(s); s->st_stale = false;
+  if (n_slots == 0) return 0;
+  unsigned row; uint64_t sig; int ho;
+  std::vector<StSeg> segs = state_layout(s, &row, &sig, &ho);
+  const size_t bytes = (size_t)n_slots * row * 4;
+#ifndef FB_EMU
+  size_t free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && bytes > free_b) { s->err = "fb_state_bank: the bank does not fit the device's free memory"; return -4; }
+#endif
+  const size_t mark = s->allocs.size();
+  s->st_bank = dalloc<unsigned>(s, (size_t)n_slots * row); s->st_segs_dev = (StSeg*)dalloc<unsigned char>(s, sizeof(StSeg) * segs.size());
+  s->st_scope.assign(s->allocs.begin() + mark, s->allocs.end());
+  if (!s->st_bank || !s->st_segs_dev) { scope_free(s, s->st_scope); s->st_bank = nullptr; s->st_segs_dev = nullptr; s->err = "fb_state_bank: out of memory"; return -4; }
+  h2d(s->st_segs_dev, segs.data(), sizeof(StSeg) * segs.size());
+  s->st_nseg = (int)segs.size(); s->st_row = row; s->st_sig = sig; s->st_hold_off = ho; s->st_slots = n_slots; s->st_written.assign(n_slots, 0);
+  return 0;
+}
+int fb_state_save(FbHandle s, const int32_t* env_ids, const int32_t* slots, int n) {
+  if (!s) return -1;
+  if (state_ready(s, "fb_state_save") != 0) return -1;
+  if (!env_ids && !slots) n = s->d.N;
+  if (n <= 0) return n == 0 ? 0 : -1;
+  std::vector<char> seen(s->st_slots, 0);
+  for (int k = 0; k < n; k++) {
+    const int e = env_ids ? env_ids[k] : k, sl = slots ? slots[k] : k;
+    if (e < 0 || e >= s->d.N) { s->err = "fb_state_save: env id out of range"; return -1; }
+    if (sl < 0 || sl >= s->st_slots) { s->err = "fb_state_save: slot out of range of the bank"; return -1; }
+    if (seen[sl]) { s->err = "fb_state_save: a slot may be written once per call"; return -1; }
+    seen[sl] = 1;
+  }
+#ifndef FB_EMU
+  cudaSetDevice(s->device);
+#endif
+  const int *ed, *sd; int rc = state_ids(s, env_ids, slots, n, &ed, &sd);
+  if (rc != 0) return rc;
+  launch_state<false>(s, ed, sd, env_ids, slots, n);
+  for (int k = 0; k < n; k++) s->st_written[slots ? slots[k] : k] = s->hold_pending ? 2 : 1;
+  return 0;
+}
+int fb_state_load(FbHandle s, const int32_t* slots, const int32_t* env_ids, int n) {
+  if (!s) return -1;
+  if (state_ready(s, "fb_state_load") != 0) return -1;
+  if (!env_ids && !slots) n = s->d.N;
+  if (n <= 0) return n == 0 ? 0 : -1;
+  std::vector<char> seen(s->d.N, 0); bool held = false;
+  for (int k = 0; k < n; k++) {
+    const int e = env_ids ? env_ids[k] : k, sl = slots ? slots[k] : k;
+    if (e < 0 || e >= s->d.N) { s->err = "fb_state_load: env id out of range"; return -1; }
+    if (sl < 0 || sl >= s->st_slots) { s->err = "fb_state_load: slot out of range of the bank"; return -1; }
+    if (!s->st_written[sl]) { s->err = "fb_state_load: slot " + std::to_string(sl) + " was never written"; return -1; }
+    if (seen[e]) { s->err = "fb_state_load: env " + std::to_string(e) + " appears twice"; return -1; }
+    seen[e] = 1; held = held || s->st_written[sl] == 2;
+  }
+#ifndef FB_EMU
+  cudaSetDevice(s->device);
+#endif
+  const int *ed, *sd; int rc = state_ids(s, env_ids, slots, n, &ed, &sd);
+  if (rc != 0) return rc;
+  launch_state<true>(s, ed, sd, env_ids, slots, n);
+  // what the row does not carry is a function of it: the position / velocity stage, for the loaded envs (all of them: the step's own launches)
+  if (n == s->d.N) launch_step1(s); else launch_step1_ids(s, ed, env_ids, n);
+  if (held) s->hold_pending = 1;             // a restored env waits for its reset: the next step holds it and clears the hold
+#ifndef FB_EMU
+  if (cudaGetLastError() != cudaSuccess) { s->err = "fb_state_load: kernel launch failed"; return -2; }
+#endif
+  return 0;
+}
+int fb_state_read(FbHandle s, const int32_t* slots, int n, void* host_dst) {
+  if (!s || !host_dst || n < 0) return -1;
+  if (state_ready(s, "fb_state_read") != 0) return -1;
+  for (int k = 0; k < n; k++) {
+    const int sl = slots ? slots[k] : k;
+    if (sl < 0 || sl >= s->st_slots) { s->err = "fb_state_read: slot out of range of the bank"; return -1; }
+    if (!s->st_written[sl]) { s->err = "fb_state_read: slot " + std::to_string(sl) + " was never written"; return -1; }
+  }
+  if (sync_stream(s) != 0) return -2;
+  const size_t rb = (size_t)s->st_row * 4;
+  if (!slots) d2h(host_dst, s->st_bank, rb * n);
+  else for (int k = 0; k < n; k++) d2h((char*)host_dst + rb * k, s->st_bank + (size_t)s->st_row * slots[k], rb);
+  return 0;
+}
+int fb_state_substeps(FbHandle s, int n_substeps) {
+  if (!s) return -1;
+  if (n_substeps > 0) s->d.nsub_done = n_substeps;
+  return s->d.nsub_done;
+}
+int fb_state_write(FbHandle s, const int32_t* slots, int n, const void* host_src) {
+  if (!s || !host_src || n < 0) return -1;
+  if (state_ready(s, "fb_state_write") != 0) return -1;
+  for (int k = 0; k < n; k++) { const int sl = slots ? slots[k] : k; if (sl < 0 || sl >= s->st_slots) { s->err = "fb_state_write: slot out of range of the bank"; return -1; } }
+  if (sync_stream(s) != 0) return -2;
+  const size_t rb = (size_t)s->st_row * 4;
+  for (int k = 0; k < n; k++) {
+    const int sl = slots ? slots[k] : k;
+    const unsigned* src = (const unsigned*)((const char*)host_src + rb * k);
+    h2d(s->st_bank + (size_t)s->st_row * sl, src, rb);
+    s->st_written[sl] = src[s->st_hold_off] ? 2 : 1;
+  }
   return 0;
 }
 

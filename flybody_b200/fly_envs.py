@@ -381,6 +381,98 @@ class _TaskEnv:
             return TimeStep(StepType.FIRST, None, None, obs)
         return TimeStep(StepType(int(ts.step_type[0])), float(ts.reward[0]), float(ts.discount[0]), obs)
 
+    # ----------------------------------------------------------------------------- state rows
+    # physics.get_state() / set_state() for the envs of the batch, with everything the task carries per env (fb_state_* in the header).
+    # The device keeps a bank of rows; the env object's own per-env arrays that shape the coming outputs (`_state_refs`) are kept per
+    # bank slot in a host-side mirror.  Not covered, NotImplementedError: the host-side task code with a trajectory dataset (per-env
+    # snippets and their feature bank live in Python objects) and the host-side vision task (per-env terrains).  One limit: with the
+    # task on the device the draws of a reset are a counter hash of (seed, env, episode), so a row loaded into another env id
+    # continues bit for bit until that env's next reset, whose draws follow the new id.
+    def _state_refs(self):
+        """(owner, attribute) of the per-env host arrays a state row goes with"""
+        return [(self, '_time'), (self, '_needs_reset')]
+
+    def _state_prepare(self):
+        """the programs that shape the row are on the device (a fresh env uploads them at its first reset)"""
+
+    def state_bank(self, n_slots):
+        """(re)allocate the bank of `n_slots` state rows on the device and its host-side mirror (0 frees them).  Replacing the env's
+        programs (a new shared reference trajectory, `enable_eyes` does not) drops the bank: allocate it again afterwards."""
+        self._state_prepare()
+        self._sim.state_bank(n_slots)
+        self._state_mirror = [np.zeros((int(n_slots),) + getattr(o, a).shape[1:], getattr(o, a).dtype) for o, a in self._state_refs()]
+
+    def _state_ids(self, slots, env_ids):
+        if slots is None and env_ids is None:
+            env_ids = np.arange(self.n_envs)
+        e = np.arange(len(np.atleast_1d(slots))) if env_ids is None else np.asarray(env_ids, np.int64).reshape(-1)
+        s = np.arange(len(e)) if slots is None else np.asarray(slots, np.int64).reshape(-1)
+        if getattr(self, '_state_mirror', None) is None:
+            raise RuntimeError('no state bank: call state_bank(n_slots) first')
+        return s, e
+
+    def save_state(self, slots=None, env_ids=None):
+        """env `env_ids[k]` -> bank slot `slots[k]` (None: 0 .. n - 1; both None: every env k -> slot k).  Nothing leaves the device
+        and the call does not synchronise."""
+        s, e = self._state_ids(slots, env_ids)
+        self._sim.save_state(s, e)
+        for buf, (o, a) in zip(self._state_mirror, self._state_refs()):
+            buf[s] = getattr(o, a)[e]
+
+    def load_state(self, slots=None, env_ids=None):
+        """bank slot `slots[k]` -> env `env_ids[k]` (None: 0 .. n - 1); one slot may feed many envs, an env may appear once, the other
+        envs are untouched.  The views `step_device` returned and the next `step()` see the saved rows.  The env's RandomStates (the host
+        draws of later resets) are not part of a slot: `state_dict()` carries them."""
+        s, e = self._state_ids(slots, env_ids)
+        self._sim.load_state(s, e)
+        for buf, (o, a) in zip(self._state_mirror, self._state_refs()):
+            arr = np.array(getattr(o, a))
+            arr[e] = buf[s]
+            setattr(o, a, arr)
+
+    def _state_rngs(self):
+        """the RandomStates a continuation draws from, by name"""
+        return {'env': self._rs}
+
+    def state_dict(self):
+        """Every env's state as plain numpy arrays and ints (np.savez and pickle work): the rows of all envs, the layout signature, the
+        host-side mirror, the counters and the RandomStates.  Uses slots 0 .. n_envs - 1 of the bank (allocated if there is none)."""
+        self._state_prepare()
+        if getattr(self, '_state_mirror', None) is None or len(self._state_mirror[0]) < self.n_envs:
+            self.state_bank(self.n_envs)
+        self.save_state()
+        d = {'signature': np.uint64(self._sim.state_signature()), 'rows': self._sim.read_states(np.arange(self.n_envs)),
+             'nsub_done': self._sim.state_substeps(), 'n_resets': int(self.n_resets), 'n_capacity_overflows': int(self.n_capacity_overflows)}
+        for k, (o, a) in enumerate(self._state_refs()):
+            d[f'host_{k}{a}'] = np.array(getattr(o, a))
+        for name, rs in self._state_rngs().items():
+            _, keys, pos, has_gauss, cached = rs.get_state()
+            d[f'rng_{name}_keys'], d[f'rng_{name}_pos'] = np.array(keys), int(pos)
+            d[f'rng_{name}_has_gauss'], d[f'rng_{name}_cached'] = int(has_gauss), float(cached)
+        return d
+
+    def load_state_dict(self, d):
+        """continue from a `state_dict()` of an env built the same way (same factory arguments: the layout signature must match)"""
+        self._state_prepare()
+        if int(d['signature']) != self._sim.state_signature():
+            raise ValueError(f"state_dict signature {int(d['signature']):#x} does not match this env's state layout "
+                             f'{self._sim.state_signature():#x}: the model, the programs or the reference slot length differ')
+        rows = np.asarray(d['rows'])
+        if rows.shape[0] != self.n_envs:
+            raise ValueError(f'state_dict holds {rows.shape[0]} envs, this env has {self.n_envs}')
+        if getattr(self, '_state_mirror', None) is None or len(self._state_mirror[0]) < self.n_envs:
+            self.state_bank(self.n_envs)
+        ids = np.arange(self.n_envs)
+        self._sim.write_states(ids, rows)
+        for k, (buf, (o, a)) in enumerate(zip(self._state_mirror, self._state_refs())):
+            buf[ids] = np.asarray(d[f'host_{k}{a}'])
+        self.load_state(ids, ids)
+        self._sim.state_substeps(int(d['nsub_done']))
+        self.n_resets, self.n_capacity_overflows = int(d['n_resets']), int(d['n_capacity_overflows'])
+        for name, rs in self._state_rngs().items():
+            rs.set_state(('MT19937', np.asarray(d[f'rng_{name}_keys'], np.uint32), int(d[f'rng_{name}_pos']),
+                          int(d[f'rng_{name}_has_gauss']), float(d[f'rng_{name}_cached'])))
+
     def close(self):
         self._sim.close()
 
@@ -846,6 +938,29 @@ class BatchedFlyEnv(_TaskEnv):
         self.d2h_bytes_per_step = self._rec.nbytes + self._out4.nbytes
         self._step_counter = np.where(resetting, 0, self._step_counter + 1)
 
+    def _state_refs(self):
+        refs = super()._state_refs() + [(self, '_step_counter'), (self, '_ref_len'), (self, '_episode_steps'), (self, '_ref_pick')]
+        if self._variant == 'flight':
+            refs += [(self, '_wing_qpos_host'), (self._wbpg, 'freq'), (self._wbpg, 'idx'), (self._wbpg, 'pos')]
+        return refs
+
+    def _state_prepare(self):
+        if self._per_env_ref and not self._device_bank:
+            raise NotImplementedError('state rows do not cover the host-side task code with a trajectory dataset (per-env snippets are '
+                                      'Python objects): use device_task=True')
+        if self._rec is None:
+            if self._device_bank:
+                self._ensure_slots()
+            else:
+                self._load_snippet(np.arange(self.n_envs))
+
+    def _state_rngs(self):
+        rngs = super()._state_rngs()
+        tg = self.task._traj_generator
+        if isinstance(getattr(tg, '_random_state', None), np.random.RandomState):
+            rngs['loader'] = tg._random_state
+        return rngs
+
     def set_applied_forces(self, qfrc=None, xfrc=None, env_ids=None):
         """MuJoCo's `physics.data.qfrc_applied` ([nv] per env) and `xfrc_applied` ([nbody, 6] per env: world-frame force, then torque,
         at each body's CoM) for every env (`env_ids` None; a single row broadcasts) or the listed envs.  They act in every physics
@@ -1127,6 +1242,9 @@ class TemplateTaskEnv(BatchedFlyEnv):
         if random_state is not None:
             self._rs = random_state if isinstance(random_state, np.random.RandomState) else np.random.RandomState(random_state)
         self._prev_action = np.zeros((self.n_envs, self._action_spec.shape[0]))
+
+    def _state_refs(self):
+        return super()._state_refs() + [(self, '_prev_action')]
 
     @property
     def prev_action(self):

@@ -22,7 +22,8 @@ MAXCON, MAXEFC = 64, 160
 
 EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_applied_ptrs', 'fb_clear_applied', 'fb_step', 'fb_forward',
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
-           'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version']
+           'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version',
+           'fb_state_slots', 'fb_state_signature', 'fb_state_bank', 'fb_state_save', 'fb_state_load', 'fb_state_read', 'fb_state_write', 'fb_state_substeps']
 
 
 # enum FbTaskKind (FbTaskProgram.kind)
@@ -147,6 +148,15 @@ def load_library(path=None):
     lib.fb_last_error.argtypes = [C.c_void_p]
     lib.fb_last_error.restype = C.c_char_p
     lib.fb_version.restype = C.c_char_p
+    lib.fb_state_slots.argtypes = [C.c_void_p]
+    lib.fb_state_signature.argtypes = [C.c_void_p]
+    lib.fb_state_signature.restype = C.c_uint64
+    lib.fb_state_bank.argtypes = [C.c_void_p, C.c_int]
+    lib.fb_state_save.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    lib.fb_state_load.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    lib.fb_state_read.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    lib.fb_state_write.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    lib.fb_state_substeps.argtypes = [C.c_void_p, C.c_int]
     return lib
 
 
@@ -233,6 +243,60 @@ class BatchedStepper:
     def clear_applied(self):
         """drop every env's applied forces: the step goes back to the path without them"""
         self._check(self._lib.fb_clear_applied(self._h), 'fb_clear_applied')
+
+    # ---- state rows (fb_state_*: physics.get_state / set_state for the envs of the batch, see the header)
+    @property
+    def state_slots(self):
+        """4-byte slots of one state row under the current programs"""
+        return int(self._lib.fb_state_slots(self._h))
+
+    def state_signature(self):
+        """hash of the row layout; rows move between steppers with equal signatures"""
+        return int(self._lib.fb_state_signature(self._h))
+
+    def state_bank(self, n_slots):
+        """(re)allocate the device bank of `n_slots` state rows (0 frees it)"""
+        self._check(self._lib.fb_state_bank(self._h, int(n_slots)), 'fb_state_bank')
+
+    @staticmethod
+    def _id_pair(a, b):
+        a = None if a is None else np.ascontiguousarray(np.asarray(a).reshape(-1), np.int32)
+        b = None if b is None else np.ascontiguousarray(np.asarray(b).reshape(-1), np.int32)
+        if a is not None and b is not None and len(a) != len(b):
+            raise ValueError(f'{len(a)} ids against {len(b)}')
+        n = len(a) if a is not None else (len(b) if b is not None else 0)
+        return a, b, n, None if a is None else a.ctypes.data, None if b is None else b.ctypes.data
+
+    def save_state(self, slots=None, env_ids=None):
+        """env_ids[k] -> bank slot slots[k] (None: 0 .. n - 1; both None: every env k -> slot k); stream-ordered"""
+        e, s, n, ep, sp = self._id_pair(env_ids, slots)
+        self._keep_ids = (e, s)
+        self._check(self._lib.fb_state_save(self._h, ep, sp, n), 'fb_state_save')
+
+    def load_state(self, slots=None, env_ids=None):
+        """bank slot slots[k] -> env env_ids[k] (None: 0 .. n - 1; both None: slot k -> every env k); one slot may feed many envs"""
+        s, e, n, sp, ep = self._id_pair(slots, env_ids)
+        self._keep_ids = (e, s)
+        self._check(self._lib.fb_state_load(self._h, sp, ep, n), 'fb_state_load')
+
+    def read_states(self, slots):
+        """-> uint32 [len(slots), state_slots]: the listed bank rows on the host (raw bits)"""
+        s = np.ascontiguousarray(np.asarray(slots).reshape(-1), np.int32)
+        out = np.zeros((len(s), self.state_slots), np.uint32)
+        self._check(self._lib.fb_state_read(self._h, s.ctypes.data, len(s), out.ctypes.data), 'fb_state_read')
+        return out
+
+    def write_states(self, slots, rows):
+        """host rows (as read_states returns them, of a stepper with the same state_signature) -> the listed bank slots"""
+        s = np.ascontiguousarray(np.asarray(slots).reshape(-1), np.int32)
+        r = np.ascontiguousarray(rows, np.uint32)
+        if r.shape != (len(s), self.state_slots):
+            raise ValueError(f'rows {r.shape} against {(len(s), self.state_slots)}')
+        self._check(self._lib.fb_state_write(self._h, s.ctypes.data, len(s), r.ctypes.data), 'fb_state_write')
+
+    def state_substeps(self, n_substeps=0):
+        """substeps of the last control step (the divisor of the per-step sensor means); a positive argument sets it first"""
+        return int(self._lib.fb_state_substeps(self._h, int(n_substeps)))
 
     def reset(self, qpos=None, qvel=None, env_ids=None):
         n = self.n_envs if env_ids is None else len(env_ids)

@@ -163,6 +163,14 @@ class BatchedVisionFlightEnv(_TaskEnv):
             floor_contacts_fatal=1 if self._fatal else 0, **trench))
         self._dev_views = None
 
+    def _state_refs(self):
+        return super()._state_refs() + [(self, '_target_height'), (self, '_target_speed')]
+
+    def _state_prepare(self):
+        if not self._device_task:
+            raise NotImplementedError('state rows do not cover the host-side vision task (per-env terrains and draws live on the host): '
+                                      'use terrain_bank=K, device_task=True')
+
     def _before_device_step(self, resetting):
         draws = getattr(self, '_forced_draws', None)               # (tests: the draws the host-side code would make at these resets)
         if draws is not None and resetting.any():

@@ -439,6 +439,38 @@ int fb_hfield_write(FbHandle h, const int32_t* env_ids, int n, const float* heig
 int fb_render_eyes(FbHandle h);
 int fb_eyes_ptr(FbHandle h, void** dev_ptr, int* bytes_per_env);
 int fb_eyes_read(FbHandle h, uint8_t* host_dst);
+/* State rows: the batched stand-in for physics.get_state() / physics.set_state() (dm_control), extended by what a batched
+ * task env carries per env.  A row is everything the next fb_step / fb_task_step of an env reads that the position / velocity
+ * stage does not recompute from it: qpos, qvel, act, ctrl, qacc, time, flags, solver iterations, hold, the solver's warm start
+ * (previous row keys, count, forces), sensordata and the per-step sensor sums, the env's packed and task observation rows with
+ * their step index / FIRST flag, its reference slot (fb_ref_slots), its applied forces if the handle has them, and the device
+ * task's per-env arrays (counters, reset flags, staged draws, wing-beat generator, `out` row, dataset episode and pin, vision
+ * targets and terrain pick).  A rollout continued from a loaded row equals the uninterrupted one bit for bit.
+ *   After fb_state_load, fb_get returns the saved values for the fields above and freshly recomputed ones for everything the
+ * position / velocity stage writes (FB_XPOS .. FB_SITE_XMAT, FB_SUBTREE_COM, FB_QM_DENSE, FB_NCON, FB_NEFC, FB_CONTACT,
+ * FB_QFRC_BIAS, FB_QFRC_PASSIVE); the acceleration stage's leftovers (FB_QFRC_SMOOTH, FB_QFRC_CONSTRAINT, FB_QFRC_ACTUATOR,
+ * FB_EFC_FORCE) keep what the env held before the load until the next step rewrites them.  Terrains are not in the row: the
+ * device vision task copies the row's terrain of its bank when the env holds another one, terrains written by
+ * fb_hfield_write are the caller's to rewrite.  The device task's draws are a counter hash of (seed, env, episode): a row
+ * loaded into another env id continues bit for bit until that env's next reset, whose draws follow the new id.
+ *   The layout follows the handle: replacing the observation or task program, the reference slots, a bank a task program draws
+ * from, or allocating / clearing the applied-force arrays drops the bank, and save / load fail with a message until
+ * fb_state_bank is called again.  fb_state_signature hashes the layout (sizes, program kinds, slot length, layout version);
+ * rows move between handles with equal signatures.  Saving and loading change nothing a captured step graph depends on.    */
+int fb_state_slots(FbHandle h);                  /* 4-byte slots of one row under the handle's current model, programs and applied-force arrays */
+uint64_t fb_state_signature(FbHandle h);
+int fb_state_bank(FbHandle h, int n_slots);      /* (re)allocate the device bank [n_slots][fb_state_slots]; 0 frees it; -4 with a message if it does not fit */
+/* env_ids[k] -> slots[k], stream-ordered (no synchronisation); a NULL list is the identity 0 .. n - 1, both NULL: every env k -> slot k.
+ * A slot may be written once per call.                                                                                       */
+int fb_state_save(FbHandle h, const int32_t* env_ids, const int32_t* slots, int n);
+/* slots[k] -> env_ids[k], then the position / velocity stage of the loaded envs only; the other envs are untouched.  One slot may
+ * feed many envs, an env may appear once.  A row saved while envs were held for their reset makes the next step a holding one.  */
+int fb_state_load(FbHandle h, const int32_t* slots, const int32_t* env_ids, int n);
+int fb_state_read(FbHandle h, const int32_t* slots, int n, void* host_dst);          /* bank rows -> host [n][fb_state_slots], synchronises */
+int fb_state_write(FbHandle h, const int32_t* slots, int n, const void* host_src);   /* host rows -> bank */
+/* The one handle-level number a continuation on another handle needs: the substeps of the last fb_step (the divisor of the per-step
+ * sensor means).  Returns it; n_substeps > 0 sets it first (a handle that never stepped continuing another one's rows).        */
+int fb_state_substeps(FbHandle h, int n_substeps);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
