@@ -121,7 +121,9 @@ FB_DEV void body_derived(const DevModel& m, const DevData& d, int e, int b, floa
 
 FB_DEV void kpos_p0(FB_PHASE_ARGS) {
   if (y != 0) return;
-  // reference point = position of the first root's free joint
+  // reference point = position of the first root's free joint, one for all trees (MuJoCo takes each tree's own subtree CoM).  fp32
+  // positions stay resolved for bodies near that root; a second tree far from it (a ghost 1e3 cm away) loses about 100x of its
+  // inertia's accuracy (tests/smooth_states.py moves the whole scene in its far states, as the tasks keep the ghost on the walker)
   int rb = m.root_body[0];
   V3 ref = v3(0, 0, 0);
   if (m.body_jntnum[rb] > 0 && m.jnt_type[m.body_jntadr[rb]] == FB_JNT_FREE) {

@@ -62,7 +62,7 @@ struct FbSim {
   std::vector<void*> allocs;
   std::vector<void*> obs_scope, task_scope;   // device buffers of the current observation / task program: freed when the program is replaced
   std::vector<void*> applied_scope;           // qfrc_applied / xfrc_applied: freed by fb_clear_applied
-  std::vector<int> h_dof_parent, h_dof_Madr;
+  std::vector<int> h_dof_parent, h_dof_Madr, h_body_parent;
   std::vector<double> h_qpos0;
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
@@ -584,7 +584,7 @@ static int build_model(FbSim* s, const FbModel* h) {
   m.sensor_type = upi(s, h->sensor_type, m.nsensor); m.sensor_objid = upi(s, h->sensor_objid, m.nsensor);
   m.sensor_adr = upi(s, h->sensor_adr, m.nsensor); m.sensor_dim = upi(s, h->sensor_dim, m.nsensor);
   s->h_dof_parent.assign(h->dof_parentid, h->dof_parentid + nv); s->h_dof_Madr.assign(h->dof_Madr, h->dof_Madr + nv);
-  s->h_qpos0.assign(h->qpos0, h->qpos0 + m.nq);
+  s->h_qpos0.assign(h->qpos0, h->qpos0 + m.nq); s->h_body_parent.assign(h->body_parentid, h->body_parentid + m.nbody);
   return 0;
 }
 
@@ -961,8 +961,11 @@ int fb_get(FbHandle s, int field, void* dst, int is_device) {
     case FB_SUBTREE_COM: {
       std::vector<float> crb((size_t)10 * m.nbody * N), ref((size_t)3 * N);
       field_to_host_strided(s, s->d.crb10, m.nbody, 10, FB_I10S, crb.data()); field_to_host(s, s->d.ref, 3, ref.data());
-      for (int e = 0; e < N; e++) for (int b = 0; b < m.nbody; b++) { const float* c = &crb[((size_t)e * m.nbody + b) * 10];
-        for (int i = 0; i < 3; i++) out[((size_t)e * m.nbody + b) * 3 + i] = (c[0] > 0 ? c[1 + i] / c[0] : 0.0f) + ref[(size_t)e * 3 + i]; }
+      for (int e = 0; e < N; e++) {
+        float w[4] = {0, 0, 0, 0};         // the world's subtree (MuJoCo subtree_com[0]): the sum of its children's composite inertias
+        for (int b = 1; b < m.nbody; b++) if (s->h_body_parent[b] == 0) for (int k = 0; k < 4; k++) w[k] += crb[((size_t)e * m.nbody + b) * 10 + k];
+        for (int b = 0; b < m.nbody; b++) { const float* c = b ? &crb[((size_t)e * m.nbody + b) * 10] : w;
+          for (int i = 0; i < 3; i++) out[((size_t)e * m.nbody + b) * 3 + i] = (c[0] > 0 ? c[1 + i] / c[0] : 0.0f) + ref[(size_t)e * 3 + i]; } }
       return 0; }
     case FB_QM_DENSE: {
       std::vector<float> qm((size_t)m.nM * N); field_to_host(s, s->d.qM, m.nM, qm.data());
@@ -1195,7 +1198,8 @@ int fb_obs_program(FbHandle s, const FbObsProgram* p) {
     if ((k == FB_OBS_QPOS || k == FB_OBS_QVEL || k == FB_OBS_SITES_EGO || k == FB_OBS_DOF_AXIS_EGO) && (p->a[i] < 0 || b < 0 || p->a[i] + b > p->n_list)) { s->err = "fb_obs_program: list range"; return -1; }
     if ((k == FB_OBS_SENSOR_MEAN || k == FB_OBS_SENSOR_NOW) && (p->a[i] < 0 || b < 0 || p->a[i] + b > m.nsensordata)) { s->err = "fb_obs_program: sensor range"; return -1; }
     if (k == FB_OBS_ACT && (p->a[i] < 0 || b < 0 || p->a[i] + b > m.na)) { s->err = "fb_obs_program: activation range"; return -1; }
-    if (k == FB_OBS_SUBTREE_COM && (p->a[i] < 0 || p->a[i] >= m.nbody)) { s->err = "fb_obs_program: subtree_com body id"; return -1; }
+    // (the kernels keep no composite inertia of the world body: its subtree CoM is only on the host, fb_get(FB_SUBTREE_COM))
+    if (k == FB_OBS_SUBTREE_COM && (p->a[i] < 1 || p->a[i] >= m.nbody)) { s->err = "fb_obs_program: subtree_com body id (1 .. nbody - 1)"; return -1; }
     if ((k == FB_OBS_REF_DISP || k == FB_OBS_REF_QUAT) && b < 0) { s->err = "fb_obs_program: negative count"; return -1; }
   }
   for (int i = 0; i < p->n_items; i++) {          // entries of the index list, by the kind that reads them

@@ -262,7 +262,7 @@ enum FbObsItem {
   FB_OBS_REF_QUAT = 8,    /* b = future_steps+1 : root_quat^-1 * ref_quat[step+i]                            */
   FB_OBS_SCALARS = 9,     /* flags, |qacc|^2, time                                                           */
   FB_OBS_ROOT_POSE = 10,  /* root xpos[3] + quat[4]                                                          */
-  FB_OBS_SUBTREE_COM = 11,/* a = body id : physics.data.subtree_com[body]                                    */
+  FB_OBS_SUBTREE_COM = 11,/* a = body id, 1 .. nbody - 1 (not the world) : physics.data.subtree_com[body]      */
   FB_OBS_DOF_AXIS_EGO = 12,/* a = offset into list (dof ids), b = count : world joint axis (physics.bind(joints).xaxis,
                               tasks/rewards.py:48-50) rotated into the root frame                                */
   FB_OBS_TASK_TARGET = 14,   /* b floats of the device task's per-episode targets (FB_TASK_VISION: target height, target speed = the reference's
