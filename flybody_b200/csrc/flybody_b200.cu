@@ -16,6 +16,8 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <cmath>
+#include <limits>
 
 #ifndef FB_EMU
 #include <cuda_runtime.h>
@@ -25,6 +27,7 @@
 #include "fb_hfield.h"
 #include "fb_task.h"
 #include "fb_state.h"
+#include "fb_ik.h"
 
 #ifdef FB_EMU
 typedef int cudaStream_t_;
@@ -63,7 +66,9 @@ struct FbSim {
   std::vector<void*> obs_scope, task_scope;   // device buffers of the current observation / task program: freed when the program is replaced
   std::vector<void*> applied_scope;           // qfrc_applied / xfrc_applied: freed by fb_clear_applied
   std::vector<int> h_dof_parent, h_dof_Madr, h_body_parent;
+  std::vector<int> h_jnt_type, h_jnt_qadr, h_jnt_dofadr, h_jnt_body, h_site_body;   // joint / site tables an IK program is checked and built against
   std::vector<double> h_qpos0;
+  DevIk ik = {}; std::vector<void*> ik_scope; int ik_solved = 0;   // inverse kinematics (fb_ik_program): parameters and buffers; problems of the last solve
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -585,6 +590,9 @@ static int build_model(FbSim* s, const FbModel* h) {
   m.sensor_adr = upi(s, h->sensor_adr, m.nsensor); m.sensor_dim = upi(s, h->sensor_dim, m.nsensor);
   s->h_dof_parent.assign(h->dof_parentid, h->dof_parentid + nv); s->h_dof_Madr.assign(h->dof_Madr, h->dof_Madr + nv);
   s->h_qpos0.assign(h->qpos0, h->qpos0 + m.nq); s->h_body_parent.assign(h->body_parentid, h->body_parentid + m.nbody);
+  s->h_jnt_type.assign(h->jnt_type, h->jnt_type + nj); s->h_jnt_qadr.assign(h->jnt_qposadr, h->jnt_qposadr + nj);
+  s->h_jnt_dofadr.assign(h->jnt_dofadr, h->jnt_dofadr + nj); s->h_jnt_body.assign(h->jnt_bodyid, h->jnt_bodyid + nj);
+  s->h_site_body.assign(h->site_bodyid, h->site_bodyid + m.nsite);
   return 0;
 }
 
@@ -1875,6 +1883,144 @@ int fb_state_write(FbHandle s, const int32_t* slots, int n, const void* host_src
     s->st_written[sl] = src[s->st_hold_off] ? 2 : 1;
   }
   return 0;
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------
+// inverse kinematics (fb_ik_*; fb_ik.h): its own kernel parameter (DevIk) and buffers (ik_scope), bounded launches
+#define FB_IK_LAUNCH_ITERS (4 * FB_IK_CHECK)       // iterations per launch: the host reads the live count once per launch
+#ifndef FB_EMU
+__global__ void __launch_bounds__(32 * FB_WPB) fb_ik_kernel(DevModel m, DevData d, DevIk p) {
+  extern __shared__ __align__(16) float fb_smem_ik[];
+  kik_run(m, d, p, fb_smem_ik + (size_t)threadIdx.y * FB_IK_SH(p.n_fdof), blockIdx.x * FB_WPB + threadIdx.y);
+}
+#endif
+static int ik_launch(FbSim* s, int* live) {
+  DevIk& p = s->ik;
+#ifndef FB_EMU
+  FB_CUDA_OK(cudaMemsetAsync(p.live, 0, sizeof(int), s->stream));
+  const size_t bytes = sizeof(float) * FB_IK_SH(p.n_fdof) * FB_WPB;
+  fb_ik_kernel<<<(p.n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), bytes, s->stream>>>(s->m, s->d, p);
+  FB_CUDA_OK(cudaGetLastError());
+  FB_CUDA_OK(cudaMemcpyAsync(live, p.live, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+  FB_CUDA_OK(cudaStreamSynchronize(s->stream));
+#else
+  *p.live = 0;
+  std::vector<float> sh(FB_IK_SH(p.n_fdof) + 64, 0.0f);
+  for (int e = 0; e < p.n; e++) kik_run(s->m, s->d, p, sh.data(), e);
+  *live = *p.live;
+#endif
+  s->launches++;
+  return 0;
+}
+
+extern "C" {
+
+int fb_ik_program(FbHandle s, const FbIkProgram* p) {
+  if (!s || !p) return -1;
+  const DevModel& m = s->m;
+  if (p->n_sites < 1 || p->n_sites > FB_IK_MAXSITE || !p->site_ids) { s->err = "fb_ik_program: 1 .. 64 sites"; return -1; }
+  if (p->n_jnts < 1 || !p->jnt_ids) { s->err = "fb_ik_program: no joints to fit"; return -1; }
+  for (int k = 0; k < p->n_sites; k++) if (p->site_ids[k] < 0 || p->site_ids[k] >= m.nsite) { s->err = "fb_ik_program: site id out of range"; return -1; }
+  std::vector<char> seen(m.njnt, 0);
+  for (int k = 0; k < p->n_jnts; k++) {
+    const int j = p->jnt_ids[k];
+    if (j < 0 || j >= m.njnt) { s->err = "fb_ik_program: joint id out of range"; return -1; }
+    if (seen[j]++) { s->err = "fb_ik_program: joint listed twice"; return -1; }
+    if (s->h_jnt_type[j] != FB_JNT_HINGE && s->h_jnt_type[j] != FB_JNT_FREE) { s->err = "fb_ik_program: only hinge and free joints can be fitted (ball joints cannot)"; return -1; }
+  }
+  if (!(std::isfinite(p->reg_strength) && std::isfinite(p->lr) && std::isfinite(p->beta) && std::isfinite(p->progress_threshold)) || p->max_steps < 1) {
+    s->err = "fb_ik_program: non-finite parameter or max_steps < 1"; return -1;
+  }
+  if (sync_stream(s) != 0) return -2;
+  // fitted dofs in joint order; the sites below each (site body at or under the dof's body)
+  std::vector<int> fdof, hq, jt, jq, jf; std::vector<unsigned long long> below;
+  for (int k = 0; k < p->n_jnts; k++) {
+    const int j = p->jnt_ids[k], t = s->h_jnt_type[j], nd = t == FB_JNT_FREE ? 6 : 1, b = s->h_jnt_body[j];
+    jt.push_back(t); jq.push_back(s->h_jnt_qadr[j]); jf.push_back((int)fdof.size());
+    unsigned long long mask = 0;
+    for (int q = 0; q < p->n_sites; q++) for (int a = s->h_site_body[p->site_ids[q]]; a > 0; a = s->h_body_parent[a]) if (a == b) { mask |= 1ull << q; break; }
+    for (int i = 0; i < nd; i++) { fdof.push_back(s->h_jnt_dofadr[j] + i); hq.push_back(t == FB_JNT_HINGE ? s->h_jnt_qadr[j] : -1); below.push_back(mask); }
+  }
+  std::vector<unsigned char> inc(3 * p->n_sites, 1);
+  if (p->include) for (int k = 0; k < 3 * p->n_sites; k++) inc[k] = p->include[k] ? 1 : 0;
+  std::vector<int> sid(p->site_ids, p->site_ids + p->n_sites);
+  scope_free(s, s->ik_scope);
+  const size_t mark = s->allocs.size(); const int Np = s->d.Np, nfd = (int)fdof.size();
+  DevIk& k = s->ik; k = DevIk{};
+  k.n_site = p->n_sites; k.n_fdof = nfd; k.n_fjnt = p->n_jnts; k.iters = FB_IK_LAUNCH_ITERS; k.max_steps = p->max_steps;
+  k.reg = p->reg_strength; k.lr = p->lr; k.beta = p->beta; k.thr = p->progress_threshold;
+  k.site_id = up(s, sid); k.include = up(s, inc); k.fdof = up(s, fdof); k.fdof_hqadr = up(s, hq); k.below = up(s, below);
+  k.fjnt_type = up(s, jt); k.fjnt_qadr = up(s, jq); k.fjnt_fd0 = up(s, jf);
+  k.target = dalloc<float>(s, (size_t)Np * 3 * p->n_sites); k.u = dalloc<float>(s, (size_t)Np * nfd);
+  k.step = dalloc<int>(s, Np); k.done = dalloc<int>(s, Np); k.err = dalloc<float>(s, Np); k.err_first = dalloc<float>(s, Np);
+  k.steps = dalloc<int>(s, Np); k.success = dalloc<unsigned char>(s, Np); k.live = dalloc<int>(s, 1);
+  s->ik_scope.assign(s->allocs.begin() + mark, s->allocs.end());
+  for (void* q : s->ik_scope) if (!q) { scope_free(s, s->ik_scope); s->ik = DevIk{}; s->err = "out of device memory (IK program)"; return -4; }
+  s->ik_solved = 0;
+  return 0;
+}
+
+int fb_ik_solve(FbHandle s, int n, const float* target_xpos, const float* init_qpos) {
+  if (!s) return -1;
+  DevIk& p = s->ik;
+  if (!p.live) { s->err = "fb_ik_solve: no IK program (fb_ik_program)"; return -1; }
+  if (n < 1 || n > s->d.N || !target_xpos) { s->err = "fb_ik_solve: 1 <= n <= n_envs problems with targets"; return -1; }
+  const int nq = s->m.nq, nt = 3 * p.n_site;
+  for (size_t i = 0; i < (size_t)n * nt; i++) if (std::isinf(target_xpos[i])) { s->err = "fb_ik_solve: infinite target component"; return -1; }
+  if (init_qpos) for (size_t i = 0; i < (size_t)n * nq; i++) if (!std::isfinite(init_qpos[i])) { s->err = "fb_ik_solve: non-finite init_qpos"; return -1; }
+#ifndef FB_EMU
+  cudaSetDevice(s->device);
+#endif
+  if (sync_stream(s) != 0) return -2;
+  const int Np = s->d.Np;
+  std::vector<int> done(Np, 1); std::fill(done.begin(), done.begin() + n, 0);
+  std::vector<float> nan(Np, std::numeric_limits<float>::quiet_NaN()), zero((size_t)Np * p.n_fdof, 0.0f);
+  std::vector<int> zi(Np, 0);
+  upload_async(s, (void*)p.target, target_xpos, sizeof(float) * (size_t)n * nt);
+  upload_async(s, p.u, zero.data(), sizeof(float) * zero.size()); upload_async(s, p.step, zi.data(), sizeof(int) * Np);
+  upload_async(s, p.done, done.data(), sizeof(int) * Np); upload_async(s, p.err, nan.data(), sizeof(float) * Np);
+  upload_async(s, p.err_first, nan.data(), sizeof(float) * Np); upload_async(s, p.steps, zi.data(), sizeof(int) * Np);
+  std::vector<unsigned char> zb(Np, 0); upload_async(s, p.success, zb.data(), Np);
+  if (init_qpos) {
+#ifndef FB_EMU
+    FB_CUDA_OK(cudaMemcpy2DAsync(s->d.qpos, (size_t)s->d.rec * 4, init_qpos, (size_t)nq * 4, (size_t)nq * 4, n, cudaMemcpyHostToDevice, s->stream));
+#else
+    for (int e = 0; e < n; e++) memcpy(s->d.qpos + (size_t)e * s->d.rec, init_qpos + (size_t)e * nq, sizeof(float) * nq);
+#endif
+  }
+  if (sync_stream(s) != 0) return -2;           // the host vectors go out of scope below
+  p.n = n; s->ik_solved = n;
+  for (int live = n; live > 0;) if (ik_launch(s, &live) != 0) return -2;
+  return 0;
+}
+
+int fb_ik_read(FbHandle s, float* qpos, float* err, float* err_first, int32_t* steps, uint8_t* success) {
+  if (!s) return -1;
+  const DevIk& p = s->ik;
+  if (!p.live || s->ik_solved < 1) { s->err = "fb_ik_read: no IK solve to read"; return -1; }
+  if (sync_stream(s) != 0) return -2;
+  const int n = s->ik_solved, nq = s->m.nq;
+  if (qpos) {
+#ifndef FB_EMU
+    FB_CUDA_OK(cudaMemcpy2DAsync(qpos, (size_t)nq * 4, s->d.qpos, (size_t)s->d.rec * 4, (size_t)nq * 4, n, cudaMemcpyDeviceToHost, s->stream));
+#else
+    for (int e = 0; e < n; e++) memcpy(qpos + (size_t)e * nq, s->d.qpos + (size_t)e * s->d.rec, sizeof(float) * nq);
+#endif
+  }
+#ifndef FB_EMU
+  if (err) FB_CUDA_OK(cudaMemcpyAsync(err, p.err, sizeof(float) * n, cudaMemcpyDeviceToHost, s->stream));
+  if (err_first) FB_CUDA_OK(cudaMemcpyAsync(err_first, p.err_first, sizeof(float) * n, cudaMemcpyDeviceToHost, s->stream));
+  if (steps) FB_CUDA_OK(cudaMemcpyAsync(steps, p.steps, sizeof(int) * n, cudaMemcpyDeviceToHost, s->stream));
+  if (success) FB_CUDA_OK(cudaMemcpyAsync(success, p.success, n, cudaMemcpyDeviceToHost, s->stream));
+#else
+  if (err) memcpy(err, p.err, sizeof(float) * n);
+  if (err_first) memcpy(err_first, p.err_first, sizeof(float) * n);
+  if (steps) memcpy(steps, p.steps, sizeof(int) * n);
+  if (success) memcpy(success, p.success, n);
+#endif
+  return sync_stream(s);
 }
 
 }  // extern "C"

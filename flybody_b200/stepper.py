@@ -23,7 +23,8 @@ MAXCON, MAXEFC = 64, 160
 EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_applied_ptrs', 'fb_clear_applied', 'fb_step', 'fb_forward',
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
            'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version',
-           'fb_state_slots', 'fb_state_signature', 'fb_state_bank', 'fb_state_save', 'fb_state_load', 'fb_state_read', 'fb_state_write', 'fb_state_substeps']
+           'fb_state_slots', 'fb_state_signature', 'fb_state_bank', 'fb_state_save', 'fb_state_load', 'fb_state_read', 'fb_state_write', 'fb_state_substeps',
+           'fb_ik_program', 'fb_ik_solve', 'fb_ik_read']
 
 
 # enum FbTaskKind (FbTaskProgram.kind)
@@ -73,6 +74,13 @@ class FbEyeProgram(C.Structure):
                 ('fovy_deg', C.c_float), ('size', C.c_int32), ('nrow', C.c_int32), ('ncol', C.c_int32), ('half_size', C.c_float),
                 ('z_offset', C.c_float), ('zfar', C.c_float), ('sky_top', C.c_float * 3), ('sky_horizon', C.c_float * 3),
                 ('ground', C.c_float * 3), ('ambient', C.c_float), ('diffuse', C.c_float)]
+
+
+class FbIkProgram(C.Structure):
+    """include/flybody_b200.h: FbIkProgram (multi-site inverse kinematics)."""
+    _fields_ = [('n_sites', C.c_int32), ('site_ids', C.POINTER(C.c_int32)), ('n_jnts', C.c_int32), ('jnt_ids', C.POINTER(C.c_int32)),
+                ('include', C.POINTER(C.c_uint8)), ('reg_strength', C.c_float), ('lr', C.c_float), ('beta', C.c_float),
+                ('progress_threshold', C.c_float), ('max_steps', C.c_int32)]
 
 
 class StepperError(RuntimeError):
@@ -157,6 +165,9 @@ def load_library(path=None):
     lib.fb_state_read.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.fb_state_write.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.fb_state_substeps.argtypes = [C.c_void_p, C.c_int]
+    lib.fb_ik_program.argtypes = [C.c_void_p, C.c_void_p]
+    lib.fb_ik_solve.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.fb_ik_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5
     return lib
 
 
@@ -297,6 +308,36 @@ class BatchedStepper:
     def state_substeps(self, n_substeps=0):
         """substeps of the last control step (the divisor of the per-step sensor means); a positive argument sets it first"""
         return int(self._lib.fb_state_substeps(self._h, int(n_substeps)))
+
+    # ---- multi-site inverse kinematics (fb_ik_*; flybody_b200.inverse_kinematics is the reference-shaped front end)
+    def ik_program(self, site_ids, jnt_ids, include=None, reg_strength=0.0, lr=0.01, beta=0.99, progress_threshold=0.01, max_steps=20_000):
+        """fit the listed joints (hinge / free) to the listed sites; include: [3 * n_sites] component mask (None: all)"""
+        sid = np.ascontiguousarray(site_ids, np.int32).reshape(-1)
+        jid = np.ascontiguousarray(jnt_ids, np.int32).reshape(-1)
+        inc = None if include is None else np.ascontiguousarray(include, np.uint8).reshape(-1)
+        if inc is not None and len(inc) != 3 * len(sid):
+            raise ValueError(f'include has {len(inc)} entries for {len(sid)} sites')
+        p = FbIkProgram(len(sid), sid.ctypes.data_as(C.POINTER(C.c_int32)), len(jid), jid.ctypes.data_as(C.POINTER(C.c_int32)),
+                        None if inc is None else inc.ctypes.data_as(C.POINTER(C.c_uint8)), float(reg_strength), float(lr), float(beta),
+                        float(progress_threshold), int(max_steps))
+        self._check(self._lib.fb_ik_program(self._h, C.byref(p)), 'fb_ik_program')
+        self._ik_nsite = len(sid)
+
+    def ik_solve(self, target_xpos, init_qpos=None):
+        """solve problems 0 .. n-1 (envs) for targets [n, n_sites, 3] from init_qpos [n, nq] (None: the envs' current qpos)"""
+        t = np.ascontiguousarray(target_xpos, np.float32).reshape(-1, self._ik_nsite, 3)
+        n = t.shape[0]
+        q = None if init_qpos is None else np.ascontiguousarray(np.broadcast_to(np.asarray(init_qpos, np.float32), (n, self.model.nq)))
+        self._check(self._lib.fb_ik_solve(self._h, n, t.ctypes.data, None if q is None else q.ctypes.data), 'fb_ik_solve')
+        self._ik_n = n
+
+    def ik_read(self):
+        """-> (qpos [n, nq] f32, err_norm [n] f32, err_norm_first_term [n] f32, steps [n] i32, success [n] bool) of the last solve"""
+        n = self._ik_n
+        q, e, e1 = np.zeros((n, self.model.nq), np.float32), np.zeros(n, np.float32), np.zeros(n, np.float32)
+        k, ok = np.zeros(n, np.int32), np.zeros(n, np.uint8)
+        self._check(self._lib.fb_ik_read(self._h, q.ctypes.data, e.ctypes.data, e1.ctypes.data, k.ctypes.data, ok.ctypes.data), 'fb_ik_read')
+        return q, e, e1, k, ok.astype(bool)
 
     def reset(self, qpos=None, qvel=None, env_ids=None):
         n = self.n_envs if env_ids is None else len(env_ids)

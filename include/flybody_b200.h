@@ -471,6 +471,29 @@ int fb_state_write(FbHandle h, const int32_t* slots, int n, const void* host_src
 /* The one handle-level number a continuation on another handle needs: the substeps of the last fb_step (the divisor of the per-step
  * sensor means).  Returns it; n_substeps > 0 sets it first (a handle that never stepped continuing another one's rows).        */
 int fb_state_substeps(FbHandle h, int n_substeps);
+/* Multi-site inverse kinematics (reference flybody/inverse_kinematics.py: qpos_from_site_xpos), one problem per env, one warp each.
+ * Gradient descent with momentum on  sum over included components of (site_xpos - target)^2 + reg_strength * |hinge qpos|^2  (the
+ * fitted hinges' raw qpos, as the reference), the step applied as mj_integratePos; every 100 iterations (from iteration 0) the
+ * objective is evaluated and the problem stops with success when lr |u| / objective < progress_threshold (an objective of 0 counts
+ * as converged: the reference divides by it).  Fitted joints are hinge or free joints; ball joints cannot be fitted, unfitted ones
+ * keep their qpos.  The program owns its buffers; the record layout, the state rows and fb_state_signature do not change.   */
+typedef struct FbIkProgram {
+  int32_t n_sites; const int32_t* site_ids;    /* model site ids, 1 .. 64 of them                                         */
+  int32_t n_jnts; const int32_t* jnt_ids;      /* fitted joints (hinge or free), each once                                 */
+  const uint8_t* include;                      /* [3 * n_sites] components in the objective (include_inds); NULL = all      */
+  float reg_strength, lr, beta, progress_threshold;
+  int32_t max_steps;                           /* >= 1                                                                      */
+} FbIkProgram;
+int fb_ik_program(FbHandle h, const FbIkProgram* p);
+/* Envs 0 .. n-1: qpos <- init_qpos rows [n][nq] (NULL: keep the current qpos), then solve for targets [n][n_sites][3] (world frame).
+ * A NaN target component is excluded for that problem (a tracking dropout); an infinite target or a non-finite init_qpos is an
+ * error.  Runs bounded launches on the handle's stream and reads one live count per launch, so it returns when every problem has
+ * stopped.  Afterwards qpos holds the fits; the other forward quantities are stale until fb_forward / fb_reset.             */
+int fb_ik_solve(FbHandle h, int n, const float* target_xpos, const float* init_qpos);
+/* Results of the last solve for its n problems, each pointer may be NULL (synchronises): qpos [n][nq]; err: the objective at the
+ * last check; err_first: the site term at the returned qpos; steps: the loop index at the stop (max_steps - 1 without success);
+ * success: 1 when the progress test stopped the problem.                                                                   */
+int fb_ik_read(FbHandle h, float* qpos, float* err, float* err_first, int32_t* steps, uint8_t* success);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
