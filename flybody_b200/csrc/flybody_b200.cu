@@ -28,6 +28,7 @@
 #include "fb_task.h"
 #include "fb_state.h"
 #include "fb_ik.h"
+#include "fb_inverse.h"
 
 #ifdef FB_EMU
 typedef int cudaStream_t_;
@@ -69,6 +70,7 @@ struct FbSim {
   std::vector<int> h_jnt_type, h_jnt_qadr, h_jnt_dofadr, h_jnt_body, h_site_body;   // joint / site tables an IK program is checked and built against
   std::vector<double> h_qpos0;
   DevIk ik = {}; std::vector<void*> ik_scope; int ik_solved = 0;   // inverse kinematics (fb_ik_program): parameters and buffers; problems of the last solve
+  DevInv inv = {}; std::vector<void*> inv_scope; int inv_done = 0;   // inverse dynamics (fb_inverse): buffers, allocated on first use; problems of the last call
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -2019,6 +2021,84 @@ int fb_ik_read(FbHandle s, float* qpos, float* err, float* err_first, int32_t* s
   if (err_first) memcpy(err_first, p.err_first, sizeof(float) * n);
   if (steps) memcpy(steps, p.steps, sizeof(int) * n);
   if (success) memcpy(success, p.success, n);
+#endif
+  return sync_stream(s);
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------
+// inverse dynamics (fb_inverse*; fb_inverse.h): its own kernel parameter (DevInv) and buffers (inv_scope), allocated on first use
+#ifndef FB_EMU
+__global__ void __launch_bounds__(32 * FB_WPB) fb_inv_kernel(DevModel m, DevData d, DevInv p) {
+  __shared__ float fb_smem_inv[FB_WPB][FB_INV_SH];
+  kinv_run(m, d, p, fb_smem_inv[threadIdx.y], blockIdx.x * FB_WPB + threadIdx.y);
+}
+#endif
+static int inv_alloc(FbSim* s) {
+  if (s->inv.qacc) return 0;
+  const size_t mark = s->allocs.size(), Np = (size_t)s->d.Np, nv = (size_t)s->m.nv;
+  DevInv& p = s->inv;
+  p.qacc = dalloc<float>(s, Np * nv); p.qfrc_inverse = dalloc<float>(s, Np * nv); p.qfrc_constraint = dalloc<float>(s, Np * nv);
+  p.efc_force = dalloc<float>(s, Np * FB_MAXEFC);
+  s->inv_scope.assign(s->allocs.begin() + mark, s->allocs.end());
+  for (void* q : s->inv_scope) if (!q) { scope_free(s, s->inv_scope); s->inv = DevInv{}; s->err = "out of device memory (inverse dynamics)"; return -4; }
+  return 0;
+}
+static int inv_launch(FbSim* s) {
+  const DevInv& p = s->inv;
+#ifndef FB_EMU
+  fb_inv_kernel<<<(p.n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, p);
+  FB_CUDA_OK(cudaGetLastError());
+#else
+  std::vector<float> sh(FB_INV_SH + 64, 0.0f);
+  for (int e = 0; e < p.n; e++) kinv_run(s->m, s->d, p, sh.data(), e);
+  for (int i = FB_INV_SH; i < FB_INV_SH + 64; i++) if (sh[i] != 0.0f) { fprintf(stderr, "fb_emu: shared-memory slice overrun in the inverse kernel\n"); abort(); }
+#endif
+  s->launches++;
+  return 0;
+}
+
+extern "C" {
+
+int fb_inverse(FbHandle s, int n, const float* qacc, int is_device) {
+  if (!s) return -1;
+  if (n < 1 || n > s->d.N) { s->err = "fb_inverse: 1 <= n <= n_envs problems"; return -1; }
+  if (!qacc) { s->err = "fb_inverse: qacc is NULL"; return -1; }
+  const size_t cnt = (size_t)n * s->m.nv;
+  if (!is_device) for (size_t i = 0; i < cnt; i++) if (!std::isfinite(qacc[i])) { s->err = "fb_inverse: non-finite qacc"; return -1; }
+#ifndef FB_EMU
+  cudaSetDevice(s->device);
+#endif
+  if (int rc = inv_alloc(s)) return rc;
+  DevInv& p = s->inv;
+#ifndef FB_EMU
+  FB_CUDA_OK(cudaMemcpyAsync(p.qacc, qacc, sizeof(float) * cnt, is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s->stream));
+#else
+  memcpy(p.qacc, qacc, sizeof(float) * cnt);
+#endif
+  p.n = n;
+  launch_step1(s);                             // the position / velocity stage fb_forward runs (sens_mode -1: no sensor sums)
+  if (inv_launch(s) != 0) return -2;
+  s->inv_done = n;
+  return is_device ? 0 : sync_stream(s);       // a host qacc may be reused once the call returns
+}
+
+int fb_inverse_read(FbHandle s, float* qfrc_inverse, float* qfrc_constraint, float* efc_force, int is_device) {
+  if (!s) return -1;
+  const DevInv& p = s->inv;
+  if (s->inv_done < 1) { s->err = "fb_inverse_read: no inverse to read (fb_inverse)"; return -1; }
+  const size_t n = (size_t)s->inv_done, nv = (size_t)s->m.nv;
+#ifndef FB_EMU
+  const cudaMemcpyKind k = is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  if (qfrc_inverse) FB_CUDA_OK(cudaMemcpyAsync(qfrc_inverse, p.qfrc_inverse, sizeof(float) * n * nv, k, s->stream));
+  if (qfrc_constraint) FB_CUDA_OK(cudaMemcpyAsync(qfrc_constraint, p.qfrc_constraint, sizeof(float) * n * nv, k, s->stream));
+  if (efc_force) FB_CUDA_OK(cudaMemcpyAsync(efc_force, p.efc_force, sizeof(float) * n * FB_MAXEFC, k, s->stream));
+#else
+  (void)is_device;
+  if (qfrc_inverse) memcpy(qfrc_inverse, p.qfrc_inverse, sizeof(float) * n * nv);
+  if (qfrc_constraint) memcpy(qfrc_constraint, p.qfrc_constraint, sizeof(float) * n * nv);
+  if (efc_force) memcpy(efc_force, p.efc_force, sizeof(float) * n * FB_MAXEFC);
 #endif
   return sync_stream(s);
 }

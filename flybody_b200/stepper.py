@@ -24,7 +24,7 @@ EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl'
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
            'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version',
            'fb_state_slots', 'fb_state_signature', 'fb_state_bank', 'fb_state_save', 'fb_state_load', 'fb_state_read', 'fb_state_write', 'fb_state_substeps',
-           'fb_ik_program', 'fb_ik_solve', 'fb_ik_read']
+           'fb_ik_program', 'fb_ik_solve', 'fb_ik_read', 'fb_inverse', 'fb_inverse_read']
 
 
 # enum FbTaskKind (FbTaskProgram.kind)
@@ -168,6 +168,8 @@ def load_library(path=None):
     lib.fb_ik_program.argtypes = [C.c_void_p, C.c_void_p]
     lib.fb_ik_solve.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     lib.fb_ik_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5
+    lib.fb_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+    lib.fb_inverse_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     return lib
 
 
@@ -338,6 +340,29 @@ class BatchedStepper:
         k, ok = np.zeros(n, np.int32), np.zeros(n, np.uint8)
         self._check(self._lib.fb_ik_read(self._h, q.ctypes.data, e.ctypes.data, e1.ctypes.data, k.ctypes.data, ok.ctypes.data), 'fb_ik_read')
         return q, e, e1, k, ok.astype(bool)
+
+    # ---- inverse dynamics (fb_inverse; flybody_b200.inverse_dynamics is the batched front end)
+    def inverse(self, qacc, n=None, is_device=False):
+        """mj_inverse for envs 0 .. n-1 at their current qpos / qvel: qacc [n, nv] (host array), or a device pointer (int) with
+        is_device=True and n given.  Stream-ordered; read the results with inverse_read()."""
+        if is_device:
+            if n is None:
+                raise ValueError('a device qacc needs n')
+            self._check(self._lib.fb_inverse(self._h, int(n), C.c_void_p(int(qacc)), 1), 'fb_inverse')
+        else:
+            q = np.ascontiguousarray(np.asarray(qacc, np.float32).reshape(-1, self.model.nv))
+            n = q.shape[0] if n is None else int(n)
+            if n > q.shape[0]:
+                raise ValueError(f'{q.shape[0]} qacc rows for n = {n}')
+            self._check(self._lib.fb_inverse(self._h, n, q.ctypes.data, 0), 'fb_inverse')
+        self._inv_n = int(n)
+
+    def inverse_read(self):
+        """-> (qfrc_inverse [n, nv], qfrc_constraint [n, nv], efc_force [n, MAXEFC]) f32 of the last inverse"""
+        n, nv = getattr(self, '_inv_n', 0), self.model.nv
+        qi, qc, f = np.zeros((n, nv), np.float32), np.zeros((n, nv), np.float32), np.zeros((n, MAXEFC), np.float32)
+        self._check(self._lib.fb_inverse_read(self._h, qi.ctypes.data, qc.ctypes.data, f.ctypes.data, 0), 'fb_inverse_read')
+        return qi, qc, f
 
     def reset(self, qpos=None, qvel=None, env_ids=None):
         n = self.n_envs if env_ids is None else len(env_ids)

@@ -494,6 +494,24 @@ int fb_ik_solve(FbHandle h, int n, const float* target_xpos, const float* init_q
  * last check; err_first: the site term at the returned qpos; steps: the loop index at the stop (max_steps - 1 without success);
  * success: 1 when the progress test stopped the problem.                                                                   */
 int fb_ik_read(FbHandle h, float* qpos, float* err, float* err_first, int32_t* steps, uint8_t* success);
+/* Inverse dynamics (MuJoCo mj_inverse, continuous time; dm_control `mjlib.mj_inverse` then `data.qfrc_inverse`, `data.efc_force`):
+ * the forces that give envs 0 .. n-1 the accelerations qacc [n][nv] (host rows, or a device pointer on the handle's stream when
+ * is_device) at their current qpos, qvel and act.  Runs the position / velocity stage of every env (the launches fb_forward starts
+ * with, without sensor sums), then one inverse kernel; it writes nothing else into the record, so on a current state (after fb_reset,
+ * fb_forward or fb_step) the record is bit for bit unchanged and the next fb_step is too.  Per problem:
+ *   efc_force       = the soft constraint model's forces at jar = J qacc - aref, aref = -B J qvel - K imp (pos - margin)
+ *                     (mj_constraintUpdate: limits, frictionless and elliptic contacts);
+ *   qfrc_constraint = J^T efc_force;  qfrc_inverse = M qacc + qfrc_bias - qfrc_passive - qfrc_constraint.
+ * qfrc_inverse excludes applied and actuator forces: for the continuous-time qacc fb_forward leaves in FB_QACC it equals
+ * qfrc_applied + J^T xfrc_applied + qfrc_actuator up to the forward solve's tolerance.  Noslip is not inverted (as in MuJoCo): on a
+ * model with noslip iterations the forces are the soft model's, not the forward step's post-noslip friction.  The discrete inverse
+ * (mjENBL_INVDISCRETE) is not implemented.  Errors: n outside 1 .. n_envs, a NULL qacc, a non-finite host qacc.  A device qacc is
+ * not checked and the call returns without synchronising; with a host qacc it synchronises.                                    */
+int fb_inverse(FbHandle h, int n, const float* qacc, int is_device);
+/* Results of the last fb_inverse for its n problems (synchronises; any pointer may be NULL; is_device: the pointers are device
+ * memory): qfrc_inverse [n][nv], qfrc_constraint [n][nv], efc_force [n][fb_field_size(FB_EFC_FORCE)], rows as FB_CONTACT's efc_adr
+ * and FB_NEFC index them after the call (rows >= nefc hold 0).  An error before the first fb_inverse.                         */
+int fb_inverse_read(FbHandle h, float* qfrc_inverse, float* qfrc_constraint, float* efc_force, int is_device);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
