@@ -30,42 +30,16 @@
 #include "fb_ik.h"
 #include "fb_inverse.h"
 
-#ifdef FB_EMU
-typedef int cudaStream_t_;
-#endif
-
-// -------------------------------------------------------------------------------------------
-// memory / launch abstraction
-#ifndef FB_EMU
-#define FB_CUDA_OK(call) do { cudaError_t err_ = (call); if (err_ != cudaSuccess) { s->err = std::string(#call) + ": " + cudaGetErrorString(err_); return -2; } } while (0)
-static void* dev_alloc(size_t bytes) {   // rare (create / first use): zero-fill and make it visible to every stream
-  void* p = nullptr; if (cudaMalloc(&p, bytes ? bytes : 4) != cudaSuccess) return nullptr; cudaMemset(p, 0, bytes ? bytes : 4); cudaDeviceSynchronize(); return p; }
-static void dev_free(void* p) { cudaFree(p); }
-static void h2d(void* dst, const void* src, size_t n) { cudaMemcpy(dst, src, n, cudaMemcpyHostToDevice); cudaDeviceSynchronize(); }
-static void d2h(void* dst, const void* src, size_t n) { cudaMemcpy(dst, src, n, cudaMemcpyDeviceToHost); }
-#else
-#define FB_CUDA_OK(call) do { } while (0)
-static void* dev_alloc(size_t bytes) { return calloc(bytes ? bytes : 4, 1); }
-static void dev_free(void* p) { free(p); }
-static void h2d(void* dst, const void* src, size_t n) { memcpy(dst, src, n); }
-static void d2h(void* dst, const void* src, size_t n) { memcpy(dst, src, n); }
-#endif
-
 enum { K_ACT = 0, K_SMOOTH, K_REF, K_SOLVE, K_FINISH, K_POS, K_COL, K_CON, K_PROJ, K_VEL, K_SENS, K_PACK, K_MISC, K_NKIND };
 static const char* const kKindNames[K_NKIND] = {"act", "smooth", "ref", "solve", "finish", "pos", "col", "con", "proj", "vel", "sens", "pack", "misc"};
-#ifndef FB_EMU
-struct ProfEvent { int kind; cudaEvent_t a, b; };
-#endif
 struct FbSim {
   DevModel m; DevData d;
   int prof_on; double prof_ms[K_NKIND]; long long prof_n[K_NKIND];
-#ifndef FB_EMU
-  std::vector<ProfEvent> prof_events;
-#endif
   FbModel hm;                       // host copy of scalar fields (pointers invalid after create)
   std::vector<void*> allocs;
   std::vector<void*> obs_scope, task_scope;   // device buffers of the current observation / task program: freed when the program is replaced
   std::vector<void*> applied_scope;           // qfrc_applied / xfrc_applied: freed by fb_clear_applied
+  std::vector<void*> ref_scope, bank_scope;   // reference slots (fb_ref_slots) / terrain bank (fb_hfield_bank): freed when replaced
   std::vector<int> h_dof_parent, h_dof_Madr, h_body_parent;
   std::vector<int> h_jnt_type, h_jnt_qadr, h_jnt_dofadr, h_jnt_body, h_site_body;   // joint / site tables an IK program is checked and built against
   std::vector<double> h_qpos0;
@@ -90,12 +64,96 @@ struct FbSim {
   std::vector<char> st_written;            // per slot: 0 never written, 1 written, 2 written while an env may be held for its reset
   int* st_ids_dev = nullptr; int st_ids_cap = 0;
 #ifndef FB_EMU
+  struct ProfEvent { int kind; cudaEvent_t a, b; };
+  std::vector<ProfEvent> prof_events;
   cudaStream_t stream; cudaEvent_t ev0, ev1;
   struct StepGraph { cudaGraphExec_t exec; bool seen, failed; int n_sub; long long launches; DevData d; DevModel m; };
   StepGraph graph[2];          // [hold pending?]
   bool graphs_on;
 #endif
 };
+
+// -------------------------------------------------------------------------------------------
+// host / device seam: the one place that knows whether there is a device.  Under FB_EMU "device" memory is host memory, a copy
+// is a memcpy that is done when it returns, and a launch runs its envs one after the other (emu_launch).
+#ifndef FB_EMU
+#define FB_CUDA_OK(call) do { cudaError_t err_ = (call); if (err_ != cudaSuccess) { s->err = std::string(#call) + ": " + cudaGetErrorString(err_); return -2; } } while (0)
+static const char* const kVersion = "flybody_b200 0.2 (sm_90a)";
+static void* dev_alloc(size_t bytes) {   // rare (create / first use): zero-fill and make it visible to every stream
+  void* p = nullptr; if (cudaMalloc(&p, bytes ? bytes : 4) != cudaSuccess) return nullptr; cudaMemset(p, 0, bytes ? bytes : 4); cudaDeviceSynchronize(); return p; }
+static void dev_free(void* p) { cudaFree(p); }
+static int dev_open(FbSim* s, int n_envs) {
+  if (cudaSetDevice(s->device) != cudaSuccess) return -2;
+  cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
+  cudaEventCreate(&s->ev0); cudaEventCreate(&s->ev1);
+  s->graphs_on = getenv("FB_NO_GRAPH") == nullptr;
+  // small batches are latency-bound (a per-CTA copy of the sweep program in shared memory halves the sweeps' latency);
+  // at full occupancy the copy costs more than it saves and the compact program is read in place.  FB_BLOB=0/1 overrides.
+  s->blob_in_smem = getenv("FB_BLOB") ? atoi(getenv("FB_BLOB")) : (n_envs <= 1024);
+  return 0;
+}
+static void dev_close(FbSim* s) {
+  cudaSetDevice(s->device); cudaStreamSynchronize(s->stream);
+  for (auto& g : s->graph) if (g.exec) cudaGraphExecDestroy(g.exec);
+  cudaEventDestroy(s->ev0); cudaEventDestroy(s->ev1); cudaStreamDestroy(s->stream);
+}
+static void dev_select(FbSim* s) { cudaSetDevice(s->device); }
+// stream-ordered copies in any direction (the handle's stream is non-blocking: legacy default-stream copies would not order with
+// its kernels); copy_rows_async moves `rows` rows of `width` bytes, `spitch` bytes apart in the source and `dpitch` in the destination
+static int copy_async(FbSim* s, void* dst, const void* src, size_t bytes) {
+  FB_CUDA_OK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, s->stream));
+  return 0;
+}
+static int copy_rows_async(FbSim* s, void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t rows) {
+  FB_CUDA_OK(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, rows, cudaMemcpyDefault, s->stream));
+  return 0;
+}
+static int sync_stream(FbSim* s) {
+  FB_CUDA_OK(cudaStreamSynchronize(s->stream));
+  FB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+static int launch_check(FbSim* s, const char* who) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { s->err = std::string(who) + ": kernel launch failed (" + cudaGetErrorString(e) + ")"; return -2; }
+  return 0;
+}
+static size_t dev_free_bytes() {      // (no answer: no limit)
+  size_t free_b = 0, total_b = 0;
+  return cudaMemGetInfo(&free_b, &total_b) == cudaSuccess ? free_b : std::numeric_limits<size_t>::max();
+}
+#else
+static const char* const kVersion = "flybody_b200 0.2 (host emulation build: tests only)";
+static void* dev_alloc(size_t bytes) { return calloc(bytes ? bytes : 4, 1); }
+static void dev_free(void* p) { free(p); }
+static int dev_open(FbSim*, int) { return 0; }
+static void dev_close(FbSim*) {}
+static void dev_select(FbSim*) {}
+static int copy_async(FbSim*, void* dst, const void* src, size_t bytes) { memcpy(dst, src, bytes); return 0; }
+static int copy_rows_async(FbSim*, void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t rows) {
+  for (size_t r = 0; r < rows; r++) memcpy((char*)dst + r * dpitch, (const char*)src + r * spitch, width);
+  return 0;
+}
+static int sync_stream(FbSim*) { return 0; }
+static int launch_check(FbSim*, const char*) { return 0; }
+static size_t dev_free_bytes() { return std::numeric_limits<size_t>::max(); }
+// One emulated launch: the envs of [0, n), or of the list `ids`, one after the other, each through a zeroed slice exactly as large
+// as the GPU launch makes a warp's shared memory, followed by a canary: a kernel that writes past its slice (on the GPU: into the
+// next warp's slice or out of the block's allocation) aborts the CPU tests instead of passing.
+template <typename Body> static void emu_launch(FbSim* s, const char* kernel, size_t slice, int n, const int* ids, Body body) {
+  std::vector<unsigned char> buf(slice + 256, 0);
+  memset(buf.data() + slice, 0xAB, 256);
+  for (int k = 0; k < n; k++) body(buf.data(), ids ? ids[k] : k);
+  for (size_t i = 0; i < 256; i++)
+    if (buf[slice + i] != 0xAB) { fprintf(stderr, "fb_emu: shared-memory slice overrun in the %s kernel (slice %zu bytes)\n", kernel, slice); abort(); }
+  s->launches++;
+}
+#endif
+// a copy whose source the caller may reuse (or whose destination it reads) once the call returns
+static int copy_sync(FbSim* s, void* dst, const void* src, size_t bytes) {
+  const int rc = copy_async(s, dst, src, bytes);
+  return rc != 0 ? rc : sync_stream(s);
+}
 
 static size_t slice_bytes(size_t fixed, size_t dyn_floats) { return ((((fixed + 15) & ~(size_t)15) + dyn_floats * sizeof(float)) + 15) & ~(size_t)15; }
 // kernel = sequence of stages for one env.  Ph<f>: per-lane phase f(m, d, sh, e, y), a warp barrier follows;
@@ -145,27 +203,34 @@ __global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_run(DevModel m, DevDa
   ((St::run(m, d, sh, e, y), __syncwarp()), ...);
 #endif
 }
-template <typename Sh, typename... St>
-static void fb_launch(FbSim* s, int kind, size_t dyn_floats = 0, int nwarps = -1, int blob_words = 0) {
-  if (nwarps < 0) nwarps = s->d.Np;          // step kernels cover the padded batch
+// a step-stage launch on the handle's stream, between a pair of events while fb_profile is on
+template <typename L> static void dev_launch(FbSim* s, int kind, L launch) {
 #ifdef FB_CLK
   s->d.clk_launch = (int)(s->launches % 4096);
 #endif
+  if (s->prof_on) {
+    cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
+    cudaEventRecord(a, s->stream);
+    launch();
+    cudaEventRecord(b, s->stream);
+    s->prof_events.push_back({kind, a, b});
+  } else {
+    launch();
+  }
+  s->launches++;
+}
+static void prof_collect(FbSim* s) {      // the recorded launches into prof_ms / prof_n (the stream is idle)
+  for (auto& ev : s->prof_events) { float t = 0; cudaEventElapsedTime(&t, ev.a, ev.b); s->prof_ms[ev.kind] += t; s->prof_n[ev.kind]++; cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
+  s->prof_events.clear();
+}
+template <typename Sh, typename... St>
+static void fb_launch(FbSim* s, int kind, size_t dyn_floats = 0, int nwarps = -1, int blob_words = 0) {
+  if (nwarps < 0) nwarps = s->d.Np;          // step kernels cover the padded batch
   dim3 block(32, FB_WPB), grid((nwarps + FB_WPB - 1) / FB_WPB);
   size_t slice = slice_bytes(sizeof(Sh), dyn_floats), bytes = slice * FB_WPB + (size_t)blob_words * 4;
   static size_t configured = 0;
   if (bytes > configured) { cudaFuncSetAttribute(fb_run<Sh, St...>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); configured = bytes; }
-  cudaStream_t st = s->stream;
-  if (s->prof_on) {
-    cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
-    cudaEventRecord(a, st);
-    fb_run<Sh, St...><<<grid, block, bytes, st>>>(s->m, s->d, (int)slice, 0, nwarps, blob_words);
-    cudaEventRecord(b, st);
-    s->prof_events.push_back({kind, a, b});
-  } else {
-    fb_run<Sh, St...><<<grid, block, bytes, st>>>(s->m, s->d, (int)slice, 0, nwarps, blob_words);
-  }
-  s->launches++;
+  dev_launch(s, kind, [&] { fb_run<Sh, St...><<<grid, block, bytes, s->stream>>>(s->m, s->d, (int)slice, 0, nwarps, blob_words); });
 }
 __global__ void __launch_bounds__(32 * FB_SOLVE_WPB, FB_MINB) fb_run_solve(DevModel m, DevData d, int nwarps) {
   extern __shared__ __align__(16) float fb_smem_w[];
@@ -180,50 +245,31 @@ __global__ void __launch_bounds__(32 * FB_SOLVE_WPB, FB_MINB) fb_run_solve(DevMo
 #endif
 }
 static void fb_launch_warp(FbSim* s, int kind) {
-#ifdef FB_CLK
-  s->d.clk_launch = (int)(s->launches % 4096);
-#endif
   dim3 block(32, FB_SOLVE_WPB), grid((s->d.Np + FB_SOLVE_WPB - 1) / FB_SOLVE_WPB);
   size_t bytes = sizeof(float) * FB_SOLVE_WARP_FLOATS * FB_SOLVE_WPB;
   static bool configured = false;
   if (!configured) { cudaFuncSetAttribute(fb_run_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); configured = true; }
-  cudaStream_t st = s->stream;
-  if (s->prof_on) {
-    cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
-    cudaEventRecord(a, st);
-    fb_run_solve<<<grid, block, bytes, st>>>(s->m, s->d, s->d.Np);
-    cudaEventRecord(b, st);
-    s->prof_events.push_back({kind, a, b});
-  } else {
-    fb_run_solve<<<grid, block, bytes, st>>>(s->m, s->d, s->d.Np);
-  }
-  s->launches++;
+  dev_launch(s, kind, [&] { fb_run_solve<<<grid, block, bytes, s->stream>>>(s->m, s->d, s->d.Np); });
 }
 #else
 template <typename Sh> static void set_prog(Sh&, const unsigned*) {}
 static void set_prog(ShTree& sh, const unsigned* p) { sh.prog = p; }
+static void prof_collect(FbSim*) {}
+// the stage list St over the envs of [0, n) or of the list `ids`
+template <typename Sh, typename... St> static void emu_stages(FbSim* s, int kind, size_t dyn_floats, int n, const int* ids) {
+  emu_launch(s, kKindNames[kind], slice_bytes(sizeof(Sh), dyn_floats), n, ids, [&](unsigned char* buf, int e) {
+    Sh& sh = *reinterpret_cast<Sh*>(buf);
+    set_prog(sh, s->m.tsolve_blob);        // host emulation: the program is read in place
+    (St::emu(s->m, s->d, sh, e), ...);
+  });
+}
 template <typename Sh, typename... St>
-static void fb_launch(FbSim* s, int kind, size_t dyn_floats = 0, int nwarps = -1, int blob_words = 0) {
-  (void)kind;
-  if (nwarps < 0) nwarps = s->d.Np;
-  // the slice is exactly as large as the GPU launch makes it, followed by a canary: a phase that writes past its shared-memory
-  // slice (on the GPU: into the next warp's slice or out of the block's allocation) aborts the CPU tests instead of passing
-  const size_t used = slice_bytes(sizeof(Sh), dyn_floats);
-  std::vector<unsigned char> buf(used + 256, 0);
-  memset(buf.data() + used, 0xAB, 256);
-  Sh& sh = *reinterpret_cast<Sh*>(buf.data());
-  (void)blob_words; set_prog(sh, s->m.tsolve_blob);        // host emulation: the program is read in place
-  for (int e = 0; e < nwarps; e++) (St::emu(s->m, s->d, sh, e), ...);
-  for (size_t i = 0; i < 256; i++) if (buf[used + i] != 0xAB) { fprintf(stderr, "fb_emu: shared-memory slice overrun in a kernel of kind %d (slice %zu bytes)\n", kind, used); abort(); }
-  s->launches++;
+static void fb_launch(FbSim* s, int kind, size_t dyn_floats = 0, int nwarps = -1, int = 0) {
+  emu_stages<Sh, St...>(s, kind, dyn_floats, nwarps < 0 ? s->d.Np : nwarps, nullptr);
 }
 static void fb_launch_warp(FbSim* s, int kind) {
-  const size_t used = sizeof(float) * FB_SOLVE_WARP_FLOATS;      // as fb_launch: the slice as the GPU launch sizes it, then a canary
-  std::vector<unsigned char> buf(used + 256, 0);
-  memset(buf.data() + used, 0xAB, 256);
-  for (int e = 0; e < s->d.Np; e++) ksolve_warp(s->m, s->d, reinterpret_cast<float*>(buf.data()), e);
-  for (size_t i = 0; i < 256; i++) if (buf[used + i] != 0xAB) { fprintf(stderr, "fb_emu: shared-memory slice overrun in a kernel of kind %d (slice %zu bytes)\n", kind, used); abort(); }
-  s->launches++;
+  emu_launch(s, kKindNames[kind], sizeof(float) * FB_SOLVE_WARP_FLOATS, s->d.Np, nullptr,
+             [&](unsigned char* buf, int e) { ksolve_warp(s->m, s->d, reinterpret_cast<float*>(buf), e); });
 }
 #endif
 
@@ -231,25 +277,6 @@ static void fb_launch_warp(FbSim* s, int kind) {
 FB_DEV void ph_reset_scatter(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kreset_scatter(m, d, e, y); }
 FB_DEV void ph_scatter(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kscatter(m, d, e, y); }
 FB_DEV void ph_clear_hold(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kclear_hold(m, d, e, y); }
-// heightfield contacts: DevHf travels in its own kernel (not in DevModel / DevData: the step kernels of models without a
-// heightfield keep their parameter layout)
-#ifndef FB_EMU
-__global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_hf_kernel(DevModel m, DevData d, DevHf p, int nwarps) {
-  const int e = blockIdx.x * FB_WPB + threadIdx.y;
-  if (e >= nwarps) return;
-  khf_narrow(m, d, p, e, threadIdx.x); __syncwarp();
-  khf_append(m, d, p, e, threadIdx.x);
-}
-#endif
-static void launch_hfield(FbSim* s) {
-#ifndef FB_EMU
-  dim3 block(32, FB_WPB), grid((s->d.N + FB_WPB - 1) / FB_WPB);
-  fb_hf_kernel<<<grid, block, 0, s->stream>>>(s->m, s->d, s->hf, s->d.N);
-#else
-  for (int e = 0; e < s->d.N; e++) { for (int y = 0; y < FB_NY; y++) khf_narrow(s->m, s->d, s->hf, e, y); for (int y = 0; y < FB_NY; y++) khf_append(s->m, s->d, s->hf, e, y); }
-#endif
-  s->launches++;
-}
 FB_DEV void ph_task_reset(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reset(m, d, e, y); }
 FB_DEV void ph_task_reset2(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reset2(m, d, e, y); }
 FB_DEV void ph_task_reset3(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reset3(m, d, e, y); }
@@ -287,17 +314,18 @@ static size_t dyn_proj(const DevModel&) { return (size_t)FB_NY * FB_ZCAP; }
 static size_t dyn_vel(const DevModel&) { return (size_t)FB_PARTF; }
 static size_t dyn_tsolve(const DevModel& m) { return (size_t)(FB_NXS(m) + ((m.nM + 3) & ~3)); }
 
-static void launch_step1(FbSim* s) {
-  fb_launch<ShTree, FB_ST_POS>(s, K_POS, dyn_pos(s->m));
-  fb_launch<ShCol, FB_ST_COL>(s, K_COL, dyn_col(s->m));
-  if (s->hf_on) launch_hfield(s);              // heightfield contacts join the contact list before the constraint rows are built
-  fb_launch<ShCon, FB_ST_PROJ>(s, K_PROJ, dyn_proj(s->m));
-  fb_launch<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m));
-}
-// The position / velocity stage for a list of envs (fb_state_load recomputes what a state row does not carry), through the stage
-// functions of the step kernels.  One env per block: the collision stage pools the jobs of a block's envs on warp 0 and takes them
-// to be consecutive envs, so a listed env runs as warp 0 of a block whose other slices report no jobs.
+// Heightfield contacts: DevHf travels in its own kernel (not in DevModel / DevData: the step kernels of models without a
+// heightfield keep their parameter layout).  launch_hfield covers the envs of [0, n) or of a device list, as fb_launch_ids does
+// for the position / velocity stage (fb_state_load recomputes what a state row does not carry), through the stage functions of
+// the step kernels.  One env per block: the collision stage pools the jobs of a block's envs on warp 0 and takes them to be
+// consecutive envs, so a listed env runs as warp 0 of a block whose other slices report no jobs.
 #ifndef FB_EMU
+__global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_hf_kernel(DevModel m, DevData d, DevHf p, int nwarps) {
+  const int e = blockIdx.x * FB_WPB + threadIdx.y;
+  if (e >= nwarps) return;
+  khf_narrow(m, d, p, e, threadIdx.x); __syncwarp();
+  khf_append(m, d, p, e, threadIdx.x);
+}
 template <typename Sh, typename... St>
 __global__ void __launch_bounds__(32 * FB_WPB, FB_MINB) fb_run_ids(DevModel m, DevData d, int slice, const int* ids) {
   extern __shared__ __align__(16) unsigned char fb_smem[];
@@ -313,37 +341,62 @@ DevModel m, DevData d, DevHf p, const int* ids) {
   khf_narrow(m, d, p, e, threadIdx.x); __syncwarp();
   khf_append(m, d, p, e, threadIdx.x);
 }
-#endif
-template <typename Sh, typename... St>
-static void fb_launch_ids(FbSim* s, size_t dyn_floats, const int* ids_dev, const int* ids_host, int n) {
-  const size_t slice = slice_bytes(sizeof(Sh), dyn_floats);
-#ifndef FB_EMU
-  const size_t bytes = slice * FB_WPB; (void)ids_host;
-  static size_t configured = 0;
-  if (bytes > configured) { cudaFuncSetAttribute(fb_run_ids<Sh, St...>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); configured = bytes; }
-  fb_run_ids<Sh, St...><<<n, dim3(32, 1), bytes, s->stream>>>(s->m, s->d, (int)slice, ids_dev);
-#else
-  (void)ids_dev;
-  std::vector<unsigned char> buf(slice, 0);
-  Sh& sh = *reinterpret_cast<Sh*>(buf.data());
-  set_prog(sh, s->m.tsolve_blob);
-  for (int k = 0; k < n; k++) (St::emu(s->m, s->d, sh, ids_host[k]), ...);
-#endif
+static void launch_hfield(FbSim* s, const int* ids, int n) {
+  if (ids) fb_hf_kernel_ids<<<n, 32, 0, s->stream>>>(s->m, s->d, s->hf, ids);
+  else fb_hf_kernel<<<(n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->hf, n);
   s->launches++;
 }
-static void launch_step1_ids(FbSim* s, const int* ids_dev, const int* ids_host, int n) {
-  fb_launch_ids<ShTree, FB_ST_POS>(s, dyn_pos(s->m), ids_dev, ids_host, n);
-  fb_launch_ids<ShCol, FB_ST_COL>(s, dyn_col(s->m), ids_dev, ids_host, n);
-  if (s->hf_on) {
-#ifndef FB_EMU
-    fb_hf_kernel_ids<<<n, 32, 0, s->stream>>>(s->m, s->d, s->hf, ids_dev);
-#else
-    for (int k = 0; k < n; k++) { const int e = ids_host[k]; for (int y = 0; y < FB_NY; y++) khf_narrow(s->m, s->d, s->hf, e, y); for (int y = 0; y < FB_NY; y++) khf_append(s->m, s->d, s->hf, e, y); }
-#endif
-    s->launches++;
+template <typename Sh, typename... St>
+static void fb_launch_ids(FbSim* s, int, size_t dyn_floats, const int* ids, int n) {
+  const size_t slice = slice_bytes(sizeof(Sh), dyn_floats), bytes = slice * FB_WPB;
+  static size_t configured = 0;
+  if (bytes > configured) { cudaFuncSetAttribute(fb_run_ids<Sh, St...>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); configured = bytes; }
+  fb_run_ids<Sh, St...><<<n, dim3(32, 1), bytes, s->stream>>>(s->m, s->d, (int)slice, ids);
+  s->launches++;
+}
+static const void* step_kernel_fn(int kind) {
+  switch (kind) {
+    case K_SMOOTH: return (const void*)fb_run<ShTree, FB_ST_SMOOTH>;
+    case K_SOLVE: return (const void*)fb_run_solve;
+    case K_FINISH: return (const void*)fb_run<ShTree, FB_ST_FINISH>;
+    case K_POS: return (const void*)fb_run<ShTree, FB_ST_POS>;
+    case K_COL: return (const void*)fb_run<ShCol, FB_ST_COL>;
+    case K_PROJ: return (const void*)fb_run<ShCon, FB_ST_PROJ>;
+    case K_VEL: return (const void*)fb_run<ShTree, FB_ST_VEL>;
+    default: return nullptr;
   }
-  fb_launch_ids<ShCon, FB_ST_PROJ>(s, dyn_proj(s->m), ids_dev, ids_host, n);
-  fb_launch_ids<ShTree, FB_ST_VEL>(s, dyn_vel(s->m), ids_dev, ids_host, n);
+}
+// the occupancy query of fb_step_kernel_smem (0 under emulation)
+static int step_kernel_blocks_per_sm(FbSim* s, int kind, size_t bytes, int* blocks) {
+  FB_CUDA_OK(cudaSetDevice(s->device));
+  FB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks, step_kernel_fn(kind), 32 * FB_WPB, bytes));
+  return 0;
+}
+#else
+static void launch_hfield(FbSim* s, const int* ids, int n) {
+  emu_launch(s, "hfield", 0, n, ids, [&](unsigned char*, int e) {
+    for (int y = 0; y < FB_NY; y++) khf_narrow(s->m, s->d, s->hf, e, y);
+    for (int y = 0; y < FB_NY; y++) khf_append(s->m, s->d, s->hf, e, y);
+  });
+}
+template <typename Sh, typename... St>
+static void fb_launch_ids(FbSim* s, int kind, size_t dyn_floats, const int* ids, int n) { emu_stages<Sh, St...>(s, kind, dyn_floats, n, ids); }
+static int step_kernel_blocks_per_sm(FbSim*, int, size_t, int* blocks) { *blocks = 0; return 0; }
+#endif
+
+static void launch_step1(FbSim* s) {
+  fb_launch<ShTree, FB_ST_POS>(s, K_POS, dyn_pos(s->m));
+  fb_launch<ShCol, FB_ST_COL>(s, K_COL, dyn_col(s->m));
+  if (s->hf_on) launch_hfield(s, nullptr, s->d.N);     // heightfield contacts join the contact list before the constraint rows are built
+  fb_launch<ShCon, FB_ST_PROJ>(s, K_PROJ, dyn_proj(s->m));
+  fb_launch<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m));
+}
+static void launch_step1_ids(FbSim* s, const int* ids, int n) {      // ids: a device list
+  fb_launch_ids<ShTree, FB_ST_POS>(s, K_POS, dyn_pos(s->m), ids, n);
+  fb_launch_ids<ShCol, FB_ST_COL>(s, K_COL, dyn_col(s->m), ids, n);
+  if (s->hf_on) launch_hfield(s, ids, n);
+  fb_launch_ids<ShCon, FB_ST_PROJ>(s, K_PROJ, dyn_proj(s->m), ids, n);
+  fb_launch_ids<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m), ids, n);
 }
 static void launch_step2(FbSim* s, bool integrate) {
   s->d.do_integrate = integrate ? 1 : 0;     // read by the solve (warm-start bookkeeping) and the finish kernel
@@ -356,7 +409,7 @@ static void launch_step2(FbSim* s, bool integrate) {
 // model upload
 template <typename T> static const T* up(FbSim* s, const std::vector<T>& v) {
   void* p = dev_alloc(sizeof(T) * std::max<size_t>(v.size(), 1));
-  if (v.size()) h2d(p, v.data(), sizeof(T) * v.size());
+  if (p && v.size()) copy_sync(s, p, v.data(), sizeof(T) * v.size());
   s->allocs.push_back(p);
   return (const T*)p;
 }
@@ -372,6 +425,15 @@ template <typename T> static T* dalloc(FbSim* s, size_t n) { void* p = dev_alloc
 static void scope_free(FbSim* s, std::vector<void*>& scope) {
   for (void* p : scope) { if (!p) continue; for (auto& a : s->allocs) if (a == p) { a = nullptr; break; } dev_free(p); }
   scope.clear();
+}
+// the buffers `alloc` allocates (dalloc / up) become `scope`; if one of them is missing the whole group is freed again and the
+// call fails with `oom` as its message
+template <typename F> static int scope_alloc(FbSim* s, std::vector<void*>& scope, const char* oom, F alloc) {
+  const size_t mark = s->allocs.size();
+  alloc();
+  scope.assign(s->allocs.begin() + mark, s->allocs.end());
+  for (void* p : scope) if (!p) { scope_free(s, scope); s->err = oom; return -4; }
+  return 0;
 }
 
 static int build_model(FbSim* s, const FbModel* h) {
@@ -648,12 +710,8 @@ static int alloc_data(FbSim* s, int N) {
 // host <-> device transfers of one field: host side is AoS [N][n]; device side is n slots of every record
 static void field_to_host(FbSim* s, const void* dev, int n, void* dst) {
   if (n <= 0) return;
-#ifndef FB_EMU
-  cudaMemcpy2DAsync(dst, (size_t)n * 4, dev, (size_t)s->d.rec * 4, (size_t)n * 4, s->d.N, cudaMemcpyDeviceToHost, s->stream);
-  cudaStreamSynchronize(s->stream);
-#else
-  for (int e = 0; e < s->d.N; e++) memcpy((char*)dst + (size_t)e * n * 4, (const char*)dev + (size_t)e * s->d.rec * 4, (size_t)n * 4);
-#endif
+  copy_rows_async(s, dst, (size_t)n * 4, dev, (size_t)s->d.rec * 4, (size_t)n * 4, s->d.N);
+  sync_stream(s);
 }
 // padded device array (count elements of `width` floats every `stride` slots) -> compact host array [N][count * width]
 static void field_to_host_strided(FbSim* s, const void* dev, int count, int width, int stride, float* dst) {
@@ -664,37 +722,15 @@ static void field_to_host_strided(FbSim* s, const void* dev, int count, int widt
 }
 static void field_from_host(FbSim* s, void* dev, int n, const void* src) {
   if (n <= 0) return;
-#ifndef FB_EMU
-  // stream-ordered (the handle's stream is non-blocking: legacy default-stream copies would not order with its kernels)
-  cudaMemcpy2DAsync(dev, (size_t)s->d.rec * 4, src, (size_t)n * 4, (size_t)n * 4, s->d.N, cudaMemcpyHostToDevice, s->stream);
-  for (int e = s->d.N; e < s->d.Np; e++) cudaMemcpyAsync((char*)dev + (size_t)e * s->d.rec * 4, src, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream);   // pad envs mirror env 0
-  cudaStreamSynchronize(s->stream);
-#else
-  for (int e = 0; e < s->d.Np; e++) memcpy((char*)dev + (size_t)e * s->d.rec * 4, (const char*)src + (size_t)(e < s->d.N ? e : 0) * n * 4, (size_t)n * 4);
-#endif
+  copy_rows_async(s, dev, (size_t)s->d.rec * 4, src, (size_t)n * 4, (size_t)n * 4, s->d.N);
+  for (int e = s->d.N; e < s->d.Np; e++) copy_async(s, (char*)dev + (size_t)e * s->d.rec * 4, src, (size_t)n * 4);   // pad envs mirror env 0
+  sync_stream(s);
 }
 // device staging buffer for scatter-style uploads (ctrl, ghost pose, partial resets)
 static int ensure_stage(FbSim* s, size_t floats, size_t ints) {
-#ifndef FB_EMU
-  if (floats > s->stage_cap || ints > s->stage_icap) cudaDeviceSynchronize();
-#endif
+  if (floats > s->stage_cap || ints > s->stage_icap) sync_stream(s);
   if (floats > s->stage_cap) { s->stage = dalloc<float>(s, floats); s->stage_cap = floats; if (!s->stage) return -4; }
   if (ints > s->stage_icap) { s->stage_i = dalloc<int>(s, ints); s->stage_icap = ints; if (!s->stage_i) return -4; }
-  return 0;
-}
-static void upload_async(FbSim* s, void* dst, const void* src, size_t bytes) {
-#ifndef FB_EMU
-  cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s->stream);
-#else
-  memcpy(dst, src, bytes);
-#endif
-}
-
-static int sync_stream(FbSim* s) {
-#ifndef FB_EMU
-  FB_CUDA_OK(cudaStreamSynchronize(s->stream));
-  FB_CUDA_OK(cudaGetLastError());
-#endif
   return 0;
 }
 
@@ -714,23 +750,17 @@ static int ensure_applied(FbSim* s) {
   if (s->d.qfrc_applied) return 0;
   if (sync_stream(s) != 0) return -2;
   state_drop(s);
-  const size_t mark = s->allocs.size();
-  float* q = dalloc<float>(s, (size_t)s->d.Np * s->m.nv); float* x = dalloc<float>(s, (size_t)s->d.Np * 6 * s->m.nbody);
-  s->applied_scope.assign(s->allocs.begin() + mark, s->allocs.end());
-  if (!q || !x) { scope_free(s, s->applied_scope); s->err = "out of device memory (applied forces)"; return -4; }
+  float *q, *x;
+  if (int rc = scope_alloc(s, s->applied_scope, "out of device memory (applied forces)", [&] {
+        q = dalloc<float>(s, (size_t)s->d.Np * s->m.nv); x = dalloc<float>(s, (size_t)s->d.Np * 6 * s->m.nbody); }))
+    return rc;
   s->d.qfrc_applied = q; s->d.xfrc_applied = x;      // the step graph is captured again: DevData changed
   return 0;
 }
 
 extern "C" {
 
-const char* fb_version(void) {
-#ifdef FB_EMU
-  return "flybody_b200 0.2 (host emulation build: tests only)";
-#else
-  return "flybody_b200 0.2 (sm_90a)";
-#endif
-}
+const char* fb_version(void) { return kVersion; }
 
 int fb_create(const FbModel* hm, int n_envs, int device, FbHandle* out) {
   if (!hm || !out || n_envs <= 0) return -1;
@@ -739,22 +769,11 @@ int fb_create(const FbModel* hm, int n_envs, int device, FbHandle* out) {
   s->ref_slots = nullptr; s->ref_slot_len = 0; s->eye_out = nullptr; s->hfield_dev = nullptr; s->hmax_dev = nullptr; s->cmax_dev = nullptr; s->hf_nbr = s->hf_nbc = 0; s->bank_dev = s->bank_hmax_dev = s->bank_cmax_dev = nullptr; s->bank_n = 0; s->eye_bytes = 0; s->hf_on = false; s->hf_nrow = s->hf_ncol = 0;
   s->rbank_dev = nullptr; s->rbank_off_dev = s->rbank_len_dev = nullptr; s->rbank_w = 0;
   s->op_step_dev = nullptr; s->op_first_dev = nullptr; s->stage_cap = 0; s->stage_icap = 0; s->stage = nullptr; s->stage_i = nullptr;
-#ifndef FB_EMU
-  if (cudaSetDevice(device) != cudaSuccess) { delete s; return -2; }
-  cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-  cudaEventCreate(&s->ev0); cudaEventCreate(&s->ev1);
-  s->graphs_on = getenv("FB_NO_GRAPH") == nullptr;
-  // small batches are latency-bound (a per-CTA copy of the sweep program in shared memory halves the sweeps' latency);
-  // at full occupancy the copy costs more than it saves and the compact program is read in place.  FB_BLOB=0/1 overrides.
-  s->blob_in_smem = getenv("FB_BLOB") ? atoi(getenv("FB_BLOB")) : (n_envs <= 1024);
-#endif
-  int rc = build_model(s, hm);
+  if (dev_open(s, n_envs) != 0) { delete s; return -2; }
+  int rc = build_model(s, hm);             // (every upload and allocation has completed when it returns)
   if (rc == 0) rc = alloc_data(s, n_envs);
   *out = s;
   if (rc != 0) return rc;
-#ifndef FB_EMU
-  cudaDeviceSynchronize();                 // model uploads / memsets ran on the legacy stream
-#endif
   std::vector<float> q0((size_t)n_envs * hm->nq);
   for (int e = 0; e < n_envs; e++) for (int i = 0; i < hm->nq; i++) q0[(size_t)e * hm->nq + i] = (float)hm->qpos0[i];
   field_from_host(s, s->d.qpos, hm->nq, q0.data());
@@ -763,11 +782,7 @@ int fb_create(const FbModel* hm, int n_envs, int device, FbHandle* out) {
 
 int fb_destroy(FbHandle s) {
   if (!s) return -1;
-#ifndef FB_EMU
-  cudaSetDevice(s->device); cudaStreamSynchronize(s->stream);
-  for (auto& g : s->graph) if (g.exec) cudaGraphExecDestroy(g.exec);
-  cudaEventDestroy(s->ev0); cudaEventDestroy(s->ev1); cudaStreamDestroy(s->stream);
-#endif
+  dev_close(s);
   for (void* p : s->allocs) dev_free(p);
   delete s;
   return 0;
@@ -800,20 +815,6 @@ int fb_n_envs(FbHandle s) { return s ? s->d.N : -1; }
 int fb_n_envs_padded(FbHandle s) { return s ? s->d.Np : -1; }
 int fb_record_stride(FbHandle s) { return s ? (int)s->d.rec : -1; }
 long long fb_launch_count(FbHandle s) { return s ? s->launches : -1; }
-float fb_last_step_ms(FbHandle s) {
-#ifndef FB_EMU
-  if (!s) return -1; float ms = 0; cudaEventSynchronize(s->ev1); cudaEventElapsedTime(&ms, s->ev0, s->ev1); return ms;
-#else
-  return 0;
-#endif
-}
-void* fb_stream(FbHandle s) {
-#ifndef FB_EMU
-  return s ? (void*)s->stream : nullptr;
-#else
-  return nullptr;
-#endif
-}
 int fb_sync(FbHandle s) { if (!s) return -1; return sync_stream(s); }
 int fb_set_solver(FbHandle s, float tolerance, int max_iter) {
   if (!s) return -1;
@@ -824,9 +825,7 @@ int fb_set_solver(FbHandle s, float tolerance, int max_iter) {
 
 int fb_forward(FbHandle s) {
   if (!s) return -1;
-#ifndef FB_EMU
-  cudaSetDevice(s->device);
-#endif
+  dev_select(s);
   launch_step1(s);
   launch_step2(s, false);
   return sync_stream(s);
@@ -853,14 +852,10 @@ static DevData canonical(const DevData& d) {
   c.rst_ids = nullptr; c.rst_qpos = nullptr; c.rst_qvel = nullptr; c.rst_n = 0; c.rst_has_qvel = 0; c.rst_hold = 0;
   return c;
 }
-#endif
-int fb_step(FbHandle s, int n_substeps) {
-  if (!s || n_substeps <= 0) return -1;
-#ifndef FB_EMU
-  cudaSetDevice(s->device);
+// One control step, between the events fb_last_step_ms reads.  Its 7 n launches are replayed from a CUDA graph: captured the
+// second time the same (n_substeps, hold) signature is stepped with unchanged handle state, so the first call still runs (and configures) plain launches.
+static void step_run(FbSim* s, int n_substeps) {
   cudaEventRecord(s->ev0, s->stream);
-  // The 7 n launches of a control step are replayed from a CUDA graph: captured the second time the same (n_substeps,
-  // hold) signature is stepped with unchanged handle state, so the first call still runs (and configures) plain launches.
   const int hold = s->hold_pending ? 1 : 0;
   bool done = false;
   if (s->graphs_on && !s->prof_on) {
@@ -889,11 +884,25 @@ int fb_step(FbHandle s, int n_substeps) {
   }
   if (!done) step_sequence(s, n_substeps);
   cudaEventRecord(s->ev1, s->stream);
-  if (cudaGetLastError() != cudaSuccess) { s->err = "kernel launch failed"; return -2; }
+}
+static void graphs_drop(FbSim* s) {       // the launch sequence changed
+  for (auto& g : s->graph) { if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; } g.seen = false; }
+}
+float fb_last_step_ms(FbHandle s) {
+  if (!s) return -1; float ms = 0; cudaEventSynchronize(s->ev1); cudaEventElapsedTime(&ms, s->ev0, s->ev1); return ms;
+}
+void* fb_stream(FbHandle s) { return s ? (void*)s->stream : nullptr; }
 #else
-  step_sequence(s, n_substeps);
+static void step_run(FbSim* s, int n_substeps) { step_sequence(s, n_substeps); }
+static void graphs_drop(FbSim*) {}
+float fb_last_step_ms(FbHandle) { return 0; }
+void* fb_stream(FbHandle) { return nullptr; }
 #endif
-  return 0;
+int fb_step(FbHandle s, int n_substeps) {
+  if (!s || n_substeps <= 0) return -1;
+  dev_select(s);
+  step_run(s, n_substeps);
+  return launch_check(s, "fb_step");
 }
 
 static void* field_ptr(FbSim* s, int field, int* n) {
@@ -944,7 +953,8 @@ int fb_get(FbHandle s, int field, void* dst, int is_device) {
   if (field == FB_QFRC_APPLIED || field == FB_XFRC_APPLIED) {
     if (is_device) { s->err = "applied forces are compact [n_envs][n] arrays, not record fields: use fb_applied_ptrs"; return -1; }
     const float* a = applied_ptr(s, field, &n);
-    if (a) d2h(dst, a, sizeof(float) * (size_t)N * n); else memset(dst, 0, sizeof(float) * (size_t)N * n);      // unset = zero
+    if (a) return copy_sync(s, dst, a, sizeof(float) * (size_t)N * n);
+    memset(dst, 0, sizeof(float) * (size_t)N * n);      // unset = zero
     return 0;
   }
   if (is_device) { if (!p) { s->err = "field has no device array"; return -1; } *(void**)dst = p; return 0; }
@@ -1011,8 +1021,7 @@ int fb_set(FbHandle s, int field, const float* src) {
     int rc = ensure_applied(s);
     if (rc != 0) return rc;
     float* a = applied_ptr(s, field, &n);
-    h2d(a, src, sizeof(float) * (size_t)s->d.N * n);      // (pad envs keep zero applied forces)
-    return 0;
+    return copy_sync(s, a, src, sizeof(float) * (size_t)s->d.N * n);      // (pad envs keep zero applied forces)
   }
   void* p = field_ptr(s, field, &n);
   if (!p || !(field == FB_QPOS || field == FB_QVEL || field == FB_ACT || field == FB_CTRL || field == FB_QACC_WARMSTART || field == FB_QACC || field == FB_TIME)) { s->err = "field is not writable"; return -1; }
@@ -1033,11 +1042,11 @@ int fb_set_ctrl(FbHandle s, const float* ctrl, int is_device) {
   const int k = s->act_map_dev ? s->n_action : s->m.nu;     // row length: actions (mapped on the device) or ctrl
   if (!is_device) {
     if (ensure_stage(s, (size_t)s->d.N * std::max(k, s->m.nu), 0) != 0) { s->err = "out of device memory (staging)"; return -4; }
-    upload_async(s, s->stage, ctrl, sizeof(float) * (size_t)s->d.N * k);
+    if (copy_async(s, s->stage, ctrl, sizeof(float) * (size_t)s->d.N * k) != 0) return -2;
     src = s->stage;
   }
   launch_scatter(s, s->d.ctrl, s->act_map_dev, src, k, s->act_map_dev ? 1 : 0);
-  return 0;
+  return launch_check(s, "fb_set_ctrl");
 }
 int fb_set_action_map(FbHandle s, const int32_t* ctrl_index, int n_action) {
   if (!s) return -1;
@@ -1064,10 +1073,9 @@ int fb_write_state(FbHandle s, int field, const int32_t* idx, int k, const float
   int slot = s->ws_slot++ & 3;
   float* vdev = s->stage + (size_t)s->d.N * s->m.nu + (size_t)slot * s->d.N * 16;
   int* idev = s->stage_i + slot * 16;
-  upload_async(s, idev, idx, sizeof(int) * k);
-  upload_async(s, vdev, vals, sizeof(float) * (size_t)s->d.N * k);
+  if (copy_async(s, idev, idx, sizeof(int) * k) != 0 || copy_async(s, vdev, vals, sizeof(float) * (size_t)s->d.N * k) != 0) return -2;
   launch_scatter(s, p, idev, vdev, k, 0, applied ? (unsigned)n : 0u);
-  return 0;
+  return launch_check(s, "fb_write_state");
 }
 int fb_applied_ptrs(FbHandle s, void** qfrc_dev, void** xfrc_dev) {
   if (!s) return -1;
@@ -1105,12 +1113,10 @@ static int do_reset(FbSim* s, const int32_t* env_ids, int n, const float* qpos, 
     s->rst_cap = std::max(cnt, Np);
     s->rst_ids_dev = dalloc<int>(s, s->rst_cap); s->rst_qpos_dev = dalloc<float>(s, (size_t)s->rst_cap * m.nq); s->rst_qvel_dev = dalloc<float>(s, (size_t)s->rst_cap * m.nv);
   }
-  upload_async(s, s->rst_ids_dev, ids.data(), sizeof(int) * cnt);
-  upload_async(s, s->rst_qpos_dev, qp.data(), sizeof(float) * qp.size());
-  if (qvel) upload_async(s, s->rst_qvel_dev, qv.data(), sizeof(float) * qv.size());
-#ifndef FB_EMU
-  cudaStreamSynchronize(s->stream);       // the host vectors go out of scope below
-#endif
+  copy_async(s, s->rst_ids_dev, ids.data(), sizeof(int) * cnt);
+  copy_async(s, s->rst_qpos_dev, qp.data(), sizeof(float) * qp.size());
+  if (qvel) copy_async(s, s->rst_qvel_dev, qv.data(), sizeof(float) * qv.size());
+  if (sync_stream(s) != 0) return -2;       // the host vectors go out of scope below
   s->d.rst_ids = s->rst_ids_dev; s->d.rst_qpos = s->rst_qpos_dev; s->d.rst_qvel = s->rst_qvel_dev; s->d.rst_n = cnt; s->d.rst_has_qvel = qvel ? 1 : 0; s->d.rst_hold = hold;
   fb_launch<ShNone, Ph<ph_reset_scatter>>(s, K_MISC, 0, cnt);
   s->d.rst_n = 0;
@@ -1124,8 +1130,9 @@ int fb_reset(FbHandle s, const int32_t* env_ids, int n, const float* qpos, const
 int fb_reset_hold(FbHandle s, const int32_t* env_ids, int n, const float* qpos, const float* qvel) {
   if (!s || !env_ids || !qpos || n <= 0) return -1;
   int rc = do_reset(s, env_ids, n, qpos, qvel, 1);
-  if (rc == 0) s->hold_pending = 1;
-  return rc;
+  if (rc != 0) return rc;
+  s->hold_pending = 1;
+  return launch_check(s, "fb_reset_hold");
 }
 
 int fb_profile(FbHandle s, int enable) {
@@ -1136,11 +1143,8 @@ int fb_profile(FbHandle s, int enable) {
 }
 int fb_profile_read(FbHandle s, double* ms, long long* counts, int n) {
   if (!s || !ms || !counts) return -1;
-#ifndef FB_EMU
   if (sync_stream(s) != 0) return -2;
-  for (auto& ev : s->prof_events) { float t = 0; cudaEventElapsedTime(&t, ev.a, ev.b); s->prof_ms[ev.kind] += t; s->prof_n[ev.kind]++; cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
-  s->prof_events.clear();
-#endif
+  prof_collect(s);
   for (int k = 0; k < n && k < K_NKIND; k++) { ms[k] = s->prof_ms[k]; counts[k] = s->prof_n[k]; }
   return K_NKIND;
 }
@@ -1159,32 +1163,12 @@ static size_t step_kernel_bytes(const FbSim* s, int kind) {
     default: return 0;
   }
 }
-#ifndef FB_EMU
-static const void* step_kernel_fn(int kind) {
-  switch (kind) {
-    case K_SMOOTH: return (const void*)fb_run<ShTree, FB_ST_SMOOTH>;
-    case K_SOLVE: return (const void*)fb_run_solve;
-    case K_FINISH: return (const void*)fb_run<ShTree, FB_ST_FINISH>;
-    case K_POS: return (const void*)fb_run<ShTree, FB_ST_POS>;
-    case K_COL: return (const void*)fb_run<ShCol, FB_ST_COL>;
-    case K_PROJ: return (const void*)fb_run<ShCon, FB_ST_PROJ>;
-    case K_VEL: return (const void*)fb_run<ShTree, FB_ST_VEL>;
-    default: return nullptr;
-  }
-}
-#endif
 int fb_step_kernel_smem(FbHandle s, int kind, int* bytes_per_cta, int* blocks_per_sm) {
   if (!s || !bytes_per_cta || !blocks_per_sm) return -1;
   const size_t bytes = (kind >= 0 && kind < K_NKIND) ? step_kernel_bytes(s, kind) : 0;
   if (bytes == 0) return -1;
   *bytes_per_cta = (int)bytes; *blocks_per_sm = 0;
-#ifndef FB_EMU
-  int nb = 0;
-  FB_CUDA_OK(cudaSetDevice(s->device));
-  FB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, step_kernel_fn(kind), 32 * FB_WPB, bytes));
-  *blocks_per_sm = nb;
-#endif
-  return 0;
+  return step_kernel_blocks_per_sm(s, kind, bytes, blocks_per_sm);
 }
 
 int fb_obs_program(FbHandle s, const FbObsProgram* p) {
@@ -1223,18 +1207,16 @@ int fb_obs_program(FbHandle s, const FbObsProgram* p) {
   state_drop(s);
   scope_free(s, s->task_scope); s->d.task = nullptr;
   scope_free(s, s->obs_scope);
-  const size_t obs_mark = s->allocs.size();
   std::vector<int> kind(p->kind, p->kind + p->n_items), a(p->a, p->a + p->n_items), b(p->b, p->b + p->n_items), list(p->list, p->list + std::max(p->n_list, 0));
-  s->d.op_kind = up(s, kind); s->d.op_a = up(s, a); s->d.op_b = up(s, b); s->d.op_off = up(s, offs); s->d.op_list = up(s, list);
+  const int rc = scope_alloc(s, s->obs_scope, "out of device memory (observation program)", [&] {
+    s->d.op_kind = up(s, kind); s->d.op_a = up(s, a); s->d.op_b = up(s, b); s->d.op_off = up(s, offs); s->d.op_list = up(s, list);
+    if (p->ref_qpos && p->ref_len > 0) { std::vector<float> r(p->ref_qpos, p->ref_qpos + (size_t)7 * p->ref_len); s->d.op_ref = up(s, r); } else s->d.op_ref = nullptr;
+    s->d.tobs = dalloc<float>(s, (size_t)dim * s->d.Np);
+    s->op_step_dev = dalloc<int>(s, s->d.Np); s->op_first_dev = (unsigned char*)dalloc<int>(s, s->d.Np);
+  });
+  if (rc != 0) { s->d.tobs = nullptr; s->d.op_n = 0; return rc; }     // no program: the kernels skip the observation rows
   s->d.op_n = p->n_items; s->d.op_root_body = p->root_body; s->d.op_nsub = p->n_sub; s->d.op_ref_len = p->ref_len; s->d.op_ref_slot = 0;
-  if (p->ref_qpos && p->ref_len > 0) { std::vector<float> r(p->ref_qpos, p->ref_qpos + (size_t)7 * p->ref_len); s->d.op_ref = up(s, r); } else s->d.op_ref = nullptr;
-  s->d.tobs_dim = dim; s->d.tobs = dalloc<float>(s, (size_t)dim * s->d.Np);
-  s->op_step_dev = dalloc<int>(s, s->d.Np); s->op_first_dev = (unsigned char*)dalloc<int>(s, s->d.Np);
-  s->d.op_step = s->op_step_dev; s->d.op_first = s->op_first_dev;
-  s->obs_scope.assign(s->allocs.begin() + obs_mark, s->allocs.end());
-#ifndef FB_EMU
-  cudaDeviceSynchronize();
-#endif
+  s->d.tobs_dim = dim; s->d.op_step = s->op_step_dev; s->d.op_first = s->op_first_dev;
   return dim;
 }
 int fb_ref_slots(FbHandle s, int slot_len) {
@@ -1242,12 +1224,11 @@ int fb_ref_slots(FbHandle s, int slot_len) {
   if (sync_stream(s) != 0) return -2;
   if (!s->ref_slots || s->ref_slot_len != slot_len || !s->d.op_ref_slot) state_drop(s);
   if (!s->ref_slots || s->ref_slot_len != slot_len) {          // (re)allocate: one [slot_len][7] table per env
-    if (s->ref_slots) {
-      for (auto& a : s->allocs) if (a == s->ref_slots) { a = nullptr; break; }
-      dev_free(s->ref_slots);
-      if (s->d.task && s->task_host.ref_bank) { scope_free(s, s->task_scope); s->d.task = nullptr; }      // it wrote into the old slots
-    }
-    s->ref_slots = dalloc<float>(s, (size_t)s->d.Np * 7 * slot_len); s->ref_slot_len = slot_len;
+    if (s->ref_slots && s->d.task && s->task_host.ref_bank) { scope_free(s, s->task_scope); s->d.task = nullptr; }      // it wrote into the old slots
+    scope_free(s, s->ref_scope); s->ref_slots = nullptr; s->ref_slot_len = 0;
+    if (int rc = scope_alloc(s, s->ref_scope, "out of device memory (reference slots)", [&] { s->ref_slots = dalloc<float>(s, (size_t)s->d.Np * 7 * slot_len); })) {
+      s->ref_slots = nullptr; return rc; }
+    s->ref_slot_len = slot_len;
   }
   s->d.op_ref = s->ref_slots; s->d.op_ref_len = slot_len; s->d.op_ref_slot = 1;
   return 0;
@@ -1257,7 +1238,7 @@ int fb_ref_slot_write(FbHandle s, const int32_t* env_ids, int n, const float* ro
   const size_t per = (size_t)7 * s->ref_slot_len;
   for (int k = 0; k < n; k++) {
     if (env_ids[k] < 0 || env_ids[k] >= s->d.N) { s->err = "fb_ref_slot_write: env id out of range"; return -1; }
-    upload_async(s, s->ref_slots + per * env_ids[k], rows + per * k, sizeof(float) * per);
+    copy_async(s, s->ref_slots + per * env_ids[k], rows + per * k, sizeof(float) * per);
   }
   return sync_stream(s);                                        // the caller's rows may be reused right away
 }
@@ -1304,11 +1285,14 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   if (!p->reset_qpos) { s->err = "fb_task_program: reference / reset tables missing"; return -1; }
   if (p->kind == FB_TASK_VISION && (!s->bank_dev || !s->hfield_dev || s->bank_n <= 0)) { s->err = "fb_task_program: FB_TASK_VISION needs fb_hfield_collision / fb_eye_program and fb_hfield_bank first"; return -1; }
   if ((p->kind == FB_TASK_FLIGHT || p->kind == FB_TASK_VISION) && (p->n_wing <= 0 || p->n_freq <= 0 || p->tab_len <= 0 || !p->wb_traj || !p->wb_phase || !p->wb_phase_mod || !p->wb_freqs || !p->wb_len)) { s->err = "fb_task_program: wing-beat tables missing"; return -1; }
+  if (p->kind == FB_TASK_VISION && p->trench_cap > 0) {
+    if (!p->trench_y || !p->trench_x || !p->trench_len) { s->err = "fb_task_program: trench centre lines missing"; return -1; }
+    for (int k = 0; k < s->bank_n; k++) if (p->trench_len[k] < 2 || p->trench_len[k] > p->trench_cap || !(p->trench_x[2 * k + 1] > p->trench_x[2 * k])) { s->err = "fb_task_program: bad trench centre line"; return -1; }
+  }
   if (sync_stream(s) != 0) return -2;
   const DevModel& m = s->m; const int Np = s->d.Np;
   state_drop(s);
   scope_free(s, s->task_scope); s->d.task = nullptr;
-  const size_t task_mark = s->allocs.size();
   DevTask t; memset(&t, 0, sizeof(t));
   t.kind = p->kind; t.root_qadr = p->root_qadr; t.root_vadr = p->root_vadr; t.ghost_qadr = p->ghost_qadr; t.ghost_vadr = p->ghost_vadr;
   t.root_body = s->d.op_root_body; t.user_col = p->user_col;
@@ -1319,80 +1303,85 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   t.ref_len = p->ref_len; t.obs_refdisp_off = p->obs_refdisp_off; t.obs_refquat_off = p->obs_refquat_off;
   auto upf32 = [&](const float* src, size_t n) { std::vector<float> v(src, src + n); return up(s, v); };
   auto upi32 = [&](const int32_t* src, size_t n) { std::vector<int> v(src, src + n); return up(s, v); };
-  t.reset_qpos = upf32(p->reset_qpos, m.nq);
-  if (p->kind == FB_TASK_BALL) { t.ball_vadr = p->ball_vadr; for (int i = 0; i < 3; i++) t.ball_target[i] = p->ball_target[i]; t.ball_margin = p->ball_margin; }
-  if (!bank && p->kind != FB_TASK_TEMPLATE && p->kind != FB_TASK_BALL) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
-  else t.ref_len = 0;
-  t.n_noise = p->noise_qadr ? p->n_noise : 0; t.noise_qadr = t.n_noise ? upi32(p->noise_qadr, t.n_noise) : nullptr; t.noise_amp = p->noise_amp; t.seed = p->seed;
-  if (p->kind == FB_TASK_FLIGHT || p->kind == FB_TASK_VISION) {
-    t.n_wing = p->n_wing; t.wing_qadr = upi32(p->wing_qadr, p->n_wing); t.wing_vadr = upi32(p->wing_vadr, p->n_wing); t.wing_ctrl = upi32(p->wing_ctrl, p->n_wing);
-    t.n_freq = p->n_freq; t.tab_len = p->tab_len; const size_t nt = (size_t)p->n_freq * p->tab_len;
-    t.wb_traj = upf32(p->wb_traj, nt * p->n_wing); t.wb_phase = upf32(p->wb_phase, nt); t.wb_phase_mod = upf32(p->wb_phase_mod, nt);
-    t.wb_freqs = upf32(p->wb_freqs, p->n_freq); t.wb_len = upi32(p->wb_len, p->n_freq);
-    t.wb_base_freq = p->wb_base_freq; t.wb_rel_range = p->wb_rel_range; t.wb_rate = p->wb_rate;
-  }
-  t.step = dalloc<int>(s, Np); t.needs_reset = dalloc<int>(s, Np); t.resetting = dalloc<int>(s, Np); t.episode = dalloc<int>(s, Np);
-  t.wb_idx = dalloc<int>(s, Np); t.wb_pos = dalloc<int>(s, Np); t.has_uniform = dalloc<int>(s, Np);
-  t.uniform = dalloc<float>(s, (size_t)8 * Np); t.wb_freq = dalloc<float>(s, Np); t.out = dalloc<float>(s, (size_t)4 * Np);
-  t.ep_steps = dalloc<int>(s, Np);
-  if (bank) {          // episode lengths are set per env by each reset
-    t.ref_bank = 1; t.rbank = s->rbank_dev; t.traj_off = s->rbank_off_dev; t.traj_len = s->rbank_len_dev; t.rbank_w = s->rbank_w;
-    t.n_pick = p->n_pick; t.pick_traj = upi32(p->pick_traj, p->n_pick); t.randomize_start = p->randomize_start ? 1 : 0; t.start_margin = p->start_margin;
-    t.max_episode_rows = p->max_episode_rows; t.future_steps = p->future_steps; t.slots = s->ref_slots; t.slot_len = s->ref_slot_len;
-    t.ep_traj = dalloc<int>(s, Np); t.ep_start = dalloc<int>(s, Np); t.ep_row0 = dalloc<int>(s, Np); t.ep_n = dalloc<int>(s, Np); t.pin = dalloc<int>(s, (size_t)3 * Np);
-    if (p->kind == FB_TASK_WALK) {
-      t.n_mjnt = p->n_mocap_joints; t.n_msite = p->n_mocap_sites; t.mocap_qadr = upi32(p->mocap_qadr, p->n_mocap_joints);
-      t.n_wing = p->n_wing; t.wing_qadr = upi32(p->wing_qadr, p->n_wing); t.wing_spring = upf32(p->wing_spring, p->n_wing);
-      t.obs_root_pose_off = p->obs_root_pose_off; t.obs_root_qvel_off = p->obs_root_qvel_off; t.obs_mocap_qpos_off = p->obs_mocap_qpos_off;
-      t.obs_mocap_qvel_off = p->obs_mocap_qvel_off; t.obs_mocap_axes_off = p->obs_mocap_axes_off; t.obs_mocap_sites_off = p->obs_mocap_sites_off;
-      t.obs_wing_qpos_off = p->obs_wing_qpos_off;
-      for (int k = 0; k < 4; k++) { t.dm_std[k] = p->deep_mimic_std[k]; t.dm_weight[k] = p->deep_mimic_weight[k]; }
-      t.retract_margin = p->retract_margin;
-      t.rw_part = dalloc<float>(s, (size_t)Np * FB_NY * 3);
+  float *ty = nullptr, *tx = nullptr; int* tl = nullptr; DevTask* dev = nullptr;
+  const int rc = scope_alloc(s, s->task_scope, "out of device memory (task program)", [&] {
+    t.reset_qpos = upf32(p->reset_qpos, m.nq);
+    if (p->kind == FB_TASK_BALL) { t.ball_vadr = p->ball_vadr; for (int i = 0; i < 3; i++) t.ball_target[i] = p->ball_target[i]; t.ball_margin = p->ball_margin; }
+    if (!bank && p->kind != FB_TASK_TEMPLATE && p->kind != FB_TASK_BALL) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
+    else t.ref_len = 0;
+    t.n_noise = p->noise_qadr ? p->n_noise : 0; t.noise_qadr = t.n_noise ? upi32(p->noise_qadr, t.n_noise) : nullptr; t.noise_amp = p->noise_amp; t.seed = p->seed;
+    if (p->kind == FB_TASK_FLIGHT || p->kind == FB_TASK_VISION) {
+      t.n_wing = p->n_wing; t.wing_qadr = upi32(p->wing_qadr, p->n_wing); t.wing_vadr = upi32(p->wing_vadr, p->n_wing); t.wing_ctrl = upi32(p->wing_ctrl, p->n_wing);
+      t.n_freq = p->n_freq; t.tab_len = p->tab_len; const size_t nt = (size_t)p->n_freq * p->tab_len;
+      t.wb_traj = upf32(p->wb_traj, nt * p->n_wing); t.wb_phase = upf32(p->wb_phase, nt); t.wb_phase_mod = upf32(p->wb_phase_mod, nt);
+      t.wb_freqs = upf32(p->wb_freqs, p->n_freq); t.wb_len = upi32(p->wb_len, p->n_freq);
+      t.wb_base_freq = p->wb_base_freq; t.wb_rel_range = p->wb_rel_range; t.wb_rate = p->wb_rate;
     }
-  } else {
-    std::vector<int> steps((size_t)Np, p->episode_steps);
-    h2d(t.ep_steps, steps.data(), sizeof(int) * steps.size());
+    t.step = dalloc<int>(s, Np); t.needs_reset = dalloc<int>(s, Np); t.resetting = dalloc<int>(s, Np); t.episode = dalloc<int>(s, Np);
+    t.wb_idx = dalloc<int>(s, Np); t.wb_pos = dalloc<int>(s, Np); t.has_uniform = dalloc<int>(s, Np);
+    t.uniform = dalloc<float>(s, (size_t)8 * Np); t.wb_freq = dalloc<float>(s, Np); t.out = dalloc<float>(s, (size_t)4 * Np);
+    t.ep_steps = dalloc<int>(s, Np);
+    if (bank) {
+      t.ref_bank = 1; t.rbank = s->rbank_dev; t.traj_off = s->rbank_off_dev; t.traj_len = s->rbank_len_dev; t.rbank_w = s->rbank_w;
+      t.n_pick = p->n_pick; t.pick_traj = upi32(p->pick_traj, p->n_pick); t.randomize_start = p->randomize_start ? 1 : 0; t.start_margin = p->start_margin;
+      t.max_episode_rows = p->max_episode_rows; t.future_steps = p->future_steps; t.slots = s->ref_slots; t.slot_len = s->ref_slot_len;
+      t.ep_traj = dalloc<int>(s, Np); t.ep_start = dalloc<int>(s, Np); t.ep_row0 = dalloc<int>(s, Np); t.ep_n = dalloc<int>(s, Np); t.pin = dalloc<int>(s, (size_t)3 * Np);
+      if (p->kind == FB_TASK_WALK) {
+        t.n_mjnt = p->n_mocap_joints; t.n_msite = p->n_mocap_sites; t.mocap_qadr = upi32(p->mocap_qadr, p->n_mocap_joints);
+        t.n_wing = p->n_wing; t.wing_qadr = upi32(p->wing_qadr, p->n_wing); t.wing_spring = upf32(p->wing_spring, p->n_wing);
+        t.obs_root_pose_off = p->obs_root_pose_off; t.obs_root_qvel_off = p->obs_root_qvel_off; t.obs_mocap_qpos_off = p->obs_mocap_qpos_off;
+        t.obs_mocap_qvel_off = p->obs_mocap_qvel_off; t.obs_mocap_axes_off = p->obs_mocap_axes_off; t.obs_mocap_sites_off = p->obs_mocap_sites_off;
+        t.obs_wing_qpos_off = p->obs_wing_qpos_off;
+        for (int k = 0; k < 4; k++) { t.dm_std[k] = p->deep_mimic_std[k]; t.dm_weight[k] = p->deep_mimic_weight[k]; }
+        t.retract_margin = p->retract_margin;
+        t.rw_part = dalloc<float>(s, (size_t)Np * FB_NY * 3);
+      }
+    }
+    if (p->kind == FB_TASK_VISION) {
+      for (int i = 0; i < 2; i++) { t.th_rng[i] = p->target_height_range[i]; t.ts_rng[i] = p->target_speed_range[i]; t.x_rng[i] = p->init_x_range[i]; t.y_rng[i] = p->init_y_range[i]; }
+      for (int i = 0; i < 4; i++) t.hover_quat[i] = p->hover_quat[i];
+      for (int i = 0; i < 3; i++) t.target_zaxis[i] = p->target_zaxis[i];
+      t.fatal = p->floor_contacts_fatal;
+      t.n_bank = s->bank_n; t.hf_nrow = s->hf_nrow; t.hf_ncol = s->hf_ncol; t.hf_ncm = s->hf_nbr * s->hf_nbc; t.hf_half = s->hf.size[0];
+      t.bank = s->bank_dev; t.bank_hmax = s->bank_hmax_dev; t.bank_cmax = s->bank_cmax_dev; t.hf_data = s->hfield_dev; t.hf_hmax = s->hmax_dev; t.hf_cmax = s->cmax_dev;
+      t.target = dalloc<float>(s, (size_t)2 * Np); t.pick = dalloc<int>(s, Np);
+      t.trench_cap = 0; t.trench_x = t.trench_y = nullptr; t.trench_len = nullptr;
+      if (p->trench_cap > 0) {
+        ty = dalloc<float>(s, (size_t)p->trench_cap * s->bank_n); tx = dalloc<float>(s, (size_t)2 * s->bank_n); tl = dalloc<int>(s, s->bank_n);
+        t.trench_cap = p->trench_cap; t.trench_x = tx; t.trench_y = ty; t.trench_len = tl;
+      }
+    }
+    t.op_step = s->op_step_dev; t.op_first = s->op_first_dev;
+    dev = (DevTask*)dalloc<unsigned char>(s, sizeof(DevTask));
+  });
+  if (rc != 0) return rc;
+  std::vector<int> fill((size_t)Np);
+  if (!bank) {          // (a dataset program's episode lengths are set per env by each reset)
+    std::fill(fill.begin(), fill.end(), p->episode_steps); copy_sync(s, t.ep_steps, fill.data(), sizeof(int) * fill.size());
   }
   if (p->kind == FB_TASK_VISION) {
-    for (int i = 0; i < 2; i++) { t.th_rng[i] = p->target_height_range[i]; t.ts_rng[i] = p->target_speed_range[i]; t.x_rng[i] = p->init_x_range[i]; t.y_rng[i] = p->init_y_range[i]; }
-    for (int i = 0; i < 4; i++) t.hover_quat[i] = p->hover_quat[i];
-    for (int i = 0; i < 3; i++) t.target_zaxis[i] = p->target_zaxis[i];
-    t.fatal = p->floor_contacts_fatal;
-    t.n_bank = s->bank_n; t.hf_nrow = s->hf_nrow; t.hf_ncol = s->hf_ncol; t.hf_ncm = s->hf_nbr * s->hf_nbc; t.hf_half = s->hf.size[0];
-    t.bank = s->bank_dev; t.bank_hmax = s->bank_hmax_dev; t.bank_cmax = s->bank_cmax_dev; t.hf_data = s->hfield_dev; t.hf_hmax = s->hmax_dev; t.hf_cmax = s->cmax_dev;
-    t.target = dalloc<float>(s, (size_t)2 * Np); t.pick = dalloc<int>(s, Np);
-    { std::vector<int> none((size_t)Np, -1); h2d(t.pick, none.data(), sizeof(int) * none.size()); }      // no terrain yet (a reset, or a loaded state row, copies one)
-    t.trench_cap = 0; t.trench_x = t.trench_y = nullptr; t.trench_len = nullptr;
-    if (p->trench_cap > 0) {
-      if (!p->trench_y || !p->trench_x || !p->trench_len) { s->err = "fb_task_program: trench centre lines missing"; return -1; }
-      for (int k = 0; k < s->bank_n; k++) if (p->trench_len[k] < 2 || p->trench_len[k] > p->trench_cap || !(p->trench_x[2 * k + 1] > p->trench_x[2 * k])) { s->err = "fb_task_program: bad trench centre line"; return -1; }
-      float* ty = dalloc<float>(s, (size_t)p->trench_cap * s->bank_n); h2d(ty, p->trench_y, sizeof(float) * (size_t)p->trench_cap * s->bank_n);
-      float* tx = dalloc<float>(s, (size_t)2 * s->bank_n); h2d(tx, p->trench_x, sizeof(float) * 2 * s->bank_n);
-      int* tl = dalloc<int>(s, s->bank_n); h2d(tl, p->trench_len, sizeof(int) * s->bank_n);
-      t.trench_cap = p->trench_cap; t.trench_x = tx; t.trench_y = ty; t.trench_len = tl;
+    std::fill(fill.begin(), fill.end(), -1); copy_sync(s, t.pick, fill.data(), sizeof(int) * fill.size());      // no terrain yet (a reset, or a loaded state row, copies one)
+    if (t.trench_cap > 0) {
+      copy_sync(s, ty, p->trench_y, sizeof(float) * (size_t)p->trench_cap * s->bank_n);
+      copy_sync(s, tx, p->trench_x, sizeof(float) * 2 * s->bank_n);
+      copy_sync(s, tl, p->trench_len, sizeof(int) * s->bank_n);
     }
   }
-  t.op_step = s->op_step_dev; t.op_first = s->op_first_dev;
-  DevTask* dev = (DevTask*)dalloc<unsigned char>(s, sizeof(DevTask));
-  h2d(dev, &t, sizeof(t));
+  copy_sync(s, dev, &t, sizeof(t));
   s->task_host = t; s->d.task = dev;
-  s->task_scope.assign(s->allocs.begin() + task_mark, s->allocs.end());
   return fb_task_reset_all(s);
 }
 int fb_task_reset_all(FbHandle s) {
   if (!s || !s->d.task) return -1;
   if (sync_stream(s) != 0) return -2;
   std::vector<int> ones((size_t)s->d.Np, 1);
-  h2d(s->task_host.needs_reset, ones.data(), sizeof(int) * ones.size());
-  return 0;
+  return copy_sync(s, s->task_host.needs_reset, ones.data(), sizeof(int) * ones.size());
 }
 int fb_task_set_reset_noise(FbHandle s, float amp) {
   if (!s || !s->d.task || !(amp >= 0)) return -1;
   if (sync_stream(s) != 0) return -2;
   s->task_host.noise_amp = amp;
-  h2d((void*)s->d.task, &s->task_host, sizeof(DevTask));          // same pointers, new scalar
-  return 0;
+  return copy_sync(s, (void*)s->d.task, &s->task_host, sizeof(DevTask));          // same pointers, new scalar
 }
 int fb_task_request_reset(FbHandle s, const int32_t* env_ids, int n) {
   if (!s || !s->d.task || (n > 0 && !env_ids) || n < 0) return -1;
@@ -1401,15 +1390,14 @@ int fb_task_request_reset(FbHandle s, const int32_t* env_ids, int n) {
   const int one = 1;
   for (int k = 0; k < n; k++) {
     if (env_ids[k] < 0 || env_ids[k] >= s->d.N) { s->err = "fb_task_request_reset: env id out of range"; return -1; }
-    h2d(s->task_host.needs_reset + env_ids[k], &one, sizeof(int));
+    copy_sync(s, s->task_host.needs_reset + env_ids[k], &one, sizeof(int));
   }
   return 0;
 }
 int fb_task_episodes(FbHandle s, int32_t* dst) {
   if (!s || !s->d.task || !dst) return -1;
   if (sync_stream(s) != 0) return -2;
-  d2h(dst, s->task_host.episode, sizeof(int) * (size_t)s->d.N);
-  return 0;
+  return copy_sync(s, dst, s->task_host.episode, sizeof(int) * (size_t)s->d.N);
 }
 int fb_task_uniforms(FbHandle s, const int32_t* env_ids, int n, const float* u) {
   if (!s || !s->d.task || !env_ids || !u || n < 0) return -1;
@@ -1417,7 +1405,7 @@ int fb_task_uniforms(FbHandle s, const int32_t* env_ids, int n, const float* u) 
   const int one = 1;
   for (int k = 0; k < n; k++) {
     if (env_ids[k] < 0 || env_ids[k] >= s->d.N) { s->err = "fb_task_uniforms: env id out of range"; return -1; }
-    h2d(s->task_host.uniform + (size_t)8 * env_ids[k], u + k, sizeof(float)); h2d(s->task_host.has_uniform + env_ids[k], &one, sizeof(int));
+    copy_sync(s, s->task_host.uniform + (size_t)8 * env_ids[k], u + k, sizeof(float)); copy_sync(s, s->task_host.has_uniform + env_ids[k], &one, sizeof(int));
   }
   return 0;
 }
@@ -1427,35 +1415,39 @@ int fb_task_uniform_rows(FbHandle s, const int32_t* env_ids, int n, const float*
   const int one = 1;
   for (int k = 0; k < n; k++) {
     if (env_ids[k] < 0 || env_ids[k] >= s->d.N) { s->err = "fb_task_uniform_rows: env id out of range"; return -1; }
-    h2d(s->task_host.uniform + (size_t)8 * env_ids[k], u + (size_t)8 * k, 8 * sizeof(float)); h2d(s->task_host.has_uniform + env_ids[k], &one, sizeof(int));
+    copy_sync(s, s->task_host.uniform + (size_t)8 * env_ids[k], u + (size_t)8 * k, 8 * sizeof(float)); copy_sync(s, s->task_host.has_uniform + env_ids[k], &one, sizeof(int));
   }
   return 0;
+}
+// the highest point of one terrain, and of every block of FB_EYE_BLOCK x FB_EYE_BLOCK cells of it, border points included
+// (the eye ray marcher's block maxima, fb_render.h)
+static float terrain_maxima(const FbSim* s, const float* hk, float* cm) {
+  const size_t cells = (size_t)s->hf_nrow * s->hf_ncol;
+  float mx = hk[0]; for (size_t i = 1; i < cells; i++) mx = std::max(mx, hk[i]);
+  for (int br = 0; br < s->hf_nbr; br++) for (int bc = 0; bc < s->hf_nbc; bc++) {
+    float v = -3.0e38f;
+    for (int iy = br * FB_EYE_BLOCK; iy <= std::min((br + 1) * FB_EYE_BLOCK, s->hf_nrow - 1); iy++)
+      for (int ix = bc * FB_EYE_BLOCK; ix <= std::min((bc + 1) * FB_EYE_BLOCK, s->hf_ncol - 1); ix++) v = std::max(v, hk[(size_t)iy * s->hf_ncol + ix]);
+    cm[(size_t)br * s->hf_nbc + bc] = v;
+  }
+  return mx;
 }
 int fb_hfield_bank(FbHandle s, int n_terrain, const float* heights) {
   if (!s || !s->hfield_dev || n_terrain <= 0 || !heights) { if (s) s->err = "fb_hfield_bank: set up the heightfield grid first (fb_hfield_collision / fb_eye_program)"; return -1; }
   if (sync_stream(s) != 0) return -2;
   const size_t cells = (size_t)s->hf_nrow * s->hf_ncol, ncm = (size_t)s->hf_nbr * s->hf_nbc;
   std::vector<float> hmax(n_terrain), cm(ncm * n_terrain);
-  for (int k = 0; k < n_terrain; k++) {
-    const float* hk = heights + cells * k;
-    float mx = hk[0]; for (size_t i = 1; i < cells; i++) mx = std::max(mx, hk[i]);
-    hmax[k] = mx;
-    for (int br = 0; br < s->hf_nbr; br++) for (int bc = 0; bc < s->hf_nbc; bc++) {
-      float v = -3.0e38f;
-      for (int iy = br * FB_EYE_BLOCK; iy <= std::min((br + 1) * FB_EYE_BLOCK, s->hf_nrow - 1); iy++)
-        for (int ix = bc * FB_EYE_BLOCK; ix <= std::min((bc + 1) * FB_EYE_BLOCK, s->hf_ncol - 1); ix++) v = std::max(v, hk[(size_t)iy * s->hf_ncol + ix]);
-      cm[ncm * k + (size_t)br * s->hf_nbc + bc] = v;
-    }
-  }
+  for (int k = 0; k < n_terrain; k++) hmax[k] = terrain_maxima(s, heights + cells * k, cm.data() + ncm * k);
   if (s->bank_dev && s->d.task && s->task_host.kind == FB_TASK_VISION) state_drop(s);
   if (s->bank_dev) {      // a replaced bank is freed; a vision task program pointing at it has to be uploaded again
-    std::vector<void*> old = {s->bank_dev, s->bank_hmax_dev, s->bank_cmax_dev};
-    scope_free(s, old);
+    scope_free(s, s->bank_scope);
     if (s->d.task && s->task_host.kind == FB_TASK_VISION) { scope_free(s, s->task_scope); s->d.task = nullptr; }
   }
-  s->bank_dev = dalloc<float>(s, cells * n_terrain); s->bank_hmax_dev = dalloc<float>(s, n_terrain); s->bank_cmax_dev = dalloc<float>(s, ncm * n_terrain);
-  if (!s->bank_dev) { s->err = "out of device memory (terrain bank)"; return -4; }
-  h2d(s->bank_dev, heights, sizeof(float) * cells * n_terrain); h2d(s->bank_hmax_dev, hmax.data(), sizeof(float) * n_terrain); h2d(s->bank_cmax_dev, cm.data(), sizeof(float) * cm.size());
+  if (int rc = scope_alloc(s, s->bank_scope, "out of device memory (terrain bank)", [&] {
+        s->bank_dev = dalloc<float>(s, cells * n_terrain); s->bank_hmax_dev = dalloc<float>(s, n_terrain); s->bank_cmax_dev = dalloc<float>(s, ncm * n_terrain); })) {
+    s->bank_dev = s->bank_hmax_dev = s->bank_cmax_dev = nullptr; s->bank_n = 0; return rc; }
+  copy_sync(s, s->bank_dev, heights, sizeof(float) * cells * n_terrain); copy_sync(s, s->bank_hmax_dev, hmax.data(), sizeof(float) * n_terrain);
+  copy_sync(s, s->bank_cmax_dev, cm.data(), sizeof(float) * cm.size());
   s->bank_n = n_terrain;
   return 0;
 }
@@ -1472,23 +1464,17 @@ int fb_ref_bank_wide(FbHandle s, int n_traj, const int32_t* traj_len, int row_wi
     off[k] = (int)total; total += (size_t)len[k];
   }
   const size_t bytes = sizeof(float) * total * (size_t)row_width;      // (rows < 2^31, width < 2^31: no size_t overflow)
-#ifndef FB_EMU
-  size_t free_b = 0, total_b = 0;
-  if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && bytes > free_b) {
-    s->err = "fb_ref_bank: bank too large for the device's free memory"; return -4; }
-#endif
+  if (bytes > dev_free_bytes()) { s->err = "fb_ref_bank: bank too large for the device's free memory"; return -4; }
   if (sync_stream(s) != 0) return -2;
   if (s->rbank_dev && s->d.task && s->task_host.ref_bank) state_drop(s);
   if (s->rbank_dev) {      // a replaced bank is freed; a dataset program drawing from it has to be uploaded again
     scope_free(s, s->rbank_scope);
     if (s->d.task && s->task_host.ref_bank) { scope_free(s, s->task_scope); s->d.task = nullptr; }
   }
-  const size_t mark = s->allocs.size();
-  s->rbank_dev = dalloc<float>(s, total * (size_t)row_width); s->rbank_off_dev = dalloc<int>(s, n_traj); s->rbank_len_dev = dalloc<int>(s, n_traj);
-  s->rbank_scope.assign(s->allocs.begin() + mark, s->allocs.end());
-  if (!s->rbank_dev || !s->rbank_off_dev || !s->rbank_len_dev) {
-    scope_free(s, s->rbank_scope); s->rbank_dev = nullptr; s->rbank_len.clear(); s->rbank_w = 0; s->err = "out of device memory (trajectory bank)"; return -4; }
-  h2d(s->rbank_dev, rows, bytes); h2d(s->rbank_off_dev, off.data(), sizeof(int) * n_traj); h2d(s->rbank_len_dev, len.data(), sizeof(int) * n_traj);
+  if (int rc = scope_alloc(s, s->rbank_scope, "out of device memory (trajectory bank)", [&] {
+        s->rbank_dev = dalloc<float>(s, total * (size_t)row_width); s->rbank_off_dev = dalloc<int>(s, n_traj); s->rbank_len_dev = dalloc<int>(s, n_traj); })) {
+    s->rbank_dev = nullptr; s->rbank_off_dev = s->rbank_len_dev = nullptr; s->rbank_len.clear(); s->rbank_w = 0; return rc; }
+  copy_sync(s, s->rbank_dev, rows, bytes); copy_sync(s, s->rbank_off_dev, off.data(), sizeof(int) * n_traj); copy_sync(s, s->rbank_len_dev, len.data(), sizeof(int) * n_traj);
   s->rbank_len = len; s->rbank_w = row_width;
   return 0;
 }
@@ -1503,22 +1489,20 @@ int fb_task_ref_pick(FbHandle s, const int32_t* env_ids, int n, const int32_t* t
     pins[3 * k] = 1; pins[3 * k + 1] = traj[k]; pins[3 * k + 2] = start[k];
   }
   if (sync_stream(s) != 0) return -2;
-  for (int k = 0; k < n; k++) upload_async(s, s->task_host.pin + (size_t)3 * env_ids[k], pins.data() + 3 * k, 3 * sizeof(int));
+  for (int k = 0; k < n; k++) copy_async(s, s->task_host.pin + (size_t)3 * env_ids[k], pins.data() + 3 * k, 3 * sizeof(int));
   return sync_stream(s);                                        // `pins` goes out of scope
 }
 int fb_task_ref_state(FbHandle s, int32_t* traj, int32_t* start) {
   if (!s || !traj || !start) return -1;
   if (!s->d.task || !s->task_host.ref_bank) { s->err = "fb_task_ref_state: needs a task program with ref_bank"; return -1; }
   if (sync_stream(s) != 0) return -2;
-  d2h(traj, s->task_host.ep_traj, sizeof(int) * (size_t)s->d.N);
-  d2h(start, s->task_host.ep_start, sizeof(int) * (size_t)s->d.N);
-  return 0;
+  copy_async(s, traj, s->task_host.ep_traj, sizeof(int) * (size_t)s->d.N);
+  copy_async(s, start, s->task_host.ep_start, sizeof(int) * (size_t)s->d.N);
+  return sync_stream(s);
 }
 int fb_task_step(FbHandle s, const float* action, int is_device, int n_substeps) {
   if (!s || !s->d.task || !action || n_substeps <= 0) return -1;
-#ifndef FB_EMU
-  cudaSetDevice(s->device);
-#endif
+  dev_select(s);
   fb_launch<ShNone, Ph<ph_task_reset>, Ph<ph_task_reset2>, Ph<ph_task_reset3>, Ph<ph_task_reset4>, Ph<ph_task_reset5>>(s, K_MISC, 0, s->d.N);      // envs whose last step was LAST
   int rc = fb_set_ctrl(s, action, is_device);                                           // action -> ctrl (NaN -> 0), staged rows stay readable
   if (rc != 0) return rc;
@@ -1527,7 +1511,7 @@ int fb_task_step(FbHandle s, const float* action, int is_device, int n_substeps)
   rc = fb_step(s, n_substeps);
   if (rc != 0) return rc;
   fb_launch<ShNone, Ph<ph_pack>, Ph<ph_task_reward>, Ph<ph_task_after>>(s, K_PACK, 0, s->d.N);
-  return 0;
+  return launch_check(s, "fb_task_step");
 }
 int fb_task_ptrs(FbHandle s, void** obs_dev, int* obs_dim, void** out_dev) {
   if (!s || !s->d.task) return -1;
@@ -1538,20 +1522,24 @@ int fb_task_ptrs(FbHandle s, void** obs_dev, int* obs_dim, void** out_dev) {
 }
 int fb_task_read(FbHandle s, float* obs_host, float* out_host) {
   if (!s || !s->d.task) return -1;
-#ifndef FB_EMU
-  if (obs_host) FB_CUDA_OK(cudaMemcpyAsync(obs_host, s->d.tobs, sizeof(float) * (size_t)s->d.N * s->d.tobs_dim, cudaMemcpyDeviceToHost, s->stream));
-  if (out_host) FB_CUDA_OK(cudaMemcpyAsync(out_host, s->task_host.out, sizeof(float) * (size_t)4 * s->d.N, cudaMemcpyDeviceToHost, s->stream));
+  if (obs_host && copy_async(s, obs_host, s->d.tobs, sizeof(float) * (size_t)s->d.N * s->d.tobs_dim) != 0) return -2;
+  if (out_host && copy_async(s, out_host, s->task_host.out, sizeof(float) * (size_t)4 * s->d.N) != 0) return -2;
   return sync_stream(s);
-#else
-  if (obs_host) memcpy(obs_host, s->d.tobs, sizeof(float) * (size_t)s->d.N * s->d.tobs_dim);
-  if (out_host) memcpy(out_host, s->task_host.out, sizeof(float) * (size_t)4 * s->d.N);
-  return 0;
-#endif
 }
 #ifndef FB_EMU
 __global__ void __launch_bounds__(128) fb_render_kernel(DevData d, DevEye p) {
   const int e = blockIdx.x / p.n_cam, cam = blockIdx.x % p.n_cam;
   for (int px = threadIdx.x; px < p.size * p.size; px += blockDim.x) eye_pixel(d, p, e, cam, px / p.size, px % p.size);
+}
+static void launch_eyes(FbSim* s) {
+  fb_render_kernel<<<s->d.N * s->eye.n_cam, 128, 0, s->stream>>>(s->d, s->eye);
+  s->launches++;
+}
+#else
+static void launch_eyes(FbSim* s) {
+  emu_launch(s, "eye", 0, s->d.N, nullptr, [&](unsigned char*, int e) {
+    for (int c = 0; c < s->eye.n_cam; c++) for (int px = 0; px < s->eye.size * s->eye.size; px++) eye_pixel(s->d, s->eye, e, c, px / s->eye.size, px % s->eye.size);
+  });
 }
 #endif
 // per-env heightfield buffer [Np][nrow * ncol] + highest point per env, shared by the collision and the eye cameras
@@ -1578,9 +1566,7 @@ int fb_hfield_collision(FbHandle s, int geom, const float* size, int nrow, int n
   std::vector<int> pg(pair_geom, pair_geom + npair); h.pair_geom = up(s, pg);
   h.data = s->hfield_dev; h.hmax = s->hmax_dev;
   s->hf_on = true;
-#ifndef FB_EMU
-  for (auto& g : s->graph) { if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; } g.seen = false; }      // the launch sequence changed
-#endif
+  graphs_drop(s);
   return 0;
 }
 int fb_eye_program(FbHandle s, const FbEyeProgram* p) {
@@ -1606,34 +1592,20 @@ int fb_hfield_write(FbHandle s, const int32_t* env_ids, int n, const float* heig
   const size_t cells = (size_t)s->hf_nrow * s->hf_ncol;
   for (int k = 0; k < n; k++) {
     if (env_ids[k] < 0 || env_ids[k] >= s->d.N) { s->err = "fb_hfield_write: env id out of range"; return -1; }
-    float mx = heights[cells * k]; for (size_t i = 1; i < cells; i++) mx = std::max(mx, heights[cells * k + i]);
-    upload_async(s, s->hfield_dev + cells * env_ids[k], heights + cells * k, sizeof(float) * cells);
-    // highest grid point of every block of FB_EYE_BLOCK x FB_EYE_BLOCK cells, border points included
+    copy_async(s, s->hfield_dev + cells * env_ids[k], heights + cells * k, sizeof(float) * cells);
     std::vector<float> cm((size_t)s->hf_nbr * s->hf_nbc);
-    const float* hk = heights + cells * k;
-    for (int br = 0; br < s->hf_nbr; br++) for (int bc = 0; bc < s->hf_nbc; bc++) {
-      float v = -3.0e38f;
-      for (int iy = br * FB_EYE_BLOCK; iy <= std::min((br + 1) * FB_EYE_BLOCK, s->hf_nrow - 1); iy++)
-        for (int ix = bc * FB_EYE_BLOCK; ix <= std::min((bc + 1) * FB_EYE_BLOCK, s->hf_ncol - 1); ix++) v = std::max(v, hk[(size_t)iy * s->hf_ncol + ix]);
-      cm[(size_t)br * s->hf_nbc + bc] = v;
-    }
+    const float mx = terrain_maxima(s, heights + cells * k, cm.data());
     if (sync_stream(s) != 0) return -2;
-    h2d(s->cmax_dev + cm.size() * env_ids[k], cm.data(), sizeof(float) * cm.size());
-    h2d(s->hmax_dev + env_ids[k], &mx, sizeof(float));
+    copy_sync(s, s->cmax_dev + cm.size() * env_ids[k], cm.data(), sizeof(float) * cm.size());
+    copy_sync(s, s->hmax_dev + env_ids[k], &mx, sizeof(float));
   }
   return 0;
 }
 int fb_render_eyes(FbHandle s) {
   if (!s || !s->eye_out) return -1;
-#ifndef FB_EMU
-  cudaSetDevice(s->device);
-  fb_render_kernel<<<s->d.N * s->eye.n_cam, 128, 0, s->stream>>>(s->d, s->eye);
-  if (cudaGetLastError() != cudaSuccess) { s->err = "fb_render_eyes: launch failed"; return -2; }
-#else
-  for (int e = 0; e < s->d.N; e++) for (int c = 0; c < s->eye.n_cam; c++) for (int px = 0; px < s->eye.size * s->eye.size; px++) eye_pixel(s->d, s->eye, e, c, px / s->eye.size, px % s->eye.size);
-#endif
-  s->launches++;
-  return 0;
+  dev_select(s);
+  launch_eyes(s);
+  return launch_check(s, "fb_render_eyes");
 }
 int fb_eyes_ptr(FbHandle s, void** dev_ptr, int* bytes_per_env) {
   if (!s || !s->eye_out) return -1;
@@ -1643,47 +1615,26 @@ int fb_eyes_ptr(FbHandle s, void** dev_ptr, int* bytes_per_env) {
 }
 int fb_eyes_read(FbHandle s, uint8_t* host_dst) {
   if (!s || !s->eye_out || !host_dst) return -1;
-#ifndef FB_EMU
-  FB_CUDA_OK(cudaMemcpyAsync(host_dst, s->eye_out, s->eye_bytes * s->d.N, cudaMemcpyDeviceToHost, s->stream));
-  return sync_stream(s);
-#else
-  memcpy(host_dst, s->eye_out, s->eye_bytes * s->d.N);
-  return 0;
-#endif
+  return copy_sync(s, host_dst, s->eye_out, s->eye_bytes * s->d.N);
 }
 int fb_task_inputs(FbHandle s, const int32_t* step_idx, const uint8_t* first) {
   if (!s || !s->d.tobs || !step_idx || !first) return -1;
-  upload_async(s, s->op_step_dev, step_idx, sizeof(int) * s->d.N);
-  upload_async(s, s->op_first_dev, first, s->d.N);
-  return 0;
+  if (copy_async(s, s->op_step_dev, step_idx, sizeof(int) * s->d.N) != 0) return -2;
+  return copy_async(s, s->op_first_dev, first, s->d.N);
 }
 int fb_read_task_obs(FbHandle s, float* host_dst) {
   if (!s || !host_dst || !s->d.tobs) return -1;
-#ifndef FB_EMU
-  FB_CUDA_OK(cudaMemcpyAsync(host_dst, s->d.tobs, sizeof(float) * (size_t)s->d.N * s->d.tobs_dim, cudaMemcpyDeviceToHost, s->stream));
-  return sync_stream(s);
-#else
-  memcpy(host_dst, s->d.tobs, sizeof(float) * (size_t)s->d.N * s->d.tobs_dim);
-  return 0;
-#endif
+  return copy_sync(s, host_dst, s->d.tobs, sizeof(float) * (size_t)s->d.N * s->d.tobs_dim);
 }
 int fb_pack_obs(FbHandle s) {
   if (!s) return -1;
-#ifndef FB_EMU
-  cudaSetDevice(s->device);
-#endif
+  dev_select(s);
   fb_launch<ShNone, Ph<ph_pack>>(s, K_PACK);
-  return 0;
+  return launch_check(s, "fb_pack_obs");
 }
 int fb_read_obs(FbHandle s, float* host_dst) {
   if (!s || !host_dst) return -1;
-#ifndef FB_EMU
-  FB_CUDA_OK(cudaMemcpyAsync(host_dst, s->d.obs, sizeof(float) * (size_t)s->d.N * s->d.obs_dim, cudaMemcpyDeviceToHost, s->stream));
-  return sync_stream(s);
-#else
-  memcpy(host_dst, s->d.obs, sizeof(float) * (size_t)s->d.N * s->d.obs_dim);
-  return 0;
-#endif
+  return copy_sync(s, host_dst, s->d.obs, sizeof(float) * (size_t)s->d.N * s->d.obs_dim);
 }
 int fb_obs_ptr(FbHandle s, void** dev_ptr, int* floats_per_env) {
   if (!s || !dev_ptr || !floats_per_env) return -1;
@@ -1736,23 +1687,22 @@ template <bool LOAD> __global__ void __launch_bounds__(32 * FB_WPB) fb_state_ker
   kstate_copy<LOAD>(a, w, threadIdx.x);
   if (LOAD) { __syncwarp(); kstate_terrain(a, w, threadIdx.x, old_pick); }
 }
-#endif
-template <bool LOAD> static void launch_state(FbSim* s, const int* env_dev, const int* slot_dev, const int* env_host, const int* slot_host, int n) {
-#ifndef FB_EMU
-  StArgs a = {s->st_segs_dev, s->st_nseg, s->st_bank, s->st_row, env_dev, slot_dev, n, s->d.task};
-  (void)env_host; (void)slot_host;
+// the (env, slot) pairs of the device lists env_ids / slots (NULL: the identity)
+template <bool LOAD> static void launch_state(FbSim* s, const int* env_ids, const int* slots, int n) {
+  StArgs a = {s->st_segs_dev, s->st_nseg, s->st_bank, s->st_row, env_ids, slots, n, s->d.task};
   fb_state_kernel<LOAD><<<(n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(a);
+  s->launches++;
+}
 #else
-  StArgs a = {s->st_segs_dev, s->st_nseg, s->st_bank, s->st_row, env_host, slot_host, n, s->d.task};
-  (void)env_dev; (void)slot_dev;
-  for (int w = 0; w < n; w++) {
+template <bool LOAD> static void launch_state(FbSim* s, const int* env_ids, const int* slots, int n) {
+  StArgs a = {s->st_segs_dev, s->st_nseg, s->st_bank, s->st_row, env_ids, slots, n, s->d.task};
+  emu_launch(s, "state", 0, n, nullptr, [&](unsigned char*, int w) {
     const int old_pick = LOAD ? kstate_pick(a, w) : -1;
     for (int y = 0; y < FB_NY; y++) kstate_copy<LOAD>(a, w, y);
     if (LOAD) for (int y = 0; y < FB_NY; y++) kstate_terrain(a, w, y, old_pick);
-  }
-#endif
-  s->launches++;
+  });
 }
+#endif
 static int state_ready(FbSim* s, const char* who) {
   if (s->st_bank) return 0;
   s->err = std::string(who) + (s->st_stale ? ": the state bank was dropped when the handle's programs, reference slots or applied-force arrays changed: call fb_state_bank again"
@@ -1767,8 +1717,8 @@ static int state_ids(FbSim* s, const int32_t* env_ids, const int32_t* slots, int
     s->st_ids_cap = std::max(2 * n, 2 * s->d.Np); s->st_ids_dev = dalloc<int>(s, s->st_ids_cap);
     if (!s->st_ids_dev) { s->st_ids_cap = 0; s->err = "out of device memory (state id lists)"; return -4; }
   }
-  if (env_ids) { upload_async(s, s->st_ids_dev, env_ids, sizeof(int) * n); *env_dev = s->st_ids_dev; }
-  if (slots) { upload_async(s, s->st_ids_dev + n, slots, sizeof(int) * n); *slot_dev = s->st_ids_dev + n; }
+  if (env_ids) { if (copy_async(s, s->st_ids_dev, env_ids, sizeof(int) * n) != 0) return -2; *env_dev = s->st_ids_dev; }
+  if (slots) { if (copy_async(s, s->st_ids_dev + n, slots, sizeof(int) * n) != 0) return -2; *slot_dev = s->st_ids_dev + n; }
   return 0;
 }
 extern "C" {
@@ -1791,15 +1741,11 @@ int fb_state_bank(FbHandle s, int n_slots) {
   unsigned row; uint64_t sig; int ho;
   std::vector<StSeg> segs = state_layout(s, &row, &sig, &ho);
   const size_t bytes = (size_t)n_slots * row * 4;
-#ifndef FB_EMU
-  size_t free_b = 0, total_b = 0;
-  if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && bytes > free_b) { s->err = "fb_state_bank: the bank does not fit the device's free memory"; return -4; }
-#endif
-  const size_t mark = s->allocs.size();
-  s->st_bank = dalloc<unsigned>(s, (size_t)n_slots * row); s->st_segs_dev = (StSeg*)dalloc<unsigned char>(s, sizeof(StSeg) * segs.size());
-  s->st_scope.assign(s->allocs.begin() + mark, s->allocs.end());
-  if (!s->st_bank || !s->st_segs_dev) { scope_free(s, s->st_scope); s->st_bank = nullptr; s->st_segs_dev = nullptr; s->err = "fb_state_bank: out of memory"; return -4; }
-  h2d(s->st_segs_dev, segs.data(), sizeof(StSeg) * segs.size());
+  if (bytes > dev_free_bytes()) { s->err = "fb_state_bank: the bank does not fit the device's free memory"; return -4; }
+  if (int rc = scope_alloc(s, s->st_scope, "fb_state_bank: out of memory", [&] {
+        s->st_bank = dalloc<unsigned>(s, (size_t)n_slots * row); s->st_segs_dev = (StSeg*)dalloc<unsigned char>(s, sizeof(StSeg) * segs.size()); })) {
+    s->st_bank = nullptr; s->st_segs_dev = nullptr; return rc; }
+  copy_sync(s, s->st_segs_dev, segs.data(), sizeof(StSeg) * segs.size());
   s->st_nseg = (int)segs.size(); s->st_row = row; s->st_sig = sig; s->st_hold_off = ho; s->st_slots = n_slots; s->st_written.assign(n_slots, 0);
   return 0;
 }
@@ -1816,14 +1762,12 @@ int fb_state_save(FbHandle s, const int32_t* env_ids, const int32_t* slots, int 
     if (seen[sl]) { s->err = "fb_state_save: a slot may be written once per call"; return -1; }
     seen[sl] = 1;
   }
-#ifndef FB_EMU
-  cudaSetDevice(s->device);
-#endif
+  dev_select(s);
   const int *ed, *sd; int rc = state_ids(s, env_ids, slots, n, &ed, &sd);
   if (rc != 0) return rc;
-  launch_state<false>(s, ed, sd, env_ids, slots, n);
+  launch_state<false>(s, ed, sd, n);
   for (int k = 0; k < n; k++) s->st_written[slots ? slots[k] : k] = s->hold_pending ? 2 : 1;
-  return 0;
+  return launch_check(s, "fb_state_save");
 }
 int fb_state_load(FbHandle s, const int32_t* slots, const int32_t* env_ids, int n) {
   if (!s) return -1;
@@ -1839,19 +1783,14 @@ int fb_state_load(FbHandle s, const int32_t* slots, const int32_t* env_ids, int 
     if (seen[e]) { s->err = "fb_state_load: env " + std::to_string(e) + " appears twice"; return -1; }
     seen[e] = 1; held = held || s->st_written[sl] == 2;
   }
-#ifndef FB_EMU
-  cudaSetDevice(s->device);
-#endif
+  dev_select(s);
   const int *ed, *sd; int rc = state_ids(s, env_ids, slots, n, &ed, &sd);
   if (rc != 0) return rc;
-  launch_state<true>(s, ed, sd, env_ids, slots, n);
+  launch_state<true>(s, ed, sd, n);
   // what the row does not carry is a function of it: the position / velocity stage, for the loaded envs (all of them: the step's own launches)
-  if (n == s->d.N) launch_step1(s); else launch_step1_ids(s, ed, env_ids, n);
+  if (n == s->d.N) launch_step1(s); else launch_step1_ids(s, ed, n);
   if (held) s->hold_pending = 1;             // a restored env waits for its reset: the next step holds it and clears the hold
-#ifndef FB_EMU
-  if (cudaGetLastError() != cudaSuccess) { s->err = "fb_state_load: kernel launch failed"; return -2; }
-#endif
-  return 0;
+  return launch_check(s, "fb_state_load");
 }
 int fb_state_read(FbHandle s, const int32_t* slots, int n, void* host_dst) {
   if (!s || !host_dst || n < 0) return -1;
@@ -1863,8 +1802,8 @@ int fb_state_read(FbHandle s, const int32_t* slots, int n, void* host_dst) {
   }
   if (sync_stream(s) != 0) return -2;
   const size_t rb = (size_t)s->st_row * 4;
-  if (!slots) d2h(host_dst, s->st_bank, rb * n);
-  else for (int k = 0; k < n; k++) d2h((char*)host_dst + rb * k, s->st_bank + (size_t)s->st_row * slots[k], rb);
+  if (!slots) return copy_sync(s, host_dst, s->st_bank, rb * n);
+  for (int k = 0; k < n; k++) copy_sync(s, (char*)host_dst + rb * k, s->st_bank + (size_t)s->st_row * slots[k], rb);
   return 0;
 }
 int fb_state_substeps(FbHandle s, int n_substeps) {
@@ -1881,7 +1820,7 @@ int fb_state_write(FbHandle s, const int32_t* slots, int n, const void* host_src
   for (int k = 0; k < n; k++) {
     const int sl = slots ? slots[k] : k;
     const unsigned* src = (const unsigned*)((const char*)host_src + rb * k);
-    h2d(s->st_bank + (size_t)s->st_row * sl, src, rb);
+    copy_sync(s, s->st_bank + (size_t)s->st_row * sl, src, rb);
     s->st_written[sl] = src[s->st_hold_off] ? 2 : 1;
   }
   return 0;
@@ -1897,24 +1836,26 @@ __global__ void __launch_bounds__(32 * FB_WPB) fb_ik_kernel(DevModel m, DevData 
   extern __shared__ __align__(16) float fb_smem_ik[];
   kik_run(m, d, p, fb_smem_ik + (size_t)threadIdx.y * FB_IK_SH(p.n_fdof), blockIdx.x * FB_WPB + threadIdx.y);
 }
-#endif
-static int ik_launch(FbSim* s, int* live) {
-  DevIk& p = s->ik;
-#ifndef FB_EMU
-  FB_CUDA_OK(cudaMemsetAsync(p.live, 0, sizeof(int), s->stream));
+static void launch_ik(FbSim* s) {
+  const DevIk& p = s->ik;
   const size_t bytes = sizeof(float) * FB_IK_SH(p.n_fdof) * FB_WPB;
   fb_ik_kernel<<<(p.n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), bytes, s->stream>>>(s->m, s->d, p);
-  FB_CUDA_OK(cudaGetLastError());
-  FB_CUDA_OK(cudaMemcpyAsync(live, p.live, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-  FB_CUDA_OK(cudaStreamSynchronize(s->stream));
-#else
-  *p.live = 0;
-  std::vector<float> sh(FB_IK_SH(p.n_fdof) + 64, 0.0f);
-  for (int e = 0; e < p.n; e++) kik_run(s->m, s->d, p, sh.data(), e);
-  *live = *p.live;
-#endif
   s->launches++;
-  return 0;
+}
+#else
+static void launch_ik(FbSim* s) {
+  const DevIk& p = s->ik;
+  emu_launch(s, "ik", sizeof(float) * FB_IK_SH(p.n_fdof), p.n, nullptr,
+             [&](unsigned char* sh, int e) { kik_run(s->m, s->d, p, reinterpret_cast<float*>(sh), e); });
+}
+#endif
+// one bounded launch; *live: the problems still iterating after it
+static int ik_launch(FbSim* s, int* live) {
+  static const int zero = 0;
+  if (copy_async(s, s->ik.live, &zero, sizeof(int)) != 0) return -2;
+  launch_ik(s);
+  if (launch_check(s, "fb_ik_solve") != 0 || copy_async(s, live, s->ik.live, sizeof(int)) != 0) return -2;
+  return sync_stream(s);
 }
 
 extern "C" {
@@ -1949,17 +1890,17 @@ int fb_ik_program(FbHandle s, const FbIkProgram* p) {
   if (p->include) for (int k = 0; k < 3 * p->n_sites; k++) inc[k] = p->include[k] ? 1 : 0;
   std::vector<int> sid(p->site_ids, p->site_ids + p->n_sites);
   scope_free(s, s->ik_scope);
-  const size_t mark = s->allocs.size(); const int Np = s->d.Np, nfd = (int)fdof.size();
+  const int Np = s->d.Np, nfd = (int)fdof.size();
   DevIk& k = s->ik; k = DevIk{};
   k.n_site = p->n_sites; k.n_fdof = nfd; k.n_fjnt = p->n_jnts; k.iters = FB_IK_LAUNCH_ITERS; k.max_steps = p->max_steps;
   k.reg = p->reg_strength; k.lr = p->lr; k.beta = p->beta; k.thr = p->progress_threshold;
-  k.site_id = up(s, sid); k.include = up(s, inc); k.fdof = up(s, fdof); k.fdof_hqadr = up(s, hq); k.below = up(s, below);
-  k.fjnt_type = up(s, jt); k.fjnt_qadr = up(s, jq); k.fjnt_fd0 = up(s, jf);
-  k.target = dalloc<float>(s, (size_t)Np * 3 * p->n_sites); k.u = dalloc<float>(s, (size_t)Np * nfd);
-  k.step = dalloc<int>(s, Np); k.done = dalloc<int>(s, Np); k.err = dalloc<float>(s, Np); k.err_first = dalloc<float>(s, Np);
-  k.steps = dalloc<int>(s, Np); k.success = dalloc<unsigned char>(s, Np); k.live = dalloc<int>(s, 1);
-  s->ik_scope.assign(s->allocs.begin() + mark, s->allocs.end());
-  for (void* q : s->ik_scope) if (!q) { scope_free(s, s->ik_scope); s->ik = DevIk{}; s->err = "out of device memory (IK program)"; return -4; }
+  if (int rc = scope_alloc(s, s->ik_scope, "out of device memory (IK program)", [&] {
+        k.site_id = up(s, sid); k.include = up(s, inc); k.fdof = up(s, fdof); k.fdof_hqadr = up(s, hq); k.below = up(s, below);
+        k.fjnt_type = up(s, jt); k.fjnt_qadr = up(s, jq); k.fjnt_fd0 = up(s, jf);
+        k.target = dalloc<float>(s, (size_t)Np * 3 * p->n_sites); k.u = dalloc<float>(s, (size_t)Np * nfd);
+        k.step = dalloc<int>(s, Np); k.done = dalloc<int>(s, Np); k.err = dalloc<float>(s, Np); k.err_first = dalloc<float>(s, Np);
+        k.steps = dalloc<int>(s, Np); k.success = dalloc<unsigned char>(s, Np); k.live = dalloc<int>(s, 1); })) {
+    s->ik = DevIk{}; return rc; }
   s->ik_solved = 0;
   return 0;
 }
@@ -1972,26 +1913,18 @@ int fb_ik_solve(FbHandle s, int n, const float* target_xpos, const float* init_q
   const int nq = s->m.nq, nt = 3 * p.n_site;
   for (size_t i = 0; i < (size_t)n * nt; i++) if (std::isinf(target_xpos[i])) { s->err = "fb_ik_solve: infinite target component"; return -1; }
   if (init_qpos) for (size_t i = 0; i < (size_t)n * nq; i++) if (!std::isfinite(init_qpos[i])) { s->err = "fb_ik_solve: non-finite init_qpos"; return -1; }
-#ifndef FB_EMU
-  cudaSetDevice(s->device);
-#endif
+  dev_select(s);
   if (sync_stream(s) != 0) return -2;
   const int Np = s->d.Np;
   std::vector<int> done(Np, 1); std::fill(done.begin(), done.begin() + n, 0);
   std::vector<float> nan(Np, std::numeric_limits<float>::quiet_NaN()), zero((size_t)Np * p.n_fdof, 0.0f);
   std::vector<int> zi(Np, 0);
-  upload_async(s, (void*)p.target, target_xpos, sizeof(float) * (size_t)n * nt);
-  upload_async(s, p.u, zero.data(), sizeof(float) * zero.size()); upload_async(s, p.step, zi.data(), sizeof(int) * Np);
-  upload_async(s, p.done, done.data(), sizeof(int) * Np); upload_async(s, p.err, nan.data(), sizeof(float) * Np);
-  upload_async(s, p.err_first, nan.data(), sizeof(float) * Np); upload_async(s, p.steps, zi.data(), sizeof(int) * Np);
-  std::vector<unsigned char> zb(Np, 0); upload_async(s, p.success, zb.data(), Np);
-  if (init_qpos) {
-#ifndef FB_EMU
-    FB_CUDA_OK(cudaMemcpy2DAsync(s->d.qpos, (size_t)s->d.rec * 4, init_qpos, (size_t)nq * 4, (size_t)nq * 4, n, cudaMemcpyHostToDevice, s->stream));
-#else
-    for (int e = 0; e < n; e++) memcpy(s->d.qpos + (size_t)e * s->d.rec, init_qpos + (size_t)e * nq, sizeof(float) * nq);
-#endif
-  }
+  copy_async(s, (void*)p.target, target_xpos, sizeof(float) * (size_t)n * nt);
+  copy_async(s, p.u, zero.data(), sizeof(float) * zero.size()); copy_async(s, p.step, zi.data(), sizeof(int) * Np);
+  copy_async(s, p.done, done.data(), sizeof(int) * Np); copy_async(s, p.err, nan.data(), sizeof(float) * Np);
+  copy_async(s, p.err_first, nan.data(), sizeof(float) * Np); copy_async(s, p.steps, zi.data(), sizeof(int) * Np);
+  std::vector<unsigned char> zb(Np, 0); copy_async(s, p.success, zb.data(), Np);
+  if (init_qpos && copy_rows_async(s, s->d.qpos, (size_t)s->d.rec * 4, init_qpos, (size_t)nq * 4, (size_t)nq * 4, n) != 0) return -2;
   if (sync_stream(s) != 0) return -2;           // the host vectors go out of scope below
   p.n = n; s->ik_solved = n;
   for (int live = n; live > 0;) if (ik_launch(s, &live) != 0) return -2;
@@ -2004,24 +1937,11 @@ int fb_ik_read(FbHandle s, float* qpos, float* err, float* err_first, int32_t* s
   if (!p.live || s->ik_solved < 1) { s->err = "fb_ik_read: no IK solve to read"; return -1; }
   if (sync_stream(s) != 0) return -2;
   const int n = s->ik_solved, nq = s->m.nq;
-  if (qpos) {
-#ifndef FB_EMU
-    FB_CUDA_OK(cudaMemcpy2DAsync(qpos, (size_t)nq * 4, s->d.qpos, (size_t)s->d.rec * 4, (size_t)nq * 4, n, cudaMemcpyDeviceToHost, s->stream));
-#else
-    for (int e = 0; e < n; e++) memcpy(qpos + (size_t)e * nq, s->d.qpos + (size_t)e * s->d.rec, sizeof(float) * nq);
-#endif
-  }
-#ifndef FB_EMU
-  if (err) FB_CUDA_OK(cudaMemcpyAsync(err, p.err, sizeof(float) * n, cudaMemcpyDeviceToHost, s->stream));
-  if (err_first) FB_CUDA_OK(cudaMemcpyAsync(err_first, p.err_first, sizeof(float) * n, cudaMemcpyDeviceToHost, s->stream));
-  if (steps) FB_CUDA_OK(cudaMemcpyAsync(steps, p.steps, sizeof(int) * n, cudaMemcpyDeviceToHost, s->stream));
-  if (success) FB_CUDA_OK(cudaMemcpyAsync(success, p.success, n, cudaMemcpyDeviceToHost, s->stream));
-#else
-  if (err) memcpy(err, p.err, sizeof(float) * n);
-  if (err_first) memcpy(err_first, p.err_first, sizeof(float) * n);
-  if (steps) memcpy(steps, p.steps, sizeof(int) * n);
-  if (success) memcpy(success, p.success, n);
-#endif
+  if (qpos && copy_rows_async(s, qpos, (size_t)nq * 4, s->d.qpos, (size_t)s->d.rec * 4, (size_t)nq * 4, n) != 0) return -2;
+  if (err && copy_async(s, err, p.err, sizeof(float) * n) != 0) return -2;
+  if (err_first && copy_async(s, err_first, p.err_first, sizeof(float) * n) != 0) return -2;
+  if (steps && copy_async(s, steps, p.steps, sizeof(int) * n) != 0) return -2;
+  if (success && copy_async(s, success, p.success, n) != 0) return -2;
   return sync_stream(s);
 }
 
@@ -2034,28 +1954,24 @@ __global__ void __launch_bounds__(32 * FB_WPB) fb_inv_kernel(DevModel m, DevData
   __shared__ float fb_smem_inv[FB_WPB][FB_INV_SH];
   kinv_run(m, d, p, fb_smem_inv[threadIdx.y], blockIdx.x * FB_WPB + threadIdx.y);
 }
+static void launch_inv(FbSim* s) {
+  fb_inv_kernel<<<(s->inv.n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->inv);
+  s->launches++;
+}
+#else
+static void launch_inv(FbSim* s) {
+  emu_launch(s, "inverse", sizeof(float) * FB_INV_SH, s->inv.n, nullptr,
+             [&](unsigned char* sh, int e) { kinv_run(s->m, s->d, s->inv, reinterpret_cast<float*>(sh), e); });
+}
 #endif
 static int inv_alloc(FbSim* s) {
   if (s->inv.qacc) return 0;
-  const size_t mark = s->allocs.size(), Np = (size_t)s->d.Np, nv = (size_t)s->m.nv;
+  const size_t Np = (size_t)s->d.Np, nv = (size_t)s->m.nv;
   DevInv& p = s->inv;
-  p.qacc = dalloc<float>(s, Np * nv); p.qfrc_inverse = dalloc<float>(s, Np * nv); p.qfrc_constraint = dalloc<float>(s, Np * nv);
-  p.efc_force = dalloc<float>(s, Np * FB_MAXEFC);
-  s->inv_scope.assign(s->allocs.begin() + mark, s->allocs.end());
-  for (void* q : s->inv_scope) if (!q) { scope_free(s, s->inv_scope); s->inv = DevInv{}; s->err = "out of device memory (inverse dynamics)"; return -4; }
-  return 0;
-}
-static int inv_launch(FbSim* s) {
-  const DevInv& p = s->inv;
-#ifndef FB_EMU
-  fb_inv_kernel<<<(p.n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, p);
-  FB_CUDA_OK(cudaGetLastError());
-#else
-  std::vector<float> sh(FB_INV_SH + 64, 0.0f);
-  for (int e = 0; e < p.n; e++) kinv_run(s->m, s->d, p, sh.data(), e);
-  for (int i = FB_INV_SH; i < FB_INV_SH + 64; i++) if (sh[i] != 0.0f) { fprintf(stderr, "fb_emu: shared-memory slice overrun in the inverse kernel\n"); abort(); }
-#endif
-  s->launches++;
+  if (int rc = scope_alloc(s, s->inv_scope, "out of device memory (inverse dynamics)", [&] {
+        p.qacc = dalloc<float>(s, Np * nv); p.qfrc_inverse = dalloc<float>(s, Np * nv); p.qfrc_constraint = dalloc<float>(s, Np * nv);
+        p.efc_force = dalloc<float>(s, Np * FB_MAXEFC); })) {
+    s->inv = DevInv{}; return rc; }
   return 0;
 }
 
@@ -2067,19 +1983,14 @@ int fb_inverse(FbHandle s, int n, const float* qacc, int is_device) {
   if (!qacc) { s->err = "fb_inverse: qacc is NULL"; return -1; }
   const size_t cnt = (size_t)n * s->m.nv;
   if (!is_device) for (size_t i = 0; i < cnt; i++) if (!std::isfinite(qacc[i])) { s->err = "fb_inverse: non-finite qacc"; return -1; }
-#ifndef FB_EMU
-  cudaSetDevice(s->device);
-#endif
+  dev_select(s);
   if (int rc = inv_alloc(s)) return rc;
   DevInv& p = s->inv;
-#ifndef FB_EMU
-  FB_CUDA_OK(cudaMemcpyAsync(p.qacc, qacc, sizeof(float) * cnt, is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s->stream));
-#else
-  memcpy(p.qacc, qacc, sizeof(float) * cnt);
-#endif
+  if (copy_async(s, p.qacc, qacc, sizeof(float) * cnt) != 0) return -2;
   p.n = n;
   launch_step1(s);                             // the position / velocity stage fb_forward runs (sens_mode -1: no sensor sums)
-  if (inv_launch(s) != 0) return -2;
+  launch_inv(s);
+  if (launch_check(s, "fb_inverse") != 0) return -2;
   s->inv_done = n;
   return is_device ? 0 : sync_stream(s);       // a host qacc may be reused once the call returns
 }
@@ -2089,17 +2000,10 @@ int fb_inverse_read(FbHandle s, float* qfrc_inverse, float* qfrc_constraint, flo
   const DevInv& p = s->inv;
   if (s->inv_done < 1) { s->err = "fb_inverse_read: no inverse to read (fb_inverse)"; return -1; }
   const size_t n = (size_t)s->inv_done, nv = (size_t)s->m.nv;
-#ifndef FB_EMU
-  const cudaMemcpyKind k = is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-  if (qfrc_inverse) FB_CUDA_OK(cudaMemcpyAsync(qfrc_inverse, p.qfrc_inverse, sizeof(float) * n * nv, k, s->stream));
-  if (qfrc_constraint) FB_CUDA_OK(cudaMemcpyAsync(qfrc_constraint, p.qfrc_constraint, sizeof(float) * n * nv, k, s->stream));
-  if (efc_force) FB_CUDA_OK(cudaMemcpyAsync(efc_force, p.efc_force, sizeof(float) * n * FB_MAXEFC, k, s->stream));
-#else
-  (void)is_device;
-  if (qfrc_inverse) memcpy(qfrc_inverse, p.qfrc_inverse, sizeof(float) * n * nv);
-  if (qfrc_constraint) memcpy(qfrc_constraint, p.qfrc_constraint, sizeof(float) * n * nv);
-  if (efc_force) memcpy(efc_force, p.efc_force, sizeof(float) * n * FB_MAXEFC);
-#endif
+  (void)is_device;                             // (the copies take their direction from the pointers)
+  if (qfrc_inverse && copy_async(s, qfrc_inverse, p.qfrc_inverse, sizeof(float) * n * nv) != 0) return -2;
+  if (qfrc_constraint && copy_async(s, qfrc_constraint, p.qfrc_constraint, sizeof(float) * n * nv) != 0) return -2;
+  if (efc_force && copy_async(s, efc_force, p.efc_force, sizeof(float) * n * FB_MAXEFC) != 0) return -2;
   return sync_stream(s);
 }
 

@@ -186,6 +186,25 @@ def test_replacing_the_terrain_bank_invalidates_the_vision_task_program(emu):
     env.close()
 
 
+def test_a_rejected_task_program_leaves_the_running_one_in_place(emu, monkeypatch):
+    """fb_task_program checks the trench centre lines before it replaces anything: a program with a bad one is refused (-1) and
+    the vision task program already on the device keeps stepping"""
+    env = fly_envs.vision_guided_flight(n_envs=2, bumps_or_trench='trench', lib_path=emu, seed=1, terrain_bank=2, device_task=True)
+    env.reset()
+    env.step(np.zeros((2, 12), np.float32))
+    sim, args = env._sim, []
+    with monkeypatch.context() as mp:      # the arguments the env uploads, without replacing its bank or program
+        mp.setattr(sim, 'hfield_bank', lambda heights: None)
+        mp.setattr(sim, 'task_program', lambda **kw: args.append(kw))
+        env._upload_task_program(seed=1)
+    bad = dict(args[0], trench_len=np.ones(2, np.int32))        # a centre line of one point
+    with pytest.raises(st.StepperError, match=r'\(-1\).*bad trench centre line'):
+        sim.task_program(**bad)
+    ts = env.step(np.zeros((2, 12), np.float32))
+    assert np.all(np.isfinite(ts.reward))
+    env.close()
+
+
 @pytest.mark.parametrize('device_task', [False, True])
 def test_capacity_overflow_is_counted_not_a_termination(emu, device_task):
     """FB_FLAGS bits 1 / 2 (contact list or constraint rows at capacity: FB_MAXCON = 64 contacts here) are not bad physics: the
