@@ -1,0 +1,130 @@
+// fb_fd.h -- batched finite-difference transition Jacobians (MuJoCo mjd_transitionFD / mjd_stepFD): A = dx'/dx and B = dx'/du of
+// n_substeps substeps of the stepper, x = (dq [nv], qvel [nv], act [na]) with dq the tangent of qpos, u = ctrl [nu].
+//
+// One problem occupies ncol consecutive envs, every one of them a copy of the problem's state row (the state bank's fan-out).  Column 0
+// is the nominal; column c > 0 nudges one input coordinate j: centred, columns 1 + 2j / 2 + 2j by +delta / -delta; forward, column 1 + j
+// by +delta (or -delta at a ctrl's upper limit).  delta_j = eps max(1, |x_j|), with x_j the hinge angle, the free joint's translation
+// component, qvel, act or ctrl (rotational tangent coordinates: x_j = 0).  The stepper is fp32: a relative step keeps fast coordinates
+// (the wings' qvel of ~1e3 rad/s) resolved, where an absolute one would drown in their rounding.
+//   kfd_perturb (one warp per env): nudge the env's coordinate in place (mj_integratePos for dq) and record the signed step in
+//               DevFd::delta (0: the nominal, an env past the problems, or a ctrl nudge its range rules out).  The ctrl rule is
+//               MuJoCo's: forward if the actuator is not ctrl-limited or ctrl and ctrl + delta both lie in its range; backward if
+//               (centred or no forward nudge) and the same holds for ctrl - delta.  It is evaluated here only; kfd_diff reads the outcome.
+//   kfd_diff    (one warp per (problem, input coordinate)): x'(b) - x'(a) over delta(b) - delta(a), a / b the minus / plus env (the
+//               nominal where that side was not nudged); mj_differentiatePos per joint for the dq rows.  A zero column where neither
+//               side was nudged.  It writes column j of the problem's row-major A [nx][nx] or B [nx][nu] (strided stores, lanes over rows);
+//               the warp of column 0 also copies the nominal next state out of the record.
+// Fixed-order arithmetic and no atomics: a problem's A / B bits do not depend on its position in the batch or the batch size.  The
+// parameters and buffers are the kernels' own (DevFd), so DevModel / DevData, the record and the step kernels are untouched.
+#pragma once
+#include "fb_ik.h"
+
+struct DevFd {
+  int n, ncol, nx, nin, centered;         // problems, envs per problem, state size 2 nv + na, inputs nx + nu
+  float eps;
+  float* delta;                           // [Np] the signed step of the env's column
+  float *A, *B;                           // [n][nx][nx], [n][nx][nu]
+  float* next;                            // [n][nq + nv + na] the nominal column's next qpos, qvel, act
+};
+
+// the input coordinate column c nudges (-1: the nominal) and the direction it tries
+FB_DEV int fd_input(const DevFd& p, int c, int* dir) {
+  if (c == 0) { *dir = 0; return -1; }
+  if (p.centered) { *dir = ((c - 1) & 1) ? -1 : 1; return (c - 1) >> 1; }
+  *dir = 1; return c - 1;
+}
+FB_DEV bool fd_ctrl_in_range(const DevModel& m, int i, float a, float b) {
+  if (!MLD(m.actuator_ctrllimited[i])) return true;
+  const float lo = MLD(m.actuator_ctrlrange[2 * i]), hi = MLD(m.actuator_ctrlrange[2 * i + 1]);
+  return a >= lo && a <= hi && b >= lo && b <= hi;
+}
+// dof k's joint: its type, the qpos address of the coordinate (hinge, translation) or of the quaternion (rotation), and the rotation axis
+// (-1: not a rotational coordinate)
+FB_DEV void fd_dof(const DevModel& m, int k, int* qa, int* axis) {
+  const int j = MLD(m.dof_jntid[k]), t = MLD(m.jnt_type[j]), c = k - MLD(m.jnt_dofadr[j]);
+  *qa = MLD(m.jnt_qposadr[j]); *axis = -1;
+  if (t == FB_JNT_FREE) { if (c < 3) *qa += c; else { *qa += 3; *axis = c - 3; } }
+  else if (t == FB_JNT_BALL) *axis = c;
+}
+
+FB_WARPFN void kfd_perturb(const DevModel& m, const DevData& d, const DevFd& p, int e) {
+  WPAR_BEGIN
+    if (lane == 0) {
+      int dir = 0;
+      const int j = e < p.n * p.ncol ? fd_input(p, e % p.ncol, &dir) : -1;
+      const int nv = m.nv;
+      float step = 0.0f;
+      if (j >= 0) {
+        int qa = 0, axis = -1;
+        float* x;                                     // the coordinate (nullptr: a rotation)
+        if (j < nv) { fd_dof(m, j, &qa, &axis); x = axis < 0 ? &AT(d.qpos, qa) : nullptr; }
+        else if (j < 2 * nv) x = &AT(d.qvel, j - nv);
+        else if (j < p.nx) x = &AT(d.act, j - 2 * nv);
+        else x = &AT(d.ctrl, j - p.nx);
+        const float delta = p.eps * fmaxf(1.0f, x ? fabsf(*x) : 0.0f);
+        step = dir * delta;
+        if (j >= p.nx) {
+          const int i = j - p.nx;
+          const bool fwd = fd_ctrl_in_range(m, i, *x, *x + delta);
+          const bool back = (p.centered || !fwd) && fd_ctrl_in_range(m, i, *x - delta, *x);
+          step = p.centered ? (dir > 0 ? (fwd ? delta : 0.0f) : (back ? -delta : 0.0f)) : (fwd ? delta : (back ? -delta : 0.0f));
+        }
+        if (step != 0.0f) {
+          if (x) *x += step;
+          else integrate_quat(d, e, qa, v3(axis == 0 ? step : 0.0f, axis == 1 ? step : 0.0f, axis == 2 ? step : 0.0f));
+        }
+      }
+      p.delta[e] = step;
+    }
+  WPAR_END
+}
+
+// MuJoCo mju_subQuat(q2, q1): the body-frame rotation vector v with q1 exp(v) = q2.  Equal quaternions give exactly 0: in fp32 the
+// vector part of conj(q) q is rounding noise of ~1e-8, which over a step of 1e-3 would put ~1e-5 into columns that do not reach q.
+FB_DEV V3 fd_subquat(Q4 q1, Q4 q2) {
+  if (q1.w == q2.w && q1.x == q2.x && q1.y == q2.y && q1.z == q2.z) return v3(0, 0, 0);
+  const Q4 dq = qmul(q4(q1.w, -q1.x, -q1.y, -q1.z), q2);
+  const V3 ax = v3(dq.x, dq.y, dq.z);
+  const float s = norm(ax);
+  if (!(s > 0.0f)) return v3(0, 0, 0);
+  float ang = 2.0f * atan2f(s, dq.w);
+  if (ang > 3.14159265358979f) ang -= 2.0f * 3.14159265358979f;
+  return ax * (ang / s);
+}
+FB_DEV Q4 fd_quat(const DevData& d, int e, int qa) { return q4(AT(d.qpos, qa), AT(d.qpos, qa + 1), AT(d.qpos, qa + 2), AT(d.qpos, qa + 3)); }
+// state row i: env b's next state minus env a's (mj_differentiatePos for the dq rows)
+FB_DEV float fd_state_diff(const DevModel& m, const DevData& d, int b, int a, int i) {
+  const int nv = m.nv;
+  if (i < nv) {
+    int qa, axis; fd_dof(m, i, &qa, &axis);
+    if (axis >= 0) return comp(fd_subquat(fd_quat(d, a, qa), fd_quat(d, b, qa)), axis);
+    return d.qpos[(unsigned)b * d.rec + qa] - d.qpos[(unsigned)a * d.rec + qa];
+  }
+  const float* f = i < 2 * nv ? d.qvel + (i - nv) : d.act + (i - 2 * nv);
+  return f[(unsigned)b * d.rec] - f[(unsigned)a * d.rec];
+}
+FB_WARPFN void kfd_diff(const DevModel& m, const DevData& d, const DevFd& p, int w) {
+  const int pr = w / p.nin, j = w % p.nin, e0 = pr * p.ncol;
+  int a = e0, b = e0;
+  if (p.centered) {
+    const int ep = e0 + 1 + 2 * j, em = ep + 1;
+    if (p.delta[ep] != 0.0f) b = ep;
+    if (p.delta[em] != 0.0f) a = em;
+  } else {
+    const int ec = e0 + 1 + j;
+    if (p.delta[ec] > 0.0f) b = ec;
+    if (p.delta[ec] < 0.0f) a = ec;
+  }
+  const float den = p.delta[b] - p.delta[a];
+  float* out = j < p.nx ? p.A + (size_t)pr * p.nx * p.nx + j : p.B + (size_t)pr * p.nx * (p.nin - p.nx) + (j - p.nx);
+  const int stride = j < p.nx ? p.nx : p.nin - p.nx;
+  const int nq = m.nq, nv = m.nv, nnext = nq + nv + m.na;
+  WPAR_BEGIN
+    for (int i = lane; i < p.nx; i += FB_NY) out[(size_t)i * stride] = a == b ? 0.0f : fd_state_diff(m, d, b, a, i) / den;
+    if (j == 0) {
+      float* nx = p.next + (size_t)pr * nnext;
+      const int e = e0;
+      for (int i = lane; i < nnext; i += FB_NY) nx[i] = i < nq ? AT(d.qpos, i) : (i < nq + nv ? AT(d.qvel, i - nq) : AT(d.act, i - nq - nv));
+    }
+  WPAR_END
+}

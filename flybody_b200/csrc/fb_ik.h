@@ -61,6 +61,14 @@ FB_WARPFN void ik_sites(const DevModel& m, const DevData& d, const DevIk& p, flo
     }
   WPAR_END
 }
+// mj_integratePos of a free or ball joint's rotation (MuJoCo mju_quatIntegrate): the quaternion qpos[qa .. qa + 3], normalised, turned
+// by the body-frame rotation vector w.  The IK step and the finite-difference perturbation (fb_fd.h) share it.
+FB_DEV void integrate_quat(const DevData& d, int e, int qa, V3 w) {
+  const float ang = norm(w);
+  Q4 q = qnormalize(q4(AT(d.qpos, qa), AT(d.qpos, qa + 1), AT(d.qpos, qa + 2), AT(d.qpos, qa + 3)));
+  q = qnormalize(qmul(q, axisangle(normalized(w), ang)));
+  AT(d.qpos, qa) = q.w; AT(d.qpos, qa + 1) = q.x; AT(d.qpos, qa + 2) = q.y; AT(d.qpos, qa + 3) = q.z;
+}
 // warp-uniform sums in index order (every lane reads the same shared values)
 FB_DEV float ik_sum(const float* a, int n) { float s = 0; for (int i = 0; i < n; i++) s += a[i]; return s; }
 FB_DEV float ik_sumsq(const float* a, int n) { float s = 0; for (int i = 0; i < n; i++) s += a[i] * a[i]; return s; }
@@ -105,11 +113,7 @@ FB_WARPFN void kik_run(const DevModel& m, const DevData& d, const DevIk& p, floa
         const int qa = p.fjnt_qadr[j], f = p.fjnt_fd0[j];
         if (p.fjnt_type[j] == FB_JNT_HINGE) { AT(d.qpos, qa) += STP[f]; continue; }
         for (int c = 0; c < 3; c++) AT(d.qpos, qa + c) += STP[f + c];
-        V3 w = v3(STP[f + 3], STP[f + 4], STP[f + 5]);
-        const float ang = norm(w);
-        Q4 q = qnormalize(q4(AT(d.qpos, qa + 3), AT(d.qpos, qa + 4), AT(d.qpos, qa + 5), AT(d.qpos, qa + 6)));
-        q = qnormalize(qmul(q, axisangle(normalized(w), ang)));
-        AT(d.qpos, qa + 3) = q.w; AT(d.qpos, qa + 4) = q.x; AT(d.qpos, qa + 5) = q.y; AT(d.qpos, qa + 6) = q.z;
+        integrate_quat(d, e, qa + 3, v3(STP[f + 3], STP[f + 4], STP[f + 5]));
       }
     WPAR_END
     ik_kinematics(m, d, tree, e);

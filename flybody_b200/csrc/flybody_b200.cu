@@ -29,6 +29,7 @@
 #include "fb_state.h"
 #include "fb_ik.h"
 #include "fb_inverse.h"
+#include "fb_fd.h"
 
 enum { K_ACT = 0, K_SMOOTH, K_REF, K_SOLVE, K_FINISH, K_POS, K_COL, K_CON, K_PROJ, K_VEL, K_SENS, K_PACK, K_MISC, K_NKIND };
 static const char* const kKindNames[K_NKIND] = {"act", "smooth", "ref", "solve", "finish", "pos", "col", "con", "proj", "vel", "sens", "pack", "misc"};
@@ -45,6 +46,7 @@ struct FbSim {
   std::vector<double> h_qpos0;
   DevIk ik = {}; std::vector<void*> ik_scope; int ik_solved = 0;   // inverse kinematics (fb_ik_program): parameters and buffers; problems of the last solve
   DevInv inv = {}; std::vector<void*> inv_scope; int inv_done = 0;   // inverse dynamics (fb_inverse): buffers, allocated on first use; problems of the last call
+  DevFd fd = {}; std::vector<void*> fd_scope; int fd_cap = 0, fd_done = 0;   // transition Jacobians (fb_fd_transition): buffers for fd_cap problems, allocated on first use; problems of the last call
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -2004,6 +2006,104 @@ int fb_inverse_read(FbHandle s, float* qfrc_inverse, float* qfrc_constraint, flo
   if (qfrc_inverse && copy_async(s, qfrc_inverse, p.qfrc_inverse, sizeof(float) * n * nv) != 0) return -2;
   if (qfrc_constraint && copy_async(s, qfrc_constraint, p.qfrc_constraint, sizeof(float) * n * nv) != 0) return -2;
   if (efc_force && copy_async(s, efc_force, p.efc_force, sizeof(float) * n * FB_MAXEFC) != 0) return -2;
+  return sync_stream(s);
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------
+// transition Jacobians (fb_fd_*; fb_fd.h): its own kernel parameter (DevFd) and buffers (fd_scope), allocated on first use
+#ifndef FB_EMU
+__global__ void __launch_bounds__(32 * FB_WPB) fb_fd_perturb(DevModel m, DevData d, DevFd p) {
+  const int e = blockIdx.x * FB_WPB + threadIdx.y;
+  if (e < d.N) kfd_perturb(m, d, p, e);
+}
+__global__ void __launch_bounds__(32 * FB_WPB) fb_fd_diff(DevModel m, DevData d, DevFd p) {
+  const int w = blockIdx.x * FB_WPB + threadIdx.y;
+  if (w < p.n * p.nin) kfd_diff(m, d, p, w);
+}
+static void launch_fd_perturb(FbSim* s) {
+  dev_launch(s, K_MISC, [&] { fb_fd_perturb<<<(s->d.N + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->fd); });
+}
+static void launch_fd_diff(FbSim* s) {
+  const int n = s->fd.n * s->fd.nin;
+  dev_launch(s, K_MISC, [&] { fb_fd_diff<<<(n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->fd); });
+}
+#else
+static void launch_fd_perturb(FbSim* s) {
+  emu_launch(s, "fd_perturb", 0, s->d.N, nullptr, [&](unsigned char*, int e) { kfd_perturb(s->m, s->d, s->fd, e); });
+}
+static void launch_fd_diff(FbSim* s) {
+  emu_launch(s, "fd_diff", 0, s->fd.n * s->fd.nin, nullptr, [&](unsigned char*, int w) { kfd_diff(s->m, s->d, s->fd, w); });
+}
+#endif
+static int fd_columns(const FbSim* s, int centered) {
+  const int nin = 2 * s->m.nv + s->m.na + s->m.nu;
+  return centered ? 1 + 2 * nin : 1 + nin;
+}
+static int fd_alloc(FbSim* s) {
+  if (s->fd.delta) return 0;
+  const DevModel& m = s->m;
+  const size_t nx = 2 * (size_t)m.nv + m.na, cap = std::max(1, s->d.N / fd_columns(s, 0));
+  DevFd& p = s->fd;
+  if (int rc = scope_alloc(s, s->fd_scope, "out of device memory (transition Jacobians)", [&] {
+        p.delta = dalloc<float>(s, s->d.Np); p.A = dalloc<float>(s, cap * nx * nx); p.B = dalloc<float>(s, cap * nx * std::max(m.nu, 1));
+        p.next = dalloc<float>(s, cap * (m.nq + m.nv + m.na)); })) {
+    s->fd = DevFd{}; return rc; }
+  s->fd_cap = (int)cap;
+  return 0;
+}
+
+extern "C" {
+
+int fb_fd_columns(FbHandle s, int centered) { return s ? fd_columns(s, centered != 0) : -1; }
+
+int fb_fd_transition(FbHandle s, const int32_t* slots, int n, float eps, int centered, int n_substeps) {
+  if (!s) return -1;
+  if (state_ready(s, "fb_fd_transition") != 0) return -1;
+  const int N = s->d.N, ncol = fd_columns(s, centered != 0);
+  if (!slots || n < 1 || (long long)n * ncol > N) {
+    s->err = "fb_fd_transition: 1 <= n problems with n * fb_fd_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
+  if (!(eps > 0.0f) || !std::isfinite(eps)) { s->err = "fb_fd_transition: eps must be positive and finite"; return -1; }
+  if (n_substeps < 1) { s->err = "fb_fd_transition: n_substeps >= 1"; return -1; }
+  for (int k = 0; k < n; k++) {
+    const int sl = slots[k];
+    if (sl < 0 || sl >= s->st_slots) { s->err = "fb_fd_transition: slot out of range of the bank"; return -1; }
+    if (!s->st_written[sl]) { s->err = "fb_fd_transition: slot " + std::to_string(sl) + " was never written"; return -1; }
+    if (s->st_written[sl] == 2) { s->err = "fb_fd_transition: slot " + std::to_string(sl) + " was saved while its env was held for a reset (a held env does not integrate)"; return -1; }
+  }
+  dev_select(s);
+  if (int rc = fd_alloc(s)) return rc;
+  // every env a copy of its problem's row, warm start included; the envs past the problems copy the last problem's
+  std::vector<int32_t> fan(N);
+  for (int e = 0; e < N; e++) fan[e] = slots[std::min(e / ncol, n - 1)];
+  const int *ed, *sd;
+  if (int rc = state_ids(s, nullptr, fan.data(), N, &ed, &sd)) return rc;
+  DevFd& p = s->fd;
+  p.n = n; p.ncol = ncol; p.nx = 2 * s->m.nv + s->m.na; p.nin = p.nx + s->m.nu; p.centered = centered != 0; p.eps = eps;
+  s->fd_done = 0;
+  launch_state<true>(s, nullptr, sd, N);
+  launch_fd_perturb(s);
+  launch_step1(s);                             // the position / velocity stage of the nudged states
+  step_run(s, n_substeps);                     // fb_step's launches
+  launch_fd_diff(s);
+  if (launch_check(s, "fb_fd_transition") != 0) return -2;
+  s->fd_done = n;
+  return sync_stream(s);                       // (the fan-out list is a host vector)
+}
+
+int fb_fd_read(FbHandle s, float* A, float* B, float* qpos_next, float* qvel_next, float* act_next, int is_device) {
+  if (!s) return -1;
+  if (s->fd_done < 1) { s->err = "fb_fd_read: no transition to read (fb_fd_transition)"; return -1; }
+  const DevFd& p = s->fd;
+  const size_t n = (size_t)s->fd_done, nx = (size_t)p.nx, nu = (size_t)(p.nin - p.nx);
+  const size_t nq = s->m.nq, nv = s->m.nv, na = s->m.na, row = (nq + nv + na) * 4;
+  (void)is_device;                             // (the copies take their direction from the pointers)
+  if (A && copy_async(s, A, p.A, sizeof(float) * n * nx * nx) != 0) return -2;
+  if (B && nu && copy_async(s, B, p.B, sizeof(float) * n * nx * nu) != 0) return -2;
+  if (qpos_next && copy_rows_async(s, qpos_next, nq * 4, p.next, row, nq * 4, n) != 0) return -2;
+  if (qvel_next && copy_rows_async(s, qvel_next, nv * 4, p.next + nq, row, nv * 4, n) != 0) return -2;
+  if (act_next && na && copy_rows_async(s, act_next, na * 4, p.next + nq + nv, row, na * 4, n) != 0) return -2;
   return sync_stream(s);
 }
 

@@ -1,0 +1,68 @@
+"""Batched finite-difference transition Jacobians on the device (MuJoCo `mjd_transitionFD`; dm_control `mjlib.mjd_transitionFD`).
+
+`transition_fd` linearises the stepper around a batch of states: A = dx'/dx and B = dx'/du, with x = (dq, qvel, act) (dq: the tangent of
+qpos, as MuJoCo's) and u = ctrl, for the transition of n_substeps substeps with ctrl held fixed -- n_substeps = 1 is mjd_transitionFD,
+the task's substep count the transition a policy sees over one control step.  This is what LQR stabilisers, iLQR / MPC around a gait and
+system identification are built on.
+
+Every nudged copy of a state is one env of one batched step (`fb_fd_transition`): a centred Jacobian of the walking fly takes
+1 + 2 (nx + nu) = 693 envs, so one handle runs several problems per launch.  There is no CPU fallback: without the CUDA library the call
+raises `StepperError`.
+
+Two deliberate differences from MuJoCo:
+- the step is relative: coordinate j is nudged by eps max(1, |x_j|) (rotational tangent coordinates by eps), because the stepper is
+  fp32 and the flight model's wings move at ~1e3 rad/s, where an absolute step would carry the rounding of the coordinate itself;
+  MuJoCo's absolute step is the case |x_j| <= 1, and its usual eps of 1e-6 means nothing in fp32.  The default 1e-2 is where a sweep
+  against the fp64 limit (DESIGN section 6) put the error lowest: on contact states it is lowest there, on constraint-free flight states
+  within 3x of the lowest (3e-2);
+- no heightfield program is set up, so the vision model is stepped without terrain contacts (as `inverse_dynamics.inverse` steps it).
+Every column starts from a cold solver warm start: the states are written and `forward` run on a fresh handle.
+"""
+from collections import namedtuple
+
+import numpy as np
+
+from . import stepper as st
+
+ENVS = 4096          # envs of the handle: max(1, ENVS // columns) problems per launch
+
+Transition = namedtuple('Transition', ['A', 'B', 'qpos_next', 'qvel_next', 'act_next'])
+
+
+def transition_fd(model, qpos, qvel, ctrl, act=None, eps=1e-2, centered=True, n_substeps=1, device=0, lib_path=None):
+    """A = dx'/dx [B, nx, nx] and B = dx'/du [B, nx, nu] (row-major, as MuJoCo's) of B states qpos [B, nq], qvel [B, nv], ctrl [B, nu],
+    act [B, na] (zeros when None), or of one state without the batch dimension; nx = 2 nv + na.
+
+    Returns Transition(A, B, qpos_next, qvel_next, act_next) as fp64 arrays of the device's fp32 values; *_next is the unperturbed
+    state after the n_substeps substeps."""
+    m = model
+    q = np.asarray(qpos, np.float64)
+    single = q.ndim == 1
+    q = q.reshape(-1, m.nq)
+    n = q.shape[0]
+    v = np.asarray(qvel, np.float64).reshape(-1, m.nv)
+    u = np.asarray(ctrl, np.float64).reshape(-1, m.nu)
+    a = np.zeros((n, m.na)) if act is None else np.asarray(act, np.float64).reshape(-1 if m.na else n, m.na)
+    if not (v.shape[0] == u.shape[0] == a.shape[0] == n):
+        raise ValueError(f'{n} qpos rows, {v.shape[0]} qvel rows, {u.shape[0]} ctrl rows, {a.shape[0]} act rows')
+    ncol = 1 + (2 if centered else 1) * (2 * m.nv + m.na + m.nu)
+    per = max(1, ENVS // ncol)
+    sim = st.BatchedStepper(m, per * ncol, device=device, lib_path=lib_path)
+    outs = []
+    try:
+        sim.state_bank(per)
+        for p0 in range(0, n, per):
+            k = min(per, n - p0)
+            rows = np.minimum(np.arange(sim.n_envs), k - 1) + p0        # the chunk's states in envs 0 .. k-1, the last one repeated
+            sim.reset(q[rows], v[rows])
+            if m.na:
+                sim.set(st.ACT, a[rows])
+            sim.set_control(u[rows])
+            sim.forward()
+            sim.save_state(slots=np.arange(k), env_ids=np.arange(k))
+            sim.fd_transition(np.arange(k), eps=eps, centered=centered, n_substeps=n_substeps)
+            outs.append(sim.fd_read())
+    finally:
+        sim.close()
+    res = Transition(*(np.concatenate([o[i] for o in outs]).astype(np.float64) for i in range(5)))
+    return Transition(*(x[0] for x in res)) if single else res

@@ -24,7 +24,8 @@ EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl'
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
            'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version',
            'fb_state_slots', 'fb_state_signature', 'fb_state_bank', 'fb_state_save', 'fb_state_load', 'fb_state_read', 'fb_state_write', 'fb_state_substeps',
-           'fb_ik_program', 'fb_ik_solve', 'fb_ik_read', 'fb_inverse', 'fb_inverse_read']
+           'fb_ik_program', 'fb_ik_solve', 'fb_ik_read', 'fb_inverse', 'fb_inverse_read',
+           'fb_fd_columns', 'fb_fd_transition', 'fb_fd_read']
 
 
 # enum FbTaskKind (FbTaskProgram.kind)
@@ -170,6 +171,9 @@ def load_library(path=None):
     lib.fb_ik_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5
     lib.fb_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
     lib.fb_inverse_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    lib.fb_fd_columns.argtypes = [C.c_void_p, C.c_int]
+    lib.fb_fd_transition.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int]
+    lib.fb_fd_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_int]
     return lib
 
 
@@ -363,6 +367,28 @@ class BatchedStepper:
         qi, qc, f = np.zeros((n, nv), np.float32), np.zeros((n, nv), np.float32), np.zeros((n, MAXEFC), np.float32)
         self._check(self._lib.fb_inverse_read(self._h, qi.ctypes.data, qc.ctypes.data, f.ctypes.data, 0), 'fb_inverse_read')
         return qi, qc, f
+
+    # ---- finite-difference transition Jacobians (fb_fd_*; flybody_b200.derivatives is the batched front end)
+    def fd_columns(self, centered=True):
+        """envs one problem of fd_transition takes"""
+        return int(self._lib.fb_fd_columns(self._h, int(bool(centered))))
+
+    def fd_transition(self, slots, eps=1e-2, centered=True, n_substeps=1):
+        """A = dx'/dx, B = dx'/du of the bank rows `slots` over n_substeps substeps (see the header); the envs' states are a workspace
+        afterwards.  Read the results with fd_read()."""
+        s = np.ascontiguousarray(np.asarray(slots).reshape(-1), np.int32)
+        self._check(self._lib.fb_fd_transition(self._h, s.ctypes.data, len(s), float(eps), int(bool(centered)), int(n_substeps)),
+                    'fb_fd_transition')
+        self._fd_n = len(s)
+
+    def fd_read(self):
+        """-> (A [n, nx, nx], B [n, nx, nu], qpos_next [n, nq], qvel_next [n, nv], act_next [n, na]) f32 of the last fd_transition"""
+        m, n = self.model, getattr(self, '_fd_n', 0)
+        nx = 2 * m.nv + m.na
+        A, B = np.zeros((n, nx, nx), np.float32), np.zeros((n, nx, m.nu), np.float32)
+        q, v, a = np.zeros((n, m.nq), np.float32), np.zeros((n, m.nv), np.float32), np.zeros((n, m.na), np.float32)
+        self._check(self._lib.fb_fd_read(self._h, A.ctypes.data, B.ctypes.data, q.ctypes.data, v.ctypes.data, a.ctypes.data, 0), 'fb_fd_read')
+        return A, B, q, v, a
 
     def reset(self, qpos=None, qvel=None, env_ids=None):
         n = self.n_envs if env_ids is None else len(env_ids)

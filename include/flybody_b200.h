@@ -512,6 +512,29 @@ int fb_inverse(FbHandle h, int n, const float* qacc, int is_device);
  * memory): qfrc_inverse [n][nv], qfrc_constraint [n][nv], efc_force [n][fb_field_size(FB_EFC_FORCE)], rows as FB_CONTACT's efc_adr
  * and FB_NEFC index them after the call (rows >= nefc hold 0).  An error before the first fb_inverse.                         */
 int fb_inverse_read(FbHandle h, float* qfrc_inverse, float* qfrc_constraint, float* efc_force, int is_device);
+/* Finite-difference transition Jacobians (MuJoCo mjd_transitionFD without sensors; dm_control `mjlib.mjd_transitionFD`):
+ *   A [nx][nx] = dx'/dx and B [nx][nu] = dx'/du, row-major as MuJoCo's, x = (dq [nv], qvel [nv], act [na]) with dq the tangent of qpos
+ *   (mj_integratePos to nudge, mj_differentiatePos to difference), nx = 2 nv + na, u = ctrl [nu];
+ *   x' = the state after n_substeps substeps (mj_step2; mj_step1: fb_step's launches) with ctrl held fixed; n_substeps = 1 is
+ *   mjd_transitionFD, the task's substep count the transition of one control step.
+ * A problem is a state row of the bank (fb_state_save / fb_state_write).  It takes fb_fd_columns(h, centered) envs: 1 + 2 (nx + nu)
+ * centred, 1 + nx + nu forward; column 0 is the unperturbed nominal.  Every column starts from the row, its warm start included (as
+ * MuJoCo restores qacc_warmstart before each nudged step), and from its applied forces when the rows carry them (held fixed, as
+ * mjData's are).  Coordinate j is nudged by delta_j = eps max(1, |x_j|) (x_j: the hinge angle, the free joint's translation component,
+ * qvel, act or ctrl; rotational tangent coordinates delta = eps): the stepper is fp32, and a step relative to the coordinate keeps fast
+ * ones resolved (MuJoCo's absolute step is the case |x_j| <= 1; flybody_b200.derivatives defaults to eps 1e-2).  ctrl at its limits follows MuJoCo: forward if the actuator is not
+ * ctrl-limited or ctrl and ctrl + delta lie in its range, backward if (centred or no forward nudge) and ctrl - delta and ctrl do;
+ * centred, one-sided or a zero column.
+ * fb_fd_transition runs problems slots[0 .. n-1] (host ints) on envs k ncol .. (k+1) ncol - 1; the envs past n ncol run copies of the
+ * last problem.  The handle is a workspace: afterwards every env's state is unspecified; the bank is untouched.  Errors: no bank, a slot
+ * out of range, never written or saved while its env was held for a reset, n < 1 or n ncol > n_envs, eps <= 0 or not finite,
+ * n_substeps < 1.  It synchronises.                                                                                                  */
+int fb_fd_columns(FbHandle h, int centered);
+int fb_fd_transition(FbHandle h, const int32_t* slots, int n, float eps, int centered, int n_substeps);
+/* Results of the last fb_fd_transition for its n problems (synchronises; any pointer may be NULL; is_device: the pointers are device
+ * memory): A [n][nx][nx], B [n][nx][nu], and the nominal column's next state qpos_next [n][nq], qvel_next [n][nv], act_next [n][na].
+ * An error before the first fb_fd_transition.                                                                                        */
+int fb_fd_read(FbHandle h, float* A, float* B, float* qpos_next, float* qvel_next, float* act_next, int is_device);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
