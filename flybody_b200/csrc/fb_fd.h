@@ -16,8 +16,13 @@
 //               the warp of column 0 also copies the nominal next state out of the record.
 // Fixed-order arithmetic and no atomics: a problem's A / B bits do not depend on its position in the batch or the batch size.  The
 // parameters and buffers are the kernels' own (DevFd), so DevModel / DevData, the record and the step kernels are untouched.
+//
+// The second half of this file differentiates the inverse dynamics (MuJoCo mjd_inverseFD, flg_actuation = 0) with the same columns
+// and step rule: inputs (dq [nv], qvel [nv], qacc [nv]), outputs in MuJoCo's transposed layout (row i = the derivative with respect
+// to input i), see DevFdInv.
 #pragma once
 #include "fb_ik.h"
+#include "fb_inverse.h"
 
 struct DevFd {
   int n, ncol, nx, nin, centered;         // problems, envs per problem, state size 2 nv + na, inputs nx + nu
@@ -27,8 +32,8 @@ struct DevFd {
   float* next;                            // [n][nq + nv + na] the nominal column's next qpos, qvel, act
 };
 
-// the input coordinate column c nudges (-1: the nominal) and the direction it tries
-FB_DEV int fd_input(const DevFd& p, int c, int* dir) {
+// the input coordinate column c nudges (-1: the nominal) and the direction it tries (p: DevFd or DevFdInv)
+template <typename P> FB_DEV int fd_input(const P& p, int c, int* dir) {
   if (c == 0) { *dir = 0; return -1; }
   if (p.centered) { *dir = ((c - 1) & 1) ? -1 : 1; return (c - 1) >> 1; }
   *dir = 1; return c - 1;
@@ -125,6 +130,78 @@ FB_WARPFN void kfd_diff(const DevModel& m, const DevData& d, const DevFd& p, int
       float* nx = p.next + (size_t)pr * nnext;
       const int e = e0;
       for (int i = lane; i < nnext; i += FB_NY) nx[i] = i < nq ? AT(d.qpos, i) : (i < nq + nv ? AT(d.qvel, i - nq) : AT(d.act, i - nq - nv));
+    }
+  WPAR_END
+}
+
+// ---- inverse-dynamics Jacobians (MuJoCo mjd_inverseFD with flg_actuation = 0): of qfrc_inverse = M qacc + qfrc_bias - qfrc_passive
+// - qfrc_constraint (fb_inverse.h) and of qM, with respect to the inputs (dq [nv], qvel [nv], qacc [nv]).  One problem (qpos, qvel,
+// qacc) occupies ncol consecutive envs: centred 1 + 2 (3 nv), forward 1 + 3 nv; column 0 is the nominal; fd_input maps a column to its
+// input and direction, and the step is kfd_perturb's: delta_j = eps max(1, |x_j|) with x_j the hinge angle or the free joint's
+// translation component, qvel or qacc (rotational tangent coordinates: eps).  Outputs are transposed (MuJoCo's layout; the transpose
+// of DevFd's row-major A and B): row i is the derivative with respect to input i.
+//   kfdi_perturb (one warp per env; env e belongs to problem e / ncol, the envs past the problems to the last one): the problem's qpos
+//                and qvel rows into the record, its qacc row into inv.qacc, then the column's nudge (mj_integratePos for dq) and its
+//                signed step in delta.  launch_step1 and kinv_run (on inv) follow.
+//   kfdi_diff    (one warp per (problem, input i)): (f(b) - f(a)) / (delta_b - delta_a), b / a the plus / minus env (forward: a the
+//                nominal), into row i of DfDq, DfDv or DfDa (contiguous stores, lanes over the outputs); for a dq input also the qM
+//                difference into row i of DmDq (MuJoCo's sparse qM order: the record's).  The warp of input 0 copies out the nominal
+//                qfrc_inverse.
+struct DevFdInv {
+  int n, ncol, nin, centered;             // problems, envs per problem, inputs 3 nv, centred
+  float eps;
+  float *qpos, *qvel, *qacc;              // [cap][nq], [cap][nv], [cap][nv] the problems
+  float* delta;                           // [Np] the signed step of the env's column
+  DevInv inv;                             // the inverse kernel's parameter: inv.qacc holds every env's (nudged) qacc
+  float *DfDq, *DfDv, *DfDa;              // [n][nv][nv]: DfDq[i][j] = d qfrc_inverse_j / d dq_i
+  float* DmDq;                            // [n][nv][nM]: d qM / d dq_i in the sparse qM order
+  float* qfrc;                            // [n][nv] the nominal column's qfrc_inverse
+};
+
+FB_WARPFN void kfdi_perturb(const DevModel& m, const DevData& d, const DevFdInv& p, int e) {
+  const int nq = m.nq, nv = m.nv, pr = e / p.ncol < p.n ? e / p.ncol : p.n - 1;
+  float* qa_e = p.inv.qacc + (size_t)e * nv;
+  WPAR_BEGIN
+    for (int i = lane; i < nq; i += FB_NY) AT(d.qpos, i) = p.qpos[(size_t)pr * nq + i];
+    for (int i = lane; i < nv; i += FB_NY) { AT(d.qvel, i) = p.qvel[(size_t)pr * nv + i]; qa_e[i] = p.qacc[(size_t)pr * nv + i]; }
+  WPAR_END
+  WPAR_BEGIN
+    if (lane == 0) {
+      int dir = 0;
+      const int j = e < p.n * p.ncol ? fd_input(p, e % p.ncol, &dir) : -1;
+      float step = 0.0f;
+      if (j >= 0) {
+        int qa = 0, axis = -1;
+        float* x;                                     // the coordinate (nullptr: a rotation)
+        if (j < nv) { fd_dof(m, j, &qa, &axis); x = axis < 0 ? &AT(d.qpos, qa) : nullptr; }
+        else if (j < 2 * nv) x = &AT(d.qvel, j - nv);
+        else x = qa_e + (j - 2 * nv);
+        step = dir * (p.eps * fmaxf(1.0f, x ? fabsf(*x) : 0.0f));
+        if (x) *x += step;
+        else integrate_quat(d, e, qa, v3(axis == 0 ? step : 0.0f, axis == 1 ? step : 0.0f, axis == 2 ? step : 0.0f));
+      }
+      p.delta[e] = step;
+    }
+  WPAR_END
+}
+
+FB_WARPFN void kfdi_diff(const DevModel& m, const DevData& d, const DevFdInv& p, int w) {
+  const int nv = m.nv, nM = m.nM, pr = w / p.nin, i = w % p.nin, e0 = pr * p.ncol;
+  const int b = p.centered ? e0 + 1 + 2 * i : e0 + 1 + i, a = p.centered ? b + 1 : e0;
+  const float den = p.delta[b] - p.delta[a];
+  const int blk = i / nv, r = i % nv;
+  float* out = (blk == 0 ? p.DfDq : blk == 1 ? p.DfDv : p.DfDa) + ((size_t)pr * nv + r) * nv;
+  const float *fb = p.inv.qfrc_inverse + (size_t)b * nv, *fa = p.inv.qfrc_inverse + (size_t)a * nv;
+  WPAR_BEGIN
+    for (int k = lane; k < nv; k += FB_NY) out[k] = (fb[k] - fa[k]) / den;
+    if (blk == 0) {
+      float* dm = p.DmDq + ((size_t)pr * nv + r) * nM;
+      const float *mb = d.qM + (size_t)b * d.rec, *ma = d.qM + (size_t)a * d.rec;
+      for (int t = lane; t < nM; t += FB_NY) dm[t] = (mb[t] - ma[t]) / den;
+    }
+    if (i == 0) {
+      const float* f0 = p.inv.qfrc_inverse + (size_t)e0 * nv;
+      for (int k = lane; k < nv; k += FB_NY) p.qfrc[(size_t)pr * nv + k] = f0[k];
     }
   WPAR_END
 }

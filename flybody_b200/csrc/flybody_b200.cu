@@ -47,6 +47,7 @@ struct FbSim {
   DevIk ik = {}; std::vector<void*> ik_scope; int ik_solved = 0;   // inverse kinematics (fb_ik_program): parameters and buffers; problems of the last solve
   DevInv inv = {}; std::vector<void*> inv_scope; int inv_done = 0;   // inverse dynamics (fb_inverse): buffers, allocated on first use; problems of the last call
   DevFd fd = {}; std::vector<void*> fd_scope; int fd_cap = 0, fd_done = 0;   // transition Jacobians (fb_fd_transition): buffers for fd_cap problems, allocated on first use; problems of the last call
+  DevFdInv fdi = {}; std::vector<void*> fdi_scope; int fdi_cap = 0, fdi_done = 0;   // inverse-dynamics Jacobians (fb_fd_inverse): the same, with their own DevInv
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -1956,14 +1957,14 @@ __global__ void __launch_bounds__(32 * FB_WPB) fb_inv_kernel(DevModel m, DevData
   __shared__ float fb_smem_inv[FB_WPB][FB_INV_SH];
   kinv_run(m, d, p, fb_smem_inv[threadIdx.y], blockIdx.x * FB_WPB + threadIdx.y);
 }
-static void launch_inv(FbSim* s) {
-  fb_inv_kernel<<<(s->inv.n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->inv);
+static void launch_inv(FbSim* s, const DevInv& p) {
+  fb_inv_kernel<<<(p.n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, p);
   s->launches++;
 }
 #else
-static void launch_inv(FbSim* s) {
-  emu_launch(s, "inverse", sizeof(float) * FB_INV_SH, s->inv.n, nullptr,
-             [&](unsigned char* sh, int e) { kinv_run(s->m, s->d, s->inv, reinterpret_cast<float*>(sh), e); });
+static void launch_inv(FbSim* s, const DevInv& p) {
+  emu_launch(s, "inverse", sizeof(float) * FB_INV_SH, p.n, nullptr,
+             [&](unsigned char* sh, int e) { kinv_run(s->m, s->d, p, reinterpret_cast<float*>(sh), e); });
 }
 #endif
 static int inv_alloc(FbSim* s) {
@@ -1991,7 +1992,7 @@ int fb_inverse(FbHandle s, int n, const float* qacc, int is_device) {
   if (copy_async(s, p.qacc, qacc, sizeof(float) * cnt) != 0) return -2;
   p.n = n;
   launch_step1(s);                             // the position / velocity stage fb_forward runs (sens_mode -1: no sensor sums)
-  launch_inv(s);
+  launch_inv(s, s->inv);
   if (launch_check(s, "fb_inverse") != 0) return -2;
   s->inv_done = n;
   return is_device ? 0 : sync_stream(s);       // a host qacc may be reused once the call returns
@@ -2104,6 +2105,102 @@ int fb_fd_read(FbHandle s, float* A, float* B, float* qpos_next, float* qvel_nex
   if (qpos_next && copy_rows_async(s, qpos_next, nq * 4, p.next, row, nq * 4, n) != 0) return -2;
   if (qvel_next && copy_rows_async(s, qvel_next, nv * 4, p.next + nq, row, nv * 4, n) != 0) return -2;
   if (act_next && na && copy_rows_async(s, act_next, na * 4, p.next + nq + nv, row, na * 4, n) != 0) return -2;
+  return sync_stream(s);
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------
+// inverse-dynamics Jacobians (fb_fd_inverse*; fb_fd.h): their own kernel parameter (DevFdInv, with its own DevInv) and buffers
+// (fdi_scope), allocated on first use; fb_inverse's DevInv is not touched
+#ifndef FB_EMU
+__global__ void __launch_bounds__(32 * FB_WPB) fb_fdi_perturb(DevModel m, DevData d, DevFdInv p) {
+  const int e = blockIdx.x * FB_WPB + threadIdx.y;
+  if (e < d.N) kfdi_perturb(m, d, p, e);
+}
+__global__ void __launch_bounds__(32 * FB_WPB) fb_fdi_diff(DevModel m, DevData d, DevFdInv p) {
+  const int w = blockIdx.x * FB_WPB + threadIdx.y;
+  if (w < p.n * p.nin) kfdi_diff(m, d, p, w);
+}
+static void launch_fdi_perturb(FbSim* s) {
+  dev_launch(s, K_MISC, [&] { fb_fdi_perturb<<<(s->d.N + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->fdi); });
+}
+static void launch_fdi_diff(FbSim* s) {
+  const int n = s->fdi.n * s->fdi.nin;
+  dev_launch(s, K_MISC, [&] { fb_fdi_diff<<<(n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->fdi); });
+}
+#else
+static void launch_fdi_perturb(FbSim* s) {
+  emu_launch(s, "fdi_perturb", 0, s->d.N, nullptr, [&](unsigned char*, int e) { kfdi_perturb(s->m, s->d, s->fdi, e); });
+}
+static void launch_fdi_diff(FbSim* s) {
+  emu_launch(s, "fdi_diff", 0, s->fdi.n * s->fdi.nin, nullptr, [&](unsigned char*, int w) { kfdi_diff(s->m, s->d, s->fdi, w); });
+}
+#endif
+static int fdi_columns(const FbSim* s, int centered) { return centered ? 1 + 6 * s->m.nv : 1 + 3 * s->m.nv; }
+static int fdi_alloc(FbSim* s) {
+  if (s->fdi.delta) return 0;
+  const size_t Np = (size_t)s->d.Np, nq = (size_t)s->m.nq, nv = (size_t)s->m.nv, nM = (size_t)s->m.nM;
+  const size_t cap = std::max(1, s->d.N / fdi_columns(s, 0));
+  DevFdInv& p = s->fdi;
+  if (int rc = scope_alloc(s, s->fdi_scope, "out of device memory (inverse-dynamics Jacobians)", [&] {
+        p.qpos = dalloc<float>(s, cap * nq); p.qvel = dalloc<float>(s, cap * nv); p.qacc = dalloc<float>(s, cap * nv);
+        p.delta = dalloc<float>(s, Np);
+        p.inv.qacc = dalloc<float>(s, Np * nv); p.inv.qfrc_inverse = dalloc<float>(s, Np * nv);
+        p.inv.qfrc_constraint = dalloc<float>(s, Np * nv); p.inv.efc_force = dalloc<float>(s, Np * FB_MAXEFC);
+        p.DfDq = dalloc<float>(s, cap * nv * nv); p.DfDv = dalloc<float>(s, cap * nv * nv); p.DfDa = dalloc<float>(s, cap * nv * nv);
+        p.DmDq = dalloc<float>(s, cap * nv * nM); p.qfrc = dalloc<float>(s, cap * nv); })) {
+    s->fdi = DevFdInv{}; return rc; }
+  s->fdi_cap = (int)cap;
+  return 0;
+}
+
+extern "C" {
+
+int fb_fd_inverse_columns(FbHandle s, int centered) { return s ? fdi_columns(s, centered != 0) : -1; }
+
+int fb_fd_inverse(FbHandle s, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device) {
+  if (!s) return -1;
+  const int N = s->d.N, ncol = fdi_columns(s, centered != 0);
+  if (n < 1 || (long long)n * ncol > N) {
+    s->err = "fb_fd_inverse: 1 <= n problems with n * fb_fd_inverse_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
+  if (!qpos || !qvel || !qacc) { s->err = "fb_fd_inverse: qpos, qvel and qacc must not be NULL"; return -1; }
+  const size_t nq = s->m.nq, nv = s->m.nv;
+  if (!is_device) {
+    const struct { const float* x; size_t cnt; const char* what; } ins[3] = {{qpos, n * nq, "qpos"}, {qvel, n * nv, "qvel"}, {qacc, n * nv, "qacc"}};
+    for (const auto& in : ins)
+      for (size_t i = 0; i < in.cnt; i++)
+        if (!std::isfinite(in.x[i])) { s->err = std::string("fb_fd_inverse: non-finite ") + in.what; return -1; }
+  }
+  if (!(eps > 0.0f) || !std::isfinite(eps)) { s->err = "fb_fd_inverse: eps must be positive and finite"; return -1; }
+  dev_select(s);
+  if (int rc = fdi_alloc(s)) return rc;
+  DevFdInv& p = s->fdi;
+  if (copy_async(s, p.qpos, qpos, sizeof(float) * n * nq) != 0 || copy_async(s, p.qvel, qvel, sizeof(float) * n * nv) != 0 ||
+      copy_async(s, p.qacc, qacc, sizeof(float) * n * nv) != 0) return -2;
+  p.n = n; p.ncol = ncol; p.nin = 3 * (int)nv; p.centered = centered != 0; p.eps = eps;
+  p.inv.n = n * ncol;
+  s->fdi_done = 0;
+  launch_fdi_perturb(s);                       // fan-out and nudge
+  launch_step1(s);                             // the position / velocity stage of every env, as fb_inverse runs it
+  launch_inv(s, p.inv);
+  launch_fdi_diff(s);
+  if (launch_check(s, "fb_fd_inverse") != 0) return -2;
+  s->fdi_done = n;
+  return is_device ? 0 : sync_stream(s);       // host rows may be reused once the call returns
+}
+
+int fb_fd_inverse_read(FbHandle s, float* DfDq, float* DfDv, float* DfDa, float* DmDq, float* qfrc_inverse, int is_device) {
+  if (!s) return -1;
+  if (s->fdi_done < 1) { s->err = "fb_fd_inverse_read: no Jacobians to read (fb_fd_inverse)"; return -1; }
+  const DevFdInv& p = s->fdi;
+  const size_t n = (size_t)s->fdi_done, nv = (size_t)s->m.nv, nM = (size_t)s->m.nM;
+  (void)is_device;                             // (the copies take their direction from the pointers)
+  if (DfDq && copy_async(s, DfDq, p.DfDq, sizeof(float) * n * nv * nv) != 0) return -2;
+  if (DfDv && copy_async(s, DfDv, p.DfDv, sizeof(float) * n * nv * nv) != 0) return -2;
+  if (DfDa && copy_async(s, DfDa, p.DfDa, sizeof(float) * n * nv * nv) != 0) return -2;
+  if (DmDq && copy_async(s, DmDq, p.DmDq, sizeof(float) * n * nv * nM) != 0) return -2;
+  if (qfrc_inverse && copy_async(s, qfrc_inverse, p.qfrc, sizeof(float) * n * nv) != 0) return -2;
   return sync_stream(s);
 }
 

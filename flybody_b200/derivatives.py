@@ -17,6 +17,13 @@ Two deliberate differences from MuJoCo:
   within 3x of the lowest (3e-2);
 - no heightfield program is set up, so the vision model is stepped without terrain contacts (as `inverse_dynamics.inverse` steps it).
 Every column starts from a cold solver warm start: the states are written and `forward` run on a fresh handle.
+
+`inverse_fd` differentiates the inverse dynamics (MuJoCo `mjd_inverseFD` with flg_actuation = 0; `fb_fd_inverse`): the Jacobians of
+`inverse_dynamics.inverse`'s qfrc_inverse = M qacc + qfrc_bias - qfrc_passive - qfrc_constraint with respect to (dq, qvel, qacc), and of
+the sparse inertia qM with respect to dq.  They are what Gauss-Newton needs to make a tracked trajectory dynamically consistent (drive the
+root's "ghost force" to zero), and what direct trajectory optimisation and system identification from inverse dynamics use.  The
+columns and the relative step are transition_fd's; the outputs are transposed as MuJoCo's (row i: the derivative with respect to input
+i), the transpose of transition_fd's row-major A and B.  The vision model runs without terrain contacts here too.
 """
 from collections import namedtuple
 
@@ -27,6 +34,7 @@ from . import stepper as st
 ENVS = 4096          # envs of the handle: max(1, ENVS // columns) problems per launch
 
 Transition = namedtuple('Transition', ['A', 'B', 'qpos_next', 'qvel_next', 'act_next'])
+InverseJacobians = namedtuple('InverseJacobians', ['DfDq', 'DfDv', 'DfDa', 'DmDq', 'qfrc_inverse'])
 
 
 def transition_fd(model, qpos, qvel, ctrl, act=None, eps=1e-2, centered=True, n_substeps=1, device=0, lib_path=None):
@@ -66,3 +74,34 @@ def transition_fd(model, qpos, qvel, ctrl, act=None, eps=1e-2, centered=True, n_
         sim.close()
     res = Transition(*(np.concatenate([o[i] for o in outs]).astype(np.float64) for i in range(5)))
     return Transition(*(x[0] for x in res)) if single else res
+
+
+def inverse_fd(model, qpos, qvel, qacc, eps=1e-2, centered=True, device=0, lib_path=None):
+    """The inverse-dynamics Jacobians of B states qpos [B, nq], qvel [B, nv], qacc [B, nv], or of one state without the batch dimension.
+
+    Returns InverseJacobians(DfDq, DfDv, DfDa, DmDq, qfrc_inverse) as fp64 arrays of the device's fp32 values, transposed as MuJoCo's
+    mjd_inverseFD: DfDq [B, nv, nv] with DfDq[p, i, j] = d qfrc_inverse_j / d dq_i (dq: the tangent of qpos), DfDv and DfDa likewise
+    for qvel and qacc, DmDq [B, nv, nM] = d qM / d dq_i in MuJoCo's sparse qM order (the diagonal at dof_Madr, then the ancestors), and
+    the unperturbed qfrc_inverse [B, nv].  centered=False is MuJoCo's forward difference."""
+    m = model
+    q = np.asarray(qpos, np.float64)
+    single = q.ndim == 1
+    q = q.reshape(-1, m.nq)
+    n = q.shape[0]
+    v = np.asarray(qvel, np.float64).reshape(-1, m.nv)
+    a = np.asarray(qacc, np.float64).reshape(-1, m.nv)
+    if not (v.shape[0] == a.shape[0] == n):
+        raise ValueError(f'{n} qpos rows, {v.shape[0]} qvel rows, {a.shape[0]} qacc rows')
+    ncol = 1 + (2 if centered else 1) * 3 * m.nv
+    per = max(1, ENVS // ncol)
+    sim = st.BatchedStepper(m, per * ncol, device=device, lib_path=lib_path)
+    outs = []
+    try:
+        for p0 in range(0, n, per):
+            k = min(per, n - p0)
+            sim.fd_inverse(q[p0:p0 + k], v[p0:p0 + k], a[p0:p0 + k], eps=eps, centered=centered)
+            outs.append(sim.fd_inverse_read())
+    finally:
+        sim.close()
+    res = InverseJacobians(*(np.concatenate([o[i] for o in outs]).astype(np.float64) for i in range(5)))
+    return InverseJacobians(*(x[0] for x in res)) if single else res

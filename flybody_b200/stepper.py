@@ -25,7 +25,7 @@ EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl'
            'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version',
            'fb_state_slots', 'fb_state_signature', 'fb_state_bank', 'fb_state_save', 'fb_state_load', 'fb_state_read', 'fb_state_write', 'fb_state_substeps',
            'fb_ik_program', 'fb_ik_solve', 'fb_ik_read', 'fb_inverse', 'fb_inverse_read',
-           'fb_fd_columns', 'fb_fd_transition', 'fb_fd_read']
+           'fb_fd_columns', 'fb_fd_transition', 'fb_fd_read', 'fb_fd_inverse_columns', 'fb_fd_inverse', 'fb_fd_inverse_read']
 
 
 # enum FbTaskKind (FbTaskProgram.kind)
@@ -174,6 +174,9 @@ def load_library(path=None):
     lib.fb_fd_columns.argtypes = [C.c_void_p, C.c_int]
     lib.fb_fd_transition.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int]
     lib.fb_fd_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_int]
+    lib.fb_fd_inverse_columns.argtypes = [C.c_void_p, C.c_int]
+    lib.fb_fd_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int]
+    lib.fb_fd_inverse_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_int]
     return lib
 
 
@@ -389,6 +392,40 @@ class BatchedStepper:
         q, v, a = np.zeros((n, m.nq), np.float32), np.zeros((n, m.nv), np.float32), np.zeros((n, m.na), np.float32)
         self._check(self._lib.fb_fd_read(self._h, A.ctypes.data, B.ctypes.data, q.ctypes.data, v.ctypes.data, a.ctypes.data, 0), 'fb_fd_read')
         return A, B, q, v, a
+
+    # ---- finite-difference inverse-dynamics Jacobians (fb_fd_inverse*; flybody_b200.derivatives.inverse_fd is the batched front end)
+    def fd_inverse_columns(self, centered=True):
+        """envs one problem of fd_inverse takes"""
+        return int(self._lib.fb_fd_inverse_columns(self._h, int(bool(centered))))
+
+    def fd_inverse(self, qpos, qvel, qacc, eps=1e-2, centered=True, n=None, is_device=False):
+        """the Jacobians of qfrc_inverse (and qM) of problems qpos [n, nq], qvel [n, nv], qacc [n, nv] (host arrays), or of device
+        pointers (ints) with is_device=True and n given (see the header); the envs' states are a workspace afterwards.  Read the results
+        with fd_inverse_read()."""
+        m = self.model
+        if is_device:
+            if n is None:
+                raise ValueError('device inputs need n')
+            ptrs = [C.c_void_p(int(x)) for x in (qpos, qvel, qacc)]
+        else:
+            rows = [np.ascontiguousarray(np.asarray(x, np.float32).reshape(-1, k)) for x, k in ((qpos, m.nq), (qvel, m.nv), (qacc, m.nv))]
+            if len({r.shape[0] for r in rows}) != 1:
+                raise ValueError(f'{rows[0].shape[0]} qpos rows, {rows[1].shape[0]} qvel rows, {rows[2].shape[0]} qacc rows')
+            n = rows[0].shape[0] if n is None else int(n)
+            if n > rows[0].shape[0]:
+                raise ValueError(f'{rows[0].shape[0]} rows for n = {n}')
+            ptrs = [r.ctypes.data for r in rows]
+        self._check(self._lib.fb_fd_inverse(self._h, int(n), *ptrs, float(eps), int(bool(centered)), int(bool(is_device))), 'fb_fd_inverse')
+        self._fdi_n = int(n)
+
+    def fd_inverse_read(self):
+        """-> (DfDq, DfDv, DfDa [n, nv, nv], DmDq [n, nv, nM], qfrc_inverse [n, nv]) f32 of the last fd_inverse, transposed as MuJoCo's:
+        DfDq[p, i, j] = d qfrc_inverse_j / d dq_i"""
+        m, n = self.model, getattr(self, '_fdi_n', 0)
+        out = [np.zeros((n, m.nv, m.nv), np.float32) for _ in range(3)]
+        out += [np.zeros((n, m.nv, int(m.nM)), np.float32), np.zeros((n, m.nv), np.float32)]
+        self._check(self._lib.fb_fd_inverse_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_inverse_read')
+        return tuple(out)
 
     def reset(self, qpos=None, qvel=None, env_ids=None):
         n = self.n_envs if env_ids is None else len(env_ids)

@@ -535,6 +535,31 @@ int fb_fd_transition(FbHandle h, const int32_t* slots, int n, float eps, int cen
  * memory): A [n][nx][nx], B [n][nx][nu], and the nominal column's next state qpos_next [n][nq], qvel_next [n][nv], act_next [n][na].
  * An error before the first fb_fd_transition.                                                                                        */
 int fb_fd_read(FbHandle h, float* A, float* B, float* qpos_next, float* qvel_next, float* act_next, int is_device);
+/* Finite-difference inverse-dynamics Jacobians (MuJoCo mjd_inverseFD with flg_actuation = 0, without sensors): the derivatives of
+ * fb_inverse's qfrc_inverse = M qacc + qfrc_bias - qfrc_passive - qfrc_constraint, and of qM, with respect to the inputs
+ * (dq [nv], qvel [nv], qacc [nv]), dq the tangent of qpos (mj_integratePos to nudge).  The outputs are TRANSPOSED, as MuJoCo's
+ * ("all outputs are transposed"), and so the transpose of fb_fd_transition's row-major A and B: row i is the derivative with respect
+ * to input i,
+ *   DfDq [nv][nv], DfDv [nv][nv], DfDa [nv][nv]  with DfDq[i][j] = d qfrc_inverse_j / d dq_i;
+ *   DmDq [nv][nM]  d qM / d dq_i in MuJoCo's sparse qM order (the diagonal at dof_Madr, then the ancestors).
+ * A problem is one state (qpos [nq], qvel [nv], qacc [nv]) and takes fb_fd_inverse_columns(h, centered) envs: 1 + 2 (3 nv) centred,
+ * 1 + 3 nv forward (MuJoCo's mjd_inverseFD is forward-only); column 0 is the nominal.  The columns and step are fb_fd_transition's:
+ * input j is nudged by delta_j = eps max(1, |x_j|) (x_j: the hinge angle, the free joint's translation component, qvel or qacc;
+ * rotational tangent coordinates delta = eps).  flybody_b200.derivatives defaults to eps 1e-2.
+ * fb_fd_inverse runs problems qpos [n][nq], qvel [n][nv], qacc [n][nv] (host rows, or device pointers on the handle's stream when
+ * is_device) on envs k ncol .. (k+1) ncol - 1; the envs past n ncol hold copies of the last problem.  Every env runs the position /
+ * velocity stage (as fb_inverse), then the inverse kernel.  Each env's other inputs (act, ctrl, applied forces) are whatever it
+ * holds; none of them reaches qfrc_inverse.  The handle is a workspace: afterwards every env's qpos / qvel and the record are
+ * unspecified; fb_inverse_read still returns the last fb_inverse and the state bank is untouched.  Noslip is not inverted (as in
+ * fb_inverse and MuJoCo): on a model with noslip iterations the forces are the soft model's.  Errors: n < 1 or n ncol > n_envs, a
+ * NULL input, a non-finite host input, eps <= 0 or not finite.  A device input is not checked and the call returns without
+ * synchronising; with host inputs it synchronises.                                                                                   */
+int fb_fd_inverse_columns(FbHandle h, int centered);
+int fb_fd_inverse(FbHandle h, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device);
+/* Results of the last fb_fd_inverse for its n problems (synchronises; any pointer may be NULL; is_device: the pointers are device
+ * memory): DfDq, DfDv, DfDa [n][nv][nv], DmDq [n][nv][nM] and the nominal column's qfrc_inverse [n][nv].  An error before the first
+ * fb_fd_inverse.                                                                                                                     */
+int fb_fd_inverse_read(FbHandle h, float* DfDq, float* DfDv, float* DfDa, float* DmDq, float* qfrc_inverse, int is_device);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
