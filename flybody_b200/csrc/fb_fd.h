@@ -1,39 +1,41 @@
-// fb_fd.h -- batched finite-difference transition Jacobians (MuJoCo mjd_transitionFD / mjd_stepFD): A = dx'/dx and B = dx'/du of
-// n_substeps substeps of the stepper, x = (dq [nv], qvel [nv], act [na]) with dq the tangent of qpos, u = ctrl [nu].
+// fb_fd.h -- batched finite-difference Jacobians: of the stepper's transition (MuJoCo mjd_transitionFD / mjd_stepFD; DevFd) and of
+// the inverse dynamics (mjd_inverseFD with flg_actuation = 0; DevFdInv).  Both use one column scheme (FdCols):
 //
-// One problem occupies ncol consecutive envs, every one of them a copy of the problem's state row (the state bank's fan-out).  Column 0
-// is the nominal; column c > 0 nudges one input coordinate j: centred, columns 1 + 2j / 2 + 2j by +delta / -delta; forward, column 1 + j
-// by +delta (or -delta at a ctrl's upper limit).  delta_j = eps max(1, |x_j|), with x_j the hinge angle, the free joint's translation
-// component, qvel, act or ctrl (rotational tangent coordinates: x_j = 0).  The stepper is fp32: a relative step keeps fast coordinates
-// (the wings' qvel of ~1e3 rad/s) resolved, where an absolute one would drown in their rounding.
-//   kfd_perturb (one warp per env): nudge the env's coordinate in place (mj_integratePos for dq) and record the signed step in
-//               DevFd::delta (0: the nominal, an env past the problems, or a ctrl nudge its range rules out).  The ctrl rule is
-//               MuJoCo's: forward if the actuator is not ctrl-limited or ctrl and ctrl + delta both lie in its range; backward if
-//               (centred or no forward nudge) and the same holds for ctrl - delta.  It is evaluated here only; kfd_diff reads the outcome.
-//   kfd_diff    (one warp per (problem, input coordinate)): x'(b) - x'(a) over delta(b) - delta(a), a / b the minus / plus env (the
-//               nominal where that side was not nudged); mj_differentiatePos per joint for the dq rows.  A zero column where neither
-//               side was nudged.  It writes column j of the problem's row-major A [nx][nx] or B [nx][nu] (strided stores, lanes over rows);
-//               the warp of column 0 also copies the nominal next state out of the record.
-// Fixed-order arithmetic and no atomics: a problem's A / B bits do not depend on its position in the batch or the batch size.  The
-// parameters and buffers are the kernels' own (DevFd), so DevModel / DevData, the record and the step kernels are untouched.
-//
-// The second half of this file differentiates the inverse dynamics (MuJoCo mjd_inverseFD, flg_actuation = 0) with the same columns
-// and step rule: inputs (dq [nv], qvel [nv], qacc [nv]), outputs in MuJoCo's transposed layout (row i = the derivative with respect
-// to input i), see DevFdInv.
+// One problem occupies ncol consecutive envs.  Column 0 is the nominal; column c > 0 nudges one input j: centred, columns 1 + 2j / 2 + 2j
+// by +delta / -delta; forward, column 1 + j by +delta.  delta_j = eps max(1, |x_j|), with x_j the hinge angle, the free joint's
+// translation component, qvel, act, ctrl or qacc (rotational tangent coordinates: x_j = 0).  The stepper is fp32: a relative step keeps
+// fast coordinates (the wings' qvel of ~1e3 rad/s) resolved, where an absolute one would drown in their rounding.  A perturb kernel (one
+// warp per env) nudges the env's input in place (mj_integratePos for dq) and records the signed step in delta (0: the nominal, an env
+// past the problems, or a ctrl nudge its range rules out); a diff kernel (one warp per (problem, input)) divides the outputs' difference
+// between the plus and the minus env (the nominal where that side was not nudged) by the difference of their steps.
+//   transition: x = (dq [nv], qvel [nv], act [na]), u = ctrl [nu]; the envs are copies of the problem's state row (the state bank's
+//               fan-out), stepped n_substeps substeps.  The ctrl rule is MuJoCo's, evaluated in kfd_perturb only: forward if the
+//               actuator is not ctrl-limited or ctrl and ctrl + delta both lie in its range; backward if (centred or no forward nudge)
+//               and the same holds for ctrl - delta.  kfd_diff writes column j of row-major A [nx][nx] or B [nx][nu], mj_differentiatePos
+//               per joint for the dq rows; column 0's warp copies out the nominal next state.
+//   inverse:    inputs (dq [nv], qvel [nv], qacc [nv]); kfdi_perturb writes the problem's qpos, qvel and qacc rows (the envs past the
+//               problems take the last one's), launch_step1 and kinv_run (on DevFdInv::inv) follow, and kfdi_diff writes row i (MuJoCo's
+//               transposed layout: the derivative with respect to input i) of DfDq, DfDv or DfDa, and of DmDq (the sparse qM order) for
+//               a dq input; input 0's warp copies out the nominal qfrc_inverse.
+// Fixed-order arithmetic and no atomics: a problem's bits do not depend on its position in the batch or the batch size.  The parameters
+// and buffers are the kernels' own, so DevModel / DevData, the record and the step kernels are untouched.
 #pragma once
 #include "fb_ik.h"
 #include "fb_inverse.h"
 
-struct DevFd {
-  int n, ncol, nx, nin, centered;         // problems, envs per problem, state size 2 nv + na, inputs nx + nu
+struct FdCols {
+  int n, ncol, nin, centered;             // problems, envs per problem, inputs, centred
   float eps;
   float* delta;                           // [Np] the signed step of the env's column
+};
+struct DevFd : FdCols {
+  int nx;                                 // state size 2 nv + na (inputs nx + nu)
   float *A, *B;                           // [n][nx][nx], [n][nx][nu]
   float* next;                            // [n][nq + nv + na] the nominal column's next qpos, qvel, act
 };
 
-// the input coordinate column c nudges (-1: the nominal) and the direction it tries (p: DevFd or DevFdInv)
-template <typename P> FB_DEV int fd_input(const P& p, int c, int* dir) {
+// the input column c nudges (-1: the nominal) and the direction it tries
+FB_DEV int fd_input(const FdCols& p, int c, int* dir) {
   if (c == 0) { *dir = 0; return -1; }
   if (p.centered) { *dir = ((c - 1) & 1) ? -1 : 1; return (c - 1) >> 1; }
   *dir = 1; return c - 1;
@@ -51,33 +53,51 @@ FB_DEV void fd_dof(const DevModel& m, int k, int* qa, int* axis) {
   if (t == FB_JNT_FREE) { if (c < 3) *qa += c; else { *qa += 3; *axis = c - 3; } }
   else if (t == FB_JNT_BALL) *axis = c;
 }
+// nudge input j of env e in place: dq (j < nv), qvel (j < 2 nv) or the caller's coordinate xhi (inputs past 2 nv).  step(x, delta_j)
+// gives the signed step (0: no nudge; x nullptr for a rotation).  -> that step
+template <typename S> FB_DEV float fd_nudge(const DevModel& m, const DevData& d, const FdCols& p, int e, int j, float* xhi, S step) {
+  const int nv = m.nv;
+  int qa = 0, axis = -1;
+  float* x = xhi;                                 // the coordinate (nullptr: a rotation)
+  if (j < nv) { fd_dof(m, j, &qa, &axis); x = axis < 0 ? &AT(d.qpos, qa) : nullptr; }
+  else if (j < 2 * nv) x = &AT(d.qvel, j - nv);
+  const float s = step(x, p.eps * fmaxf(1.0f, x ? fabsf(*x) : 0.0f));
+  if (s != 0.0f) {
+    if (x) *x += s;
+    else integrate_quat(d, e, qa, v3(axis == 0 ? s : 0.0f, axis == 1 ? s : 0.0f, axis == 2 ? s : 0.0f));
+  }
+  return s;
+}
+// the envs input j of problem pr differences: b / a the plus / minus env, the nominal where that side was not nudged
+FB_DEV void fd_pair(const FdCols& p, int pr, int j, int* a, int* b) {
+  const int e0 = pr * p.ncol;
+  *a = *b = e0;
+  if (p.centered) {
+    const int ep = e0 + 1 + 2 * j, em = ep + 1;
+    if (p.delta[ep] != 0.0f) *b = ep;
+    if (p.delta[em] != 0.0f) *a = em;
+  } else {
+    const int ec = e0 + 1 + j;
+    if (p.delta[ec] > 0.0f) *b = ec;
+    if (p.delta[ec] < 0.0f) *a = ec;
+  }
+}
 
 FB_WARPFN void kfd_perturb(const DevModel& m, const DevData& d, const DevFd& p, int e) {
   WPAR_BEGIN
     if (lane == 0) {
       int dir = 0;
-      const int j = e < p.n * p.ncol ? fd_input(p, e % p.ncol, &dir) : -1;
-      const int nv = m.nv;
+      const int j = e < p.n * p.ncol ? fd_input(p, e % p.ncol, &dir) : -1, nv = m.nv;
       float step = 0.0f;
       if (j >= 0) {
-        int qa = 0, axis = -1;
-        float* x;                                     // the coordinate (nullptr: a rotation)
-        if (j < nv) { fd_dof(m, j, &qa, &axis); x = axis < 0 ? &AT(d.qpos, qa) : nullptr; }
-        else if (j < 2 * nv) x = &AT(d.qvel, j - nv);
-        else if (j < p.nx) x = &AT(d.act, j - 2 * nv);
-        else x = &AT(d.ctrl, j - p.nx);
-        const float delta = p.eps * fmaxf(1.0f, x ? fabsf(*x) : 0.0f);
-        step = dir * delta;
-        if (j >= p.nx) {
+        float* xhi = j < 2 * nv ? nullptr : j < p.nx ? &AT(d.act, j - 2 * nv) : &AT(d.ctrl, j - p.nx);
+        step = fd_nudge(m, d, p, e, j, xhi, [&](const float* x, float delta) {
+          if (j < p.nx) return dir * delta;
           const int i = j - p.nx;
           const bool fwd = fd_ctrl_in_range(m, i, *x, *x + delta);
           const bool back = (p.centered || !fwd) && fd_ctrl_in_range(m, i, *x - delta, *x);
-          step = p.centered ? (dir > 0 ? (fwd ? delta : 0.0f) : (back ? -delta : 0.0f)) : (fwd ? delta : (back ? -delta : 0.0f));
-        }
-        if (step != 0.0f) {
-          if (x) *x += step;
-          else integrate_quat(d, e, qa, v3(axis == 0 ? step : 0.0f, axis == 1 ? step : 0.0f, axis == 2 ? step : 0.0f));
-        }
+          return p.centered ? (dir > 0 ? (fwd ? delta : 0.0f) : (back ? -delta : 0.0f)) : (fwd ? delta : (back ? -delta : 0.0f));
+        });
       }
       p.delta[e] = step;
     }
@@ -110,16 +130,7 @@ FB_DEV float fd_state_diff(const DevModel& m, const DevData& d, int b, int a, in
 }
 FB_WARPFN void kfd_diff(const DevModel& m, const DevData& d, const DevFd& p, int w) {
   const int pr = w / p.nin, j = w % p.nin, e0 = pr * p.ncol;
-  int a = e0, b = e0;
-  if (p.centered) {
-    const int ep = e0 + 1 + 2 * j, em = ep + 1;
-    if (p.delta[ep] != 0.0f) b = ep;
-    if (p.delta[em] != 0.0f) a = em;
-  } else {
-    const int ec = e0 + 1 + j;
-    if (p.delta[ec] > 0.0f) b = ec;
-    if (p.delta[ec] < 0.0f) a = ec;
-  }
+  int a, b; fd_pair(p, pr, j, &a, &b);
   const float den = p.delta[b] - p.delta[a];
   float* out = j < p.nx ? p.A + (size_t)pr * p.nx * p.nx + j : p.B + (size_t)pr * p.nx * (p.nin - p.nx) + (j - p.nx);
   const int stride = j < p.nx ? p.nx : p.nin - p.nx;
@@ -134,24 +145,9 @@ FB_WARPFN void kfd_diff(const DevModel& m, const DevData& d, const DevFd& p, int
   WPAR_END
 }
 
-// ---- inverse-dynamics Jacobians (MuJoCo mjd_inverseFD with flg_actuation = 0): of qfrc_inverse = M qacc + qfrc_bias - qfrc_passive
-// - qfrc_constraint (fb_inverse.h) and of qM, with respect to the inputs (dq [nv], qvel [nv], qacc [nv]).  One problem (qpos, qvel,
-// qacc) occupies ncol consecutive envs: centred 1 + 2 (3 nv), forward 1 + 3 nv; column 0 is the nominal; fd_input maps a column to its
-// input and direction, and the step is kfd_perturb's: delta_j = eps max(1, |x_j|) with x_j the hinge angle or the free joint's
-// translation component, qvel or qacc (rotational tangent coordinates: eps).  Outputs are transposed (MuJoCo's layout; the transpose
-// of DevFd's row-major A and B): row i is the derivative with respect to input i.
-//   kfdi_perturb (one warp per env; env e belongs to problem e / ncol, the envs past the problems to the last one): the problem's qpos
-//                and qvel rows into the record, its qacc row into inv.qacc, then the column's nudge (mj_integratePos for dq) and its
-//                signed step in delta.  launch_step1 and kinv_run (on inv) follow.
-//   kfdi_diff    (one warp per (problem, input i)): (f(b) - f(a)) / (delta_b - delta_a), b / a the plus / minus env (forward: a the
-//                nominal), into row i of DfDq, DfDv or DfDa (contiguous stores, lanes over the outputs); for a dq input also the qM
-//                difference into row i of DmDq (MuJoCo's sparse qM order: the record's).  The warp of input 0 copies out the nominal
-//                qfrc_inverse.
-struct DevFdInv {
-  int n, ncol, nin, centered;             // problems, envs per problem, inputs 3 nv, centred
-  float eps;
+// ---- inverse-dynamics Jacobians: of qfrc_inverse = M qacc + qfrc_bias - qfrc_passive - qfrc_constraint (fb_inverse.h) and of qM
+struct DevFdInv : FdCols {
   float *qpos, *qvel, *qacc;              // [cap][nq], [cap][nv], [cap][nv] the problems
-  float* delta;                           // [Np] the signed step of the env's column
   DevInv inv;                             // the inverse kernel's parameter: inv.qacc holds every env's (nudged) qacc
   float *DfDq, *DfDv, *DfDa;              // [n][nv][nv]: DfDq[i][j] = d qfrc_inverse_j / d dq_i
   float* DmDq;                            // [n][nv][nM]: d qM / d dq_i in the sparse qM order
@@ -169,25 +165,14 @@ FB_WARPFN void kfdi_perturb(const DevModel& m, const DevData& d, const DevFdInv&
     if (lane == 0) {
       int dir = 0;
       const int j = e < p.n * p.ncol ? fd_input(p, e % p.ncol, &dir) : -1;
-      float step = 0.0f;
-      if (j >= 0) {
-        int qa = 0, axis = -1;
-        float* x;                                     // the coordinate (nullptr: a rotation)
-        if (j < nv) { fd_dof(m, j, &qa, &axis); x = axis < 0 ? &AT(d.qpos, qa) : nullptr; }
-        else if (j < 2 * nv) x = &AT(d.qvel, j - nv);
-        else x = qa_e + (j - 2 * nv);
-        step = dir * (p.eps * fmaxf(1.0f, x ? fabsf(*x) : 0.0f));
-        if (x) *x += step;
-        else integrate_quat(d, e, qa, v3(axis == 0 ? step : 0.0f, axis == 1 ? step : 0.0f, axis == 2 ? step : 0.0f));
-      }
-      p.delta[e] = step;
+      p.delta[e] = j < 0 ? 0.0f : fd_nudge(m, d, p, e, j, j < 2 * nv ? nullptr : qa_e + (j - 2 * nv), [&](const float*, float delta) { return dir * delta; });
     }
   WPAR_END
 }
 
 FB_WARPFN void kfdi_diff(const DevModel& m, const DevData& d, const DevFdInv& p, int w) {
   const int nv = m.nv, nM = m.nM, pr = w / p.nin, i = w % p.nin, e0 = pr * p.ncol;
-  const int b = p.centered ? e0 + 1 + 2 * i : e0 + 1 + i, a = p.centered ? b + 1 : e0;
+  int a, b; fd_pair(p, pr, i, &a, &b);
   const float den = p.delta[b] - p.delta[a];
   const int blk = i / nv, r = i % nv;
   float* out = (blk == 0 ? p.DfDq : blk == 1 ? p.DfDv : p.DfDa) + ((size_t)pr * nv + r) * nv;

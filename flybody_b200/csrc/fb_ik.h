@@ -75,7 +75,7 @@ FB_DEV float ik_sumsq(const float* a, int n) { float s = 0; for (int i = 0; i < 
 
 // run up to p.iters iterations of problem e (one warp)
 FB_WARPFN void kik_run(const DevModel& m, const DevData& d, const DevIk& p, float* sh, int e) {
-  if (e >= p.n || p.done[e]) return;
+  if (p.done[e]) return;
   float *R = sh, *M = sh + 3 * FB_IK_MAXSITE, *D2 = sh + 6 * FB_IK_MAXSITE;
   float *U = sh + 7 * FB_IK_MAXSITE, *STP = U + ((p.n_fdof + 3) & ~3);
   ShTree tree;                  // the slice argument of kpos_p0 / kpos_p1 (neither touches it)

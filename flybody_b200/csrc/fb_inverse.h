@@ -39,7 +39,6 @@ FB_DEV float inv_jar(const DevModel& m, const DevData& d, const float* qa, int e
 }
 
 FB_WARPFN void kinv_run(const DevModel& m, const DevData& d, const DevInv& p, float* sh, int e) {
-  if (e >= p.n) return;
   const int nv = m.nv, n = AT(d.nefc, 0);
   const float* qa = p.qacc + (size_t)e * nv;
   float* fo = p.efc_force + (size_t)e * FB_MAXEFC;

@@ -15,10 +15,12 @@
 #define FB_DEV __device__ __forceinline__
 #define FB_DEVN __device__ __noinline__
 #define FB_HD __host__ __device__
+#define FB_DEVM __device__ __forceinline__   // a member function of a kernel's parameter
 #else
 #define FB_DEV static inline
 #define FB_DEVN static
 #define FB_HD
+#define FB_DEVM
 #endif
 
 #define FB_NY 32             // lanes per env (threadIdx.x); every kernel runs 32 lanes per env

@@ -157,6 +157,14 @@ static int copy_sync(FbSim* s, void* dst, const void* src, size_t bytes) {
   const int rc = copy_async(s, dst, src, bytes);
   return rc != 0 ? rc : sync_stream(s);
 }
+// the outputs of a read, host or device: `rows` rows of `width` bytes, `spitch` bytes apart in the source and packed in the destination
+// (spitch 0: a contiguous array, one row); a NULL destination is skipped.  The stream is idle when it returns.
+struct ReadOut { void* dst; const void* src; size_t spitch, width, rows; };
+static int read_out(FbSim* s, std::initializer_list<ReadOut> outs) {
+  for (const ReadOut& o : outs)
+    if (o.dst && o.width && copy_rows_async(s, o.dst, o.width, o.src, o.spitch ? o.spitch : o.width, o.width, o.rows) != 0) return -2;
+  return sync_stream(s);
+}
 
 static size_t slice_bytes(size_t fixed, size_t dyn_floats) { return ((((fixed + 15) & ~(size_t)15) + dyn_floats * sizeof(float)) + 15) & ~(size_t)15; }
 // kernel = sequence of stages for one env.  Ph<f>: per-lane phase f(m, d, sh, e, y), a warp barrier follows;
@@ -254,6 +262,16 @@ static void fb_launch_warp(FbSim* s, int kind) {
   if (!configured) { cudaFuncSetAttribute(fb_run_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); configured = true; }
   dev_launch(s, kind, [&] { fb_run_solve<<<grid, block, bytes, s->stream>>>(s->m, s->d, s->d.Np); });
 }
+// one warp per problem w of [0, n), with `slice` bytes of shared memory each: k(slice, w).  K carries the kernel's parameters.  Slices
+// are whole 16-byte units; saying so keeps the IK kernel's shared-memory addressing (and its registers) as it was without the launcher.
+template <typename K> __global__ void __launch_bounds__(32 * FB_WPB) fb_run_warps(K k, int n, unsigned slice) {
+  extern __shared__ __align__(16) unsigned char fb_smem_q[];
+  const int w = blockIdx.x * FB_WPB + threadIdx.y;
+  if (w < n) k(static_cast<unsigned char*>(__builtin_assume_aligned(fb_smem_q + (size_t)threadIdx.y * slice, 16)), w);
+}
+template <typename K> static void warp_launch(FbSim* s, const char*, int n, size_t slice, const K& k) {
+  dev_launch(s, K_MISC, [&] { fb_run_warps<<<(n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), slice * FB_WPB, s->stream>>>(k, n, (unsigned)slice); });
+}
 #else
 template <typename Sh> static void set_prog(Sh&, const unsigned*) {}
 static void set_prog(ShTree& sh, const unsigned* p) { sh.prog = p; }
@@ -274,6 +292,7 @@ static void fb_launch_warp(FbSim* s, int kind) {
   emu_launch(s, kKindNames[kind], sizeof(float) * FB_SOLVE_WARP_FLOATS, s->d.Np, nullptr,
              [&](unsigned char* buf, int e) { ksolve_warp(s->m, s->d, reinterpret_cast<float*>(buf), e); });
 }
+template <typename K> static void warp_launch(FbSim* s, const char* kernel, int n, size_t slice, const K& k) { emu_launch(s, kernel, slice, n, nullptr, k); }
 #endif
 
 // per-env kernels wrapped as single-phase functions
@@ -1682,30 +1701,19 @@ static std::vector<StSeg> state_layout(FbSim* s, unsigned* row, uint64_t* sig, i
   *row = (unsigned)off; *sig = h;
   return v;
 }
-#ifndef FB_EMU
-template <bool LOAD> __global__ void __launch_bounds__(32 * FB_WPB) fb_state_kernel(StArgs a) {
-  const int w = blockIdx.x * FB_WPB + threadIdx.y;
-  if (w >= a.n) return;
-  const int old_pick = LOAD ? kstate_pick(a, w) : -1;
-  kstate_copy<LOAD>(a, w, threadIdx.x);
-  if (LOAD) { __syncwarp(); kstate_terrain(a, w, threadIdx.x, old_pick); }
-}
+template <bool LOAD> struct StateWarp {
+  StArgs a;
+  FB_DEVM void operator()(unsigned char*, int w) const {
+    int old_pick = -1;                       // a load: the env's terrain, read before any lane copies the row's over it
+    if (LOAD) { WPAR_BEGIN old_pick = kstate_pick(a, w); WPAR_END }
+    WPAR_BEGIN kstate_copy<LOAD>(a, w, lane); WPAR_END
+    if (LOAD) { WPAR_BEGIN kstate_terrain(a, w, lane, old_pick); WPAR_END }
+  }
+};
 // the (env, slot) pairs of the device lists env_ids / slots (NULL: the identity)
 template <bool LOAD> static void launch_state(FbSim* s, const int* env_ids, const int* slots, int n) {
-  StArgs a = {s->st_segs_dev, s->st_nseg, s->st_bank, s->st_row, env_ids, slots, n, s->d.task};
-  fb_state_kernel<LOAD><<<(n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(a);
-  s->launches++;
+  warp_launch(s, "state", n, 0, StateWarp<LOAD>{{s->st_segs_dev, s->st_nseg, s->st_bank, s->st_row, env_ids, slots, n, s->d.task}});
 }
-#else
-template <bool LOAD> static void launch_state(FbSim* s, const int* env_ids, const int* slots, int n) {
-  StArgs a = {s->st_segs_dev, s->st_nseg, s->st_bank, s->st_row, env_ids, slots, n, s->d.task};
-  emu_launch(s, "state", 0, n, nullptr, [&](unsigned char*, int w) {
-    const int old_pick = LOAD ? kstate_pick(a, w) : -1;
-    for (int y = 0; y < FB_NY; y++) kstate_copy<LOAD>(a, w, y);
-    if (LOAD) for (int y = 0; y < FB_NY; y++) kstate_terrain(a, w, y, old_pick);
-  });
-}
-#endif
 static int state_ready(FbSim* s, const char* who) {
   if (s->st_bank) return 0;
   s->err = std::string(who) + (s->st_stale ? ": the state bank was dropped when the handle's programs, reference slots or applied-force arrays changed: call fb_state_bank again"
@@ -1834,29 +1842,15 @@ int fb_state_write(FbHandle s, const int32_t* slots, int n, const void* host_src
 // -------------------------------------------------------------------------------------------
 // inverse kinematics (fb_ik_*; fb_ik.h): its own kernel parameter (DevIk) and buffers (ik_scope), bounded launches
 #define FB_IK_LAUNCH_ITERS (4 * FB_IK_CHECK)       // iterations per launch: the host reads the live count once per launch
-#ifndef FB_EMU
-__global__ void __launch_bounds__(32 * FB_WPB) fb_ik_kernel(DevModel m, DevData d, DevIk p) {
-  extern __shared__ __align__(16) float fb_smem_ik[];
-  kik_run(m, d, p, fb_smem_ik + (size_t)threadIdx.y * FB_IK_SH(p.n_fdof), blockIdx.x * FB_WPB + threadIdx.y);
-}
-static void launch_ik(FbSim* s) {
-  const DevIk& p = s->ik;
-  const size_t bytes = sizeof(float) * FB_IK_SH(p.n_fdof) * FB_WPB;
-  fb_ik_kernel<<<(p.n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), bytes, s->stream>>>(s->m, s->d, p);
-  s->launches++;
-}
-#else
-static void launch_ik(FbSim* s) {
-  const DevIk& p = s->ik;
-  emu_launch(s, "ik", sizeof(float) * FB_IK_SH(p.n_fdof), p.n, nullptr,
-             [&](unsigned char* sh, int e) { kik_run(s->m, s->d, p, reinterpret_cast<float*>(sh), e); });
-}
-#endif
+struct IkWarp {
+  DevModel m; DevData d; DevIk p;
+  FB_DEVM void operator()(unsigned char* sh, int e) const { kik_run(m, d, p, reinterpret_cast<float*>(sh), e); }
+};
 // one bounded launch; *live: the problems still iterating after it
 static int ik_launch(FbSim* s, int* live) {
   static const int zero = 0;
   if (copy_async(s, s->ik.live, &zero, sizeof(int)) != 0) return -2;
-  launch_ik(s);
+  warp_launch(s, "ik", s->ik.n, sizeof(float) * FB_IK_SH(s->ik.n_fdof), IkWarp{s->m, s->d, s->ik});
   if (launch_check(s, "fb_ik_solve") != 0 || copy_async(s, live, s->ik.live, sizeof(int)) != 0) return -2;
   return sync_stream(s);
 }
@@ -1939,34 +1933,20 @@ int fb_ik_read(FbHandle s, float* qpos, float* err, float* err_first, int32_t* s
   const DevIk& p = s->ik;
   if (!p.live || s->ik_solved < 1) { s->err = "fb_ik_read: no IK solve to read"; return -1; }
   if (sync_stream(s) != 0) return -2;
-  const int n = s->ik_solved, nq = s->m.nq;
-  if (qpos && copy_rows_async(s, qpos, (size_t)nq * 4, s->d.qpos, (size_t)s->d.rec * 4, (size_t)nq * 4, n) != 0) return -2;
-  if (err && copy_async(s, err, p.err, sizeof(float) * n) != 0) return -2;
-  if (err_first && copy_async(s, err_first, p.err_first, sizeof(float) * n) != 0) return -2;
-  if (steps && copy_async(s, steps, p.steps, sizeof(int) * n) != 0) return -2;
-  if (success && copy_async(s, success, p.success, n) != 0) return -2;
-  return sync_stream(s);
+  const size_t n = s->ik_solved, nq = s->m.nq;
+  return read_out(s, {{qpos, s->d.qpos, (size_t)s->d.rec * 4, nq * 4, n}, {err, p.err, 0, 4 * n, 1}, {err_first, p.err_first, 0, 4 * n, 1},
+                      {steps, p.steps, 0, 4 * n, 1}, {success, p.success, 0, n, 1}});
 }
 
 }  // extern "C"
 
 // -------------------------------------------------------------------------------------------
 // inverse dynamics (fb_inverse*; fb_inverse.h): its own kernel parameter (DevInv) and buffers (inv_scope), allocated on first use
-#ifndef FB_EMU
-__global__ void __launch_bounds__(32 * FB_WPB) fb_inv_kernel(DevModel m, DevData d, DevInv p) {
-  __shared__ float fb_smem_inv[FB_WPB][FB_INV_SH];
-  kinv_run(m, d, p, fb_smem_inv[threadIdx.y], blockIdx.x * FB_WPB + threadIdx.y);
-}
-static void launch_inv(FbSim* s, const DevInv& p) {
-  fb_inv_kernel<<<(p.n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, p);
-  s->launches++;
-}
-#else
-static void launch_inv(FbSim* s, const DevInv& p) {
-  emu_launch(s, "inverse", sizeof(float) * FB_INV_SH, p.n, nullptr,
-             [&](unsigned char* sh, int e) { kinv_run(s->m, s->d, p, reinterpret_cast<float*>(sh), e); });
-}
-#endif
+struct InvWarp {
+  DevModel m; DevData d; DevInv p;
+  FB_DEVM void operator()(unsigned char* sh, int e) const { kinv_run(m, d, p, reinterpret_cast<float*>(sh), e); }
+};
+static void launch_inv(FbSim* s, const DevInv& p) { warp_launch(s, "inverse", p.n, sizeof(float) * FB_INV_SH, InvWarp{s->m, s->d, p}); }
 static int inv_alloc(FbSim* s) {
   if (s->inv.qacc) return 0;
   const size_t Np = (size_t)s->d.Np, nv = (size_t)s->m.nv;
@@ -2003,49 +1983,31 @@ int fb_inverse_read(FbHandle s, float* qfrc_inverse, float* qfrc_constraint, flo
   const DevInv& p = s->inv;
   if (s->inv_done < 1) { s->err = "fb_inverse_read: no inverse to read (fb_inverse)"; return -1; }
   const size_t n = (size_t)s->inv_done, nv = (size_t)s->m.nv;
-  (void)is_device;                             // (the copies take their direction from the pointers)
-  if (qfrc_inverse && copy_async(s, qfrc_inverse, p.qfrc_inverse, sizeof(float) * n * nv) != 0) return -2;
-  if (qfrc_constraint && copy_async(s, qfrc_constraint, p.qfrc_constraint, sizeof(float) * n * nv) != 0) return -2;
-  if (efc_force && copy_async(s, efc_force, p.efc_force, sizeof(float) * n * FB_MAXEFC) != 0) return -2;
-  return sync_stream(s);
+  return read_out(s, {{qfrc_inverse, p.qfrc_inverse, 0, 4 * n * nv, 1}, {qfrc_constraint, p.qfrc_constraint, 0, 4 * n * nv, 1},
+                      {efc_force, p.efc_force, 0, 4 * n * FB_MAXEFC, 1}});
 }
 
 }  // extern "C"
 
 // -------------------------------------------------------------------------------------------
 // transition Jacobians (fb_fd_*; fb_fd.h): its own kernel parameter (DevFd) and buffers (fd_scope), allocated on first use
-#ifndef FB_EMU
-__global__ void __launch_bounds__(32 * FB_WPB) fb_fd_perturb(DevModel m, DevData d, DevFd p) {
-  const int e = blockIdx.x * FB_WPB + threadIdx.y;
-  if (e < d.N) kfd_perturb(m, d, p, e);
-}
-__global__ void __launch_bounds__(32 * FB_WPB) fb_fd_diff(DevModel m, DevData d, DevFd p) {
-  const int w = blockIdx.x * FB_WPB + threadIdx.y;
-  if (w < p.n * p.nin) kfd_diff(m, d, p, w);
-}
-static void launch_fd_perturb(FbSim* s) {
-  dev_launch(s, K_MISC, [&] { fb_fd_perturb<<<(s->d.N + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->fd); });
-}
-static void launch_fd_diff(FbSim* s) {
-  const int n = s->fd.n * s->fd.nin;
-  dev_launch(s, K_MISC, [&] { fb_fd_diff<<<(n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->fd); });
-}
-#else
-static void launch_fd_perturb(FbSim* s) {
-  emu_launch(s, "fd_perturb", 0, s->d.N, nullptr, [&](unsigned char*, int e) { kfd_perturb(s->m, s->d, s->fd, e); });
-}
-static void launch_fd_diff(FbSim* s) {
-  emu_launch(s, "fd_diff", 0, s->fd.n * s->fd.nin, nullptr, [&](unsigned char*, int w) { kfd_diff(s->m, s->d, s->fd, w); });
-}
-#endif
-static int fd_columns(const FbSim* s, int centered) {
-  const int nin = 2 * s->m.nv + s->m.na + s->m.nu;
+struct FdPerturb {
+  DevModel m; DevData d; DevFd p;
+  FB_DEVM void operator()(unsigned char*, int e) const { kfd_perturb(m, d, p, e); }
+};
+struct FdDiff {
+  DevModel m; DevData d; DevFd p;
+  FB_DEVM void operator()(unsigned char*, int w) const { kfd_diff(m, d, p, w); }
+};
+// envs per problem of the transition (inputs dq, qvel, act, ctrl) or inverse-dynamics (dq, qvel, qacc) Jacobians
+static int fd_columns(const FbSim* s, bool inverse, int centered) {
+  const int nin = inverse ? 3 * s->m.nv : 2 * s->m.nv + s->m.na + s->m.nu;
   return centered ? 1 + 2 * nin : 1 + nin;
 }
 static int fd_alloc(FbSim* s) {
   if (s->fd.delta) return 0;
   const DevModel& m = s->m;
-  const size_t nx = 2 * (size_t)m.nv + m.na, cap = std::max(1, s->d.N / fd_columns(s, 0));
+  const size_t nx = 2 * (size_t)m.nv + m.na, cap = std::max(1, s->d.N / fd_columns(s, false, 0));
   DevFd& p = s->fd;
   if (int rc = scope_alloc(s, s->fd_scope, "out of device memory (transition Jacobians)", [&] {
         p.delta = dalloc<float>(s, s->d.Np); p.A = dalloc<float>(s, cap * nx * nx); p.B = dalloc<float>(s, cap * nx * std::max(m.nu, 1));
@@ -2057,12 +2019,12 @@ static int fd_alloc(FbSim* s) {
 
 extern "C" {
 
-int fb_fd_columns(FbHandle s, int centered) { return s ? fd_columns(s, centered != 0) : -1; }
+int fb_fd_columns(FbHandle s, int centered) { return s ? fd_columns(s, false, centered != 0) : -1; }
 
 int fb_fd_transition(FbHandle s, const int32_t* slots, int n, float eps, int centered, int n_substeps) {
   if (!s) return -1;
   if (state_ready(s, "fb_fd_transition") != 0) return -1;
-  const int N = s->d.N, ncol = fd_columns(s, centered != 0);
+  const int N = s->d.N, ncol = fd_columns(s, false, centered != 0);
   if (!slots || n < 1 || (long long)n * ncol > N) {
     s->err = "fb_fd_transition: 1 <= n problems with n * fb_fd_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
   if (!(eps > 0.0f) || !std::isfinite(eps)) { s->err = "fb_fd_transition: eps must be positive and finite"; return -1; }
@@ -2084,10 +2046,10 @@ int fb_fd_transition(FbHandle s, const int32_t* slots, int n, float eps, int cen
   p.n = n; p.ncol = ncol; p.nx = 2 * s->m.nv + s->m.na; p.nin = p.nx + s->m.nu; p.centered = centered != 0; p.eps = eps;
   s->fd_done = 0;
   launch_state<true>(s, nullptr, sd, N);
-  launch_fd_perturb(s);
+  warp_launch(s, "fd_perturb", N, 0, FdPerturb{s->m, s->d, p});
   launch_step1(s);                             // the position / velocity stage of the nudged states
   step_run(s, n_substeps);                     // fb_step's launches
-  launch_fd_diff(s);
+  warp_launch(s, "fd_diff", n * p.nin, 0, FdDiff{s->m, s->d, p});
   if (launch_check(s, "fb_fd_transition") != 0) return -2;
   s->fd_done = n;
   return sync_stream(s);                       // (the fan-out list is a host vector)
@@ -2099,13 +2061,8 @@ int fb_fd_read(FbHandle s, float* A, float* B, float* qpos_next, float* qvel_nex
   const DevFd& p = s->fd;
   const size_t n = (size_t)s->fd_done, nx = (size_t)p.nx, nu = (size_t)(p.nin - p.nx);
   const size_t nq = s->m.nq, nv = s->m.nv, na = s->m.na, row = (nq + nv + na) * 4;
-  (void)is_device;                             // (the copies take their direction from the pointers)
-  if (A && copy_async(s, A, p.A, sizeof(float) * n * nx * nx) != 0) return -2;
-  if (B && nu && copy_async(s, B, p.B, sizeof(float) * n * nx * nu) != 0) return -2;
-  if (qpos_next && copy_rows_async(s, qpos_next, nq * 4, p.next, row, nq * 4, n) != 0) return -2;
-  if (qvel_next && copy_rows_async(s, qvel_next, nv * 4, p.next + nq, row, nv * 4, n) != 0) return -2;
-  if (act_next && na && copy_rows_async(s, act_next, na * 4, p.next + nq + nv, row, na * 4, n) != 0) return -2;
-  return sync_stream(s);
+  return read_out(s, {{A, p.A, 0, 4 * n * nx * nx, 1}, {B, p.B, 0, 4 * n * nx * nu, 1}, {qpos_next, p.next, row, nq * 4, n},
+                      {qvel_next, p.next + nq, row, nv * 4, n}, {act_next, p.next + nq + nv, row, na * 4, n}});
 }
 
 }  // extern "C"
@@ -2113,35 +2070,18 @@ int fb_fd_read(FbHandle s, float* A, float* B, float* qpos_next, float* qvel_nex
 // -------------------------------------------------------------------------------------------
 // inverse-dynamics Jacobians (fb_fd_inverse*; fb_fd.h): their own kernel parameter (DevFdInv, with its own DevInv) and buffers
 // (fdi_scope), allocated on first use; fb_inverse's DevInv is not touched
-#ifndef FB_EMU
-__global__ void __launch_bounds__(32 * FB_WPB) fb_fdi_perturb(DevModel m, DevData d, DevFdInv p) {
-  const int e = blockIdx.x * FB_WPB + threadIdx.y;
-  if (e < d.N) kfdi_perturb(m, d, p, e);
-}
-__global__ void __launch_bounds__(32 * FB_WPB) fb_fdi_diff(DevModel m, DevData d, DevFdInv p) {
-  const int w = blockIdx.x * FB_WPB + threadIdx.y;
-  if (w < p.n * p.nin) kfdi_diff(m, d, p, w);
-}
-static void launch_fdi_perturb(FbSim* s) {
-  dev_launch(s, K_MISC, [&] { fb_fdi_perturb<<<(s->d.N + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->fdi); });
-}
-static void launch_fdi_diff(FbSim* s) {
-  const int n = s->fdi.n * s->fdi.nin;
-  dev_launch(s, K_MISC, [&] { fb_fdi_diff<<<(n + FB_WPB - 1) / FB_WPB, dim3(32, FB_WPB), 0, s->stream>>>(s->m, s->d, s->fdi); });
-}
-#else
-static void launch_fdi_perturb(FbSim* s) {
-  emu_launch(s, "fdi_perturb", 0, s->d.N, nullptr, [&](unsigned char*, int e) { kfdi_perturb(s->m, s->d, s->fdi, e); });
-}
-static void launch_fdi_diff(FbSim* s) {
-  emu_launch(s, "fdi_diff", 0, s->fdi.n * s->fdi.nin, nullptr, [&](unsigned char*, int w) { kfdi_diff(s->m, s->d, s->fdi, w); });
-}
-#endif
-static int fdi_columns(const FbSim* s, int centered) { return centered ? 1 + 6 * s->m.nv : 1 + 3 * s->m.nv; }
+struct FdiPerturb {
+  DevModel m; DevData d; DevFdInv p;
+  FB_DEVM void operator()(unsigned char*, int e) const { kfdi_perturb(m, d, p, e); }
+};
+struct FdiDiff {
+  DevModel m; DevData d; DevFdInv p;
+  FB_DEVM void operator()(unsigned char*, int w) const { kfdi_diff(m, d, p, w); }
+};
 static int fdi_alloc(FbSim* s) {
   if (s->fdi.delta) return 0;
   const size_t Np = (size_t)s->d.Np, nq = (size_t)s->m.nq, nv = (size_t)s->m.nv, nM = (size_t)s->m.nM;
-  const size_t cap = std::max(1, s->d.N / fdi_columns(s, 0));
+  const size_t cap = std::max(1, s->d.N / fd_columns(s, true, 0));
   DevFdInv& p = s->fdi;
   if (int rc = scope_alloc(s, s->fdi_scope, "out of device memory (inverse-dynamics Jacobians)", [&] {
         p.qpos = dalloc<float>(s, cap * nq); p.qvel = dalloc<float>(s, cap * nv); p.qacc = dalloc<float>(s, cap * nv);
@@ -2157,11 +2097,11 @@ static int fdi_alloc(FbSim* s) {
 
 extern "C" {
 
-int fb_fd_inverse_columns(FbHandle s, int centered) { return s ? fdi_columns(s, centered != 0) : -1; }
+int fb_fd_inverse_columns(FbHandle s, int centered) { return s ? fd_columns(s, true, centered != 0) : -1; }
 
 int fb_fd_inverse(FbHandle s, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device) {
   if (!s) return -1;
-  const int N = s->d.N, ncol = fdi_columns(s, centered != 0);
+  const int N = s->d.N, ncol = fd_columns(s, true, centered != 0);
   if (n < 1 || (long long)n * ncol > N) {
     s->err = "fb_fd_inverse: 1 <= n problems with n * fb_fd_inverse_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
   if (!qpos || !qvel || !qacc) { s->err = "fb_fd_inverse: qpos, qvel and qacc must not be NULL"; return -1; }
@@ -2181,10 +2121,10 @@ int fb_fd_inverse(FbHandle s, int n, const float* qpos, const float* qvel, const
   p.n = n; p.ncol = ncol; p.nin = 3 * (int)nv; p.centered = centered != 0; p.eps = eps;
   p.inv.n = n * ncol;
   s->fdi_done = 0;
-  launch_fdi_perturb(s);                       // fan-out and nudge
+  warp_launch(s, "fdi_perturb", N, 0, FdiPerturb{s->m, s->d, p});   // fan-out and nudge
   launch_step1(s);                             // the position / velocity stage of every env, as fb_inverse runs it
   launch_inv(s, p.inv);
-  launch_fdi_diff(s);
+  warp_launch(s, "fdi_diff", n * p.nin, 0, FdiDiff{s->m, s->d, p});
   if (launch_check(s, "fb_fd_inverse") != 0) return -2;
   s->fdi_done = n;
   return is_device ? 0 : sync_stream(s);       // host rows may be reused once the call returns
@@ -2195,13 +2135,8 @@ int fb_fd_inverse_read(FbHandle s, float* DfDq, float* DfDv, float* DfDa, float*
   if (s->fdi_done < 1) { s->err = "fb_fd_inverse_read: no Jacobians to read (fb_fd_inverse)"; return -1; }
   const DevFdInv& p = s->fdi;
   const size_t n = (size_t)s->fdi_done, nv = (size_t)s->m.nv, nM = (size_t)s->m.nM;
-  (void)is_device;                             // (the copies take their direction from the pointers)
-  if (DfDq && copy_async(s, DfDq, p.DfDq, sizeof(float) * n * nv * nv) != 0) return -2;
-  if (DfDv && copy_async(s, DfDv, p.DfDv, sizeof(float) * n * nv * nv) != 0) return -2;
-  if (DfDa && copy_async(s, DfDa, p.DfDa, sizeof(float) * n * nv * nv) != 0) return -2;
-  if (DmDq && copy_async(s, DmDq, p.DmDq, sizeof(float) * n * nv * nM) != 0) return -2;
-  if (qfrc_inverse && copy_async(s, qfrc_inverse, p.qfrc, sizeof(float) * n * nv) != 0) return -2;
-  return sync_stream(s);
+  return read_out(s, {{DfDq, p.DfDq, 0, 4 * n * nv * nv, 1}, {DfDv, p.DfDv, 0, 4 * n * nv * nv, 1}, {DfDa, p.DfDa, 0, 4 * n * nv * nv, 1},
+                      {DmDq, p.DmDq, 0, 4 * n * nv * nM, 1}, {qfrc_inverse, p.qfrc, 0, 4 * n * nv, 1}});
 }
 
 }  // extern "C"

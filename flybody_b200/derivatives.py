@@ -44,35 +44,25 @@ def transition_fd(model, qpos, qvel, ctrl, act=None, eps=1e-2, centered=True, n_
     Returns Transition(A, B, qpos_next, qvel_next, act_next) as fp64 arrays of the device's fp32 values; *_next is the unperturbed
     state after the n_substeps substeps."""
     m = model
-    q = np.asarray(qpos, np.float64)
-    single = q.ndim == 1
-    q = q.reshape(-1, m.nq)
-    n = q.shape[0]
-    v = np.asarray(qvel, np.float64).reshape(-1, m.nv)
-    u = np.asarray(ctrl, np.float64).reshape(-1, m.nu)
-    a = np.zeros((n, m.na)) if act is None else np.asarray(act, np.float64).reshape(-1 if m.na else n, m.na)
-    if not (v.shape[0] == u.shape[0] == a.shape[0] == n):
-        raise ValueError(f'{n} qpos rows, {v.shape[0]} qvel rows, {u.shape[0]} ctrl rows, {a.shape[0]} act rows')
     ncol = 1 + (2 if centered else 1) * (2 * m.nv + m.na + m.nu)
     per = max(1, ENVS // ncol)
-    sim = st.BatchedStepper(m, per * ncol, device=device, lib_path=lib_path)
-    outs = []
-    try:
-        sim.state_bank(per)
-        for p0 in range(0, n, per):
-            k = min(per, n - p0)
-            rows = np.minimum(np.arange(sim.n_envs), k - 1) + p0        # the chunk's states in envs 0 .. k-1, the last one repeated
-            sim.reset(q[rows], v[rows])
-            if m.na:
-                sim.set(st.ACT, a[rows])
-            sim.set_control(u[rows])
-            sim.forward()
-            sim.save_state(slots=np.arange(k), env_ids=np.arange(k))
-            sim.fd_transition(np.arange(k), eps=eps, centered=centered, n_substeps=n_substeps)
-            outs.append(sim.fd_read())
-    finally:
-        sim.close()
-    res = Transition(*(np.concatenate([o[i] for o in outs]).astype(np.float64) for i in range(5)))
+
+    def run(sim, rows, k):
+        q, v, u, a = rows
+        pad = np.minimum(np.arange(sim.n_envs), k - 1)         # the chunk's states in envs 0 .. k-1, the last one repeated
+        sim.reset(q[pad], v[pad])
+        if m.na:
+            sim.set(st.ACT, a[pad])
+        sim.set_control(u[pad])
+        sim.forward()
+        sim.save_state(slots=np.arange(k), env_ids=np.arange(k))
+        sim.fd_transition(np.arange(k), eps=eps, centered=centered, n_substeps=n_substeps)
+        return sim.fd_read()
+
+    act = np.zeros(np.shape(qpos)[:-1] + (m.na,)) if act is None else act
+    single, out = st._batched(m, [('qpos', qpos, (m.nq,)), ('qvel', qvel, (m.nv,)), ('ctrl', ctrl, (m.nu,)), ('act', act, (m.na,))], run,
+                              per, n_envs=per * ncol, setup=lambda sim: sim.state_bank(per), device=device, lib_path=lib_path)
+    res = Transition(*(x.astype(np.float64) for x in out))
     return Transition(*(x[0] for x in res)) if single else res
 
 
@@ -84,24 +74,14 @@ def inverse_fd(model, qpos, qvel, qacc, eps=1e-2, centered=True, device=0, lib_p
     for qvel and qacc, DmDq [B, nv, nM] = d qM / d dq_i in MuJoCo's sparse qM order (the diagonal at dof_Madr, then the ancestors), and
     the unperturbed qfrc_inverse [B, nv].  centered=False is MuJoCo's forward difference."""
     m = model
-    q = np.asarray(qpos, np.float64)
-    single = q.ndim == 1
-    q = q.reshape(-1, m.nq)
-    n = q.shape[0]
-    v = np.asarray(qvel, np.float64).reshape(-1, m.nv)
-    a = np.asarray(qacc, np.float64).reshape(-1, m.nv)
-    if not (v.shape[0] == a.shape[0] == n):
-        raise ValueError(f'{n} qpos rows, {v.shape[0]} qvel rows, {a.shape[0]} qacc rows')
     ncol = 1 + (2 if centered else 1) * 3 * m.nv
     per = max(1, ENVS // ncol)
-    sim = st.BatchedStepper(m, per * ncol, device=device, lib_path=lib_path)
-    outs = []
-    try:
-        for p0 in range(0, n, per):
-            k = min(per, n - p0)
-            sim.fd_inverse(q[p0:p0 + k], v[p0:p0 + k], a[p0:p0 + k], eps=eps, centered=centered)
-            outs.append(sim.fd_inverse_read())
-    finally:
-        sim.close()
-    res = InverseJacobians(*(np.concatenate([o[i] for o in outs]).astype(np.float64) for i in range(5)))
+
+    def run(sim, rows, k):
+        sim.fd_inverse(*rows, eps=eps, centered=centered)
+        return sim.fd_inverse_read()
+
+    single, out = st._batched(m, [('qpos', qpos, (m.nq,)), ('qvel', qvel, (m.nv,)), ('qacc', qacc, (m.nv,))], run, per, n_envs=per * ncol,
+                              device=device, lib_path=lib_path)
+    res = InverseJacobians(*(x.astype(np.float64) for x in out))
     return InverseJacobians(*(x[0] for x in res)) if single else res

@@ -14,9 +14,7 @@ from collections import namedtuple
 import numpy as np
 
 from . import stepper as st
-from .inverse_kinematics import CHUNK, _quat_velocity
-
-FREE, BALL, HINGE = 0, 1, 3
+from .inverse_kinematics import CHUNK, HINGE, _differentiate_pos
 
 InverseResult = namedtuple('InverseResult', ['qfrc_inverse', 'qfrc_constraint', 'qfrc_bias', 'qfrc_passive', 'contacts'])
 # per problem: the contacts that have constraint rows; force holds mj_contactForce's six numbers for an elliptic cone (contact frame:
@@ -30,59 +28,29 @@ def inverse(model, qpos, qvel, qacc, device=0, lib_path=None):
     Returns InverseResult(qfrc_inverse, qfrc_constraint, qfrc_bias, qfrc_passive, contacts): four [B, nv] fp64 arrays of the device's
     fp32 values, and per problem a `Contacts` of its k contacts with rows: geom [k, 2] geom ids, pos [k, 3] world position, normal
     [k, 3], force [k, 6] in the contact frame."""
-    q = np.asarray(qpos, np.float64)
-    single = q.ndim == 1
-    q = q.reshape(-1, model.nq)
-    v = np.asarray(qvel, np.float64).reshape(-1, model.nv)
-    a = np.asarray(qacc, np.float64).reshape(-1, model.nv)
-    B = q.shape[0]
-    if v.shape[0] != B or a.shape[0] != B:
-        raise ValueError(f'{B} qpos rows, {v.shape[0]} qvel rows, {a.shape[0]} qacc rows')
-    n_env = min(B, CHUNK)
-    sim = st.BatchedStepper(model, n_env, device=device, lib_path=lib_path)
-    outs = {k: [] for k in ('qi', 'qc', 'bias', 'passive')}
-    contacts = []
-    try:
-        for a0 in range(0, B, n_env):
-            n = min(n_env, B - a0)
-            pad = lambda x: np.concatenate([x[a0:a0 + n], np.repeat(x[a0 + n - 1:a0 + n], n_env - n, 0)])
-            sim.set(st.QPOS, pad(q))
-            sim.set(st.QVEL, pad(v))
-            sim.inverse(a[a0:a0 + n])
-            qi, qc, f = sim.inverse_read()
-            outs['qi'].append(qi); outs['qc'].append(qc)
-            outs['bias'].append(sim.get(st.QFRC_BIAS)[:n]); outs['passive'].append(sim.get(st.QFRC_PASSIVE)[:n])
-            con, ncon = sim.get(st.CONTACT).reshape(n_env, st.MAXCON, 16), sim.get(st.NCON)[:, 0].astype(int)
-            for i in range(n):
-                c = con[i, :ncon[i]]
-                c = c[c[:, 12] >= 0]
-                force = np.zeros((len(c), 6))
-                for k, row in enumerate(c):
-                    adr, dim = int(row[12]), int(row[9])
-                    force[k, :dim] = f[i, adr:adr + dim]
-                contacts.append(Contacts(c[:, 7:9].astype(np.int64), c[:, 1:4].astype(np.float64), c[:, 4:7].astype(np.float64), force))
-    finally:
-        sim.close()
-    res = InverseResult(*(np.concatenate(outs[k]).astype(np.float64) for k in ('qi', 'qc', 'bias', 'passive')), contacts)
-    if single:
-        return InverseResult(res.qfrc_inverse[0], res.qfrc_constraint[0], res.qfrc_bias[0], res.qfrc_passive[0], contacts[0])
-    return res
+    def run(sim, rows, n):
+        q, v, a = rows
+        pad = np.minimum(np.arange(sim.n_envs), n - 1)         # the chunk's states, the last one repeated
+        sim.set(st.QPOS, q[pad])
+        sim.set(st.QVEL, v[pad])
+        sim.inverse(a)
+        qi, qc, f = sim.inverse_read()
+        con, ncon = sim.get(st.CONTACT).reshape(sim.n_envs, st.MAXCON, 16), sim.get(st.NCON)[:, 0].astype(int)
+        contacts = []
+        for i in range(n):
+            c = con[i, :ncon[i]]
+            c = c[c[:, 12] >= 0]
+            force = np.zeros((len(c), 6))
+            for k, row in enumerate(c):
+                adr, dim = int(row[12]), int(row[9])
+                force[k, :dim] = f[i, adr:adr + dim]
+            contacts.append(Contacts(c[:, 7:9].astype(np.int64), c[:, 1:4].astype(np.float64), c[:, 4:7].astype(np.float64), force))
+        return qi, qc, sim.get(st.QFRC_BIAS)[:n], sim.get(st.QFRC_PASSIVE)[:n], contacts
 
-
-def _differentiate_pos(model, q1, q2, dt):
-    """MuJoCo mj_differentiatePos for rows of poses q1, q2 [T, nq] -> [T, nv]: hinge dq / dt; free joint world-frame linear and body-frame
-    angular velocity; ball joint body-frame angular velocity (the rotation part of inverse_kinematics._differentiate)"""
-    out = np.zeros((q1.shape[0], model.nv))
-    for j in range(model.njnt):
-        t, qa, da = int(model.jnt_type[j]), int(model.jnt_qposadr[j]), int(model.jnt_dofadr[j])
-        if t == HINGE:
-            out[:, da] = (q2[:, qa] - q1[:, qa]) / dt
-            continue
-        if t == FREE:
-            out[:, da:da + 3] = (q2[:, qa:qa + 3] - q1[:, qa:qa + 3]) / dt
-            qa, da = qa + 3, da + 3
-        out[:, da:da + 3] = _quat_velocity(q1[:, qa:qa + 4], q2[:, qa:qa + 4], dt)
-    return out
+    single, out = st._batched(model, [('qpos', qpos, (model.nq,)), ('qvel', qvel, (model.nv,)), ('qacc', qacc, (model.nv,))], run, CHUNK,
+                              device=device, lib_path=lib_path)
+    res = InverseResult(*(x.astype(np.float64) for x in out[:4]), out[4])
+    return InverseResult(*(x[0] for x in res)) if single else res
 
 
 def differentiate(model, qpos_track, dt):

@@ -18,6 +18,7 @@ from .synthetic import mult_quat
 IKResult = namedtuple('IKResult', ['qpos', 'err_norm', 'err_norm_first_term', 'steps', 'success'])
 
 CHUNK = 4096                     # problems per device batch: memory stays bounded for any B
+FREE, HINGE = 0, 3               # mjtJoint
 
 
 def _include_mask(include_inds, n_sites):
@@ -42,23 +43,18 @@ def qpos_from_site_xpos(model, site_names, target_xpos, joint_names, reg_strengt
     names = model.meta['site_names']
     site_ids = [names.index(s) for s in site_names]
     jnt_ids = [model.jnt_id(j) for j in joint_names]
-    t = np.asarray(target_xpos, np.float64)
-    single = t.ndim == 2
-    t = t.reshape(-1, len(site_ids), 3)
-    B = t.shape[0]
-    q0 = model.qpos0 if init_qpos is None else np.asarray(init_qpos, np.float64)
-    q0 = np.broadcast_to(q0.reshape(-1, model.nq), (B, model.nq))
-    n_env = min(B, CHUNK)
-    sim = st.BatchedStepper(model, n_env, device=device, lib_path=lib_path)
-    try:
-        sim.ik_program(site_ids, jnt_ids, _include_mask(include_inds, len(site_ids)), reg_strength, lr, beta, progress_threshold, max_steps)
-        outs = []
-        for a in range(0, B, n_env):
-            sim.ik_solve(t[a:a + n_env], q0[a:a + n_env])
-            outs.append(sim.ik_read())
-    finally:
-        sim.close()
-    qpos, err, err1, steps, ok = (np.concatenate(c) for c in zip(*outs))
+    B = np.size(target_xpos) // (3 * len(site_ids))
+    q0 = np.broadcast_to(np.reshape(model.qpos0 if init_qpos is None else init_qpos, (-1, model.nq)), (B, model.nq))
+
+    def run(sim, rows, k):
+        sim.ik_solve(*rows)
+        return sim.ik_read()
+
+    single, (qpos, err, err1, steps, ok) = st._batched(
+        model, [('target_xpos', target_xpos, (len(site_ids), 3)), ('init_qpos', q0, (model.nq,))], run, CHUNK,
+        setup=lambda sim: sim.ik_program(site_ids, jnt_ids, _include_mask(include_inds, len(site_ids)), reg_strength, lr, beta,
+                                         progress_threshold, max_steps),
+        device=device, lib_path=lib_path)
     res = IKResult(qpos.astype(np.float64), err.astype(np.float64), err1.astype(np.float64), steps.astype(np.int64), ok)
     if single:
         return IKResult(res.qpos[0], float(res.err_norm[0]), float(res.err_norm_first_term[0]), int(res.steps[0]), bool(res.success[0]))
@@ -84,15 +80,20 @@ def _quat_velocity(q1, q2, dt):
     return axis * angle / dt
 
 
-def _differentiate(qpos, root_qadr, hinge_qadr, dt):
-    """forward differences of [T, nq] poses, last row repeated: root linear (world frame), root angular (body frame), hinges"""
-    q = np.asarray(qpos, np.float64)
-    lin = (q[1:, root_qadr:root_qadr + 3] - q[:-1, root_qadr:root_qadr + 3]) / dt
-    ang = _quat_velocity(q[:-1, root_qadr + 3:root_qadr + 7], q[1:, root_qadr + 3:root_qadr + 7], dt)
-    hv = (q[1:, hinge_qadr] - q[:-1, hinge_qadr]) / dt
-    root_qvel = np.concatenate([lin, ang], 1)
-    rep = lambda a: np.concatenate([a, a[-1:]]) if len(a) else np.zeros((1,) + a.shape[1:])
-    return rep(root_qvel), rep(hv)
+def _differentiate_pos(model, q1, q2, dt):
+    """MuJoCo mj_differentiatePos for rows of poses q1, q2 [T, nq] -> [T, nv]: hinge dq / dt; free joint world-frame linear and body-frame
+    angular velocity; ball joint body-frame angular velocity"""
+    out = np.zeros((q1.shape[0], model.nv))
+    for j in range(model.njnt):
+        t, qa, da = int(model.jnt_type[j]), int(model.jnt_qposadr[j]), int(model.jnt_dofadr[j])
+        if t == HINGE:
+            out[:, da] = (q2[:, qa] - q1[:, qa]) / dt
+            continue
+        if t == FREE:
+            out[:, da:da + 3] = (q2[:, qa:qa + 3] - q1[:, qa:qa + 3]) / dt
+            qa, da = qa + 3, da + 3
+        out[:, da:da + 3] = _quat_velocity(q1[:, qa:qa + 4], q2[:, qa:qa + 4], dt)
+    return out
 
 
 def write_walking_dataset(path, model, qpos_tracks, timestep, joint_names, site_names, device=0, lib_path=None):
@@ -106,7 +107,7 @@ def write_walking_dataset(path, model, qpos_tracks, timestep, joint_names, site_
     from `rewards.joint_orientation_quat`."""
     tracks = [np.asarray(qpos_tracks, np.float64)] if np.ndim(qpos_tracks) == 2 else [np.asarray(t, np.float64) for t in qpos_tracks]
     rj = _root_joint(model)
-    rq, root_body = int(model.jnt_qposadr[rj]), int(model.jnt_bodyid[rj])
+    rq, rv, root_body = int(model.jnt_qposadr[rj]), int(model.jnt_dofadr[rj]), int(model.jnt_bodyid[rj])
     jid = [model.jnt_id(j) for j in joint_names]
     if any(int(model.jnt_type[j]) != 3 for j in jid):
         raise ValueError('joint_names must name hinge joints')
@@ -134,12 +135,13 @@ def write_walking_dataset(path, model, qpos_tracks, timestep, joint_names, site_
     off = 0
     for k, q in enumerate(tracks):
         T = len(q)
-        root_qvel, qvel = _differentiate(q, rq, hinge_qadr, timestep)
+        v = _differentiate_pos(model, q[:-1], q[1:], timestep)    # forward differences, last row repeated
+        v = np.concatenate([v, v[-1:]]) if len(v) else np.zeros((1, model.nv))
         g = f'trajectories/{str(k).zfill(len(str(len(tracks))))}/'
         d[g + 'root_qpos'] = q[:, rq:rq + 7]
         d[g + 'qpos'] = q[:, hinge_qadr]
-        d[g + 'root_qvel'] = root_qvel[:T]
-        d[g + 'qvel'] = qvel[:T]
+        d[g + 'root_qvel'] = v[:T, rv:rv + 6]
+        d[g + 'qvel'] = v[:T, hinge_dof]
         d[g + 'root2site'] = root2site[off:off + T]
         d[g + 'joint_quat'] = rewards.joint_orientation_quat(axes[off:off + T], q[:, hinge_qadr])
         off += T

@@ -180,6 +180,30 @@ def load_library(path=None):
     return lib
 
 
+def _batched(model, inputs, run, per, n_envs=None, setup=None, device=0, lib_path=None):
+    """The shell of the batched device front ends.  inputs: [(name, array, row shape)], coerced to fp64 rows; the first one without
+    its batch dimension makes a single problem.  One handle of n_envs envs (default: min(B, per)) solves `per` problems at a time:
+    setup(sim) once, then run(sim, chunk rows, k) -> a tuple of [k, ...] outputs (a list: per-problem objects).
+    -> (single, the outputs over all B problems)"""
+    rows = [np.asarray(x, np.float64) for _, x, _ in inputs]
+    single = rows[0].ndim == len(inputs[0][2])
+    B = rows[0].reshape((-1,) + tuple(inputs[0][2])).shape[0]
+    rows = [x.reshape((-1 if np.prod(shape) else B,) + tuple(shape)) for x, (_, _, shape) in zip(rows, inputs)]
+    if any(x.shape[0] != B for x in rows):
+        raise ValueError(', '.join(f'{x.shape[0]} {name} rows' for x, (name, _, _) in zip(rows, inputs)))
+    sim = BatchedStepper(model, min(B, per) if n_envs is None else n_envs, device=device, lib_path=lib_path)
+    outs = []
+    try:
+        if setup is not None:
+            setup(sim)
+        for p0 in range(0, B, per):
+            k = min(per, B - p0)
+            outs.append(run(sim, [x[p0:p0 + k] for x in rows], k))
+    finally:
+        sim.close()
+    return single, [np.concatenate(c) if isinstance(c[0], np.ndarray) else [x for part in c for x in part] for c in zip(*outs)]
+
+
 class BatchedStepper:
     """N fly environments stepped in lock-step on one device."""
 
@@ -349,20 +373,27 @@ class BatchedStepper:
         return q, e, e1, k, ok.astype(bool)
 
     # ---- inverse dynamics (fb_inverse; flybody_b200.inverse_dynamics is the batched front end)
+    def _problem_rows(self, inputs, n, is_device):
+        """the inputs [(name, array or device pointer, row width)] of a call on problems 0 .. n-1 -> (n, pointers, host rows): device
+        pointers (ints) with is_device=True and n given, or host arrays of equal row counts as fp32 rows (keep them alive for the call)"""
+        if is_device:
+            if n is None:
+                raise ValueError('device inputs need n')
+            return int(n), [C.c_void_p(int(x)) for _, x, _ in inputs], None
+        rows = [np.ascontiguousarray(np.asarray(x, np.float32).reshape(-1, k)) for _, x, k in inputs]
+        if len({r.shape[0] for r in rows}) != 1:
+            raise ValueError(', '.join(f'{r.shape[0]} {name} rows' for (name, _, _), r in zip(inputs, rows)))
+        n = rows[0].shape[0] if n is None else int(n)
+        if n > rows[0].shape[0]:
+            raise ValueError(f'{rows[0].shape[0]} rows for n = {n}')
+        return n, [r.ctypes.data for r in rows], rows
+
     def inverse(self, qacc, n=None, is_device=False):
         """mj_inverse for envs 0 .. n-1 at their current qpos / qvel: qacc [n, nv] (host array), or a device pointer (int) with
         is_device=True and n given.  Stream-ordered; read the results with inverse_read()."""
-        if is_device:
-            if n is None:
-                raise ValueError('a device qacc needs n')
-            self._check(self._lib.fb_inverse(self._h, int(n), C.c_void_p(int(qacc)), 1), 'fb_inverse')
-        else:
-            q = np.ascontiguousarray(np.asarray(qacc, np.float32).reshape(-1, self.model.nv))
-            n = q.shape[0] if n is None else int(n)
-            if n > q.shape[0]:
-                raise ValueError(f'{q.shape[0]} qacc rows for n = {n}')
-            self._check(self._lib.fb_inverse(self._h, n, q.ctypes.data, 0), 'fb_inverse')
-        self._inv_n = int(n)
+        n, ptrs, _rows = self._problem_rows([('qacc', qacc, self.model.nv)], n, is_device)
+        self._check(self._lib.fb_inverse(self._h, n, *ptrs, int(bool(is_device))), 'fb_inverse')
+        self._inv_n = n
 
     def inverse_read(self):
         """-> (qfrc_inverse [n, nv], qfrc_constraint [n, nv], efc_force [n, MAXEFC]) f32 of the last inverse"""
@@ -403,20 +434,9 @@ class BatchedStepper:
         pointers (ints) with is_device=True and n given (see the header); the envs' states are a workspace afterwards.  Read the results
         with fd_inverse_read()."""
         m = self.model
-        if is_device:
-            if n is None:
-                raise ValueError('device inputs need n')
-            ptrs = [C.c_void_p(int(x)) for x in (qpos, qvel, qacc)]
-        else:
-            rows = [np.ascontiguousarray(np.asarray(x, np.float32).reshape(-1, k)) for x, k in ((qpos, m.nq), (qvel, m.nv), (qacc, m.nv))]
-            if len({r.shape[0] for r in rows}) != 1:
-                raise ValueError(f'{rows[0].shape[0]} qpos rows, {rows[1].shape[0]} qvel rows, {rows[2].shape[0]} qacc rows')
-            n = rows[0].shape[0] if n is None else int(n)
-            if n > rows[0].shape[0]:
-                raise ValueError(f'{rows[0].shape[0]} rows for n = {n}')
-            ptrs = [r.ctypes.data for r in rows]
-        self._check(self._lib.fb_fd_inverse(self._h, int(n), *ptrs, float(eps), int(bool(centered)), int(bool(is_device))), 'fb_fd_inverse')
-        self._fdi_n = int(n)
+        n, ptrs, _rows = self._problem_rows([('qpos', qpos, m.nq), ('qvel', qvel, m.nv), ('qacc', qacc, m.nv)], n, is_device)
+        self._check(self._lib.fb_fd_inverse(self._h, n, *ptrs, float(eps), int(bool(centered)), int(bool(is_device))), 'fb_fd_inverse')
+        self._fdi_n = n
 
     def fd_inverse_read(self):
         """-> (DfDq, DfDv, DfDa [n, nv, nv], DmDq [n, nv, nM], qfrc_inverse [n, nv]) f32 of the last fd_inverse, transposed as MuJoCo's:

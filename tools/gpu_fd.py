@@ -5,8 +5,8 @@
 1. Jacobians/s of the template (walking, 4096 // 669 or 4096 // 335 problems per call) and flight (4096 // 215, 4096 // 108) models,
    centred and forward, at n_substeps 1 and 10, on full-size handles (derivatives.ENVS envs): --reps back-to-back fd_transition calls
    (each ends in a device synchronise) timed on the host, --repeats times, after a warm-up call of every configuration.
-2. The per-launch split of one call of each configuration from fb_profile events (the step kinds; "misc" = the perturbation and
-   differencing kernels); the fan-out (one state-copy launch) is not evented and is the remainder of the call.
+2. The per-launch split of one call of each configuration from fb_profile events (the step kinds; "misc" = the fan-out (one
+   state-copy launch), perturbation and differencing kernels).
 3. An eps sweep: the device's centred A / B at eps 3e-1 ... 1e-4 against the fp64 reference (tests/fd_reference.py) at eps 1e-6, on 9
    constraint-free flight states (tests/smooth_states.py, without the two far from the origin) and 8 template states with ground contacts
    taken from a rollout.  Per state the per-column errors of tests/test_transition_fd.py; reported: the median and max over the states

@@ -6,7 +6,7 @@
    centred and forward, on full-size handles (derivatives.ENVS envs): --reps back-to-back fd_inverse calls with host inputs (each
    ends in a device synchronise) timed on the host, --repeats times, after a warm-up call of every configuration.
 2. The per-launch split of one call of each configuration from fb_profile events (the step kinds of the position / velocity stage;
-   "misc" = the fan-out / nudge and differencing kernels); the inverse kernel is not evented and is the remainder of the call.
+   "misc" = the fan-out / nudge, inverse and differencing kernels).
 3. An eps sweep: the device's centred Jacobians at eps 3e-1 ... 1e-4 against the fp64 reference (tests/inverse_fd_reference.py) at
    eps 1e-6, on 9 constraint-free flight states (tests/smooth_states.py, without the two far from the origin) and 8 states with ground
    contacts from a rollout of the analytic-contact template model (tests/solver_states.py).  Per state the per-row errors of
