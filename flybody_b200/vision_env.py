@@ -7,7 +7,7 @@ is the `vision` model variant (flight model without a ghost, ground contacts on,
 heightfield narrowphase (`fb_hfield_collision`, MuJoCo's prism walk + MPR, restated from memory), the eyes from the device ray
 caster (`fb_render_eyes`: MuJoCo's camera model, not its OpenGL image).  The task logic -- episode initialisation, the
 wing-beat generator in `before_step`, the seven reward factors, termination -- mirrors the reference in vectorised numpy on
-the read-back record, like the host path of `BatchedFlyEnv`.
+the read-back record, in the host control step every env shares (`fly_envs._TaskEnv`).
 """
 import collections
 
@@ -15,8 +15,8 @@ import numpy as np
 
 from . import arenas
 from . import stepper as st
-from .dm_env_shim import Array, StepType, TimeStep
-from .fly_envs import BatchedFlyEnv, BatchedWingBeatPatternGenerator, _TaskEnv, _device_tensor, _pinned
+from .dm_env_shim import Array
+from .fly_envs import BatchedWingBeatPatternGenerator, _TaskEnv, _device_tensor, _pinned
 from .flymodel import load_model
 from .synthetic import _FLY_CONTROL_TIMESTEP
 
@@ -32,7 +32,8 @@ def _tolerance_linear(x, lo, hi, margin):
 
 class BatchedVisionFlightEnv(_TaskEnv):
     """dm_env-shaped environment over N lock-stepped flies on their own terrains."""
-
+    # head 3, wings 6, abdomen 2 actions + 1 user action (beat frequency); the wing-beat generator builds ctrl on the host
+    _CONTROL_TIMESTEP, _KIND, _N_USER, _HOST_CTRL = _FLY_CONTROL_TIMESTEP, st.TASK_VISION, 1, True
     _OBS = ('accelerometer', 'actuator_activation', 'gyro', 'joints_pos', 'joints_vel', 'left_eye', 'right_eye', 'velocimeter', 'world_zaxis',
             'task_input')
 
@@ -41,9 +42,7 @@ class BatchedVisionFlightEnv(_TaskEnv):
                  init_pos_y_range=(0, 0), time_limit=0.4, floor_contacts_fatal=True, terrain_bank=None, device_task=False, **kwargs_arena):
         if bumps_or_trench not in ('bumps', 'trench'):
             raise ValueError("Only 'bumps' and 'trench' terrains are supported.")
-        # head 3, wings 6, abdomen 2 actions + 1 user action (beat frequency)
-        super().__init__(load_model('vision'), n_envs, device, lib_path, _FLY_CONTROL_TIMESTEP, time_limit, n_user=1, seed=seed,
-                         kind=st.TASK_VISION, device_task=device_task)
+        super().__init__(load_model('vision'), n_envs, device, lib_path, time_limit, seed, device_task)
         m, N = self.model, self.n_envs
         self._fatal = floor_contacts_fatal
         self._wbpg = BatchedWingBeatPatternGenerator(N, base_pattern_path=wpg_pattern_path)
@@ -63,15 +62,7 @@ class BatchedVisionFlightEnv(_TaskEnv):
                 self._bank.append((t.astype(np.float32), a0.trench_specs))
         self._sim.hfield_collision(m.meta['hf_geom'], m.hf_size, a0.nrow, a0.ncol, m.hf_pair_geom)
         self._ranges = dict(h=target_height_range, v=target_speed_range, x=init_pos_x_range, y=init_pos_y_range)
-        # index tables
-        jn, sens = m.meta['jnt_names'], m.meta['sensor_names']
-        self._root_q, self._root_v = m.jnt_qposadr_of('walker/'), m.jnt_dofadr_of('walker/')
-        obsj = [jn.index(n) for n in m.meta['observable_joints']]
-        self._obs_qadr, self._obs_vadr = m.jnt_qposadr[obsj], m.jnt_dofadr[obsj]
-        wing = [f'walker/wing_{a}_{s}' for s in ('left', 'right') for a in ('yaw', 'roll', 'pitch')]
-        self._wing_qadr = np.array([m.jnt_qposadr_of(n) for n in wing])
-        self._wing_vadr = np.array([m.jnt_dofadr_of(n) for n in wing])
-        self._wing_in_obs = np.array([m.meta['observable_joints'].index(n) for n in wing])
+        sens = m.meta['sensor_names']
         sd = lambda n: int(m.sensor_adr[sens.index('walker/' + n)])
         up = m.site_quat[m.meta['site_names'].index('walker/hover_up_dir')].copy()
         up[0] *= -1.0                                        # neg_quat(up_dir): the hover pose (vision_flight.py:124-126)
@@ -86,19 +77,11 @@ class BatchedVisionFlightEnv(_TaskEnv):
                 ('_velocimeter_now', 3, (st.OBS_SENSOR_NOW, sd('velocimeter'), 3)), ('_root_pose', 7, (st.OBS_ROOT_POSE, 0, 7)),
                 ('_root_qvel', 6, (st.OBS_QVEL, 2 * nq, 6)), ('_scalars', 3, (st.OBS_SCALARS, 0, 3)),
                 ('_world_contact', 1, (st.OBS_WORLD_CONTACT, 0, 1)), ('_task_target', 2, (st.OBS_TASK_TARGET, 0, 2))]
-        lists = list(self._obs_qadr) + list(self._obs_vadr) + list(range(self._root_v, self._root_v + 6))
-        dim = self._sim.obs_program([r[2] for r in rows], lists, m.body_id('walker/thorax'), self._n_sub, None)
-        off = np.concatenate([[0], np.cumsum([r[1] for r in rows])])
-        assert off[-1] == dim
-        # column slices of the rows (`_obs_slices`: the name the shared shell reads)
-        self._sl = self._obs_slices = {r[0]: slice(int(off[i]), int(off[i + 1])) for i, r in enumerate(rows)}
-        self._rec = _pinned((N, dim), np.float32)
-        self._out4 = _pinned((N, 4), np.float32)
+        self._upload_obs_program([(n, w, (w,), item) for n, w, item in rows],
+                                 list(self._obs_qadr) + list(self._obs_vadr) + list(range(self._root_v, self._root_v + 6)))
+        self._sl = self._obs_slices
         # eyes
-        quats = [np.asarray(q, np.float64) / np.linalg.norm(q) for _, _, q in BatchedFlyEnv._EYE_CAMERAS]
-        head = m.body_id('walker/head')
-        self._sim.eye_program([head, head], [p for _, p, _ in BatchedFlyEnv._EYE_CAMERAS], quats, fovy_deg=eye_camera_fovy, size=eye_camera_size,
-                              nrow=a0.nrow, ncol=a0.ncol, half_size=self._half, z_offset=float(m.geom_pos[m.meta['hf_geom']][2]))
+        self._eye_program(eye_camera_size, eye_camera_fovy, a0.nrow, a0.ncol, self._half, float(m.geom_pos[m.meta['hf_geom']][2]))
         self._eye_size = eye_camera_size
         self._eyes_host = _pinned((N, 2, eye_camera_size, eye_camera_size, 3), np.uint8)      # D2H target of every step's render
         self._eyes_dev = None
@@ -141,8 +124,7 @@ class BatchedVisionFlightEnv(_TaskEnv):
         """fb_task_program FB_TASK_VISION: the hooks of this env as a device-side program (same constants as the host path); `seed`
         seeds the device's counter-hash draws."""
         self._seed = seed
-        wb, r = self._wbpg, self._ranges
-        self._sim.set_action_map(np.concatenate([self._ctrl_of_action, [-1]]))      # the user action (beat frequency) has no ctrl slot
+        r = self._ranges
         self._sim.hfield_bank(np.stack([t for t, _ in self._bank]))
         dummy = np.zeros((1, 7), np.float32); dummy[0, 3] = 1.0
         trench = {}
@@ -153,12 +135,8 @@ class BatchedVisionFlightEnv(_TaskEnv):
                 ty[k, :len(sp['y_coords'])] = sp['y_coords']
             trench = dict(trench_cap=cap, trench_y=ty, trench_len=np.array([len(sp['y_coords']) for _, sp in self._bank], np.int32),
                           trench_x=np.array([[sp['x_coords'][0], sp['x_coords'][-1]] for _, sp in self._bank], np.float32))
-        self._sim.task_program(**self._task_program_base() | dict(
-            episode_steps=1 << 30, ref_len=1, ref_qpos=dummy, ref_qvel=np.zeros((1, 6), np.float32), n_wing=6, wing_qadr=self._wing_qadr,
-            wing_vadr=self._wing_vadr, wing_ctrl=self._ctrl_of_action[self._action_indices['wings']], n_freq=wb.traj.shape[0],
-            tab_len=wb.traj.shape[1], wb_traj=wb.traj, wb_phase=np.where(np.isfinite(wb.phase), wb.phase, 3e38),
-            wb_phase_mod=np.where(np.isfinite(wb.phase_mod), wb.phase_mod, 3e38), wb_freqs=wb.beat_freqs, wb_len=wb.lengths,
-            wb_base_freq=wb.base_beat_freq, wb_rel_range=wb.rel_freq_range, wb_rate=wb._rate, target_height_range=r['h'],
+        self._sim.task_program(**self._task_program() | self._wing_beat_program() | dict(
+            episode_steps=1 << 30, ref_len=1, ref_qpos=dummy, ref_qvel=np.zeros((1, 6), np.float32), target_height_range=r['h'],
             target_speed_range=r['v'], init_x_range=r['x'], init_y_range=r['y'], hover_quat=self._hover_quat, target_zaxis=self._target_zaxis,
             floor_contacts_fatal=1 if self._fatal else 0, **trench))
         self._dev_views = None
@@ -177,19 +155,17 @@ class BatchedVisionFlightEnv(_TaskEnv):
             ids = np.nonzero(resetting)[0]
             self._sim.task_uniform_rows(ids, draws[ids])
 
-    def _after_device_step(self, action, resetting):
+    def _after_device_step(self, resetting):
         tgt = self._rec[:, self._sl['_task_target']]
         self._target_height, self._target_speed = tgt[:, 0].astype(np.float64), tgt[:, 1].astype(np.float64)
 
     def step_device(self, action):
-        """Device-resident control step (see `BatchedFlyEnv.step_device`): `action` a CUDA tensor [n_envs, 12]; returns zero-copy torch
+        """Device-resident control step (see `_TaskEnv.step_device`): `action` a CUDA tensor [n_envs, 12]; returns zero-copy torch
         views (observation rows, out [n_envs, 4] = reward, discount, step_type, 0, eyes uint8 [n_envs, 2, S, S, 3]); nothing is copied to
         the host and the call does not synchronise.  Column slices of the rows: `observation_layout()`."""
-        if not self._device_task:
-            raise RuntimeError('step_device needs device_task=True')
-        self._task_step_device(action)
+        views = super().step_device(action)
         self._sim.render_eyes_async()
-        return self._device_views() + (self.eyes_device(),)
+        return views + (self.eyes_device(),)
 
     def observation_layout(self):
         """{observable name: column slice} of the observation rows `step_device` returns (eyes come as their own tensor)"""
@@ -201,7 +177,7 @@ class BatchedVisionFlightEnv(_TaskEnv):
         return arenas.hfield_height(self._terrain, x, y, self._half)
 
     # -------------------------------------------------------------------------------- episode
-    def _reset_envs(self, ids, hold):
+    def _reset_envs(self, ids, hold=False):
         """initialize_episode_mjcf + initialize_episode (vision_flight.py:97-139): targets, start point, wing-beat phase, a new
         terrain (hills.py:442-473 / 333-392), the fly in its hover pose `target_height` above the terrain at the target speed."""
         m, r = self.model, self._ranges
@@ -228,13 +204,19 @@ class BatchedVisionFlightEnv(_TaskEnv):
             qvel[k, self._root_v] = self._target_speed[e]
             self._wing_qpos[e] = wq[0]
         self._sim.hfield_write(ids, self._terrain[ids])
-        if hold:
-            self._sim.reset_hold(ids, qpos, qvel)
-        else:
-            self._sim.reset(qpos=qpos, qvel=qvel, env_ids=None if n == self.n_envs else ids)
-        self._time[ids] = 0.0
-        self._needs_reset[ids] = False
-        self.n_resets += n
+        self._start_episodes(ids, qpos, qvel, hold)
+
+    def _before_step(self, action, resetting):
+        # before_step (vision_flight.py:141-155): wing-beat pattern at the requested frequency, position target -> force command
+        action[np.isnan(action)] = 0.0
+        wb = self._wbpg
+        target = wb.step(wb.base_beat_freq * (1 + wb.rel_freq_range * action[:, -1]), active=~resetting)
+        action[:, self._action_indices['wings']] += np.where(resetting[:, None], 0.0, target - self._wing_qpos)
+        ctrl = self._host_ctrl(action)
+        return ctrl, ctrl.nbytes
+
+    def _after_read(self, rec):
+        self._wing_qpos = rec[:, self._sl['walker/joints_pos']][:, self._wing_in_obs].astype(np.float64)
 
     def _observation(self, rec):
         sl, N = self._sl, self.n_envs
@@ -253,43 +235,6 @@ class BatchedVisionFlightEnv(_TaskEnv):
             else:
                 obs[name] = rec[:, sl[name]]
         return obs
-
-    def reset(self):
-        N = self.n_envs
-        if self._device_task:
-            return self._device_reset()
-        self._reset_envs(np.arange(N), hold=False)
-        self._sim.task_inputs(np.zeros(N, np.int32), np.ones(N, np.uint8))
-        obs = self._observation(self._sim.read_task_obs(self._rec))
-        return self._unbatch(TimeStep(np.full(N, StepType.FIRST), np.zeros(N), np.ones(N), obs), first=True)
-
-    def step(self, action):
-        m, N = self.model, self.n_envs
-        if self._device_task:
-            a = np.asarray(action, np.float32).reshape(N, -1)
-            assert a.shape[1] == self._action_spec.shape[0], f'action must have {self._action_spec.shape[0]} entries'
-            return self._unbatch(self._device_step(a))
-        action = np.array(action, np.float64, copy=True).reshape(N, -1)
-        assert action.shape[1] == self._action_spec.shape[0], f'action must have {self._action_spec.shape[0]} entries'
-        resetting = self._needs_reset.copy()
-        if resetting.any():
-            self._reset_envs(np.nonzero(resetting)[0], hold=True)
-        # before_step (vision_flight.py:141-155): wing-beat pattern at the requested frequency, position target -> force command
-        action[np.isnan(action)] = 0.0
-        wb = self._wbpg
-        target = wb.step(wb.base_beat_freq * (1 + wb.rel_freq_range * action[:, -1]), active=~resetting)
-        action[:, self._action_indices['wings']] += np.where(resetting[:, None], 0.0, target - self._wing_qpos)
-        ctrl = np.zeros((N, m.nu), np.float32)
-        ctrl[:, self._ctrl_of_action] = action[:, :len(self._ctrl_of_action)]
-        self._sim.set_control(ctrl)
-        self._sim.task_inputs(np.zeros(N, np.int32), resetting)
-        self._sim.step(self._n_sub)
-        rec = self._sim.read_task_obs(self._rec)
-        self._time = np.where(resetting, 0.0, self._time + self._control_timestep)
-        self._wing_qpos = rec[:, self._sl['walker/joints_pos']][:, self._wing_in_obs].astype(np.float64)
-        obs = self._observation(rec)
-        step_type, reward, discount, self._needs_reset = self._task_after(rec, obs, resetting, self._time, None)
-        return self._unbatch(TimeStep(step_type, reward, discount, obs))
 
     def _task_after(self, rec, obs, resetting, time, ghost):
         """get_reward (vision_flight.py:157-233), check_termination (a bad state, base.py:222-225, or a fatal floor contact), get_discount;
