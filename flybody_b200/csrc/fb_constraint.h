@@ -613,11 +613,12 @@ FB_DEV void kcon_p3(FB_CON_ARGS) {
   int ncon = AT(d.ncon, 0);
   int n = sh.base; for (int yy = 0; yy < y; yy++) n += sh.cnt[yy];
   int c0 = y * ncon / FB_ROWPAR, c1 = (y + 1) * ncon / FB_ROWPAR;
+  const float* fric = PRM(FB_P_GEOM_FRICTION, m.geom_friction);
   for (int ci = c0; ci < c1; ci++) {
     float includemargin; bool incl; int dim = contact_dim(m, d, e, ci, includemargin, incl);
     int g1 = AT(d.con_geom1, ci), g2 = AT(d.con_geom2, ci);
     float dist = AT(d.con_dist, ci);
-    float fr0 = fmaxf(m.geom_friction[3 * g1], m.geom_friction[3 * g2]);
+    float fr0 = fmaxf(fric[3 * g1], fric[3 * g2]);
     AT(d.con_dim, ci) = dim; AT(d.con_mu, ci) = fr0 * sqrtf(1.0f / m.impratio);
     CON_F(d.con_fric, ci, 0, 2) = fr0; CON_F(d.con_fric, ci, 1, 2) = fr0;
     AT(d.con_efcadr, ci) = -1;
@@ -793,6 +794,7 @@ FB_DEV void kref(FB_PHASE_ARGS) {
 FB_DEV void kact_p0(FB_PHASE_ARGS) {
   tsolve_stage_issue(m, d, sh, e, y, d.qLD); for (int k = y; k < m.nv; k += FB_NY) AT(d.qfrc_actuator, k) = 0; }
 FB_DEV void kact_p1(FB_PHASE_ARGS) {
+  const float *gain = PRM(FB_P_ACTUATOR_GAINPRM, m.actuator_gainprm), *bias = PRM(FB_P_ACTUATOR_BIASPRM, m.actuator_biasprm);
   for (int i = y; i < m.nu; i += FB_NY) {
     float ctrl = AT(d.ctrl, i);
     if (MLD(m.actuator_ctrllimited[i])) ctrl = clampf(ctrl, MLD(m.actuator_ctrlrange[2 * i]), MLD(m.actuator_ctrlrange[2 * i + 1]));
@@ -804,8 +806,8 @@ FB_DEV void kact_p1(FB_PHASE_ARGS) {
     }
     float input = ctrl; int aa = MLD(m.actuator_actadr[i]);
     if (aa >= 0) { AT(d.act_dot, aa) = (ctrl - AT(d.act, aa)) / fmaxf(FB_MINVAL, MLD(m.actuator_dynprm[3 * i])); input = AT(d.act, aa); }
-    float force = MLD(m.actuator_gainprm[3 * i]) * input;
-    if (MLD(m.actuator_biastype[i]) == 1) force += MLD(m.actuator_biasprm[3 * i]) + MLD(m.actuator_biasprm[3 * i + 1]) * len + MLD(m.actuator_biasprm[3 * i + 2]) * vel;
+    float force = MLD(gain[3 * i]) * input;
+    if (MLD(m.actuator_biastype[i]) == 1) force += MLD(bias[3 * i]) + MLD(bias[3 * i + 1]) * len + MLD(bias[3 * i + 2]) * vel;
     if (MLD(m.actuator_forcelimited[i])) force = clampf(force, MLD(m.actuator_forcerange[2 * i]), MLD(m.actuator_forcerange[2 * i + 1]));
     AT(d.actuator_force, i) = force;
     // joint / tendon transmissions touch disjoint dofs (one actuator per joint or tendon in the fly model)

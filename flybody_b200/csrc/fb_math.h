@@ -58,6 +58,11 @@ FB_DEV float clampf(float x, float lo, float hi) { return x < lo ? lo : (x > hi 
 // record accessor: slot i of array `arr` of env e (arr = record base + array offset).  32-bit index
 // arithmetic: rec * Np stays below 2^32 (checked in fb_create).
 #define AT(arr, i) (arr)[(unsigned)e * d.rec + (unsigned)(i)]
+// model parameter p (enum FbParam) of env e: its row of the overlay when the handle has one (fb_param_*), else the compiled table.
+// One test, uniform over the launch; the element index is the table's.
+#define PRM(p, table) (d.prm ? (const float*)d.prm + (unsigned)e * d.prm_stride + (unsigned)d.prm_off[p] : (table))
+// ... a scalar one (mjModel.opt), `val` the compiled value
+#define PRMS(p, k, val) (d.prm ? d.prm[(unsigned)e * d.prm_stride + (unsigned)d.prm_off[p] + (k)] : (val))
 
 // Record arrays of 3-vectors, quaternions, 3x3 matrices, spatial 6-vectors and 10-parameter inertias are PADDED to multiples of
 // four floats (V3 -> 4, M3 -> 12, S6 -> 2 x 4, I10 -> 12) and start on 16-byte boundaries (alloc_data), so that every element is

@@ -19,6 +19,29 @@ FB_DEV unsigned tk_mix(unsigned x) { x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 1
 FB_DEV float tk_u01(const DevTask& t, int e, int episode, int k) {
   return (float)(tk_mix(t.seed ^ tk_mix((unsigned)e * 0x9e3779b9u + (unsigned)episode * 0x85ebca6bu + (unsigned)k * 0xc2b2ae35u)) >> 8) * (1.0f / 16777216.0f);
 }
+// Model-parameter draws of a resetting env (fb_param_draws), the same device functions for fb_reset / fb_reset_hold and the device
+// task's resets.  u is a counter hash of (seed, env, the env's draw count, parameter, element) in an index space of its own (an extra
+// seed word); every lane reads the draw count, which kprm_count advances in a later phase.
+FB_DEV float prm_u01(unsigned seed, int e, unsigned count, int p, int i) {
+  return (float)(tk_mix(seed ^ 0x5bd1e995u ^ tk_mix((unsigned)e * 0x9e3779b9u + count * 0x85ebca6bu + ((unsigned)p << 24 | (unsigned)i) * 0xc2b2ae35u)) >> 8) *
+         (1.0f / 16777216.0f);
+}
+FB_DEV void kprm_draw(const DevModel& m, const DevData& d, int e, int y) {
+  if (!d.prm_draw) return;
+  const DevPrmDraw& g = *d.prm_draw;
+  const unsigned count = d.prm_count[e];
+  float* row = d.prm + (size_t)e * d.prm_stride;
+  for (int p = 0; p < FB_NPARAMS; p++) {
+    if (!g.on[p]) continue;
+    for (int i = y; i < g.n[p]; i += FB_NY) {
+      const int s = d.prm_off[p] + (p == FB_P_BODY_INERTIA ? i + i / 3 : i);      // (body_inertia: four slots per body)
+      const float lo = g.lo[s], hi = g.hi[s], u = prm_u01(g.seed, e, count, p, g.shared[p] ? 0 : i);
+      row[s] = fminf(fmaxf(lo + u * (hi - lo), lo), hi);
+      if (p == FB_P_DOF_DAMPING) row[d.prm_mdamp + m.dof_Madr[i]] = row[s];      // the diagonal of the implicit damping
+    }
+  }
+}
+FB_DEV void kprm_count(const DevData& d, int e, int y) { if (d.prm_draw && y == 0) d.prm_count[e]++; }
 FB_DEV int wb_nearest(const DevTask& t, float f) {          // np.abs(beat_freqs - f).argmin(): first minimum
   int best = 0; float bd = fabsf(t.wb_freqs[0] - f);
   for (int i = 1; i < t.n_freq; i++) { float dd = fabsf(t.wb_freqs[i] - f); if (dd < bd) { bd = dd; best = i; } }
@@ -125,11 +148,13 @@ FB_DEV void ktask_reset(const DevModel& m, const DevData& d, int e, int y) {
   for (int i = y; i < m.na; i += FB_NY) AT(d.act, i) = 0.0f;
   for (int i = y; i < m.nu; i += FB_NY) AT(d.ctrl, i) = 0.0f;      // physics.reset() = mj_resetData: the FIRST observation does not see the old controls
   zero_applied(m, d, e, y);
+  kprm_draw(m, d, e, y);
 }
 FB_DEV void ktask_reset2(const DevModel& m, const DevData& d, int e, int y) {      // after the template copy (other lanes wrote it)
   if (!d.task || e >= d.N) return;
   const DevTask& t = *d.task;
   if (!t.needs_reset[e]) return;
+  kprm_count(d, e, y);                     // (every lane read the draw count in ktask_reset)
   const int episode = t.episode[e];
   if (t.kind == FB_TASK_VISION) { ktask_reset_vision(m, d, t, e, y, episode); return; }
   if (t.kind == FB_TASK_TEMPLATE || t.kind == FB_TASK_BALL) {          // the template pose as copied, at rest (no reference, no ghost)

@@ -101,8 +101,8 @@ FB_DEV void body_derived(const DevModel& m, const DevData& d, int e, int b, floa
   V3 ipos = pos + mul(R, mld3(m.body_ipos, b));
   M3 iR = q2m(qmul(quat, mld4(m.body_iquat, b)));
   st3(d.xipos, b, d, e, ipos); st9(d.ximat, b, d, e, iR);
-  float mass = m.body_mass[b];
-  V3 di = mld3(m.body_inertia, b);
+  float mass = PRM(FB_P_BODY_MASS, m.body_mass)[b];
+  V3 di = mld3(PRM(FB_P_BODY_INERTIA, m.body_inertia), b);
   float Ic[6];   // xx yy zz xy xz yz of R diag(di) R^T
   Ic[0] = iR.m[0] * iR.m[0] * di.x + iR.m[1] * iR.m[1] * di.y + iR.m[2] * iR.m[2] * di.z;
   Ic[1] = iR.m[3] * iR.m[3] * di.x + iR.m[4] * iR.m[4] * di.y + iR.m[5] * iR.m[5] * di.z;
@@ -209,6 +209,7 @@ FB_DEV void mass_row(const DevModel& m, const DevData& d, int e, float* ldsh, in
   V3 L, p;
   inert_mul(I, ld3(d.Sang, i, d, e), ld3(d.Slin, i, d, e), L, p);
   const int adr = m.dof_Madr[i], len = m.dof_chainlen[i];
+  const float* arm = PRM(FB_P_DOF_ARMATURE, m.dof_armature);
   int t = 0;
   for (; t + 4 <= len; t += 4) {       // four ancestors at a time: their motion-axis loads are in flight together (a store to qM between
     // two loads would otherwise order them: the compiler cannot rule out that the arrays overlap)
@@ -216,14 +217,14 @@ FB_DEV void mass_row(const DevModel& m, const DevData& d, int e, float* ldsh, in
     const V3 a0 = ld3(d.Sang, j0, d, e), l0 = ld3(d.Slin, j0, d, e), a1 = ld3(d.Sang, j1, d, e), l1 = ld3(d.Slin, j1, d, e);
     const V3 a2 = ld3(d.Sang, j2, d, e), l2 = ld3(d.Slin, j2, d, e), a3 = ld3(d.Sang, j3, d, e), l3 = ld3(d.Slin, j3, d, e);
     float v0 = dot(a0, L) + dot(l0, p), v1 = dot(a1, L) + dot(l1, p), v2 = dot(a2, L) + dot(l2, p), v3_ = dot(a3, L) + dot(l3, p);
-    if (t == 0) v0 += m.dof_armature[i];
+    if (t == 0) v0 += arm[i];
     AT(d.qM, adr + t) = v0; LS(adr + t) = v0; AT(d.qM, adr + t + 1) = v1; LS(adr + t + 1) = v1;
     AT(d.qM, adr + t + 2) = v2; LS(adr + t + 2) = v2; AT(d.qM, adr + t + 3) = v3_; LS(adr + t + 3) = v3_;
   }
   for (; t < len; t++) {
     const int j = m.dof_anc[adr + t];
     float v = dot(ld3(d.Sang, j, d, e), L) + dot(ld3(d.Slin, j, d, e), p);
-    if (t == 0) v += m.dof_armature[i];
+    if (t == 0) v += arm[i];
     AT(d.qM, adr + t) = v; LS(adr + t) = v;
   }
 }
@@ -238,10 +239,12 @@ FB_DEV void ld_writeout(const DevModel& m, const DevData& d, ShTree& sh, int e, 
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF; (void)part_;
   for (int k = y; k < m.nM; k += FB_NY) AT(dst, k) = LS(k);
 }
-// re-initialise the shared rows with M + h*diag(damping) for the second factorisation (Euler with implicit damping)
+// re-initialise the shared rows with M + h*diag(damping) for the second factorisation (Euler with implicit damping); with a parameter
+// overlay the env's own M_damp, which follows its dof_damping (fb_param_set, kprm_draw)
 FB_DEV void ld_reinit_damped(const DevModel& m, const DevData& d, ShTree& sh, int e, int y) {
   float* part_ = sh_dyn(sh); float* ldsh = part_ + FB_PARTF; (void)part_;
-  for (int k = y; k < m.nM; k += FB_NY) LS(k) = AT(d.qM, k) + m.timestep * m.M_damp[k];
+  const float* md = d.prm ? (const float*)d.prm + (unsigned)e * d.prm_stride + (unsigned)d.prm_mdamp : m.M_damp;
+  for (int k = y; k < m.nM; k += FB_NY) LS(k) = AT(d.qM, k) + m.timestep * md[k];
 }
 
 // sparse L^T D L factorisation (Featherstone; MuJoCo mj_factorM).  Row k of LD holds (k,k), (k,parent(k)), ...
@@ -570,17 +573,21 @@ FB_DEV S6 body_inertial_force(const DevModel& m, const DevData& d, int e, int b,
   return f;
 }
 FB_DEV float pow4(float x) { float y = x * x; return y * y; }
-// fluid wrench on body b about ref (inertia-box model, or ellipsoid model for flagged bodies)
-FB_DEV S6 body_fluid_wrench(const DevModel& m, const DevData& d, int e, int b) {
+// fluid wrench on body b about ref (inertia-box model, or ellipsoid model for flagged bodies).  OVL: density, viscosity, wind, mass
+// and inertia of the env's overlay row.  The velocity kernel runs at its register limit, so the overlay gets a kernel instance of its
+// own (launch_step1) instead of a test in this one: the instance without it is the code of a handle that never set parameters.
+template <bool OVL> FB_DEV S6 body_fluid_wrench(const DevModel& m, const DevData& d, int e, int b) {
   S6 out; out.a = v3(0, 0, 0); out.l = v3(0, 0, 0);
-  float rho = m.density, eta = m.viscosity;
-  float mass = m.body_mass[b];
+  const float* prm = d.prm + (unsigned)e * d.prm_stride;
+  float rho = OVL ? prm[d.prm_off[FB_P_DENSITY]] : m.density, eta = OVL ? prm[d.prm_off[FB_P_VISCOSITY]] : m.viscosity;
+  float mass = OVL ? prm[d.prm_off[FB_P_BODY_MASS] + b] : m.body_mass[b];
   if ((rho <= 0 && eta <= 0) || mass < FB_MINVAL) return out;
   S6 bv = ld6(d.bvel, b, d, e);
-  V3 wind = v3(m.wind[0], m.wind[1], m.wind[2]);
+  const float* wp = prm + d.prm_off[FB_P_WIND];
+  V3 wind = OVL ? v3(wp[0], wp[1], wp[2]) : v3(m.wind[0], m.wind[1], m.wind[2]);
   const float PI = 3.14159265358979f;
   if (!m.body_fluid_ellipsoid[b]) {
-    V3 I = mld3(m.body_inertia, b);
+    V3 I = mld3(OVL ? prm + d.prm_off[FB_P_BODY_INERTIA] : m.body_inertia, b);
     float bx = sqrtf(fmaxf(FB_MINVAL, I.y + I.z - I.x) / mass * 6.0f);
     float by = sqrtf(fmaxf(FB_MINVAL, I.x + I.z - I.y) / mass * 6.0f);
     float bz = sqrtf(fmaxf(FB_MINVAL, I.x + I.y - I.z) / mass * 6.0f);
@@ -694,7 +701,7 @@ FB_DEV void kvel_p0(FB_PHASE_ARGS) {
   if (y != 0) return;
   S6 z; z.a = v3(0, 0, 0); z.l = v3(0, 0, 0);
   st6(d.bvel, 0, d, e, z);
-  S6 g = z; g.l = v3(-m.gravity[0], -m.gravity[1], -m.gravity[2]);
+  S6 g = z; g.l = v3(-PRMS(FB_P_GRAVITY, 0, m.gravity[0]), -PRMS(FB_P_GRAVITY, 1, m.gravity[1]), -PRMS(FB_P_GRAVITY, 2, m.gravity[2]));
   st6(d.bacc, 0, d, e, g);
   for (int r = 0; r < m.nroot; r++) { S6 v = z, a = g; vel_acc_from_parent(m, d, e, m.root_body[r], v, a); }
 }
@@ -711,10 +718,10 @@ FB_DEV void kvel_p1(FB_PHASE_ARGS) {
 // (Subtree sums of the velocity stage stay in the record: moving them to shared memory as in the position kernel costs 3.3 KB more
 // shared memory per warp, which shrinks the L1 the scattered record loads live in.)
 // all lanes over bodies: bias force (kept un-accumulated in bfrc0 for the sensor pass) and fluid wrench
-FB_DEV void kvel_p1b(FB_PHASE_ARGS) {
+template <bool OVL> FB_DEV void kvel_p1b(FB_PHASE_ARGS) {
   for (int b = y; b < m.nbody; b += FB_NY) {
     S6 f; f.a = f.l = v3(0, 0, 0); S6 fl = f;
-    if (b > 0) { f = body_inertial_force(m, d, e, b, d.bvel, d.bacc); fl = body_fluid_wrench(m, d, e, b); }
+    if (b > 0) { f = body_inertial_force(m, d, e, b, d.bvel, d.bacc); fl = body_fluid_wrench<OVL>(m, d, e, b); }
     st6(d.bfrc, b, d, e, f); st6(d.bfrc0, b, d, e, f); st6(d.bfl, b, d, e, fl);
   }
 }
@@ -751,14 +758,15 @@ FB_DEV void kvel_p3(FB_PHASE_ARGS) {
 }
 // all lanes over dofs: qfrc_bias = S . f_subtree ; qfrc_passive = S . fluid_subtree + springs + dampers
 FB_DEV void kvel_p3b(FB_PHASE_ARGS) {
+  const float *damp = PRM(FB_P_DOF_DAMPING, m.dof_damping), *stiff = PRM(FB_P_JNT_STIFFNESS, m.jnt_stiffness);
   for (int k = y; k < m.nv; k += FB_NY) {
     int b = m.dof_bodyid[k];
     V3 Sa = ld3(d.Sang, k, d, e), Sl = ld3(d.Slin, k, d, e);
     S6 f = ld6(d.bfrc, b, d, e), fl = ld6(d.bfl, b, d, e);
     AT(d.qfrc_bias, k) = dot(Sa, f.a) + dot(Sl, f.l);
-    float pas = dot(Sa, fl.a) + dot(Sl, fl.l) - m.dof_damping[k] * AT(d.qvel, k);
+    float pas = dot(Sa, fl.a) + dot(Sl, fl.l) - damp[k] * AT(d.qvel, k);
     int j = m.dof_jntid[k];
-    if (m.jnt_type[j] == FB_JNT_HINGE) { int qa = m.jnt_qposadr[j]; pas -= m.jnt_stiffness[j] * (AT(d.qpos, qa) - m.qpos_spring[qa]); }
+    if (m.jnt_type[j] == FB_JNT_HINGE) { int qa = m.jnt_qposadr[j]; pas -= stiff[j] * (AT(d.qpos, qa) - m.qpos_spring[qa]); }
     AT(d.qfrc_passive, k) = pas;
   }
 }

@@ -159,6 +159,17 @@ struct DevData {
   // body's CoM), allocated together on first use (fb_applied_ptrs / fb_set / fb_write_state); nullptr until then and after
   // fb_clear_applied, so a step that never set them runs without the term
   float *qfrc_applied, *xfrc_applied;
+  // model-parameter overlay (fb_param_*): compact [Np][prm_stride], parameter p (enum FbParam) of an env at prm_off[p] of its row,
+  // body_inertia padded to four floats per body as the model table; nullptr until first use and after fb_param_clear, so a step that
+  // never set parameters reads the compiled tables.  prm_mdamp: the row's derived M_damp [nM] (DevModel::M_damp of the env's dof_damping).
+  // prm_count: the env's draws so far; prm_draw: the draw program of resets, or nullptr
+  float* prm; unsigned prm_stride; int prm_off[FB_NPARAMS], prm_mdamp; unsigned* prm_count; const struct DevPrmDraw* prm_draw;
+};
+// draw program of the overlay (fb_param_draws): parameter p with on[p] takes lo + u (hi - lo) at each reset, u one draw per element
+// (or one for all of them: shared[p]); n[p] values per env; lo, hi are laid out as an overlay row
+struct DevPrmDraw {
+  unsigned seed; int on[FB_NPARAMS], shared[FB_NPARAMS], n[FB_NPARAMS];
+  const float *lo, *hi;
 };
 
 // Device-side task logic (fb_task_program): what the reference's task hooks do around the physics step -- auto-reset,

@@ -40,6 +40,9 @@ struct FbSim {
   std::vector<void*> allocs;
   std::vector<void*> obs_scope, task_scope;   // device buffers of the current observation / task program: freed when the program is replaced
   std::vector<void*> applied_scope;           // qfrc_applied / xfrc_applied: freed by fb_clear_applied
+  std::vector<void*> prm_scope;               // parameter overlay, draw counters and draw program (fb_param_*): freed by fb_param_clear
+  std::vector<float> h_prm0; int prm_n[FB_NPARAMS];   // the overlay row of the compiled model; values per env of each parameter
+  DevPrmDraw prm_draw_host; DevPrmDraw* prm_draw_dev; std::vector<float> h_prm_lo, h_prm_hi;   // the draw program and its ranges (row layout)
   std::vector<void*> ref_scope, bank_scope;   // reference slots (fb_ref_slots) / terrain bank (fb_hfield_bank): freed when replaced
   std::vector<int> h_dof_parent, h_dof_Madr, h_body_parent;
   std::vector<int> h_jnt_type, h_jnt_qadr, h_jnt_dofadr, h_jnt_body, h_site_body;   // joint / site tables an IK program is checked and built against
@@ -297,6 +300,8 @@ template <typename K> static void warp_launch(FbSim* s, const char* kernel, int 
 
 // per-env kernels wrapped as single-phase functions
 FB_DEV void ph_reset_scatter(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kreset_scatter(m, d, e, y); }
+FB_DEV void ph_reset_draw(const DevModel& m, const DevData& d, ShNone&, int w, int y) { if (w < d.rst_n) kprm_draw(m, d, d.rst_ids[w], y); }
+FB_DEV void ph_reset_count(const DevModel&, const DevData& d, ShNone&, int w, int y) { if (w < d.rst_n) kprm_count(d, d.rst_ids[w], y); }
 FB_DEV void ph_scatter(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kscatter(m, d, e, y); }
 FB_DEV void ph_clear_hold(const DevModel& m, const DevData& d, ShNone&, int e, int y) { kclear_hold(m, d, e, y); }
 FB_DEV void ph_task_reset(const DevModel& m, const DevData& d, ShNone&, int e, int y) { ktask_reset(m, d, e, y); }
@@ -327,7 +332,8 @@ FB_DEV void ph_smooth_out(FB_PHASE_ARGS) {
 #define FB_ST_POS Ph<kpos_p0>, Ph<kpos_p1>, Ph<kpos_p1b>, Ph<kpos_p2>, Ph<kpos_p3>, Ph<kpos_p3b>, Ph<kpos_p4>, Wf<kpos_factor>, Ph<kpos_p6w>, Ph<kpos_p6d>, Wf<kpos_factor>, Ph<kpos_p9>
 #define FB_ST_COL Ph<kcol_stage>, Wf<kcol_broad>, Ph<kcol_narrow>, Wf<kcol_mpr>, Ph<kcol_compact>
 #define FB_ST_PROJ Ph<kcon_p0>, Ph<kcon_p1>, Ph<kcon_p2>, Ph<kcon_p3>, Ph<kproj_p0>, Ph<kproj_p1>
-#define FB_ST_VEL Ph<kvel_p0>, Ph<kvel_p1>, Ph<kvel_p1b>, Ph<kvel_p2>, Ph<kvel_p3>, Ph<kvel_p3b>, Ph<kvel_p4>
+#define FB_ST_VEL Ph<kvel_p0>, Ph<kvel_p1>, Ph<kvel_p1b<false>>, Ph<kvel_p2>, Ph<kvel_p3>, Ph<kvel_p3b>, Ph<kvel_p4>
+#define FB_ST_VEL_PRM Ph<kvel_p0>, Ph<kvel_p1>, Ph<kvel_p1b<true>>, Ph<kvel_p2>, Ph<kvel_p3>, Ph<kvel_p3b>, Ph<kvel_p4>    // with a parameter overlay
 #define FB_ST_SMOOTH Ph<kact_p0>, Ph<kact_p1>, Ph<kact_p2>, Ph<kact_p2b>, Ph<kact_p3>, Wf<wf_smooth_solve>, Ph<ph_smooth_out>, Ph<kref>
 #define FB_ST_FINISH Ph<kfin_f1>, Wf<kfin_solve>, Ph<kfin_f5>, Ph<kfin_f6>, Ph<kfin_f7>, Wf<kfin_solve_euler>, Ph<kfin_f8>, Ph<kfin_f9>, Ph<kfin_f10>
 static size_t dyn_pos(const DevModel& m) { return (size_t)FB_PARTF + std::max((size_t)m.nM, (size_t)10 * m.nbody); }   // LS region: inertia matrix rows, before that the composite inertias (CRBS)
@@ -376,7 +382,7 @@ static void fb_launch_ids(FbSim* s, int, size_t dyn_floats, const int* ids, int 
   fb_run_ids<Sh, St...><<<n, dim3(32, 1), bytes, s->stream>>>(s->m, s->d, (int)slice, ids);
   s->launches++;
 }
-static const void* step_kernel_fn(int kind) {
+static const void* step_kernel_fn(int kind, bool prm) {
   switch (kind) {
     case K_SMOOTH: return (const void*)fb_run<ShTree, FB_ST_SMOOTH>;
     case K_SOLVE: return (const void*)fb_run_solve;
@@ -384,14 +390,14 @@ static const void* step_kernel_fn(int kind) {
     case K_POS: return (const void*)fb_run<ShTree, FB_ST_POS>;
     case K_COL: return (const void*)fb_run<ShCol, FB_ST_COL>;
     case K_PROJ: return (const void*)fb_run<ShCon, FB_ST_PROJ>;
-    case K_VEL: return (const void*)fb_run<ShTree, FB_ST_VEL>;
+    case K_VEL: return prm ? (const void*)fb_run<ShTree, FB_ST_VEL_PRM> : (const void*)fb_run<ShTree, FB_ST_VEL>;
     default: return nullptr;
   }
 }
 // the occupancy query of fb_step_kernel_smem (0 under emulation)
 static int step_kernel_blocks_per_sm(FbSim* s, int kind, size_t bytes, int* blocks) {
   FB_CUDA_OK(cudaSetDevice(s->device));
-  FB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks, step_kernel_fn(kind), 32 * FB_WPB, bytes));
+  FB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks, step_kernel_fn(kind, s->d.prm != nullptr), 32 * FB_WPB, bytes));
   return 0;
 }
 #else
@@ -411,14 +417,16 @@ static void launch_step1(FbSim* s) {
   fb_launch<ShCol, FB_ST_COL>(s, K_COL, dyn_col(s->m));
   if (s->hf_on) launch_hfield(s, nullptr, s->d.N);     // heightfield contacts join the contact list before the constraint rows are built
   fb_launch<ShCon, FB_ST_PROJ>(s, K_PROJ, dyn_proj(s->m));
-  fb_launch<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m));
+  if (s->d.prm) fb_launch<ShTree, FB_ST_VEL_PRM>(s, K_VEL, dyn_vel(s->m));
+  else fb_launch<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m));
 }
 static void launch_step1_ids(FbSim* s, const int* ids, int n) {      // ids: a device list
   fb_launch_ids<ShTree, FB_ST_POS>(s, K_POS, dyn_pos(s->m), ids, n);
   fb_launch_ids<ShCol, FB_ST_COL>(s, K_COL, dyn_col(s->m), ids, n);
   if (s->hf_on) launch_hfield(s, ids, n);
   fb_launch_ids<ShCon, FB_ST_PROJ>(s, K_PROJ, dyn_proj(s->m), ids, n);
-  fb_launch_ids<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m), ids, n);
+  if (s->d.prm) fb_launch_ids<ShTree, FB_ST_VEL_PRM>(s, K_VEL, dyn_vel(s->m), ids, n);
+  else fb_launch_ids<ShTree, FB_ST_VEL>(s, K_VEL, dyn_vel(s->m), ids, n);
 }
 static void launch_step2(FbSim* s, bool integrate) {
   s->d.do_integrate = integrate ? 1 : 0;     // read by the solve (warm-start bookkeeping) and the finish kernel
@@ -756,8 +764,8 @@ static int ensure_stage(FbSim* s, size_t floats, size_t ints) {
   return 0;
 }
 
-// The state bank's rows follow the handle's arrays: whatever replaces an observation / task program, the reference slots or the
-// applied-force arrays drops the bank (the stream is idle: the callers synchronise first); fb_state_bank lays it out again.
+// The state bank's rows follow the handle's arrays: whatever replaces an observation / task program, the reference slots, the
+// applied-force arrays or the parameter overlay drops the bank (the stream is idle: the callers synchronise first); fb_state_bank lays it out again.
 static void state_drop(FbSim* s) {
   if (!s->st_bank) return;
   scope_free(s, s->st_scope);
@@ -779,6 +787,57 @@ static int ensure_applied(FbSim* s) {
   s->d.qfrc_applied = q; s->d.xfrc_applied = x;      // the step graph is captured again: DevData changed
   return 0;
 }
+// model-parameter overlay (fb_param_*): a row of every FbParam field in enum order, each segment on a 16-byte boundary; body_inertia
+// takes four slots per body, as the model table the kernels read with 128-bit loads.  Last the env's M_damp [nM], derived from its
+// dof_damping (the diagonal at dof_Madr), so that the damped factorisation reads it exactly as the compiled table
+static int prm_slot(int p, int i) { return p == FB_P_BODY_INERTIA ? i + i / 3 : i; }
+static void prm_layout(FbSim* s, const FbModel* h) {
+  const int nb = h->nbody, nv = h->nv, nj = h->njnt, ng = h->ngeom, nu = h->nu;
+  const int n[FB_NPARAMS] = {nb, 3 * nb, nv, nv, nj, 3 * ng, 3 * nu, 3 * nu, 3, 3, 1, 1};
+  const double* src[FB_NPARAMS] = {h->body_mass, h->body_inertia, h->dof_armature, h->dof_damping, h->jnt_stiffness, h->geom_friction,
+                                   h->actuator_gainprm, h->actuator_biasprm, h->opt_gravity, h->opt_wind, &h->opt_density, &h->opt_viscosity};
+  unsigned off = 0;
+  for (int p = 0; p < FB_NPARAMS; p++) {
+    s->prm_n[p] = n[p]; s->d.prm_off[p] = (int)off;
+    off += ((unsigned)(p == FB_P_BODY_INERTIA ? 4 * nb : n[p]) + 3) & ~3u;
+  }
+  s->d.prm_mdamp = (int)off; off += ((unsigned)h->nM + 3) & ~3u;
+  s->d.prm_stride = off;
+  s->h_prm0.assign(off, 0.0f);
+  for (int p = 0; p < FB_NPARAMS; p++) for (int i = 0; i < n[p]; i++) s->h_prm0[s->d.prm_off[p] + prm_slot(p, i)] = (float)src[p][i];
+  for (int i = 0; i < nv; i++) s->h_prm0[s->d.prm_mdamp + h->dof_Madr[i]] = (float)h->dof_damping[i];
+}
+static int ensure_prm(FbSim* s) {
+  if (s->d.prm) return 0;
+  if (sync_stream(s) != 0) return -2;
+  state_drop(s);
+  const size_t Np = s->d.Np, P = s->d.prm_stride;
+  float *p, *lo, *hi; unsigned* cnt; DevPrmDraw* g;
+  if (int rc = scope_alloc(s, s->prm_scope, "out of device memory (model parameters)", [&] {
+        p = dalloc<float>(s, Np * P); cnt = dalloc<unsigned>(s, Np); lo = dalloc<float>(s, P); hi = dalloc<float>(s, P);
+        g = (DevPrmDraw*)dalloc<unsigned char>(s, sizeof(DevPrmDraw)); }))
+    return rc;
+  std::vector<float> rows(Np * P);
+  for (size_t e = 0; e < Np; e++) std::copy(s->h_prm0.begin(), s->h_prm0.end(), rows.begin() + e * P);
+  if (copy_sync(s, p, rows.data(), sizeof(float) * rows.size()) != 0) return -2;
+  s->prm_draw_host = DevPrmDraw{}; s->prm_draw_host.lo = lo; s->prm_draw_host.hi = hi;
+  for (int k = 0; k < FB_NPARAMS; k++) s->prm_draw_host.n[k] = s->prm_n[k];
+  s->prm_draw_dev = g; s->h_prm_lo = s->h_prm0; s->h_prm_hi = s->h_prm0;
+  s->d.prm = p; s->d.prm_count = cnt; s->d.prm_draw = nullptr;      // (the counters start at 0; the step graph is captured again)
+  return 0;
+}
+// values from outside, `rows` rows of the parameter: finite, non-negative where MuJoCo's field is, no stiffness on a joint without a spring
+static bool prm_valid(FbSim* s, const char* who, int p, const float* v, size_t rows) {
+  const bool nonneg = p != FB_P_ACTUATOR_GAINPRM && p != FB_P_ACTUATOR_BIASPRM && p != FB_P_GRAVITY && p != FB_P_WIND;
+  const size_t k = (size_t)s->prm_n[p];
+  for (size_t i = 0; i < rows * k; i++) {
+    if (!std::isfinite(v[i])) { s->err = std::string(who) + ": non-finite value"; return false; }
+    if (nonneg && v[i] < 0) { s->err = std::string(who) + ": negative value (mass, inertia, armature, damping, stiffness, friction, density and viscosity are >= 0)"; return false; }
+    if (p == FB_P_JNT_STIFFNESS && v[i] != 0 && s->h_jnt_type[i % k] != FB_JNT_HINGE) {
+      s->err = std::string(who) + ": joint " + std::to_string(i % k) + " is not a hinge: its stiffness must stay 0 (the step has springs on hinge joints only)"; return false; }
+  }
+  return true;
+}
 
 extern "C" {
 
@@ -794,6 +853,7 @@ int fb_create(const FbModel* hm, int n_envs, int device, FbHandle* out) {
   if (dev_open(s, n_envs) != 0) { delete s; return -2; }
   int rc = build_model(s, hm);             // (every upload and allocation has completed when it returns)
   if (rc == 0) rc = alloc_data(s, n_envs);
+  if (rc == 0) prm_layout(s, hm);
   *out = s;
   if (rc != 0) return rc;
   std::vector<float> q0((size_t)n_envs * hm->nq);
@@ -1117,6 +1177,79 @@ int fb_clear_applied(FbHandle s) {
   return 0;
 }
 
+int fb_param_size(FbHandle s, int p) { return (!s || p < 0 || p >= FB_NPARAMS) ? -1 : s->prm_n[p]; }
+int fb_param_set(FbHandle s, int p, const int32_t* env_ids, int n, const float* vals, int) {
+  if (!s) return -1;
+  if (p < 0 || p >= FB_NPARAMS) { s->err = "fb_param_set: unknown parameter"; return -1; }
+  if (!vals) { s->err = "fb_param_set: vals is NULL"; return -1; }
+  const int N = s->d.N;
+  if (!env_ids && n != N) { s->err = "fb_param_set: without env_ids, n must be n_envs"; return -1; }
+  if (env_ids && n < 1) { s->err = "fb_param_set: n >= 1 envs"; return -1; }
+  for (int k = 0; env_ids && k < n; k++) if (env_ids[k] < 0 || env_ids[k] >= N) { s->err = "fb_param_set: env id out of range"; return -1; }
+  const size_t K = (size_t)s->prm_n[p];
+  std::vector<float> v((size_t)n * K);
+  if (copy_sync(s, v.data(), vals, sizeof(float) * v.size()) != 0) return -2;      // (host or device rows)
+  if (!prm_valid(s, "fb_param_set", p, v.data(), n)) return -1;
+  if (int rc = ensure_prm(s)) return rc;
+  // read-modify-write of the parameter's segment of every env's row (dof_damping: and of the M_damp diagonal)
+  const size_t P = s->d.prm_stride;
+  auto write = [&](size_t off, size_t w, auto slot) {
+    std::vector<float> rows((size_t)N * w);
+    if (read_out(s, {{rows.data(), s->d.prm + off, P * 4, w * 4, (size_t)N}}) != 0) return -2;
+    for (int k = 0; k < n; k++) {
+      const size_t e = env_ids ? env_ids[k] : k;
+      for (size_t i = 0; i < K; i++) rows[e * w + slot((int)i)] = v[k * K + i];
+    }
+    if (copy_rows_async(s, s->d.prm + off, P * 4, rows.data(), w * 4, w * 4, N) != 0) return -2;
+    return sync_stream(s);
+  };
+  int rc = write(s->d.prm_off[p], p == FB_P_BODY_INERTIA ? 4 * K / 3 : K, [&](int i) { return prm_slot(p, i); });
+  if (rc == 0 && p == FB_P_DOF_DAMPING) rc = write(s->d.prm_mdamp, s->m.nM, [&](int i) { return s->h_dof_Madr[i]; });
+  return rc;
+}
+int fb_param_get(FbHandle s, int p, float* dst, int) {
+  if (!s) return -1;
+  if (p < 0 || p >= FB_NPARAMS) { s->err = "fb_param_get: unknown parameter"; return -1; }
+  if (!dst) { s->err = "fb_param_get: dst is NULL"; return -1; }
+  const int N = s->d.N;
+  const size_t P = s->d.prm_stride, K = (size_t)s->prm_n[p], w = (size_t)(p == FB_P_BODY_INERTIA ? 4 * K / 3 : K);
+  std::vector<float> rows((size_t)N * w), out((size_t)N * K);
+  if (s->d.prm) { if (read_out(s, {{rows.data(), s->d.prm + s->d.prm_off[p], P * 4, w * 4, (size_t)N}}) != 0) return -2; }
+  else for (int e = 0; e < N; e++) std::copy(s->h_prm0.begin() + s->d.prm_off[p], s->h_prm0.begin() + s->d.prm_off[p] + w, rows.begin() + (size_t)e * w);
+  for (int e = 0; e < N; e++) for (size_t i = 0; i < K; i++) out[(size_t)e * K + i] = rows[(size_t)e * w + prm_slot(p, (int)i)];
+  return copy_sync(s, dst, out.data(), sizeof(float) * out.size());      // (host or device memory)
+}
+int fb_param_draws(FbHandle s, int p, const float* lo, const float* hi, int shared, uint32_t seed) {
+  if (!s) return -1;
+  if (p < 0 || p >= FB_NPARAMS) { s->err = "fb_param_draws: unknown parameter"; return -1; }
+  if (!lo != !hi) { s->err = "fb_param_draws: lo and hi are both given or both NULL"; return -1; }
+  const int K = s->prm_n[p];
+  if (lo) {
+    if (!prm_valid(s, "fb_param_draws", p, lo, 1) || !prm_valid(s, "fb_param_draws", p, hi, 1)) return -1;
+    for (int i = 0; i < K; i++) if (!(lo[i] <= hi[i])) { s->err = "fb_param_draws: lo > hi at element " + std::to_string(i); return -1; }
+  } else if (!s->d.prm) return 0;          // nothing to stop
+  if (int rc = ensure_prm(s)) return rc;
+  DevPrmDraw& g = s->prm_draw_host;
+  g.seed = seed; g.on[p] = lo ? 1 : 0; g.shared[p] = shared ? 1 : 0;
+  for (int i = 0; lo && i < K; i++) { s->h_prm_lo[s->d.prm_off[p] + prm_slot(p, i)] = lo[i]; s->h_prm_hi[s->d.prm_off[p] + prm_slot(p, i)] = hi[i]; }
+  const size_t bytes = sizeof(float) * s->d.prm_stride;
+  if (copy_sync(s, (void*)g.lo, s->h_prm_lo.data(), bytes) != 0 || copy_sync(s, (void*)g.hi, s->h_prm_hi.data(), bytes) != 0 ||
+      copy_sync(s, s->prm_draw_dev, &g, sizeof(g)) != 0) return -2;
+  bool any = false;
+  for (int k = 0; k < FB_NPARAMS; k++) any = any || g.on[k];
+  s->d.prm_draw = any ? s->prm_draw_dev : nullptr;
+  return 0;
+}
+int fb_param_clear(FbHandle s) {
+  if (!s) return -1;
+  if (!s->d.prm) return 0;
+  if (sync_stream(s) != 0) return -2;
+  state_drop(s);
+  scope_free(s, s->prm_scope);
+  s->d.prm = nullptr; s->d.prm_count = nullptr; s->d.prm_draw = nullptr; s->prm_draw_dev = nullptr;
+  return 0;
+}
+
 static int do_reset(FbSim* s, const int32_t* env_ids, int n, const float* qpos, const float* qvel, int hold) {
   const DevModel& m = s->m; int N = s->d.N, Np = s->d.Np;
   if (sync_stream(s) != 0) return -2;
@@ -1140,7 +1273,7 @@ static int do_reset(FbSim* s, const int32_t* env_ids, int n, const float* qpos, 
   if (qvel) copy_async(s, s->rst_qvel_dev, qv.data(), sizeof(float) * qv.size());
   if (sync_stream(s) != 0) return -2;       // the host vectors go out of scope below
   s->d.rst_ids = s->rst_ids_dev; s->d.rst_qpos = s->rst_qpos_dev; s->d.rst_qvel = s->rst_qvel_dev; s->d.rst_n = cnt; s->d.rst_has_qvel = qvel ? 1 : 0; s->d.rst_hold = hold;
-  fb_launch<ShNone, Ph<ph_reset_scatter>>(s, K_MISC, 0, cnt);
+  fb_launch<ShNone, Ph<ph_reset_scatter>, Ph<ph_reset_draw>, Ph<ph_reset_count>>(s, K_MISC, 0, cnt);
   s->d.rst_n = 0;
   return 0;
 }
@@ -1689,6 +1822,7 @@ static std::vector<StSeg> state_layout(FbSim* s, unsigned* row, uint64_t* sig, i
   if (d.tobs) { add(16, d.tobs, (unsigned)d.tobs_dim, d.tobs_dim); add(17, s->op_step_dev, 1, 1); add(18, s->op_first_dev, 1, 1, 1); }
   if (d.op_ref_slot && s->ref_slots) add(19, s->ref_slots, (unsigned)(7 * s->ref_slot_len), 7 * s->ref_slot_len);
   if (d.qfrc_applied) { add(20, d.qfrc_applied, (unsigned)m.nv, m.nv); add(21, d.xfrc_applied, (unsigned)(6 * m.nbody), 6 * m.nbody); }
+  if (d.prm) { add(22, d.prm, d.prm_stride, (int)d.prm_stride); add(23, d.prm_count, 1, 1); }
   mix(d.task ? (uint64_t)s->task_host.kind + 1 : 0); mix(d.task ? (uint64_t)s->task_host.ref_bank : 0);
   if (d.task) {
     const DevTask& t = s->task_host;
@@ -1716,7 +1850,7 @@ template <bool LOAD> static void launch_state(FbSim* s, const int* env_ids, cons
 }
 static int state_ready(FbSim* s, const char* who) {
   if (s->st_bank) return 0;
-  s->err = std::string(who) + (s->st_stale ? ": the state bank was dropped when the handle's programs, reference slots or applied-force arrays changed: call fb_state_bank again"
+  s->err = std::string(who) + (s->st_stale ? ": the state bank was dropped when the handle's programs, reference slots, applied-force arrays or parameter overlay changed: call fb_state_bank again"
                                            : ": no state bank (fb_state_bank)");
   return -1;
 }
@@ -2101,6 +2235,7 @@ int fb_fd_inverse_columns(FbHandle s, int centered) { return s ? fd_columns(s, t
 
 int fb_fd_inverse(FbHandle s, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device) {
   if (!s) return -1;
+  if (s->d.prm) { s->err = "fb_fd_inverse: the handle has a parameter overlay, and the columns are written from qpos, qvel and qacc alone (fb_param_clear first)"; return -1; }
   const int N = s->d.N, ncol = fd_columns(s, true, centered != 0);
   if (n < 1 || (long long)n * ncol > N) {
     s->err = "fb_fd_inverse: 1 <= n problems with n * fb_fd_inverse_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }

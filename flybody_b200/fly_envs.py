@@ -722,6 +722,35 @@ class BatchedFlyEnv(_TaskEnv):
         """zero every env's applied forces (the step goes back to the path without the applied-force term)"""
         self._sim.clear_applied()
 
+    def set_model_params(self, env_ids=None, **fields):
+        """`physics.model` writes without mj_setConst, per env: fields named as mjModel's (`stepper.PARAMS`: body_mass [nbody],
+        body_inertia [nbody, 3], dof_armature, dof_damping [nv], jnt_stiffness [njnt], geom_friction [ngeom, 3], actuator_gainprm,
+        actuator_biasprm [nu, 3] (MuJoCo's first three entries), gravity, wind [3], density, viscosity [1]) for every env (`env_ids`
+        None; a single row broadcasts) or the listed envs.  They persist across steps and resets until overwritten or cleared."""
+        for name, v in fields.items():
+            self._sim.param_set(name, v, env_ids)
+
+    def model_params(self):
+        """-> {field: [n_envs, ...] float32} of every per-env model parameter (the compiled values where none was set)"""
+        m = self.model
+        shapes = {'body_inertia': (m.nbody, 3), 'geom_friction': (m.ngeom, 3), 'actuator_gainprm': (m.nu, 3), 'actuator_biasprm': (m.nu, 3)}
+        return {name: self._sim.param_get(name).reshape((self.n_envs,) + shapes.get(name, (-1,))) for name in st.PARAMS}
+
+    def randomize_model_params(self, seed=0, shared=(), **ranges):
+        """domain randomisation: at every reset of an env from now on, each named field is drawn from U(lo, hi) per element (`name=(lo,
+        hi)`, each broadcast to the field's shape), or with one draw for all its elements for the names in `shared` (lo = 0.8 m,
+        hi = 1.2 m scales every element by one factor).  Draws are a counter hash of (seed, env, the env's reset count, field, element):
+        the same on the host-side and the device-side task code.  Fields not named keep their values."""
+        for name in shared:
+            if name not in ranges:
+                raise ValueError(f'shared names {name!r}, which has no range')
+        for name, (lo, hi) in ranges.items():
+            self._sim.param_draws(name, lo, hi, shared=name in shared, seed=seed)
+
+    def clear_model_params(self):
+        """every env back to the compiled model's parameters, and no draws (the step goes back to the model's tables)"""
+        self._sim.param_clear()
+
     def set_reset_noise(self, amp):
         """U(-amp, amp) rad added to the actuated leg joints of the start pose at the resets from now on (0: the reference's exact
         start pose).  `reset_noise=` of the factory sets the initial value; a batch is typically started with noise once, so that the

@@ -20,12 +20,17 @@ LIB_PATH = os.path.join(_HERE, 'lib', 'libflybody_b200.so')
  QFRC_BIAS, QFRC_ACTUATOR, CONTACT, EFC_FORCE, FLAGS, QFRC_APPLIED, XFRC_APPLIED) = range(28)
 MAXCON, MAXEFC = 64, 160
 
+# enum FbParam: the per-env model parameters (fb_param_*), by their mjModel names, and their shape per env
+PARAMS = ('body_mass', 'body_inertia', 'dof_armature', 'dof_damping', 'jnt_stiffness', 'geom_friction', 'actuator_gainprm',
+          'actuator_biasprm', 'gravity', 'wind', 'density', 'viscosity')
+
 EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_applied_ptrs', 'fb_clear_applied', 'fb_step', 'fb_forward',
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
            'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version',
            'fb_state_slots', 'fb_state_signature', 'fb_state_bank', 'fb_state_save', 'fb_state_load', 'fb_state_read', 'fb_state_write', 'fb_state_substeps',
            'fb_ik_program', 'fb_ik_solve', 'fb_ik_read', 'fb_inverse', 'fb_inverse_read',
-           'fb_fd_columns', 'fb_fd_transition', 'fb_fd_read', 'fb_fd_inverse_columns', 'fb_fd_inverse', 'fb_fd_inverse_read']
+           'fb_fd_columns', 'fb_fd_transition', 'fb_fd_read', 'fb_fd_inverse_columns', 'fb_fd_inverse', 'fb_fd_inverse_read',
+           'fb_param_size', 'fb_param_set', 'fb_param_get', 'fb_param_draws', 'fb_param_clear']
 
 
 # enum FbTaskKind (FbTaskProgram.kind)
@@ -177,6 +182,11 @@ def load_library(path=None):
     lib.fb_fd_inverse_columns.argtypes = [C.c_void_p, C.c_int]
     lib.fb_fd_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int]
     lib.fb_fd_inverse_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_int]
+    lib.fb_param_size.argtypes = [C.c_void_p, C.c_int]
+    lib.fb_param_set.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+    lib.fb_param_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+    lib.fb_param_draws.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_uint32]
+    lib.fb_param_clear.argtypes = [C.c_void_p]
     return lib
 
 
@@ -287,6 +297,43 @@ class BatchedStepper:
     def clear_applied(self):
         """drop every env's applied forces: the step goes back to the path without them"""
         self._check(self._lib.fb_clear_applied(self._h), 'fb_clear_applied')
+
+    # ---- per-env model parameters (fb_param_*: physics.model writes without mj_setConst, per env; see the header)
+    def _param(self, name):
+        if name not in PARAMS:
+            raise KeyError(f'{name!r} is not a per-env model parameter ({", ".join(PARAMS)})')
+        p = PARAMS.index(name)
+        return p, int(self._lib.fb_param_size(self._h, p))
+
+    def param_set(self, name, vals, env_ids=None):
+        """vals [n_envs or len(env_ids), size] (a [size] row broadcasts) -> every env (env_ids None) or the listed ones"""
+        p, k = self._param(name)
+        ids = None if env_ids is None else np.ascontiguousarray(np.asarray(env_ids).reshape(-1), np.int32)
+        n = self.n_envs if ids is None else len(ids)
+        v = np.ascontiguousarray(np.broadcast_to(np.asarray(vals, np.float32).reshape(-1, k), (n, k)))
+        self._check(self._lib.fb_param_set(self._h, p, None if ids is None else ids.ctypes.data, n, v.ctypes.data, 0), 'fb_param_set')
+
+    def param_get(self, name):
+        """-> [n_envs, size] f32 (the compiled values while there is no overlay)"""
+        p, k = self._param(name)
+        out = np.zeros((self.n_envs, k), np.float32)
+        self._check(self._lib.fb_param_get(self._h, p, out.ctypes.data, 0), 'fb_param_get')
+        return out
+
+    def param_draws(self, name, lo=None, hi=None, shared=False, seed=0):
+        """draw `name` from [lo, hi] ([size] each, broadcast) at every reset of an env; lo = hi = None stops drawing it"""
+        p, k = self._param(name)
+        if lo is None and hi is None:
+            self._check(self._lib.fb_param_draws(self._h, p, None, None, 0, int(seed)), 'fb_param_draws')
+            return
+        lo = np.ascontiguousarray(np.broadcast_to(np.asarray(lo, np.float32).reshape(-1), (k,)))
+        hi = np.ascontiguousarray(np.broadcast_to(np.asarray(hi, np.float32).reshape(-1), (k,)))
+        self._check(self._lib.fb_param_draws(self._h, p, lo.ctypes.data, hi.ctypes.data, int(bool(shared)), int(seed) & 0xffffffff),
+                    'fb_param_draws')
+
+    def param_clear(self):
+        """drop every env's parameters and the draw program: the step goes back to the compiled model's tables"""
+        self._check(self._lib.fb_param_clear(self._h), 'fb_param_clear')
 
     # ---- state rows (fb_state_*: physics.get_state / set_state for the envs of the batch, see the header)
     @property

@@ -227,6 +227,48 @@ int fb_applied_ptrs(FbHandle h, void** qfrc_applied_dev, void** xfrc_applied_dev
  * back to the path without the applied-force term).  Pointers of fb_applied_ptrs become invalid.                      */
 int fb_clear_applied(FbHandle h);
 
+/* Per-env model parameters: writes to physics.model without mj_setConst (what dm_control does), for every env of the batch on its
+ * own.  Each parameter is named as its mjModel field; its size per env is fb_param_size (the step reads column 0 of geom_friction at
+ * the model's condim <= 3, and entries 0 .. 2 of MuJoCo's ten gainprm / biasprm entries; all are stored).  Derived constants keep
+ * their compiled values (body_invweight0, dof_invweight0, meaninertia, body_subtreemass, the task programs' constants); the
+ * implicit-damping diagonal of the Euler step follows the env's dof_damping.  jnt_stiffness acts on hinge joints only, so the other
+ * joints' entries must stay 0.
+ *   The overlay [n_envs][parameters] is allocated on first use (fb_param_set / fb_param_draws) with every env at the compiled
+ * values; it persists across steps and resets until overwritten or cleared (it is model, not data: resets do not restore it).
+ * Allocating or clearing it drops the state bank (a state row then carries the env's parameters and draw counter) and
+ * the captured step graphs.
+ *   A draw program (fb_param_draws) redraws the listed parameters of an env at each of its resets (fb_reset, fb_reset_hold, a
+ * device-task reset): lo + u (hi - lo) per element, u a counter hash of (seed, env, the env's draw count, parameter, element), or of
+ * element 0 for every element of a `shared` parameter (one factor for all of them).  The same reset sequence gives the same rows
+ * through the host-side and the device-side task code.
+ *   Inputs are checked: parameter ids, sizes, env ids, finite values, no negative mass, inertia, armature, damping, stiffness,
+ * friction, density or viscosity, lo <= hi.                                                                                        */
+enum FbParam {
+  FB_P_BODY_MASS = 0,        /* nbody                                                    */
+  FB_P_BODY_INERTIA = 1,     /* nbody * 3 (principal inertia)                            */
+  FB_P_DOF_ARMATURE = 2,     /* nv                                                       */
+  FB_P_DOF_DAMPING = 3,      /* nv                                                       */
+  FB_P_JNT_STIFFNESS = 4,    /* njnt                                                     */
+  FB_P_GEOM_FRICTION = 5,    /* ngeom * 3                                                */
+  FB_P_ACTUATOR_GAINPRM = 6, /* nu * 3                                                   */
+  FB_P_ACTUATOR_BIASPRM = 7, /* nu * 3                                                   */
+  FB_P_GRAVITY = 8,          /* 3 (mjModel.opt)                                          */
+  FB_P_WIND = 9,             /* 3                                                        */
+  FB_P_DENSITY = 10,         /* 1                                                        */
+  FB_P_VISCOSITY = 11,       /* 1                                                        */
+  FB_NPARAMS = 12
+};
+int fb_param_size(FbHandle h, int param);     /* values per env, -1 for an unknown id */
+/* vals [n][size] (host, or device memory when is_device) -> the listed envs; env_ids NULL: every env, n must be n_envs. */
+int fb_param_set(FbHandle h, int param, const int32_t* env_ids, int n, const float* vals, int is_device);
+/* -> dst [n_envs][size] (host, or device memory when is_device); the compiled values while there is no overlay.  Synchronises. */
+int fb_param_get(FbHandle h, int param, float* dst, int is_device);
+/* Draw `param` at every reset from [lo, hi] ([size] host arrays each); shared != 0: one draw for all its elements.  NULL lo and hi
+ * stop drawing it.  seed is the program's (every call sets it).                                                                  */
+int fb_param_draws(FbHandle h, int param, const float* lo, const float* hi, int shared, uint32_t seed);
+/* Free the overlay, the draw counters and the draw program: the step goes back to the compiled model's tables. */
+int fb_param_clear(FbHandle h);
+
 /* n_substeps x physics.step() with legacy_step=True, i.e. (mj_step2; mj_step1) per substep
  * (SURVEY.md App. A), accumulating the per-substep sensor mean.  Asynchronous on the handle's
  * stream.                                                                                     */
@@ -443,7 +485,8 @@ int fb_eyes_read(FbHandle h, uint8_t* host_dst);
  * task env carries per env.  A row is everything the next fb_step / fb_task_step of an env reads that the position / velocity
  * stage does not recompute from it: qpos, qvel, act, ctrl, qacc, time, flags, solver iterations, hold, the solver's warm start
  * (previous row keys, count, forces), sensordata and the per-step sensor sums, the env's packed and task observation rows with
- * their step index / FIRST flag, its reference slot (fb_ref_slots), its applied forces if the handle has them, and the device
+ * their step index / FIRST flag, its reference slot (fb_ref_slots), its applied forces if the handle has them, its model parameters
+ * and draw counter if the handle has a parameter overlay (fb_param_set), and the device
  * task's per-env arrays (counters, reset flags, staged draws, wing-beat generator, `out` row, dataset episode and pin, vision
  * targets and terrain pick).  A rollout continued from a loaded row equals the uninterrupted one bit for bit.
  *   After fb_state_load, fb_get returns the saved values for the fields above and freshly recomputed ones for everything the
@@ -454,7 +497,7 @@ int fb_eyes_read(FbHandle h, uint8_t* host_dst);
  * fb_hfield_write are the caller's to rewrite.  The device task's draws are a counter hash of (seed, env, episode): a row
  * loaded into another env id continues bit for bit until that env's next reset, whose draws follow the new id.
  *   The layout follows the handle: replacing the observation or task program, the reference slots, a bank a task program draws
- * from, or allocating / clearing the applied-force arrays drops the bank, and save / load fail with a message until
+ * from, or allocating / clearing the applied-force arrays or the parameter overlay drops the bank, and save / load fail with a message until
  * fb_state_bank is called again.  fb_state_signature hashes the layout (sizes, program kinds, slot length, layout version);
  * rows move between handles with equal signatures.  Saving and loading change nothing a captured step graph depends on.    */
 int fb_state_slots(FbHandle h);                  /* 4-byte slots of one row under the handle's current model, programs and applied-force arrays */
@@ -505,7 +548,8 @@ int fb_ik_read(FbHandle h, float* qpos, float* err, float* err_first, int32_t* s
  * qfrc_inverse excludes applied and actuator forces: for the continuous-time qacc fb_forward leaves in FB_QACC it equals
  * qfrc_applied + J^T xfrc_applied + qfrc_actuator up to the forward solve's tolerance.  Noslip is not inverted (as in MuJoCo): on a
  * model with noslip iterations the forces are the soft model's, not the forward step's post-noslip friction.  The discrete inverse
- * (mjENBL_INVDISCRETE) is not implemented.  Errors: n outside 1 .. n_envs, a NULL qacc, a non-finite host qacc.  A device qacc is
+ * (mjENBL_INVDISCRETE) is not implemented.  Problem i runs in env i, so with a parameter overlay (fb_param_set) it uses env i's
+ * model parameters.  Errors: n outside 1 .. n_envs, a NULL qacc, a non-finite host qacc.  A device qacc is
  * not checked and the call returns without synchronising; with a host qacc it synchronises.                                    */
 int fb_inverse(FbHandle h, int n, const float* qacc, int is_device);
 /* Results of the last fb_inverse for its n problems (synchronises; any pointer may be NULL; is_device: the pointers are device
@@ -520,7 +564,7 @@ int fb_inverse_read(FbHandle h, float* qfrc_inverse, float* qfrc_constraint, flo
  * A problem is a state row of the bank (fb_state_save / fb_state_write).  It takes fb_fd_columns(h, centered) envs: 1 + 2 (nx + nu)
  * centred, 1 + nx + nu forward; column 0 is the unperturbed nominal.  Every column starts from the row, its warm start included (as
  * MuJoCo restores qacc_warmstart before each nudged step), and from its applied forces when the rows carry them (held fixed, as
- * mjData's are).  Coordinate j is nudged by delta_j = eps max(1, |x_j|) (x_j: the hinge angle, the free joint's translation component,
+ * mjData's are), and from its model parameters when the rows carry an overlay (fb_param_set).  Coordinate j is nudged by delta_j = eps max(1, |x_j|) (x_j: the hinge angle, the free joint's translation component,
  * qvel, act or ctrl; rotational tangent coordinates delta = eps): the stepper is fp32, and a step relative to the coordinate keeps fast
  * ones resolved (MuJoCo's absolute step is the case |x_j| <= 1; flybody_b200.derivatives defaults to eps 1e-2).  ctrl at its limits follows MuJoCo: forward if the actuator is not
  * ctrl-limited or ctrl and ctrl + delta lie in its range, backward if (centred or no forward nudge) and ctrl - delta and ctrl do;
@@ -552,7 +596,8 @@ int fb_fd_read(FbHandle h, float* A, float* B, float* qpos_next, float* qvel_nex
  * holds; none of them reaches qfrc_inverse.  The handle is a workspace: afterwards every env's qpos / qvel and the record are
  * unspecified; fb_inverse_read still returns the last fb_inverse and the state bank is untouched.  Noslip is not inverted (as in
  * fb_inverse and MuJoCo): on a model with noslip iterations the forces are the soft model's.  Errors: n < 1 or n ncol > n_envs, a
- * NULL input, a non-finite host input, eps <= 0 or not finite.  A device input is not checked and the call returns without
+ * NULL input, a non-finite host input, eps <= 0 or not finite, a parameter overlay on the handle (the columns are written from
+ * qpos, qvel and qacc alone and would run with the parameters of whichever env they land in: fb_param_clear first).  A device input is not checked and the call returns without
  * synchronising; with host inputs it synchronises.                                                                                   */
 int fb_fd_inverse_columns(FbHandle h, int centered);
 int fb_fd_inverse(FbHandle h, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device);
