@@ -44,13 +44,17 @@ FB_DEV int col_plane_capsule(RawCon* c, float margin, V3 pp, V3 n, V3 cp, const 
   for (int i = 0; i < k; i++) c[i].t = axis;
   return k;
 }
+// |axis (n.axis) - n|^2 below which a cylinder stands upright on the plane (MuJoCo: 1e-15).  On a plane whose normal is a
+// coordinate axis (the floor) its part across n has no cancellation and fp32 resolves it down to 1e-15 as well; on a tilted
+// plane fp32 resolves it to ~1e-14 only (DESIGN.md section 2)
+#define FB_CYLINDER_UPRIGHT 1e-15f
 FB_DEV int col_plane_cylinder(RawCon* c, float margin, V3 pp, V3 n, V3 cp, const M3& cm, V3 size) {
   V3 axis = col(cm, 2);
   float dist0 = dot(cp - pp, n), prjaxis = dot(n, axis);
   if (prjaxis > 0) { axis = axis * -1.0f; prjaxis = -prjaxis; }
   V3 vec = axis * prjaxis - n;
   float len2 = dot(vec, vec);
-  if (len2 >= 1e-12f) vec = vec * (size.x / sqrtf(len2)); else vec = col(cm, 0) * size.x;
+  if (len2 >= FB_CYLINDER_UPRIGHT) vec = vec * (size.x / sqrtf(len2)); else vec = col(cm, 0) * size.x;
   float prjvec = dot(vec, n);
   axis = axis * size.y; prjaxis *= size.y;
   int cnt = 0;
@@ -88,13 +92,18 @@ FB_DEV int col_sphere_capsule(RawCon* c, float margin, V3 sp, float sr, V3 cp, c
   float x = clampf(dot(axis, sp - cp), -csize.y, csize.y);
   return raw_sphere_sphere(c, margin, sp, sr, cp + axis * x, csize.x);
 }
+#define FB_CAPSULE_PARALLEL 1e-15f     // |a1 x a2|^2 below which two capsule axes count as parallel
 FB_DEV int col_capsule_capsule(RawCon* c, float margin, V3 p1, const M3& m1, V3 s1, V3 p2, const M3& m2, V3 s2) {
   V3 a1 = col(m1, 2), a2 = col(m2, 2), dif = p1 - p2;
   float ma = dot(a1, a1), mb = -dot(a1, a2), mc = dot(a2, a2), u = -dot(a1, dif), v = dot(a2, dif);
-  float det = ma * mc - mb * mb;
-  // fp32: 1 - cos^2 loses its digits long before the fp64 threshold (1e-15) of the reference
-  if (fabsf(det) >= 1e-6f) {
-    float x1 = (mc * u - mb * v) / det, x2 = (ma * v - mb * u) / det;
+  // det = ma mc - mb^2 = |a1 x a2|^2, and the closest-point numerators mc u - mb v = n.(a2 x dif), ma v - mb u = n.(a1 x dif)
+  // with n = a1 x a2 (Binet-Cauchy).  In the cross-product form they keep their relative precision for nearly parallel axes,
+  // where ma mc - mb^2 cancels in fp32 (5 % off at 1e-3 rad, exactly 0 below 2.4e-4 rad).  DESIGN.md section 2 gives the
+  // angles at which fp32 and the fp64 reference still take different branches.
+  const V3 n = cross(a1, a2);
+  const float det = dot(n, n);
+  if (det >= FB_CAPSULE_PARALLEL) {
+    float x1 = dot(n, cross(a2, dif)) / det, x2 = dot(n, cross(a1, dif)) / det;
     if (x1 > s1.y) { x1 = s1.y; x2 = (v - mb * s1.y) / mc; }
     else if (x1 < -s1.y) { x1 = -s1.y; x2 = (v + mb * s1.y) / mc; }
     if (x2 > s2.y) { x2 = s2.y; x1 = clampf((u - mb * s2.y) / ma, -s1.y, s1.y); }
@@ -426,6 +435,35 @@ FB_DEV void col_store(const DevModel& m, const DevData& d, int e, int j, const R
     AT(d.tmp_geom, 2 * slot) = g1; AT(d.tmp_geom, 2 * slot + 1) = g2;
   }
 }
+// narrowphase dispatch of one pair (the lower type first, a plane first of all; pn: the plane's normal): its contacts into
+// rc[0..3], or -1 for a generic convex pair that the cheap tests cannot rule out (its MPR runs as a job of kcol_mpr).  `g` gives
+// a geom's size and rotation (k = 1, 2), loaded only where the pair type needs them.  kcol_narrow and the test hook
+// fb_emu_pair both call this, so the hook runs the kernel's own decisions.
+template <class G>
+FB_DEV int col_narrow_pair(RawCon* rc, float margin, bool plane, int t1, V3 x1, int t2, V3 x2, V3 pn, const G& g) {
+  int n = 0;
+  if (plane) {
+    V3 s2 = g.size(2);
+    if (t2 == FB_GEOM_SPHERE) n = raw_plane_sphere(rc, margin, x1, pn, x2, s2.x);
+    else { M3 R2 = g.rot(2);
+      if (t2 == FB_GEOM_CAPSULE) n = col_plane_capsule(rc, margin, x1, pn, x2, R2, s2);
+      else if (t2 == FB_GEOM_CYLINDER) n = col_plane_cylinder(rc, margin, x1, pn, x2, R2, s2);
+      else if (t2 == FB_GEOM_ELLIPSOID) n = col_plane_ellipsoid(rc, margin, x1, pn, x2, R2, s2); }
+  } else {
+    V3 s1 = g.size(1), s2 = g.size(2);
+    if (t1 == FB_GEOM_SPHERE && t2 == FB_GEOM_SPHERE) n = raw_sphere_sphere(rc, margin, x1, s1.x, x2, s2.x);
+    else if (t1 == FB_GEOM_SPHERE && t2 == FB_GEOM_CAPSULE) { M3 R2 = g.rot(2); n = col_sphere_capsule(rc, margin, x1, s1.x, x2, R2, s2); }
+    else if (t1 == FB_GEOM_CAPSULE && t2 == FB_GEOM_CAPSULE) { M3 R1 = g.rot(1), R2 = g.rot(2); n = col_capsule_capsule(rc, margin, x1, R1, s1, x2, R2, s2); }
+    else { M3 R1 = g.rot(1), R2 = g.rot(2);      // generic convex pair: MPR job if the cheap tests cannot rule it out
+      n = convex_prefilter(margin, t1, x1, R1, s1, t2, x2, R2, s2) ? -1 : 0; }
+  }
+  return n;
+}
+struct ColGeoms {         // col_narrow_pair's geoms in the kernel: sizes from the model, rotations from the env's record
+  const DevModel& m; const DevData& d; int e, g1, g2;
+  FB_DEVM V3 size(int k) const { return mld3(m.geom_size, k == 1 ? g1 : g2); }
+  FB_DEVM M3 rot(int k) const { return ld9(d.geom_xmat, k == 1 ? g1 : g2, d, e); }
+};
 // 2. narrowphase: one candidate per lane, up to 4 contacts each into tmp_con[4 j + i]
 FB_DEV void kcol_narrow(FB_COL_ARGS) {
   FB_COL_PTRS
@@ -436,23 +474,9 @@ FB_DEV void kcol_narrow(FB_COL_ARGS) {
     V3 x1 = v3(gx[3 * g1], gx[3 * g1 + 1], gx[3 * g1 + 2]), x2 = v3(gx[3 * g2], gx[3 * g2 + 1], gx[3 * g2 + 2]);
     const int t1 = m.geom_type[g1], t2 = m.geom_type[g2];
     const float margin = fmaxf(m.geom_margin[g1], m.geom_margin[g2]);
-    RawCon rc[4]; int n = 0;
-    if (plane) {
-      V3 pn = v3(gn[3 * g1], gn[3 * g1 + 1], gn[3 * g1 + 2]);
-      V3 s2 = mld3(m.geom_size, g2);
-      if (t2 == FB_GEOM_SPHERE) n = raw_plane_sphere(rc, margin, x1, pn, x2, s2.x);
-      else { M3 R2 = ld9(d.geom_xmat, g2, d, e);
-        if (t2 == FB_GEOM_CAPSULE) n = col_plane_capsule(rc, margin, x1, pn, x2, R2, s2);
-        else if (t2 == FB_GEOM_CYLINDER) n = col_plane_cylinder(rc, margin, x1, pn, x2, R2, s2);
-        else if (t2 == FB_GEOM_ELLIPSOID) n = col_plane_ellipsoid(rc, margin, x1, pn, x2, R2, s2); }
-    } else {
-      V3 s1 = mld3(m.geom_size, g1), s2 = mld3(m.geom_size, g2);
-      if (t1 == FB_GEOM_SPHERE && t2 == FB_GEOM_SPHERE) n = raw_sphere_sphere(rc, margin, x1, s1.x, x2, s2.x);
-      else if (t1 == FB_GEOM_SPHERE && t2 == FB_GEOM_CAPSULE) { M3 R2 = ld9(d.geom_xmat, g2, d, e); n = col_sphere_capsule(rc, margin, x1, s1.x, x2, R2, s2); }
-      else if (t1 == FB_GEOM_CAPSULE && t2 == FB_GEOM_CAPSULE) { M3 R1 = ld9(d.geom_xmat, g1, d, e), R2 = ld9(d.geom_xmat, g2, d, e); n = col_capsule_capsule(rc, margin, x1, R1, s1, x2, R2, s2); }
-      else { M3 R1 = ld9(d.geom_xmat, g1, d, e), R2 = ld9(d.geom_xmat, g2, d, e);      // generic convex pair: MPR job if the cheap tests cannot rule it out
-        n = convex_prefilter(margin, t1, x1, R1, s1, t2, x2, R2, s2) ? -1 : 0; }
-    }
+    RawCon rc[4];
+    const V3 pn = plane ? v3(gn[3 * g1], gn[3 * g1 + 1], gn[3 * g1 + 2]) : v3(0, 0, 0);
+    const int n = col_narrow_pair(rc, margin, plane, t1, x1, t2, x2, pn, ColGeoms{m, d, e, g1, g2});
     col_store(m, d, e, j, rc, n, g1, g2);
     ccnt[j] = n;
   }

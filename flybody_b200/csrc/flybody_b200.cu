@@ -891,6 +891,27 @@ extern "C" int fb_emu_convex_pair(int t1, const float* p1, const float* m1, cons
   if (n) { out[0] = c.dist; out[1] = c.pos.x; out[2] = c.pos.y; out[3] = c.pos.z; out[4] = c.n.x; out[5] = c.n.y; out[6] = c.n.z; }
   return n;
 }
+// host-emulation build only (tests): one pair of any type the collision stage handles, through kcol_narrow's dispatch (a plane
+// is t1 = FB_GEOM_PLANE with its normal the third column of m1; a generic pair the prefilter keeps then runs MPR as in kcol_mpr),
+// then the contact frames as col_store makes them; out [4][13] = dist, pos[3], frame[9] per contact
+struct PairGeoms { V3 s1, s2; M3 R1, R2; V3 size(int k) const { return k == 1 ? s1 : s2; } M3 rot(int k) const { return k == 1 ? R1 : R2; } };
+extern "C" int fb_emu_pair(int t1, const float* p1, const float* m1, const float* s1, int t2, const float* p2, const float* m2, const float* s2,
+                           float margin, float* out) {
+  PairGeoms g; for (int k = 0; k < 9; k++) { g.R1.m[k] = m1[k]; g.R2.m[k] = m2[k]; }
+  g.s1 = v3(s1[0], s1[1], s1[2]); g.s2 = v3(s2[0], s2[1], s2[2]);
+  const V3 x1 = v3(p1[0], p1[1], p1[2]), x2 = v3(p2[0], p2[1], p2[2]);
+  const bool plane = t1 == FB_GEOM_PLANE;
+  RawCon rc[4];
+  int n = col_narrow_pair(rc, margin, plane, t1, x1, t2, x2, plane ? col(g.R1, 2) : v3(0, 0, 0), g);
+  if (n < 0) n = convex_mpr(rc, margin, t1, x1, g.R1, g.s1, t2, x2, g.R2, g.s2);
+  for (int i = 0; i < n; i++) {
+    V3 f1, f2; make_frame(rc[i].n, rc[i].t, f1, f2);
+    float* o = out + 13 * i;
+    o[0] = rc[i].dist; o[1] = rc[i].pos.x; o[2] = rc[i].pos.y; o[3] = rc[i].pos.z; o[4] = rc[i].n.x; o[5] = rc[i].n.y; o[6] = rc[i].n.z;
+    o[7] = f1.x; o[8] = f1.y; o[9] = f1.z; o[10] = f2.x; o[11] = f2.y; o[12] = f2.z;
+  }
+  return n;
+}
 #endif
 const char* fb_last_error(FbHandle s) { return s ? s->err.c_str() : "null handle"; }
 int fb_n_envs(FbHandle s) { return s ? s->d.N : -1; }
@@ -1089,6 +1110,7 @@ int fb_get(FbHandle s, int field, void* dst, int is_device) {
         for (int i = 0; i < 3; i++) { o[1 + i] = pos[ec * 3 + i] + ref[(size_t)e * 3 + i]; o[4 + i] = frame[ec * 9 + i]; }
         o[7] = (float)g1[ec]; o[8] = (float)g2[ec]; o[9] = (float)dm[ec];
         o[12] = (float)ea[ec]; o[10] = o[12] >= 0 ? 1.0f : 0.0f; o[11] = mu[ec];
+        for (int i = 0; i < 3; i++) o[13 + i] = frame[ec * 9 + 3 + i];
       }
       return 0; }
     default: s->err = "unknown field"; return -1;

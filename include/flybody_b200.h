@@ -174,7 +174,8 @@ enum FbField {
   FB_QFRC_PASSIVE = 20,    /* nv                                                    */
   FB_QFRC_BIAS = 21,       /* nv                                                    */
   FB_QFRC_ACTUATOR = 22,   /* nv                                                    */
-  FB_CONTACT = 23,    /* FB_MAXCON * 16: per contact [dist, pos3, normal3, geom1, geom2, dim, incl, mu, efc_adr, pad3] */
+  FB_CONTACT = 23,    /* FB_MAXCON * 16: per contact [dist, pos3, normal3, geom1, geom2, dim, incl, mu, efc_adr, tangent3]
+                         (tangent3: the frame's first tangent; the second is normal x tangent) */
   FB_EFC_FORCE = 24,  /* FB_MAXEFC                                                  */
   FB_FLAGS = 25,      /* 1 (as float): bit0 bad state (nan/inf or |qacc|>1e14), bit1 contact overflow, bit2 efc overflow */
   FB_QFRC_APPLIED = 26, /* nv : physics.data.qfrc_applied, generalized forces added to qfrc_smooth every substep           */

@@ -901,6 +901,33 @@ int orc_convex_pair(int t1, const double* p1, const double* m1, const double* s1
 int orc_convex_hfield(int type, const double* gpos, const double* gmat, const double* gsize, double margin,
                       const double* hf_pos, const double* hf_mat, const double* hf_size, int nrow, int ncol, const double* data,
                       double* out, int max);
+/* narrowphase dispatch of one geom pair (the lower type first, a plane first of all): up to 4 contacts into rc */
+static int narrow_pair(RawCon* rc, double margin, int t1, const double* p1, const double* m1, const double* s1,
+                       int t2, const double* p2, const double* m2, const double* s2) {
+  if (t1==FB_GEOM_PLANE) {
+    if (t2==FB_GEOM_SPHERE) return raw_plane_sphere(rc,margin,p1,m1,p2,s2[0]);
+    if (t2==FB_GEOM_CAPSULE) return col_plane_capsule(rc,margin,p1,m1,p2,m2,s2);
+    if (t2==FB_GEOM_CYLINDER) return col_plane_cylinder(rc,margin,p1,m1,p2,m2,s2);
+    if (t2==FB_GEOM_ELLIPSOID) return col_plane_ellipsoid(rc,margin,p1,m1,p2,m2,s2);
+    return 0;
+  }
+  if (t1==FB_GEOM_SPHERE && t2==FB_GEOM_SPHERE) return raw_sphere_sphere(rc,margin,p1,s1[0],p2,s2[0]);
+  if (t1==FB_GEOM_SPHERE && t2==FB_GEOM_CAPSULE) return col_sphere_capsule(rc,margin,p1,s1[0],p2,m2,s2);
+  if (t1==FB_GEOM_CAPSULE && t2==FB_GEOM_CAPSULE) return col_capsule_capsule(rc,margin,p1,m1,s1,p2,m2,s2);
+  return col_convex(rc,margin,t1,p1,m1,s1,t2,p2,m2,s2);   /* generic convex pairs: MPR */
+}
+/* exported for the tests: one pair of any type through the collision stage's narrowphase and make_frame (no broadphase);
+ * out [4][13] = dist, pos[3], frame[9] per contact */
+int orc_pair(int t1, const double* p1, const double* m1, const double* s1, int t2, const double* p2, const double* m2, const double* s2,
+             double margin, double* out) {
+  RawCon rc[4]; int n=narrow_pair(rc,margin,t1,p1,m1,s1,t2,p2,m2,s2);
+  for (int i=0;i<n;i++) {
+    double* o=out+13*i; double f[9];
+    copy3(f,rc[i].normal); copy3(f+3,rc[i].tangent); make_frame(f);
+    o[0]=rc[i].dist; copy3(o+1,rc[i].pos); memcpy(o+4,f,sizeof f);
+  }
+  return n;
+}
 /* contacts of one geom pair -> d->con with mj_contactParam mixing */
 static void add_contacts(OrcData* d, const RawCon* rc, int n, int g1, int g2, double margin, double gap) {
   const FbModel* m=d->m;
@@ -951,16 +978,7 @@ static void orc_collision(OrcData* d) {
       double t[3]; sub3(t,p2,p1); double r=margin+m->geom_rbound[g1]+m->geom_rbound[g2];
       if (dot3(t,t)>r*r) continue;
     }
-    RawCon rc[4]; int n=0;
-    if (t1==FB_GEOM_PLANE) {
-      if (t2==FB_GEOM_SPHERE) n=raw_plane_sphere(rc,margin,p1,m1,p2,s2[0]);
-      else if (t2==FB_GEOM_CAPSULE) n=col_plane_capsule(rc,margin,p1,m1,p2,m2,s2);
-      else if (t2==FB_GEOM_CYLINDER) n=col_plane_cylinder(rc,margin,p1,m1,p2,m2,s2);
-      else if (t2==FB_GEOM_ELLIPSOID) n=col_plane_ellipsoid(rc,margin,p1,m1,p2,m2,s2);
-    } else if (t1==FB_GEOM_SPHERE && t2==FB_GEOM_SPHERE) n=raw_sphere_sphere(rc,margin,p1,s1[0],p2,s2[0]);
-    else if (t1==FB_GEOM_SPHERE && t2==FB_GEOM_CAPSULE) n=col_sphere_capsule(rc,margin,p1,s1[0],p2,m2,s2);
-    else if (t1==FB_GEOM_CAPSULE && t2==FB_GEOM_CAPSULE) n=col_capsule_capsule(rc,margin,p1,m1,s1,p2,m2,s2);
-    else n=col_convex(rc,margin,t1,p1,m1,s1,t2,p2,m2,s2);   /* generic convex pairs: MPR */
+    RawCon rc[4]; int n=narrow_pair(rc,margin,t1,p1,m1,s1,t2,p2,m2,s2);
     add_contacts(d,rc,n,g1,g2,margin,gap);
   }
   /* terrain: every listed geom against the heightfield (mjc_ConvexHField), up to 4 contacts per geom, in list order */
@@ -1635,7 +1653,7 @@ int orc_get(OrcData* d, int field, double* out) {
       for (int i=0;i<d->ncon && i<FB_MAXCON;i++) {
         const OrcContact* c=&d->con[i]; double* o=out+16*i;
         o[0]=c->dist; copy3(o+1,c->pos); copy3(o+4,c->frame); o[7]=c->geom1; o[8]=c->geom2; o[9]=c->dim;
-        o[10]=c->exclude?0:1; o[11]=c->mu; o[12]=c->efc_address; o[13]=o[14]=o[15]=0;
+        o[10]=c->exclude?0:1; o[11]=c->mu; o[12]=c->efc_address; copy3(o+13,c->frame+3);
       }
       return 16*(d->ncon<FB_MAXCON?d->ncon:FB_MAXCON);
     case FB_EFC_FORCE: memcpy(out,d->efc_force,sizeof(double)*d->nefc); return d->nefc;

@@ -40,7 +40,18 @@ def lib():
         _LIB.orc_set_tolerance.argtypes = [C.c_void_p, C.c_double]
         _LIB.orc_set_dense.argtypes = [C.c_void_p, C.c_int]
         _LIB.orc_get_efc.argtypes = [C.c_void_p] + [C.c_void_p] * 6
+        _LIB.orc_pair.argtypes = [C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 3 + [C.c_double, C.c_void_p]
     return _LIB
+
+
+def pair(t1, p1, R1, s1, t2, p2, R2, s2, margin):
+    """one geom pair through the collision stage's narrowphase (no broadphase; a plane is t1 = 0 with its normal the third column of
+    R1): the contacts as rows [n, 13] of dist, pos[3], frame[9] (normal, first tangent, second tangent)"""
+    d = [np.ascontiguousarray(x, np.float64).ravel() for x in (p1, R1, s1, p2, R2, s2)]
+    out = np.zeros((4, 13), np.float64)
+    n = lib().orc_pair(int(t1), *[x.ctypes.data for x in d[:3]], int(t2), *[x.ctypes.data for x in d[3:]], float(margin),
+                       out.ctypes.data)
+    return out[:n].copy()
 
 
 class Oracle:
