@@ -190,3 +190,56 @@ FB_WARPFN void kfdi_diff(const DevModel& m, const DevData& d, const DevFdInv& p,
     }
   WPAR_END
 }
+
+// ---- sensor Jacobians (fb_query_sensors on).  Their own parameters beside DevFd / DevFdInv, whose kernels keep their layout.
+//   transition: C = ds/dx [n][nsd][nx] and D = ds/du [n][nsd][nu] (row-major, as A and B), s the sensors of x, the state before the
+//               step (MuJoCo's definition).  kfd_snap copies an env's sensors of one stage into snap: the velocity stage after the
+//               launch_step1 of the nudged x, the acceleration stage after the first substep's step2 (which the step1 of x' leaves).
+//               kfd_sdiff writes column j of C or D and, for j = 0, the nominal sensordata.
+//   inverse:    DsDq, DsDv, DsDa [n][nv][nsd] (MuJoCo's transposed layout); kinv_sensors writes every env's sensordata after the
+//               inverse, kfdi_sdiff writes row i of one block and, for i = 0, the nominal sensordata.
+struct DevFdSens {
+  DevFd fd;
+  float* snap;                            // [Np][nsd] the sensors of each env's x
+  float *C, *D;                           // [n][nsd][nx], [n][nsd][nu]
+  float* sensordata;                      // [n][nsd] the nominal column's
+};
+FB_WARPFN void kfd_snap(const DevModel& m, const DevData& d, const DevFdSens& p, int e, bool acc) {
+  float* out = p.snap + (size_t)e * m.nsensordata;
+  WPAR_BEGIN
+    for (int s = lane; s < m.nsensor; s += FB_NY)
+      if (sens_acc_stage(m.sensor_type[s]) == acc) for (int k = 0; k < m.sensor_dim[s]; k++) out[m.sensor_adr[s] + k] = AT(d.sensordata, m.sensor_adr[s] + k);
+  WPAR_END
+}
+FB_WARPFN void kfd_sdiff(const DevModel& m, const DevFdSens& p, int w) {
+  const FdCols& c = p.fd;
+  const int pr = w / c.nin, j = w % c.nin, nsd = m.nsensordata, nx = p.fd.nx, nu = c.nin - nx;
+  int a, b; fd_pair(c, pr, j, &a, &b);
+  const float den = c.delta[b] - c.delta[a];
+  float* out = j < nx ? p.C + (size_t)pr * nsd * nx + j : p.D + (size_t)pr * nsd * nu + (j - nx);
+  const int stride = j < nx ? nx : nu;
+  const float *sb = p.snap + (size_t)b * nsd, *sa = p.snap + (size_t)a * nsd;
+  WPAR_BEGIN
+    for (int i = lane; i < nsd; i += FB_NY) out[(size_t)i * stride] = a == b ? 0.0f : (sb[i] - sa[i]) / den;
+    if (j == 0) for (int i = lane; i < nsd; i += FB_NY) p.sensordata[(size_t)pr * nsd + i] = p.snap[(size_t)pr * c.ncol * nsd + i];
+  WPAR_END
+}
+struct DevFdInvSens {
+  DevFdInv fdi;
+  const float* sens;                      // [Np][nsd] every env's sensordata (kinv_sensors on fdi.inv)
+  float *DsDq, *DsDv, *DsDa;              // [n][nv][nsd]: DsDq[i][k] = d sensordata_k / d dq_i
+  float* sensordata;                      // [n][nsd] the nominal column's
+};
+FB_WARPFN void kfdi_sdiff(const DevModel& m, const DevFdInvSens& p, int w) {
+  const FdCols& c = p.fdi;
+  const int nv = m.nv, nsd = m.nsensordata, pr = w / c.nin, i = w % c.nin;
+  int a, b; fd_pair(c, pr, i, &a, &b);
+  const float den = c.delta[b] - c.delta[a];
+  const int blk = i / nv, r = i % nv;
+  float* out = (blk == 0 ? p.DsDq : blk == 1 ? p.DsDv : p.DsDa) + ((size_t)pr * nv + r) * nsd;
+  const float *sb = p.sens + (size_t)b * nsd, *sa = p.sens + (size_t)a * nsd;
+  WPAR_BEGIN
+    for (int k = lane; k < nsd; k += FB_NY) out[k] = (sb[k] - sa[k]) / den;
+    if (i == 0) for (int k = lane; k < nsd; k += FB_NY) p.sensordata[(size_t)pr * nsd + k] = p.sens[(size_t)pr * c.ncol * nsd + k];
+  WPAR_END
+}

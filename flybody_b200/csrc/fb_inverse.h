@@ -92,3 +92,123 @@ FB_WARPFN void kinv_run(const DevModel& m, const DevData& d, const DevInv& p, fl
     }
   WPAR_END
 }
+
+// ---- sensordata under the inverse (fb_query_sensors on).  Its own parameter beside DevInv, so the inverse kernels keep their layout.
+// Velocity-stage sensors (gyro, velocimeter) are copied from what launch_step1 left in the record; the acceleration-stage ones restate
+// the finish kernel's F5 - F9 (mj_rnePostConstraint + mj_sensorAcc) at the problem's qacc and the inverse's efc_force instead of the
+// solver's.  The scratch (contact wrench, delta acceleration and force per body) lives in the warp's shared-memory slice, so the record
+// is only read.  As in the step, xfrc_applied does not enter the force sensors (MuJoCo's cfrc_ext has it).
+struct DevInvSens {
+  DevInv inv;                             // the inverse: its qacc and efc_force
+  float* sensordata;                      // [Np][nsensordata]
+};
+#define FB_INVS_SH(nbody) (18 * (nbody))  // per-warp floats: contact wrench, delta acceleration and force of every body, 6 each
+FB_DEV bool sens_acc_stage(int type) { return type != FB_SENS_GYRO && type != FB_SENS_VELOCIMETER; }
+FB_DEV S6 sh_ld6(const float* a, int b) { S6 s; s.a = v3(a[6 * b], a[6 * b + 1], a[6 * b + 2]); s.l = v3(a[6 * b + 3], a[6 * b + 4], a[6 * b + 5]); return s; }
+FB_DEV void sh_st6(float* a, int b, const S6& s) {
+  a[6 * b] = s.a.x; a[6 * b + 1] = s.a.y; a[6 * b + 2] = s.a.z; a[6 * b + 3] = s.l.x; a[6 * b + 4] = s.l.y; a[6 * b + 5] = s.l.z; }
+// delta_from_parent (fb_constraint.h) with the accelerations qa of the caller
+FB_DEV void inv_delta_from_parent(const DevModel& m, const DevData& d, int e, const float* qa, int b, S6& dl) {
+  for (int kk = 0; kk < m.body_dofnum[b]; kk++) {
+    const int k = m.body_dofadr[b] + kk; const float a = qa[k];
+    dl.a = dl.a + ld3(d.Sang, k, d, e) * a; dl.l = dl.l + ld3(d.Slin, k, d, e) * a;
+  }
+}
+FB_WARPFN void kinv_sensors(const DevModel& m, const DevData& d, const DevInvSens& p, float* sh, int e) {
+  const int nb = m.nbody, ncon = AT(d.ncon, 0);
+  const float* qa = p.inv.qacc + (size_t)e * m.nv;
+  const float* fo = p.inv.efc_force + (size_t)e * FB_MAXEFC;
+  float* out = p.sensordata + (size_t)e * m.nsensordata;
+  float *xw = sh, *bdel = sh + 6 * nb, *bfrc = sh + 12 * nb;
+  // velocity stage; the contact wrenches (F5: lane 0, contacts in order) and the roots' deltas (F6)
+  WPAR_BEGIN
+    for (int s = lane; s < m.nsensor; s += FB_NY)
+      if (!sens_acc_stage(m.sensor_type[s])) for (int k = 0; k < m.sensor_dim[s]; k++) out[m.sensor_adr[s] + k] = AT(d.sensordata, m.sensor_adr[s] + k);
+    for (int k = lane; k < 6 * nb; k += FB_NY) xw[k] = 0.0f;
+  WPAR_END
+  WPAR_BEGIN
+    if (lane == 0) {
+      for (int ci = 0; ci < ncon; ci++) {
+        const int adr = AT(d.con_efcadr, ci); if (adr < 0) continue;
+        const int dim = AT(d.con_dim, ci);
+        V3 F = v3(0, 0, 0);
+        for (int r = 0; r < dim; r++) F = F + v3(CON_F(d.con_frame, ci, 3 * r, 9), CON_F(d.con_frame, ci, 3 * r + 1, 9), CON_F(d.con_frame, ci, 3 * r + 2, 9)) * fo[adr + r];
+        const V3 pos = v3(CON_F(d.con_pos, ci, 0, 3), CON_F(d.con_pos, ci, 1, 3), CON_F(d.con_pos, ci, 2, 3));
+        const V3 tq = cross(pos, F);
+        const int b1 = m.geom_bodyid[AT(d.con_geom1, ci)], b2 = m.geom_bodyid[AT(d.con_geom2, ci)];
+        S6 w2 = sh_ld6(xw, b2); w2.a = w2.a + tq; w2.l = w2.l + F; sh_st6(xw, b2, w2);
+        S6 w1 = sh_ld6(xw, b1); w1.a = w1.a - tq; w1.l = w1.l - F; sh_st6(xw, b1, w1);
+      }
+    }
+    if (lane == 1) for (int r = 0; r < m.nroot; r++) { const int b = m.root_body[r]; S6 dl; dl.a = dl.l = v3(0, 0, 0); inv_delta_from_parent(m, d, e, qa, b, dl); sh_st6(bdel, b, dl); }
+  WPAR_END
+  // F7: the delta-acceleration chains and body forces f_b = f0_b + I_b delta_b - ext_b, one lane per list
+  WPAR_BEGIN
+    const int y = lane;
+    if (y < m.nlist) {
+      int prev = -1; S6 cd; cd.a = cd.l = v3(0, 0, 0);
+      FB_LIST_LOOP_FWD {
+        if (!m.body_sensacc[b]) { prev = -1; continue; }
+        const int pa = m.body_parentid[b];
+        if (pa != prev) cd = sh_ld6(bdel, pa);
+        inv_delta_from_parent(m, d, e, qa, b, cd);
+        sh_st6(bdel, b, cd);
+        prev = b;
+        if (m.body_sensfrc[b]) {
+          I10 I = ld10(d.inert10, b, d, e); V3 L, pm; inert_mul(I, cd.a, cd.l, L, pm);
+          S6 f = ld6(d.bfrc0, b, d, e), x = sh_ld6(xw, b);
+          f.a = f.a + L - x.a; f.l = f.l + pm - x.l;
+          sh_st6(bfrc, b, f);
+        }
+      }
+    }
+  WPAR_END
+  // F8: subtree sums of the force-sensor bodies
+  WPAR_BEGIN
+    const int y = lane;
+    if (y < m.nlist) {
+      FB_LIST_LOOP_REV {
+        if (!m.body_sensfrc[b]) continue;
+        const int pa = m.body_parentid[b];
+        if (!m.body_sensfrc[pa]) continue;
+        S6 f = sh_ld6(bfrc, b), pf = sh_ld6(bfrc, pa);
+        pf.a = pf.a + f.a; pf.l = pf.l + f.l; sh_st6(bfrc, pa, pf);
+      }
+    }
+  WPAR_END
+  // F9: accelerometer, force, touch
+  WPAR_BEGIN
+    for (int s = lane; s < m.nsensor; s += FB_NY) {
+      const int tp = m.sensor_type[s], site = m.sensor_objid[s], adr = m.sensor_adr[s], b = m.site_bodyid[site];
+      if (tp == FB_SENS_ACCELEROMETER) {
+        S6 a = ld6(d.bacc, b, d, e), v = ld6(d.bvel, b, d, e); const S6 dl = sh_ld6(bdel, b);
+        a.a = a.a + dl.a; a.l = a.l + dl.l;
+        const V3 ps = ld3(d.site_xpos, site, d, e);
+        const V3 vp = v.l + cross(v.a, ps);
+        const V3 acc = a.l + cross(a.a, ps) + cross(v.a, vp);
+        const V3 o = mulT(ld9(d.site_xmat, site, d, e), acc);
+        out[adr] = o.x; out[adr + 1] = o.y; out[adr + 2] = o.z;
+      } else if (tp == FB_SENS_FORCE) {
+        const V3 o = mulT(ld9(d.site_xmat, site, d, e), sh_ld6(bfrc, b).l);
+        out[adr] = o.x; out[adr + 1] = o.y; out[adr + 2] = o.z;
+      } else if (tp == FB_SENS_TOUCH) {
+        float sum = 0;
+        for (int ci = 0; ci < ncon; ci++) {
+          const int ea = AT(d.con_efcadr, ci); if (ea < 0) continue;
+          const int b1 = m.geom_bodyid[AT(d.con_geom1, ci)], b2 = m.geom_bodyid[AT(d.con_geom2, ci)];
+          if (b != b1 && b != b2) continue;
+          const float fn = fo[ea]; if (fn <= 0) continue;
+          V3 ray = v3(CON_F(d.con_frame, ci, 0, 9), CON_F(d.con_frame, ci, 1, 9), CON_F(d.con_frame, ci, 2, 9));
+          if (b == b2) ray = ray * -1.0f;
+          const V3 pos = v3(CON_F(d.con_pos, ci, 0, 3), CON_F(d.con_pos, ci, 1, 3), CON_F(d.con_pos, ci, 2, 3));
+          const V3 ssz = mld3(m.site_size, site);
+          float hit;
+          if (m.site_type[site] == FB_GEOM_CAPSULE) hit = ray_capsule(ld3(d.site_xpos, site, d, e), ld9(d.site_xmat, site, d, e), ssz, pos, ray);
+          else { float xx[2]; const V3 dif = pos - ld3(d.site_xpos, site, d, e); hit = ray_quad(dot(ray, ray), dot(ray, dif), dot(dif, dif) - ssz.x * ssz.x, xx); }
+          if (hit >= 0) sum += fn;
+        }
+        out[adr] = sum;
+      }
+    }
+  WPAR_END
+}

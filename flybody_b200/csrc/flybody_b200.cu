@@ -51,6 +51,12 @@ struct FbSim {
   DevInv inv = {}; std::vector<void*> inv_scope; int inv_done = 0;   // inverse dynamics (fb_inverse): buffers, allocated on first use; problems of the last call
   DevFd fd = {}; std::vector<void*> fd_scope; int fd_cap = 0, fd_done = 0;   // transition Jacobians (fb_fd_transition): buffers for fd_cap problems, allocated on first use; problems of the last call
   DevFdInv fdi = {}; std::vector<void*> fdi_scope; int fdi_cap = 0, fdi_done = 0;   // inverse-dynamics Jacobians (fb_fd_inverse): the same, with their own DevInv
+  // sensor outputs of the three dynamics queries (fb_query_sensors): buffers allocated on the first call with sensors on; *_sens: the
+  // last call of that query ran with sensors on
+  int sens_on = 0;
+  float* inv_sd = nullptr; std::vector<void*> inv_sd_scope; bool inv_sens = false;              // fb_inverse: sensordata [Np][nsd]
+  DevFdSens fds = {}; std::vector<void*> fds_scope; bool fd_sens = false;                        // fb_fd_transition: C, D, sensordata
+  DevFdInvSens fdis = {}; float* fdi_env_sd = nullptr; std::vector<void*> fdis_scope; bool fdi_sens = false;   // fb_fd_inverse: every env's sensordata, DsD*
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -2113,8 +2119,27 @@ static int inv_alloc(FbSim* s) {
     s->inv = DevInv{}; return rc; }
   return 0;
 }
+// the sensor pass of an inverse (fb_inverse.h kinv_sensors) over its p.n envs; a model without sensordata launches nothing
+struct InvSensWarp {
+  DevModel m; DevData d; DevInvSens p;
+  FB_DEVM void operator()(unsigned char* sh, int e) const { kinv_sensors(m, d, p, reinterpret_cast<float*>(sh), e); }
+};
+static size_t inv_sens_slice(const FbSim* s) { return slice_bytes(0, FB_INVS_SH(s->m.nbody)); }
+static void launch_inv_sensors(FbSim* s, const DevInv& inv, float* sensordata) {
+  if (s->m.nsensordata > 0) warp_launch(s, "inverse_sensors", inv.n, inv_sens_slice(s), InvSensWarp{s->m, s->d, DevInvSens{inv, sensordata}});
+}
 
 extern "C" {
+
+int fb_query_sensors(FbHandle s, int on) {
+  if (!s) return -1;
+  if (on && inv_sens_slice(s) * FB_WPB > 48 * 1024) {
+    s->err = "fb_query_sensors: the sensor pass keeps 18 floats per body in shared memory, and " + std::to_string(s->m.nbody) + " bodies do not fit";
+    return -1;
+  }
+  s->sens_on = on != 0;
+  return 0;
+}
 
 int fb_inverse(FbHandle s, int n, const float* qacc, int is_device) {
   if (!s) return -1;
@@ -2124,14 +2149,27 @@ int fb_inverse(FbHandle s, int n, const float* qacc, int is_device) {
   if (!is_device) for (size_t i = 0; i < cnt; i++) if (!std::isfinite(qacc[i])) { s->err = "fb_inverse: non-finite qacc"; return -1; }
   dev_select(s);
   if (int rc = inv_alloc(s)) return rc;
+  const bool sens = s->sens_on != 0;
+  if (sens && !s->inv_sd) {
+    if (int rc = scope_alloc(s, s->inv_sd_scope, "out of device memory (inverse sensordata)",
+                             [&] { s->inv_sd = dalloc<float>(s, (size_t)s->d.Np * s->m.nsensordata); })) { s->inv_sd = nullptr; return rc; }
+  }
   DevInv& p = s->inv;
   if (copy_async(s, p.qacc, qacc, sizeof(float) * cnt) != 0) return -2;
   p.n = n;
   launch_step1(s);                             // the position / velocity stage fb_forward runs (sens_mode -1: no sensor sums)
   launch_inv(s, s->inv);
+  if (sens) launch_inv_sensors(s, s->inv, s->inv_sd);
   if (launch_check(s, "fb_inverse") != 0) return -2;
-  s->inv_done = n;
+  s->inv_done = n; s->inv_sens = sens;
   return is_device ? 0 : sync_stream(s);       // a host qacc may be reused once the call returns
+}
+
+int fb_inverse_sensor_read(FbHandle s, float* sensordata, int is_device) {
+  if (!s) return -1;
+  if (s->inv_done < 1) { s->err = "fb_inverse_sensor_read: no inverse to read (fb_inverse)"; return -1; }
+  if (!s->inv_sens) { s->err = "fb_inverse_sensor_read: the last fb_inverse ran with sensors off (fb_query_sensors)"; return -1; }
+  return read_out(s, {{sensordata, s->inv_sd, 0, 4 * (size_t)s->inv_done * s->m.nsensordata, 1}});
 }
 
 int fb_inverse_read(FbHandle s, float* qfrc_inverse, float* qfrc_constraint, float* efc_force, int is_device) {
@@ -2172,6 +2210,25 @@ static int fd_alloc(FbSim* s) {
   s->fd_cap = (int)cap;
   return 0;
 }
+template <bool ACC> struct FdSnap {
+  DevModel m; DevData d; DevFdSens p;
+  FB_DEVM void operator()(unsigned char*, int e) const { kfd_snap(m, d, p, e, ACC); }
+};
+struct FdSDiff {
+  DevModel m; DevFdSens p;
+  FB_DEVM void operator()(unsigned char*, int w) const { kfd_sdiff(m, p, w); }
+};
+static int fds_alloc(FbSim* s) {
+  if (s->fds.snap) return 0;
+  const DevModel& m = s->m;
+  const size_t nsd = m.nsensordata, nx = 2 * (size_t)m.nv + m.na, cap = s->fd_cap;
+  DevFdSens& q = s->fds;
+  if (int rc = scope_alloc(s, s->fds_scope, "out of device memory (transition sensor Jacobians)", [&] {
+        q.snap = dalloc<float>(s, (size_t)s->d.Np * nsd); q.C = dalloc<float>(s, cap * nsd * nx); q.D = dalloc<float>(s, cap * nsd * m.nu);
+        q.sensordata = dalloc<float>(s, cap * nsd); })) {
+    s->fds = DevFdSens{}; return rc; }
+  return 0;
+}
 
 extern "C" {
 
@@ -2193,6 +2250,8 @@ int fb_fd_transition(FbHandle s, const int32_t* slots, int n, float eps, int cen
   }
   dev_select(s);
   if (int rc = fd_alloc(s)) return rc;
+  const bool sens = s->sens_on != 0, snap = sens && s->m.nsensordata > 0;
+  if (sens) if (int rc = fds_alloc(s)) return rc;
   // every env a copy of its problem's row, warm start included; the envs past the problems copy the last problem's
   std::vector<int32_t> fan(N);
   for (int e = 0; e < N; e++) fan[e] = slots[std::min(e / ncol, n - 1)];
@@ -2204,11 +2263,29 @@ int fb_fd_transition(FbHandle s, const int32_t* slots, int n, float eps, int cen
   launch_state<true>(s, nullptr, sd, N);
   warp_launch(s, "fd_perturb", N, 0, FdPerturb{s->m, s->d, p});
   launch_step1(s);                             // the position / velocity stage of the nudged states
-  step_run(s, n_substeps);                     // fb_step's launches
+  if (!snap) {
+    step_run(s, n_substeps);                   // fb_step's launches
+  } else {                                     // the same launches, split after the first substep: the sensors of x
+    DevFdSens& q = s->fds; q.fd = p;
+    warp_launch(s, "fd_snap", n * ncol, 0, FdSnap<false>{s->m, s->d, q});
+    step_run(s, 1);
+    warp_launch(s, "fd_snap", n * ncol, 0, FdSnap<true>{s->m, s->d, q});
+    if (n_substeps > 1) step_run(s, n_substeps - 1);
+  }
   warp_launch(s, "fd_diff", n * p.nin, 0, FdDiff{s->m, s->d, p});
+  if (snap) warp_launch(s, "fd_sdiff", n * p.nin, 0, FdSDiff{s->m, s->fds});
   if (launch_check(s, "fb_fd_transition") != 0) return -2;
-  s->fd_done = n;
+  s->fd_done = n; s->fd_sens = sens;
   return sync_stream(s);                       // (the fan-out list is a host vector)
+}
+
+int fb_fd_sensor_read(FbHandle s, float* C, float* D, float* sensordata, int is_device) {
+  if (!s) return -1;
+  if (s->fd_done < 1) { s->err = "fb_fd_sensor_read: no transition to read (fb_fd_transition)"; return -1; }
+  if (!s->fd_sens) { s->err = "fb_fd_sensor_read: the last fb_fd_transition ran with sensors off (fb_query_sensors)"; return -1; }
+  const DevFdSens& q = s->fds;
+  const size_t n = (size_t)s->fd_done, nsd = (size_t)s->m.nsensordata, nx = (size_t)s->fd.nx, nu = (size_t)(s->fd.nin - s->fd.nx);
+  return read_out(s, {{C, q.C, 0, 4 * n * nsd * nx, 1}, {D, q.D, 0, 4 * n * nsd * nu, 1}, {sensordata, q.sensordata, 0, 4 * n * nsd, 1}});
 }
 
 int fb_fd_read(FbHandle s, float* A, float* B, float* qpos_next, float* qvel_next, float* act_next, int is_device) {
@@ -2250,6 +2327,22 @@ static int fdi_alloc(FbSim* s) {
   s->fdi_cap = (int)cap;
   return 0;
 }
+struct FdiSDiff {
+  DevModel m; DevFdInvSens p;
+  FB_DEVM void operator()(unsigned char*, int w) const { kfdi_sdiff(m, p, w); }
+};
+static int fdis_alloc(FbSim* s) {
+  if (s->fdi_env_sd) return 0;
+  const size_t nsd = s->m.nsensordata, nv = s->m.nv, cap = s->fdi_cap;
+  DevFdInvSens& q = s->fdis;
+  if (int rc = scope_alloc(s, s->fdis_scope, "out of device memory (inverse-dynamics sensor Jacobians)", [&] {
+        s->fdi_env_sd = dalloc<float>(s, (size_t)s->d.Np * nsd);
+        q.DsDq = dalloc<float>(s, cap * nv * nsd); q.DsDv = dalloc<float>(s, cap * nv * nsd); q.DsDa = dalloc<float>(s, cap * nv * nsd);
+        q.sensordata = dalloc<float>(s, cap * nsd); })) {
+    s->fdis = DevFdInvSens{}; s->fdi_env_sd = nullptr; return rc; }
+  q.sens = s->fdi_env_sd;
+  return 0;
+}
 
 extern "C" {
 
@@ -2272,6 +2365,8 @@ int fb_fd_inverse(FbHandle s, int n, const float* qpos, const float* qvel, const
   if (!(eps > 0.0f) || !std::isfinite(eps)) { s->err = "fb_fd_inverse: eps must be positive and finite"; return -1; }
   dev_select(s);
   if (int rc = fdi_alloc(s)) return rc;
+  const bool sens = s->sens_on != 0, sdiff = sens && s->m.nsensordata > 0;
+  if (sens) if (int rc = fdis_alloc(s)) return rc;
   DevFdInv& p = s->fdi;
   if (copy_async(s, p.qpos, qpos, sizeof(float) * n * nq) != 0 || copy_async(s, p.qvel, qvel, sizeof(float) * n * nv) != 0 ||
       copy_async(s, p.qacc, qacc, sizeof(float) * n * nv) != 0) return -2;
@@ -2281,10 +2376,22 @@ int fb_fd_inverse(FbHandle s, int n, const float* qpos, const float* qvel, const
   warp_launch(s, "fdi_perturb", N, 0, FdiPerturb{s->m, s->d, p});   // fan-out and nudge
   launch_step1(s);                             // the position / velocity stage of every env, as fb_inverse runs it
   launch_inv(s, p.inv);
+  if (sdiff) launch_inv_sensors(s, p.inv, s->fdi_env_sd);
   warp_launch(s, "fdi_diff", n * p.nin, 0, FdiDiff{s->m, s->d, p});
+  if (sdiff) { s->fdis.fdi = p; warp_launch(s, "fdi_sdiff", n * p.nin, 0, FdiSDiff{s->m, s->fdis}); }
   if (launch_check(s, "fb_fd_inverse") != 0) return -2;
-  s->fdi_done = n;
+  s->fdi_done = n; s->fdi_sens = sens;
   return is_device ? 0 : sync_stream(s);       // host rows may be reused once the call returns
+}
+
+int fb_fd_inverse_sensor_read(FbHandle s, float* DsDq, float* DsDv, float* DsDa, float* sensordata, int is_device) {
+  if (!s) return -1;
+  if (s->fdi_done < 1) { s->err = "fb_fd_inverse_sensor_read: no Jacobians to read (fb_fd_inverse)"; return -1; }
+  if (!s->fdi_sens) { s->err = "fb_fd_inverse_sensor_read: the last fb_fd_inverse ran with sensors off (fb_query_sensors)"; return -1; }
+  const DevFdInvSens& q = s->fdis;
+  const size_t n = (size_t)s->fdi_done, nv = (size_t)s->m.nv, nsd = (size_t)s->m.nsensordata;
+  return read_out(s, {{DsDq, q.DsDq, 0, 4 * n * nv * nsd, 1}, {DsDv, q.DsDv, 0, 4 * n * nv * nsd, 1}, {DsDa, q.DsDa, 0, 4 * n * nv * nsd, 1},
+                      {sensordata, q.sensordata, 0, 4 * n * nsd, 1}});
 }
 
 int fb_fd_inverse_read(FbHandle s, float* DfDq, float* DfDv, float* DfDa, float* DmDq, float* qfrc_inverse, int is_device) {

@@ -35,14 +35,18 @@ ENVS = 4096          # envs of the handle: max(1, ENVS // columns) problems per 
 
 Transition = namedtuple('Transition', ['A', 'B', 'qpos_next', 'qvel_next', 'act_next'])
 InverseJacobians = namedtuple('InverseJacobians', ['DfDq', 'DfDv', 'DfDa', 'DmDq', 'qfrc_inverse'])
+TransitionSensors = namedtuple('TransitionSensors', Transition._fields + ('C', 'D', 'sensordata'))
+InverseSensorJacobians = namedtuple('InverseSensorJacobians', InverseJacobians._fields + ('DsDq', 'DsDv', 'DsDa', 'sensordata'))
 
 
-def transition_fd(model, qpos, qvel, ctrl, act=None, eps=1e-2, centered=True, n_substeps=1, device=0, lib_path=None):
+def transition_fd(model, qpos, qvel, ctrl, act=None, eps=1e-2, centered=True, n_substeps=1, device=0, lib_path=None, sensors=False):
     """A = dx'/dx [B, nx, nx] and B = dx'/du [B, nx, nu] (row-major, as MuJoCo's) of B states qpos [B, nq], qvel [B, nv], ctrl [B, nu],
     act [B, na] (zeros when None), or of one state without the batch dimension; nx = 2 nv + na.
 
     Returns Transition(A, B, qpos_next, qvel_next, act_next) as fp64 arrays of the device's fp32 values; *_next is the unperturbed
-    state after the n_substeps substeps."""
+    state after the n_substeps substeps.  sensors=True returns TransitionSensors, the same followed by MuJoCo's C = ds/dx [B, nsd, nx],
+    D = ds/du [B, nsd, nu] and the nominal sensordata [B, nsd], s the sensors of x, the state before the step (columns in the model's
+    sensor_adr order).  That holds for every n_substeps: C and D are not derivatives of the substep-mean sensors a policy observes."""
     m = model
     ncol = 1 + (2 if centered else 1) * (2 * m.nv + m.na + m.nu)
     per = max(1, ENVS // ncol)
@@ -57,31 +61,41 @@ def transition_fd(model, qpos, qvel, ctrl, act=None, eps=1e-2, centered=True, n_
         sim.forward()
         sim.save_state(slots=np.arange(k), env_ids=np.arange(k))
         sim.fd_transition(np.arange(k), eps=eps, centered=centered, n_substeps=n_substeps)
-        return sim.fd_read()
+        return sim.fd_read() + (sim.fd_sensor_read() if sensors else ())
 
     act = np.zeros(np.shape(qpos)[:-1] + (m.na,)) if act is None else act
     single, out = st._batched(m, [('qpos', qpos, (m.nq,)), ('qvel', qvel, (m.nv,)), ('ctrl', ctrl, (m.nu,)), ('act', act, (m.na,))], run,
-                              per, n_envs=per * ncol, setup=lambda sim: sim.state_bank(per), device=device, lib_path=lib_path)
-    res = Transition(*(x.astype(np.float64) for x in out))
-    return Transition(*(x[0] for x in res)) if single else res
+                              per, n_envs=per * ncol, setup=lambda sim: _setup(sim, per, sensors), device=device, lib_path=lib_path)
+    kind = TransitionSensors if sensors else Transition
+    res = kind(*(x.astype(np.float64) for x in out))
+    return kind(*(x[0] for x in res)) if single else res
 
 
-def inverse_fd(model, qpos, qvel, qacc, eps=1e-2, centered=True, device=0, lib_path=None):
+def _setup(sim, slots, sensors):
+    sim.state_bank(slots)
+    if sensors:
+        sim.query_sensors(True)
+
+
+def inverse_fd(model, qpos, qvel, qacc, eps=1e-2, centered=True, device=0, lib_path=None, sensors=False):
     """The inverse-dynamics Jacobians of B states qpos [B, nq], qvel [B, nv], qacc [B, nv], or of one state without the batch dimension.
 
     Returns InverseJacobians(DfDq, DfDv, DfDa, DmDq, qfrc_inverse) as fp64 arrays of the device's fp32 values, transposed as MuJoCo's
     mjd_inverseFD: DfDq [B, nv, nv] with DfDq[p, i, j] = d qfrc_inverse_j / d dq_i (dq: the tangent of qpos), DfDv and DfDa likewise
     for qvel and qacc, DmDq [B, nv, nM] = d qM / d dq_i in MuJoCo's sparse qM order (the diagonal at dof_Madr, then the ancestors), and
-    the unperturbed qfrc_inverse [B, nv].  centered=False is MuJoCo's forward difference."""
+    the unperturbed qfrc_inverse [B, nv].  centered=False is MuJoCo's forward difference.  sensors=True returns InverseSensorJacobians,
+    the same followed by DsDq, DsDv, DsDa [B, nv, nsd] (transposed alike: DsDq[p, i, k] = d sensordata_k / d dq_i) of the sensordata
+    `inverse_dynamics.inverse(..., sensors=True)` returns, and the nominal sensordata [B, nsd]."""
     m = model
     ncol = 1 + (2 if centered else 1) * 3 * m.nv
     per = max(1, ENVS // ncol)
 
     def run(sim, rows, k):
         sim.fd_inverse(*rows, eps=eps, centered=centered)
-        return sim.fd_inverse_read()
+        return sim.fd_inverse_read() + (sim.fd_inverse_sensor_read() if sensors else ())
 
     single, out = st._batched(m, [('qpos', qpos, (m.nq,)), ('qvel', qvel, (m.nv,)), ('qacc', qacc, (m.nv,))], run, per, n_envs=per * ncol,
-                              device=device, lib_path=lib_path)
-    res = InverseJacobians(*(x.astype(np.float64) for x in out))
-    return InverseJacobians(*(x[0] for x in res)) if single else res
+                              setup=(lambda sim: sim.query_sensors(True)) if sensors else None, device=device, lib_path=lib_path)
+    kind = InverseSensorJacobians if sensors else InverseJacobians
+    res = kind(*(x.astype(np.float64) for x in out))
+    return kind(*(x[0] for x in res)) if single else res

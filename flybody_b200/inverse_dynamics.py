@@ -17,17 +17,20 @@ from . import stepper as st
 from .inverse_kinematics import CHUNK, HINGE, _differentiate_pos
 
 InverseResult = namedtuple('InverseResult', ['qfrc_inverse', 'qfrc_constraint', 'qfrc_bias', 'qfrc_passive', 'contacts'])
+InverseSensorResult = namedtuple('InverseSensorResult', InverseResult._fields + ('sensordata',))
 # per problem: the contacts that have constraint rows; force holds mj_contactForce's six numbers for an elliptic cone (contact frame:
 # normal, then the two tangent directions, then torques, which the fly's condim <= 3 contacts leave at 0)
 Contacts = namedtuple('Contacts', ['geom', 'pos', 'normal', 'force'])
 
 
-def inverse(model, qpos, qvel, qacc, device=0, lib_path=None):
+def inverse(model, qpos, qvel, qacc, device=0, lib_path=None, sensors=False):
     """mj_inverse of B states: qpos [B, nq], qvel [B, nv], qacc [B, nv] (or one state without the batch dimension).
 
     Returns InverseResult(qfrc_inverse, qfrc_constraint, qfrc_bias, qfrc_passive, contacts): four [B, nv] fp64 arrays of the device's
     fp32 values, and per problem a `Contacts` of its k contacts with rows: geom [k, 2] geom ids, pos [k, 3] world position, normal
-    [k, 3], force [k, 6] in the contact frame."""
+    [k, 3], force [k, 6] in the contact frame.  sensors=True returns InverseSensorResult, the same followed by sensordata [B, nsd]
+    (columns in the model's sensor_adr order), evaluated as mj_inverse does: gyro and velocimeter of the state, accelerometer, force
+    and touch at the given qacc and the inverse's contact forces (xfrc_applied does not enter the force sensors, as in the step)."""
     def run(sim, rows, n):
         q, v, a = rows
         pad = np.minimum(np.arange(sim.n_envs), n - 1)         # the chunk's states, the last one repeated
@@ -35,6 +38,7 @@ def inverse(model, qpos, qvel, qacc, device=0, lib_path=None):
         sim.set(st.QVEL, v[pad])
         sim.inverse(a)
         qi, qc, f = sim.inverse_read()
+        sd = (sim.inverse_sensor_read(),) if sensors else ()
         con, ncon = sim.get(st.CONTACT).reshape(sim.n_envs, st.MAXCON, 16), sim.get(st.NCON)[:, 0].astype(int)
         contacts = []
         for i in range(n):
@@ -45,12 +49,13 @@ def inverse(model, qpos, qvel, qacc, device=0, lib_path=None):
                 adr, dim = int(row[12]), int(row[9])
                 force[k, :dim] = f[i, adr:adr + dim]
             contacts.append(Contacts(c[:, 7:9].astype(np.int64), c[:, 1:4].astype(np.float64), c[:, 4:7].astype(np.float64), force))
-        return qi, qc, sim.get(st.QFRC_BIAS)[:n], sim.get(st.QFRC_PASSIVE)[:n], contacts
+        return (qi, qc, sim.get(st.QFRC_BIAS)[:n], sim.get(st.QFRC_PASSIVE)[:n], contacts) + sd
 
     single, out = st._batched(model, [('qpos', qpos, (model.nq,)), ('qvel', qvel, (model.nv,)), ('qacc', qacc, (model.nv,))], run, CHUNK,
-                              device=device, lib_path=lib_path)
-    res = InverseResult(*(x.astype(np.float64) for x in out[:4]), out[4])
-    return InverseResult(*(x[0] for x in res)) if single else res
+                              setup=(lambda sim: sim.query_sensors(True)) if sensors else None, device=device, lib_path=lib_path)
+    kind = InverseSensorResult if sensors else InverseResult
+    res = kind(*(x.astype(np.float64) for x in out[:4]), out[4], *(x.astype(np.float64) for x in out[5:]))
+    return kind(*(x[0] for x in res)) if single else res
 
 
 def differentiate(model, qpos_track, dt):

@@ -30,6 +30,7 @@ EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl'
            'fb_state_slots', 'fb_state_signature', 'fb_state_bank', 'fb_state_save', 'fb_state_load', 'fb_state_read', 'fb_state_write', 'fb_state_substeps',
            'fb_ik_program', 'fb_ik_solve', 'fb_ik_read', 'fb_inverse', 'fb_inverse_read',
            'fb_fd_columns', 'fb_fd_transition', 'fb_fd_read', 'fb_fd_inverse_columns', 'fb_fd_inverse', 'fb_fd_inverse_read',
+           'fb_query_sensors', 'fb_inverse_sensor_read', 'fb_fd_sensor_read', 'fb_fd_inverse_sensor_read',
            'fb_param_size', 'fb_param_set', 'fb_param_get', 'fb_param_draws', 'fb_param_clear']
 
 
@@ -182,6 +183,10 @@ def load_library(path=None):
     lib.fb_fd_inverse_columns.argtypes = [C.c_void_p, C.c_int]
     lib.fb_fd_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int]
     lib.fb_fd_inverse_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_int]
+    lib.fb_query_sensors.argtypes = [C.c_void_p, C.c_int]
+    lib.fb_inverse_sensor_read.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    lib.fb_fd_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 3 + [C.c_int]
+    lib.fb_fd_inverse_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int]
     lib.fb_param_size.argtypes = [C.c_void_p, C.c_int]
     lib.fb_param_set.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
     lib.fb_param_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
@@ -492,6 +497,34 @@ class BatchedStepper:
         out = [np.zeros((n, m.nv, m.nv), np.float32) for _ in range(3)]
         out += [np.zeros((n, m.nv, int(m.nM)), np.float32), np.zeros((n, m.nv), np.float32)]
         self._check(self._lib.fb_fd_inverse_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_inverse_read')
+        return tuple(out)
+
+    # ---- sensors in the dynamics queries (fb_query_sensors; see the header)
+    def query_sensors(self, on=True):
+        """while on, inverse, fd_transition and fd_inverse also produce sensor outputs (read with the *_sensor_read calls)"""
+        self._check(self._lib.fb_query_sensors(self._h, int(bool(on))), 'fb_query_sensors')
+
+    def inverse_sensor_read(self):
+        """-> sensordata [n, nsd] f32 of the last inverse (run with sensors on)"""
+        out = np.zeros((getattr(self, '_inv_n', 0), self.model.nsensordata), np.float32)
+        self._check(self._lib.fb_inverse_sensor_read(self._h, out.ctypes.data, 0), 'fb_inverse_sensor_read')
+        return out
+
+    def fd_sensor_read(self):
+        """-> (C [n, nsd, nx], D [n, nsd, nu], sensordata [n, nsd]) f32 of the last fd_transition (run with sensors on): the sensors
+        of the state before the step and their derivatives"""
+        m, n = self.model, getattr(self, '_fd_n', 0)
+        nsd = m.nsensordata
+        out = [np.zeros((n, nsd, 2 * m.nv + m.na), np.float32), np.zeros((n, nsd, m.nu), np.float32), np.zeros((n, nsd), np.float32)]
+        self._check(self._lib.fb_fd_sensor_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_sensor_read')
+        return tuple(out)
+
+    def fd_inverse_sensor_read(self):
+        """-> (DsDq, DsDv, DsDa [n, nv, nsd], sensordata [n, nsd]) f32 of the last fd_inverse (run with sensors on), transposed as
+        MuJoCo's: DsDq[p, i, k] = d sensordata_k / d dq_i"""
+        m, n = self.model, getattr(self, '_fdi_n', 0)
+        out = [np.zeros((n, m.nv, m.nsensordata), np.float32) for _ in range(3)] + [np.zeros((n, m.nsensordata), np.float32)]
+        self._check(self._lib.fb_fd_inverse_sensor_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_inverse_sensor_read')
         return tuple(out)
 
     def reset(self, qpos=None, qvel=None, env_ids=None):

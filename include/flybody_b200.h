@@ -557,7 +557,7 @@ int fb_inverse(FbHandle h, int n, const float* qacc, int is_device);
  * memory): qfrc_inverse [n][nv], qfrc_constraint [n][nv], efc_force [n][fb_field_size(FB_EFC_FORCE)], rows as FB_CONTACT's efc_adr
  * and FB_NEFC index them after the call (rows >= nefc hold 0).  An error before the first fb_inverse.                         */
 int fb_inverse_read(FbHandle h, float* qfrc_inverse, float* qfrc_constraint, float* efc_force, int is_device);
-/* Finite-difference transition Jacobians (MuJoCo mjd_transitionFD without sensors; dm_control `mjlib.mjd_transitionFD`):
+/* Finite-difference transition Jacobians (MuJoCo mjd_transitionFD; C and D: fb_query_sensors; dm_control `mjlib.mjd_transitionFD`):
  *   A [nx][nx] = dx'/dx and B [nx][nu] = dx'/du, row-major as MuJoCo's, x = (dq [nv], qvel [nv], act [na]) with dq the tangent of qpos
  *   (mj_integratePos to nudge, mj_differentiatePos to difference), nx = 2 nv + na, u = ctrl [nu];
  *   x' = the state after n_substeps substeps (mj_step2; mj_step1: fb_step's launches) with ctrl held fixed; n_substeps = 1 is
@@ -580,7 +580,7 @@ int fb_fd_transition(FbHandle h, const int32_t* slots, int n, float eps, int cen
  * memory): A [n][nx][nx], B [n][nx][nu], and the nominal column's next state qpos_next [n][nq], qvel_next [n][nv], act_next [n][na].
  * An error before the first fb_fd_transition.                                                                                        */
 int fb_fd_read(FbHandle h, float* A, float* B, float* qpos_next, float* qvel_next, float* act_next, int is_device);
-/* Finite-difference inverse-dynamics Jacobians (MuJoCo mjd_inverseFD with flg_actuation = 0, without sensors): the derivatives of
+/* Finite-difference inverse-dynamics Jacobians (MuJoCo mjd_inverseFD with flg_actuation = 0; DsD*: fb_query_sensors): the derivatives of
  * fb_inverse's qfrc_inverse = M qacc + qfrc_bias - qfrc_passive - qfrc_constraint, and of qM, with respect to the inputs
  * (dq [nv], qvel [nv], qacc [nv]), dq the tangent of qpos (mj_integratePos to nudge).  The outputs are TRANSPOSED, as MuJoCo's
  * ("all outputs are transposed"), and so the transpose of fb_fd_transition's row-major A and B: row i is the derivative with respect
@@ -606,6 +606,26 @@ int fb_fd_inverse(FbHandle h, int n, const float* qpos, const float* qvel, const
  * memory): DfDq, DfDv, DfDa [n][nv][nv], DmDq [n][nv][nM] and the nominal column's qfrc_inverse [n][nv].  An error before the first
  * fb_fd_inverse.                                                                                                                     */
 int fb_fd_inverse_read(FbHandle h, float* DfDq, float* DfDv, float* DfDa, float* DmDq, float* qfrc_inverse, int is_device);
+/* Sensors in the dynamics queries.  While fb_query_sensors(h, 1) is on, fb_inverse, fb_fd_transition and fb_fd_inverse also produce
+ * sensor outputs, columns in the model's sensor_adr order (nsd = nsensordata); while it is off (the default) they launch exactly the
+ * kernels they launch without it.  Either way their other outputs, the record after fb_inverse and the state bank are bit for bit
+ * the same.  Its buffers are allocated on the first call with sensors on.  A model with nsensordata = 0 launches nothing more and
+ * reads empty outputs.  Errors: a model whose sensor pass (18 floats per body per warp) does not fit in shared memory.
+ *   fb_inverse:       sensordata [n][nsd] as MuJoCo's mj_inverse evaluates it: gyro and velocimeter of the state; accelerometer,
+ *                     force and touch of the finish kernel's sensor pass at the given qacc and the inverse's efc_force (touch: the
+ *                     normal forces of the contacts whose ray hits the site volume).  As in the step, xfrc_applied does not enter
+ *                     the force sensors (MuJoCo's cfrc_ext has it); on a noslip model touch and force are the soft model's.
+ *   fb_fd_transition: C [n][nsd][nx] = ds/dx and D [n][nsd][nu] = ds/du, row-major as A and B, s the sensors of x, the state before
+ *                     the step (MuJoCo's mjd_transitionFD), for any n_substeps: not the substep mean a policy observes.  The first
+ *                     substep is launched on its own (the same launches), and the nominal sensordata [n][nsd] is that of x.
+ *   fb_fd_inverse:    DsDq, DsDv, DsDa [n][nv][nsd], transposed as DfD* (DsDq[i][k] = d sensordata_k / d dq_i), of the inverse's
+ *                     sensordata, and the nominal column's sensordata [n][nsd].                                              */
+int fb_query_sensors(FbHandle h, int on);
+/* The sensor outputs of the last call of each query (synchronises; any pointer may be NULL; is_device: the pointers are device memory).
+ * Errors: a read before any call of the query, a read after a call made with sensors off.                                      */
+int fb_inverse_sensor_read(FbHandle h, float* sensordata, int is_device);
+int fb_fd_sensor_read(FbHandle h, float* C, float* D, float* sensordata, int is_device);
+int fb_fd_inverse_sensor_read(FbHandle h, float* DsDq, float* DsDv, float* DsDa, float* sensordata, int is_device);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
