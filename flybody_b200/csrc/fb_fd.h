@@ -1,5 +1,6 @@
 // fb_fd.h -- batched finite-difference Jacobians: of the stepper's transition (MuJoCo mjd_transitionFD / mjd_stepFD; DevFd) and of
-// the inverse dynamics (mjd_inverseFD with flg_actuation = 0; DevFdInv).  Both use one column scheme (FdCols):
+// the inverse dynamics (mjd_inverseFD with flg_actuation = 0; DevFdInv), and of both with respect to the per-env model parameters
+// (DevFdPrm, DevFdPrmInv; below).  All use one column scheme (FdCols):
 //
 // One problem occupies ncol consecutive envs.  Column 0 is the nominal; column c > 0 nudges one input j: centred, columns 1 + 2j / 2 + 2j
 // by +delta / -delta; forward, column 1 + j by +delta.  delta_j = eps max(1, |x_j|), with x_j the hinge angle, the free joint's
@@ -39,6 +40,10 @@ FB_DEV int fd_input(const FdCols& p, int c, int* dir) {
   if (c == 0) { *dir = 0; return -1; }
   if (p.centered) { *dir = ((c - 1) & 1) ? -1 : 1; return (c - 1) >> 1; }
   *dir = 1; return c - 1;
+}
+// the signed step of a ranged input (MuJoCo's ctrl rule): fwd / back tell whether x + delta / x - delta (with x) lie in the range
+FB_DEV float fd_ranged_step(const FdCols& p, int dir, float delta, bool fwd, bool back) {
+  return p.centered ? (dir > 0 ? (fwd ? delta : 0.0f) : (back ? -delta : 0.0f)) : (fwd ? delta : (back ? -delta : 0.0f));
 }
 FB_DEV bool fd_ctrl_in_range(const DevModel& m, int i, float a, float b) {
   if (!MLD(m.actuator_ctrllimited[i])) return true;
@@ -96,7 +101,7 @@ FB_WARPFN void kfd_perturb(const DevModel& m, const DevData& d, const DevFd& p, 
           const int i = j - p.nx;
           const bool fwd = fd_ctrl_in_range(m, i, *x, *x + delta);
           const bool back = (p.centered || !fwd) && fd_ctrl_in_range(m, i, *x - delta, *x);
-          return p.centered ? (dir > 0 ? (fwd ? delta : 0.0f) : (back ? -delta : 0.0f)) : (fwd ? delta : (back ? -delta : 0.0f));
+          return fd_ranged_step(p, dir, delta, fwd, back);
         });
       }
       p.delta[e] = step;
@@ -241,5 +246,119 @@ FB_WARPFN void kfdi_sdiff(const DevModel& m, const DevFdInvSens& p, int w) {
   WPAR_BEGIN
     for (int k = lane; k < nsd; k += FB_NY) out[k] = (sb[k] - sa[k]) / den;
     if (i == 0) for (int k = lane; k < nsd; k += FB_NY) p.sensordata[(size_t)pr * nsd + k] = p.sens[(size_t)pr * c.ncol * nsd + k];
+  WPAR_END
+}
+
+// ---- parameter Jacobians (fb_fd_param_*): the inputs are directions in the model-parameter overlay (DevData::prm) instead of the
+// state.  The host resolves a direction program (fb_fd_param_program) to overlay slots once, so the kernels know nothing of the field
+// layout.  An element direction nudges one slot by delta = eps max(|theta|, floor) (the column: d / d theta); a scale direction
+// multiplies each of its slots by (1 +- eps) (the column: d / ds at s = 1 of theta <- s theta).  A dof_damping entry also writes the
+// row's derived M_damp slot (as kprm_draw).  The range rule is the ctrl rule (fd_ranged_step) on [0, inf) for the non-negative fields;
+// a scale direction (0 < eps < 1) never leaves it.  The columns (FdCols, nin = k directions) and fd_pair are the state columns'.
+//   transition: kfdp_perturb nudges the fanned-out rows' overlay in place; kfdp_diff writes column j of dxdp [n][nx][k] (row-major as
+//               B, fd_state_diff) and, for j = 0, the nominal next state; the sensors reuse kfd_snap and kfd_sdiff (DevFdSens with
+//               nx = 0: dsdp [n][nsd][k] in the D slot).
+//   inverse:    kfdpi_rows saves env pr's overlay row for problem pr (the fan-out overwrites it); kfdpi_perturb writes an env's
+//               qpos, qvel, qacc and row and nudges it; kfdpi_diff writes row j of DfDp [n][k][nv] (transposed as DfDq) and of DsDp
+//               [n][k][nsd], and for j = 0 the nominal qfrc_inverse and sensordata.
+enum { FB_FD_ELEMENT = 0, FB_FD_SCALE = 1 };
+struct DevFdPrmProg {
+  const int* kind;                        // [k] FB_FD_ELEMENT / FB_FD_SCALE
+  const int* ptr;                         // [k + 1] direction j's entries ptr[j] .. ptr[j + 1] - 1 (an element direction has one)
+  const int *slot, *mslot, *nonneg;       // per entry: the overlay slot, the derived M_damp slot (-1: none), a non-negative field
+  const float* floor;                     // per entry: the floor of an element direction's step
+};
+struct DevFdPrm : FdCols {
+  DevFdPrmProg g;
+  int nx;                                 // 2 nv + na
+  float* dxdp;                            // [n][nx][k]
+  float* next;                            // [n][nq + nv + na] the nominal column's next qpos, qvel, act
+};
+// the signed step of direction j of an env whose overlay row is `row` (every lane computes the same)
+FB_DEV float fdp_step(const FdCols& p, const DevFdPrmProg& g, const float* row, int j, int dir) {
+  if (g.kind[j] == FB_FD_SCALE) return dir * p.eps;
+  const int t = g.ptr[j];
+  const float x = row[g.slot[t]], delta = p.eps * fmaxf(fabsf(x), g.floor[t]);
+  const bool nn = g.nonneg[t] != 0, fwd = !nn || x + delta >= 0.0f;
+  const bool back = (p.centered || !fwd) && (!nn || x - delta >= 0.0f);
+  return fd_ranged_step(p, dir, delta, fwd, back);
+}
+// lane's share of moving direction j of `row` by the step s
+FB_DEV void fdp_apply(const DevFdPrmProg& g, float* row, int j, float s, int lane) {
+  const bool scale = g.kind[j] == FB_FD_SCALE;
+  for (int t = g.ptr[j] + lane; t < g.ptr[j + 1]; t += FB_NY) {
+    const float v = row[g.slot[t]], w = scale ? fmaf(v, s, v) : v + s;
+    row[g.slot[t]] = w;
+    if (g.mslot[t] >= 0) row[g.mslot[t]] = w;
+  }
+}
+// nudge env e's overlay row for its column and record the step in delta
+FB_WARPFN void fdp_nudge_row(const DevData& d, const FdCols& p, const DevFdPrmProg& g, int e) {
+  float* row = d.prm + (size_t)e * d.prm_stride;
+  int dir = 0;
+  const int j = e < p.n * p.ncol ? fd_input(p, e % p.ncol, &dir) : -1;
+  float s = 0.0f;
+  WPAR_BEGIN s = j < 0 ? 0.0f : fdp_step(p, g, row, j, dir); WPAR_END      // (every lane reads the row before any writes it)
+  WPAR_BEGIN
+    if (s != 0.0f) fdp_apply(g, row, j, s, lane);
+    if (lane == 0) p.delta[e] = s;
+  WPAR_END
+}
+FB_WARPFN void kfdp_perturb(const DevData& d, const DevFdPrm& p, int e) { fdp_nudge_row(d, p, p.g, e); }
+FB_WARPFN void kfdp_diff(const DevModel& m, const DevData& d, const DevFdPrm& p, int w) {
+  const int pr = w / p.nin, j = w % p.nin, e0 = pr * p.ncol;
+  int a, b; fd_pair(p, pr, j, &a, &b);
+  const float den = p.delta[b] - p.delta[a];
+  float* out = p.dxdp + (size_t)pr * p.nx * p.nin + j;
+  const int nq = m.nq, nv = m.nv, nnext = nq + nv + m.na;
+  WPAR_BEGIN
+    for (int i = lane; i < p.nx; i += FB_NY) out[(size_t)i * p.nin] = a == b ? 0.0f : fd_state_diff(m, d, b, a, i) / den;
+    if (j == 0) {
+      float* nx = p.next + (size_t)pr * nnext;
+      const int e = e0;
+      for (int i = lane; i < nnext; i += FB_NY) nx[i] = i < nq ? AT(d.qpos, i) : (i < nq + nv ? AT(d.qvel, i - nq) : AT(d.act, i - nq - nv));
+    }
+  WPAR_END
+}
+
+struct DevFdPrmInv : FdCols {
+  DevFdPrmProg g;
+  const float *qpos, *qvel, *qacc;        // [cap][nq], [cap][nv], [cap][nv] the problems
+  float* rows;                            // [cap][prm_stride] problem pr's overlay row: env pr's at call time
+  DevInv inv;                             // the inverse kernel's parameter (inv.qacc: every env's qacc)
+  float* DfDp;                            // [n][k][nv]: DfDp[j][i] = d qfrc_inverse_i / d direction j
+  float* qfrc;                            // [n][nv] the nominal column's qfrc_inverse
+  const float* sens;                      // [Np][nsd] every env's sensordata (kinv_sensors), nullptr: sensors off
+  float *DsDp, *sensordata;               // [n][k][nsd], [n][nsd]
+};
+FB_WARPFN void kfdpi_rows(const DevData& d, const DevFdPrmInv& p, int pr) {
+  const unsigned P = d.prm_stride;
+  WPAR_BEGIN for (unsigned t = lane; t < P; t += FB_NY) p.rows[(size_t)pr * P + t] = d.prm[(size_t)pr * P + t]; WPAR_END
+}
+FB_WARPFN void kfdpi_perturb(const DevModel& m, const DevData& d, const DevFdPrmInv& p, int e) {
+  const int nq = m.nq, nv = m.nv, pr = e / p.ncol < p.n ? e / p.ncol : p.n - 1;
+  const unsigned P = d.prm_stride;
+  WPAR_BEGIN
+    for (int i = lane; i < nq; i += FB_NY) AT(d.qpos, i) = p.qpos[(size_t)pr * nq + i];
+    for (int i = lane; i < nv; i += FB_NY) { AT(d.qvel, i) = p.qvel[(size_t)pr * nv + i]; p.inv.qacc[(size_t)e * nv + i] = p.qacc[(size_t)pr * nv + i]; }
+    for (unsigned t = lane; t < P; t += FB_NY) d.prm[(size_t)e * P + t] = p.rows[(size_t)pr * P + t];
+  WPAR_END
+  fdp_nudge_row(d, p, p.g, e);
+}
+FB_WARPFN void kfdpi_diff(const DevModel& m, const DevFdPrmInv& p, int w) {
+  const int nv = m.nv, nsd = m.nsensordata, pr = w / p.nin, j = w % p.nin, e0 = pr * p.ncol;
+  int a, b; fd_pair(p, pr, j, &a, &b);
+  const float den = p.delta[b] - p.delta[a];
+  float* out = p.DfDp + ((size_t)pr * p.nin + j) * nv;
+  const float *fb = p.inv.qfrc_inverse + (size_t)b * nv, *fa = p.inv.qfrc_inverse + (size_t)a * nv;
+  WPAR_BEGIN
+    for (int k = lane; k < nv; k += FB_NY) out[k] = a == b ? 0.0f : (fb[k] - fa[k]) / den;
+    if (j == 0) for (int k = lane; k < nv; k += FB_NY) p.qfrc[(size_t)pr * nv + k] = p.inv.qfrc_inverse[(size_t)e0 * nv + k];
+    if (p.sens) {
+      float* so = p.DsDp + ((size_t)pr * p.nin + j) * nsd;
+      const float *sb = p.sens + (size_t)b * nsd, *sa = p.sens + (size_t)a * nsd;
+      for (int k = lane; k < nsd; k += FB_NY) so[k] = a == b ? 0.0f : (sb[k] - sa[k]) / den;
+      if (j == 0) for (int k = lane; k < nsd; k += FB_NY) p.sensordata[(size_t)pr * nsd + k] = p.sens[(size_t)e0 * nsd + k];
+    }
   WPAR_END
 }

@@ -57,6 +57,13 @@ struct FbSim {
   float* inv_sd = nullptr; std::vector<void*> inv_sd_scope; bool inv_sens = false;              // fb_inverse: sensordata [Np][nsd]
   DevFdSens fds = {}; std::vector<void*> fds_scope; bool fd_sens = false;                        // fb_fd_transition: C, D, sensordata
   DevFdInvSens fdis = {}; float* fdi_env_sd = nullptr; std::vector<void*> fdis_scope; bool fdi_sens = false;   // fb_fd_inverse: every env's sensordata, DsD*
+  // parameter Jacobians (fb_fd_param_*): the direction program (k directions, any scale among them) and its device tables; the
+  // transition's and the inverse's buffers, allocated on first use for any program (n k < n ncol <= n_envs); problems of the last call
+  DevFdPrmProg fdp_prog = {}; std::vector<void*> fdp_prog_scope; int fdp_k = 0; bool fdp_scale = false;
+  DevFdPrm fdp = {}; std::vector<void*> fdp_scope; int fdp_done = 0; bool fdp_sens = false;
+  DevFdSens fdps = {}; std::vector<void*> fdps_scope;                    // its sensors: snap, dsdp (the D slot), sensordata
+  DevFdPrmInv fdpi = {}; std::vector<void*> fdpi_scope; int fdpi_done = 0; bool fdpi_sens = false;
+  float* fdpi_env_sd = nullptr; std::vector<void*> fdpis_scope;            // its sensors: every env's sensordata (DsDp, sensordata in fdpi)
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -2229,6 +2236,33 @@ static int fds_alloc(FbSim* s) {
     s->fds = DevFdSens{}; return rc; }
   return 0;
 }
+// the problems of a transition query: written bank rows, none saved while its env was held for a reset
+static int fd_slots_valid(FbSim* s, const char* who, const int32_t* slots, int n) {
+  for (int k = 0; k < n; k++) {
+    const int sl = slots[k];
+    if (sl < 0 || sl >= s->st_slots) { s->err = std::string(who) + ": slot out of range of the bank"; return -1; }
+    if (!s->st_written[sl]) { s->err = std::string(who) + ": slot " + std::to_string(sl) + " was never written"; return -1; }
+    if (s->st_written[sl] == 2) { s->err = std::string(who) + ": slot " + std::to_string(sl) + " was saved while its env was held for a reset (a held env does not integrate)"; return -1; }
+  }
+  return 0;
+}
+// every env a copy of its problem's row, warm start included; the envs past the problems copy the last problem's
+static int fd_fan_out(FbSim* s, const int32_t* slots, int n, int ncol) {
+  const int N = s->d.N;
+  std::vector<int32_t> fan(N);
+  for (int e = 0; e < N; e++) fan[e] = slots[std::min(e / ncol, n - 1)];
+  const int *ed, *sd;
+  if (int rc = state_ids(s, nullptr, fan.data(), N, &ed, &sd)) return rc;
+  launch_state<true>(s, nullptr, sd, N);
+  return 0;
+}
+// fb_step's launches, split after the first substep to snapshot the sensors of x (q.snap) of the first n envs
+static void fd_step_snap(FbSim* s, const DevFdSens& q, int n, int n_substeps) {
+  warp_launch(s, "fd_snap", n, 0, FdSnap<false>{s->m, s->d, q});
+  step_run(s, 1);
+  warp_launch(s, "fd_snap", n, 0, FdSnap<true>{s->m, s->d, q});
+  if (n_substeps > 1) step_run(s, n_substeps - 1);
+}
 
 extern "C" {
 
@@ -2242,36 +2276,19 @@ int fb_fd_transition(FbHandle s, const int32_t* slots, int n, float eps, int cen
     s->err = "fb_fd_transition: 1 <= n problems with n * fb_fd_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
   if (!(eps > 0.0f) || !std::isfinite(eps)) { s->err = "fb_fd_transition: eps must be positive and finite"; return -1; }
   if (n_substeps < 1) { s->err = "fb_fd_transition: n_substeps >= 1"; return -1; }
-  for (int k = 0; k < n; k++) {
-    const int sl = slots[k];
-    if (sl < 0 || sl >= s->st_slots) { s->err = "fb_fd_transition: slot out of range of the bank"; return -1; }
-    if (!s->st_written[sl]) { s->err = "fb_fd_transition: slot " + std::to_string(sl) + " was never written"; return -1; }
-    if (s->st_written[sl] == 2) { s->err = "fb_fd_transition: slot " + std::to_string(sl) + " was saved while its env was held for a reset (a held env does not integrate)"; return -1; }
-  }
+  if (fd_slots_valid(s, "fb_fd_transition", slots, n) != 0) return -1;
   dev_select(s);
   if (int rc = fd_alloc(s)) return rc;
   const bool sens = s->sens_on != 0, snap = sens && s->m.nsensordata > 0;
   if (sens) if (int rc = fds_alloc(s)) return rc;
-  // every env a copy of its problem's row, warm start included; the envs past the problems copy the last problem's
-  std::vector<int32_t> fan(N);
-  for (int e = 0; e < N; e++) fan[e] = slots[std::min(e / ncol, n - 1)];
-  const int *ed, *sd;
-  if (int rc = state_ids(s, nullptr, fan.data(), N, &ed, &sd)) return rc;
+  if (int rc = fd_fan_out(s, slots, n, ncol)) return rc;
   DevFd& p = s->fd;
   p.n = n; p.ncol = ncol; p.nx = 2 * s->m.nv + s->m.na; p.nin = p.nx + s->m.nu; p.centered = centered != 0; p.eps = eps;
   s->fd_done = 0;
-  launch_state<true>(s, nullptr, sd, N);
   warp_launch(s, "fd_perturb", N, 0, FdPerturb{s->m, s->d, p});
   launch_step1(s);                             // the position / velocity stage of the nudged states
-  if (!snap) {
-    step_run(s, n_substeps);                   // fb_step's launches
-  } else {                                     // the same launches, split after the first substep: the sensors of x
-    DevFdSens& q = s->fds; q.fd = p;
-    warp_launch(s, "fd_snap", n * ncol, 0, FdSnap<false>{s->m, s->d, q});
-    step_run(s, 1);
-    warp_launch(s, "fd_snap", n * ncol, 0, FdSnap<true>{s->m, s->d, q});
-    if (n_substeps > 1) step_run(s, n_substeps - 1);
-  }
+  if (!snap) step_run(s, n_substeps);          // fb_step's launches
+  else { s->fds.fd = p; fd_step_snap(s, s->fds, n * ncol, n_substeps); }
   warp_launch(s, "fd_diff", n * p.nin, 0, FdDiff{s->m, s->d, p});
   if (snap) warp_launch(s, "fd_sdiff", n * p.nin, 0, FdSDiff{s->m, s->fds});
   if (launch_check(s, "fb_fd_transition") != 0) return -2;
@@ -2401,6 +2418,214 @@ int fb_fd_inverse_read(FbHandle s, float* DfDq, float* DfDv, float* DfDa, float*
   const size_t n = (size_t)s->fdi_done, nv = (size_t)s->m.nv, nM = (size_t)s->m.nM;
   return read_out(s, {{DfDq, p.DfDq, 0, 4 * n * nv * nv, 1}, {DfDv, p.DfDv, 0, 4 * n * nv * nv, 1}, {DfDa, p.DfDa, 0, 4 * n * nv * nv, 1},
                       {DmDq, p.DmDq, 0, 4 * n * nv * nM, 1}, {qfrc_inverse, p.qfrc, 0, 4 * n * nv, 1}});
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------
+// parameter Jacobians (fb_fd_param_*; fb_fd.h): a direction program resolved to overlay slots, and their own kernel parameters
+// (DevFdPrm, DevFdPrmInv with its own DevInv) and buffers
+struct FdpPerturb {
+  DevData d; DevFdPrm p;
+  FB_DEVM void operator()(unsigned char*, int e) const { kfdp_perturb(d, p, e); }
+};
+struct FdpDiff {
+  DevModel m; DevData d; DevFdPrm p;
+  FB_DEVM void operator()(unsigned char*, int w) const { kfdp_diff(m, d, p, w); }
+};
+struct FdpiRows {
+  DevData d; DevFdPrmInv p;
+  FB_DEVM void operator()(unsigned char*, int w) const { kfdpi_rows(d, p, w); }
+};
+struct FdpiPerturb {
+  DevModel m; DevData d; DevFdPrmInv p;
+  FB_DEVM void operator()(unsigned char*, int e) const { kfdpi_perturb(m, d, p, e); }
+};
+struct FdpiDiff {
+  DevModel m; DevFdPrmInv p;
+  FB_DEVM void operator()(unsigned char*, int w) const { kfdpi_diff(m, p, w); }
+};
+static int fdp_columns(const FbSim* s, int centered) { return 1 + (centered ? 2 : 1) * s->fdp_k; }
+// the checks both queries share: an overlay, a program, eps
+static int fdp_ready(FbSim* s, const char* who, const char* todo, float eps) {
+  if (!s->d.prm) { s->err = std::string(who) + ": the handle has no parameter overlay, and the columns nudge each problem's own parameters: " + todo; return -1; }
+  if (s->fdp_k < 1) { s->err = std::string(who) + ": no direction program (fb_fd_param_program)"; return -1; }
+  if (!(eps > 0.0f) || !std::isfinite(eps)) { s->err = std::string(who) + ": eps must be positive and finite"; return -1; }
+  if (s->fdp_scale && !(eps < 1.0f)) { s->err = std::string(who) + ": the program has scale directions, which need eps < 1"; return -1; }
+  return 0;
+}
+
+extern "C" {
+
+int fb_fd_param_program(FbHandle s, int k, const int32_t* kind, const int32_t* dir_ptr, const int32_t* param, const int32_t* elem, const float* floor) {
+  if (!s) return -1;
+  const char* who = "fb_fd_param_program: ";
+  if (k < 0) { s->err = std::string(who) + "k >= 1 directions (0 clears the program)"; return -1; }
+  if (k > 0 && (!kind || !dir_ptr || !param || !elem || !floor)) { s->err = std::string(who) + "kind, dir_ptr, param, elem and floor must not be NULL"; return -1; }
+  if (k > 0 && dir_ptr[0] != 0) { s->err = std::string(who) + "dir_ptr[0] must be 0"; return -1; }
+  std::vector<int> kd(k), ptr(k + 1, 0), slot, mslot, nonneg; std::vector<float> fl;
+  bool scale = false;
+  for (int j = 0; j < k; j++) {
+    const int a = dir_ptr[j], b = dir_ptr[j + 1], dj = kind[j];
+    const std::string at = "direction " + std::to_string(j) + ": ";
+    if (dj != FB_FD_ELEMENT && dj != FB_FD_SCALE) { s->err = who + at + "kind is 0 (element) or 1 (scale)"; return -1; }
+    if (b <= a) { s->err = who + at + "no entries (dir_ptr must increase)"; return -1; }
+    if (dj == FB_FD_ELEMENT && b != a + 1) { s->err = who + at + "an element direction has one entry"; return -1; }
+    scale = scale || dj == FB_FD_SCALE;
+    std::vector<int> seen;
+    for (int t = a; t < b; t++) {
+      const int p = param[t], i = elem[t];
+      if (p < 0 || p >= FB_NPARAMS) { s->err = who + at + "unknown parameter " + std::to_string(p); return -1; }
+      if (i < 0 || i >= s->prm_n[p]) { s->err = who + at + "element " + std::to_string(i) + " out of range of parameter " + std::to_string(p) + " (fb_param_size " + std::to_string(s->prm_n[p]) + ")"; return -1; }
+      if (p == FB_P_JNT_STIFFNESS && s->h_jnt_type[i] != FB_JNT_HINGE) {
+        s->err = who + at + "joint " + std::to_string(i) + " is not a hinge: the step has springs on hinge joints only"; return -1; }
+      if (dj == FB_FD_ELEMENT && !(std::isfinite(floor[t]) && floor[t] > 0.0f)) { s->err = who + at + "the floor must be positive and finite"; return -1; }
+      const int sl = s->d.prm_off[p] + prm_slot(p, i);
+      if (std::find(seen.begin(), seen.end(), sl) != seen.end()) { s->err = who + at + "an element appears twice"; return -1; }
+      seen.push_back(sl);
+      slot.push_back(sl);
+      mslot.push_back(p == FB_P_DOF_DAMPING ? s->d.prm_mdamp + s->h_dof_Madr[i] : -1);
+      nonneg.push_back(p != FB_P_ACTUATOR_GAINPRM && p != FB_P_ACTUATOR_BIASPRM && p != FB_P_GRAVITY && p != FB_P_WIND);
+      fl.push_back(dj == FB_FD_ELEMENT ? floor[t] : 1.0f);
+    }
+    kd[j] = dj; ptr[j + 1] = b;
+  }
+  if (sync_stream(s) != 0) return -2;          // a call in flight may still read the old tables
+  scope_free(s, s->fdp_prog_scope);
+  s->fdp_prog = DevFdPrmProg{}; s->fdp_k = 0; s->fdp_scale = false;
+  if (k == 0) return 0;
+  DevFdPrmProg& g = s->fdp_prog;
+  if (int rc = scope_alloc(s, s->fdp_prog_scope, "out of device memory (parameter direction program)", [&] {
+        g.kind = up(s, kd); g.ptr = up(s, ptr); g.slot = up(s, slot); g.mslot = up(s, mslot); g.nonneg = up(s, nonneg); g.floor = up(s, fl); })) {
+    g = DevFdPrmProg{}; return rc; }
+  s->fdp_k = k; s->fdp_scale = scale;
+  return 0;
+}
+
+int fb_fd_param_columns(FbHandle s, int centered) {
+  if (!s) return -1;
+  if (s->fdp_k < 1) { s->err = "fb_fd_param_columns: no direction program (fb_fd_param_program)"; return -1; }
+  return fdp_columns(s, centered);
+}
+
+int fb_fd_param_transition(FbHandle s, const int32_t* slots, int n, float eps, int centered, int n_substeps) {
+  if (!s) return -1;
+  const char* who = "fb_fd_param_transition";
+  if (fdp_ready(s, who, "fb_param_set first, then fb_state_bank and fb_state_save the rows", eps) != 0 || state_ready(s, who) != 0) return -1;
+  const int N = s->d.N, ncol = fdp_columns(s, centered != 0);
+  if (!slots || n < 1 || (long long)n * ncol > N) {
+    s->err = std::string(who) + ": 1 <= n problems with n * fb_fd_param_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
+  if (n_substeps < 1) { s->err = std::string(who) + ": n_substeps >= 1"; return -1; }
+  if (fd_slots_valid(s, who, slots, n) != 0) return -1;
+  dev_select(s);
+  const DevModel& m = s->m;
+  const size_t Np = s->d.Np, nx = 2 * (size_t)m.nv + m.na, nsd = m.nsensordata, half = std::max(1, s->d.N / 2);   // n k < N, n <= N / 2
+  DevFdPrm& p = s->fdp;
+  if (!p.delta && scope_alloc(s, s->fdp_scope, "out of device memory (parameter Jacobians)", [&] {
+        p.delta = dalloc<float>(s, Np); p.dxdp = dalloc<float>(s, Np * nx); p.next = dalloc<float>(s, half * (m.nq + m.nv + m.na)); })) {
+    p = DevFdPrm{}; return -4; }
+  const bool sens = s->sens_on != 0, snap = sens && nsd > 0;
+  DevFdSens& q = s->fdps;
+  if (sens && !q.snap && scope_alloc(s, s->fdps_scope, "out of device memory (parameter sensor Jacobians)", [&] {
+        q.snap = dalloc<float>(s, Np * nsd); q.D = dalloc<float>(s, Np * nsd); q.sensordata = dalloc<float>(s, half * nsd); })) {
+    q = DevFdSens{}; return -4; }
+  if (int rc = fd_fan_out(s, slots, n, ncol)) return rc;
+  p.n = n; p.ncol = ncol; p.nin = s->fdp_k; p.centered = centered != 0; p.eps = eps; p.nx = (int)nx; p.g = s->fdp_prog;
+  s->fdp_done = 0;
+  warp_launch(s, "fdp_perturb", N, 0, FdpPerturb{s->d, p});
+  launch_step1(s);                             // the position / velocity stage of the nudged parameters
+  if (!snap) step_run(s, n_substeps);
+  else {                                       // kfd_sdiff with no state inputs: its D block is dsdp [n][nsd][k]
+    q.fd = DevFd{}; static_cast<FdCols&>(q.fd) = p;
+    fd_step_snap(s, q, n * ncol, n_substeps);
+  }
+  warp_launch(s, "fdp_diff", n * p.nin, 0, FdpDiff{s->m, s->d, p});
+  if (snap) warp_launch(s, "fd_sdiff", n * p.nin, 0, FdSDiff{s->m, q});
+  if (launch_check(s, who) != 0) return -2;
+  s->fdp_done = n; s->fdp_sens = sens;
+  return sync_stream(s);                       // (the fan-out list is a host vector)
+}
+
+int fb_fd_param_read(FbHandle s, float* dxdp, float* qpos_next, float* qvel_next, float* act_next, int is_device) {
+  if (!s) return -1;
+  if (s->fdp_done < 1) { s->err = "fb_fd_param_read: no parameter Jacobians to read (fb_fd_param_transition)"; return -1; }
+  const DevFdPrm& p = s->fdp;
+  const size_t n = (size_t)s->fdp_done, nx = (size_t)p.nx, k = (size_t)p.nin;
+  const size_t nq = s->m.nq, nv = s->m.nv, na = s->m.na, row = (nq + nv + na) * 4;
+  return read_out(s, {{dxdp, p.dxdp, 0, 4 * n * nx * k, 1}, {qpos_next, p.next, row, nq * 4, n}, {qvel_next, p.next + nq, row, nv * 4, n},
+                      {act_next, p.next + nq + nv, row, na * 4, n}});
+}
+
+int fb_fd_param_sensor_read(FbHandle s, float* dsdp, float* sensordata, int is_device) {
+  if (!s) return -1;
+  if (s->fdp_done < 1) { s->err = "fb_fd_param_sensor_read: no parameter Jacobians to read (fb_fd_param_transition)"; return -1; }
+  if (!s->fdp_sens) { s->err = "fb_fd_param_sensor_read: the last fb_fd_param_transition ran with sensors off (fb_query_sensors)"; return -1; }
+  const size_t n = (size_t)s->fdp_done, nsd = (size_t)s->m.nsensordata, k = (size_t)s->fdp.nin;
+  return read_out(s, {{dsdp, s->fdps.D, 0, 4 * n * nsd * k, 1}, {sensordata, s->fdps.sensordata, 0, 4 * n * nsd, 1}});
+}
+
+int fb_fd_param_inverse(FbHandle s, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device) {
+  if (!s) return -1;
+  const char* who = "fb_fd_param_inverse";
+  if (fdp_ready(s, who, "fb_param_set first (problem i takes env i's parameters)", eps) != 0) return -1;
+  const int N = s->d.N, ncol = fdp_columns(s, centered != 0);
+  if (n < 1 || (long long)n * ncol > N) {
+    s->err = std::string(who) + ": 1 <= n problems with n * fb_fd_param_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
+  if (!qpos || !qvel || !qacc) { s->err = std::string(who) + ": qpos, qvel and qacc must not be NULL"; return -1; }
+  const size_t nq = s->m.nq, nv = s->m.nv, nsd = s->m.nsensordata, Np = s->d.Np, P = s->d.prm_stride, half = std::max(1, N / 2);
+  if (!is_device) {
+    const struct { const float* x; size_t cnt; const char* what; } ins[3] = {{qpos, n * nq, "qpos"}, {qvel, n * nv, "qvel"}, {qacc, n * nv, "qacc"}};
+    for (const auto& in : ins)
+      for (size_t i = 0; i < in.cnt; i++)
+        if (!std::isfinite(in.x[i])) { s->err = std::string(who) + ": non-finite " + in.what; return -1; }
+  }
+  dev_select(s);
+  DevFdPrmInv& p = s->fdpi;
+  if (!p.delta && scope_alloc(s, s->fdpi_scope, "out of device memory (inverse parameter Jacobians)", [&] {
+        float *qp = dalloc<float>(s, half * nq), *qv = dalloc<float>(s, half * nv), *qa = dalloc<float>(s, half * nv);
+        p.qpos = qp; p.qvel = qv; p.qacc = qa;
+        p.rows = dalloc<float>(s, half * P); p.delta = dalloc<float>(s, Np);
+        p.inv.qacc = dalloc<float>(s, Np * nv); p.inv.qfrc_inverse = dalloc<float>(s, Np * nv);
+        p.inv.qfrc_constraint = dalloc<float>(s, Np * nv); p.inv.efc_force = dalloc<float>(s, Np * FB_MAXEFC);
+        p.DfDp = dalloc<float>(s, Np * nv); p.qfrc = dalloc<float>(s, half * nv); })) {
+    p = DevFdPrmInv{}; return -4; }
+  const bool sens = s->sens_on != 0, sdiff = sens && nsd > 0;
+  if (sens && !s->fdpi_env_sd && scope_alloc(s, s->fdpis_scope, "out of device memory (inverse parameter sensor Jacobians)", [&] {
+        s->fdpi_env_sd = dalloc<float>(s, Np * nsd); p.DsDp = dalloc<float>(s, Np * nsd); p.sensordata = dalloc<float>(s, half * nsd); })) {
+    s->fdpi_env_sd = p.DsDp = p.sensordata = nullptr; return -4; }
+  if (copy_async(s, (void*)p.qpos, qpos, sizeof(float) * n * nq) != 0 || copy_async(s, (void*)p.qvel, qvel, sizeof(float) * n * nv) != 0 ||
+      copy_async(s, (void*)p.qacc, qacc, sizeof(float) * n * nv) != 0) return -2;
+  p.n = n; p.ncol = ncol; p.nin = s->fdp_k; p.centered = centered != 0; p.eps = eps; p.g = s->fdp_prog;
+  p.inv.n = n * ncol;
+  p.sens = sdiff ? s->fdpi_env_sd : nullptr;
+  float* env_sd = s->fdpi_env_sd;
+  s->fdpi_done = 0;
+  warp_launch(s, "fdpi_rows", n, 0, FdpiRows{s->d, p});                 // problem i's parameters: env i's, before the fan-out
+  warp_launch(s, "fdpi_perturb", N, 0, FdpiPerturb{s->m, s->d, p});      // fan-out and nudge
+  launch_step1(s);                             // the position / velocity stage of every env, as fb_inverse runs it
+  launch_inv(s, p.inv);
+  if (sdiff) launch_inv_sensors(s, p.inv, env_sd);
+  warp_launch(s, "fdpi_diff", n * p.nin, 0, FdpiDiff{s->m, p});
+  if (launch_check(s, who) != 0) return -2;
+  s->fdpi_done = n; s->fdpi_sens = sens;
+  return is_device ? 0 : sync_stream(s);       // host rows may be reused once the call returns
+}
+
+int fb_fd_param_inverse_read(FbHandle s, float* DfDp, float* qfrc_inverse, int is_device) {
+  if (!s) return -1;
+  if (s->fdpi_done < 1) { s->err = "fb_fd_param_inverse_read: no parameter Jacobians to read (fb_fd_param_inverse)"; return -1; }
+  const DevFdPrmInv& p = s->fdpi;
+  const size_t n = (size_t)s->fdpi_done, nv = (size_t)s->m.nv, k = (size_t)p.nin;
+  return read_out(s, {{DfDp, p.DfDp, 0, 4 * n * k * nv, 1}, {qfrc_inverse, p.qfrc, 0, 4 * n * nv, 1}});
+}
+
+int fb_fd_param_inverse_sensor_read(FbHandle s, float* DsDp, float* sensordata, int is_device) {
+  if (!s) return -1;
+  if (s->fdpi_done < 1) { s->err = "fb_fd_param_inverse_sensor_read: no parameter Jacobians to read (fb_fd_param_inverse)"; return -1; }
+  if (!s->fdpi_sens) { s->err = "fb_fd_param_inverse_sensor_read: the last fb_fd_param_inverse ran with sensors off (fb_query_sensors)"; return -1; }
+  const DevFdPrmInv& p = s->fdpi;
+  const size_t n = (size_t)s->fdpi_done, nsd = (size_t)s->m.nsensordata, k = (size_t)p.nin;
+  return read_out(s, {{DsDp, p.DsDp, 0, 4 * n * k * nsd, 1}, {sensordata, p.sensordata, 0, 4 * n * nsd, 1}});
 }
 
 }  // extern "C"

@@ -23,6 +23,7 @@ MAXCON, MAXEFC = 64, 160
 # enum FbParam: the per-env model parameters (fb_param_*), by their mjModel names, and their shape per env
 PARAMS = ('body_mass', 'body_inertia', 'dof_armature', 'dof_damping', 'jnt_stiffness', 'geom_friction', 'actuator_gainprm',
           'actuator_biasprm', 'gravity', 'wind', 'density', 'viscosity')
+FD_ELEMENT, FD_SCALE = 0, 1           # kinds of a parameter direction (fb_fd_param_program)
 
 EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_applied_ptrs', 'fb_clear_applied', 'fb_step', 'fb_forward',
            'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
@@ -31,7 +32,9 @@ EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl'
            'fb_ik_program', 'fb_ik_solve', 'fb_ik_read', 'fb_inverse', 'fb_inverse_read',
            'fb_fd_columns', 'fb_fd_transition', 'fb_fd_read', 'fb_fd_inverse_columns', 'fb_fd_inverse', 'fb_fd_inverse_read',
            'fb_query_sensors', 'fb_inverse_sensor_read', 'fb_fd_sensor_read', 'fb_fd_inverse_sensor_read',
-           'fb_param_size', 'fb_param_set', 'fb_param_get', 'fb_param_draws', 'fb_param_clear']
+           'fb_param_size', 'fb_param_set', 'fb_param_get', 'fb_param_draws', 'fb_param_clear',
+           'fb_fd_param_program', 'fb_fd_param_columns', 'fb_fd_param_transition', 'fb_fd_param_read', 'fb_fd_param_sensor_read',
+           'fb_fd_param_inverse', 'fb_fd_param_inverse_read', 'fb_fd_param_inverse_sensor_read']
 
 
 # enum FbTaskKind (FbTaskProgram.kind)
@@ -192,6 +195,14 @@ def load_library(path=None):
     lib.fb_param_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
     lib.fb_param_draws.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_uint32]
     lib.fb_param_clear.argtypes = [C.c_void_p]
+    lib.fb_fd_param_program.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
+    lib.fb_fd_param_columns.argtypes = [C.c_void_p, C.c_int]
+    lib.fb_fd_param_transition.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int]
+    lib.fb_fd_param_read.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int]
+    lib.fb_fd_param_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
+    lib.fb_fd_param_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int]
+    lib.fb_fd_param_inverse_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
+    lib.fb_fd_param_inverse_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
     return lib
 
 
@@ -525,6 +536,74 @@ class BatchedStepper:
         m, n = self.model, getattr(self, '_fdi_n', 0)
         out = [np.zeros((n, m.nv, m.nsensordata), np.float32) for _ in range(3)] + [np.zeros((n, m.nsensordata), np.float32)]
         self._check(self._lib.fb_fd_inverse_sensor_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_inverse_sensor_read')
+        return tuple(out)
+
+    # ---- finite-difference parameter Jacobians (fb_fd_param_*; flybody_b200.derivatives.parameter_fd / inverse_parameter_fd are the
+    # batched front ends)
+    def fd_param_program(self, directions):
+        """directions: [(kind, [(parameter name, element), ...], [floor per entry] or None)], kind FD_ELEMENT (one entry) or FD_SCALE;
+        an empty list clears the program (see the header)"""
+        kind, ptr, par, elem, floor = [], [0], [], [], []
+        for k, entries, floors in directions:
+            kind.append(int(k))
+            for t, (name, i) in enumerate(entries):
+                par.append(self._param(name)[0])
+                elem.append(int(i))
+                floor.append(1.0 if floors is None else float(floors[t]))
+            ptr.append(len(par))
+        arrs = [np.ascontiguousarray(x, np.int32) for x in (kind, ptr, par, elem)] + [np.ascontiguousarray(floor, np.float32)]
+        self._check(self._lib.fb_fd_param_program(self._h, len(kind), *[x.ctypes.data for x in arrs]), 'fb_fd_param_program')
+        self._fdp_k = len(kind)
+
+    def fd_param_columns(self, centered=True):
+        """envs one problem of fd_param_transition / fd_param_inverse takes"""
+        n = int(self._lib.fb_fd_param_columns(self._h, int(bool(centered))))
+        self._check(0 if n > 0 else -1, 'fb_fd_param_columns')
+        return n
+
+    def fd_param_transition(self, slots, eps=1e-2, centered=True, n_substeps=1):
+        """dx'/dtheta of the bank rows `slots` along the program's directions over n_substeps substeps; read with fd_param_read()"""
+        s = np.ascontiguousarray(np.asarray(slots).reshape(-1), np.int32)
+        self._check(self._lib.fb_fd_param_transition(self._h, s.ctypes.data, len(s), float(eps), int(bool(centered)), int(n_substeps)),
+                    'fb_fd_param_transition')
+        self._fdp_n = (len(s), self._fdp_k)
+
+    def fd_param_read(self):
+        """-> (dxdp [n, nx, k], qpos_next [n, nq], qvel_next [n, nv], act_next [n, na]) f32 of the last fd_param_transition"""
+        m, (n, k) = self.model, getattr(self, '_fdp_n', (0, 0))
+        out = [np.zeros((n, 2 * m.nv + m.na, k), np.float32), np.zeros((n, m.nq), np.float32), np.zeros((n, m.nv), np.float32),
+               np.zeros((n, m.na), np.float32)]
+        self._check(self._lib.fb_fd_param_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_param_read')
+        return tuple(out)
+
+    def fd_param_sensor_read(self):
+        """-> (dsdp [n, nsd, k], sensordata [n, nsd]) f32 of the last fd_param_transition (run with sensors on): the sensors of x"""
+        m, (n, k) = self.model, getattr(self, '_fdp_n', (0, 0))
+        out = [np.zeros((n, m.nsensordata, k), np.float32), np.zeros((n, m.nsensordata), np.float32)]
+        self._check(self._lib.fb_fd_param_sensor_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_param_sensor_read')
+        return tuple(out)
+
+    def fd_param_inverse(self, qpos, qvel, qacc, eps=1e-2, centered=True, n=None, is_device=False):
+        """d qfrc_inverse / dtheta of problems qpos [n, nq], qvel [n, nv], qacc [n, nv] along the program's directions, problem i with
+        env i's parameters (host arrays, or device pointers with is_device=True and n given); read with fd_param_inverse_read()"""
+        m = self.model
+        n, ptrs, _rows = self._problem_rows([('qpos', qpos, m.nq), ('qvel', qvel, m.nv), ('qacc', qacc, m.nv)], n, is_device)
+        self._check(self._lib.fb_fd_param_inverse(self._h, n, *ptrs, float(eps), int(bool(centered)), int(bool(is_device))),
+                    'fb_fd_param_inverse')
+        self._fdpi_n = (n, self._fdp_k)
+
+    def fd_param_inverse_read(self):
+        """-> (DfDp [n, k, nv], qfrc_inverse [n, nv]) f32 of the last fd_param_inverse: DfDp[p, j, i] = d qfrc_inverse_i / d direction j"""
+        m, (n, k) = self.model, getattr(self, '_fdpi_n', (0, 0))
+        out = [np.zeros((n, k, m.nv), np.float32), np.zeros((n, m.nv), np.float32)]
+        self._check(self._lib.fb_fd_param_inverse_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_param_inverse_read')
+        return tuple(out)
+
+    def fd_param_inverse_sensor_read(self):
+        """-> (DsDp [n, k, nsd], sensordata [n, nsd]) f32 of the last fd_param_inverse (run with sensors on)"""
+        m, (n, k) = self.model, getattr(self, '_fdpi_n', (0, 0))
+        out = [np.zeros((n, k, m.nsensordata), np.float32), np.zeros((n, m.nsensordata), np.float32)]
+        self._check(self._lib.fb_fd_param_inverse_sensor_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_param_inverse_sensor_read')
         return tuple(out)
 
     def reset(self, qpos=None, qvel=None, env_ids=None):

@@ -626,6 +626,40 @@ int fb_query_sensors(FbHandle h, int on);
 int fb_inverse_sensor_read(FbHandle h, float* sensordata, int is_device);
 int fb_fd_sensor_read(FbHandle h, float* C, float* D, float* sensordata, int is_device);
 int fb_fd_inverse_sensor_read(FbHandle h, float* DsDq, float* DsDv, float* DsDa, float* sensordata, int is_device);
+/* Finite-difference parameter Jacobians (system identification): the derivatives of fb_fd_transition's next state and of
+ * fb_inverse's qfrc_inverse (and of their sensors while fb_query_sensors is on) with respect to directions in the per-env model
+ * parameters (fb_param_*).  Derived constants hold as in the overlay (no mj_setConst); the implicit-damping diagonal follows dof_damping.
+ *   A direction program (fb_fd_param_program) lists k >= 1 directions; direction j has the entries dir_ptr[j] .. dir_ptr[j+1] - 1 of
+ *   param[] (FbParam ids) and elem[] (elements as fb_param_size counts them):
+ *     kind 0, element: one entry theta_i, nudged by +-delta_i = eps max(|theta_i|, floor_i), theta_i the problem's own value; the column
+ *                      is d / d theta_i in the parameter's units.  A side whose value would be negative on a non-negative field (those
+ *                      fb_param_set keeps >= 0) is skipped, as fb_fd_transition skips a ctrl nudge out of range: a one-sided column.
+ *     kind 1, scale:   every entry multiplied by (1 +- eps); the column is d / ds at s = 1 of theta_set <- s theta_set.  Needs eps < 1.
+ *   floor[] is read for element entries only (positive, finite).  Errors: k < 0, NULL arrays, dir_ptr not starting at 0 or not
+ *   increasing, an unknown kind or parameter, an element out of range, an element direction of more than one entry, jnt_stiffness of
+ *   a joint that is not a hinge, an element twice in one direction.  k = 0 clears the program.  fb_fd_param_columns(h, centered): the
+ *   envs of one problem, 1 + 2k centred, 1 + k forward (column 0 the nominal); -1 without a program.
+ * Both queries need a parameter overlay (fb_param_set) and a program; eps > 0 and finite.  The handle is a workspace: afterwards every
+ * env's state and parameters are unspecified (the overlay rows of the columns hold their nudged values); the bank is untouched.
+ *   fb_fd_param_transition: fb_fd_transition's contract (problems are state-bank rows, which carry the parameters; columns fanned out
+ *     and stepped n_substeps substeps with ctrl held; the same errors).  Outputs (fb_fd_param_read): dxdp [n][nx][k] row-major as B
+ *     (mj_differentiatePos rows for dq), the nominal next state; with sensors (fb_fd_param_sensor_read): dsdp [n][nsd][k] and the
+ *     nominal sensordata, the sensors of x, the state before the step (as C and D).  It synchronises.
+ *   fb_fd_param_inverse: problems qpos [n][nq], qvel [n][nv], qacc [n][nv] (host rows, or device pointers when is_device) as
+ *     fb_fd_inverse; problem i takes env i's parameter row at call time (as fb_inverse).  Outputs (fb_fd_param_inverse_read):
+ *     DfDp [n][k][nv] transposed as DfDq (DfDp[j][i] = d qfrc_inverse_i / d direction j), the nominal qfrc_inverse; with sensors
+ *     (fb_fd_param_inverse_sensor_read): DsDp [n][k][nsd] and the nominal sensordata.  qfrc_inverse excludes actuation, so actuator
+ *     gain / bias columns are 0.  Errors: fb_fd_inverse's.  A device input is not checked and the call does not synchronise.
+ * The reads synchronise (any pointer may be NULL; is_device: device pointers).  Errors: a read before any call, a sensor read after a
+ * call made with sensors off.                                                                                                        */
+int fb_fd_param_program(FbHandle h, int k, const int32_t* kind, const int32_t* dir_ptr, const int32_t* param, const int32_t* elem, const float* floor);
+int fb_fd_param_columns(FbHandle h, int centered);
+int fb_fd_param_transition(FbHandle h, const int32_t* slots, int n, float eps, int centered, int n_substeps);
+int fb_fd_param_read(FbHandle h, float* dxdp, float* qpos_next, float* qvel_next, float* act_next, int is_device);
+int fb_fd_param_sensor_read(FbHandle h, float* dsdp, float* sensordata, int is_device);
+int fb_fd_param_inverse(FbHandle h, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device);
+int fb_fd_param_inverse_read(FbHandle h, float* DfDp, float* qfrc_inverse, int is_device);
+int fb_fd_param_inverse_sensor_read(FbHandle h, float* DsDp, float* sensordata, int is_device);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
