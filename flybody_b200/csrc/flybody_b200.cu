@@ -30,6 +30,7 @@
 #include "fb_ik.h"
 #include "fb_inverse.h"
 #include "fb_fd.h"
+#include "fb_rollout.h"
 
 enum { K_ACT = 0, K_SMOOTH, K_REF, K_SOLVE, K_FINISH, K_POS, K_COL, K_CON, K_PROJ, K_VEL, K_SENS, K_PACK, K_MISC, K_NKIND };
 static const char* const kKindNames[K_NKIND] = {"act", "smooth", "ref", "solve", "finish", "pos", "col", "con", "proj", "vel", "sens", "pack", "misc"};
@@ -64,6 +65,12 @@ struct FbSim {
   DevFdSens fdps = {}; std::vector<void*> fdps_scope;                    // its sensors: snap, dsdp (the D slot), sensordata
   DevFdPrmInv fdpi = {}; std::vector<void*> fdpi_scope; int fdpi_done = 0; bool fdpi_sens = false;
   float* fdpi_env_sd = nullptr; std::vector<void*> fdpis_scope;            // its sensors: every env's sensordata (DsDp, sensordata in fdpi)
+  // rollouts (fb_rollout*; fb_rollout.h): inputs and records of roll_cap rows (n T), grown on demand in three groups (ctrl and the
+  // records; applied-force inputs; sensor records); the feedback law of roll_fb_T steps (fb_rollout_feedback); rows of the last call
+  DevRoll roll = {}; std::vector<void*> roll_scope, roll_app_scope, roll_sd_scope; size_t roll_cap = 0, roll_app_cap = 0, roll_sd_cap = 0;
+  float *roll_xref = nullptr, *roll_K = nullptr; std::vector<void*> roll_fb_scope; int roll_fb_T = 0;
+  float *roll_qf = nullptr, *roll_xf = nullptr, *roll_sd = nullptr, *roll_sm = nullptr;   // applied-force inputs, sensor records
+  int roll_done = 0; bool roll_sens = false;
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -2626,6 +2633,131 @@ int fb_fd_param_inverse_sensor_read(FbHandle s, float* DsDp, float* sensordata, 
   const DevFdPrmInv& p = s->fdpi;
   const size_t n = (size_t)s->fdpi_done, nsd = (size_t)s->m.nsensordata, k = (size_t)p.nin;
   return read_out(s, {{DsDp, p.DsDp, 0, 4 * n * k * nsd, 1}, {sensordata, p.sensordata, 0, 4 * n * nsd, 1}});
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------
+// rollouts (fb_rollout*; fb_rollout.h): their own kernel parameter (DevRoll) and buffers, allocated on first use and grown with n T
+struct RollInput {
+  DevModel m; DevData d; DevRoll p;
+  FB_DEVM void operator()(unsigned char* sh, int e) const { kroll_input(m, d, p, reinterpret_cast<float*>(sh), e); }
+};
+struct RollRecord {
+  DevModel m; DevData d; DevRoll p;
+  FB_DEVM void operator()(unsigned char*, int e) const { kroll_record(m, d, p, e); }
+};
+// one group of buffers for `rows` rows of `row_bytes` bytes, made by alloc(rows) unless `cap` rows fit already
+template <typename F> static int roll_grow(FbSim* s, std::vector<void*>& scope, size_t& cap, size_t rows, size_t row_bytes, const char* what, F alloc) {
+  if (rows <= cap) return 0;
+  if (sync_stream(s) != 0) return -2;
+  scope_free(s, scope); cap = 0;
+  if (rows * row_bytes > dev_free_bytes()) {
+    s->err = std::string("fb_rollout: the ") + what + " of " + std::to_string(rows) + " rows (n T) do not fit the device's free memory"; return -4; }
+  const std::string oom = std::string("fb_rollout: out of device memory (") + what + ")";
+  if (int rc = scope_alloc(s, scope, oom.c_str(), [&] { alloc(rows); })) return rc;
+  cap = rows;
+  return 0;
+}
+static bool all_finite(const float* x, size_t n) { for (size_t i = 0; i < n; i++) if (!std::isfinite(x[i])) return false; return true; }
+
+extern "C" {
+
+int fb_rollout_feedback(FbHandle s, int T, const float* xref, const float* K, int is_device) {
+  if (!s) return -1;
+  const DevModel& m = s->m;
+  const size_t nx = 2 * (size_t)m.nv + m.na, nr = (size_t)m.nq + m.nv + m.na;
+  const bool clear = T == 0 || (!xref && !K);
+  if (!clear && (T < 1 || !xref || !K)) { s->err = "fb_rollout_feedback: T >= 1 steps with both xref and K (T = 0, or both NULL, clears the law)"; return -1; }
+  if (!clear && slice_bytes(0, nx) * FB_WPB > 48 * 1024) {
+    s->err = "fb_rollout_feedback: the input kernel keeps the tangent (2 nv + na = " + std::to_string(nx) + " floats) in shared memory, and it does not fit"; return -1; }
+  if (!clear && !is_device && (!all_finite(xref, T * nr) || !all_finite(K, T * m.nu * nx))) { s->err = "fb_rollout_feedback: non-finite xref or K"; return -1; }
+  dev_select(s);
+  if (sync_stream(s) != 0) return -2;          // a rollout in flight may still read the old law
+  scope_free(s, s->roll_fb_scope);
+  s->roll_xref = s->roll_K = nullptr; s->roll_fb_T = 0;
+  if (clear) return 0;
+  float *x, *k;
+  if (int rc = scope_alloc(s, s->roll_fb_scope, "out of device memory (rollout feedback)", [&] { x = dalloc<float>(s, T * nr); k = dalloc<float>(s, T * m.nu * nx); }))
+    return rc;
+  if (copy_async(s, x, xref, sizeof(float) * T * nr) != 0 || copy_async(s, k, K, sizeof(float) * T * m.nu * nx) != 0) return -2;
+  s->roll_xref = x; s->roll_K = k; s->roll_fb_T = T;
+  return is_device ? 0 : sync_stream(s);       // host arrays may be reused once the call returns
+}
+
+int fb_rollout(FbHandle s, const int32_t* slots, int n, int T, int n_substeps, const float* ctrl, const float* qfrc_applied,
+               const float* xfrc_applied, int is_device) {
+  if (!s) return -1;
+  const char* who = "fb_rollout";
+  if (state_ready(s, who) != 0) return -1;
+  const int N = s->d.N;
+  if (!slots || n < 1 || n > N) { s->err = "fb_rollout: 1 <= n <= n_envs (" + std::to_string(N) + ") rollouts, each with its slot"; return -1; }
+  if (T < 1) { s->err = "fb_rollout: T >= 1 control steps"; return -1; }
+  if (n_substeps < 1) { s->err = "fb_rollout: n_substeps >= 1"; return -1; }
+  if (!ctrl) { s->err = "fb_rollout: ctrl is NULL"; return -1; }
+  const bool app = qfrc_applied || xfrc_applied;
+  if (app && !s->d.qfrc_applied) {
+    s->err = "fb_rollout: applied-force sequences need the handle's applied-force arrays, which the state rows carry: allocate them (fb_applied_ptrs) before fb_state_bank";
+    return -1; }
+  if (s->roll_fb_T && s->roll_fb_T != T) {
+    s->err = "fb_rollout: the feedback law has " + std::to_string(s->roll_fb_T) + " steps and the call " + std::to_string(T) + " (fb_rollout_feedback)"; return -1; }
+  if (fd_slots_valid(s, who, slots, n) != 0) return -1;
+  const DevModel& m = s->m;
+  const size_t rows = (size_t)n * T, nq = m.nq, nv = m.nv, na = m.na, nu = m.nu, nsd = m.nsensordata, nxf = 6 * (size_t)m.nbody;
+  if (!is_device) {
+    if (!all_finite(ctrl, rows * nu)) { s->err = "fb_rollout: non-finite ctrl"; return -1; }
+    if ((qfrc_applied && !all_finite(qfrc_applied, rows * nv)) || (xfrc_applied && !all_finite(xfrc_applied, rows * nxf))) {
+      s->err = "fb_rollout: non-finite applied force"; return -1; }
+  }
+  dev_select(s);
+  s->roll_done = 0;
+  DevRoll& p = s->roll;
+  if (int rc = roll_grow(s, s->roll_scope, s->roll_cap, rows, 4 * (2 * nu + nq + nv + na + 2), "records", [&](size_t r) {
+        p.ctrl = dalloc<float>(s, r * nu); p.qpos = dalloc<float>(s, r * nq); p.qvel = dalloc<float>(s, r * nv); p.act = dalloc<float>(s, r * na);
+        p.ctrl_out = dalloc<float>(s, r * nu); p.time = dalloc<float>(s, r); p.flags = dalloc<int>(s, r); }))
+    return rc;
+  if (int rc = app ? roll_grow(s, s->roll_app_scope, s->roll_app_cap, rows, 4 * (nv + nxf), "applied-force inputs", [&](size_t r) {
+        s->roll_qf = dalloc<float>(s, r * nv); s->roll_xf = dalloc<float>(s, r * nxf); }) : 0)
+    return rc;
+  const bool sens = s->sens_on != 0;
+  if (int rc = sens ? roll_grow(s, s->roll_sd_scope, s->roll_sd_cap, rows, 8 * nsd, "sensor records", [&](size_t r) {
+        s->roll_sd = dalloc<float>(s, r * nsd); s->roll_sm = dalloc<float>(s, r * nsd); }) : 0)
+    return rc;
+  p.qfrc = qfrc_applied ? s->roll_qf : nullptr; p.xfrc = xfrc_applied ? s->roll_xf : nullptr;
+  p.sensordata = sens ? s->roll_sd : nullptr; p.sensor_mean = sens ? s->roll_sm : nullptr;
+  if (copy_async(s, (void*)p.ctrl, ctrl, 4 * rows * nu) != 0 || (qfrc_applied && copy_async(s, (void*)p.qfrc, qfrc_applied, 4 * rows * nv) != 0) ||
+      (xfrc_applied && copy_async(s, (void*)p.xfrc, xfrc_applied, 4 * rows * nxf) != 0)) return -2;
+  p.n = n; p.T = T; p.nsub = n_substeps;
+  p.xref = s->roll_fb_T ? s->roll_xref : nullptr; p.K = s->roll_fb_T ? s->roll_K : nullptr;
+  const size_t slice = p.K ? slice_bytes(0, 2 * nv + na) : 0;
+  if (int rc = fd_fan_out(s, slots, n, 1)) return rc;
+  launch_step1(s);                             // what the rows do not carry, as fb_state_load runs it
+  for (int t = 0; t < T; t++) {                // no host synchronisation or copy inside the horizon
+    p.t = t;
+    warp_launch(s, "rollout_input", N, slice, RollInput{s->m, s->d, p});
+    step_run(s, n_substeps);                   // fb_step's launches (the step graph)
+    warp_launch(s, "rollout_record", n, 0, RollRecord{s->m, s->d, p});
+  }
+  if (launch_check(s, who) != 0) return -2;
+  s->roll_done = n; s->roll_sens = sens;
+  return sync_stream(s);                       // (the fan-out list is a host vector)
+}
+
+int fb_rollout_read(FbHandle s, float* qpos, float* qvel, float* act, float* ctrl, float* time, int32_t* flags, int is_device) {
+  if (!s) return -1;
+  if (s->roll_done < 1) { s->err = "fb_rollout_read: no rollout to read (fb_rollout)"; return -1; }
+  const DevRoll& p = s->roll;
+  const size_t r = (size_t)s->roll_done * p.T;
+  return read_out(s, {{qpos, p.qpos, 0, 4 * r * s->m.nq, 1}, {qvel, p.qvel, 0, 4 * r * s->m.nv, 1}, {act, p.act, 0, 4 * r * s->m.na, 1},
+                      {ctrl, p.ctrl_out, 0, 4 * r * s->m.nu, 1}, {time, p.time, 0, 4 * r, 1}, {flags, p.flags, 0, 4 * r, 1}});
+}
+
+int fb_rollout_sensor_read(FbHandle s, float* sensordata, float* sensor_mean, int is_device) {
+  if (!s) return -1;
+  if (s->roll_done < 1) { s->err = "fb_rollout_sensor_read: no rollout to read (fb_rollout)"; return -1; }
+  if (!s->roll_sens) { s->err = "fb_rollout_sensor_read: the last fb_rollout ran with sensors off (fb_query_sensors)"; return -1; }
+  const size_t r = (size_t)s->roll_done * s->roll.T * s->m.nsensordata;
+  return read_out(s, {{sensordata, s->roll_sd, 0, 4 * r, 1}, {sensor_mean, s->roll_sm, 0, 4 * r, 1}});
 }
 
 }  // extern "C"

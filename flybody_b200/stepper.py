@@ -34,7 +34,8 @@ EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl'
            'fb_query_sensors', 'fb_inverse_sensor_read', 'fb_fd_sensor_read', 'fb_fd_inverse_sensor_read',
            'fb_param_size', 'fb_param_set', 'fb_param_get', 'fb_param_draws', 'fb_param_clear',
            'fb_fd_param_program', 'fb_fd_param_columns', 'fb_fd_param_transition', 'fb_fd_param_read', 'fb_fd_param_sensor_read',
-           'fb_fd_param_inverse', 'fb_fd_param_inverse_read', 'fb_fd_param_inverse_sensor_read']
+           'fb_fd_param_inverse', 'fb_fd_param_inverse_read', 'fb_fd_param_inverse_sensor_read',
+           'fb_rollout_feedback', 'fb_rollout', 'fb_rollout_read', 'fb_rollout_sensor_read']
 
 
 # enum FbTaskKind (FbTaskProgram.kind)
@@ -203,6 +204,10 @@ def load_library(path=None):
     lib.fb_fd_param_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int]
     lib.fb_fd_param_inverse_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
     lib.fb_fd_param_inverse_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
+    lib.fb_rollout_feedback.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+    lib.fb_rollout.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 3 + [C.c_int]
+    lib.fb_rollout_read.argtypes = [C.c_void_p] + [C.c_void_p] * 6 + [C.c_int]
+    lib.fb_rollout_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
     return lib
 
 
@@ -604,6 +609,77 @@ class BatchedStepper:
         m, (n, k) = self.model, getattr(self, '_fdpi_n', (0, 0))
         out = [np.zeros((n, k, m.nsensordata), np.float32), np.zeros((n, m.nsensordata), np.float32)]
         self._check(self._lib.fb_fd_param_inverse_sensor_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_fd_param_inverse_sensor_read')
+        return tuple(out)
+
+    # ---- batched rollouts (fb_rollout*; flybody_b200.rollout is the batched front end)
+    def _inputs(self, inputs, is_device):
+        """[(name, array, shape)] -> (pointers, host fp32 arrays to keep alive); device pointers (ints) pass through with is_device"""
+        if is_device:
+            return [None if x is None else C.c_void_p(int(x)) for _, x, _ in inputs], None
+        keep = [None if x is None else np.ascontiguousarray(np.asarray(x, np.float32)) for _, x, _ in inputs]
+        for (name, _, shape), x in zip(inputs, keep):
+            if x is not None and x.shape != shape:
+                raise ValueError(f'{name} {x.shape} against {shape}')
+        return [None if x is None else x.ctypes.data for x in keep], keep
+
+    def rollout_feedback(self, x_ref=None, K=None, T=None, is_device=False):
+        """the feedback law of the rollouts that follow: ctrl = ctrl_t + K_t (x_t - x_ref_t), x_ref [T, nq + nv + na], K [T, nu, nx]
+        (host arrays, or device pointers with is_device=True and T given); None for both clears it (see the header)"""
+        m = self.model
+        if x_ref is None and K is None:
+            self._check(self._lib.fb_rollout_feedback(self._h, 0, None, None, 0), 'fb_rollout_feedback')
+            return
+        T = int(T if is_device else np.shape(x_ref)[0])
+        ptrs, _keep = self._inputs([('x_ref', x_ref, (T, m.nq + m.nv + m.na)), ('K', K, (T, m.nu, 2 * m.nv + m.na))], is_device)
+        self._check(self._lib.fb_rollout_feedback(self._h, T, *ptrs, int(bool(is_device))), 'fb_rollout_feedback')
+
+    def rollout(self, slots, ctrl, n_substeps=1, qfrc_applied=None, xfrc_applied=None, T=None, is_device=False):
+        """rollout i from bank row slots[i] in env i: ctrl [n, T, nu], optional qfrc_applied [n, T, nv] and xfrc_applied [n, T, nbody, 6]
+        (host arrays, or device pointers with is_device=True and T given); T control steps of n_substeps substeps.  The envs' states
+        are a workspace afterwards.  Read the records with rollout_read()."""
+        m = self.model
+        s = np.ascontiguousarray(np.asarray(slots).reshape(-1), np.int32)
+        n = len(s)
+        T = int(T if is_device else np.shape(ctrl)[1])
+        ptrs, _keep = self._inputs([('ctrl', ctrl, (n, T, m.nu)), ('qfrc_applied', qfrc_applied, (n, T, m.nv)),
+                                    ('xfrc_applied', xfrc_applied, (n, T, m.nbody, 6))], is_device)
+        self._check(self._lib.fb_rollout(self._h, s.ctypes.data, n, T, int(n_substeps), *ptrs, int(bool(is_device))), 'fb_rollout')
+        self._roll = (n, T)
+
+    def _outputs(self, out, shapes, dtypes):
+        """caller-provided outputs (numpy arrays or torch tensors, C-contiguous, of the given shapes and dtypes) or new numpy arrays ->
+        (arrays, pointers, is_device: a CUDA tensor among them)"""
+        if out is None:
+            out = [np.zeros(sh, dt) for sh, dt in zip(shapes, dtypes)]
+        if len(out) != len(shapes):
+            raise ValueError(f'{len(out)} outputs against {len(shapes)}')
+        ptrs, dev = [], False
+        for x, sh, dt in zip(out, shapes, dtypes):
+            if isinstance(x, np.ndarray):
+                ok = x.dtype == dt and x.flags.c_contiguous
+                ptrs.append(x.ctypes.data)
+            else:                                                    # a torch tensor
+                ok = str(x.dtype) == f'torch.{np.dtype(dt).name}' and x.is_contiguous()
+                ptrs.append(x.data_ptr())
+                dev = dev or x.is_cuda
+            if not ok or tuple(x.shape) != tuple(sh):
+                raise ValueError(f'output {tuple(x.shape)} {x.dtype} against a contiguous {tuple(sh)} {np.dtype(dt).name}')
+        return out, ptrs, dev
+
+    def rollout_read(self, out=None):
+        """-> (qpos [n, T, nq], qvel [n, T, nv], act [n, T, na], ctrl [n, T, nu], time [n, T] f32, flags [n, T] i32) of the last
+        rollout; out: the six arrays to fill instead (numpy arrays, or torch tensors, CUDA ones by device pointer)"""
+        m, (n, T) = self.model, getattr(self, '_roll', (0, 0))
+        shapes = [(n, T, m.nq), (n, T, m.nv), (n, T, m.na), (n, T, m.nu), (n, T), (n, T)]
+        out, ptrs, dev = self._outputs(out, shapes, [np.float32] * 5 + [np.int32])
+        self._check(self._lib.fb_rollout_read(self._h, *ptrs, int(dev)), 'fb_rollout_read')
+        return tuple(out)
+
+    def rollout_sensor_read(self, out=None):
+        """-> (sensordata [n, T, nsd], sensor_mean [n, T, nsd]) f32 of the last rollout (run with sensors on); out as rollout_read's"""
+        m, (n, T) = self.model, getattr(self, '_roll', (0, 0))
+        out, ptrs, dev = self._outputs(out, [(n, T, m.nsensordata)] * 2, [np.float32] * 2)
+        self._check(self._lib.fb_rollout_sensor_read(self._h, *ptrs, int(dev)), 'fb_rollout_sensor_read')
         return tuple(out)
 
     def reset(self, qpos=None, qvel=None, env_ids=None):

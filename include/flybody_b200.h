@@ -660,6 +660,35 @@ int fb_fd_param_sensor_read(FbHandle h, float* dsdp, float* sensordata, int is_d
 int fb_fd_param_inverse(FbHandle h, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device);
 int fb_fd_param_inverse_read(FbHandle h, float* DfDp, float* qfrc_inverse, int is_device);
 int fb_fd_param_inverse_sensor_read(FbHandle h, float* DsDp, float* sensordata, int is_device);
+/* Batched rollouts (MuJoCo's mujoco.rollout.rollout, and the host loop of set_control, step and field reads it replaces): n rollouts
+ * of T control steps, each step n_substeps substeps (mj_step2; mj_step1) with ctrl held over them.  Rollout i runs in env i from
+ * state-bank row slots[i] (slots may repeat: K rollouts from one state); envs n .. n_envs-1 run a copy of the last rollout, whose
+ * outputs are not written (the transition query's fan-out).  Each control step is an input kernel, the step graph fb_step replays and
+ * a record kernel: no host synchronisation or copy inside the horizon, and no change to the step kernels.  Afterwards the envs are a
+ * workspace (their state is that of the rollouts' last step); the bank and the other queries' results are untouched.
+ *   Inputs (host rows, or device pointers when is_device): ctrl [n][T][nu]; step t writes row t into d->ctrl before its first substep,
+ *   unclamped (the actuation stage clamps ctrl-limited actuators, as it does for d->ctrl).  qfrc_applied [n][T][nv] and xfrc_applied
+ *   [n][T][nbody][6] (either may be NULL) are written the same way (MuJoCo rollout's control_spec for applied forces); without them the
+ *   row's applied forces persist.  They need the applied-force arrays (fb_applied_ptrs) before the bank is laid out.
+ *   Feedback (fb_rollout_feedback, set once for the calls that follow; T = 0 or both NULL clears it): nominal states xref
+ *   [T][nq + nv + na] and gains K [T][nu][nx], nx = 2 nv + na, shared by every rollout.  Step t writes ctrl = u_t + K_t (x_t - xref_t),
+ *   x_t the state the step starts from and the difference fb_fd_transition's tangent (mj_differentiatePos(xref qpos, qpos) per joint,
+ *   then qvel and act), so gains from a Riccati recursion on its A and B apply without conversion.  Fixed order: a rollout's bits do
+ *   not depend on its slot or on the batch size.
+ *   Records (fb_rollout_read), after control step t in row [i][t]: qpos [n][T][nq], qvel, act, ctrl as written, time [n][T] and the
+ *   env's flags [n][T].  With fb_query_sensors on (fb_rollout_sensor_read): sensordata [n][T][nsd], what fb_get(FB_SENSORDATA) returns
+ *   after the step, and sensor_mean, what fb_get(FB_SENSOR_MEAN) returns (the same division by n_substeps).  The buffers are allocated
+ *   on first use and grown when n T grows; -4 with a message when they do not fit.
+ * Errors: no bank, n < 1 or n > n_envs, T < 1, n_substeps < 1, NULL ctrl, a slot out of range, never written or saved while its env
+ * was held for a reset, a non-finite host input, applied-force sequences without the applied-force arrays, a feedback law of another
+ * horizon.  fb_rollout synchronises; a device input is not checked.  fb_rollout_feedback: T >= 1 with both arrays, a tangent that does
+ * not fit in shared memory, non-finite host values; it synchronises with host arrays.  The reads synchronise (any pointer may be NULL;
+ * is_device: device pointers) and refuse before any rollout, or for sensors after a rollout with sensors off.                      */
+int fb_rollout_feedback(FbHandle h, int T, const float* xref, const float* K, int is_device);
+int fb_rollout(FbHandle h, const int32_t* slots, int n, int T, int n_substeps, const float* ctrl, const float* qfrc_applied,
+               const float* xfrc_applied, int is_device);
+int fb_rollout_read(FbHandle h, float* qpos, float* qvel, float* act, float* ctrl, float* time, int32_t* flags, int is_device);
+int fb_rollout_sensor_read(FbHandle h, float* sensordata, float* sensor_mean, int is_device);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
