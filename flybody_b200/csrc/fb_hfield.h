@@ -1,7 +1,7 @@
 // fb_hfield.h -- convex geom against a heightfield (MuJoCo mjc_ConvexHField, engine_collision_convex.c; restated from memory).
-// GROUNDWORK for SURVEY.md 8(f).1 (vision_guided_flight): no compiled model carries a heightfield yet and no
-// step kernel calls this; it is compiled into the library, exercised through the emulation hook fb_emu_convex_hfield and held
-// against the fp64 CPU restatement (`orc_convex_hfield`) in tests/test_hfield.py.
+// The heightfield stage of the step (fb_hf_kernel / fb_hf_kernel_ids, models with a terrain geom: the `vision` variant) calls
+// col_convex_hfield through khf_narrow; the test hook fb_emu_convex_hfield runs it alone.  Both are held against the fp64 CPU
+// restatement (`orc_convex_hfield`) prism by prism and contact by contact in tests/test_hfield_gates.py.
 //
 // In the heightfield's frame the grid cells under the geom's bounding box are walked row by row as a triangle strip; every
 // triangle tops a prism that reaches down to the base, its top raised by the margin; each prism goes through MPR against the
@@ -81,10 +81,11 @@ FB_DEVN int hf_mpr_penetration(const HfPrism& o1, D3 c1, const MprObj& o2, float
     MPR_EXPAND()
   }
 }
-// contacts of one geom with the heightfield, in world coordinates; returns their number (<= max)
+// contacts of one geom with the heightfield, in world coordinates; returns their number (<= max).  prism (optional, the tests'
+// hook): per contact the triangle it came from, (row * ncol + column) * 2 + i, the triangle completed at strip vertex (column, row + i)
 struct HfCon { float dist; V3 pos, n; };
 FB_DEV int col_convex_hfield(HfCon* out, int max, float margin, int type, V3 gp, const M3& gm, V3 gs,
-                             V3 hp, const M3& hm, const float* hf_size, int nrow, int ncol, const float* data) {
+                             V3 hp, const M3& hm, const float* hf_size, int nrow, int ncol, const float* data, int* prism = nullptr) {
   // the geom in the heightfield's frame, origin shifted to the geom's footprint for fp32 resolution
   const V3 rel = mulT(hm, gp - hp);
   MprObj g; g.size = d3(gs.x, gs.y, gs.z); g.type = type; g.margin = 0;
@@ -120,6 +121,7 @@ FB_DEV int col_convex_hfield(HfCon* out, int max, float margin, int type, V3 gp,
       o.dist = (float)(margin - depth);
       o.pos = mul(hm, v3((float)cp.x, (float)cp.y, (float)cp.z) + rel) + hp;
       o.n = mul(hm, v3((float)dir.x, (float)dir.y, (float)dir.z));
+      if (prism) prism[cnt] = (r * ncol + c) * 2 + i;
       if (++cnt >= max) return cnt;
     }
   }
@@ -130,10 +132,11 @@ FB_DEV int col_convex_hfield(HfCon* out, int max, float margin, int type, V3 gp,
 // Heightfield contacts of one env, appended to the contact list after the collision kernel (fb_hfield_collision).  Runs as
 // its own launch between `col` and `proj`, and only for models that carry a heightfield: the step kernels of the other
 // models are untouched.  Phase 0: lane l takes the pairs l, l + 32, ... (terrain, geom): bounding-sphere test against the
-// highest point of the env's terrain, then the prism walk; up to FB_HF_PER_GEOM contacts per geom go to the staging
-// slots 4 k + i of pair k (free again after the collision kernel's compaction).  Phase 1: lane 0 appends them in pair order.
+// highest point under the geom's footprint, then the prism walk; up to FB_HF_PER_GEOM contacts per geom go to the staging
+// slots 4 k + i of pair k (free again after the collision kernel's compaction), and the first unused slot of the four is marked
+// with geom id -1.  Phase 1: lane 0 appends them in pair order, each pair up to its mark.  The staging record holds the 4 slots
+// of all FB_MAXCAND pairs and nothing else, so every npair the ABI accepts keeps its contacts apart.
 #define FB_HF_PER_GEOM 4
-#define FB_HF_CNT(k) AT(d.tmp_geom, 1000 + (k))
 struct DevHf { int geom, nrow, ncol, npair; float size[4]; const int* pair_geom; const float* data; const float* hmax; };
 FB_DEV void khf_narrow(const DevModel& m, const DevData& d, const DevHf& p, int e, int y) {
   // (geom positions are stored relative to the env's reference point, like every spatial quantity of the step: only
@@ -146,14 +149,14 @@ FB_DEV void khf_narrow(const DevModel& m, const DevData& d, const DevHf& p, int 
     const float margin = fmaxf(m.geom_margin[p.geom], m.geom_margin[g]);
     int n = 0;
     // bounding sphere against the highest grid point under its footprint (the arena's rim rises to "horizon mountains" of 4-5
-    // length units, so the terrain-wide maximum would never reject a fly cruising at 0.5-0.8; the terrain frame is upright,
-    // hills.py:205-211)
+    // length units, so the terrain-wide maximum would never reject a fly cruising at 0.5-0.8).  The test runs in the terrain's
+    // frame, as the prism walk does: the sphere is the same in every frame, only its centre is carried over.
     const float rb = m.geom_rbound[g] + margin;
-    const bool upright = hm.m[0] > 0.9999f && hm.m[4] > 0.9999f && hm.m[8] > 0.9999f;      // any other terrain frame: no pre-test
-    bool near = !upright || gp.z - rb <= hp.z + p.hmax[e] * p.size[2];
-    if (near && upright) {
-      const float fx0 = (gp.x - hp.x - rb + p.size[0]) / (2 * p.size[0]) * (p.ncol - 1), fx1 = (gp.x - hp.x + rb + p.size[0]) / (2 * p.size[0]) * (p.ncol - 1);
-      const float fy0 = (gp.y - hp.y - rb + p.size[1]) / (2 * p.size[1]) * (p.nrow - 1), fy1 = (gp.y - hp.y + rb + p.size[1]) / (2 * p.size[1]) * (p.nrow - 1);
+    const V3 rel = mulT(hm, gp - hp);
+    bool near = rel.z - rb <= p.hmax[e] * p.size[2];
+    if (near) {
+      const float fx0 = (rel.x - rb + p.size[0]) / (2 * p.size[0]) * (p.ncol - 1), fx1 = (rel.x + rb + p.size[0]) / (2 * p.size[0]) * (p.ncol - 1);
+      const float fy0 = (rel.y - rb + p.size[1]) / (2 * p.size[1]) * (p.nrow - 1), fy1 = (rel.y + rb + p.size[1]) / (2 * p.size[1]) * (p.nrow - 1);
       int c0 = (int)floorf(fx0), c1 = (int)ceilf(fx1), r0 = (int)floorf(fy0), r1 = (int)ceilf(fy1);
       if (c1 < 0 || r1 < 0 || c0 > p.ncol - 1 || r0 > p.nrow - 1) near = false;            // beside the terrain
       else {
@@ -161,7 +164,7 @@ FB_DEV void khf_narrow(const DevModel& m, const DevData& d, const DevHf& p, int 
         float top = 0.0f;
         if ((c1 - c0 + 1) * (r1 - r0 + 1) <= 64) { for (int r = r0; r <= r1; r++) for (int c = c0; c <= c1; c++) top = fmaxf(top, data[(size_t)r * p.ncol + c]); }
         else top = p.hmax[e];
-        near = gp.z - rb <= hp.z + top * p.size[2];
+        near = rel.z - rb <= top * p.size[2];
       }
     }
     if (near) {
@@ -170,16 +173,16 @@ FB_DEV void khf_narrow(const DevModel& m, const DevData& d, const DevHf& p, int 
       for (int i = 0; i < n; i++) { rc[i].dist = c[i].dist; rc[i].pos = c[i].pos; rc[i].n = c[i].n; rc[i].t = v3(0, 0, 0); }
       col_store(m, d, e, k, rc, n, p.geom, g);
     }
-    FB_HF_CNT(k) = n;
+    if (n < FB_HF_PER_GEOM) AT(d.tmp_geom, 2 * (FB_HF_PER_GEOM * k + n)) = -1;
   }
 }
 FB_DEV void khf_append(const DevModel& m, const DevData& d, const DevHf& p, int e, int y) {
   if (y != 0) return;
   int dst = AT(d.ncon, 0);
   for (int k = 0; k < p.npair; k++) {
-    const int cnt = FB_HF_CNT(k);
-    for (int i = 0; i < cnt; i++, dst++) {
-      const int src = 4 * k + i;
+    for (int i = 0; i < FB_HF_PER_GEOM; i++, dst++) {
+      const int src = FB_HF_PER_GEOM * k + i;
+      if (AT(d.tmp_geom, 2 * src) < 0) break;
       if (dst >= FB_MAXCON) { FB_FLAG_OR(2); AT(d.ncon, 0) = FB_MAXCON; return; }
       AT(d.con_dist, dst) = CON_F(d.tmp_con, src, 0, 13);
       for (int c = 0; c < 3; c++) CON_F(d.con_pos, dst, c, 3) = CON_F(d.tmp_con, src, 1 + c, 13);

@@ -894,13 +894,19 @@ int fb_destroy(FbHandle s) {
 extern "C" int fb_clk_read(FbHandle s, long long* dst) { if (!s) return -1; cudaStreamSynchronize(s->stream); cudaMemcpy(dst, s->d.clk, sizeof(long long) * 32 * 4096, cudaMemcpyDeviceToHost); return (int)(s->launches % 4096); }
 #endif
 #ifdef FB_EMU
-extern "C" int fb_emu_convex_hfield(int type, const float* gp, const float* gm, const float* gs, float margin, const float* hp, const float* hm,
-                                    const float* hf_size, int nrow, int ncol, const float* data, float* out /* [max][7] */, int max) {
+// host-emulation build only (tests): one geom against a heightfield; out [max][7] = dist, pos[3], normal[3]; prism (may be null):
+// per contact the triangle of the walk it came from (col_convex_hfield)
+extern "C" int fb_emu_convex_hfield_prisms(int type, const float* gp, const float* gm, const float* gs, float margin, const float* hp, const float* hm,
+                                           const float* hf_size, int nrow, int ncol, const float* data, float* out, int max, int* prism) {
   HfCon c[64]; M3 Gm, Hm; for (int k = 0; k < 9; k++) { Gm.m[k] = gm[k]; Hm.m[k] = hm[k]; }
   if (max > 64) max = 64;
-  int n = col_convex_hfield(c, max, margin, type, v3(gp[0], gp[1], gp[2]), Gm, v3(gs[0], gs[1], gs[2]), v3(hp[0], hp[1], hp[2]), Hm, hf_size, nrow, ncol, data);
+  int n = col_convex_hfield(c, max, margin, type, v3(gp[0], gp[1], gp[2]), Gm, v3(gs[0], gs[1], gs[2]), v3(hp[0], hp[1], hp[2]), Hm, hf_size, nrow, ncol, data, prism);
   for (int k = 0; k < n; k++) { out[7 * k] = c[k].dist; out[7 * k + 1] = c[k].pos.x; out[7 * k + 2] = c[k].pos.y; out[7 * k + 3] = c[k].pos.z; out[7 * k + 4] = c[k].n.x; out[7 * k + 5] = c[k].n.y; out[7 * k + 6] = c[k].n.z; }
   return n;
+}
+extern "C" int fb_emu_convex_hfield(int type, const float* gp, const float* gm, const float* gs, float margin, const float* hp, const float* hm,
+                                    const float* hf_size, int nrow, int ncol, const float* data, float* out /* [max][7] */, int max) {
+  return fb_emu_convex_hfield_prisms(type, gp, gm, gs, margin, hp, hm, hf_size, nrow, ncol, data, out, max, nullptr);
 }
 extern "C" void fb_emu_convex_stats(long* out) { for (int i = 0; i < 4; i++) { out[i] = g_convex_stats[i]; g_convex_stats[i] = 0; } }
 // host-emulation build only (tests): the fp32 generic-convex narrowphase on one pair; out = dist, pos[3], normal[3]

@@ -444,8 +444,8 @@ int fb_task_set_reset_noise(FbHandle h, float amp);
 int fb_task_request_reset(FbHandle h, const int32_t* env_ids, int n);
 /* Per-env count of episodes started so far (resets done by the device-side task logic), int32 [n_envs] to the host.    */
 int fb_task_episodes(FbHandle h, int32_t* dst);
-/* Terrain bank for the device-side vision task: K heightfields [K][nrow * ncol] (world units, the grid of fb_hfield_collision /
- * fb_eye_program); a resetting env copies one of them into its own heightfield (collision + eyes).                      */
+/* Terrain bank for the device-side vision task: K heightfields [K][nrow * ncol] (heights as fb_hfield_write takes them, the grid
+ * of fb_hfield_collision / fb_eye_program); a resetting env copies one of them into its own heightfield (collision + eyes).  */
 int fb_hfield_bank(FbHandle h, int n_terrain, const float* heights);
 /* Rows of 8 uniform numbers in [0,1) consumed by the listed envs' next reset instead of the device's counter hash (FB_TASK_VISION:
  * target height, target speed, start x, start y, wing-beat phase, terrain pick; FB_TASK_FLIGHT: wing-beat phase) -- lets a test feed the device the
@@ -472,11 +472,13 @@ typedef struct FbEyeProgram {
 } FbEyeProgram;
 int fb_eye_program(FbHandle h, const FbEyeProgram* p);
 /* Heightfield collision (MuJoCo mjc_ConvexHField; the terrain of tasks/arenas/hills.py): `geom` is the model's heightfield geom
- * (pose and contact parameters come from the model), size = (x half extent, y half extent, elevation scale, base depth), the grid
- * is nrow x ncol, pair_geom lists the geoms that can touch it.  Adds one kernel between collision and constraint rows.  The
- * per-env heights are the ones of fb_hfield_write (shared with the eye cameras), as fractions of the elevation scale.       */
+ * (pose and contact parameters come from the model; any pose), size = (x half extent, y half extent, elevation scale, base depth),
+ * the grid is nrow x ncol, pair_geom lists the 1 .. 192 (FB_MAXCAND) geoms that can touch it (repeats allowed), up to 4 contacts
+ * each.  Adds one kernel between collision and constraint rows.  The per-env heights h are the ones of fb_hfield_write (shared
+ * with the eye cameras): the surface lies h * size[2] above the terrain geom's frame.                                       */
 int fb_hfield_collision(FbHandle h, int geom, const float* size, int nrow, int ncol, const int32_t* pair_geom, int npair);
-/* Heights (world units) of the listed envs' terrains, rows [n][nrow * ncol]; envs never written are flat.            */
+/* Heights h of the listed envs' terrains, rows [n][nrow * ncol]; envs never written are flat.  The collision stage scales them
+ * by the elevation scale size[2] of fb_hfield_collision (1 for the `vision` model, where h is in world units).             */
 int fb_hfield_write(FbHandle h, const int32_t* env_ids, int n, const float* heights);
 /* Render every env's eyes from the current poses into the library's buffer [n_envs][n_cam][size][size][3] (uint8).   */
 int fb_render_eyes(FbHandle h);

@@ -68,7 +68,7 @@ typedef struct OrcData {
   int solver_niter, flags;
   double solver_tolerance;      /* <=0 -> use model opt_tolerance */
   double *wk;                   /* scratch nv*nv + ... */
-  /* optional heightfield terrain (orc_set_hfield): geom id, grid, heights as fractions of the elevation scale, geoms that can touch it */
+  /* optional heightfield terrain (orc_set_hfield): geom id, grid, heights (scaled by hf_size[2]), geoms that can touch it */
   int hf_geom, hf_nrow, hf_ncol, hf_npair; int* hf_pair; double hf_size[4]; double* hf_data;
 } OrcData;
 
@@ -847,13 +847,15 @@ static int col_convex(RawCon* c, double margin, int t1, const double* p1, const 
  * heightfield's frame, the grid cells under the geom's bounding box are walked row by row as a triangle strip; every triangle is
  * the top of a prism that reaches down to the base (-size[3]), its top raised by the margin, and each prism runs through the same
  * MPR as any convex pair (the prism's support function is the farthest of its six vertices, its centre their mean).  Every
- * intersecting prism yields one contact (MuJoCo caps them at mjMAXCONPAIR = 50): dist = margin - depth, normal from the
- * heightfield into the geom.  GROUNDWORK for SURVEY.md 8(f).1 (vision_guided_flight): no compiled model carries a heightfield
- * yet, so orc_collision does not call this; tests/test_hfield.py holds it against closed forms and the device code against it.
- * hf_size = (x half extent, y half extent, elevation scale, base depth); data [nrow][ncol] in [0, 1], row = y, col = x.        */
-int orc_convex_hfield(int type, const double* gpos, const double* gmat, const double* gsize, double margin,
-                      const double* hf_pos, const double* hf_mat, const double* hf_size, int nrow, int ncol, const double* data,
-                      double* out /* [max][7]: dist, pos[3], normal[3] */, int max) {
+ * intersecting prism yields one contact (MuJoCo caps them at mjMAXCONPAIR = 50; orc_collision keeps 4 per geom, as the device
+ * does): dist = margin - depth, normal from the heightfield into the geom.  orc_collision calls this for the terrain of a model
+ * with a heightfield (orc_set_hfield); tests/test_hfield.py holds it against closed forms, tests/test_hfield_gates.py the device
+ * code against it.  hf_size = (x half extent, y half extent, elevation scale, base depth); data [nrow][ncol] is scaled by
+ * hf_size[2], row = y, col = x.  tri (may be null): per contact the triangle it came from, (row * ncol + column) * 2 + i, the
+ * triangle completed at strip vertex (column, row + i).                                                                        */
+int orc_convex_hfield_prisms(int type, const double* gpos, const double* gmat, const double* gsize, double margin,
+                             const double* hf_pos, const double* hf_mat, const double* hf_size, int nrow, int ncol, const double* data,
+                             double* out /* [max][7]: dist, pos[3], normal[3] */, int max, int* tri) {
   double pos[3], mat[9], tmp[3];
   sub3(tmp,gpos,hf_pos); mulmatT3(pos,hf_mat,tmp);
   for (int c=0;c<3;c++) { double col[3]={gmat[c],gmat[3+c],gmat[6+c]}, r[3]; mulmatT3(r,hf_mat,col); mat[c]=r[0]; mat[3+c]=r[1]; mat[6+c]=r[2]; }
@@ -885,10 +887,16 @@ int orc_convex_hfield(int type, const double* gpos, const double* gmat, const do
       if (ccd_eq(dir[0],0)&&ccd_eq(dir[1],0)&&ccd_eq(dir[2],0)) continue;
       double* o=out+7*cnt;
       o[0]=margin-depth; mulmat3(tmp,hf_mat,cp); add3(o+1,tmp,hf_pos); mulmat3(o+4,hf_mat,dir);
+      if (tri) tri[cnt]=(r*ncol+c)*2+i;
       if (++cnt>=max) return cnt;
     }
   }
   return cnt;
+}
+int orc_convex_hfield(int type, const double* gpos, const double* gmat, const double* gsize, double margin,
+                      const double* hf_pos, const double* hf_mat, const double* hf_size, int nrow, int ncol, const double* data,
+                      double* out, int max) {
+  return orc_convex_hfield_prisms(type,gpos,gmat,gsize,margin,hf_pos,hf_mat,hf_size,nrow,ncol,data,out,max,NULL);
 }
 /* exported for the tests: one generic pair */
 int orc_convex_pair(int t1, const double* p1, const double* m1, const double* s1, int t2, const double* p2, const double* m2, const double* s2,

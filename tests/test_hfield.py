@@ -1,5 +1,6 @@
-"""Convex geom against a heightfield (MuJoCo mjc_ConvexHField; groundwork for SURVEY.md 8(f).1): the fp64 oracle
-(`orc_convex_hfield`) against closed forms, the device code (`fb_hfield.h`, through the host-emulation hook) against the oracle."""
+"""Convex geom against a heightfield (MuJoCo mjc_ConvexHField): the fp64 oracle (`orc_convex_hfield`) against closed forms, and the
+`vision` model's forward pass on a terrain against the oracle.  The device code (`fb_hfield.h`) is gated prism by prism and contact by
+contact in tests/test_hfield_gates.py."""
 import ctypes as C
 
 import numpy as np
@@ -7,17 +8,10 @@ import pytest
 
 import __graft_entry__ as ge
 from oracle import fly_oracle as fo
-from test_oracle_invariants import SPH, CAP, ELL, CYL, _rot
+from test_oracle_invariants import SPH, _rot
 
 dp = lambda a: np.ascontiguousarray(a, np.float64).ctypes.data_as(C.POINTER(C.c_double))
-fp = lambda a: np.ascontiguousarray(a, np.float32).ctypes.data_as(C.POINTER(C.c_float))
 EYE = np.eye(3)
-
-
-def _small_rot(ax, ay, az):
-    cx, sx, cy, sy, cz, sz = np.cos(ax), np.sin(ax), np.cos(ay), np.sin(ay), np.cos(az), np.sin(az)
-    Rx = np.array([[1, 0, 0], [0, cx, -sx], [0, sx, cx]]); Ry = np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]]); Rz = np.array([[cz, -sz, 0], [sz, cz, 0], [0, 0, 1]])
-    return Rz @ Ry @ Rx
 
 
 @pytest.fixture(scope='module')
@@ -25,9 +19,7 @@ def libs():
     ge.build()
     o = C.CDLL(fo.build())
     o.orc_convex_hfield.argtypes = [C.c_int] + [C.POINTER(C.c_double)] * 3 + [C.c_double] + [C.POINTER(C.c_double)] * 3 + [C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int]
-    e = C.CDLL(ge.EMU)
-    e.fb_emu_convex_hfield.argtypes = [C.c_int] + [C.POINTER(C.c_float)] * 3 + [C.c_float] + [C.POINTER(C.c_float)] * 3 + [C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int]
-    return o, e
+    return o
 
 
 def oracle_hf(o, t, p, R, s, margin, hp, hR, hsize, data, kmax=50):
@@ -37,19 +29,12 @@ def oracle_hf(o, t, p, R, s, margin, hp, hR, hsize, data, kmax=50):
     return out[:n]
 
 
-def device_hf(e, t, p, R, s, margin, hp, hR, hsize, data, kmax=50):
-    out = np.zeros((kmax, 7), np.float32)
-    n = e.fb_emu_convex_hfield(t, fp(p), fp(np.asarray(R).reshape(9)), fp(s), margin, fp(hp), fp(np.asarray(hR).reshape(9)), fp(hsize), data.shape[0], data.shape[1],
-                               fp(data), out.ctypes.data_as(C.POINTER(C.c_float)), kmax)
-    return out[:n].astype(np.float64)
-
-
 HSIZE = np.array([2.0, 2.0, 1.0, 0.05])            # 4 x 4 arena, elevation scale 1, base 0.05
 GRID = 41                                           # 0.1 spacing, as the flight arenas (hills.py:172-176)
 
 
 def test_oracle_sphere_on_flat_and_tilted_terrain(libs):
-    o, _ = libs
+    o = libs
     flat = np.full((GRID, GRID), 0.3)
     r = 0.04
     for z, hit in ((0.3 + r - 0.004, True), (0.3 + r + 0.003, False)):
@@ -82,44 +67,6 @@ def test_oracle_sphere_on_flat_and_tilted_terrain(libs):
     # outside the footprint or above the tallest point: nothing
     assert len(oracle_hf(o, SPH, [2.2, 0, 0.3], EYE, [r, 0, 0], 0.0, [0, 0, 0], EYE, HSIZE, flat)) == 0
     assert len(oracle_hf(o, SPH, [0, 0, 1.2], EYE, [r, 0, 0], 0.0, [0, 0, 0], EYE, HSIZE, flat)) == 0
-
-
-def test_device_matches_oracle_on_a_bumpy_terrain(libs):
-    o, e = libs
-    rs = np.random.RandomState(3)
-    xs = np.linspace(-2, 2, GRID)
-    terr = 0.3 + 0.15 * np.sin(2.1 * xs)[None, :] * np.cos(1.7 * xs)[:, None] + 0.02 * rs.uniform(size=(GRID, GRID))
-    hp, hR = np.array([0.2, -0.1, -0.01]), _small_rot(0.15, -0.1, 0.4)
-
-    def height(x, y):
-        fx, fy = (x + 2) / 0.1, (y + 2) / 0.1
-        ix, iy = int(np.clip(np.floor(fx), 0, GRID - 2)), int(np.clip(np.floor(fy), 0, GRID - 2))
-        tx, ty = fx - ix, fy - iy
-        return (terr[iy, ix] * (1 - tx) + terr[iy, ix + 1] * tx) * (1 - ty) + (terr[iy + 1, ix] * (1 - tx) + terr[iy + 1, ix + 1] * tx) * ty
-    n_hit = n_cmp = n_close = 0
-    for trial in range(120):
-        t = [SPH, CAP, ELL, CYL][trial % 4]
-        s = {SPH: [rs.uniform(0.02, 0.06), 0, 0], CAP: [rs.uniform(0.01, 0.03), rs.uniform(0.02, 0.08), 0],
-             ELL: list(rs.uniform(0.015, 0.07, 3)), CYL: [rs.uniform(0.01, 0.04), rs.uniform(0.01, 0.05), 0]}[t]
-        x, y = rs.uniform(-1.7, 1.7, 2)
-        # centre a little above / into the surface: shallow contacts and near misses
-        local = np.array([x, y, height(x, y) + max(s) * rs.uniform(0.2, 1.1)])
-        R = _rot(rs)
-        p, Rg = hR @ local + hp, hR @ R
-        a = oracle_hf(o, t, p, Rg, s, 0.0, hp, hR, HSIZE, terr)
-        b = device_hf(e, t, p, Rg, s, 0.0, hp, hR, HSIZE, terr)
-        n_hit += len(a) > 0
-        if len(a) == 0 and len(b) == 0:
-            continue
-        n_cmp += 1
-        # fp32 MPR against fp64 MPR: the deepest contact agrees; grazing prisms at the edge of the footprint may differ
-        if len(a) and len(b) and abs(a[:, 0].min() - b[:, 0].min()) < 5e-5 and abs(len(a) - len(b)) <= 1:
-            ka, kb = np.argmin(a[:, 0]), np.argmin(b[:, 0])
-            if np.allclose(a[ka, 4:], b[kb, 4:], atol=2e-2) and np.allclose(a[ka, 1:4], b[kb, 1:4], atol=2e-3):
-                n_close += 1
-    print("hfield parity: oracle hits", n_hit, "compared", n_cmp, "close", n_close)
-    assert n_hit > 40 and n_cmp > 40
-    assert n_close >= 0.95 * n_cmp, (n_close, n_cmp)
 
 
 def test_vision_model_terrain_contacts_match_the_oracle_through_the_step():
