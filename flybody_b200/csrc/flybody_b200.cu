@@ -34,6 +34,21 @@
 
 enum { K_ACT = 0, K_SMOOTH, K_REF, K_SOLVE, K_FINISH, K_POS, K_COL, K_CON, K_PROJ, K_VEL, K_SENS, K_PACK, K_MISC, K_NKIND };
 static const char* const kKindNames[K_NKIND] = {"act", "smooth", "ref", "solve", "finish", "pos", "col", "con", "proj", "vel", "sens", "pack", "misc"};
+// one finite-difference query (fb_fd.h): what it is, and its last call
+struct FdQuery {
+  const char *name, *cols, *what;         // the compute entry, its columns entry, what a read before any call finds missing
+  bool inverse, param;                    // evaluation: the inverse dynamics (else the step); inputs: parameter directions (else the state)
+  DevFdQ p = {};                          // the last call's kernel parameter; the blocks' and nominals' out are the query's outputs
+  std::vector<void*> scope, sens_scope;   // the outputs and the sensor outputs, allocated on the first call (with sensors on)
+  int done = 0; bool sens = false;        // problems of the last call; it ran with sensors on
+};
+// the scratch the queries share, no read returns it; each part is allocated on the first call that needs it
+struct FdScratch {
+  float* delta;                           // [Np]
+  DevInv inv; float *qpos, *qvel, *qacc;  // the inverses': every env's DevInv; the problems [N/2][nq], [N/2][nv], [N/2][nv]
+  float* rows;                            // [N/2][prm_stride] the parameter inverse's overlay rows
+  float* sens;                            // [Np][nsd] every env's sensors (of x for a transition, kinv_sensors' for an inverse)
+};
 struct FbSim {
   DevModel m; DevData d;
   int prof_on; double prof_ms[K_NKIND]; long long prof_n[K_NKIND];
@@ -50,21 +65,18 @@ struct FbSim {
   std::vector<double> h_qpos0;
   DevIk ik = {}; std::vector<void*> ik_scope; int ik_solved = 0;   // inverse kinematics (fb_ik_program): parameters and buffers; problems of the last solve
   DevInv inv = {}; std::vector<void*> inv_scope; int inv_done = 0;   // inverse dynamics (fb_inverse): buffers, allocated on first use; problems of the last call
-  DevFd fd = {}; std::vector<void*> fd_scope; int fd_cap = 0, fd_done = 0;   // transition Jacobians (fb_fd_transition): buffers for fd_cap problems, allocated on first use; problems of the last call
-  DevFdInv fdi = {}; std::vector<void*> fdi_scope; int fdi_cap = 0, fdi_done = 0;   // inverse-dynamics Jacobians (fb_fd_inverse): the same, with their own DevInv
-  // sensor outputs of the three dynamics queries (fb_query_sensors): buffers allocated on the first call with sensors on; *_sens: the
-  // last call of that query ran with sensors on
+  // sensor outputs of the dynamics queries (fb_query_sensors): buffers allocated on the first call with sensors on; inv_sens: the last
+  // fb_inverse ran with sensors on
   int sens_on = 0;
   float* inv_sd = nullptr; std::vector<void*> inv_sd_scope; bool inv_sens = false;              // fb_inverse: sensordata [Np][nsd]
-  DevFdSens fds = {}; std::vector<void*> fds_scope; bool fd_sens = false;                        // fb_fd_transition: C, D, sensordata
-  DevFdInvSens fdis = {}; float* fdi_env_sd = nullptr; std::vector<void*> fdis_scope; bool fdi_sens = false;   // fb_fd_inverse: every env's sensordata, DsD*
-  // parameter Jacobians (fb_fd_param_*): the direction program (k directions, any scale among them) and its device tables; the
-  // transition's and the inverse's buffers, allocated on first use for any program (n k < n ncol <= n_envs); problems of the last call
+  // finite-difference Jacobians (fb_fd_*; fb_fd.h): the four queries, the scratch they share, and the parameter direction program
+  // (k directions, any scale among them) with its device tables
+  FdQuery fd_tr{"fb_fd_transition", "fb_fd_columns", "transition", false, false};
+  FdQuery fd_inv{"fb_fd_inverse", "fb_fd_inverse_columns", "Jacobians", true, false};
+  FdQuery fd_ptr{"fb_fd_param_transition", "fb_fd_param_columns", "parameter Jacobians", false, true};
+  FdQuery fd_pinv{"fb_fd_param_inverse", "fb_fd_param_columns", "parameter Jacobians", true, true};
+  FdScratch fdx = {};
   DevFdPrmProg fdp_prog = {}; std::vector<void*> fdp_prog_scope; int fdp_k = 0; bool fdp_scale = false;
-  DevFdPrm fdp = {}; std::vector<void*> fdp_scope; int fdp_done = 0; bool fdp_sens = false;
-  DevFdSens fdps = {}; std::vector<void*> fdps_scope;                    // its sensors: snap, dsdp (the D slot), sensordata
-  DevFdPrmInv fdpi = {}; std::vector<void*> fdpi_scope; int fdpi_done = 0; bool fdpi_sens = false;
-  float* fdpi_env_sd = nullptr; std::vector<void*> fdpis_scope;            // its sensors: every env's sensordata (DsDp, sensordata in fdpi)
   // rollouts (fb_rollout*; fb_rollout.h): inputs and records of roll_cap rows (n T), grown on demand in three groups (ctrl and the
   // records; applied-force inputs; sensor records); the feedback law of roll_fb_T steps (fb_rollout_feedback); rows of the last call
   DevRoll roll = {}; std::vector<void*> roll_scope, roll_app_scope, roll_sd_scope; size_t roll_cap = 0, roll_app_cap = 0, roll_sd_cap = 0;
@@ -183,7 +195,7 @@ static int copy_sync(FbSim* s, void* dst, const void* src, size_t bytes) {
 // the outputs of a read, host or device: `rows` rows of `width` bytes, `spitch` bytes apart in the source and packed in the destination
 // (spitch 0: a contiguous array, one row); a NULL destination is skipped.  The stream is idle when it returns.
 struct ReadOut { void* dst; const void* src; size_t spitch, width, rows; };
-static int read_out(FbSim* s, std::initializer_list<ReadOut> outs) {
+static int read_out(FbSim* s, const std::vector<ReadOut>& outs) {
   for (const ReadOut& o : outs)
     if (o.dst && o.width && copy_rows_async(s, o.dst, o.width, o.src, o.spitch ? o.spitch : o.width, o.width, o.rows) != 0) return -2;
   return sync_stream(s);
@@ -2204,51 +2216,28 @@ int fb_inverse_read(FbHandle s, float* qfrc_inverse, float* qfrc_constraint, flo
 }  // extern "C"
 
 // -------------------------------------------------------------------------------------------
-// transition Jacobians (fb_fd_*; fb_fd.h): its own kernel parameter (DevFd) and buffers (fd_scope), allocated on first use
+// finite-difference Jacobians (fb_fd_*; fb_fd.h): the four queries run one path.  Each keeps its own outputs, so a query's results can
+// be read after another has run; the scratch (FdScratch) is shared
 struct FdPerturb {
-  DevModel m; DevData d; DevFd p;
+  DevModel m; DevData d; DevFdQ p;
   FB_DEVM void operator()(unsigned char*, int e) const { kfd_perturb(m, d, p, e); }
 };
 struct FdDiff {
-  DevModel m; DevData d; DevFd p;
+  DevModel m; DevData d; DevFdQ p;
   FB_DEVM void operator()(unsigned char*, int w) const { kfd_diff(m, d, p, w); }
 };
-// envs per problem of the transition (inputs dq, qvel, act, ctrl) or inverse-dynamics (dq, qvel, qacc) Jacobians
-static int fd_columns(const FbSim* s, bool inverse, int centered) {
-  const int nin = inverse ? 3 * s->m.nv : 2 * s->m.nv + s->m.na + s->m.nu;
-  return centered ? 1 + 2 * nin : 1 + nin;
-}
-static int fd_alloc(FbSim* s) {
-  if (s->fd.delta) return 0;
-  const DevModel& m = s->m;
-  const size_t nx = 2 * (size_t)m.nv + m.na, cap = std::max(1, s->d.N / fd_columns(s, false, 0));
-  DevFd& p = s->fd;
-  if (int rc = scope_alloc(s, s->fd_scope, "out of device memory (transition Jacobians)", [&] {
-        p.delta = dalloc<float>(s, s->d.Np); p.A = dalloc<float>(s, cap * nx * nx); p.B = dalloc<float>(s, cap * nx * std::max(m.nu, 1));
-        p.next = dalloc<float>(s, cap * (m.nq + m.nv + m.na)); })) {
-    s->fd = DevFd{}; return rc; }
-  s->fd_cap = (int)cap;
-  return 0;
-}
+struct FdRows {
+  DevData d; DevFdQ p;
+  FB_DEVM void operator()(unsigned char*, int w) const { kfd_rows(d, p, w); }
+};
 template <bool ACC> struct FdSnap {
-  DevModel m; DevData d; DevFdSens p;
-  FB_DEVM void operator()(unsigned char*, int e) const { kfd_snap(m, d, p, e, ACC); }
+  DevModel m; DevData d; float* snap;
+  FB_DEVM void operator()(unsigned char*, int e) const { kfd_snap(m, d, snap, e, ACC); }
 };
-struct FdSDiff {
-  DevModel m; DevFdSens p;
-  FB_DEVM void operator()(unsigned char*, int w) const { kfd_sdiff(m, p, w); }
-};
-static int fds_alloc(FbSim* s) {
-  if (s->fds.snap) return 0;
-  const DevModel& m = s->m;
-  const size_t nsd = m.nsensordata, nx = 2 * (size_t)m.nv + m.na, cap = s->fd_cap;
-  DevFdSens& q = s->fds;
-  if (int rc = scope_alloc(s, s->fds_scope, "out of device memory (transition sensor Jacobians)", [&] {
-        q.snap = dalloc<float>(s, (size_t)s->d.Np * nsd); q.C = dalloc<float>(s, cap * nsd * nx); q.D = dalloc<float>(s, cap * nsd * m.nu);
-        q.sensordata = dalloc<float>(s, cap * nsd); })) {
-    s->fds = DevFdSens{}; return rc; }
-  return 0;
-}
+static bool all_finite(const float* x, size_t n) { for (size_t i = 0; i < n; i++) if (!std::isfinite(x[i])) return false; return true; }
+// the inputs of one problem: (dq, qvel, act, ctrl), (dq, qvel, qacc) or the program's directions; and the envs it takes
+static int fd_inputs(const FbSim* s, const FdQuery& q) { return q.param ? s->fdp_k : q.inverse ? 3 * s->m.nv : 2 * s->m.nv + s->m.na + s->m.nu; }
+static int fd_columns(const FbSim* s, const FdQuery& q, int centered) { return 1 + (centered ? 2 : 1) * fd_inputs(s, q); }
 // the problems of a transition query: written bank rows, none saved while its env was held for a reset
 static int fd_slots_valid(FbSim* s, const char* who, const int32_t* slots, int n) {
   for (int k = 0; k < n; k++) {
@@ -2269,206 +2258,172 @@ static int fd_fan_out(FbSim* s, const int32_t* slots, int n, int ncol) {
   launch_state<true>(s, nullptr, sd, N);
   return 0;
 }
-// fb_step's launches, split after the first substep to snapshot the sensors of x (q.snap) of the first n envs
-static void fd_step_snap(FbSim* s, const DevFdSens& q, int n, int n_substeps) {
-  warp_launch(s, "fd_snap", n, 0, FdSnap<false>{s->m, s->d, q});
-  step_run(s, 1);
-  warp_launch(s, "fd_snap", n, 0, FdSnap<true>{s->m, s->d, q});
-  if (n_substeps > 1) step_run(s, n_substeps - 1);
+
+// the arguments of a compute entry: n problems (bank slots of a transition; host or device rows qpos, qvel, qacc of an inverse)
+struct FdCall { int n; const int32_t* slots; const float* in[3]; float eps; int centered, n_substeps, is_device; };
+static int fd_check(FbSim* s, const FdQuery& q, const FdCall& c) {
+  const std::string who = q.name;
+  if (q.inverse && !q.param && s->d.prm) {
+    s->err = who + ": the handle has a parameter overlay, and the columns are written from qpos, qvel and qacc alone (fb_param_clear first)"; return -1; }
+  if (q.param && !s->d.prm) {
+    s->err = who + ": the handle has no parameter overlay, and the columns nudge each problem's own parameters: " +
+             (q.inverse ? "fb_param_set first (problem i takes env i's parameters)" : "fb_param_set first, then fb_state_bank and fb_state_save the rows");
+    return -1; }
+  if (q.param && s->fdp_k < 1) { s->err = who + ": no direction program (fb_fd_param_program)"; return -1; }
+  if (!q.inverse && state_ready(s, q.name) != 0) return -1;
+  const int N = s->d.N, ncol = fd_columns(s, q, c.centered);
+  if ((!q.inverse && !c.slots) || c.n < 1 || (long long)c.n * ncol > N) {
+    s->err = who + ": 1 <= n problems with n * " + q.cols + " (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
+  if (q.inverse) {
+    if (!c.in[0] || !c.in[1] || !c.in[2]) { s->err = who + ": qpos, qvel and qacc must not be NULL"; return -1; }
+    const size_t cnt[3] = {(size_t)c.n * s->m.nq, (size_t)c.n * s->m.nv, (size_t)c.n * s->m.nv};
+    const char* what[3] = {"qpos", "qvel", "qacc"};
+    if (!c.is_device) for (int t = 0; t < 3; t++) if (!all_finite(c.in[t], cnt[t])) { s->err = who + ": non-finite " + what[t]; return -1; }
+  }
+  if (!(c.eps > 0.0f) || !std::isfinite(c.eps)) { s->err = who + ": eps must be positive and finite"; return -1; }
+  if (q.param && s->fdp_scale && !(c.eps < 1.0f)) { s->err = who + ": the program has scale directions, which need eps < 1"; return -1; }
+  if (!q.inverse && c.n_substeps < 1) { s->err = who + ": n_substeps >= 1"; return -1; }
+  return q.inverse ? 0 : fd_slots_valid(s, q.name, c.slots, c.n);
+}
+// the parts of the shared scratch a call of q needs, allocated on first use
+static int fd_scratch(FbSim* s, const FdQuery& q, bool sens) {
+  FdScratch x = s->fdx;                        // kept once every part this call adds is there
+  const size_t Np = s->d.Np, half = std::max(1, s->d.N / 2), nq = s->m.nq, nv = s->m.nv;
+  std::vector<void*> scope;
+  if (int rc = scope_alloc(s, scope, "out of device memory (finite-difference scratch)", [&] {
+        if (!x.delta) x.delta = dalloc<float>(s, Np);
+        if (q.inverse && !x.inv.qacc) {
+          x.inv.qacc = dalloc<float>(s, Np * nv); x.inv.qfrc_inverse = dalloc<float>(s, Np * nv);
+          x.inv.qfrc_constraint = dalloc<float>(s, Np * nv); x.inv.efc_force = dalloc<float>(s, Np * FB_MAXEFC);
+          x.qpos = dalloc<float>(s, half * nq); x.qvel = dalloc<float>(s, half * nv); x.qacc = dalloc<float>(s, half * nv);
+        }
+        if (q.inverse && q.param && !x.rows) x.rows = dalloc<float>(s, half * s->d.prm_stride);
+        if (sens && !x.sens) x.sens = dalloc<float>(s, Np * s->m.nsensordata); }))
+    return rc;
+  s->fdx = x;
+  return 0;
+}
+// the outputs of a call of nin inputs, their pointers aside: a block per range of inputs ((dq, qvel, act) and ctrl; dq, qvel and qacc;
+// the directions) and per source (the state or qfrc_inverse, qM for the dq inputs of the state inverse, the sensors), then the nominal
+// column's.  The sensor blocks are empty when sens is off.
+static void fd_layout(FbSim* s, FdQuery& q, int nin, bool sens) {
+  const DevModel& m = s->m;
+  const int nv = m.nv, nx = 2 * nv + m.na, nsd = sens ? m.nsensordata : 0;
+  const int nparts = q.param ? 1 : q.inverse ? 3 : 2, part[3] = {q.param ? nin : q.inverse ? nv : nx, q.inverse ? nv : m.nu, nv};
+  const float *src = q.inverse ? s->fdx.inv.qfrc_inverse : nullptr, *sd = s->fdx.sens;
+  DevFdQ& p = q.p;
+  p.nblk = 0;
+  auto blk = [&](const float* f, int stride, int L, int j0, int w, bool sensor) {
+    FdBlock& k = p.blk[p.nblk++];
+    k = FdBlock{f, (unsigned)stride, L, j0, w, q.inverse, sensor, k.out};
+  };
+  for (int t = 0, j0 = 0; t < nparts; j0 += part[t++]) blk(src, nv, q.inverse ? nv : nx, j0, part[t], false);
+  if (q.inverse && !q.param) blk(s->d.qM, s->d.rec, m.nM, 0, nv, false);
+  for (int t = 0, j0 = 0; t < nparts; j0 += part[t++]) blk(sd, nsd, nsd, j0, part[t], true);
+  p.nom[0] = FdNom{src, (unsigned)nv, q.inverse ? nv : m.nq + nv + m.na, p.nom[0].out};
+  p.nom[1] = FdNom{sd, (unsigned)nsd, nsd, p.nom[1].out};
+}
+// the outputs (sens: the sensor outputs), allocated once for every call the capacity rule admits: a problem takes 1 + nin envs or more,
+// so n nin < N and n <= N / 2.  A program's k is not known beforehand: its blocks (w = k) take the bound N - 1 of n k.
+static int fd_outputs(FbSim* s, FdQuery& q, int nin, bool sens) {
+  std::vector<void*>& scope = sens ? q.sens_scope : q.scope;
+  if (!scope.empty()) return 0;
+  const int N = s->d.N;
+  const size_t cap = std::max(1, q.param ? N / 2 : std::min(N / 2, (N - 1) / nin)), all = std::max(1, N - 1);
+  DevFdQ p = q.p;
+  if (int rc = scope_alloc(s, scope, sens ? "out of device memory (finite-difference sensor outputs)" : "out of device memory (finite-difference outputs)", [&] {
+        for (int o = 0; o < p.nblk; o++)
+          if (p.blk[o].sensor == sens) p.blk[o].out = dalloc<float>(s, p.blk[o].L * (q.param ? all : cap * p.blk[o].w));
+        p.nom[sens].out = dalloc<float>(s, cap * p.nom[sens].L); }))
+    return rc;
+  q.p = p;
+  return 0;
+}
+// a compute entry: the checks, scratch and outputs, the problems into the envs (the fan-out of bank rows, or an inverse's rows), then
+// perturb, evaluate and difference
+static int fd_run(FbSim* s, FdQuery& q, const FdCall& c) {
+  if (fd_check(s, q, c) != 0) return -1;
+  const int N = s->d.N, n = c.n, nin = fd_inputs(s, q), ncol = fd_columns(s, q, c.centered);
+  const bool sens = s->sens_on != 0, snap = sens && s->m.nsensordata > 0;
+  q.done = 0;
+  dev_select(s);
+  if (int rc = fd_scratch(s, q, sens)) return rc;
+  fd_layout(s, q, nin, sens);
+  if (int rc = fd_outputs(s, q, nin, false)) return rc;
+  if (sens) if (int rc = fd_outputs(s, q, nin, true)) return rc;
+  const FdScratch& x = s->fdx;
+  if (!q.inverse) { if (int rc = fd_fan_out(s, c.slots, n, ncol)) return rc; }
+  else if (copy_async(s, x.qpos, c.in[0], sizeof(float) * n * s->m.nq) != 0 || copy_async(s, x.qvel, c.in[1], sizeof(float) * n * s->m.nv) != 0 ||
+           copy_async(s, x.qacc, c.in[2], sizeof(float) * n * s->m.nv) != 0) return -2;
+  DevFdQ& p = q.p;
+  p.n = n; p.ncol = ncol; p.nin = nin; p.centered = c.centered != 0; p.eps = c.eps; p.delta = x.delta;
+  p.ju = q.inverse || q.param ? nin : 2 * s->m.nv + s->m.na;
+  p.g = q.param ? s->fdp_prog : DevFdPrmProg{};
+  p.qpos = q.inverse ? x.qpos : nullptr; p.qvel = x.qvel; p.qacc = x.qacc;
+  p.rows = q.inverse && q.param ? x.rows : nullptr;
+  p.inv = x.inv; p.inv.n = n * ncol;
+  if (p.rows) warp_launch(s, "fd_rows", n, 0, FdRows{s->d, p});
+  warp_launch(s, "fd_perturb", N, 0, FdPerturb{s->m, s->d, p});
+  launch_step1(s);                             // the position / velocity stage of the nudged states (an inverse's as fb_inverse runs it)
+  if (q.inverse) {
+    launch_inv(s, p.inv);
+    if (sens) launch_inv_sensors(s, p.inv, x.sens);
+  } else if (!snap) {
+    step_run(s, c.n_substeps);                 // fb_step's launches
+  } else {                                     // the same, split after the first substep to snapshot the sensors of x
+    warp_launch(s, "fd_snap", n * ncol, 0, FdSnap<false>{s->m, s->d, x.sens});
+    step_run(s, 1);
+    warp_launch(s, "fd_snap", n * ncol, 0, FdSnap<true>{s->m, s->d, x.sens});
+    if (c.n_substeps > 1) step_run(s, c.n_substeps - 1);
+  }
+  warp_launch(s, "fd_diff", n * nin, 0, FdDiff{s->m, s->d, p});
+  if (launch_check(s, q.name) != 0) return -2;
+  q.done = n; q.sens = sens;
+  return q.inverse && c.is_device ? 0 : sync_stream(s);   // host rows may be reused once the call returns; the fan-out list is a host vector
+}
+// a read entry: the outputs (sens: the sensor outputs) in the entry's order, the blocks and then the nominal column's (the next state:
+// qpos, qvel, act)
+static int fd_read(FbSim* s, const FdQuery& q, const char* who, bool sens, std::initializer_list<void*> dst) {
+  if (q.done < 1) { s->err = std::string(who) + ": no " + q.what + " to read (" + q.name + ")"; return -1; }
+  if (sens && !q.sens) { s->err = std::string(who) + ": the last " + q.name + " ran with sensors off (fb_query_sensors)"; return -1; }
+  const size_t n = q.done;
+  const DevFdQ& p = q.p;
+  void* const* d = dst.begin();
+  std::vector<ReadOut> outs;
+  for (int o = 0; o < p.nblk; o++) if (p.blk[o].sensor == sens) outs.push_back({*d++, p.blk[o].out, 0, 4 * n * p.blk[o].L * p.blk[o].w, 1});
+  const FdNom& c = p.nom[sens];
+  if (c.src || sens) outs.push_back({*d, c.out, 0, 4 * n * c.L, 1});
+  else {
+    const size_t w[3] = {(size_t)s->m.nq, (size_t)s->m.nv, (size_t)s->m.na};
+    for (size_t t = 0, at = 0; t < 3; at += w[t++]) outs.push_back({d[t], c.out + at, 4 * (size_t)c.L, 4 * w[t], n});
+  }
+  return read_out(s, outs);
 }
 
 extern "C" {
 
-int fb_fd_columns(FbHandle s, int centered) { return s ? fd_columns(s, false, centered != 0) : -1; }
+int fb_fd_columns(FbHandle s, int centered) { return s ? fd_columns(s, s->fd_tr, centered) : -1; }
+int fb_fd_inverse_columns(FbHandle s, int centered) { return s ? fd_columns(s, s->fd_inv, centered) : -1; }
 
 int fb_fd_transition(FbHandle s, const int32_t* slots, int n, float eps, int centered, int n_substeps) {
-  if (!s) return -1;
-  if (state_ready(s, "fb_fd_transition") != 0) return -1;
-  const int N = s->d.N, ncol = fd_columns(s, false, centered != 0);
-  if (!slots || n < 1 || (long long)n * ncol > N) {
-    s->err = "fb_fd_transition: 1 <= n problems with n * fb_fd_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
-  if (!(eps > 0.0f) || !std::isfinite(eps)) { s->err = "fb_fd_transition: eps must be positive and finite"; return -1; }
-  if (n_substeps < 1) { s->err = "fb_fd_transition: n_substeps >= 1"; return -1; }
-  if (fd_slots_valid(s, "fb_fd_transition", slots, n) != 0) return -1;
-  dev_select(s);
-  if (int rc = fd_alloc(s)) return rc;
-  const bool sens = s->sens_on != 0, snap = sens && s->m.nsensordata > 0;
-  if (sens) if (int rc = fds_alloc(s)) return rc;
-  if (int rc = fd_fan_out(s, slots, n, ncol)) return rc;
-  DevFd& p = s->fd;
-  p.n = n; p.ncol = ncol; p.nx = 2 * s->m.nv + s->m.na; p.nin = p.nx + s->m.nu; p.centered = centered != 0; p.eps = eps;
-  s->fd_done = 0;
-  warp_launch(s, "fd_perturb", N, 0, FdPerturb{s->m, s->d, p});
-  launch_step1(s);                             // the position / velocity stage of the nudged states
-  if (!snap) step_run(s, n_substeps);          // fb_step's launches
-  else { s->fds.fd = p; fd_step_snap(s, s->fds, n * ncol, n_substeps); }
-  warp_launch(s, "fd_diff", n * p.nin, 0, FdDiff{s->m, s->d, p});
-  if (snap) warp_launch(s, "fd_sdiff", n * p.nin, 0, FdSDiff{s->m, s->fds});
-  if (launch_check(s, "fb_fd_transition") != 0) return -2;
-  s->fd_done = n; s->fd_sens = sens;
-  return sync_stream(s);                       // (the fan-out list is a host vector)
+  return s ? fd_run(s, s->fd_tr, {n, slots, {}, eps, centered, n_substeps, 0}) : -1;
 }
-
-int fb_fd_sensor_read(FbHandle s, float* C, float* D, float* sensordata, int is_device) {
-  if (!s) return -1;
-  if (s->fd_done < 1) { s->err = "fb_fd_sensor_read: no transition to read (fb_fd_transition)"; return -1; }
-  if (!s->fd_sens) { s->err = "fb_fd_sensor_read: the last fb_fd_transition ran with sensors off (fb_query_sensors)"; return -1; }
-  const DevFdSens& q = s->fds;
-  const size_t n = (size_t)s->fd_done, nsd = (size_t)s->m.nsensordata, nx = (size_t)s->fd.nx, nu = (size_t)(s->fd.nin - s->fd.nx);
-  return read_out(s, {{C, q.C, 0, 4 * n * nsd * nx, 1}, {D, q.D, 0, 4 * n * nsd * nu, 1}, {sensordata, q.sensordata, 0, 4 * n * nsd, 1}});
-}
-
 int fb_fd_read(FbHandle s, float* A, float* B, float* qpos_next, float* qvel_next, float* act_next, int is_device) {
-  if (!s) return -1;
-  if (s->fd_done < 1) { s->err = "fb_fd_read: no transition to read (fb_fd_transition)"; return -1; }
-  const DevFd& p = s->fd;
-  const size_t n = (size_t)s->fd_done, nx = (size_t)p.nx, nu = (size_t)(p.nin - p.nx);
-  const size_t nq = s->m.nq, nv = s->m.nv, na = s->m.na, row = (nq + nv + na) * 4;
-  return read_out(s, {{A, p.A, 0, 4 * n * nx * nx, 1}, {B, p.B, 0, 4 * n * nx * nu, 1}, {qpos_next, p.next, row, nq * 4, n},
-                      {qvel_next, p.next + nq, row, nv * 4, n}, {act_next, p.next + nq + nv, row, na * 4, n}});
+  return s ? fd_read(s, s->fd_tr, "fb_fd_read", false, {A, B, qpos_next, qvel_next, act_next}) : -1;
 }
-
-}  // extern "C"
-
-// -------------------------------------------------------------------------------------------
-// inverse-dynamics Jacobians (fb_fd_inverse*; fb_fd.h): their own kernel parameter (DevFdInv, with its own DevInv) and buffers
-// (fdi_scope), allocated on first use; fb_inverse's DevInv is not touched
-struct FdiPerturb {
-  DevModel m; DevData d; DevFdInv p;
-  FB_DEVM void operator()(unsigned char*, int e) const { kfdi_perturb(m, d, p, e); }
-};
-struct FdiDiff {
-  DevModel m; DevData d; DevFdInv p;
-  FB_DEVM void operator()(unsigned char*, int w) const { kfdi_diff(m, d, p, w); }
-};
-static int fdi_alloc(FbSim* s) {
-  if (s->fdi.delta) return 0;
-  const size_t Np = (size_t)s->d.Np, nq = (size_t)s->m.nq, nv = (size_t)s->m.nv, nM = (size_t)s->m.nM;
-  const size_t cap = std::max(1, s->d.N / fd_columns(s, true, 0));
-  DevFdInv& p = s->fdi;
-  if (int rc = scope_alloc(s, s->fdi_scope, "out of device memory (inverse-dynamics Jacobians)", [&] {
-        p.qpos = dalloc<float>(s, cap * nq); p.qvel = dalloc<float>(s, cap * nv); p.qacc = dalloc<float>(s, cap * nv);
-        p.delta = dalloc<float>(s, Np);
-        p.inv.qacc = dalloc<float>(s, Np * nv); p.inv.qfrc_inverse = dalloc<float>(s, Np * nv);
-        p.inv.qfrc_constraint = dalloc<float>(s, Np * nv); p.inv.efc_force = dalloc<float>(s, Np * FB_MAXEFC);
-        p.DfDq = dalloc<float>(s, cap * nv * nv); p.DfDv = dalloc<float>(s, cap * nv * nv); p.DfDa = dalloc<float>(s, cap * nv * nv);
-        p.DmDq = dalloc<float>(s, cap * nv * nM); p.qfrc = dalloc<float>(s, cap * nv); })) {
-    s->fdi = DevFdInv{}; return rc; }
-  s->fdi_cap = (int)cap;
-  return 0;
+int fb_fd_sensor_read(FbHandle s, float* C, float* D, float* sensordata, int is_device) {
+  return s ? fd_read(s, s->fd_tr, "fb_fd_sensor_read", true, {C, D, sensordata}) : -1;
 }
-struct FdiSDiff {
-  DevModel m; DevFdInvSens p;
-  FB_DEVM void operator()(unsigned char*, int w) const { kfdi_sdiff(m, p, w); }
-};
-static int fdis_alloc(FbSim* s) {
-  if (s->fdi_env_sd) return 0;
-  const size_t nsd = s->m.nsensordata, nv = s->m.nv, cap = s->fdi_cap;
-  DevFdInvSens& q = s->fdis;
-  if (int rc = scope_alloc(s, s->fdis_scope, "out of device memory (inverse-dynamics sensor Jacobians)", [&] {
-        s->fdi_env_sd = dalloc<float>(s, (size_t)s->d.Np * nsd);
-        q.DsDq = dalloc<float>(s, cap * nv * nsd); q.DsDv = dalloc<float>(s, cap * nv * nsd); q.DsDa = dalloc<float>(s, cap * nv * nsd);
-        q.sensordata = dalloc<float>(s, cap * nsd); })) {
-    s->fdis = DevFdInvSens{}; s->fdi_env_sd = nullptr; return rc; }
-  q.sens = s->fdi_env_sd;
-  return 0;
-}
-
-extern "C" {
-
-int fb_fd_inverse_columns(FbHandle s, int centered) { return s ? fd_columns(s, true, centered != 0) : -1; }
 
 int fb_fd_inverse(FbHandle s, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device) {
-  if (!s) return -1;
-  if (s->d.prm) { s->err = "fb_fd_inverse: the handle has a parameter overlay, and the columns are written from qpos, qvel and qacc alone (fb_param_clear first)"; return -1; }
-  const int N = s->d.N, ncol = fd_columns(s, true, centered != 0);
-  if (n < 1 || (long long)n * ncol > N) {
-    s->err = "fb_fd_inverse: 1 <= n problems with n * fb_fd_inverse_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
-  if (!qpos || !qvel || !qacc) { s->err = "fb_fd_inverse: qpos, qvel and qacc must not be NULL"; return -1; }
-  const size_t nq = s->m.nq, nv = s->m.nv;
-  if (!is_device) {
-    const struct { const float* x; size_t cnt; const char* what; } ins[3] = {{qpos, n * nq, "qpos"}, {qvel, n * nv, "qvel"}, {qacc, n * nv, "qacc"}};
-    for (const auto& in : ins)
-      for (size_t i = 0; i < in.cnt; i++)
-        if (!std::isfinite(in.x[i])) { s->err = std::string("fb_fd_inverse: non-finite ") + in.what; return -1; }
-  }
-  if (!(eps > 0.0f) || !std::isfinite(eps)) { s->err = "fb_fd_inverse: eps must be positive and finite"; return -1; }
-  dev_select(s);
-  if (int rc = fdi_alloc(s)) return rc;
-  const bool sens = s->sens_on != 0, sdiff = sens && s->m.nsensordata > 0;
-  if (sens) if (int rc = fdis_alloc(s)) return rc;
-  DevFdInv& p = s->fdi;
-  if (copy_async(s, p.qpos, qpos, sizeof(float) * n * nq) != 0 || copy_async(s, p.qvel, qvel, sizeof(float) * n * nv) != 0 ||
-      copy_async(s, p.qacc, qacc, sizeof(float) * n * nv) != 0) return -2;
-  p.n = n; p.ncol = ncol; p.nin = 3 * (int)nv; p.centered = centered != 0; p.eps = eps;
-  p.inv.n = n * ncol;
-  s->fdi_done = 0;
-  warp_launch(s, "fdi_perturb", N, 0, FdiPerturb{s->m, s->d, p});   // fan-out and nudge
-  launch_step1(s);                             // the position / velocity stage of every env, as fb_inverse runs it
-  launch_inv(s, p.inv);
-  if (sdiff) launch_inv_sensors(s, p.inv, s->fdi_env_sd);
-  warp_launch(s, "fdi_diff", n * p.nin, 0, FdiDiff{s->m, s->d, p});
-  if (sdiff) { s->fdis.fdi = p; warp_launch(s, "fdi_sdiff", n * p.nin, 0, FdiSDiff{s->m, s->fdis}); }
-  if (launch_check(s, "fb_fd_inverse") != 0) return -2;
-  s->fdi_done = n; s->fdi_sens = sens;
-  return is_device ? 0 : sync_stream(s);       // host rows may be reused once the call returns
+  return s ? fd_run(s, s->fd_inv, {n, nullptr, {qpos, qvel, qacc}, eps, centered, 1, is_device}) : -1;
 }
-
-int fb_fd_inverse_sensor_read(FbHandle s, float* DsDq, float* DsDv, float* DsDa, float* sensordata, int is_device) {
-  if (!s) return -1;
-  if (s->fdi_done < 1) { s->err = "fb_fd_inverse_sensor_read: no Jacobians to read (fb_fd_inverse)"; return -1; }
-  if (!s->fdi_sens) { s->err = "fb_fd_inverse_sensor_read: the last fb_fd_inverse ran with sensors off (fb_query_sensors)"; return -1; }
-  const DevFdInvSens& q = s->fdis;
-  const size_t n = (size_t)s->fdi_done, nv = (size_t)s->m.nv, nsd = (size_t)s->m.nsensordata;
-  return read_out(s, {{DsDq, q.DsDq, 0, 4 * n * nv * nsd, 1}, {DsDv, q.DsDv, 0, 4 * n * nv * nsd, 1}, {DsDa, q.DsDa, 0, 4 * n * nv * nsd, 1},
-                      {sensordata, q.sensordata, 0, 4 * n * nsd, 1}});
-}
-
 int fb_fd_inverse_read(FbHandle s, float* DfDq, float* DfDv, float* DfDa, float* DmDq, float* qfrc_inverse, int is_device) {
-  if (!s) return -1;
-  if (s->fdi_done < 1) { s->err = "fb_fd_inverse_read: no Jacobians to read (fb_fd_inverse)"; return -1; }
-  const DevFdInv& p = s->fdi;
-  const size_t n = (size_t)s->fdi_done, nv = (size_t)s->m.nv, nM = (size_t)s->m.nM;
-  return read_out(s, {{DfDq, p.DfDq, 0, 4 * n * nv * nv, 1}, {DfDv, p.DfDv, 0, 4 * n * nv * nv, 1}, {DfDa, p.DfDa, 0, 4 * n * nv * nv, 1},
-                      {DmDq, p.DmDq, 0, 4 * n * nv * nM, 1}, {qfrc_inverse, p.qfrc, 0, 4 * n * nv, 1}});
+  return s ? fd_read(s, s->fd_inv, "fb_fd_inverse_read", false, {DfDq, DfDv, DfDa, DmDq, qfrc_inverse}) : -1;
 }
-
-}  // extern "C"
-
-// -------------------------------------------------------------------------------------------
-// parameter Jacobians (fb_fd_param_*; fb_fd.h): a direction program resolved to overlay slots, and their own kernel parameters
-// (DevFdPrm, DevFdPrmInv with its own DevInv) and buffers
-struct FdpPerturb {
-  DevData d; DevFdPrm p;
-  FB_DEVM void operator()(unsigned char*, int e) const { kfdp_perturb(d, p, e); }
-};
-struct FdpDiff {
-  DevModel m; DevData d; DevFdPrm p;
-  FB_DEVM void operator()(unsigned char*, int w) const { kfdp_diff(m, d, p, w); }
-};
-struct FdpiRows {
-  DevData d; DevFdPrmInv p;
-  FB_DEVM void operator()(unsigned char*, int w) const { kfdpi_rows(d, p, w); }
-};
-struct FdpiPerturb {
-  DevModel m; DevData d; DevFdPrmInv p;
-  FB_DEVM void operator()(unsigned char*, int e) const { kfdpi_perturb(m, d, p, e); }
-};
-struct FdpiDiff {
-  DevModel m; DevFdPrmInv p;
-  FB_DEVM void operator()(unsigned char*, int w) const { kfdpi_diff(m, p, w); }
-};
-static int fdp_columns(const FbSim* s, int centered) { return 1 + (centered ? 2 : 1) * s->fdp_k; }
-// the checks both queries share: an overlay, a program, eps
-static int fdp_ready(FbSim* s, const char* who, const char* todo, float eps) {
-  if (!s->d.prm) { s->err = std::string(who) + ": the handle has no parameter overlay, and the columns nudge each problem's own parameters: " + todo; return -1; }
-  if (s->fdp_k < 1) { s->err = std::string(who) + ": no direction program (fb_fd_param_program)"; return -1; }
-  if (!(eps > 0.0f) || !std::isfinite(eps)) { s->err = std::string(who) + ": eps must be positive and finite"; return -1; }
-  if (s->fdp_scale && !(eps < 1.0f)) { s->err = std::string(who) + ": the program has scale directions, which need eps < 1"; return -1; }
-  return 0;
+int fb_fd_inverse_sensor_read(FbHandle s, float* DsDq, float* DsDv, float* DsDa, float* sensordata, int is_device) {
+  return s ? fd_read(s, s->fd_inv, "fb_fd_inverse_sensor_read", true, {DsDq, DsDv, DsDa, sensordata}) : -1;
 }
-
-extern "C" {
 
 int fb_fd_param_program(FbHandle s, int k, const int32_t* kind, const int32_t* dir_ptr, const int32_t* param, const int32_t* elem, const float* floor) {
   if (!s) return -1;
@@ -2518,127 +2473,27 @@ int fb_fd_param_program(FbHandle s, int k, const int32_t* kind, const int32_t* d
 int fb_fd_param_columns(FbHandle s, int centered) {
   if (!s) return -1;
   if (s->fdp_k < 1) { s->err = "fb_fd_param_columns: no direction program (fb_fd_param_program)"; return -1; }
-  return fdp_columns(s, centered);
+  return fd_columns(s, s->fd_ptr, centered);
 }
 
 int fb_fd_param_transition(FbHandle s, const int32_t* slots, int n, float eps, int centered, int n_substeps) {
-  if (!s) return -1;
-  const char* who = "fb_fd_param_transition";
-  if (fdp_ready(s, who, "fb_param_set first, then fb_state_bank and fb_state_save the rows", eps) != 0 || state_ready(s, who) != 0) return -1;
-  const int N = s->d.N, ncol = fdp_columns(s, centered != 0);
-  if (!slots || n < 1 || (long long)n * ncol > N) {
-    s->err = std::string(who) + ": 1 <= n problems with n * fb_fd_param_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
-  if (n_substeps < 1) { s->err = std::string(who) + ": n_substeps >= 1"; return -1; }
-  if (fd_slots_valid(s, who, slots, n) != 0) return -1;
-  dev_select(s);
-  const DevModel& m = s->m;
-  const size_t Np = s->d.Np, nx = 2 * (size_t)m.nv + m.na, nsd = m.nsensordata, half = std::max(1, s->d.N / 2);   // n k < N, n <= N / 2
-  DevFdPrm& p = s->fdp;
-  if (!p.delta && scope_alloc(s, s->fdp_scope, "out of device memory (parameter Jacobians)", [&] {
-        p.delta = dalloc<float>(s, Np); p.dxdp = dalloc<float>(s, Np * nx); p.next = dalloc<float>(s, half * (m.nq + m.nv + m.na)); })) {
-    p = DevFdPrm{}; return -4; }
-  const bool sens = s->sens_on != 0, snap = sens && nsd > 0;
-  DevFdSens& q = s->fdps;
-  if (sens && !q.snap && scope_alloc(s, s->fdps_scope, "out of device memory (parameter sensor Jacobians)", [&] {
-        q.snap = dalloc<float>(s, Np * nsd); q.D = dalloc<float>(s, Np * nsd); q.sensordata = dalloc<float>(s, half * nsd); })) {
-    q = DevFdSens{}; return -4; }
-  if (int rc = fd_fan_out(s, slots, n, ncol)) return rc;
-  p.n = n; p.ncol = ncol; p.nin = s->fdp_k; p.centered = centered != 0; p.eps = eps; p.nx = (int)nx; p.g = s->fdp_prog;
-  s->fdp_done = 0;
-  warp_launch(s, "fdp_perturb", N, 0, FdpPerturb{s->d, p});
-  launch_step1(s);                             // the position / velocity stage of the nudged parameters
-  if (!snap) step_run(s, n_substeps);
-  else {                                       // kfd_sdiff with no state inputs: its D block is dsdp [n][nsd][k]
-    q.fd = DevFd{}; static_cast<FdCols&>(q.fd) = p;
-    fd_step_snap(s, q, n * ncol, n_substeps);
-  }
-  warp_launch(s, "fdp_diff", n * p.nin, 0, FdpDiff{s->m, s->d, p});
-  if (snap) warp_launch(s, "fd_sdiff", n * p.nin, 0, FdSDiff{s->m, q});
-  if (launch_check(s, who) != 0) return -2;
-  s->fdp_done = n; s->fdp_sens = sens;
-  return sync_stream(s);                       // (the fan-out list is a host vector)
+  return s ? fd_run(s, s->fd_ptr, {n, slots, {}, eps, centered, n_substeps, 0}) : -1;
 }
-
 int fb_fd_param_read(FbHandle s, float* dxdp, float* qpos_next, float* qvel_next, float* act_next, int is_device) {
-  if (!s) return -1;
-  if (s->fdp_done < 1) { s->err = "fb_fd_param_read: no parameter Jacobians to read (fb_fd_param_transition)"; return -1; }
-  const DevFdPrm& p = s->fdp;
-  const size_t n = (size_t)s->fdp_done, nx = (size_t)p.nx, k = (size_t)p.nin;
-  const size_t nq = s->m.nq, nv = s->m.nv, na = s->m.na, row = (nq + nv + na) * 4;
-  return read_out(s, {{dxdp, p.dxdp, 0, 4 * n * nx * k, 1}, {qpos_next, p.next, row, nq * 4, n}, {qvel_next, p.next + nq, row, nv * 4, n},
-                      {act_next, p.next + nq + nv, row, na * 4, n}});
+  return s ? fd_read(s, s->fd_ptr, "fb_fd_param_read", false, {dxdp, qpos_next, qvel_next, act_next}) : -1;
 }
-
 int fb_fd_param_sensor_read(FbHandle s, float* dsdp, float* sensordata, int is_device) {
-  if (!s) return -1;
-  if (s->fdp_done < 1) { s->err = "fb_fd_param_sensor_read: no parameter Jacobians to read (fb_fd_param_transition)"; return -1; }
-  if (!s->fdp_sens) { s->err = "fb_fd_param_sensor_read: the last fb_fd_param_transition ran with sensors off (fb_query_sensors)"; return -1; }
-  const size_t n = (size_t)s->fdp_done, nsd = (size_t)s->m.nsensordata, k = (size_t)s->fdp.nin;
-  return read_out(s, {{dsdp, s->fdps.D, 0, 4 * n * nsd * k, 1}, {sensordata, s->fdps.sensordata, 0, 4 * n * nsd, 1}});
+  return s ? fd_read(s, s->fd_ptr, "fb_fd_param_sensor_read", true, {dsdp, sensordata}) : -1;
 }
 
 int fb_fd_param_inverse(FbHandle s, int n, const float* qpos, const float* qvel, const float* qacc, float eps, int centered, int is_device) {
-  if (!s) return -1;
-  const char* who = "fb_fd_param_inverse";
-  if (fdp_ready(s, who, "fb_param_set first (problem i takes env i's parameters)", eps) != 0) return -1;
-  const int N = s->d.N, ncol = fdp_columns(s, centered != 0);
-  if (n < 1 || (long long)n * ncol > N) {
-    s->err = std::string(who) + ": 1 <= n problems with n * fb_fd_param_columns (" + std::to_string(ncol) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
-  if (!qpos || !qvel || !qacc) { s->err = std::string(who) + ": qpos, qvel and qacc must not be NULL"; return -1; }
-  const size_t nq = s->m.nq, nv = s->m.nv, nsd = s->m.nsensordata, Np = s->d.Np, P = s->d.prm_stride, half = std::max(1, N / 2);
-  if (!is_device) {
-    const struct { const float* x; size_t cnt; const char* what; } ins[3] = {{qpos, n * nq, "qpos"}, {qvel, n * nv, "qvel"}, {qacc, n * nv, "qacc"}};
-    for (const auto& in : ins)
-      for (size_t i = 0; i < in.cnt; i++)
-        if (!std::isfinite(in.x[i])) { s->err = std::string(who) + ": non-finite " + in.what; return -1; }
-  }
-  dev_select(s);
-  DevFdPrmInv& p = s->fdpi;
-  if (!p.delta && scope_alloc(s, s->fdpi_scope, "out of device memory (inverse parameter Jacobians)", [&] {
-        float *qp = dalloc<float>(s, half * nq), *qv = dalloc<float>(s, half * nv), *qa = dalloc<float>(s, half * nv);
-        p.qpos = qp; p.qvel = qv; p.qacc = qa;
-        p.rows = dalloc<float>(s, half * P); p.delta = dalloc<float>(s, Np);
-        p.inv.qacc = dalloc<float>(s, Np * nv); p.inv.qfrc_inverse = dalloc<float>(s, Np * nv);
-        p.inv.qfrc_constraint = dalloc<float>(s, Np * nv); p.inv.efc_force = dalloc<float>(s, Np * FB_MAXEFC);
-        p.DfDp = dalloc<float>(s, Np * nv); p.qfrc = dalloc<float>(s, half * nv); })) {
-    p = DevFdPrmInv{}; return -4; }
-  const bool sens = s->sens_on != 0, sdiff = sens && nsd > 0;
-  if (sens && !s->fdpi_env_sd && scope_alloc(s, s->fdpis_scope, "out of device memory (inverse parameter sensor Jacobians)", [&] {
-        s->fdpi_env_sd = dalloc<float>(s, Np * nsd); p.DsDp = dalloc<float>(s, Np * nsd); p.sensordata = dalloc<float>(s, half * nsd); })) {
-    s->fdpi_env_sd = p.DsDp = p.sensordata = nullptr; return -4; }
-  if (copy_async(s, (void*)p.qpos, qpos, sizeof(float) * n * nq) != 0 || copy_async(s, (void*)p.qvel, qvel, sizeof(float) * n * nv) != 0 ||
-      copy_async(s, (void*)p.qacc, qacc, sizeof(float) * n * nv) != 0) return -2;
-  p.n = n; p.ncol = ncol; p.nin = s->fdp_k; p.centered = centered != 0; p.eps = eps; p.g = s->fdp_prog;
-  p.inv.n = n * ncol;
-  p.sens = sdiff ? s->fdpi_env_sd : nullptr;
-  float* env_sd = s->fdpi_env_sd;
-  s->fdpi_done = 0;
-  warp_launch(s, "fdpi_rows", n, 0, FdpiRows{s->d, p});                 // problem i's parameters: env i's, before the fan-out
-  warp_launch(s, "fdpi_perturb", N, 0, FdpiPerturb{s->m, s->d, p});      // fan-out and nudge
-  launch_step1(s);                             // the position / velocity stage of every env, as fb_inverse runs it
-  launch_inv(s, p.inv);
-  if (sdiff) launch_inv_sensors(s, p.inv, env_sd);
-  warp_launch(s, "fdpi_diff", n * p.nin, 0, FdpiDiff{s->m, p});
-  if (launch_check(s, who) != 0) return -2;
-  s->fdpi_done = n; s->fdpi_sens = sens;
-  return is_device ? 0 : sync_stream(s);       // host rows may be reused once the call returns
+  return s ? fd_run(s, s->fd_pinv, {n, nullptr, {qpos, qvel, qacc}, eps, centered, 1, is_device}) : -1;
 }
-
 int fb_fd_param_inverse_read(FbHandle s, float* DfDp, float* qfrc_inverse, int is_device) {
-  if (!s) return -1;
-  if (s->fdpi_done < 1) { s->err = "fb_fd_param_inverse_read: no parameter Jacobians to read (fb_fd_param_inverse)"; return -1; }
-  const DevFdPrmInv& p = s->fdpi;
-  const size_t n = (size_t)s->fdpi_done, nv = (size_t)s->m.nv, k = (size_t)p.nin;
-  return read_out(s, {{DfDp, p.DfDp, 0, 4 * n * k * nv, 1}, {qfrc_inverse, p.qfrc, 0, 4 * n * nv, 1}});
+  return s ? fd_read(s, s->fd_pinv, "fb_fd_param_inverse_read", false, {DfDp, qfrc_inverse}) : -1;
 }
-
 int fb_fd_param_inverse_sensor_read(FbHandle s, float* DsDp, float* sensordata, int is_device) {
-  if (!s) return -1;
-  if (s->fdpi_done < 1) { s->err = "fb_fd_param_inverse_sensor_read: no parameter Jacobians to read (fb_fd_param_inverse)"; return -1; }
-  if (!s->fdpi_sens) { s->err = "fb_fd_param_inverse_sensor_read: the last fb_fd_param_inverse ran with sensors off (fb_query_sensors)"; return -1; }
-  const DevFdPrmInv& p = s->fdpi;
-  const size_t n = (size_t)s->fdpi_done, nsd = (size_t)s->m.nsensordata, k = (size_t)p.nin;
-  return read_out(s, {{DsDp, p.DsDp, 0, 4 * n * k * nsd, 1}, {sensordata, p.sensordata, 0, 4 * n * nsd, 1}});
+  return s ? fd_read(s, s->fd_pinv, "fb_fd_param_inverse_sensor_read", true, {DsDp, sensordata}) : -1;
 }
 
 }  // extern "C"
@@ -2665,7 +2520,6 @@ template <typename F> static int roll_grow(FbSim* s, std::vector<void*>& scope, 
   cap = rows;
   return 0;
 }
-static bool all_finite(const float* x, size_t n) { for (size_t i = 0; i < n; i++) if (!std::isfinite(x[i])) return false; return true; }
 
 extern "C" {
 

@@ -57,29 +57,45 @@ def transition_fd(model, qpos, qvel, ctrl, act=None, eps=1e-2, centered=True, n_
     per = max(1, ENVS // ncol)
 
     def run(sim, rows, k):
-        q, v, u, a = rows
-        pad = np.minimum(np.arange(sim.n_envs), k - 1)         # the chunk's states in envs 0 .. k-1, the last one repeated
-        sim.reset(q[pad], v[pad])
-        if m.na:
-            sim.set(st.ACT, a[pad])
-        sim.set_control(u[pad])
-        sim.forward()
-        sim.save_state(slots=np.arange(k), env_ids=np.arange(k))
+        _bank_rows(sim, m, rows, k)
         sim.fd_transition(np.arange(k), eps=eps, centered=centered, n_substeps=n_substeps)
         return sim.fd_read() + (sim.fd_sensor_read() if sensors else ())
 
     act = np.zeros(np.shape(qpos)[:-1] + (m.na,)) if act is None else act
     single, out = st._batched(m, [('qpos', qpos, (m.nq,)), ('qvel', qvel, (m.nv,)), ('ctrl', ctrl, (m.nu,)), ('act', act, (m.na,))], run,
                               per, n_envs=per * ncol, setup=lambda sim: _setup(sim, per, sensors), device=device, lib_path=lib_path)
-    kind = TransitionSensors if sensors else Transition
-    res = kind(*(x.astype(np.float64) for x in out))
-    return kind(*(x[0] for x in res)) if single else res
+    return _result(TransitionSensors if sensors else Transition, single, out)
 
 
 def _setup(sim, slots, sensors):
     sim.state_bank(slots)
     if sensors:
         sim.query_sensors(True)
+
+
+def _bank_rows(sim, model, rows, k, vals=()):
+    """the chunk's k states (qpos, qvel, ctrl, act) into envs 0 .. k-1 (the last one repeated over the handle), each parameter of vals
+    (name, rows or None: compiled) into those envs, forward, then bank rows 0 .. k-1"""
+    q, v, u, a = rows[:4]
+    pad = np.minimum(np.arange(sim.n_envs), k - 1)
+    sim.reset(q[pad], v[pad])
+    if model.na:
+        sim.set(st.ACT, a[pad])
+    sim.set_control(u[pad])
+    _write_values(sim, model, vals, k)
+    sim.forward()
+    sim.save_state(slots=np.arange(k), env_ids=np.arange(k))
+
+
+def _result(kind, single, out, labels=None):
+    """the device's fp32 outputs as fp64 arrays in the namedtuple `kind` (one state: without the batch dimension); labels: its
+    `columns`"""
+    out = [x.astype(np.float64) for x in out]
+    if single:
+        out = [x[0] for x in out]
+    if labels is not None:
+        out.insert(kind._fields.index('columns'), list(labels))
+    return kind(*out)
 
 
 def inverse_fd(model, qpos, qvel, qacc, eps=1e-2, centered=True, device=0, lib_path=None, sensors=False):
@@ -101,9 +117,7 @@ def inverse_fd(model, qpos, qvel, qacc, eps=1e-2, centered=True, device=0, lib_p
 
     single, out = st._batched(m, [('qpos', qpos, (m.nq,)), ('qvel', qvel, (m.nv,)), ('qacc', qacc, (m.nv,))], run, per, n_envs=per * ncol,
                               setup=(lambda sim: sim.query_sensors(True)) if sensors else None, device=device, lib_path=lib_path)
-    kind = InverseSensorJacobians if sensors else InverseJacobians
-    res = kind(*(x.astype(np.float64) for x in out))
-    return kind(*(x[0] for x in res)) if single else res
+    return _result(InverseSensorJacobians if sensors else InverseJacobians, single, out)
 
 
 # ---- parameter Jacobians (fb_fd_param_*): derivatives with respect to the per-env model parameters, for system identification --------
@@ -234,16 +248,8 @@ def parameter_fd(model, qpos, qvel, ctrl, act=None, *, params, values=None, floo
     names = [n for n, _, _ in given]
 
     def run(sim, rows, k):
-        q, v, u, a = rows[:4]
-        pad = np.minimum(np.arange(sim.n_envs), k - 1)
-        sim.reset(q[pad], v[pad])
-        if m.na:
-            sim.set(st.ACT, a[pad])
-        sim.set_control(u[pad])
         chunk = dict(zip(names, rows[4:]))
-        _write_values(sim, m, [(n, chunk.get(n)) for n, _, _ in vals], k)
-        sim.forward()
-        sim.save_state(slots=np.arange(k), env_ids=np.arange(k))
+        _bank_rows(sim, m, rows, k, [(n, chunk.get(n)) for n, _, _ in vals])
         sim.fd_param_transition(np.arange(k), eps=eps, centered=centered, n_substeps=n_substeps)
         return sim.fd_param_read() + (sim.fd_param_sensor_read() if sensors else ())
 
@@ -251,12 +257,7 @@ def parameter_fd(model, qpos, qvel, ctrl, act=None, *, params, values=None, floo
     single, out = st._batched(m, [('qpos', qpos, (m.nq,)), ('qvel', qvel, (m.nv,)), ('ctrl', ctrl, (m.nu,)), ('act', act, (m.na,))] + given,
                               run, per, n_envs=per * ncol, setup=lambda sim: _param_setup(sim, m, dirs, sensors, per), device=device,
                               lib_path=lib_path)
-    out = [x.astype(np.float64) for x in out]
-    if single:
-        out = [x[0] for x in out]
-    if sensors:
-        return ParamTransitionSensors(*out[:4], list(labels), *out[4:])
-    return ParamTransition(*out, list(labels))
+    return _result(ParamTransitionSensors if sensors else ParamTransition, single, out, labels)
 
 
 def inverse_parameter_fd(model, qpos, qvel, qacc, *, params, values=None, floors=None, eps=1e-2, centered=True, sensors=False, device=0,
@@ -284,9 +285,4 @@ def inverse_parameter_fd(model, qpos, qvel, qacc, *, params, values=None, floors
 
     single, out = st._batched(m, [('qpos', qpos, (m.nq,)), ('qvel', qvel, (m.nv,)), ('qacc', qacc, (m.nv,))] + given, run, per,
                               n_envs=per * ncol, setup=lambda sim: _param_setup(sim, m, dirs, sensors), device=device, lib_path=lib_path)
-    out = [x.astype(np.float64) for x in out]
-    if single:
-        out = [x[0] for x in out]
-    if sensors:
-        return InverseParamSensorJacobians(*out[:2], list(labels), *out[2:])
-    return InverseParamJacobians(*out, list(labels))
+    return _result(InverseParamSensorJacobians if sensors else InverseParamJacobians, single, out, labels)

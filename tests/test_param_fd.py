@@ -108,7 +108,7 @@ def check_mechanics(lib, variant, n_envs=None, n_sub=2):
     _, _, q2, v2, a2 = sim.fd_read()
     assert np.array_equal(bits(q2), bits(qn)) and np.array_equal(bits(v2), bits(vn)) and np.array_equal(bits(a2), bits(an))
     assert np.array_equal(bits(sim.fd_sensor_read()[2]), bits(sd0))
-    # dsdp (kfd_sdiff with no state inputs): column j is the difference of its two columns' sensors of x over their steps
+    # dsdp (kfd_diff's sensor block): column j is the difference of its two columns' sensors of x over their steps
     sd = []
     for c in range(ncol):
         one = st.BatchedStepper(patched(m, {k: x[c] for k, x in vals.items()}), 1 + 2 * m.nv + m.na + m.nu, lib_path=lib)

@@ -165,10 +165,11 @@ def check_isolation(lib):
         sim.close()
     for x, y in zip(out[False][0] + out[False][1], out[True][0] + out[True][1]):
         assert np.array_equal(bits(x), bits(y))
-    assert out[True][2] == out[False][2] + 3 and out[True][3] == out[False][3] + 2
+    # sensors on adds the two snapshots of x (transition) and kinv_sensors (inverse); the sensor differences are in the one diff launch
+    assert out[True][2] == out[False][2] + 2 and out[True][3] == out[False][3] + 1
 
 
-def test_isolation_under_emulation(emu):
+def test_isolation_and_launch_counts_under_emulation(emu):
     check_isolation(emu)
 
 
@@ -433,7 +434,7 @@ def test_python_front_ends(emu):
 
 # ---- GPU tier ------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_gpu_isolation_determinism_and_refusals():
+def test_gpu_isolation_launch_counts_determinism_and_refusals():
     ge.build()
     check_isolation(None)
     check_positions(None, 4096)
