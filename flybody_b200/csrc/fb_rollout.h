@@ -1,5 +1,5 @@
 // fb_rollout.h -- batched rollouts (MuJoCo mujoco.rollout.rollout; fb_rollout): n rollouts of T control steps, rollout i in env i from a
-// state-bank row, driven by its own control sequence and, optionally, one time-varying linear feedback law shared by every rollout.
+// state-bank row, driven by its own control sequence and, optionally, a time-varying linear feedback law from a bank of L laws.
 // A control step is three launches: kroll_input (one warp per env) writes the step's inputs into the env's record, step_run replays the
 // step graph (n_substeps x [step2 ; step1], ctrl held), kroll_record (one warp per rollout) copies the state after the step into the
 // rollout's row t.  DevRoll is the kernels' own parameter: DevData and the step kernels are untouched, so the step graph is captured
@@ -8,10 +8,11 @@
 //   inputs:   ctrl [n][T][nu] (written as given: the actuation stage clamps ctrl-limited actuators, as for d->ctrl); optional
 //             qfrc_applied [n][T][nv] and xfrc_applied [n][T][nbody][6] (nullptr: the row's applied forces persist, as in mjData).
 //             Envs past n take the last rollout's sequence (the state bank's fan-out).
-//   feedback: ctrl = u_t + K_t (x_t (-) xref_t), x_t the env's state before step t, xref [T][nq + nv + na], K [T][nu][nx] with
-//             nx = 2 nv + na; (-) is transition_fd's tangent (fd_dof / fd_subquat per dof, mj_differentiatePos(xref qpos, qpos), then
-//             the qvel and act differences), so gains from a Riccati recursion on its A and B apply as they are.  The tangent goes to the
-//             warp's shared slice; lane r sums row r of K_t in column order (every env reads the same K_t, which stays in L2).
+//   feedback: ctrl = u_t + K_t (x_t (-) xref_t), x_t the env's state before step t, xref and K the rows of law[i] (law 0 without
+//             a law list) in the bank xref [L][T][nq + nv + na], K [L][T][nu][nx] with nx = 2 nv + na; (-) is transition_fd's tangent
+//             (fd_dof / fd_subquat per dof, mj_differentiatePos(xref qpos, qpos), then the qvel and act differences), so gains from a
+//             Riccati recursion on its A and B apply as they are.  The tangent goes to the warp's shared slice; lane r sums row r of K_t
+//             in column order (the rollouts of one law read the same K_t, which stays in L2).
 //   records:  after step t, row [i][t] of qpos, qvel, act, ctrl as written, time and the env's flags; with sensors, sensordata and
 //             sensor_mean = sensor_sum / n_substeps (fb_get's FB_SENSOR_MEAN, the same division).
 #pragma once
@@ -20,7 +21,7 @@
 struct DevRoll {
   int n, T, t, nsub;                      // rollouts, control steps, the step a launch serves, substeps per control step
   const float *ctrl, *qfrc, *xfrc;        // [n][T][nu], [n][T][nv], [n][T][6 nbody] (qfrc / xfrc nullptr: not written)
-  const float *xref, *K;                  // [T][nq + nv + na], [T][nu][nx] (nullptr: open loop)
+  const float *xref, *K;                  // [L][T][nq + nv + na], [L][T][nu][nx] (nullptr: open loop)
   float *qpos, *qvel, *act, *ctrl_out, *time;   // [n][T][nq], [nv], [na], [nu], [1]
   int* flags;                             // [n][T]
   float *sensordata, *sensor_mean;        // [n][T][nsd] (nullptr: not recorded)
@@ -38,14 +39,17 @@ FB_DEV float roll_tangent(const DevModel& m, const DevData& d, int e, const floa
   return AT(d.act, i - 2 * nv) - xr[nq + i - nv];
 }
 
-FB_WARPFN void kroll_input(const DevModel& m, const DevData& d, const DevRoll& p, float* dx, int e) {
+// law [n]: the law of each rollout (nullptr: law 0).  It is the input kernel's own parameter, so the record kernel's is unchanged.
+FB_WARPFN void kroll_input(const DevModel& m, const DevData& d, const DevRoll& p, const int* law, float* dx, int e) {
   const int nu = m.nu, nv = m.nv, nxf = 6 * m.nbody;
-  const size_t row = (size_t)(e < p.n ? e : p.n - 1) * p.T + p.t;
+  const int i = e < p.n ? e : p.n - 1;
+  const size_t row = (size_t)i * p.T + p.t;
   const float* u = p.ctrl + row * nu;
   if (p.K) {
     const int nx = 2 * nv + m.na;
-    const float* xr = p.xref + (size_t)p.t * (m.nq + nv + m.na);
-    const float* K = p.K + (size_t)p.t * nu * nx;
+    const size_t lt = (size_t)(law ? law[i] : 0) * p.T + p.t;
+    const float* xr = p.xref + lt * (m.nq + nv + m.na);
+    const float* K = p.K + lt * nu * nx;
     WPAR_BEGIN for (int c = lane; c < nx; c += FB_NY) dx[c] = roll_tangent(m, d, e, xr, c); WPAR_END
     WPAR_BEGIN
       for (int r = lane; r < nu; r += FB_NY) {

@@ -31,6 +31,7 @@
 #include "fb_inverse.h"
 #include "fb_fd.h"
 #include "fb_rollout.h"
+#include "fb_lqr.h"
 
 enum { K_ACT = 0, K_SMOOTH, K_REF, K_SOLVE, K_FINISH, K_POS, K_COL, K_CON, K_PROJ, K_VEL, K_SENS, K_PACK, K_MISC, K_NKIND };
 static const char* const kKindNames[K_NKIND] = {"act", "smooth", "ref", "solve", "finish", "pos", "col", "con", "proj", "vel", "sens", "pack", "misc"};
@@ -78,11 +79,16 @@ struct FbSim {
   FdScratch fdx = {};
   DevFdPrmProg fdp_prog = {}; std::vector<void*> fdp_prog_scope; int fdp_k = 0; bool fdp_scale = false;
   // rollouts (fb_rollout*; fb_rollout.h): inputs and records of roll_cap rows (n T), grown on demand in three groups (ctrl and the
-  // records; applied-force inputs; sensor records); the feedback law of roll_fb_T steps (fb_rollout_feedback); rows of the last call
+  // records; applied-force inputs; sensor records); the feedback bank of roll_fb_L laws of roll_fb_T steps (fb_rollout_feedback_bank)
+  // in buffers of roll_fb_cap law steps (L T), and its law list of roll_fb_n rollouts (0: every rollout takes law 0); rows of the last call
   DevRoll roll = {}; std::vector<void*> roll_scope, roll_app_scope, roll_sd_scope; size_t roll_cap = 0, roll_app_cap = 0, roll_sd_cap = 0;
-  float *roll_xref = nullptr, *roll_K = nullptr; std::vector<void*> roll_fb_scope; int roll_fb_T = 0;
+  float *roll_xref = nullptr, *roll_K = nullptr; int* roll_law = nullptr; std::vector<void*> roll_fb_scope, roll_law_scope;
+  size_t roll_fb_cap = 0, roll_law_cap = 0; int roll_fb_T = 0, roll_fb_L = 0, roll_fb_n = 0;
   float *roll_qf = nullptr, *roll_xf = nullptr, *roll_sd = nullptr, *roll_sm = nullptr;   // applied-force inputs, sensor records
   int roll_done = 0; bool roll_sens = false;
+  // the iLQR backward pass (fb_lqr; fb_lqr.h): inputs and outputs of lqr_cap problem steps (L (T + 1)) and the workspace of lqr_ws_cap
+  // problems, grown on demand; problems and steps of the last call
+  DevLqr lqr = {}; std::vector<void*> lqr_scope, lqr_ws_scope; size_t lqr_cap = 0, lqr_ws_cap = 0; int lqr_done = 0;
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -2234,7 +2240,7 @@ template <bool ACC> struct FdSnap {
   DevModel m; DevData d; float* snap;
   FB_DEVM void operator()(unsigned char*, int e) const { kfd_snap(m, d, snap, e, ACC); }
 };
-static bool all_finite(const float* x, size_t n) { for (size_t i = 0; i < n; i++) if (!std::isfinite(x[i])) return false; return true; }
+template <typename F> static bool all_finite(const F* x, size_t n) { for (size_t i = 0; i < n; i++) if (!std::isfinite(x[i])) return false; return true; }
 // the inputs of one problem: (dq, qvel, act, ctrl), (dq, qvel, qacc) or the program's directions; and the envs it takes
 static int fd_inputs(const FbSim* s, const FdQuery& q) { return q.param ? s->fdp_k : q.inverse ? 3 * s->m.nv : 2 * s->m.nv + s->m.na + s->m.nu; }
 static int fd_columns(const FbSim* s, const FdQuery& q, int centered) { return 1 + (centered ? 2 : 1) * fd_inputs(s, q); }
@@ -2501,48 +2507,69 @@ int fb_fd_param_inverse_sensor_read(FbHandle s, float* DsDp, float* sensordata, 
 // -------------------------------------------------------------------------------------------
 // rollouts (fb_rollout*; fb_rollout.h): their own kernel parameter (DevRoll) and buffers, allocated on first use and grown with n T
 struct RollInput {
-  DevModel m; DevData d; DevRoll p;
-  FB_DEVM void operator()(unsigned char* sh, int e) const { kroll_input(m, d, p, reinterpret_cast<float*>(sh), e); }
+  DevModel m; DevData d; DevRoll p; const int* law;
+  FB_DEVM void operator()(unsigned char* sh, int e) const { kroll_input(m, d, p, law, reinterpret_cast<float*>(sh), e); }
 };
 struct RollRecord {
   DevModel m; DevData d; DevRoll p;
   FB_DEVM void operator()(unsigned char*, int e) const { kroll_record(m, d, p, e); }
 };
-// one group of buffers for `rows` rows of `row_bytes` bytes, made by alloc(rows) unless `cap` rows fit already
-template <typename F> static int roll_grow(FbSim* s, std::vector<void*>& scope, size_t& cap, size_t rows, size_t row_bytes, const char* what, F alloc) {
+// one group of buffers for `rows` rows (`unit` says what a row is) of `row_bytes` bytes, made by alloc(rows) unless `cap` rows fit already
+template <typename F> static int grow(FbSim* s, const char* who, std::vector<void*>& scope, size_t& cap, size_t rows, size_t row_bytes,
+                                      const char* what, const char* unit, F alloc) {
   if (rows <= cap) return 0;
   if (sync_stream(s) != 0) return -2;
   scope_free(s, scope); cap = 0;
   if (rows * row_bytes > dev_free_bytes()) {
-    s->err = std::string("fb_rollout: the ") + what + " of " + std::to_string(rows) + " rows (n T) do not fit the device's free memory"; return -4; }
-  const std::string oom = std::string("fb_rollout: out of device memory (") + what + ")";
+    s->err = std::string(who) + ": the " + what + " of " + std::to_string(rows) + " rows (" + unit + ") do not fit the device's free memory"; return -4; }
+  const std::string oom = std::string(who) + ": out of device memory (" + what + ")";
   if (int rc = scope_alloc(s, scope, oom.c_str(), [&] { alloc(rows); })) return rc;
   cap = rows;
   return 0;
+}
+template <typename F> static int roll_grow(FbSim* s, std::vector<void*>& scope, size_t& cap, size_t rows, size_t row_bytes, const char* what, F alloc) {
+  return grow(s, "fb_rollout", scope, cap, rows, row_bytes, what, "n T", alloc);
+}
+// the feedback bank (fb_rollout_feedback_bank; fb_rollout_feedback is L = 1 without a law list)
+static int rollout_feedback(FbSim* s, const char* who, int L, int T, const float* xref, const float* K, const int32_t* law, int n, int is_device) {
+  const DevModel& m = s->m;
+  const std::string w = who;
+  const size_t nx = 2 * (size_t)m.nv + m.na, nr = (size_t)m.nq + m.nv + m.na;
+  const bool clear = T == 0 || (!xref && !K);
+  if (!clear && (T < 1 || !xref || !K)) { s->err = w + ": T >= 1 steps with both xref and K (T = 0, or both NULL, clears the law)"; return -1; }
+  if (!clear && L < 1) { s->err = w + ": L >= 1 laws"; return -1; }
+  if (!clear && law && n < 1) { s->err = w + ": a law list of n >= 1 rollouts"; return -1; }
+  if (!clear && !law && L != 1) { s->err = w + ": a bank of " + std::to_string(L) + " laws needs a law list"; return -1; }
+  if (!clear && law)
+    for (int i = 0; i < n; i++)
+      if (law[i] < 0 || law[i] >= L) { s->err = w + ": law[" + std::to_string(i) + "] = " + std::to_string(law[i]) + " is outside [0, L = " + std::to_string(L) + ")"; return -1; }
+  if (!clear && slice_bytes(0, nx) * FB_WPB > 48 * 1024) {
+    s->err = w + ": the input kernel keeps the tangent (2 nv + na = " + std::to_string(nx) + " floats) in shared memory, and it does not fit"; return -1; }
+  const size_t lt = (size_t)L * T;
+  if (!clear && !is_device && (!all_finite(xref, lt * nr) || !all_finite(K, lt * m.nu * nx))) { s->err = w + ": non-finite xref or K"; return -1; }
+  dev_select(s);
+  if (sync_stream(s) != 0) return -2;          // a rollout in flight may still read the old law
+  s->roll_fb_T = s->roll_fb_L = s->roll_fb_n = 0;
+  if (clear) return 0;
+  if (int rc = grow(s, who, s->roll_fb_scope, s->roll_fb_cap, lt, 4 * (nr + m.nu * nx), "feedback laws", "L T", [&](size_t r) {
+        s->roll_xref = dalloc<float>(s, r * nr); s->roll_K = dalloc<float>(s, r * m.nu * nx); }))
+    return rc;
+  if (law) if (int rc = grow(s, who, s->roll_law_scope, s->roll_law_cap, n, 4, "law list", "n", [&](size_t r) { s->roll_law = dalloc<int>(s, r); }))
+    return rc;
+  if (copy_async(s, s->roll_xref, xref, sizeof(float) * lt * nr) != 0 || copy_async(s, s->roll_K, K, sizeof(float) * lt * m.nu * nx) != 0 ||
+      (law && copy_async(s, s->roll_law, law, sizeof(int) * n) != 0)) return -2;
+  s->roll_fb_T = T; s->roll_fb_L = L; s->roll_fb_n = law ? n : 0;
+  return is_device && !law ? 0 : sync_stream(s);   // host arrays may be reused once the call returns
 }
 
 extern "C" {
 
 int fb_rollout_feedback(FbHandle s, int T, const float* xref, const float* K, int is_device) {
-  if (!s) return -1;
-  const DevModel& m = s->m;
-  const size_t nx = 2 * (size_t)m.nv + m.na, nr = (size_t)m.nq + m.nv + m.na;
-  const bool clear = T == 0 || (!xref && !K);
-  if (!clear && (T < 1 || !xref || !K)) { s->err = "fb_rollout_feedback: T >= 1 steps with both xref and K (T = 0, or both NULL, clears the law)"; return -1; }
-  if (!clear && slice_bytes(0, nx) * FB_WPB > 48 * 1024) {
-    s->err = "fb_rollout_feedback: the input kernel keeps the tangent (2 nv + na = " + std::to_string(nx) + " floats) in shared memory, and it does not fit"; return -1; }
-  if (!clear && !is_device && (!all_finite(xref, T * nr) || !all_finite(K, T * m.nu * nx))) { s->err = "fb_rollout_feedback: non-finite xref or K"; return -1; }
-  dev_select(s);
-  if (sync_stream(s) != 0) return -2;          // a rollout in flight may still read the old law
-  scope_free(s, s->roll_fb_scope);
-  s->roll_xref = s->roll_K = nullptr; s->roll_fb_T = 0;
-  if (clear) return 0;
-  float *x, *k;
-  if (int rc = scope_alloc(s, s->roll_fb_scope, "out of device memory (rollout feedback)", [&] { x = dalloc<float>(s, T * nr); k = dalloc<float>(s, T * m.nu * nx); }))
-    return rc;
-  if (copy_async(s, x, xref, sizeof(float) * T * nr) != 0 || copy_async(s, k, K, sizeof(float) * T * m.nu * nx) != 0) return -2;
-  s->roll_xref = x; s->roll_K = k; s->roll_fb_T = T;
-  return is_device ? 0 : sync_stream(s);       // host arrays may be reused once the call returns
+  return s ? rollout_feedback(s, "fb_rollout_feedback", 1, T, xref, K, nullptr, 0, is_device) : -1;
+}
+
+int fb_rollout_feedback_bank(FbHandle s, int L, int T, const float* xref, const float* K, const int32_t* law, int n, int is_device) {
+  return s ? rollout_feedback(s, "fb_rollout_feedback_bank", L, T, xref, K, law, n, is_device) : -1;
 }
 
 int fb_rollout(FbHandle s, const int32_t* slots, int n, int T, int n_substeps, const float* ctrl, const float* qfrc_applied,
@@ -2561,6 +2588,8 @@ int fb_rollout(FbHandle s, const int32_t* slots, int n, int T, int n_substeps, c
     return -1; }
   if (s->roll_fb_T && s->roll_fb_T != T) {
     s->err = "fb_rollout: the feedback law has " + std::to_string(s->roll_fb_T) + " steps and the call " + std::to_string(T) + " (fb_rollout_feedback)"; return -1; }
+  if (s->roll_fb_n && s->roll_fb_n != n) {
+    s->err = "fb_rollout: the law list has " + std::to_string(s->roll_fb_n) + " rollouts and the call " + std::to_string(n) + " (fb_rollout_feedback_bank)"; return -1; }
   if (fd_slots_valid(s, who, slots, n) != 0) return -1;
   const DevModel& m = s->m;
   const size_t rows = (size_t)n * T, nq = m.nq, nv = m.nv, na = m.na, nu = m.nu, nsd = m.nsensordata, nxf = 6 * (size_t)m.nbody;
@@ -2594,7 +2623,7 @@ int fb_rollout(FbHandle s, const int32_t* slots, int n, int T, int n_substeps, c
   launch_step1(s);                             // what the rows do not carry, as fb_state_load runs it
   for (int t = 0; t < T; t++) {                // no host synchronisation or copy inside the horizon
     p.t = t;
-    warp_launch(s, "rollout_input", N, slice, RollInput{s->m, s->d, p});
+    warp_launch(s, "rollout_input", N, slice, RollInput{s->m, s->d, p, s->roll_fb_n ? s->roll_law : nullptr});
     step_run(s, n_substeps);                   // fb_step's launches (the step graph)
     warp_launch(s, "rollout_record", n, 0, RollRecord{s->m, s->d, p});
   }
@@ -2618,6 +2647,83 @@ int fb_rollout_sensor_read(FbHandle s, float* sensordata, float* sensor_mean, in
   if (!s->roll_sens) { s->err = "fb_rollout_sensor_read: the last fb_rollout ran with sensors off (fb_query_sensors)"; return -1; }
   const size_t r = (size_t)s->roll_done * s->roll.T * s->m.nsensordata;
   return read_out(s, {{sensordata, s->roll_sd, 0, 4 * r, 1}, {sensor_mean, s->roll_sm, 0, 4 * r, 1}});
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------
+// the iLQR backward pass (fb_lqr; fb_lqr.h): its own kernel parameter (DevLqr) and buffers, allocated on first use and grown with L T and L
+template <int KIND> struct LqrWarp {
+  DevLqr p;
+  FB_DEVM void operator()(unsigned char*, int w) const {
+    if (KIND == 0) klqr_init(p, w); else if (KIND == 1) klqr_w(p, w); else if (KIND == 2) klqr_h(p, w);
+    else if (KIND == 3) klqr_chol(p, w); else if (KIND == 4) klqr_solve(p, w); else klqr_p(p, w);
+  }
+};
+
+extern "C" {
+
+int fb_lqr(FbHandle s, int L, int T, const float* A, const float* B, const double* q, const double* r, const double* Q, const double* R,
+           const double* Qf, const double* mu, int is_device) {
+  if (!s) return -1;
+  const char* who = "fb_lqr";
+  const DevModel& m = s->m;
+  const int nx = 2 * m.nv + m.na, nu = m.nu, nz = nx + nu;
+  if (L < 1 || T < 1) { s->err = "fb_lqr: L >= 1 problems of T >= 1 steps"; return -1; }
+  if (!A || !B || !q || !r || !Q || !R || !Qf || !mu) { s->err = "fb_lqr: A, B, q, r, Q, R, Qf and mu must not be NULL"; return -1; }
+  if (nu < 1) { s->err = "fb_lqr: the model has no actuators"; return -1; }
+  if ((size_t)nz * (nz + 1) >= ((size_t)1 << 31)) {
+    s->err = "fb_lqr: nx + nu = " + std::to_string(nz) + " is too large for the 32-bit offsets inside a problem's workspace"; return -1; }
+  const size_t lt = (size_t)L * T, l1 = (size_t)L * (T + 1);
+  if (!is_device) {
+    const char* name[8] = {"A", "B", "q", "r", "Q", "R", "Qf", "mu"};
+    const bool ok[8] = {all_finite(A, lt * nx * nx), all_finite(B, lt * nx * nu), all_finite(q, l1 * nx), all_finite(r, lt * nu),
+                        all_finite(Q, (size_t)nx), all_finite(R, (size_t)nu), all_finite(Qf, (size_t)nx), all_finite(mu, (size_t)L)};
+    for (int i = 0; i < 8; i++) if (!ok[i]) { s->err = std::string("fb_lqr: non-finite ") + name[i]; return -1; }
+  }
+  dev_select(s);
+  s->lqr_done = 0;
+  DevLqr& p = s->lqr;
+  // per problem step (L (T + 1) rows, the last T + 1st unused by A, B, r, K, k): the inputs A, B, q, r and the outputs K, k
+  if (int rc = grow(s, who, s->lqr_scope, s->lqr_cap, l1, 4 * ((size_t)nx * nx + (size_t)nx * nu) + 8 * ((size_t)nx + nu + (size_t)nu * nx + nu),
+                    "inputs and gains", "L (T + 1)", [&](size_t n) {
+        p.A = dalloc<float>(s, n * nx * nx); p.B = dalloc<float>(s, n * nx * nu); p.q = dalloc<double>(s, n * nx); p.r = dalloc<double>(s, n * nu);
+        p.K = dalloc<double>(s, n * nu * nx); p.k = dalloc<double>(s, n * nu); }))
+    return rc;
+  // per problem: the workspace, mu, dV and status (and the shared weights)
+  const size_t ws = (size_t)nx * nx + nx + (size_t)nx * (nz + 1) + (size_t)nz * (nz + 1) + (size_t)nu * nu + 2 * (size_t)nu * (nx + 1) + 3;
+  if (int rc = grow(s, who, s->lqr_ws_scope, s->lqr_ws_cap, (size_t)L, 8 * ws + 4, "workspace", "L", [&](size_t n) {
+        p.P = dalloc<double>(s, n * nx * nx); p.s = dalloc<double>(s, n * nx); p.W = dalloc<double>(s, n * nx * (nz + 1));
+        p.H = dalloc<double>(s, n * nz * (nz + 1)); p.C = dalloc<double>(s, n * nu * nu); p.X = dalloc<double>(s, n * nu * (nx + 1));
+        p.G = dalloc<double>(s, n * nu * (nx + 1)); p.mu = dalloc<double>(s, n); p.dV = dalloc<double>(s, 2 * n); p.status = dalloc<int>(s, n);
+        p.Q = dalloc<double>(s, nx); p.R = dalloc<double>(s, nu); p.Qf = dalloc<double>(s, nx); }))
+    return rc;
+  if (copy_async(s, (void*)p.A, A, 4 * lt * nx * nx) != 0 || copy_async(s, (void*)p.B, B, 4 * lt * nx * nu) != 0 ||
+      copy_async(s, (void*)p.q, q, 8 * l1 * nx) != 0 || copy_async(s, (void*)p.r, r, 8 * lt * nu) != 0 ||
+      copy_async(s, (void*)p.Q, Q, 8 * (size_t)nx) != 0 || copy_async(s, (void*)p.R, R, 8 * (size_t)nu) != 0 ||
+      copy_async(s, (void*)p.Qf, Qf, 8 * (size_t)nx) != 0 || copy_async(s, (void*)p.mu, mu, 8 * (size_t)L) != 0) return -2;
+  p.L = L; p.T = T; p.nx = nx; p.nu = nu;
+  warp_launch(s, "lqr_init", L, 0, LqrWarp<0>{p});
+  for (int t = T - 1; t >= 0; t--) {           // no host synchronisation inside the pass
+    p.t = t;
+    warp_launch(s, "lqr_w", L * lqr_tiles(nx, nz + 1), 0, LqrWarp<1>{p});
+    warp_launch(s, "lqr_h", L * lqr_tiles(nz, nz + 1), 0, LqrWarp<2>{p});
+    warp_launch(s, "lqr_chol", L, 0, LqrWarp<3>{p});
+    warp_launch(s, "lqr_solve", L * ((nx + 1 + 31) / 32), 0, LqrWarp<4>{p});
+    warp_launch(s, "lqr_p", L * lqr_tiles(nx, nx + 1), 0, LqrWarp<5>{p});
+  }
+  if (launch_check(s, who) != 0) return -2;
+  s->lqr_done = L;
+  return sync_stream(s);                       // host inputs may be reused once the call returns
+}
+
+int fb_lqr_read(FbHandle s, double* K, double* k, double* dV, int32_t* status, int is_device) {
+  if (!s) return -1;
+  if (s->lqr_done < 1) { s->err = "fb_lqr_read: no backward pass to read (fb_lqr)"; return -1; }
+  const DevLqr& p = s->lqr;
+  const size_t lt = (size_t)p.L * p.T;
+  return read_out(s, {{K, p.K, 0, 8 * lt * p.nu * p.nx, 1}, {k, p.k, 0, 8 * lt * p.nu, 1}, {dV, p.dV, 0, 16 * (size_t)p.L, 1},
+                      {status, p.status, 0, 4 * (size_t)p.L, 1}});
 }
 
 }  // extern "C"

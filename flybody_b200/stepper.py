@@ -35,7 +35,8 @@ EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl'
            'fb_param_size', 'fb_param_set', 'fb_param_get', 'fb_param_draws', 'fb_param_clear',
            'fb_fd_param_program', 'fb_fd_param_columns', 'fb_fd_param_transition', 'fb_fd_param_read', 'fb_fd_param_sensor_read',
            'fb_fd_param_inverse', 'fb_fd_param_inverse_read', 'fb_fd_param_inverse_sensor_read',
-           'fb_rollout_feedback', 'fb_rollout', 'fb_rollout_read', 'fb_rollout_sensor_read']
+           'fb_rollout_feedback', 'fb_rollout', 'fb_rollout_read', 'fb_rollout_sensor_read', 'fb_rollout_feedback_bank',
+           'fb_lqr', 'fb_lqr_read']
 
 
 # enum FbTaskKind (FbTaskProgram.kind)
@@ -208,6 +209,9 @@ def load_library(path=None):
     lib.fb_rollout.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 3 + [C.c_int]
     lib.fb_rollout_read.argtypes = [C.c_void_p] + [C.c_void_p] * 6 + [C.c_int]
     lib.fb_rollout_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
+    lib.fb_rollout_feedback_bank.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    lib.fb_lqr.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 8 + [C.c_int]
+    lib.fb_lqr_read.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int]
     return lib
 
 
@@ -633,6 +637,18 @@ class BatchedStepper:
         ptrs, _keep = self._inputs([('x_ref', x_ref, (T, m.nq + m.nv + m.na)), ('K', K, (T, m.nu, 2 * m.nv + m.na))], is_device)
         self._check(self._lib.fb_rollout_feedback(self._h, T, *ptrs, int(bool(is_device))), 'fb_rollout_feedback')
 
+    def rollout_feedback_bank(self, x_ref, K, law, L=None, T=None, is_device=False):
+        """a bank of L feedback laws, x_ref [L, T, nq + nv + na] and K [L, T, nu, nx] (host arrays, or device pointers with is_device=True
+        and L, T given), and law [n] (host ints in [0, L)): rollout i of the n-rollout calls that follow applies law law[i]"""
+        m = self.model
+        if not is_device:
+            L, T = np.shape(x_ref)[:2]
+        L, T = int(L), int(T)
+        lw = np.ascontiguousarray(np.asarray(law).reshape(-1), np.int32)
+        ptrs, _keep = self._inputs([('x_ref', x_ref, (L, T, m.nq + m.nv + m.na)), ('K', K, (L, T, m.nu, 2 * m.nv + m.na))], is_device)
+        self._check(self._lib.fb_rollout_feedback_bank(self._h, L, T, *ptrs, lw.ctypes.data, len(lw), int(bool(is_device))),
+                    'fb_rollout_feedback_bank')
+
     def rollout(self, slots, ctrl, n_substeps=1, qfrc_applied=None, xfrc_applied=None, T=None, is_device=False):
         """rollout i from bank row slots[i] in env i: ctrl [n, T, nu], optional qfrc_applied [n, T, nv] and xfrc_applied [n, T, nbody, 6]
         (host arrays, or device pointers with is_device=True and T given); T control steps of n_substeps substeps.  The envs' states
@@ -680,6 +696,30 @@ class BatchedStepper:
         m, (n, T) = self.model, getattr(self, '_roll', (0, 0))
         out, ptrs, dev = self._outputs(out, [(n, T, m.nsensordata)] * 2, [np.float32] * 2)
         self._check(self._lib.fb_rollout_sensor_read(self._h, *ptrs, int(dev)), 'fb_rollout_sensor_read')
+        return tuple(out)
+
+    # ---- the iLQR backward pass (fb_lqr*; flybody_b200.trajopt is the front end)
+    def lqr(self, A, B, q, r, Q, R, Qf, mu):
+        """the Riccati backward pass of L problems: A [L, T, nx, nx], B [L, T, nx, nu] (fp32), q [L, T + 1, nx], r [L, T, nu], the
+        diagonal weights Q [nx], R [nu], Qf [nx] and mu [L] (fp64), host arrays (see the header); read with lqr_read()"""
+        m = self.model
+        nx, nu = 2 * m.nv + m.na, m.nu
+        L, T = np.shape(A)[:2]
+        want = [('A', (L, T, nx, nx), np.float32), ('B', (L, T, nx, nu), np.float32), ('q', (L, T + 1, nx), np.float64),
+                ('r', (L, T, nu), np.float64), ('Q', (nx,), np.float64), ('R', (nu,), np.float64), ('Qf', (nx,), np.float64),
+                ('mu', (L,), np.float64)]
+        keep = [np.ascontiguousarray(x, dt) for x, (_, _, dt) in zip((A, B, q, r, Q, R, Qf, mu), want)]
+        for x, (name, shape, _) in zip(keep, want):
+            if x.shape != shape:
+                raise ValueError(f'{name} {x.shape} against {shape}')
+        self._check(self._lib.fb_lqr(self._h, int(L), int(T), *[x.ctypes.data for x in keep], 0), 'fb_lqr')
+        self._lqr = (int(L), int(T))
+
+    def lqr_read(self):
+        """-> (K [L, T, nu, nx], k [L, T, nu], dV [L, 2] fp64, status [L] int32) of the last lqr"""
+        m, (L, T) = self.model, getattr(self, '_lqr', (0, 0))
+        out = [np.zeros((L, T, m.nu, 2 * m.nv + m.na)), np.zeros((L, T, m.nu)), np.zeros((L, 2)), np.zeros(L, np.int32)]
+        self._check(self._lib.fb_lqr_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_lqr_read')
         return tuple(out)
 
     def reset(self, qpos=None, qvel=None, env_ids=None):

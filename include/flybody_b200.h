@@ -677,6 +677,12 @@ int fb_fd_param_inverse_sensor_read(FbHandle h, float* DsDp, float* sensordata, 
  *   x_t the state the step starts from and the difference fb_fd_transition's tangent (mj_differentiatePos(xref qpos, qpos) per joint,
  *   then qvel and act), so gains from a Riccati recursion on its A and B apply without conversion.  Fixed order: a rollout's bits do
  *   not depend on its slot or on the batch size.
+ *   A bank of laws (fb_rollout_feedback_bank, in place of the shared law): xref [L][T][nq + nv + na] and K [L][T][nu][nx] (fp32, host
+ *   rows or device pointers as is_device says), and the host list law [n] (int32, values in [0, L)): rollout i applies law law[i], with
+ *   the same arithmetic as the shared law, so its bits equal a shared-law call with that law.  The fb_rollout calls that follow must
+ *   have n rollouts.  fb_rollout_feedback is the bank of L = 1 without a list (any n).  The buffers are kept and grown on use; -4 with
+ *   a message when they do not fit.  Errors: fb_rollout_feedback's, L < 1, L > 1 without a list, a list of n < 1, a law out of range;
+ *   it synchronises with host arrays or a list.
  *   Records (fb_rollout_read), after control step t in row [i][t]: qpos [n][T][nq], qvel, act, ctrl as written, time [n][T] and the
  *   env's flags [n][T].  With fb_query_sensors on (fb_rollout_sensor_read): sensordata [n][T][nsd], what fb_get(FB_SENSORDATA) returns
  *   after the step, and sensor_mean, what fb_get(FB_SENSOR_MEAN) returns (the same division by n_substeps).  The buffers are allocated
@@ -685,12 +691,32 @@ int fb_fd_param_inverse_sensor_read(FbHandle h, float* DsDp, float* sensordata, 
  * was held for a reset, a non-finite host input, applied-force sequences without the applied-force arrays, a feedback law of another
  * horizon.  fb_rollout synchronises; a device input is not checked.  fb_rollout_feedback: T >= 1 with both arrays, a tangent that does
  * not fit in shared memory, non-finite host values; it synchronises with host arrays.  The reads synchronise (any pointer may be NULL;
- * is_device: device pointers) and refuse before any rollout, or for sensors after a rollout with sensors off.                      */
+ * is_device: device pointers) and refuse before any rollout, or for sensors after a rollout with sensors off.  fb_rollout refuses a
+ * call whose n differs from the law list's.                                                                                          */
 int fb_rollout_feedback(FbHandle h, int T, const float* xref, const float* K, int is_device);
+int fb_rollout_feedback_bank(FbHandle h, int L, int T, const float* xref, const float* K, const int32_t* law, int n, int is_device);
 int fb_rollout(FbHandle h, const int32_t* slots, int n, int T, int n_substeps, const float* ctrl, const float* qfrc_applied,
                const float* xfrc_applied, int is_device);
 int fb_rollout_read(FbHandle h, float* qpos, float* qvel, float* act, float* ctrl, float* time, int32_t* flags, int is_device);
 int fb_rollout_sensor_read(FbHandle h, float* sensordata, float* sensor_mean, int is_device);
+/* The iLQR backward pass (Tassa, Erez & Todorov 2012), batched over L problems of T steps, all in fp64 (nx = 2 nv + na, nu):
+ *   inputs (host arrays, or device pointers when is_device): A [L][T][nx][nx] and B [L][T][nx][nu] (fp32, as fb_fd_read writes them),
+ *   the cost gradients q [L][T+1][nx] and r [L][T][nu], the diagonal weights Q [nx], R [nu] and Qf [nx] shared by every problem, and
+ *   the regularisation mu [L].  For t = T-1 .. 0 from s = q_T, P = diag(Qf):
+ *     Qx = q_t + A's,  Qu = r_t + B's,  Qxx = diag(Q) + A'PA,  Quu = diag(R) + B'PB + mu I,  Qux = B'PA,
+ *     k = -Quu^-1 Qu,  K = -Quu^-1 Qux  (Cholesky of Quu),  dV1 += k'Qu,  dV2 += k'Quu k / 2,
+ *     s = Qx + K'Quu k + K'Qu + Qux'k,  P = sym(Qxx + K'Quu K + K'Qux + Qux'K).
+ *   A Cholesky pivot that is not positive and finite sets status = t + 1 and stops that problem (its K, k and dV are then incomplete).
+ * Five launches per step with no host synchronisation inside the pass; fixed-order sums and no atomics, so a problem's bits depend on
+ * neither its index nor L.  The buffers are allocated on first use and grown with L T and L (a problem's workspace is
+ * 8 (nx^2 + (nx + nu + 1)(2 nx + nu) + nu^2 + 2 nu (nx + 1)) bytes); -4 with a message when they do not fit.  Errors: L < 1, T < 1, a
+ * NULL input, a model without actuators, nx + nu too large for the workspace's 32-bit offsets, a non-finite host input.  Weights of
+ * any sign are accepted (an indefinite Quu reports its status).  It synchronises; a device input is not checked.
+ * fb_lqr_read (synchronises; any pointer may be NULL; is_device: device pointers): K [L][T][nu][nx], k [L][T][nu], dV [L][2] (dV1, dV2)
+ * and status [L] (int32); an error before any pass.                                                                                  */
+int fb_lqr(FbHandle h, int L, int T, const float* A, const float* B, const double* q, const double* r, const double* Q, const double* R,
+           const double* Qf, const double* mu, int is_device);
+int fb_lqr_read(FbHandle h, double* K, double* k, double* dV, int32_t* status, int is_device);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
