@@ -524,6 +524,13 @@ static int build_model(FbSim* s, const FbModel* h) {
     if (bt != 0 && bt != 1) { s->err = who + "biastype " + std::to_string(bt) + " is not implemented (none = 0, affine = 1 are)"; return -3; }
     if ((dt == 2) != (aa >= 0) || aa >= h->na) { s->err = who + "activation address " + std::to_string(aa) + " does not match dyntype " + std::to_string(dt); return -3; }
   }
+  // the touch ray test (kfin_f9, kinv_sensors) knows capsule sites and treats every other site as a sphere of radius size[0]: a touch
+  // sensor on an ellipsoid, box or cylinder site would be tested against the wrong shape, so such a model is refused
+  for (int i = 0; i < h->nsensor; i++) {
+    if (h->sensor_type[i] != FB_SENS_TOUCH) continue;
+    int t = h->site_type[h->sensor_objid[i]];
+    if (t != FB_GEOM_SPHERE && t != FB_GEOM_CAPSULE) { s->err = "sensor " + std::to_string(i) + ": touch site of type " + std::to_string(t) + " is not implemented (sphere = 2, capsule = 3 are)"; return -3; }
+  }
   { const char* rt = getenv("FB_SOLVE_RTOL"); m.solve_rtol = rt ? (float)atof(rt) : 1e-6f; }     // relative improvement that ends the Newton iteration (test hook)
   { const char* nc = getenv("FB_SOLVE_NCAP"); m.solve_ncap = nc ? atoi(nc) : FB_SOLVE_NCAP; if (m.solve_ncap > FB_SOLVE_NCAP) m.solve_ncap = FB_SOLVE_NCAP; }   // test hook: smaller cap -> global-memory path
   m.timestep = (float)h->opt_timestep; m.density = (float)h->opt_density; m.viscosity = (float)h->opt_viscosity;

@@ -193,7 +193,9 @@ enum FbField {
 typedef struct FbSim* FbHandle;
 
 /* mjcf.Physics.from_mjcf_model + mj_makeData, batched: uploads the model, allocates SoA state
- * for n_envs environments on `device`, all envs at qpos0 / zero velocity.                     */
+ * for n_envs environments on `device`, all envs at qpos0 / zero velocity.
+ * Refuses (-3, fb_last_error says why) a model the step would integrate as something else: among others, a touch sensor on a site
+ * that is neither a sphere nor a capsule (the touch ray test knows those two shapes only; MuJoCo ray-tests the site's own shape). */
 int fb_create(const FbModel* m, int n_envs, int device, FbHandle* out);
 int fb_destroy(FbHandle h);
 

@@ -149,6 +149,10 @@ OrcData* orc_create(const FbModel* m) {
     int dt=m->actuator_dyntype[i], bt=m->actuator_biastype[i], aa=m->actuator_actadr[i];
     if ((dt!=0 && dt!=2) || (bt!=0 && bt!=1) || (dt==2)!=(aa>=0) || aa>=m->na) return NULL;
   }
+  /* the touch ray test (orc_sensors_acc) knows capsule and sphere sites only: refuse a touch sensor on any other site type */
+  for (int i=0;i<m->nsensor;i++)
+    if (m->sensor_type[i]==FB_SENS_TOUCH && m->site_type[m->sensor_objid[i]]!=FB_GEOM_SPHERE && m->site_type[m->sensor_objid[i]]!=FB_GEOM_CAPSULE)
+      return NULL;
   OrcData* d = (OrcData*)calloc(1, sizeof(OrcData));
   d->m = m;
   int nv=m->nv, nb=m->nbody;

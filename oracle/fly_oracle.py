@@ -65,7 +65,8 @@ class Oracle:
         self._d = self._l.orc_create(C.byref(model.c))
         if not self._d:
             raise ValueError('orc_create refused the model: an actuator has a dynamics or bias type the oracle does not implement '
-                             '(dyntype none / filter, biastype none / affine) or an activation address that does not match its dyntype')
+                             '(dyntype none / filter, biastype none / affine) or an activation address that does not match its dyntype, '
+                             'or a touch sensor is on a site that is neither a sphere nor a capsule')
         self._l.orc_set_dense(self._d, 1 if dense else 0)
         if tolerance is not None:
             self._l.orc_set_tolerance(self._d, float(tolerance))

@@ -7,6 +7,9 @@ cannot be tighter than the 1e-3 of tests/parity_common.py.  `analytic_model` kee
 sphere, capsule), so the oracle and the stepper solve the same problem up to the fp32 rounding of the model, and the solver's own
 error can be held about ten times tighter, per contact.
 """
+import os
+import subprocess
+
 import numpy as np
 
 from flybody_b200 import stepper as st
@@ -43,6 +46,18 @@ STATES = {
     'middle_mu1_a':  ((36, 0.3, 1.0),   dict(nefc=97, nlimit=16, ncontact=27, cond1=0, cond3=27, top=21, bottom=1, middle=5, cols=24)),
     'middle_mu1_b':  ((29, 0.3, 1.0),   dict(nefc=99, nlimit=15, ncontact=28, cond1=0, cond3=28, top=24, bottom=2, middle=2, cols=19)),
 }
+
+
+def build_chol_variants(out_dir, csrc):
+    """the host-emulation build of the kernel source with FB_CHOL_REG = 0 (every Hessian block factorised in the record) and 8 (both
+    forms), compiled in parallel into out_dir: {0: path, 8: path}"""
+    out, procs = {}, []
+    for reg in (0, 8):
+        out[reg] = os.path.join(str(out_dir), f'libfb_emu_chol{reg}.so')
+        procs.append(subprocess.Popen(['g++', '-x', 'c++', '-DFB_EMU', f'-DFB_CHOL_REG={reg}', '-O2', '-std=c++17', '-fPIC', '-shared',
+                                       '-o', out[reg], os.path.join(csrc, 'flybody_b200.cu'), '-lm']))
+    assert all(p.wait() == 0 for p in procs)
+    return out
 
 
 def analytic_model(m, noslip=None):

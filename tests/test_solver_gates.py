@@ -18,9 +18,6 @@ force, and the terms that cancel in their jar are 1e4 times larger than their fo
 not move with the fp32 rounding of the model (solver_states.fp32_model: 5.60e-3 -> 5.44e-3, 1.87e-3 -> 1.87e-3), and it is 11 - 13
 units of 2^-24 of those terms, like the other rows' (up to 37): RES_ULPS holds them at that resolution.
 """
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
@@ -119,15 +116,7 @@ def emu():
 @pytest.fixture(scope='module')
 def emu_chol(tmp_path_factory):
     """the host-emulation build with FB_CHOL_REG = 0 (every Hessian block factorised in the record) and 8 (both forms)"""
-    out = {}
-    d = tmp_path_factory.mktemp('emu_chol')
-    procs = []
-    for reg in (0, 8):
-        out[reg] = str(d / f'libfb_emu_chol{reg}.so')
-        procs.append(subprocess.Popen(['g++', '-x', 'c++', '-DFB_EMU', f'-DFB_CHOL_REG={reg}', '-O2', '-std=c++17', '-fPIC', '-shared', '-o',
-                                       out[reg], os.path.join(ge.CSRC, 'flybody_b200.cu'), '-lm']))
-    assert all(p.wait() == 0 for p in procs)
-    return out
+    return ss.build_chol_variants(tmp_path_factory.mktemp('emu_chol'), ge.CSRC)
 
 
 @pytest.mark.parametrize('placement', ['default', 'ncap0', 'chol_reg0', 'chol_reg8'])
