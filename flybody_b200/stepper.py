@@ -1,4 +1,5 @@
-"""ctypes binding of the CUDA stepper's C ABI (`include/flybody_b200.h`).
+"""ctypes binding of the CUDA stepper's C ABI (`include/flybody_b200.h`; its prototypes, enums and program structs are read from
+the header by `abi.py`).
 
 `BatchedStepper` is the batched stand-in for the `physics` object that dm_control hands to the
 reference's task hooks (SURVEY.md 8(b)): `set_control`, `step`, state reads.  It fails loudly
@@ -9,209 +10,39 @@ import os
 
 import numpy as np
 
-from .flymodel import FbModel, FlyModel
+from . import abi
+from .abi import StepperError
+from .flymodel import FlyModel
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libflybody_b200.so')
 
-# enum FbField
-(QPOS, QVEL, ACT, CTRL, QACC, QACC_WARMSTART, SENSORDATA, SENSOR_MEAN, XPOS, XMAT, SITE_XPOS, SITE_XMAT,
- SUBTREE_COM, NCON, NEFC, TIME, QFRC_SMOOTH, QM_DENSE, QFRC_CONSTRAINT, SOLVER_NITER, QFRC_PASSIVE,
- QFRC_BIAS, QFRC_ACTUATOR, CONTACT, EFC_FORCE, FLAGS, QFRC_APPLIED, XFRC_APPLIED) = range(28)
-MAXCON, MAXEFC = 64, 160
+_ABI = abi.read()
+# enum FbField (fb_get / fb_set fields: QPOS .. XFRC_APPLIED), enum FbObsItem (OBS_*) and enum FbTaskKind (TASK_*, FbTaskProgram.kind),
+# by their header names without FB_
+globals().update({name[3:]: v for enum in ('FbField', 'FbObsItem', 'FbTaskKind') for name, v in _ABI.enums[enum].items()})
+MAXCON, MAXEFC = _ABI.defines['FB_MAXCON'], _ABI.defines['FB_MAXEFC']
 
-# enum FbParam: the per-env model parameters (fb_param_*), by their mjModel names, and their shape per env
-PARAMS = ('body_mass', 'body_inertia', 'dof_armature', 'dof_damping', 'jnt_stiffness', 'geom_friction', 'actuator_gainprm',
-          'actuator_biasprm', 'gravity', 'wind', 'density', 'viscosity')
+# enum FbParam: the per-env model parameters (fb_param_*), by their mjModel names, in id order
+PARAMS = tuple(name[5:].lower() for name, _ in sorted(_ABI.enums['FbParam'].items(), key=lambda e: e[1]) if name != 'FB_NPARAMS')
 FD_ELEMENT, FD_SCALE = 0, 1           # kinds of a parameter direction (fb_fd_param_program)
 
-EXPORTS = ['fb_create', 'fb_destroy', 'fb_reset', 'fb_reset_hold', 'fb_set_ctrl', 'fb_set_action_map', 'fb_write_state', 'fb_applied_ptrs', 'fb_clear_applied', 'fb_step', 'fb_forward',
-           'fb_get', 'fb_field_size', 'fb_record_stride', 'fb_set', 'fb_obs_ptr', 'fb_n_envs', 'fb_n_envs_padded', 'fb_stream',
-           'fb_sync', 'fb_pack_obs', 'fb_read_obs', 'fb_obs_program', 'fb_ref_slots', 'fb_ref_slot_write', 'fb_task_program', 'fb_task_step', 'fb_task_reset_all', 'fb_task_request_reset', 'fb_task_set_reset_noise', 'fb_task_episodes', 'fb_task_uniforms', 'fb_task_uniform_rows', 'fb_hfield_bank', 'fb_ref_bank', 'fb_ref_bank_wide', 'fb_task_ref_pick', 'fb_task_ref_state', 'fb_task_ptrs', 'fb_task_read', 'fb_eye_program', 'fb_hfield_collision', 'fb_hfield_write', 'fb_render_eyes', 'fb_eyes_ptr', 'fb_eyes_read', 'fb_task_inputs', 'fb_read_task_obs', 'fb_profile', 'fb_profile_read', 'fb_profile_name', 'fb_step_kernel_smem', 'fb_launch_count', 'fb_last_step_ms', 'fb_set_solver', 'fb_last_error', 'fb_version',
-           'fb_state_slots', 'fb_state_signature', 'fb_state_bank', 'fb_state_save', 'fb_state_load', 'fb_state_read', 'fb_state_write', 'fb_state_substeps',
-           'fb_ik_program', 'fb_ik_solve', 'fb_ik_read', 'fb_inverse', 'fb_inverse_read',
-           'fb_fd_columns', 'fb_fd_transition', 'fb_fd_read', 'fb_fd_inverse_columns', 'fb_fd_inverse', 'fb_fd_inverse_read',
-           'fb_query_sensors', 'fb_inverse_sensor_read', 'fb_fd_sensor_read', 'fb_fd_inverse_sensor_read',
-           'fb_param_size', 'fb_param_set', 'fb_param_get', 'fb_param_draws', 'fb_param_clear',
-           'fb_fd_param_program', 'fb_fd_param_columns', 'fb_fd_param_transition', 'fb_fd_param_read', 'fb_fd_param_sensor_read',
-           'fb_fd_param_inverse', 'fb_fd_param_inverse_read', 'fb_fd_param_inverse_sensor_read',
-           'fb_rollout_feedback', 'fb_rollout', 'fb_rollout_read', 'fb_rollout_sensor_read', 'fb_rollout_feedback_bank',
-           'fb_lqr', 'fb_lqr_read']
-
-
-# enum FbTaskKind (FbTaskProgram.kind)
-TASK_WALK, TASK_FLIGHT, TASK_VISION, TASK_TEMPLATE, TASK_BALL = range(5)
-
-# enum FbObsItem
-(OBS_SENSOR_MEAN, OBS_SENSOR_NOW, OBS_ACT, OBS_QPOS, OBS_QVEL, OBS_SITES_EGO, OBS_ROOT_ZAXIS, OBS_REF_DISP,
- OBS_REF_QUAT, OBS_SCALARS, OBS_ROOT_POSE, OBS_SUBTREE_COM, OBS_DOF_AXIS_EGO, OBS_WORLD_CONTACT, OBS_TASK_TARGET) = range(15)
-
-
-class FbObsProgram(C.Structure):
-    _fields_ = [('n_items', C.c_int32), ('kind', C.POINTER(C.c_int32)), ('a', C.POINTER(C.c_int32)),
-                ('b', C.POINTER(C.c_int32)), ('n_list', C.c_int32), ('list', C.POINTER(C.c_int32)),
-                ('root_body', C.c_int32), ('n_sub', C.c_int32), ('ref_len', C.c_int32),
-                ('ref_qpos', C.POINTER(C.c_float))]
-
-
-class FbTaskProgram(C.Structure):
-    """include/flybody_b200.h: FbTaskProgram (device-side task logic)."""
-    _fields_ = [('kind', C.c_int32), ('root_qadr', C.c_int32), ('root_vadr', C.c_int32), ('ghost_qadr', C.c_int32), ('ghost_vadr', C.c_int32),
-                ('user_col', C.c_int32), ('ghost_offset', C.c_float * 3), ('control_timestep', C.c_float), ('time_limit', C.c_float),
-                ('terminal_com_dist', C.c_float), ('terminal_linvel', C.c_float), ('terminal_angvel', C.c_float), ('terminal_qacc', C.c_float),
-                ('terminal_height', C.c_float), ('velocimeter_adr', C.c_int32), ('gyro_adr', C.c_int32), ('com_body', C.c_int32),
-                ('episode_steps', C.c_int32), ('ref_len', C.c_int32), ('ref_qpos', C.POINTER(C.c_float)), ('ref_qvel', C.POINTER(C.c_float)),
-                ('obs_refdisp_off', C.c_int32), ('obs_refquat_off', C.c_int32), ('reset_qpos', C.POINTER(C.c_float)),
-                ('n_noise', C.c_int32), ('noise_qadr', C.POINTER(C.c_int32)), ('noise_amp', C.c_float), ('seed', C.c_uint32),
-                ('n_wing', C.c_int32), ('wing_qadr', C.POINTER(C.c_int32)), ('wing_vadr', C.POINTER(C.c_int32)), ('wing_ctrl', C.POINTER(C.c_int32)),
-                ('n_freq', C.c_int32), ('tab_len', C.c_int32), ('wb_traj', C.POINTER(C.c_float)), ('wb_phase', C.POINTER(C.c_float)),
-                ('wb_phase_mod', C.POINTER(C.c_float)), ('wb_freqs', C.POINTER(C.c_float)), ('wb_len', C.POINTER(C.c_int32)),
-                ('wb_base_freq', C.c_float), ('wb_rel_range', C.c_float), ('wb_rate', C.c_float), ('com_offset', C.c_float * 3),
-                ('target_height_range', C.c_float * 2), ('target_speed_range', C.c_float * 2), ('init_x_range', C.c_float * 2), ('init_y_range', C.c_float * 2),
-                ('hover_quat', C.c_float * 4), ('target_zaxis', C.c_float * 3), ('floor_contacts_fatal', C.c_int32),
-                ('trench_cap', C.c_int32), ('trench_x', C.POINTER(C.c_float)), ('trench_len', C.POINTER(C.c_int32)), ('trench_y', C.POINTER(C.c_float)),
-                ('ref_bank', C.c_int32), ('n_pick', C.c_int32), ('pick_traj', C.POINTER(C.c_int32)), ('randomize_start', C.c_int32),
-                ('start_margin', C.c_int32), ('max_episode_rows', C.c_int32), ('future_steps', C.c_int32),
-                ('n_mocap_joints', C.c_int32), ('mocap_qadr', C.POINTER(C.c_int32)), ('n_mocap_sites', C.c_int32),
-                ('obs_root_pose_off', C.c_int32), ('obs_root_qvel_off', C.c_int32), ('obs_mocap_qpos_off', C.c_int32),
-                ('obs_mocap_qvel_off', C.c_int32), ('obs_mocap_axes_off', C.c_int32), ('obs_mocap_sites_off', C.c_int32),
-                ('obs_wing_qpos_off', C.c_int32), ('wing_spring', C.POINTER(C.c_float)), ('deep_mimic_std', C.c_float * 4),
-                ('deep_mimic_weight', C.c_float * 4), ('retract_margin', C.c_float),
-                ('ball_vadr', C.c_int32), ('ball_target', C.c_float * 3), ('ball_margin', C.c_float)]
-
-
-class FbEyeProgram(C.Structure):
-    """include/flybody_b200.h: FbEyeProgram (eye cameras)."""
-    _fields_ = [('n_cam', C.c_int32), ('body', C.c_int32 * 2), ('pos', (C.c_float * 3) * 2), ('quat', (C.c_float * 4) * 2),
-                ('fovy_deg', C.c_float), ('size', C.c_int32), ('nrow', C.c_int32), ('ncol', C.c_int32), ('half_size', C.c_float),
-                ('z_offset', C.c_float), ('zfar', C.c_float), ('sky_top', C.c_float * 3), ('sky_horizon', C.c_float * 3),
-                ('ground', C.c_float * 3), ('ambient', C.c_float), ('diffuse', C.c_float)]
-
-
-class FbIkProgram(C.Structure):
-    """include/flybody_b200.h: FbIkProgram (multi-site inverse kinematics)."""
-    _fields_ = [('n_sites', C.c_int32), ('site_ids', C.POINTER(C.c_int32)), ('n_jnts', C.c_int32), ('jnt_ids', C.POINTER(C.c_int32)),
-                ('include', C.POINTER(C.c_uint8)), ('reg_strength', C.c_float), ('lr', C.c_float), ('beta', C.c_float),
-                ('progress_threshold', C.c_float), ('max_steps', C.c_int32)]
-
-
-class StepperError(RuntimeError):
-    pass
+# the programs of fb_obs_program, fb_task_program, fb_eye_program and fb_ik_program
+FbObsProgram, FbTaskProgram, FbEyeProgram, FbIkProgram = (_ABI.structs[n] for n in ('FbObsProgram', 'FbTaskProgram', 'FbEyeProgram',
+                                                                                      'FbIkProgram'))
 
 
 def load_library(path=None):
+    """the stepper library with every function the header declares bound to its prototype"""
     path = path or os.environ.get('FLYBODY_B200_LIB') or LIB_PATH      # the env override is for A/B timing of kernel variants
     if not os.path.exists(path):
         raise StepperError(
             f'CUDA stepper library not found at {path}. Build it with `python -c "import __graft_entry__ as g; '
             f'g.build()"` (nvcc, sm_90a). There is no CPU fallback.')
     lib = C.CDLL(path)
-    lib.fb_create.argtypes = [C.POINTER(FbModel), C.c_int, C.c_int, C.POINTER(C.c_void_p)]
-    lib.fb_destroy.argtypes = [C.c_void_p]
-    lib.fb_reset.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.fb_reset_hold.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.fb_set_ctrl.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    lib.fb_set_action_map.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    lib.fb_write_state.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_applied_ptrs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    lib.fb_clear_applied.argtypes = [C.c_void_p]
-    lib.fb_step.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_forward.argtypes = [C.c_void_p]
-    lib.fb_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    lib.fb_field_size.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_record_stride.argtypes = [C.c_void_p]
-    lib.fb_set.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_obs_ptr.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]
-    lib.fb_obs_program.argtypes = [C.c_void_p, C.c_void_p]
-    lib.fb_task_inputs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.fb_ref_slots.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_task_program.argtypes = [C.c_void_p, C.c_void_p]
-    lib.fb_task_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    lib.fb_task_reset_all.argtypes = [C.c_void_p]
-    lib.fb_task_uniforms.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_task_request_reset.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    lib.fb_task_episodes.argtypes = [C.c_void_p, C.c_void_p]
-    lib.fb_task_set_reset_noise.argtypes = [C.c_void_p, C.c_float]
-    lib.fb_task_uniform_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_hfield_bank.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_ref_bank.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.fb_ref_bank_wide.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_task_ref_pick.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.fb_task_ref_state.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.fb_task_ptrs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p)]
-    lib.fb_task_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.fb_eye_program.argtypes = [C.c_void_p, C.c_void_p]
-    lib.fb_hfield_write.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_hfield_collision.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]
-    lib.fb_render_eyes.argtypes = [C.c_void_p]
-    lib.fb_eyes_ptr.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]
-    lib.fb_eyes_read.argtypes = [C.c_void_p, C.c_void_p]
-    lib.fb_ref_slot_write.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_read_task_obs.argtypes = [C.c_void_p, C.c_void_p]
-    lib.fb_pack_obs.argtypes = [C.c_void_p]
-    lib.fb_read_obs.argtypes = [C.c_void_p, C.c_void_p]
-    lib.fb_profile.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_profile_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-    lib.fb_profile_name.argtypes = [C.c_int]
-    lib.fb_profile_name.restype = C.c_char_p
-    lib.fb_step_kernel_smem.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    lib.fb_n_envs.argtypes = [C.c_void_p]
-    lib.fb_n_envs_padded.argtypes = [C.c_void_p]
-    lib.fb_stream.argtypes = [C.c_void_p]
-    lib.fb_stream.restype = C.c_void_p
-    lib.fb_sync.argtypes = [C.c_void_p]
-    lib.fb_launch_count.argtypes = [C.c_void_p]
-    lib.fb_launch_count.restype = C.c_longlong
-    lib.fb_last_step_ms.argtypes = [C.c_void_p]
-    lib.fb_last_step_ms.restype = C.c_float
-    lib.fb_set_solver.argtypes = [C.c_void_p, C.c_float, C.c_int]
-    lib.fb_last_error.argtypes = [C.c_void_p]
-    lib.fb_last_error.restype = C.c_char_p
-    lib.fb_version.restype = C.c_char_p
-    lib.fb_state_slots.argtypes = [C.c_void_p]
-    lib.fb_state_signature.argtypes = [C.c_void_p]
-    lib.fb_state_signature.restype = C.c_uint64
-    lib.fb_state_bank.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_state_save.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-    lib.fb_state_load.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-    lib.fb_state_read.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_state_write.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    lib.fb_state_substeps.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_ik_program.argtypes = [C.c_void_p, C.c_void_p]
-    lib.fb_ik_solve.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.fb_ik_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5
-    lib.fb_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    lib.fb_inverse_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-    lib.fb_fd_columns.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_fd_transition.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int]
-    lib.fb_fd_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_int]
-    lib.fb_fd_inverse_columns.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_fd_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int]
-    lib.fb_fd_inverse_read.argtypes = [C.c_void_p] + [C.c_void_p] * 5 + [C.c_int]
-    lib.fb_query_sensors.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_inverse_sensor_read.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    lib.fb_fd_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 3 + [C.c_int]
-    lib.fb_fd_inverse_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int]
-    lib.fb_param_size.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_param_set.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    lib.fb_param_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    lib.fb_param_draws.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_uint32]
-    lib.fb_param_clear.argtypes = [C.c_void_p]
-    lib.fb_fd_param_program.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
-    lib.fb_fd_param_columns.argtypes = [C.c_void_p, C.c_int]
-    lib.fb_fd_param_transition.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int]
-    lib.fb_fd_param_read.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int]
-    lib.fb_fd_param_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
-    lib.fb_fd_param_inverse.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int]
-    lib.fb_fd_param_inverse_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
-    lib.fb_fd_param_inverse_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
-    lib.fb_rollout_feedback.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
-    lib.fb_rollout.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 3 + [C.c_int]
-    lib.fb_rollout_read.argtypes = [C.c_void_p] + [C.c_void_p] * 6 + [C.c_int]
-    lib.fb_rollout_sensor_read.argtypes = [C.c_void_p] + [C.c_void_p] * 2 + [C.c_int]
-    lib.fb_rollout_feedback_bank.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    lib.fb_lqr.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 8 + [C.c_int]
-    lib.fb_lqr_read.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int]
+    for name, (restype, argtypes) in _ABI.functions.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     return lib
 
 

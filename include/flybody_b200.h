@@ -11,6 +11,9 @@
  * One handle = one device + one stream; calls on a handle are not re-entrant.
  * Device side: one fp32/int32 record per env (one warp steps one env); host-side buffers passed to fb_*
  * are rows [env][component] (what numpy/dm_env code holds).
+ *
+ * flybody_b200/abi.py binds this header from its text: prototypes, enums (with explicit values), integer #defines and
+ * structs of scalar, pointer and array fields.  It refuses any other construct or type, naming the line.
  */
 #ifndef FLYBODY_B200_H_
 #define FLYBODY_B200_H_

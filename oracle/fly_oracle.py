@@ -7,13 +7,13 @@ import subprocess
 
 import numpy as np
 
+from flybody_b200 import abi
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 
-# field ids (include/flybody_b200.h enum FbField)
-QPOS, QVEL, ACT, CTRL, QACC, QACC_WARMSTART, SENSORDATA, SENSOR_MEAN, XPOS, XMAT, SITE_XPOS, SITE_XMAT, \
-    SUBTREE_COM, NCON, NEFC, TIME, QFRC_SMOOTH, QM_DENSE, QFRC_CONSTRAINT, SOLVER_NITER, QFRC_PASSIVE, \
-    QFRC_BIAS, QFRC_ACTUATOR, CONTACT, EFC_FORCE, FLAGS = range(26)
+# field ids: include/flybody_b200.h enum FbField without FB_ (QPOS, QVEL, ...), the names orc_get / orc_set switch on
+globals().update({name[3:]: v for name, v in abi.read().enums['FbField'].items()})
 
 
 def build(force=False):
