@@ -32,6 +32,7 @@
 #include "fb_fd.h"
 #include "fb_rollout.h"
 #include "fb_lqr.h"
+#include "fb_plan.h"
 
 enum { K_ACT = 0, K_SMOOTH, K_REF, K_SOLVE, K_FINISH, K_POS, K_COL, K_CON, K_PROJ, K_VEL, K_SENS, K_PACK, K_MISC, K_NKIND };
 static const char* const kKindNames[K_NKIND] = {"act", "smooth", "ref", "solve", "finish", "pos", "col", "con", "proj", "vel", "sens", "pack", "misc"};
@@ -89,6 +90,11 @@ struct FbSim {
   // the iLQR backward pass (fb_lqr; fb_lqr.h): inputs and outputs of lqr_cap problem steps (L (T + 1)) and the workspace of lqr_ws_cap
   // problems, grown on demand; problems and steps of the last call
   DevLqr lqr = {}; std::vector<void*> lqr_scope, lqr_ws_scope; size_t lqr_cap = 0, lqr_ws_cap = 0; int lqr_done = 0;
+  // sampling-based MPC (fb_plan_program / fb_plan; fb_plan.h): the program (plan.K > 0: set) and its weights; the buffers, grown on demand
+  // with L K T (the samples), L K (their costs and weights), L (T + 1) (mean, xref, uref and the per-problem words) and L n_iter (the
+  // record); the rollout parameter of the samples; problems of the last call
+  DevPlan plan = {}; DevRoll plan_roll = {}; std::vector<void*> plan_prog_scope, plan_s_scope, plan_k_scope, plan_l_scope, plan_h_scope;
+  size_t plan_s_cap = 0, plan_k_cap = 0, plan_l_cap = 0, plan_h_cap = 0; int plan_done = 0;
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -2261,14 +2267,19 @@ static int fd_slots_valid(FbSim* s, const char* who, const int32_t* slots, int n
   }
   return 0;
 }
-// every env a copy of its problem's row, warm start included; the envs past the problems copy the last problem's
-static int fd_fan_out(FbSim* s, const int32_t* slots, int n, int ncol) {
+// the slot of every env (its problem's; the envs past the problems take the last problem's), uploaded as a device list
+static int fan_out_ids(FbSim* s, const int32_t* slots, int n, int ncol, const int** slot_dev) {
   const int N = s->d.N;
   std::vector<int32_t> fan(N);
   for (int e = 0; e < N; e++) fan[e] = slots[std::min(e / ncol, n - 1)];
-  const int *ed, *sd;
-  if (int rc = state_ids(s, nullptr, fan.data(), N, &ed, &sd)) return rc;
-  launch_state<true>(s, nullptr, sd, N);
+  const int* ed;
+  return state_ids(s, nullptr, fan.data(), N, &ed, slot_dev);
+}
+// every env a copy of its problem's row, warm start included; the envs past the problems copy the last problem's
+static int fd_fan_out(FbSim* s, const int32_t* slots, int n, int ncol) {
+  const int* sd;
+  if (int rc = fan_out_ids(s, slots, n, ncol, &sd)) return rc;
+  launch_state<true>(s, nullptr, sd, s->d.N);
   return 0;
 }
 
@@ -2731,6 +2742,128 @@ int fb_lqr_read(FbHandle s, double* K, double* k, double* dV, int32_t* status, i
   const size_t lt = (size_t)p.L * p.T;
   return read_out(s, {{K, p.K, 0, 8 * lt * p.nu * p.nx, 1}, {k, p.k, 0, 8 * lt * p.nu, 1}, {dV, p.dV, 0, 16 * (size_t)p.L, 1},
                       {status, p.status, 0, 4 * (size_t)p.L, 1}});
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------
+// sampling-based MPC (fb_plan; fb_plan.h): its own kernel parameter (DevPlan) and buffers, the samples rolled out through the rollout
+// input kernel with a DevRoll of their own
+template <int KIND> struct PlanWarp {
+  DevModel m; DevData d; DevPlan p;
+  FB_DEVM void operator()(unsigned char*, int w) const {
+    if (KIND == 0) kplan_sample(m, p, w); else if (KIND == 1) kplan_cost(m, d, p, w); else if (KIND == 2) kplan_weights(p, w);
+    else kplan_update(m, p, w);
+  }
+};
+
+extern "C" {
+
+int fb_plan_program(FbHandle s, const FbPlanProgram* g) {
+  if (!s) return -1;
+  const DevModel& m = s->m;
+  const size_t nx = 2 * (size_t)m.nv + m.na, nu = m.nu;
+  const bool clear = !g || g->n_samples == 0;
+  if (!clear) {
+    if (nu < 1) { s->err = "fb_plan_program: the model has no actuators"; return -1; }
+    if (g->n_samples < 2) { s->err = "fb_plan_program: n_samples >= 2 (0 clears the program)"; return -1; }
+    if (g->hold < 1) { s->err = "fb_plan_program: hold >= 1 control steps per knot"; return -1; }
+    if (!g->sigma || !g->Q || !g->R || !g->Qf) { s->err = "fb_plan_program: sigma, Q, R and Qf must not be NULL"; return -1; }
+    if (!(g->temperature >= 0.0) || !std::isfinite(g->temperature)) { s->err = "fb_plan_program: the temperature must be >= 0 and finite"; return -1; }
+    const void* arr[4] = {g->sigma, g->Q, g->R, g->Qf};
+    const size_t cnt[4] = {nu, nx, nu, nx};
+    const char* name[4] = {"sigma", "Q", "R", "Qf"};
+    for (int k = 0; k < 4; k++)
+      for (size_t i = 0; i < cnt[k]; i++) {
+        const double v = k ? ((const double*)arr[k])[i] : (double)((const float*)arr[k])[i];
+        if (!(v >= 0.0) || !std::isfinite(v)) { s->err = std::string("fb_plan_program: ") + name[k] + " must be >= 0 and finite"; return -1; }
+      }
+  }
+  dev_select(s);
+  if (sync_stream(s) != 0) return -2;          // a plan in flight may still read the old weights
+  scope_free(s, s->plan_prog_scope);
+  DevPlan& p = s->plan;
+  p.K = 0; p.sigma = nullptr; p.Q = p.R = p.Qf = nullptr;
+  s->plan_done = 0;
+  if (clear) return 0;
+  if (int rc = scope_alloc(s, s->plan_prog_scope, "fb_plan_program: out of device memory", [&] {
+        p.sigma = up(s, std::vector<float>(g->sigma, g->sigma + nu)); p.Q = up(s, std::vector<double>(g->Q, g->Q + nx));
+        p.R = up(s, std::vector<double>(g->R, g->R + nu)); p.Qf = up(s, std::vector<double>(g->Qf, g->Qf + nx)); })) {
+    p.sigma = nullptr; p.Q = p.R = p.Qf = nullptr; return rc; }
+  p.K = g->n_samples; p.hold = g->hold; p.temperature = g->temperature;
+  return 0;
+}
+
+int fb_plan(FbHandle s, const int32_t* slots, int L, int T, int n_substeps, int n_iter, const uint32_t* seeds, const float* mean,
+            const float* xref, const float* uref, int is_device) {
+  if (!s) return -1;
+  const char* who = "fb_plan";
+  if (state_ready(s, who) != 0) return -1;
+  DevPlan& p = s->plan;
+  if (p.K < 1) { s->err = "fb_plan: no plan program (fb_plan_program)"; return -1; }
+  const int N = s->d.N, K = p.K;
+  if (L < 1 || (long long)L * K > N) {
+    s->err = "fb_plan: 1 <= L problems with L * n_samples (" + std::to_string(K) + ") <= n_envs (" + std::to_string(N) + ")"; return -1; }
+  if (T < 1 || n_substeps < 1 || n_iter < 1) { s->err = "fb_plan: T >= 1 control steps, n_substeps >= 1 and n_iter >= 1"; return -1; }
+  if (!slots || !seeds || !mean || !xref) { s->err = "fb_plan: slots, seeds, mean and xref must not be NULL"; return -1; }
+  if (fd_slots_valid(s, who, slots, L) != 0) return -1;
+  const DevModel& m = s->m;
+  const size_t nu = m.nu, nr = (size_t)m.nq + m.nv + m.na, lt = (size_t)L * T, l1 = (size_t)L * (T + 1);
+  if (!is_device && (!all_finite(mean, lt * nu) || !all_finite(xref, l1 * nr) || (uref && !all_finite(uref, lt * nu)))) {
+    s->err = "fb_plan: non-finite mean, xref or uref"; return -1; }
+  dev_select(s);
+  s->plan_done = 0;
+  const size_t n = (size_t)L * K;
+  if (int rc = grow(s, who, s->plan_s_scope, s->plan_s_cap, n * T, 4 * nu, "samples", "L n_samples T", [&](size_t r) { p.ctrl = dalloc<float>(s, r * nu); }))
+    return rc;
+  if (int rc = grow(s, who, s->plan_k_scope, s->plan_k_cap, n, 16, "sample costs", "L n_samples", [&](size_t r) {
+        p.J = dalloc<double>(s, r); p.w = dalloc<double>(s, r); }))
+    return rc;
+  if (int rc = grow(s, who, s->plan_l_scope, s->plan_l_cap, l1, 4 * (2 * nu + nr) + 24, "means and references", "L (T + 1)", [&](size_t r) {
+        p.mean = dalloc<float>(s, r * nu); p.xref = dalloc<float>(s, r * nr); p.uref = dalloc<float>(s, r * nu);
+        p.seed = dalloc<unsigned>(s, r); p.wsum = dalloc<double>(s, r); p.sel = dalloc<int>(s, r); p.status = dalloc<int>(s, r); }))
+    return rc;
+  if (int rc = grow(s, who, s->plan_h_scope, s->plan_h_cap, (size_t)L * n_iter, 16, "cost record", "L n_iter", [&](size_t r) { p.hist = dalloc<double>(s, 2 * r); }))
+    return rc;
+  if (copy_async(s, p.mean, mean, 4 * lt * nu) != 0 || copy_async(s, (void*)p.xref, xref, 4 * l1 * nr) != 0 ||
+      (uref && copy_async(s, (void*)p.uref, uref, 4 * lt * nu) != 0) || copy_async(s, (void*)p.seed, seeds, 4 * (size_t)L) != 0) return -2;
+  DevPlan q = p;
+  q.L = L; q.T = T; q.n_iter = n_iter;
+  if (!uref) q.uref = nullptr;
+  DevRoll& r = s->plan_roll;
+  r = DevRoll{};
+  r.n = (int)n; r.T = T; r.nsub = n_substeps; r.ctrl = p.ctrl;
+  const int* fan;                              // the fan-out list, uploaded once: no host copy inside the iterations
+  if (int rc = fan_out_ids(s, slots, L, K, &fan)) return rc;
+  for (int it = 0; it < n_iter; it++) {        // no host synchronisation inside the iterations
+    q.iter = it;
+    warp_launch(s, "plan_sample", (int)n, 0, PlanWarp<0>{s->m, s->d, q});
+    launch_state<true>(s, nullptr, fan, N);      // the state bank's fan-out (fd_fan_out with K columns)
+    launch_step1(s);                           // what the rows do not carry, as fb_rollout runs it
+    q.t = -1;
+    warp_launch(s, "plan_cost", (int)n, 0, PlanWarp<1>{s->m, s->d, q});
+    for (int t = 0; t < T; t++) {
+      r.t = q.t = t;
+      warp_launch(s, "rollout_input", N, 0, RollInput{s->m, s->d, r, nullptr});
+      step_run(s, n_substeps);                 // fb_step's launches (the step graph)
+      warp_launch(s, "plan_cost", (int)n, 0, PlanWarp<1>{s->m, s->d, q});
+    }
+    warp_launch(s, "plan_weights", L, 0, PlanWarp<2>{s->m, s->d, q});
+    warp_launch(s, "plan_update", L * ((T + PLAN_STEPS - 1) / PLAN_STEPS), 0, PlanWarp<3>{s->m, s->d, q});
+  }
+  if (launch_check(s, who) != 0) return -2;
+  p.L = L; p.T = T; p.n_iter = n_iter;
+  s->plan_done = L;
+  return sync_stream(s);                       // host inputs may be reused once the call returns
+}
+
+int fb_plan_read(FbHandle s, float* mean, double* cost, double* sample_cost, float* samples, int32_t* status, int is_device) {
+  if (!s) return -1;
+  if (s->plan_done < 1) { s->err = "fb_plan_read: no plan to read (fb_plan)"; return -1; }
+  const DevPlan& p = s->plan;
+  const size_t L = p.L, n = L * p.K, nu = s->m.nu;
+  return read_out(s, {{mean, p.mean, 0, 4 * L * p.T * nu, 1}, {cost, p.hist, 0, 16 * L * p.n_iter, 1}, {sample_cost, p.J, 0, 8 * n, 1},
+                      {samples, p.ctrl, 0, 4 * n * p.T * nu, 1}, {status, p.status, 0, 4 * L, 1}});
 }
 
 }  // extern "C"

@@ -27,9 +27,10 @@ MAXCON, MAXEFC = _ABI.defines['FB_MAXCON'], _ABI.defines['FB_MAXEFC']
 PARAMS = tuple(name[5:].lower() for name, _ in sorted(_ABI.enums['FbParam'].items(), key=lambda e: e[1]) if name != 'FB_NPARAMS')
 FD_ELEMENT, FD_SCALE = 0, 1           # kinds of a parameter direction (fb_fd_param_program)
 
-# the programs of fb_obs_program, fb_task_program, fb_eye_program and fb_ik_program
-FbObsProgram, FbTaskProgram, FbEyeProgram, FbIkProgram = (_ABI.structs[n] for n in ('FbObsProgram', 'FbTaskProgram', 'FbEyeProgram',
-                                                                                      'FbIkProgram'))
+# the programs of fb_obs_program, fb_task_program, fb_eye_program, fb_ik_program and fb_plan_program
+FbObsProgram, FbTaskProgram, FbEyeProgram, FbIkProgram, FbPlanProgram = (_ABI.structs[n] for n in ('FbObsProgram', 'FbTaskProgram',
+                                                                                                     'FbEyeProgram', 'FbIkProgram',
+                                                                                                     'FbPlanProgram'))
 
 
 def load_library(path=None):
@@ -494,14 +495,17 @@ class BatchedStepper:
         self._roll = (n, T)
 
     def _outputs(self, out, shapes, dtypes):
-        """caller-provided outputs (numpy arrays or torch tensors, C-contiguous, of the given shapes and dtypes) or new numpy arrays ->
-        (arrays, pointers, is_device: a CUDA tensor among them)"""
+        """caller-provided outputs (numpy arrays or torch tensors, C-contiguous, of the given shapes and dtypes; None: not read) or new
+        numpy arrays -> (arrays, pointers, is_device: a CUDA tensor among them)"""
         if out is None:
             out = [np.zeros(sh, dt) for sh, dt in zip(shapes, dtypes)]
         if len(out) != len(shapes):
             raise ValueError(f'{len(out)} outputs against {len(shapes)}')
         ptrs, dev = [], False
         for x, sh, dt in zip(out, shapes, dtypes):
+            if x is None:                                            # an output the caller skips (the ABI's NULL)
+                ptrs.append(None)
+                continue
             if isinstance(x, np.ndarray):
                 ok = x.dtype == dt and x.flags.c_contiguous
                 ptrs.append(x.ctypes.data)
@@ -551,6 +555,57 @@ class BatchedStepper:
         m, (L, T) = self.model, getattr(self, '_lqr', (0, 0))
         out = [np.zeros((L, T, m.nu, 2 * m.nv + m.na)), np.zeros((L, T, m.nu)), np.zeros((L, 2)), np.zeros(L, np.int32)]
         self._check(self._lib.fb_lqr_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_lqr_read')
+        return tuple(out)
+
+    # ---- sampling-based MPC (fb_plan*; flybody_b200.trajopt.sample_plan / mpc are the front ends)
+    def plan_program(self, n_samples=0, sigma=None, Q=None, R=None, Qf=None, temperature=0.0, hold=1):
+        """the program of the plans that follow: n_samples samples per problem, noise scale sigma [nu], diagonal weights Q [nx], R [nu],
+        Qf [nx] (Q when None), temperature (> 0: MPPI, 0: predictive sampling) and hold control steps per noise knot; n_samples = 0
+        clears it (see the header)"""
+        m = self.model
+        if not n_samples:
+            self._check(self._lib.fb_plan_program(self._h, None), 'fb_plan_program')
+            return
+        nx = 2 * m.nv + m.na
+        Qf = Q if Qf is None else Qf
+        keep = [np.ascontiguousarray(np.broadcast_to(np.asarray(x, dt), (n,))) for x, dt, n in
+                ((sigma, np.float32, m.nu), (Q, np.float64, nx), (R, np.float64, m.nu), (Qf, np.float64, nx))]
+        f64 = C.POINTER(C.c_double)
+        prog = FbPlanProgram(n_samples=int(n_samples), hold=int(hold), temperature=float(temperature),
+                           sigma=keep[0].ctypes.data_as(C.POINTER(C.c_float)), Q=keep[1].ctypes.data_as(f64),
+                           R=keep[2].ctypes.data_as(f64), Qf=keep[3].ctypes.data_as(f64))
+        self._check(self._lib.fb_plan_program(self._h, C.byref(prog)), 'fb_plan_program')
+        self._plan_k = int(n_samples)
+
+    def plan(self, slots, mean, x_ref, seeds, u_ref=None, n_substeps=1, n_iter=1, T=None, is_device=False):
+        """n_iter iterations of the program's planner for L problems: problem l from bank row slots[l] with seed seeds[l] (host ints),
+        mean [L, T, nu], x_ref [L, T + 1, nq + nv + na], u_ref [L, T, nu] (None: 0) (host arrays, or device pointers / CUDA tensors'
+        data_ptr() with is_device=True and T given).  The envs' states are a workspace afterwards.  Read the results with plan_read()."""
+        m = self.model
+        s = np.ascontiguousarray(np.asarray(slots).reshape(-1), np.int32)
+        L = len(s)
+        sd = np.ascontiguousarray(np.asarray(seeds, np.int64).reshape(-1) & 0xffffffff, np.uint32)
+        if len(sd) != L:
+            raise ValueError(f'{len(sd)} seeds for {L} problems')
+        T = int(T if is_device else np.shape(mean)[1])
+        ptrs, _keep = self._inputs([('mean', mean, (L, T, m.nu)), ('x_ref', x_ref, (L, T + 1, m.nq + m.nv + m.na)),
+                                    ('u_ref', u_ref, (L, T, m.nu))], is_device)
+        self._check(self._lib.fb_plan(self._h, s.ctypes.data, L, T, int(n_substeps), int(n_iter), sd.ctypes.data, *ptrs,
+                                      int(bool(is_device))), 'fb_plan')
+        self._plan = (L, T, int(n_iter), getattr(self, '_plan_k', 0))
+
+    def plan_read(self, out=None, samples=True):
+        """-> (mean [L, T, nu] f32, cost [L, n_iter, 2] f64 (the nominal's and the best cost of each iteration), sample_cost [L, K] f64
+        and samples [L, K, T, nu] f32 of the last iteration, status [L] i32) of the last plan; samples=False leaves sample_cost and
+        samples on the device (None); out: the five arrays to fill instead (numpy arrays, or torch tensors, CUDA ones by device pointer;
+        None: not read)"""
+        m, (L, T, n_iter, K) = self.model, getattr(self, '_plan', (0, 0, 0, 0))
+        shapes = [(L, T, m.nu), (L, n_iter, 2), (L, K), (L, K, T, m.nu), (L,)]
+        dtypes = [np.float32, np.float64, np.float64, np.float32, np.int32]
+        if out is None and not samples:
+            out = [np.zeros(sh, dt) if i in (0, 1, 4) else None for i, (sh, dt) in enumerate(zip(shapes, dtypes))]
+        out, ptrs, dev = self._outputs(out, shapes, dtypes)
+        self._check(self._lib.fb_plan_read(self._h, *ptrs, int(dev)), 'fb_plan_read')
         return tuple(out)
 
     def reset(self, qpos=None, qvel=None, env_ids=None):

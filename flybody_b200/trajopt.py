@@ -7,6 +7,9 @@ L x len(alphas) line-search rollouts, rollout (l, alpha) applying problem l's la
 ctrl = u_t + alpha k_t + K_t (x_t - xbar_t).  The returned gains K are a TVLQR law around the returned trajectory that
 `rollout.rollout` applies as it is.  `lqr_backward` is the backward pass alone, e.g. for a TVLQR stabiliser (q = r = 0).
 
+`sample_plan` is sampling-based trajectory optimisation on the same cost, MPPI or predictive sampling, with every iteration (noise,
+rollouts, cost and update) on the device in one `fb_plan` call; `mpc` runs it in a receding-horizon loop for L plants.
+
 The cost is sum_t |x_t - xref_t|^2_Q / 2 + |u_t - uref_t|^2_R / 2 + |x_T - xref_T|^2_Qf / 2 with diagonal weights, the state difference
 in transition_fd's tangent (mj_differentiatePos for qpos), evaluated in fp64 on the host.  The nominal ctrl is the recorded ctrl clamped
 to actuator_ctrlrange where the actuator is ctrl-limited (what the step applied), so an open-loop `rollout.rollout` of the returned ctrl
@@ -281,3 +284,140 @@ def ilqr(model, qpos, qvel, ctrl, x_ref, Q, R, Qf=None, act=None, u_ref=None, n_
         sim.close()
     n = int(iters.max()) + 1
     return ILQR(xbar[..., :nq], xbar[..., nq:nq + nv], xbar[..., nq + nv:], ubar, K, hist[:, :n], iters, converged)
+
+
+SamplePlan = namedtuple('SamplePlan', ['qpos', 'qvel', 'act', 'ctrl', 'cost', 'status'])
+MPC = namedtuple('MPC', ['qpos', 'qvel', 'act', 'ctrl', 'cost', 'status'])
+
+
+def _plan_inputs(m, qpos, qvel, act, x_ref, u_ref, Q, R, Qf, L, T, sigma, temperature, n_samples, hold, n_iter, n_substeps):
+    """the checked inputs of sample_plan / mpc: x0 [L, nr], x_ref [L, T', nr], u_ref [L, T' - 1, nu], Q, R, Qf, sigma [nu]"""
+    nq, nv, na, nu = m.nq, m.nv, m.na, m.nu
+    nx, nr = 2 * nv + na, nq + nv + na
+    q0, v0 = _check('qpos', qpos, (L, nq)), _check('qvel', qvel, (L, nv))
+    a0 = _check('act', np.zeros((L, na)) if act is None else act, (L, na))
+    x_ref = _check('x_ref', x_ref, (L, T + 1, nr))
+    u_ref = _check('u_ref', np.zeros((L, T, nu)) if u_ref is None else u_ref, (L, T, nu))
+    Q, R = _check('Q', Q, (nx,), True), _check('R', R, (nu,), True)
+    Qf = Q if Qf is None else _check('Qf', Qf, (nx,), True)
+    sigma = _check('sigma', np.broadcast_to(np.asarray(sigma, np.float64), (nu,)), (nu,), True)
+    if not (np.isfinite(temperature) and temperature >= 0):
+        raise ValueError('temperature must be >= 0 and finite')
+    if n_samples < 2 or hold < 1 or n_iter < 1 or n_substeps < 1:
+        raise ValueError('n_samples >= 2, hold >= 1, n_iter >= 1 and n_substeps >= 1')
+    return np.concatenate([q0, v0, a0], -1), x_ref, u_ref, Q, R, Qf, sigma
+
+
+def _seeds(seed, L):
+    """one seed per problem: seed + l for a scalar, else the given [L]"""
+    s = np.asarray(seed, np.int64)
+    return (s + np.arange(L)) if s.ndim == 0 else s.reshape(L)
+
+
+def sample_plan(model, qpos, qvel, ctrl0, x_ref, Q, R, Qf=None, act=None, u_ref=None, n_samples=256, sigma=0.1, temperature=0.0,
+                hold=1, n_iter=10, n_substeps=1, seed=0, device=0, lib_path=None):
+    """Sampling-based trajectory optimisation of L tracking problems on the device (`fb_plan`): initial states qpos [L, nq], qvel [L, nv],
+    act [L, na] (zeros when None), the initial nominal controls ctrl0 [L, T, nu], reference states x_ref [L, T + 1, nq + nv + na] and
+    controls u_ref [L, T, nu] (zeros when None), diagonal weights Q [nx], R [nu], Qf [nx] (Q when None) of `cost`.  Each of n_iter
+    iterations rolls out n_samples samples per problem, mean + sigma (scalar or [nu]) times standard normal noise held over `hold`
+    control steps (sample 0 the mean itself), clamped to the ctrl range of ctrl-limited actuators, and moves the mean: temperature > 0,
+    MPPI's exp(-(J - J_min) / temperature)-weighted average; temperature = 0, predictive sampling's lowest-cost sample.  seed: a scalar
+    (problem l takes seed + l) or [L] seeds; a problem's result depends on its seed and inputs alone.  Problems run 4096 // n_samples at
+    a time on one handle, each from a cold warm start (its state written and `forward` run), as `ilqr`'s.
+
+    Returns SamplePlan(qpos, qvel, act [L, T + 1, .], ctrl [L, T, nu], cost [L, n_iter, 2], status [L]): the final mean and its
+    trajectory from one rollout on the device (bit for bit what `rollout.rollout` gives for it), each iteration's nominal (the mean's
+    clamped sequence, before that iteration's update) and best cost, and per problem 0 or 1 + the first iteration whose samples all
+    scored +inf (a bad state: the mean was kept)."""
+    m = model
+    nq, nv, nu = m.nq, m.nv, m.nu
+    u0 = np.asarray(ctrl0, np.float64)
+    if u0.ndim != 3 or u0.shape[2] != nu or u0.shape[1] < 1:
+        raise ValueError(f'ctrl0 {u0.shape} against [L, T, {nu}]')
+    L, T = u0.shape[:2]
+    u0 = _check('ctrl0', u0, (L, T, nu))
+    x0, x_ref, u_ref, Q, R, Qf, sigma = _plan_inputs(m, qpos, qvel, act, x_ref, u_ref, Q, R, Qf, L, T, sigma, temperature, n_samples,
+                                                     hold, n_iter, n_substeps)
+    seeds = _seeds(seed, L)
+    per = max(1, ENVS // n_samples)
+    sim = st.BatchedStepper(m, min(L, per) * n_samples, device=device, lib_path=lib_path)
+    means, costs, status, xs = [], [], [], []
+    try:
+        sim.state_bank(min(L, per))
+        sim.plan_program(n_samples, sigma, Q, R, Qf, temperature, hold)
+        for c0 in range(0, L, per):
+            k, sl = min(per, L - c0), slice(c0, c0 + min(per, L - c0))
+            _write_rows(sim, m, 0, x0[sl].astype(np.float32), u0[sl, 0].astype(np.float32))
+            sim.plan(np.arange(k), u0[sl], x_ref[sl], seeds[sl], u_ref[sl], n_substeps, n_iter)
+            mean, cost_k, _, _, status_k = sim.plan_read(samples=False)
+            x_held = _write_rows(sim, m, 0, x0[sl].astype(np.float32), mean[:, 0])      # rollout.rollout's rows for the mean
+            sim.rollout(np.arange(k), mean, n_substeps)
+            q, v, a = sim.rollout_read()[:3]
+            xs.append(np.concatenate([x_held[:, None], np.concatenate([q, v, a], -1)], 1))
+            means.append(mean)
+            costs.append(cost_k)
+            status.append(status_k)
+    finally:
+        sim.close()
+    x = np.concatenate(xs).astype(np.float64)
+    return SamplePlan(x[..., :nq], x[..., nq:nq + nv], x[..., nq + nv:], np.concatenate(means).astype(np.float64), np.concatenate(costs),
+                      np.concatenate(status))
+
+
+def mpc(model, qpos, qvel, x_ref, n_steps, horizon, Q, R, Qf=None, act=None, u_ref=None, ctrl0=None, n_samples=256, sigma=0.1,
+        temperature=0.0, hold=1, n_iter=1, n_substeps=1, seed=0, device=0, lib_path=None):
+    """Receding-horizon sampling MPC of L plants: initial states qpos [L, nq], qvel [L, nv], act [L, na] (zeros when None), reference
+    states x_ref [L, n_steps + horizon, nq + nv + na] and controls u_ref [L, n_steps + horizon - 1, nu] (zeros when None), the
+    planner's arguments as `sample_plan`'s, ctrl0 [L, horizon, nu] the first warm start (zeros when None).  At control step s each plant
+    plans n_iter iterations from its state against x_ref[:, s : s + horizon + 1], warm-started from the previous plan shifted by one step
+    (its last step repeated), applies the plan's first control for one control step (a T = 1 rollout from the plant's state row) and
+    saves the env back into that row, so the solver warm start carries over as in one continuous rollout.  The plant's first row is
+    written with the first applied control (as `rollout.rollout` writes it), so the plant trajectory is bit for bit `rollout.rollout`
+    of the applied controls.  The plan of step s uses problem seeds of (seed, plant, s).  Plants run 4096 // n_samples at a time.
+
+    Returns MPC(qpos, qvel, act [L, n_steps + 1, .], ctrl [L, n_steps, nu], cost [L, n_steps, n_iter, 2], status [L, n_steps]): the
+    plant trajectory, the applied controls, and each step's plan record (nominal and best cost per iteration, status)."""
+    m = model
+    nq, nv, nu = m.nq, m.nv, m.nu
+    L = np.shape(qpos)[0]
+    H, S = int(horizon), int(n_steps)
+    if H < 1 or S < 1:
+        raise ValueError('horizon >= 1 and n_steps >= 1')
+    x0, x_ref, u_ref, Q, R, Qf, sigma = _plan_inputs(m, qpos, qvel, act, x_ref, u_ref, Q, R, Qf, L, S + H - 1, sigma, temperature,
+                                                     n_samples, hold, n_iter, n_substeps)
+    u0 = _check('ctrl0', np.zeros((L, H, nu)) if ctrl0 is None else ctrl0, (L, H, nu)).astype(np.float32)
+    seeds = _seeds(seed, L)
+    per = max(1, ENVS // n_samples)
+    sim = st.BatchedStepper(m, min(L, per) * n_samples, device=device, lib_path=lib_path)
+    xs, us, costs, stats = [], [], [], []
+    try:
+        sim.state_bank(min(L, per))
+        sim.plan_program(n_samples, sigma, Q, R, Qf, temperature, hold)
+        for c0 in range(0, L, per):
+            k, sl = min(per, L - c0), slice(c0, c0 + min(per, L - c0))
+            rows = np.arange(k)
+            mean = u0[sl]
+            _write_rows(sim, m, 0, x0[sl].astype(np.float32), mean[:, 0])
+            x, u, cost, status = [], [], [], []
+            for s in range(S):
+                sim.plan(rows, mean, x_ref[sl, s:s + H + 1], (seeds[sl] * 1000003 + s) & 0xffffffff, u_ref[sl, s:s + H], n_substeps, n_iter)
+                mean, cost_s, _, _, status_s = sim.plan_read(samples=False)
+                if s == 0:
+                    x.append(_write_rows(sim, m, 0, x0[sl].astype(np.float32), mean[:, 0]))
+                sim.rollout(rows, mean[:, :1], n_substeps)
+                q, v, a, uc = sim.rollout_read()[:4]
+                sim.save_state(slots=rows, env_ids=rows)
+                x.append(np.concatenate([q[:, 0], v[:, 0], a[:, 0]], -1))
+                u.append(uc[:, 0])
+                cost.append(cost_s)
+                status.append(status_s)
+                mean = np.concatenate([mean[:, 1:], mean[:, -1:]], 1)
+            xs.append(np.stack(x, 1))
+            us.append(np.stack(u, 1))
+            costs.append(np.stack(cost, 1))
+            stats.append(np.stack(status, 1))
+    finally:
+        sim.close()
+    x = np.concatenate(xs).astype(np.float64)
+    return MPC(x[..., :nq], x[..., nq:nq + nv], x[..., nq + nv:], np.concatenate(us).astype(np.float64), np.concatenate(costs),
+               np.concatenate(stats))

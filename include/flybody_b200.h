@@ -722,6 +722,49 @@ int fb_rollout_sensor_read(FbHandle h, float* sensordata, float* sensor_mean, in
 int fb_lqr(FbHandle h, int L, int T, const float* A, const float* B, const double* q, const double* r, const double* Q, const double* R,
            const double* Qf, const double* mu, int is_device);
 int fb_lqr_read(FbHandle h, double* K, double* k, double* dV, int32_t* status, int is_device);
+/* Sampling-based MPC: MPPI (Williams et al. 2017, the information-theoretic update without the control cross term, R pricing the
+ * controls) and predictive sampling (Howell et al. 2022, MuJoCo MPC), batched over L tracking problems of K = n_samples samples each
+ * (nx = 2 nv + na, nr = nq + nv + na).  Problem l starts from state-bank row slots[l] with the nominal control sequence mean[l] [T][nu].
+ * One iteration:
+ *   sample:   sample k of problem l is u_k,t = clamp(mean_t + sigma * eps_k,floor(t / hold)), the clamp on ctrl-limited actuators only
+ *             (what the actuation stage applies), eps a standard normal (Box-Muller in fp64) of a counter hash of (seeds[l], iteration,
+ *             k, knot, actuator): the noise of a problem depends on its seed alone, never on its index or L.  Sample 0 has eps = 0
+ *             (the clamped mean).  hold >= 1 is the zero-order-hold knot spacing in control steps.
+ *   roll out: all L K samples open loop, T control steps of n_substeps substeps, sample (l, k) in env l K + k from row slots[l] (its
+ *             parameter overlay and applied forces included, as fb_rollout); envs past L K run copies of the last sample.  The step
+ *             kernels, the rollout input kernel and the step graph run as fb_rollout runs them.
+ *   score:    J_k = 1/2 sum_{t<T} (|x_t (-) xref_t|^2_Q + |u_k,t - uref_t|^2_R) + 1/2 |x_T (-) xref_T|^2_Qf, (-) fb_fd_transition's
+ *             tangent, summed in fp64 from the fp32 state, the lane partials in lane order.  A sample whose env sets the bad-state
+ *             flag (flag bit value 1: |qacc|^2 >= 1e28, or a non-finite qacc or qvel) scores +inf, and so does a NaN cost.
+ *   update:   temperature > 0 (MPPI): w_k = exp(-(J_k - J_min) / temperature) (+inf: 0), mean_t = sum_k w_k u_k,t / sum_k w_k in fp64,
+ *             stored fp32.  temperature = 0 (predictive sampling): mean = the lowest-cost sample, bit for bit (ties: the lowest k).
+ *             If every sample scores +inf the mean stays and status = 1 + the iteration (the first such).
+ * One warp per work unit (a sample, a problem, or a problem's block of steps), no atomics and no shared memory: every sum has a fixed
+ * order, so a problem's bits depend on neither its index, nor L, nor the other problems.
+ * fb_plan_program sets the program for the calls that follow: n_samples >= 2, hold >= 1, temperature >= 0 and finite, sigma [nu] (fp32),
+ * Q [nx], R [nu], Qf [nx] (fp64 diagonal weights) >= 0 and finite, read when the call is made.  NULL or n_samples = 0 clears it.  Errors
+ * also: a model without actuators.  It synchronises.
+ * fb_plan copies its inputs and the fan-out list once, then runs n_iter iterations with no host copy or synchronisation: inputs
+ * (host rows, or device pointers when is_device) mean [L][T][nu], xref [L][T + 1][nr] and uref [L][T][nu] (NULL: 0); slots [L] and
+ * seeds [L] are host arrays.  Its buffers are its own,
+ * allocated on first use and grown with L n_samples T, L (T + 1) and L n_iter; -4 with a message when they do not fit.  It does not
+ * touch fb_rollout_read's records, the feedback law or the bank; afterwards the envs are a workspace.  Errors: no bank, no program,
+ * L < 1 or L n_samples > n_envs, T < 1, n_substeps < 1, n_iter < 1, a NULL input, a slot out of range, never written or saved while
+ * its env was held for a reset, a non-finite host input.  It synchronises; a device input is not checked.
+ * fb_plan_read (synchronises; any pointer may be NULL; is_device: device pointers): mean [L][T][nu] after the last update, cost
+ * [L][n_iter][2] (per iteration: the nominal's cost, i.e. sample 0's, and the lowest cost), sample_cost [L][n_samples] and samples
+ * [L][n_samples][T][nu] of the last iteration, status [L] (int32); an error before any plan.                                        */
+typedef struct FbPlanProgram {
+  int32_t n_samples;                           /* K >= 2 samples per problem (0: clear)                                      */
+  int32_t hold;                                /* control steps per noise knot, >= 1                                           */
+  double temperature;                          /* > 0: MPPI; 0: predictive sampling                                           */
+  const float* sigma;                          /* [nu] noise scale per actuator                                               */
+  const double *Q, *R, *Qf;                    /* [nx], [nu], [nx] diagonal weights                                           */
+} FbPlanProgram;
+int fb_plan_program(FbHandle h, const FbPlanProgram* p);
+int fb_plan(FbHandle h, const int32_t* slots, int L, int T, int n_substeps, int n_iter, const uint32_t* seeds, const float* mean,
+            const float* xref, const float* uref, int is_device);
+int fb_plan_read(FbHandle h, float* mean, double* cost, double* sample_cost, float* samples, int32_t* status, int is_device);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
