@@ -33,6 +33,7 @@
 #include "fb_rollout.h"
 #include "fb_lqr.h"
 #include "fb_plan.h"
+#include "fb_sid.h"
 
 enum { K_ACT = 0, K_SMOOTH, K_REF, K_SOLVE, K_FINISH, K_POS, K_COL, K_CON, K_PROJ, K_VEL, K_SENS, K_PACK, K_MISC, K_NKIND };
 static const char* const kKindNames[K_NKIND] = {"act", "smooth", "ref", "solve", "finish", "pos", "col", "con", "proj", "vel", "sens", "pack", "misc"};
@@ -43,6 +44,7 @@ struct FdQuery {
   DevFdQ p = {};                          // the last call's kernel parameter; the blocks' and nominals' out are the query's outputs
   std::vector<void*> scope, sens_scope;   // the outputs and the sensor outputs, allocated on the first call (with sensors on)
   int done = 0; bool sens = false;        // problems of the last call; it ran with sensors on
+  long long at = 0;                       // fb_launch_count when the last call returned (fb_sid_accumulate reads its outputs and flags)
 };
 // the scratch the queries share, no read returns it; each part is allocated on the first call that needs it
 struct FdScratch {
@@ -95,6 +97,10 @@ struct FbSim {
   // record); the rollout parameter of the samples; problems of the last call
   DevPlan plan = {}; DevRoll plan_roll = {}; std::vector<void*> plan_prog_scope, plan_s_scope, plan_k_scope, plan_l_scope, plan_h_scope;
   size_t plan_s_cap = 0, plan_k_cap = 0, plan_l_cap = 0, plan_h_cap = 0; int plan_done = 0;
+  // system identification (fb_sid_accumulate / fb_sid_read; fb_sid.h): the transition scratch (grown with n), the sums of sid_L problems
+  // of sid_k directions (grown with L (k^2 + k + 1); sid_L = 0: none yet) and the per-problem words (grown with L + 1)
+  DevSid sid = {}; std::vector<void*> sid_t_scope, sid_s_scope, sid_l_scope; size_t sid_t_cap = 0, sid_s_cap = 0, sid_l_cap = 0;
+  int sid_L = 0, sid_k = 0;
   int device; long long launches; float last_ms; std::string err;
   int first_substep; int hold_pending;
   int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
@@ -2402,7 +2408,7 @@ static int fd_run(FbSim* s, FdQuery& q, const FdCall& c) {
   }
   warp_launch(s, "fd_diff", n * nin, 0, FdDiff{s->m, s->d, p});
   if (launch_check(s, q.name) != 0) return -2;
-  q.done = n; q.sens = sens;
+  q.done = n; q.sens = sens; q.at = s->launches;
   return q.inverse && c.is_device ? 0 : sync_stream(s);   // host rows may be reused once the call returns; the fan-out list is a host vector
 }
 // a read entry: the outputs (sens: the sensor outputs) in the entry's order, the blocks and then the nominal column's (the next state:
@@ -2864,6 +2870,96 @@ int fb_plan_read(FbHandle s, float* mean, double* cost, double* sample_cost, flo
   const size_t L = p.L, n = L * p.K, nu = s->m.nu;
   return read_out(s, {{mean, p.mean, 0, 4 * L * p.T * nu, 1}, {cost, p.hist, 0, 16 * L * p.n_iter, 1}, {sample_cost, p.J, 0, 8 * n, 1},
                       {samples, p.ctrl, 0, 4 * n * p.T * nu, 1}, {status, p.status, 0, 4 * L, 1}});
+}
+
+}  // extern "C"
+
+// -------------------------------------------------------------------------------------------
+// system identification (fb_sid_accumulate; fb_sid.h): its own kernel parameter (DevSid) and buffers, reading the outputs of the last
+// parameter-Jacobian query in place
+template <int KIND> struct SidWarp {
+  DevModel m; DevData d; DevSid p;
+  FB_DEVM void operator()(unsigned char*, int w) const { if (KIND == 0) ksid_resid(m, d, p, w); else ksid_sum(p, w); }
+};
+
+extern "C" {
+
+int fb_sid_accumulate(FbHandle s, int query, int L, const int32_t* problem, int n, const float* target, const double* weight,
+                      const float* sample_weight, int reset, int is_device) {
+  if (!s) return -1;
+  const char* who = "fb_sid_accumulate";
+  if (query != FB_SID_TRANSITION && query != FB_SID_INVERSE) { s->err = "fb_sid_accumulate: query is FB_SID_TRANSITION or FB_SID_INVERSE"; return -1; }
+  const bool inv = query == FB_SID_INVERSE;
+  const FdQuery& q = inv ? s->fd_pinv : s->fd_ptr;
+  if (q.done < 1) { s->err = std::string(who) + ": no parameter Jacobians to accumulate (" + q.name + ")"; return -1; }
+  if (s->launches != q.at) {
+    s->err = std::string(who) + ": the handle launched kernels since the last " + q.name + ", so its outputs and its nominal envs' flags are no longer that call's";
+    return -1; }
+  if (n != q.done) { s->err = std::string(who) + ": n = " + std::to_string(n) + " against the " + std::to_string(q.done) + " problems of the last " + q.name; return -1; }
+  const DevModel& m = s->m;
+  const int k = q.p.nin, rows = inv ? m.nv : 2 * m.nv + m.na, nr = inv ? m.nv : m.nq + m.nv + m.na;
+  if (L < 1) { s->err = "fb_sid_accumulate: L >= 1 fit problems"; return -1; }
+  if (!reset && (L != s->sid_L || k != s->sid_k)) {
+    s->err = s->sid_L < 1 ? std::string(who) + ": no sums to add to (reset = 1 starts them)" :
+             std::string(who) + ": without reset, L and k must be the sums' (L = " + std::to_string(s->sid_L) + ", k = " + std::to_string(s->sid_k) + ")";
+    return -1; }
+  if (!problem || !weight) { s->err = "fb_sid_accumulate: problem and weight must not be NULL"; return -1; }
+  if (!inv && !target) { s->err = "fb_sid_accumulate: a transition residual needs its target x'_obs"; return -1; }
+  std::vector<int> ptr(L + 1, 0), order;
+  for (int i = 0; i < n; i++) {
+    if (problem[i] < -1 || problem[i] >= L) {
+      s->err = std::string(who) + ": problem[" + std::to_string(i) + "] = " + std::to_string(problem[i]) + " is not in [-1, L)"; return -1; }
+    if (problem[i] >= 0) ptr[problem[i] + 1]++;
+  }
+  for (int l = 0; l < L; l++) ptr[l + 1] += ptr[l];
+  order.resize(ptr[L]);
+  { std::vector<int> at(ptr.begin(), ptr.end() - 1); for (int i = 0; i < n; i++) if (problem[i] >= 0) order[at[problem[i]]++] = i; }
+  for (int c = 0; c < rows; c++)
+    if (!(weight[c] >= 0.0) || !std::isfinite(weight[c])) { s->err = "fb_sid_accumulate: the weights must be >= 0 and finite"; return -1; }
+  if (!is_device) {
+    if (sample_weight) for (int i = 0; i < n; i++)
+      if (!(sample_weight[i] >= 0.0f) || !std::isfinite(sample_weight[i])) { s->err = "fb_sid_accumulate: the sample weights must be >= 0 and finite"; return -1; }
+    if (target && !all_finite(target, (size_t)n * nr)) { s->err = "fb_sid_accumulate: non-finite target"; return -1; }
+  }
+  dev_select(s);
+  DevSid& p = s->sid;
+  if (reset) s->sid_L = 0;                     // (growing the sums drops them)
+  if (int rc = grow(s, who, s->sid_t_scope, s->sid_t_cap, (size_t)n, 8 * (size_t)(2 * m.nv + m.na + 1) + 4 * (size_t)(m.nq + m.nv + m.na + 3),
+                    "transition scratch", "n", [&](size_t r) {
+        p.res = dalloc<double>(s, r * (2 * m.nv + m.na)); p.tcost = dalloc<double>(s, r); p.tbad = dalloc<int>(s, r);
+        p.target = dalloc<float>(s, r * (m.nq + m.nv + m.na)); p.sw = dalloc<float>(s, r); p.order = dalloc<int>(s, r);
+        p.W = dalloc<double>(s, 2 * m.nv + m.na); }))
+    return rc;
+  const size_t E = (size_t)k * k + k + 1;
+  if (int rc = grow(s, who, s->sid_s_scope, s->sid_s_cap, (size_t)L * E, 8, "sums", "L (k^2 + k + 1)", [&](size_t r) { p.H = dalloc<double>(s, r); }))
+    return rc;
+  if (int rc = grow(s, who, s->sid_l_scope, s->sid_l_cap, (size_t)L + 1, 12, "per-problem words", "L + 1", [&](size_t r) {
+        p.count = dalloc<int>(s, r); p.bad = dalloc<int>(s, r); p.ptr = dalloc<int>(s, r); }))
+    return rc;
+  if (copy_async(s, (void*)p.order, order.data(), 4 * order.size()) != 0 || copy_async(s, (void*)p.ptr, ptr.data(), 4 * (size_t)(L + 1)) != 0 ||
+      copy_async(s, (void*)p.W, weight, 8 * (size_t)rows) != 0 || (target && copy_async(s, (void*)p.target, target, 4 * (size_t)n * nr) != 0) ||
+      (sample_weight && copy_async(s, (void*)p.sw, sample_weight, 4 * (size_t)n) != 0)) return -2;
+  DevSid c = p;
+  c.L = L; c.k = k; c.rows = rows; c.nr = nr; c.ncol = q.p.ncol; c.inverse = inv; c.reset = reset != 0;
+  c.J = q.p.blk[0].out; c.pred = q.p.nom[0].out;
+  if (!target) c.target = nullptr;
+  if (!sample_weight) c.sw = nullptr;
+  c.g = p.H + (size_t)L * k * k; c.cost = c.g + (size_t)L * k;      // the sums' layout: H, g, cost
+  if (ptr[L] > 0) warp_launch(s, "sid_resid", ptr[L], 0, SidWarp<0>{s->m, s->d, c});
+  warp_launch(s, "sid_sum", L * (k * (k + 1) / 2 + k + 1), 0, SidWarp<1>{s->m, s->d, c});
+  if (launch_check(s, who) != 0) return -2;
+  s->sid_L = L; s->sid_k = k;
+  return sync_stream(s);                       // host inputs may be reused once the call returns
+}
+
+int fb_sid_read(FbHandle s, double* H, double* g, double* cost, int32_t* count, int32_t* bad, int is_device) {
+  if (!s) return -1;
+  if (s->sid_L < 1) { s->err = "fb_sid_read: no sums to read (fb_sid_accumulate)"; return -1; }
+  const DevSid& p = s->sid;
+  const size_t L = s->sid_L, k = s->sid_k;
+  const double *pg = p.H + L * k * k, *pc = pg + L * k;      // (the sums' layout: H, g, cost)
+  return read_out(s, {{H, p.H, 0, 8 * L * k * k, 1}, {g, pg, 0, 8 * L * k, 1}, {cost, pc, 0, 8 * L, 1}, {count, p.count, 0, 4 * L, 1},
+                      {bad, p.bad, 0, 4 * L, 1}});
 }
 
 }  // extern "C"

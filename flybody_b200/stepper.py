@@ -18,9 +18,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libflybody_b200.so')
 
 _ABI = abi.read()
-# enum FbField (fb_get / fb_set fields: QPOS .. XFRC_APPLIED), enum FbObsItem (OBS_*) and enum FbTaskKind (TASK_*, FbTaskProgram.kind),
-# by their header names without FB_
-globals().update({name[3:]: v for enum in ('FbField', 'FbObsItem', 'FbTaskKind') for name, v in _ABI.enums[enum].items()})
+# enum FbField (fb_get / fb_set fields: QPOS .. XFRC_APPLIED), enum FbObsItem (OBS_*), enum FbTaskKind (TASK_*, FbTaskProgram.kind)
+# and enum FbSidQuery (SID_TRANSITION, SID_INVERSE), by their header names without FB_
+globals().update({name[3:]: v for enum in ('FbField', 'FbObsItem', 'FbTaskKind', 'FbSidQuery') for name, v in _ABI.enums[enum].items()})
 MAXCON, MAXEFC = _ABI.defines['FB_MAXCON'], _ABI.defines['FB_MAXEFC']
 
 # enum FbParam: the per-env model parameters (fb_param_*), by their mjModel names, in id order
@@ -606,6 +606,32 @@ class BatchedStepper:
             out = [np.zeros(sh, dt) if i in (0, 1, 4) else None for i, (sh, dt) in enumerate(zip(shapes, dtypes))]
         out, ptrs, dev = self._outputs(out, shapes, dtypes)
         self._check(self._lib.fb_plan_read(self._h, *ptrs, int(dev)), 'fb_plan_read')
+        return tuple(out)
+
+    # ---- system identification (fb_sid_*; flybody_b200.sysid is the front end)
+    def sid_accumulate(self, query, L, problem, weight, target=None, sample_weight=None, reset=True, is_device=False):
+        """add the weighted normal equations of the last fd_param_transition (query SID_TRANSITION; target: x'_obs [n, nq + nv + na],
+        weight [nx]) or fd_param_inverse (SID_INVERSE; target: the qfrc_inverse target [n, nv], None: 0; weight [nv]) to L fit problems:
+        FD problem i goes to fit problem problem[i] (host ints, -1: skipped), with sample_weight [n] (None: 1).  target and sample_weight
+        are host arrays, or device pointers / CUDA tensors' data_ptr() with is_device=True; weight is a host array (fp64).  reset starts
+        the L problems' sums from 0, else the call adds to them (see the header).  Read the sums with sid_read()."""
+        m = self.model
+        inv = query == SID_INVERSE
+        pb = np.ascontiguousarray(np.asarray(problem).reshape(-1), np.int32)
+        n = len(pb)
+        rows, nr = (m.nv, m.nv) if inv else (2 * m.nv + m.na, m.nq + m.nv + m.na)
+        w = np.ascontiguousarray(np.broadcast_to(np.asarray(weight, np.float64), (rows,)))
+        ptrs, _keep = self._inputs([('target', target, (n, nr)), ('sample_weight', sample_weight, (n,))], is_device)
+        self._check(self._lib.fb_sid_accumulate(self._h, int(query), int(L), pb.ctypes.data, n, ptrs[0], w.ctypes.data, ptrs[1],
+                                                int(bool(reset)), int(bool(is_device))), 'fb_sid_accumulate')
+        self._sid = (int(L), (getattr(self, '_fdpi_n', (0, 0)) if inv else getattr(self, '_fdp_n', (0, 0)))[1])
+
+    def sid_read(self, out=None):
+        """-> (H [L, k, k], g [L, k], cost [L] f64, count [L], bad [L] i32) of the sums; out: the five arrays to fill instead (numpy
+        arrays, or torch tensors, CUDA ones by device pointer; None: not read)"""
+        L, k = getattr(self, '_sid', (0, 0))
+        out, ptrs, dev = self._outputs(out, [(L, k, k), (L, k), (L,), (L,), (L,)], [np.float64] * 3 + [np.int32] * 2)
+        self._check(self._lib.fb_sid_read(self._h, *ptrs, int(dev)), 'fb_sid_read')
         return tuple(out)
 
     def reset(self, qpos=None, qvel=None, env_ids=None):

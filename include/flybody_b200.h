@@ -765,6 +765,32 @@ int fb_plan_program(FbHandle h, const FbPlanProgram* p);
 int fb_plan(FbHandle h, const int32_t* slots, int L, int T, int n_substeps, int n_iter, const uint32_t* seeds, const float* mean,
             const float* xref, const float* uref, int is_device);
 int fb_plan_read(FbHandle h, float* mean, double* cost, double* sample_cost, float* samples, int32_t* status, int is_device);
+/* ---- system identification: the normal equations of parameter fits (fb_sid.h; flybody_b200.sysid is the front end) -------------
+ * fb_sid_accumulate adds the weighted normal equations of L fit problems from the outputs the last parameter-Jacobian query left on the
+ * device; nothing of the Jacobians is read back.  query FB_SID_TRANSITION reads the last fb_fd_param_transition: FD problem i's residual
+ * r = x'_pred (-) x'_obs [nx], x'_pred the nominal next state (fb_fd_param_read's), (-) fb_fd_transition's tangent
+ * (mj_differentiatePos(x'_obs qpos, x'_pred qpos), then the qvel and act differences), J = dxdp [nx][k].  FB_SID_INVERSE reads the last
+ * fb_fd_param_inverse: r = qfrc_inverse - target [nv], J = DfDp^T.  Per fit problem l, over the FD problems i with problem[i] = l, in
+ * fp64 from the fp32 outputs:
+ *   H_l += c_i J^T W J,  g_l += c_i J^T W r,  cost_l += c_i r^T W r / 2,  count_l += 1
+ * W = diag(weight), c_i = sample_weight[i]; a transition with c_i = 0 adds nothing (as problem[i] = -1).  A transition whose residual or
+ * Jacobian is not finite, or (transition) whose nominal env set the bad-state flag (bit value 1), adds +inf to cost_l and 1 to bad_l and
+ * nothing to H_l or g_l.  No atomics: each transition's term is one fixed-order sum, added in transition order, so a problem's bits
+ * depend on neither its index, nor L, nor the other problems, nor on how its transitions are split across calls.
+ * Inputs: problem [n] (host int32, a fit problem in [0, L) or -1: skip), target (x'_obs [n][nq + nv + na] of a transition, the qfrc target
+ * [n][nv] of an inverse, NULL: 0), sample_weight [n] (fp32 >= 0, NULL: 1), target and sample_weight host rows or device pointers when
+ * is_device; weight [nx] or [nv] (host fp64 >= 0 and finite).  reset = 1 starts the L problems' sums from 0; reset = 0 adds to them.
+ * Its buffers are its own, allocated on first use and grown with n, L (k^2 + k + 1) and L; -4 with a message when they do not fit.
+ * Errors: an unknown query, no result of that query, any kernel launched on the handle since it (fb_launch_count: the outputs and the
+ * nominal envs' flags must be the query's own), n other than the query's, L < 1, L or k other than the sums' without reset (or no sums),
+ * a problem id out of range, a NULL problem or weight, a NULL transition target, negative or non-finite host weights, a non-finite host
+ * target.  It synchronises; a device input is not checked.
+ * fb_sid_read (synchronises; any pointer may be NULL; is_device: device pointers): H [L][k][k] (symmetric), g [L][k], cost [L], count
+ * [L] and bad [L] (int32) of the sums; an error before any fb_sid_accumulate.                                                         */
+enum FbSidQuery { FB_SID_TRANSITION = 0, FB_SID_INVERSE = 1 };
+int fb_sid_accumulate(FbHandle h, int query, int L, const int32_t* problem, int n, const float* target, const double* weight,
+                      const float* sample_weight, int reset, int is_device);
+int fb_sid_read(FbHandle h, double* H, double* g, double* cost, int32_t* count, int32_t* bad, int is_device);
 int fb_n_envs(FbHandle h);
 int fb_n_envs_padded(FbHandle h);
 void* fb_stream(FbHandle h);                 /* cudaStream_t the handle launches on */
