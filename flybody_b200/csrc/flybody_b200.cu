@@ -53,6 +53,9 @@ struct FdScratch {
   float* rows;                            // [N/2][prm_stride] the parameter inverse's overlay rows
   float* sens;                            // [Np][nsd] every env's sensors (of x for a transition, kinv_sensors' for an inverse)
 };
+struct Pool { std::vector<void*> bufs; size_t cap = 0; };   // buffers for `cap` rows, replaced as a whole when a call needs more (grow)
+// Every device buffer allocated after fb_create belongs to one scope (a list of buffers, or a Pool's): it is freed after a stream sync
+// when its scope is replaced or grown, and by fb_destroy.
 struct FbSim {
   DevModel m; DevData d;
   int prof_on; double prof_ms[K_NKIND]; long long prof_n[K_NKIND];
@@ -81,44 +84,43 @@ struct FbSim {
   FdQuery fd_pinv{"fb_fd_param_inverse", "fb_fd_param_columns", "parameter Jacobians", true, true};
   FdScratch fdx = {};
   DevFdPrmProg fdp_prog = {}; std::vector<void*> fdp_prog_scope; int fdp_k = 0; bool fdp_scale = false;
-  // rollouts (fb_rollout*; fb_rollout.h): inputs and records of roll_cap rows (n T), grown on demand in three groups (ctrl and the
-  // records; applied-force inputs; sensor records); the feedback bank of roll_fb_L laws of roll_fb_T steps (fb_rollout_feedback_bank)
-  // in buffers of roll_fb_cap law steps (L T), and its law list of roll_fb_n rollouts (0: every rollout takes law 0); rows of the last call
-  DevRoll roll = {}; std::vector<void*> roll_scope, roll_app_scope, roll_sd_scope; size_t roll_cap = 0, roll_app_cap = 0, roll_sd_cap = 0;
-  float *roll_xref = nullptr, *roll_K = nullptr; int* roll_law = nullptr; std::vector<void*> roll_fb_scope, roll_law_scope;
-  size_t roll_fb_cap = 0, roll_law_cap = 0; int roll_fb_T = 0, roll_fb_L = 0, roll_fb_n = 0;
+  // rollouts (fb_rollout*; fb_rollout.h): inputs and records of n T rows, grown on demand in three pools (ctrl and the records;
+  // applied-force inputs; sensor records); the feedback bank of roll_fb_L laws of roll_fb_T steps (fb_rollout_feedback_bank) in a pool
+  // of L T law steps, and its law list of roll_fb_n rollouts (0: every rollout takes law 0); rows of the last call
+  DevRoll roll = {}; Pool roll_pool, roll_app_pool, roll_sd_pool;
+  float *roll_xref = nullptr, *roll_K = nullptr; int* roll_law = nullptr; Pool roll_fb_pool, roll_law_pool; int roll_fb_T = 0, roll_fb_L = 0, roll_fb_n = 0;
   float *roll_qf = nullptr, *roll_xf = nullptr, *roll_sd = nullptr, *roll_sm = nullptr;   // applied-force inputs, sensor records
   int roll_done = 0; bool roll_sens = false;
-  // the iLQR backward pass (fb_lqr; fb_lqr.h): inputs and outputs of lqr_cap problem steps (L (T + 1)) and the workspace of lqr_ws_cap
-  // problems, grown on demand; problems and steps of the last call
-  DevLqr lqr = {}; std::vector<void*> lqr_scope, lqr_ws_scope; size_t lqr_cap = 0, lqr_ws_cap = 0; int lqr_done = 0;
+  // the iLQR backward pass (fb_lqr; fb_lqr.h): inputs and outputs of L (T + 1) problem steps and the workspace of L problems, grown on
+  // demand; problems and steps of the last call
+  DevLqr lqr = {}; Pool lqr_pool, lqr_ws_pool; int lqr_done = 0;
   // sampling-based MPC (fb_plan_program / fb_plan; fb_plan.h): the program (plan.K > 0: set) and its weights; the buffers, grown on demand
   // with L K T (the samples), L K (their costs and weights), L (T + 1) (mean, xref, uref and the per-problem words) and L n_iter (the
   // record); the rollout parameter of the samples; problems of the last call
-  DevPlan plan = {}; DevRoll plan_roll = {}; std::vector<void*> plan_prog_scope, plan_s_scope, plan_k_scope, plan_l_scope, plan_h_scope;
-  size_t plan_s_cap = 0, plan_k_cap = 0, plan_l_cap = 0, plan_h_cap = 0; int plan_done = 0;
+  DevPlan plan = {}; DevRoll plan_roll = {}; std::vector<void*> plan_prog_scope; Pool plan_s_pool, plan_k_pool, plan_l_pool, plan_h_pool; int plan_done = 0;
   // system identification (fb_sid_accumulate / fb_sid_read; fb_sid.h): the transition scratch (grown with n), the sums of sid_L problems
   // of sid_k directions (grown with L (k^2 + k + 1); sid_L = 0: none yet) and the per-problem words (grown with L + 1)
-  DevSid sid = {}; std::vector<void*> sid_t_scope, sid_s_scope, sid_l_scope; size_t sid_t_cap = 0, sid_s_cap = 0, sid_l_cap = 0;
+  DevSid sid = {}; Pool sid_t_pool, sid_s_pool, sid_l_pool;
   int sid_L = 0, sid_k = 0;
   int device; long long launches; float last_ms; std::string err;
-  int first_substep; int hold_pending;
-  int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; int rst_cap;
-  const int* act_map_dev; int n_action;
+  int first_substep = 1; int hold_pending;
+  int* rst_ids_dev; float* rst_qpos_dev; float* rst_qvel_dev; Pool rst_pool;   // reset lists (do_reset)
+  const int* act_map_dev; int n_action; std::vector<void*> act_map_scope;
   int blob_in_smem;            // copy the sweep program of the triangular solves into shared memory per CTA (default: for batches <= 1024 envs; FB_BLOB=0/1 overrides)
   int* op_step_dev; unsigned char* op_first_dev;
   float* ref_slots; int ref_slot_len;      // per-env reference tables (fb_ref_slots)
   float* rbank_dev; int *rbank_off_dev, *rbank_len_dev, rbank_w; std::vector<int> rbank_len; std::vector<void*> rbank_scope;   // trajectory bank (fb_ref_bank_wide)
-  DevHf hf; bool hf_on; int hf_nrow, hf_ncol;      // heightfield collision (fb_hfield_collision)
+  DevHf hf; bool hf_on; int hf_nrow, hf_ncol; std::vector<void*> hf_pair_scope;      // heightfield collision (fb_hfield_collision)
   float *bank_dev, *bank_hmax_dev, *bank_cmax_dev; int bank_n;      // terrain bank of the device-side vision task (fb_hfield_bank)
-  DevEye eye; float* hfield_dev; float* hmax_dev; float* cmax_dev; int hf_nbr, hf_nbc; unsigned char* eye_out; size_t eye_bytes;   // eye cameras (fb_eye_program)
+  float* hfield_dev; float* hmax_dev; float* cmax_dev; int hf_nbr, hf_nbc; std::vector<void*> hf_scope;   // per-env heightfields (ensure_hfield)
+  DevEye eye; unsigned char* eye_out; size_t eye_bytes; std::vector<void*> eye_scope;                 // eye cameras (fb_eye_program)
   DevTask task_host;                       // host copy of the device-side task program (its pointers are device pointers)
-  float* stage; int* stage_i; size_t stage_cap, stage_icap; unsigned ws_slot;
+  float* stage; int* stage_i; Pool stage_pool, stage_i_pool; unsigned ws_slot;   // staging buffers (ensure_stage)
   // state bank (fb_state_*): [st_slots][st_row] rows of the layout in st_segs; dropped (st_stale) when a program that shapes the layout is replaced
   unsigned* st_bank = nullptr; int st_slots = 0; unsigned st_row = 0; bool st_stale = false; uint64_t st_sig = 0;
   StSeg* st_segs_dev = nullptr; int st_nseg = 0, st_hold_off = 0; std::vector<void*> st_scope;
   std::vector<char> st_written;            // per slot: 0 never written, 1 written, 2 written while an env may be held for its reset
-  int* st_ids_dev = nullptr; int st_ids_cap = 0;
+  int* st_ids_dev = nullptr; Pool st_ids_pool;
 #ifndef FB_EMU
   struct ProfEvent { int kind; cudaEvent_t a, b; };
   std::vector<ProfEvent> prof_events;
@@ -489,7 +491,7 @@ static void launch_step2(FbSim* s, bool integrate) {
 // model upload
 template <typename T> static const T* up(FbSim* s, const std::vector<T>& v) {
   void* p = dev_alloc(sizeof(T) * std::max<size_t>(v.size(), 1));
-  if (p && v.size()) copy_sync(s, p, v.data(), sizeof(T) * v.size());
+  if (p && v.size() && copy_sync(s, p, v.data(), sizeof(T) * v.size()) != 0) { dev_free(p); p = nullptr; }   // a failed upload is a missing buffer
   s->allocs.push_back(p);
   return (const T*)p;
 }
@@ -503,7 +505,7 @@ static const int* upi(FbSim* s, const int32_t* src, size_t n) { std::vector<int>
 template <typename T> static T* dalloc(FbSim* s, size_t n) { void* p = dev_alloc(sizeof(T) * n); s->allocs.push_back(p); return (T*)p; }
 // free the buffers a replaced program owned (the stream is idle: the callers synchronise first)
 static void scope_free(FbSim* s, std::vector<void*>& scope) {
-  for (void* p : scope) { if (!p) continue; for (auto& a : s->allocs) if (a == p) { a = nullptr; break; } dev_free(p); }
+  for (void* p : scope) { s->allocs.erase(std::find(s->allocs.begin(), s->allocs.end(), p)); dev_free(p); }
   scope.clear();
 }
 // the buffers `alloc` allocates (dalloc / up) become `scope`; if one of them is missing the whole group is freed again and the
@@ -513,6 +515,18 @@ template <typename F> static int scope_alloc(FbSim* s, std::vector<void*>& scope
   alloc();
   scope.assign(s->allocs.begin() + mark, s->allocs.end());
   for (void* p : scope) if (!p) { scope_free(s, scope); s->err = oom; return -4; }
+  return 0;
+}
+// one pool for `rows` rows (`unit` says what a row is) of `row_bytes` bytes, made by alloc(rows) unless `cap` rows fit already
+template <typename F> static int grow(FbSim* s, const char* who, Pool& pool, size_t rows, size_t row_bytes, const char* what, const char* unit, F alloc) {
+  if (rows <= pool.cap) return 0;
+  if (sync_stream(s) != 0) return -2;
+  scope_free(s, pool.bufs); pool.cap = 0;
+  if (rows * row_bytes > dev_free_bytes()) {
+    s->err = std::string(who) + ": the " + what + " of " + std::to_string(rows) + " rows (" + unit + ") do not fit the device's free memory"; return -4; }
+  const std::string oom = std::string(who) + ": out of device memory (" + what + ")";
+  if (int rc = scope_alloc(s, pool.bufs, oom.c_str(), [&] { alloc(rows); })) return rc;
+  pool.cap = rows;
   return 0;
 }
 
@@ -790,7 +804,6 @@ static int alloc_data(FbSim* s, int N) {
 #endif
   d.obs_dim = m.nq + m.nv + m.na + 2 * m.nsensordata + 12 + 3 * m.nsite + 3;
   d.obs = dalloc<float>(s, (size_t)d.obs_dim * d.Np);
-  s->stage_cap = 0; s->stage = nullptr; s->stage_i = nullptr;
   return 0;
 }
 
@@ -814,11 +827,9 @@ static void field_from_host(FbSim* s, void* dev, int n, const void* src) {
   sync_stream(s);
 }
 // device staging buffer for scatter-style uploads (ctrl, ghost pose, partial resets)
-static int ensure_stage(FbSim* s, size_t floats, size_t ints) {
-  if (floats > s->stage_cap || ints > s->stage_icap) sync_stream(s);
-  if (floats > s->stage_cap) { s->stage = dalloc<float>(s, floats); s->stage_cap = floats; if (!s->stage) return -4; }
-  if (ints > s->stage_icap) { s->stage_i = dalloc<int>(s, ints); s->stage_icap = ints; if (!s->stage_i) return -4; }
-  return 0;
+static int ensure_stage(FbSim* s, const char* who, size_t floats, size_t ints) {
+  if (int rc = grow(s, who, s->stage_pool, floats, 4, "staging", "floats", [&](size_t r) { s->stage = dalloc<float>(s, r); })) return rc;
+  return grow(s, who, s->stage_i_pool, ints, 4, "index staging", "ints", [&](size_t r) { s->stage_i = dalloc<int>(s, r); });
 }
 
 // The state bank's rows follow the handle's arrays: whatever replaces an observation / task program, the reference slots, the
@@ -902,14 +913,13 @@ const char* fb_version(void) { return kVersion; }
 
 int fb_create(const FbModel* hm, int n_envs, int device, FbHandle* out) {
   if (!hm || !out || n_envs <= 0) return -1;
-  FbSim* s = new FbSim();
-  s->device = device; s->launches = 0; s->last_ms = 0; s->hm = *hm; s->first_substep = 1; s->hold_pending = 0; s->prof_on = 0; memset(s->prof_ms, 0, sizeof(s->prof_ms)); memset(s->prof_n, 0, sizeof(s->prof_n));
-  s->ref_slots = nullptr; s->ref_slot_len = 0; s->eye_out = nullptr; s->hfield_dev = nullptr; s->hmax_dev = nullptr; s->cmax_dev = nullptr; s->hf_nbr = s->hf_nbc = 0; s->bank_dev = s->bank_hmax_dev = s->bank_cmax_dev = nullptr; s->bank_n = 0; s->eye_bytes = 0; s->hf_on = false; s->hf_nrow = s->hf_ncol = 0;
-  s->rbank_dev = nullptr; s->rbank_off_dev = s->rbank_len_dev = nullptr; s->rbank_w = 0;
-  s->op_step_dev = nullptr; s->op_first_dev = nullptr; s->stage_cap = 0; s->stage_icap = 0; s->stage = nullptr; s->stage_i = nullptr;
+  FbSim* s = new FbSim();                  // (value-initialised: every field without an initialiser starts at zero)
+  s->device = device; s->hm = *hm;
   if (dev_open(s, n_envs) != 0) { delete s; return -2; }
   int rc = build_model(s, hm);             // (every upload and allocation has completed when it returns)
   if (rc == 0) rc = alloc_data(s, n_envs);
+  // nothing has been freed yet, so a missing entry is an upload or allocation that failed
+  if (rc == 0 && std::count(s->allocs.begin(), s->allocs.end(), nullptr)) { s->err = "out of device memory (model and env data)"; rc = -4; }
   if (rc == 0) prm_layout(s, hm);
   *out = s;
   if (rc != 0) return rc;
@@ -1208,7 +1218,7 @@ int fb_set_ctrl(FbHandle s, const float* ctrl, int is_device) {
   const float* src = ctrl;
   const int k = s->act_map_dev ? s->n_action : s->m.nu;     // row length: actions (mapped on the device) or ctrl
   if (!is_device) {
-    if (ensure_stage(s, (size_t)s->d.N * std::max(k, s->m.nu), 0) != 0) { s->err = "out of device memory (staging)"; return -4; }
+    if (int rc = ensure_stage(s, "fb_set_ctrl", (size_t)s->d.N * std::max(k, s->m.nu), 0)) return rc;
     if (copy_async(s, s->stage, ctrl, sizeof(float) * (size_t)s->d.N * k) != 0) return -2;
     src = s->stage;
   }
@@ -1217,11 +1227,14 @@ int fb_set_ctrl(FbHandle s, const float* ctrl, int is_device) {
 }
 int fb_set_action_map(FbHandle s, const int32_t* ctrl_index, int n_action) {
   if (!s) return -1;
-  if (!ctrl_index || n_action <= 0) { s->act_map_dev = nullptr; s->n_action = 0; return 0; }      // back to plain ctrl rows
-  for (int c = 0; c < n_action; c++) if (ctrl_index[c] >= s->m.nu || ctrl_index[c] < -1) { s->err = "fb_set_action_map: ctrl index out of range (valid: -1 = no target, 0..nu-1)"; return -1; }
-  if (sync_stream(s) != 0) return -2;
+  const bool clear = !ctrl_index || n_action <= 0;      // back to plain ctrl rows
+  for (int c = 0; !clear && c < n_action; c++) if (ctrl_index[c] >= s->m.nu || ctrl_index[c] < -1) { s->err = "fb_set_action_map: ctrl index out of range (valid: -1 = no target, 0..nu-1)"; return -1; }
+  if (sync_stream(s) != 0) return -2;      // a scatter in flight may still read the old map
+  scope_free(s, s->act_map_scope); s->act_map_dev = nullptr; s->n_action = 0;
+  if (clear) return 0;
   std::vector<int> v(ctrl_index, ctrl_index + n_action);
-  s->act_map_dev = up(s, v); s->n_action = n_action;
+  if (int rc = scope_alloc(s, s->act_map_scope, "fb_set_action_map: out of device memory", [&] { s->act_map_dev = up(s, v); })) { s->act_map_dev = nullptr; return rc; }
+  s->n_action = n_action;
   return 0;
 }
 
@@ -1236,7 +1249,7 @@ int fb_write_state(FbHandle s, int field, const int32_t* idx, int k, const float
   // separate staging regions so that several writes can be in flight before the next sync
   size_t need = (size_t)s->d.N * s->m.nu + (size_t)4 * s->d.N * 16;
   if (k > 16) return -1;
-  if (ensure_stage(s, need, 64) != 0) { s->err = "out of device memory (staging)"; return -4; }
+  if (int rc = ensure_stage(s, "fb_write_state", need, 64)) return rc;
   int slot = s->ws_slot++ & 3;
   float* vdev = s->stage + (size_t)s->d.N * s->m.nu + (size_t)slot * s->d.N * 16;
   int* idev = s->stage_i + slot * 16;
@@ -1349,14 +1362,12 @@ static int do_reset(FbSim* s, const int32_t* env_ids, int n, const float* qpos, 
     ids.push_back(e); qp.insert(qp.end(), qp.begin(), qp.begin() + m.nq); if (qvel) qv.insert(qv.end(), qv.begin(), qv.begin() + m.nv);
   }
   int cnt = (int)ids.size();
-  if (cnt > s->rst_cap) {
-    s->rst_cap = std::max(cnt, Np);
-    s->rst_ids_dev = dalloc<int>(s, s->rst_cap); s->rst_qpos_dev = dalloc<float>(s, (size_t)s->rst_cap * m.nq); s->rst_qvel_dev = dalloc<float>(s, (size_t)s->rst_cap * m.nv);
-  }
-  copy_async(s, s->rst_ids_dev, ids.data(), sizeof(int) * cnt);
-  copy_async(s, s->rst_qpos_dev, qp.data(), sizeof(float) * qp.size());
-  if (qvel) copy_async(s, s->rst_qvel_dev, qv.data(), sizeof(float) * qv.size());
-  if (sync_stream(s) != 0) return -2;       // the host vectors go out of scope below
+  if (int rc = grow(s, "reset", s->rst_pool, std::max(cnt, Np), 4 * (1 + (size_t)m.nq + m.nv), "reset lists", "envs", [&](size_t r) {
+        s->rst_ids_dev = dalloc<int>(s, r); s->rst_qpos_dev = dalloc<float>(s, r * m.nq); s->rst_qvel_dev = dalloc<float>(s, r * m.nv); }))
+    return rc;
+  const bool copied = copy_async(s, s->rst_ids_dev, ids.data(), sizeof(int) * cnt) == 0 && copy_async(s, s->rst_qpos_dev, qp.data(), sizeof(float) * qp.size()) == 0 &&
+                      (!qvel || copy_async(s, s->rst_qvel_dev, qv.data(), sizeof(float) * qv.size()) == 0);
+  if (sync_stream(s) != 0 || !copied) return -2;       // the host vectors go out of scope below
   s->d.rst_ids = s->rst_ids_dev; s->d.rst_qpos = s->rst_qpos_dev; s->d.rst_qvel = s->rst_qvel_dev; s->d.rst_n = cnt; s->d.rst_has_qvel = qvel ? 1 : 0; s->d.rst_hold = hold;
   fb_launch<ShNone, Ph<ph_reset_scatter>, Ph<ph_reset_draw>, Ph<ph_reset_count>>(s, K_MISC, 0, cnt);
   s->d.rst_n = 0;
@@ -1541,10 +1552,10 @@ int fb_task_program(FbHandle s, const FbTaskProgram* p) {
   t.term_angvel = p->terminal_angvel; t.term_qacc = p->terminal_qacc; t.term_height = p->terminal_height;
   t.velocimeter_adr = p->velocimeter_adr; t.gyro_adr = p->gyro_adr; t.com_body = p->com_body;
   t.ref_len = p->ref_len; t.obs_refdisp_off = p->obs_refdisp_off; t.obs_refquat_off = p->obs_refquat_off;
-  auto upf32 = [&](const float* src, size_t n) { std::vector<float> v(src, src + n); return up(s, v); };
-  auto upi32 = [&](const int32_t* src, size_t n) { std::vector<int> v(src, src + n); return up(s, v); };
   float *ty = nullptr, *tx = nullptr; int* tl = nullptr; DevTask* dev = nullptr;
   const int rc = scope_alloc(s, s->task_scope, "out of device memory (task program)", [&] {
+    auto upf32 = [&](const float* src, size_t n) { std::vector<float> v(src, src + n); return up(s, v); };
+    auto upi32 = [&](const int32_t* src, size_t n) { std::vector<int> v(src, src + n); return up(s, v); };
     t.reset_qpos = upf32(p->reset_qpos, m.nq);
     if (p->kind == FB_TASK_BALL) { t.ball_vadr = p->ball_vadr; for (int i = 0; i < 3; i++) t.ball_target[i] = p->ball_target[i]; t.ball_margin = p->ball_margin; }
     if (!bank && p->kind != FB_TASK_TEMPLATE && p->kind != FB_TASK_BALL) { t.ref_qpos = upf32(p->ref_qpos, (size_t)7 * p->ref_len); t.ref_qvel = upf32(p->ref_qvel, (size_t)6 * p->ref_len); }
@@ -1788,11 +1799,13 @@ static int ensure_hfield(FbSim* s, int nrow, int ncol) {
     if (s->hf_nrow != nrow || s->hf_ncol != ncol) { s->err = "heightfield grid differs from the one already allocated"; return -1; }
     return 0;
   }
-  s->hfield_dev = dalloc<float>(s, (size_t)nrow * ncol * s->d.Np); s->hmax_dev = dalloc<float>(s, s->d.Np);
-  s->hf_nrow = nrow; s->hf_ncol = ncol;
   // block maxima for the eye ray marcher (fb_render.h: FB_EYE_BLOCK)
-  s->hf_nbr = (nrow - 1 + FB_EYE_BLOCK - 1) / FB_EYE_BLOCK; s->hf_nbc = (ncol - 1 + FB_EYE_BLOCK - 1) / FB_EYE_BLOCK;
-  s->cmax_dev = dalloc<float>(s, (size_t)s->hf_nbr * s->hf_nbc * s->d.Np);
+  const int nbr = (nrow - 1 + FB_EYE_BLOCK - 1) / FB_EYE_BLOCK, nbc = (ncol - 1 + FB_EYE_BLOCK - 1) / FB_EYE_BLOCK;
+  if (int rc = scope_alloc(s, s->hf_scope, "out of device memory (heightfields)", [&] {
+        s->hfield_dev = dalloc<float>(s, (size_t)nrow * ncol * s->d.Np); s->hmax_dev = dalloc<float>(s, s->d.Np);
+        s->cmax_dev = dalloc<float>(s, (size_t)nbr * nbc * s->d.Np); })) {
+    s->hfield_dev = s->hmax_dev = s->cmax_dev = nullptr; return rc; }
+  s->hf_nrow = nrow; s->hf_ncol = ncol; s->hf_nbr = nbr; s->hf_nbc = nbc;
   return 0;
 }
 int fb_hfield_collision(FbHandle s, int geom, const float* size, int nrow, int ncol, const int32_t* pair_geom, int npair) {
@@ -1800,13 +1813,15 @@ int fb_hfield_collision(FbHandle s, int geom, const float* size, int nrow, int n
   if (geom < 0 || geom >= s->m.ngeom) { s->err = "fb_hfield_collision: geom id out of range"; return -1; }
   for (int k = 0; k < npair; k++) if (pair_geom[k] < 0 || pair_geom[k] >= s->m.ngeom) { s->err = "fb_hfield_collision: pair geom out of range"; return -1; }
   if (sync_stream(s) != 0) return -2;
-  if (ensure_hfield(s, nrow, ncol) != 0) return -1;
+  if (int rc = ensure_hfield(s, nrow, ncol)) return rc;
+  graphs_drop(s);                          // a captured step graph holds the old DevHf and its pair list, which is freed here
+  scope_free(s, s->hf_pair_scope); s->hf_on = false;
   DevHf& h = s->hf; h.geom = geom; h.nrow = nrow; h.ncol = ncol; h.npair = npair;
   for (int k = 0; k < 4; k++) h.size[k] = size[k];
-  std::vector<int> pg(pair_geom, pair_geom + npair); h.pair_geom = up(s, pg);
+  std::vector<int> pg(pair_geom, pair_geom + npair);
+  if (int rc = scope_alloc(s, s->hf_pair_scope, "fb_hfield_collision: out of device memory", [&] { h.pair_geom = up(s, pg); })) return rc;
   h.data = s->hfield_dev; h.hmax = s->hmax_dev;
   s->hf_on = true;
-  graphs_drop(s);
   return 0;
 }
 int fb_eye_program(FbHandle s, const FbEyeProgram* p) {
@@ -1814,15 +1829,17 @@ int fb_eye_program(FbHandle s, const FbEyeProgram* p) {
   if (p->n_cam < 1 || p->n_cam > FB_MAXCAM || p->size < 1 || p->size > 512 || !(p->fovy_deg > 0 && p->fovy_deg < 180) || p->nrow < 0 || (p->nrow > 0 && (p->nrow < 2 || p->ncol < 2 || !(p->half_size > 0)))) { s->err = "fb_eye_program: bad camera / grid parameters"; return -1; }
   for (int c = 0; c < p->n_cam; c++) if (p->body[c] <= 0 || p->body[c] >= s->m.nbody) { s->err = "fb_eye_program: camera body out of range"; return -1; }
   if (sync_stream(s) != 0) return -2;
+  scope_free(s, s->eye_scope); s->eye_out = nullptr;      // the images of the program this one replaces
   DevEye& y = s->eye; memset(&y, 0, sizeof(y));
   y.n_cam = p->n_cam; y.size = p->size; y.nrow = p->nrow; y.ncol = p->nrow > 0 ? p->ncol : 0;
   for (int c = 0; c < p->n_cam; c++) { y.body[c] = p->body[c]; for (int k = 0; k < 3; k++) y.pos[c][k] = p->pos[c][k]; for (int k = 0; k < 4; k++) y.quat[c][k] = p->quat[c][k]; }
   y.tan_half = tanf(0.5f * p->fovy_deg * 3.14159265358979f / 180.0f); y.half_size = p->half_size; y.z_offset = p->z_offset; y.zfar = p->zfar > 0 ? p->zfar : 50.0f;
   for (int k = 0; k < 3; k++) { y.sky_top[k] = p->sky_top[k]; y.sky_horizon[k] = p->sky_horizon[k]; y.ground[k] = p->ground[k]; }
   y.ambient = p->ambient; y.diffuse = p->diffuse;
-  if (y.nrow > 0 && ensure_hfield(s, y.nrow, y.ncol) != 0) return -1;
+  if (y.nrow > 0) if (int rc = ensure_hfield(s, y.nrow, y.ncol)) return rc;
   s->eye_bytes = (size_t)y.n_cam * y.size * y.size * 3;
-  s->eye_out = dalloc<unsigned char>(s, s->eye_bytes * s->d.Np);
+  if (int rc = scope_alloc(s, s->eye_scope, "fb_eye_program: out of device memory (images)", [&] { s->eye_out = dalloc<unsigned char>(s, s->eye_bytes * s->d.Np); })) {
+    s->eye_out = nullptr; return rc; }
   y.hfield = s->hfield_dev; y.hmax = s->hmax_dev; y.out = s->eye_out;
   y.cmax = (y.nrow > 0 && !getenv("FB_EYE_NO_SKIP")) ? s->cmax_dev : nullptr; y.nbr = s->hf_nbr; y.nbc = s->hf_nbc;
   return 0;
@@ -1942,11 +1959,8 @@ static int state_ready(FbSim* s, const char* who) {
 // the (env, slot) lists of a save / load on the device: envs at [0, n), slots at [n, 2n); a NULL list stays NULL (the identity)
 static int state_ids(FbSim* s, const int32_t* env_ids, const int32_t* slots, int n, const int** env_dev, const int** slot_dev) {
   *env_dev = *slot_dev = nullptr;
-  if (2 * n > s->st_ids_cap) {
-    if (sync_stream(s) != 0) return -2;
-    s->st_ids_cap = std::max(2 * n, 2 * s->d.Np); s->st_ids_dev = dalloc<int>(s, s->st_ids_cap);
-    if (!s->st_ids_dev) { s->st_ids_cap = 0; s->err = "out of device memory (state id lists)"; return -4; }
-  }
+  if (int rc = grow(s, "state bank", s->st_ids_pool, 2 * (size_t)std::max(n, s->d.Np), 4, "env and slot lists", "2 envs", [&](size_t r) {
+        s->st_ids_dev = dalloc<int>(s, r); })) return rc;
   if (env_ids) { if (copy_async(s, s->st_ids_dev, env_ids, sizeof(int) * n) != 0) return -2; *env_dev = s->st_ids_dev; }
   if (slots) { if (copy_async(s, s->st_ids_dev + n, slots, sizeof(int) * n) != 0) return -2; *slot_dev = s->st_ids_dev + n; }
   return 0;
@@ -2538,22 +2552,6 @@ struct RollRecord {
   DevModel m; DevData d; DevRoll p;
   FB_DEVM void operator()(unsigned char*, int e) const { kroll_record(m, d, p, e); }
 };
-// one group of buffers for `rows` rows (`unit` says what a row is) of `row_bytes` bytes, made by alloc(rows) unless `cap` rows fit already
-template <typename F> static int grow(FbSim* s, const char* who, std::vector<void*>& scope, size_t& cap, size_t rows, size_t row_bytes,
-                                      const char* what, const char* unit, F alloc) {
-  if (rows <= cap) return 0;
-  if (sync_stream(s) != 0) return -2;
-  scope_free(s, scope); cap = 0;
-  if (rows * row_bytes > dev_free_bytes()) {
-    s->err = std::string(who) + ": the " + what + " of " + std::to_string(rows) + " rows (" + unit + ") do not fit the device's free memory"; return -4; }
-  const std::string oom = std::string(who) + ": out of device memory (" + what + ")";
-  if (int rc = scope_alloc(s, scope, oom.c_str(), [&] { alloc(rows); })) return rc;
-  cap = rows;
-  return 0;
-}
-template <typename F> static int roll_grow(FbSim* s, std::vector<void*>& scope, size_t& cap, size_t rows, size_t row_bytes, const char* what, F alloc) {
-  return grow(s, "fb_rollout", scope, cap, rows, row_bytes, what, "n T", alloc);
-}
 // the feedback bank (fb_rollout_feedback_bank; fb_rollout_feedback is L = 1 without a law list)
 static int rollout_feedback(FbSim* s, const char* who, int L, int T, const float* xref, const float* K, const int32_t* law, int n, int is_device) {
   const DevModel& m = s->m;
@@ -2575,10 +2573,10 @@ static int rollout_feedback(FbSim* s, const char* who, int L, int T, const float
   if (sync_stream(s) != 0) return -2;          // a rollout in flight may still read the old law
   s->roll_fb_T = s->roll_fb_L = s->roll_fb_n = 0;
   if (clear) return 0;
-  if (int rc = grow(s, who, s->roll_fb_scope, s->roll_fb_cap, lt, 4 * (nr + m.nu * nx), "feedback laws", "L T", [&](size_t r) {
+  if (int rc = grow(s, who, s->roll_fb_pool, lt, 4 * (nr + m.nu * nx), "feedback laws", "L T", [&](size_t r) {
         s->roll_xref = dalloc<float>(s, r * nr); s->roll_K = dalloc<float>(s, r * m.nu * nx); }))
     return rc;
-  if (law) if (int rc = grow(s, who, s->roll_law_scope, s->roll_law_cap, n, 4, "law list", "n", [&](size_t r) { s->roll_law = dalloc<int>(s, r); }))
+  if (law) if (int rc = grow(s, who, s->roll_law_pool, n, 4, "law list", "n", [&](size_t r) { s->roll_law = dalloc<int>(s, r); }))
     return rc;
   if (copy_async(s, s->roll_xref, xref, sizeof(float) * lt * nr) != 0 || copy_async(s, s->roll_K, K, sizeof(float) * lt * m.nu * nx) != 0 ||
       (law && copy_async(s, s->roll_law, law, sizeof(int) * n) != 0)) return -2;
@@ -2625,15 +2623,15 @@ int fb_rollout(FbHandle s, const int32_t* slots, int n, int T, int n_substeps, c
   dev_select(s);
   s->roll_done = 0;
   DevRoll& p = s->roll;
-  if (int rc = roll_grow(s, s->roll_scope, s->roll_cap, rows, 4 * (2 * nu + nq + nv + na + 2), "records", [&](size_t r) {
+  if (int rc = grow(s, who, s->roll_pool, rows, 4 * (2 * nu + nq + nv + na + 2), "records", "n T", [&](size_t r) {
         p.ctrl = dalloc<float>(s, r * nu); p.qpos = dalloc<float>(s, r * nq); p.qvel = dalloc<float>(s, r * nv); p.act = dalloc<float>(s, r * na);
         p.ctrl_out = dalloc<float>(s, r * nu); p.time = dalloc<float>(s, r); p.flags = dalloc<int>(s, r); }))
     return rc;
-  if (int rc = app ? roll_grow(s, s->roll_app_scope, s->roll_app_cap, rows, 4 * (nv + nxf), "applied-force inputs", [&](size_t r) {
+  if (int rc = app ? grow(s, who, s->roll_app_pool, rows, 4 * (nv + nxf), "applied-force inputs", "n T", [&](size_t r) {
         s->roll_qf = dalloc<float>(s, r * nv); s->roll_xf = dalloc<float>(s, r * nxf); }) : 0)
     return rc;
   const bool sens = s->sens_on != 0;
-  if (int rc = sens ? roll_grow(s, s->roll_sd_scope, s->roll_sd_cap, rows, 8 * nsd, "sensor records", [&](size_t r) {
+  if (int rc = sens ? grow(s, who, s->roll_sd_pool, rows, 8 * nsd, "sensor records", "n T", [&](size_t r) {
         s->roll_sd = dalloc<float>(s, r * nsd); s->roll_sm = dalloc<float>(s, r * nsd); }) : 0)
     return rc;
   p.qfrc = qfrc_applied ? s->roll_qf : nullptr; p.xfrc = xfrc_applied ? s->roll_xf : nullptr;
@@ -2709,14 +2707,14 @@ int fb_lqr(FbHandle s, int L, int T, const float* A, const float* B, const doubl
   s->lqr_done = 0;
   DevLqr& p = s->lqr;
   // per problem step (L (T + 1) rows, the last T + 1st unused by A, B, r, K, k): the inputs A, B, q, r and the outputs K, k
-  if (int rc = grow(s, who, s->lqr_scope, s->lqr_cap, l1, 4 * ((size_t)nx * nx + (size_t)nx * nu) + 8 * ((size_t)nx + nu + (size_t)nu * nx + nu),
+  if (int rc = grow(s, who, s->lqr_pool, l1, 4 * ((size_t)nx * nx + (size_t)nx * nu) + 8 * ((size_t)nx + nu + (size_t)nu * nx + nu),
                     "inputs and gains", "L (T + 1)", [&](size_t n) {
         p.A = dalloc<float>(s, n * nx * nx); p.B = dalloc<float>(s, n * nx * nu); p.q = dalloc<double>(s, n * nx); p.r = dalloc<double>(s, n * nu);
         p.K = dalloc<double>(s, n * nu * nx); p.k = dalloc<double>(s, n * nu); }))
     return rc;
   // per problem: the workspace, mu, dV and status (and the shared weights)
   const size_t ws = (size_t)nx * nx + nx + (size_t)nx * (nz + 1) + (size_t)nz * (nz + 1) + (size_t)nu * nu + 2 * (size_t)nu * (nx + 1) + 3;
-  if (int rc = grow(s, who, s->lqr_ws_scope, s->lqr_ws_cap, (size_t)L, 8 * ws + 4, "workspace", "L", [&](size_t n) {
+  if (int rc = grow(s, who, s->lqr_ws_pool, (size_t)L, 8 * ws + 4, "workspace", "L", [&](size_t n) {
         p.P = dalloc<double>(s, n * nx * nx); p.s = dalloc<double>(s, n * nx); p.W = dalloc<double>(s, n * nx * (nz + 1));
         p.H = dalloc<double>(s, n * nz * (nz + 1)); p.C = dalloc<double>(s, n * nu * nu); p.X = dalloc<double>(s, n * nu * (nx + 1));
         p.G = dalloc<double>(s, n * nu * (nx + 1)); p.mu = dalloc<double>(s, n); p.dV = dalloc<double>(s, 2 * n); p.status = dalloc<int>(s, n);
@@ -2820,16 +2818,16 @@ int fb_plan(FbHandle s, const int32_t* slots, int L, int T, int n_substeps, int 
   dev_select(s);
   s->plan_done = 0;
   const size_t n = (size_t)L * K;
-  if (int rc = grow(s, who, s->plan_s_scope, s->plan_s_cap, n * T, 4 * nu, "samples", "L n_samples T", [&](size_t r) { p.ctrl = dalloc<float>(s, r * nu); }))
+  if (int rc = grow(s, who, s->plan_s_pool, n * T, 4 * nu, "samples", "L n_samples T", [&](size_t r) { p.ctrl = dalloc<float>(s, r * nu); }))
     return rc;
-  if (int rc = grow(s, who, s->plan_k_scope, s->plan_k_cap, n, 16, "sample costs", "L n_samples", [&](size_t r) {
+  if (int rc = grow(s, who, s->plan_k_pool, n, 16, "sample costs", "L n_samples", [&](size_t r) {
         p.J = dalloc<double>(s, r); p.w = dalloc<double>(s, r); }))
     return rc;
-  if (int rc = grow(s, who, s->plan_l_scope, s->plan_l_cap, l1, 4 * (2 * nu + nr) + 24, "means and references", "L (T + 1)", [&](size_t r) {
+  if (int rc = grow(s, who, s->plan_l_pool, l1, 4 * (2 * nu + nr) + 24, "means and references", "L (T + 1)", [&](size_t r) {
         p.mean = dalloc<float>(s, r * nu); p.xref = dalloc<float>(s, r * nr); p.uref = dalloc<float>(s, r * nu);
         p.seed = dalloc<unsigned>(s, r); p.wsum = dalloc<double>(s, r); p.sel = dalloc<int>(s, r); p.status = dalloc<int>(s, r); }))
     return rc;
-  if (int rc = grow(s, who, s->plan_h_scope, s->plan_h_cap, (size_t)L * n_iter, 16, "cost record", "L n_iter", [&](size_t r) { p.hist = dalloc<double>(s, 2 * r); }))
+  if (int rc = grow(s, who, s->plan_h_pool, (size_t)L * n_iter, 16, "cost record", "L n_iter", [&](size_t r) { p.hist = dalloc<double>(s, 2 * r); }))
     return rc;
   if (copy_async(s, p.mean, mean, 4 * lt * nu) != 0 || copy_async(s, (void*)p.xref, xref, 4 * l1 * nr) != 0 ||
       (uref && copy_async(s, (void*)p.uref, uref, 4 * lt * nu) != 0) || copy_async(s, (void*)p.seed, seeds, 4 * (size_t)L) != 0) return -2;
@@ -2924,16 +2922,16 @@ int fb_sid_accumulate(FbHandle s, int query, int L, const int32_t* problem, int 
   dev_select(s);
   DevSid& p = s->sid;
   if (reset) s->sid_L = 0;                     // (growing the sums drops them)
-  if (int rc = grow(s, who, s->sid_t_scope, s->sid_t_cap, (size_t)n, 8 * (size_t)(2 * m.nv + m.na + 1) + 4 * (size_t)(m.nq + m.nv + m.na + 3),
+  if (int rc = grow(s, who, s->sid_t_pool, (size_t)n, 8 * (size_t)(2 * m.nv + m.na + 1) + 4 * (size_t)(m.nq + m.nv + m.na + 3),
                     "transition scratch", "n", [&](size_t r) {
         p.res = dalloc<double>(s, r * (2 * m.nv + m.na)); p.tcost = dalloc<double>(s, r); p.tbad = dalloc<int>(s, r);
         p.target = dalloc<float>(s, r * (m.nq + m.nv + m.na)); p.sw = dalloc<float>(s, r); p.order = dalloc<int>(s, r);
         p.W = dalloc<double>(s, 2 * m.nv + m.na); }))
     return rc;
   const size_t E = (size_t)k * k + k + 1;
-  if (int rc = grow(s, who, s->sid_s_scope, s->sid_s_cap, (size_t)L * E, 8, "sums", "L (k^2 + k + 1)", [&](size_t r) { p.H = dalloc<double>(s, r); }))
+  if (int rc = grow(s, who, s->sid_s_pool, (size_t)L * E, 8, "sums", "L (k^2 + k + 1)", [&](size_t r) { p.H = dalloc<double>(s, r); }))
     return rc;
-  if (int rc = grow(s, who, s->sid_l_scope, s->sid_l_cap, (size_t)L + 1, 12, "per-problem words", "L + 1", [&](size_t r) {
+  if (int rc = grow(s, who, s->sid_l_pool, (size_t)L + 1, 12, "per-problem words", "L + 1", [&](size_t r) {
         p.count = dalloc<int>(s, r); p.bad = dalloc<int>(s, r); p.ptr = dalloc<int>(s, r); }))
     return rc;
   if (copy_async(s, (void*)p.order, order.data(), 4 * order.size()) != 0 || copy_async(s, (void*)p.ptr, ptr.data(), 4 * (size_t)(L + 1)) != 0 ||

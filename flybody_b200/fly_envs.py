@@ -356,6 +356,7 @@ class _TaskEnv:
         head = self.model.body_id('walker/head')
         self._sim.eye_program([head, head], [p for _, p, _ in _EYE_CAMERAS], quats, fovy_deg=fovy, size=size, nrow=nrow, ncol=ncol,
                               half_size=half_size, z_offset=z_offset)
+        self._eyes_dev = None           # a view of the images the program replaced, which it freed (made again by `eyes_device`)
 
     # -------------------------------------------------------------------------------- episode
     def request_reset(self, env_ids):

@@ -851,7 +851,8 @@ class BatchedStepper:
         self._check(self._lib.fb_hfield_write(self._h, ids.ctypes.data, len(ids), h.ctypes.data), 'fb_hfield_write')
 
     def eyes_ptr(self):
-        """(device pointer, bytes per env) of the eye-camera images (valid after eye_program; rewritten by every render_eyes)"""
+        """(device pointer, bytes per env) of the eye-camera images (valid from eye_program until the next eye_program or close;
+        rewritten by every render_eyes)"""
         p, n = C.c_void_p(), C.c_int()
         self._check(self._lib.fb_eyes_ptr(self._h, C.byref(p), C.byref(n)), 'fb_eyes_ptr')
         return p.value, n.value

@@ -84,7 +84,6 @@ class BatchedVisionFlightEnv(_TaskEnv):
         self._eye_program(eye_camera_size, eye_camera_fovy, a0.nrow, a0.ncol, self._half, float(m.geom_pos[m.meta['hf_geom']][2]))
         self._eye_size = eye_camera_size
         self._eyes_host = _pinned((N, 2, eye_camera_size, eye_camera_size, 3), np.uint8)      # D2H target of every step's render
-        self._eyes_dev = None
         # per-env episode state
         self._target_height, self._target_speed = np.zeros(N), np.zeros(N)
         self._wing_qpos = np.zeros((N, 6))

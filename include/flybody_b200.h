@@ -487,6 +487,8 @@ int fb_hfield_collision(FbHandle h, int geom, const float* size, int nrow, int n
 int fb_hfield_write(FbHandle h, const int32_t* env_ids, int n, const float* heights);
 /* Render every env's eyes from the current poses into the library's buffer [n_envs][n_cam][size][size][3] (uint8).   */
 int fb_render_eyes(FbHandle h);
+/* The device address of that buffer and its bytes per env.  The pointer is valid until the next fb_eye_program, which frees the
+ * buffer and allocates a new one, or fb_destroy.                                                                         */
 int fb_eyes_ptr(FbHandle h, void** dev_ptr, int* bytes_per_env);
 int fb_eyes_read(FbHandle h, uint8_t* host_dst);
 /* State rows: the batched stand-in for physics.get_state() / physics.set_state() (dm_control), extended by what a batched
