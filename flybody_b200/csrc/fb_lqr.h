@@ -229,3 +229,251 @@ FB_WARPFN void klqr_p(const DevLqr& p, int w) {
     }
   WPAR_END
 }
+
+// ---- control-limited DDP (Tassa, Mansard & Todorov 2014; fb_lqr_box): klqr_chol and klqr_solve give way to
+//   klqr_boxqp      k = argmin 1/2 x'Quu x + Qu'x subject to lower_t <= x <= upper_t, by the projected Newton method of Tassa's boxQP;
+//                   C the Cholesky factor of the free block Quu_ff, with identity rows and columns on the clamped controls
+//   klqr_solve_box  K = -Quu_ff^-1 Qux_f on the free rows, 0 on the clamped ones; X = (K | k) and G = Quu X + (Qux | Qu) as klqr_solve
+// and klqr_p's general value update holds for that K and k as it is.  The bounds are on the control change du = u - ubar.
+// boxQP's constants:
+#define BOXQP_MAX_ITER 100       // Newton iterations
+#define BOXQP_MIN_GRAD 1e-8      // stop when |g_free|_2 is below
+#define BOXQP_MIN_REL 1e-8       // stop when an accepted step lowers the objective by less than this times |objective|
+#define BOXQP_STEP_DEC 0.6       // the projected line search's step factor
+#define BOXQP_MIN_STEP 1e-22     // the line search gives up below this step
+#define BOXQP_ARMIJO 0.1         // accept a step when (f_try - f) / (step dx'g) >= this
+// stop reasons (qp[1]), Tassa's numbering: -1 a free block that is not positive definite (status = t + 1), 0 no descent direction,
+// 1 BOXQP_MAX_ITER iterations, 2 the line search gave up, 4 a small improvement, 5 a small free gradient, 6 every control clamped
+
+struct DevLqrBox {
+  const double *lower, *upper;              // [L][T][nu] bounds on du (+-inf allowed)
+  int *clamped, *qp;                        // outputs: [L][T][nu] -1 at lower, +1 at upper, 0 free; [L][T][2] accepted steps, stop reason
+  double *x, *dx, *g, *xt;                  // workspace per problem [nu]: the iterate, the Newton direction, the gradient, the trial point
+  int* set;                                 // [nu] per problem: the clamped set C was last factored for (1 clamped)
+};
+
+// one problem step's QP: Quu and Qu in H's rows (stride ncol), its bounds, workspace and outputs
+struct LqrQp {
+  int nu, ncol;
+  const double *Quu, *Qu, *lo, *hi;
+  double *x, *dx, *g, *xt, *C;
+  int *cl, *set;
+};
+
+// 1/2 x'Quu x + Qu'x: lane partials over rows, added in lane order (every lane returns the same value)
+FB_WARPFN double boxqp_value(const LqrQp& q, const double* x) {
+  LREG(double, part);
+  WPAR_BEGIN
+    double a = 0.0;
+    for (int i = lane; i < q.nu; i += FB_NY) {
+      const double* h = q.Quu + (size_t)i * q.ncol;
+      double v = 0.0;
+      for (int c = 0; c < q.nu; c++) v = fma(h[c], x[c], v);
+      a = fma(x[i], fma(0.5, v, q.Qu[(size_t)i * q.ncol]), a);
+    }
+    L(part) = a;
+  WPAR_END
+  double f = 0.0;
+  WPAR_BEGIN
+    double sum = 0.0;
+    for (int y = 0; y < FB_NY; y++) sum += SHF(part, y);
+    f = sum;
+  WPAR_END
+  return f;
+}
+
+// g = Qu + Quu x and the clamped set at x (into cl) -> the number of free controls; *changed: the set differs from the factored one;
+// *gsq: |g_free|^2
+FB_WARPFN int boxqp_set(const LqrQp& q, bool* changed, double* gsq) {
+  LREG(int, nf); LREG(int, ch); LREG(double, gs);
+  WPAR_BEGIN
+    int a = 0, b = 0;
+    double s = 0.0;
+    for (int i = lane; i < q.nu; i += FB_NY) {
+      const double* h = q.Quu + (size_t)i * q.ncol;
+      double v = q.Qu[(size_t)i * q.ncol];
+      for (int c = 0; c < q.nu; c++) v = fma(h[c], q.x[c], v);
+      q.g[i] = v;
+      const double xi = q.x[i];
+      const int c = xi == q.lo[i] && v > 0.0 ? -1 : xi == q.hi[i] && v < 0.0 ? 1 : 0;
+      q.cl[i] = c;
+      b |= (c != 0) != (q.set[i] != 0);
+      if (c == 0) { a++; s = fma(v, v, s); }
+    }
+    L(nf) = a; L(ch) = b; L(gs) = s;
+  WPAR_END
+  int n = 0, d = 0;
+  double s = 0.0;
+  WPAR_BEGIN
+    int a = 0, b = 0;
+    double t = 0.0;
+    for (int y = 0; y < FB_NY; y++) { a += SHF(nf, y); b |= SHF(ch, y); t += SHF(gs, y); }
+    n = a; d = b; s = t;
+  WPAR_END
+  *changed = d != 0; *gsq = s;
+  return n;
+}
+
+// C C' = the free block of Quu (klqr_chol's column order and arithmetic; identity rows and columns on clamped controls), and the set it
+// was factored for -> false on a pivot that is not positive and finite
+FB_WARPFN bool boxqp_factor(const LqrQp& q) {
+  const int nu = q.nu;
+  double* C = q.C;
+  for (int j = 0; j < nu; j++) {
+    const bool cj = q.cl[j] != 0;
+    WPAR_BEGIN
+      if (lane == 0) {
+        double d = 1.0;
+        if (!cj) {
+          d = q.Quu[(size_t)j * q.ncol + j];
+          for (int c = 0; c < j; c++) d = fma(-C[j * nu + c], C[j * nu + c], d);
+          d = d > 0.0 && d < HUGE_VAL ? sqrt(d) : 0.0;
+        }
+        C[j * nu + j] = d;
+      }
+    WPAR_END
+    const double cjj = C[j * nu + j];
+    if (!(cjj > 0.0)) return false;
+    WPAR_BEGIN
+      for (int i = j + 1 + lane; i < nu; i += FB_NY) {
+        double v = 0.0;
+        if (!cj && q.cl[i] == 0) {
+          v = q.Quu[(size_t)i * q.ncol + j];
+          for (int c = 0; c < j; c++) v = fma(-C[i * nu + c], C[j * nu + c], v);
+          v = v / cjj;
+        }
+        C[i * nu + j] = v;
+      }
+    WPAR_END
+  }
+  WPAR_BEGIN
+    for (int i = lane; i < nu; i += FB_NY) q.set[i] = q.cl[i] != 0;
+  WPAR_END
+  return true;
+}
+
+// problem l's box QP at step p.t: k_t into the workspace's x, C, the clamped set and the QP record; a failed factor sets status = t + 1
+FB_WARPFN void klqr_boxqp(const DevLqr& p, const DevLqrBox& b, int l) {
+  if (p.status[l]) return;
+  const int nx = p.nx, nu = p.nu, ncol = nx + nu + 1;
+  const size_t lt = (size_t)l * p.T + p.t, ln = (size_t)l * nu;
+  const double* Hu = p.H + (size_t)l * (nx + nu) * ncol + (size_t)nx * ncol;     // the rows of (Qux | Quu | Qu)
+  const LqrQp q = {nu, ncol, Hu + nx, Hu + nx + nu, b.lower + lt * nu, b.upper + lt * nu, b.x + ln, b.dx + ln, b.g + ln, b.xt + ln,
+                   p.C + ln * nu, b.clamped + lt * nu, b.set + ln};
+  WPAR_BEGIN
+    for (int i = lane; i < nu; i += FB_NY) { const double v = 0.0 < q.lo[i] ? q.lo[i] : 0.0; q.x[i] = v > q.hi[i] ? q.hi[i] : v; }
+  WPAR_END
+  double f = boxqp_value(q, q.x);
+  int steps = 0, reason = 1;
+  bool factored = false, changed;
+  double gsq;
+  LREG(double, sd);
+  for (int it = 0; it < BOXQP_MAX_ITER; it++) {
+    if (boxqp_set(q, &changed, &gsq) == 0) { reason = 6; break; }
+    if (!factored || changed) {
+      if (!boxqp_factor(q)) { reason = -1; break; }
+      factored = true;
+    }
+    if (sqrt(gsq) < BOXQP_MIN_GRAD) { reason = 5; break; }
+    // the Newton direction on the free controls, dx_f = -Quu_ff^-1 g_f (dx_c = 0), and dx'g
+    WPAR_BEGIN
+      if (lane == 0) {
+        const double* C = q.C;
+        for (int u = 0; u < nu; u++) {
+          double v = q.cl[u] ? 0.0 : -q.g[u];
+          for (int c = 0; c < u; c++) v = fma(-C[u * nu + c], q.dx[c], v);
+          q.dx[u] = v / C[u * nu + u];
+        }
+        double s = 0.0;
+        for (int u = nu - 1; u >= 0; u--) {
+          double v = q.dx[u];
+          for (int c = u + 1; c < nu; c++) v = fma(-C[c * nu + u], q.dx[c], v);
+          q.dx[u] = v / C[u * nu + u];
+        }
+        for (int u = 0; u < nu; u++) s = fma(q.dx[u], q.g[u], s);
+        L(sd) = s;
+      }
+    WPAR_END
+    double sdotg = 0.0;
+    WPAR_BEGIN sdotg = SHF(sd, 0); WPAR_END
+    if (!(sdotg < 0.0)) { reason = 0; break; }
+    // the projected Armijo search
+    double step = 1.0, ft = 0.0;
+    bool found = false;
+    for (;;) {
+      WPAR_BEGIN
+        for (int i = lane; i < nu; i += FB_NY) {
+          const double v = fma(step, q.dx[i], q.x[i]);
+          q.xt[i] = v < q.lo[i] ? q.lo[i] : v > q.hi[i] ? q.hi[i] : v;
+        }
+      WPAR_END
+      ft = boxqp_value(q, q.xt);
+      if ((ft - f) / (step * sdotg) >= BOXQP_ARMIJO) { found = true; break; }
+      step *= BOXQP_STEP_DEC;
+      if (step < BOXQP_MIN_STEP) break;
+    }
+    if (!found) { reason = 2; break; }
+    WPAR_BEGIN
+      for (int i = lane; i < nu; i += FB_NY) q.x[i] = q.xt[i];
+    WPAR_END
+    const double f0 = f;
+    f = ft;
+    steps++;
+    if (f0 - f < BOXQP_MIN_REL * fabs(f0)) { reason = 4; break; }
+  }
+  // the set at the final x, with the factor of its free block
+  if (reason != -1) {
+    boxqp_set(q, &changed, &gsq);
+    if ((!factored || changed) && !boxqp_factor(q)) reason = -1;
+  }
+  WPAR_BEGIN
+    if (lane == 0) {
+      b.qp[2 * lt] = steps; b.qp[2 * lt + 1] = reason;
+      if (reason == -1) p.status[l] = p.t + 1;
+    }
+  WPAR_END
+}
+
+// klqr_solve on the free block: lane j of a block of 32 columns of (Qux | Qu); the right-hand side is 0 on clamped rows, so with the
+// masked factor those rows of K are 0; the k column is the QP's x; G_j = Quu X_j + b_j with the full Quu
+FB_WARPFN void klqr_solve_box(const DevLqr& p, const DevLqrBox& b, int w) {
+  const int nx = p.nx, nu = p.nu, nz = nx + nu, ncol = nz + 1, ncx = nx + 1, ncb = (ncx + 31) / 32;
+  const int l = w / ncb, j0 = (w % ncb) * 32;
+  if (p.status[l]) return;
+  const size_t lt = (size_t)l * p.T + p.t;
+  const double* H = p.H + (size_t)l * nz * ncol;
+  const double* C = p.C + (size_t)l * nu * nu;
+  const int* cl = b.clamped + lt * nu;
+  double* X = p.X + (size_t)l * nu * ncx;
+  double* G = p.G + (size_t)l * nu * ncx;
+  WPAR_BEGIN
+    const int j = j0 + lane;
+    if (j < ncx) {
+      const int jh = j < nx ? j : nz;
+      double* x = X + j;
+      if (j < nx) {
+        for (int u = 0; u < nu; u++) {
+          double v = cl[u] ? 0.0 : H[(size_t)(nx + u) * ncol + jh];
+          for (int c = 0; c < u; c++) v = fma(-C[u * nu + c], x[(size_t)c * ncx], v);
+          x[(size_t)u * ncx] = v / C[u * nu + u];
+        }
+        for (int u = nu - 1; u >= 0; u--) {
+          double v = x[(size_t)u * ncx];
+          for (int c = u + 1; c < nu; c++) v = fma(-C[c * nu + u], x[(size_t)c * ncx], v);
+          x[(size_t)u * ncx] = v / C[u * nu + u];
+        }
+      }
+      for (int u = 0; u < nu; u++) {
+        const double v = j == nx ? b.x[(size_t)l * nu + u] : cl[u] ? 0.0 : -x[(size_t)u * ncx];
+        x[(size_t)u * ncx] = v;
+        if (j < nx) p.K[(lt * nu + u) * nx + j] = v; else p.k[lt * nu + u] = v;
+      }
+      for (int u = 0; u < nu; u++) {
+        double g = H[(size_t)(nx + u) * ncol + jh];
+        const double* quu = H + (size_t)(nx + u) * ncol + nx;
+        for (int c = 0; c < nu; c++) g = fma(quu[c], x[(size_t)c * ncx], g);
+        G[(size_t)u * ncx + j] = g;
+      }
+    }
+  WPAR_END
+}

@@ -94,6 +94,9 @@ struct FbSim {
   // the iLQR backward pass (fb_lqr; fb_lqr.h): inputs and outputs of L (T + 1) problem steps and the workspace of L problems, grown on
   // demand; problems and steps of the last call
   DevLqr lqr = {}; Pool lqr_pool, lqr_ws_pool; int lqr_done = 0;
+  // its box-constrained form (fb_lqr_box): bounds and QP records of L T problem steps, the QP workspace of L problems; lqr_box: the last
+  // pass had bounds
+  DevLqrBox lqr_b = {}; Pool lqr_box_pool, lqr_qp_pool; bool lqr_box = false;
   // sampling-based MPC (fb_plan_program / fb_plan; fb_plan.h): the program (plan.K > 0: set) and its weights; the buffers, grown on demand
   // with L K T (the samples), L K (their costs and weights), L (T + 1) (mean, xref, uref and the per-problem words) and L n_iter (the
   // record); the rollout parameter of the samples; problems of the last call
@@ -2682,30 +2685,42 @@ template <int KIND> struct LqrWarp {
     else if (KIND == 3) klqr_chol(p, w); else if (KIND == 4) klqr_solve(p, w); else klqr_p(p, w);
   }
 };
+template <int KIND> struct LqrBoxWarp {
+  DevLqr p; DevLqrBox b;
+  FB_DEVM void operator()(unsigned char*, int w) const { if (KIND == 0) klqr_boxqp(p, b, w); else klqr_solve_box(p, b, w); }
+};
 
-extern "C" {
-
-int fb_lqr(FbHandle s, int L, int T, const float* A, const float* B, const double* q, const double* r, const double* Q, const double* R,
-           const double* Qf, const double* mu, int is_device) {
-  if (!s) return -1;
-  const char* who = "fb_lqr";
+// fb_lqr, and fb_lqr_box with bounds (lower and upper non-NULL)
+static int lqr_pass(FbSim* s, const char* who, int L, int T, const float* A, const float* B, const double* q, const double* r,
+                    const double* Q, const double* R, const double* Qf, const double* mu, const double* lower, const double* upper,
+                    int is_device) {
   const DevModel& m = s->m;
   const int nx = 2 * m.nv + m.na, nu = m.nu, nz = nx + nu;
-  if (L < 1 || T < 1) { s->err = "fb_lqr: L >= 1 problems of T >= 1 steps"; return -1; }
-  if (!A || !B || !q || !r || !Q || !R || !Qf || !mu) { s->err = "fb_lqr: A, B, q, r, Q, R, Qf and mu must not be NULL"; return -1; }
-  if (nu < 1) { s->err = "fb_lqr: the model has no actuators"; return -1; }
+  const std::string w = who;
+  const bool box = lower != nullptr;
+  if (L < 1 || T < 1) { s->err = w + ": L >= 1 problems of T >= 1 steps"; return -1; }
+  if (!A || !B || !q || !r || !Q || !R || !Qf || !mu) { s->err = w + ": A, B, q, r, Q, R, Qf and mu must not be NULL"; return -1; }
+  if (nu < 1) { s->err = w + ": the model has no actuators"; return -1; }
   if ((size_t)nz * (nz + 1) >= ((size_t)1 << 31)) {
-    s->err = "fb_lqr: nx + nu = " + std::to_string(nz) + " is too large for the 32-bit offsets inside a problem's workspace"; return -1; }
+    s->err = w + ": nx + nu = " + std::to_string(nz) + " is too large for the 32-bit offsets inside a problem's workspace"; return -1; }
   const size_t lt = (size_t)L * T, l1 = (size_t)L * (T + 1);
   if (!is_device) {
     const char* name[8] = {"A", "B", "q", "r", "Q", "R", "Qf", "mu"};
     const bool ok[8] = {all_finite(A, lt * nx * nx), all_finite(B, lt * nx * nu), all_finite(q, l1 * nx), all_finite(r, lt * nu),
                         all_finite(Q, (size_t)nx), all_finite(R, (size_t)nu), all_finite(Qf, (size_t)nx), all_finite(mu, (size_t)L)};
-    for (int i = 0; i < 8; i++) if (!ok[i]) { s->err = std::string("fb_lqr: non-finite ") + name[i]; return -1; }
+    for (int i = 0; i < 8; i++) if (!ok[i]) { s->err = w + ": non-finite " + name[i]; return -1; }
+    for (size_t i = 0; box && i < lt * nu; i++) {
+      const char* bad = std::isnan(lower[i]) || std::isnan(upper[i]) ? "a NaN bound" : lower[i] > upper[i] ? "lower > upper"
+                        : lower[i] == HUGE_VAL || upper[i] == -HUGE_VAL ? "a bound that excludes every finite du" : nullptr;
+      if (bad) {
+        s->err = w + ": " + bad + " at [" + std::to_string(i / nu / T) + "][" + std::to_string(i / nu % T) + "][" + std::to_string(i % nu) + "]";
+        return -1; }
+    }
   }
   dev_select(s);
   s->lqr_done = 0;
   DevLqr& p = s->lqr;
+  DevLqrBox& b = s->lqr_b;
   // per problem step (L (T + 1) rows, the last T + 1st unused by A, B, r, K, k): the inputs A, B, q, r and the outputs K, k
   if (int rc = grow(s, who, s->lqr_pool, l1, 4 * ((size_t)nx * nx + (size_t)nx * nu) + 8 * ((size_t)nx + nu + (size_t)nu * nx + nu),
                     "inputs and gains", "L (T + 1)", [&](size_t n) {
@@ -2724,19 +2739,57 @@ int fb_lqr(FbHandle s, int L, int T, const float* A, const float* B, const doubl
       copy_async(s, (void*)p.q, q, 8 * l1 * nx) != 0 || copy_async(s, (void*)p.r, r, 8 * lt * nu) != 0 ||
       copy_async(s, (void*)p.Q, Q, 8 * (size_t)nx) != 0 || copy_async(s, (void*)p.R, R, 8 * (size_t)nu) != 0 ||
       copy_async(s, (void*)p.Qf, Qf, 8 * (size_t)nx) != 0 || copy_async(s, (void*)p.mu, mu, 8 * (size_t)L) != 0) return -2;
+  if (box) {
+    // per problem step: the bounds and the QP's outputs; per problem: the QP's workspace
+    if (int rc = grow(s, who, s->lqr_box_pool, lt, 8 * 2 * (size_t)nu + 4 * ((size_t)nu + 2), "bounds and QP records", "L T", [&](size_t n) {
+          b.lower = dalloc<double>(s, n * nu); b.upper = dalloc<double>(s, n * nu); b.clamped = dalloc<int>(s, n * nu); b.qp = dalloc<int>(s, 2 * n); }))
+      return rc;
+    if (int rc = grow(s, who, s->lqr_qp_pool, (size_t)L, 8 * 4 * (size_t)nu + 4 * (size_t)nu, "QP workspace", "L", [&](size_t n) {
+          b.x = dalloc<double>(s, n * nu); b.dx = dalloc<double>(s, n * nu); b.g = dalloc<double>(s, n * nu); b.xt = dalloc<double>(s, n * nu);
+          b.set = dalloc<int>(s, n * nu); }))
+      return rc;
+    if (copy_async(s, (void*)b.lower, lower, 8 * lt * nu) != 0 || copy_async(s, (void*)b.upper, upper, 8 * lt * nu) != 0) return -2;
+  }
   p.L = L; p.T = T; p.nx = nx; p.nu = nu;
   warp_launch(s, "lqr_init", L, 0, LqrWarp<0>{p});
   for (int t = T - 1; t >= 0; t--) {           // no host synchronisation inside the pass
     p.t = t;
     warp_launch(s, "lqr_w", L * lqr_tiles(nx, nz + 1), 0, LqrWarp<1>{p});
     warp_launch(s, "lqr_h", L * lqr_tiles(nz, nz + 1), 0, LqrWarp<2>{p});
-    warp_launch(s, "lqr_chol", L, 0, LqrWarp<3>{p});
-    warp_launch(s, "lqr_solve", L * ((nx + 1 + 31) / 32), 0, LqrWarp<4>{p});
+    if (box) {
+      warp_launch(s, "lqr_boxqp", L, 0, LqrBoxWarp<0>{p, b});
+      warp_launch(s, "lqr_solve_box", L * ((nx + 1 + 31) / 32), 0, LqrBoxWarp<1>{p, b});
+    } else {
+      warp_launch(s, "lqr_chol", L, 0, LqrWarp<3>{p});
+      warp_launch(s, "lqr_solve", L * ((nx + 1 + 31) / 32), 0, LqrWarp<4>{p});
+    }
     warp_launch(s, "lqr_p", L * lqr_tiles(nx, nx + 1), 0, LqrWarp<5>{p});
   }
   if (launch_check(s, who) != 0) return -2;
-  s->lqr_done = L;
+  s->lqr_done = L; s->lqr_box = box;
   return sync_stream(s);                       // host inputs may be reused once the call returns
+}
+
+extern "C" {
+
+int fb_lqr(FbHandle s, int L, int T, const float* A, const float* B, const double* q, const double* r, const double* Q, const double* R,
+           const double* Qf, const double* mu, int is_device) {
+  return s ? lqr_pass(s, "fb_lqr", L, T, A, B, q, r, Q, R, Qf, mu, nullptr, nullptr, is_device) : -1;
+}
+
+int fb_lqr_box(FbHandle s, int L, int T, const float* A, const float* B, const double* q, const double* r, const double* Q, const double* R,
+               const double* Qf, const double* mu, const double* lower, const double* upper, int is_device) {
+  if (!s) return -1;
+  if (!lower || !upper) { s->err = "fb_lqr_box: lower and upper must not be NULL"; return -1; }
+  return lqr_pass(s, "fb_lqr_box", L, T, A, B, q, r, Q, R, Qf, mu, lower, upper, is_device);
+}
+
+int fb_lqr_box_read(FbHandle s, int32_t* clamped, int32_t* qp, int is_device) {
+  if (!s) return -1;
+  if (s->lqr_done < 1) { s->err = "fb_lqr_box_read: no backward pass to read (fb_lqr_box)"; return -1; }
+  if (!s->lqr_box) { s->err = "fb_lqr_box_read: the last backward pass was fb_lqr, without bounds"; return -1; }
+  const size_t lt = (size_t)s->lqr.L * s->lqr.T;
+  return read_out(s, {{clamped, s->lqr_b.clamped, 0, 4 * lt * s->lqr.nu, 1}, {qp, s->lqr_b.qp, 0, 8 * lt, 1}});
 }
 
 int fb_lqr_read(FbHandle s, double* K, double* k, double* dV, int32_t* status, int is_device) {

@@ -534,21 +534,37 @@ class BatchedStepper:
         return tuple(out)
 
     # ---- the iLQR backward pass (fb_lqr*; flybody_b200.trajopt is the front end)
-    def lqr(self, A, B, q, r, Q, R, Qf, mu):
+    def lqr(self, A, B, q, r, Q, R, Qf, mu, lower=None, upper=None):
         """the Riccati backward pass of L problems: A [L, T, nx, nx], B [L, T, nx, nu] (fp32), q [L, T + 1, nx], r [L, T, nu], the
-        diagonal weights Q [nx], R [nu], Qf [nx] and mu [L] (fp64), host arrays (see the header); read with lqr_read()"""
+        diagonal weights Q [nx], R [nu], Qf [nx] and mu [L] (fp64), host arrays (see the header); read with lqr_read().  With bounds
+        lower and / or upper [L, T, nu] (fp64, the other one -inf / +inf when None) on du = u - ubar it is the box-DDP pass
+        (fb_lqr_box), whose clamped sets and QP records lqr_box_read() returns."""
         m = self.model
         nx, nu = 2 * m.nv + m.na, m.nu
         L, T = np.shape(A)[:2]
         want = [('A', (L, T, nx, nx), np.float32), ('B', (L, T, nx, nu), np.float32), ('q', (L, T + 1, nx), np.float64),
                 ('r', (L, T, nu), np.float64), ('Q', (nx,), np.float64), ('R', (nu,), np.float64), ('Qf', (nx,), np.float64),
                 ('mu', (L,), np.float64)]
-        keep = [np.ascontiguousarray(x, dt) for x, (_, _, dt) in zip((A, B, q, r, Q, R, Qf, mu), want)]
+        args = [A, B, q, r, Q, R, Qf, mu]
+        box = lower is not None or upper is not None
+        if box:
+            want += [('lower', (L, T, nu), np.float64), ('upper', (L, T, nu), np.float64)]
+            args += [np.full((L, T, nu), -np.inf) if lower is None else lower, np.full((L, T, nu), np.inf) if upper is None else upper]
+        keep = [np.ascontiguousarray(x, dt) for x, (_, _, dt) in zip(args, want)]
         for x, (name, shape, _) in zip(keep, want):
             if x.shape != shape:
                 raise ValueError(f'{name} {x.shape} against {shape}')
-        self._check(self._lib.fb_lqr(self._h, int(L), int(T), *[x.ctypes.data for x in keep], 0), 'fb_lqr')
+        fn = 'fb_lqr_box' if box else 'fb_lqr'
+        self._check(getattr(self._lib, fn)(self._h, int(L), int(T), *[x.ctypes.data for x in keep], 0), fn)
         self._lqr = (int(L), int(T))
+
+    def lqr_box_read(self):
+        """-> (clamped [L, T, nu] (-1 at lower, +1 at upper, 0 free), qp [L, T, 2] (accepted Newton steps, stop reason)) int32 of the
+        last lqr with bounds"""
+        L, T = getattr(self, '_lqr', (0, 0))
+        out = [np.zeros((L, T, self.model.nu), np.int32), np.zeros((L, T, 2), np.int32)]
+        self._check(self._lib.fb_lqr_box_read(self._h, *[x.ctypes.data for x in out], 0), 'fb_lqr_box_read')
+        return tuple(out)
 
     def lqr_read(self):
         """-> (K [L, T, nu, nx], k [L, T, nu], dV [L, 2] fp64, status [L] int32) of the last lqr"""

@@ -13,7 +13,13 @@ rollouts, cost and update) on the device in one `fb_plan` call; `mpc` runs it in
 The cost is sum_t |x_t - xref_t|^2_Q / 2 + |u_t - uref_t|^2_R / 2 + |x_T - xref_T|^2_Qf / 2 with diagonal weights, the state difference
 in transition_fd's tangent (mj_differentiatePos for qpos), evaluated in fp64 on the host.  The nominal ctrl is the recorded ctrl clamped
 to actuator_ctrlrange where the actuator is ctrl-limited (what the step applied), so an open-loop `rollout.rollout` of the returned ctrl
-reproduces the returned trajectory bit for bit.  There are no control bounds inside the backward pass.
+reproduces the returned trajectory bit for bit.
+
+The actuators' ctrl ranges can enter the backward pass too: `ilqr(box=True)` runs control-limited DDP (Tassa, Mansard & Todorov 2014,
+`fb_lqr_box`).  At each step k solves the box-constrained QP min 1/2 k'Quu k + Qu'k over lo - ubar <= k <= hi - ubar on the ctrl-limited
+actuators by projected Newton, and K has zero rows on the controls clamped at a bound, so the expected decrease dV describes the step
+the clamping plant takes and the returned TVLQR gains do not push on saturated controls.  `lqr_backward(lower=, upper=)` is that pass
+alone.
 
 As in `derivatives` and `rollout`, every Jacobian and every rollout starts from a cold solver warm start (its state is written and
 `forward` run), and no heightfield program is set up, so the vision model runs without terrain contacts.  There is no CPU fallback:
@@ -30,25 +36,34 @@ from .inverse_kinematics import _differentiate_pos
 ENVS = 4096          # envs of the handle a solve runs on (rounded down to whole Jacobian problems)
 
 LQR = namedtuple('LQR', ['K', 'k', 'dV', 'status'])
+BoxLQR = namedtuple('BoxLQR', ['K', 'k', 'dV', 'status', 'clamped', 'qp'])
 ILQR = namedtuple('ILQR', ['qpos', 'qvel', 'act', 'ctrl', 'K', 'cost', 'iterations', 'converged'])
+BoxILQR = namedtuple('BoxILQR', ILQR._fields + ('clamped',))
 
 # regularisation schedule (Tassa et al. 2012, section II-F): mu is added to Quu
 MU_MIN, MU_MAX, MU_FACTOR = 1e-6, 1e10, 2.0
 ACCEPT = 1e-4        # a step is accepted when actual / expected decrease exceeds this
 
 
-def lqr_backward(model, A, B, q, r, Q, R, Qf, mu=0.0, device=0, lib_path=None):
+def lqr_backward(model, A, B, q, r, Q, R, Qf, mu=0.0, lower=None, upper=None, device=0, lib_path=None):
     """The iLQR backward pass of L problems on the device (`fb_lqr`, fp64): A [L, T, nx, nx] and B [L, T, nx, nu] (as transition_fd
     returns them, used in fp32), gradients q [L, T + 1, nx] and r [L, T, nu], diagonal weights Q [nx], R [nu], Qf [nx] and mu (scalar or
     [L]) added to Quu.  With q = r = 0, K is the TVLQR law of the weights.
 
     Returns LQR(K [L, T, nu, nx], k [L, T, nu], dV [L, 2], status [L]): dV = (sum k'Qu, sum k'Quu k / 2), the expected change of the
-    cost for a step alpha being alpha dV1 + alpha^2 dV2; status t + 1 when Quu is not positive definite at step t (0: solved)."""
+    cost for a step alpha being alpha dV1 + alpha^2 dV2; status t + 1 when Quu is not positive definite at step t (0: solved).
+
+    With bounds lower and / or upper [L, T, nu] on du = u - ubar (+-inf allowed; the other one unbounded when None) it is the
+    control-limited pass (`fb_lqr_box`): k_t minimises the step's QP inside the bounds, K_t has zero rows on the controls clamped at
+    k_t, and status is t + 1 when the free block of Quu is not positive definite.  Returns BoxLQR(K, k, dV, status, clamped [L, T, nu]
+    (-1 at lower, +1 at upper, 0 free), qp [L, T, 2] (the QP's accepted Newton steps and stop reason, see the header))."""
     L = np.shape(A)[0]
     sim = st.BatchedStepper(model, 1, device=device, lib_path=lib_path)
     try:
-        sim.lqr(A, B, q, r, Q, R, Qf, np.broadcast_to(np.asarray(mu, np.float64), (L,)))
-        return LQR(*sim.lqr_read())
+        sim.lqr(A, B, q, r, Q, R, Qf, np.broadcast_to(np.asarray(mu, np.float64), (L,)), lower, upper)
+        if lower is None and upper is None:
+            return LQR(*sim.lqr_read())
+        return BoxLQR(*sim.lqr_read(), *sim.lqr_box_read())
     finally:
         sim.close()
 
@@ -134,17 +149,21 @@ def _check(name, x, shape, nonneg=False):
 
 
 def ilqr(model, qpos, qvel, ctrl, x_ref, Q, R, Qf=None, act=None, u_ref=None, n_substeps=1, max_iter=50, tol=1e-6,
-         alphas=2.0 ** -np.arange(8), eps=1e-2, centered=True, device=0, lib_path=None, timings=None):
+         alphas=2.0 ** -np.arange(8), eps=1e-2, centered=True, box=False, device=0, lib_path=None, timings=None):
     """iLQR for L problems: initial states qpos [L, nq], qvel [L, nv], act [L, na] (zeros when None), initial controls ctrl [L, T, nu],
     reference states x_ref [L, T + 1, nq + nv + na] and controls u_ref [L, T, nu] (zeros when None), diagonal weights Q [nx], R [nu],
     Qf [nx] (Q when None), nx = 2 nv + na; each control step is n_substeps substeps with ctrl held.  eps and centered are
     transition_fd's.  A problem stops when an accepted step lowers its cost by less than tol (relative) or the expected decrease of a
     full step is below tol (converged), after max_iter accepted steps, or when its regularisation passes MU_MAX.  timings: a dict that
     gets the seconds spent in 'fd' (Jacobians), 'backward', 'forward' (rollouts) and 'host' (row writes, reads and the fp64 cost).
+    box: every backward pass is the control-limited one (`lqr_backward` with bounds): du_t is bounded by lo - ubar_t and hi - ubar_t on
+    the ctrl-limited actuators (fp64 from the fp32 applied ubar, so lower <= 0 <= upper exactly) and unbounded on the others.  The
+    forward pass, the acceptance test and the regularisation schedule are unchanged.
 
     Returns ILQR(qpos, qvel, act [L, T + 1, .], ctrl [L, T, nu], K [L, T, nu, nx], cost [L, iters + 1], iterations [L], converged [L]):
     the trajectory as the device ran it (fp64 arrays of fp32 values), the TVLQR gains of a backward pass at it, the cost before the first
-    step and after each accepted one (nan after the problem stopped), and the accepted steps."""
+    step and after each accepted one (nan after the problem stopped), and the accepted steps.  With box, BoxILQR: the same fields and
+    clamped [L, T, nu], the clamped sets of the final gains' pass (their rows of K are zero)."""
     m = model
     nq, nv, na, nu = m.nq, m.nv, m.na, m.nu
     nx, nr = 2 * nv + na, nq + nv + na
@@ -209,10 +228,11 @@ def ilqr(model, qpos, qvel, ctrl, x_ref, Q, R, Qf=None, act=None, u_ref=None, n_
             dx = np.stack([tangent(m, xbar[l], x_ref[l]) for l in idx])
             q = np.concatenate([dx[:, :T] * Q, dx[:, T:] * Qf], 1)
             r = (ubar[idx] - u_ref[idx]) * R
+            bounds = (np.where(limited, lo - ubar[idx], -np.inf), np.where(limited, hi - ubar[idx], np.inf)) if box else ()
             clock.lap('host')
-            sim.lqr(A[idx], B[idx], q, r, Q, R, Qf, mu[idx])
+            sim.lqr(A[idx], B[idx], q, r, Q, R, Qf, mu[idx], *bounds)
             clock.lap('backward')
-            return sim.lqr_read()
+            return sim.lqr_read() + (sim.lqr_box_read()[:1] if box else ())
 
         def raise_mu(l):
             delta[l] = max(MU_FACTOR, delta[l] * MU_FACTOR)
@@ -223,7 +243,7 @@ def ilqr(model, qpos, qvel, ctrl, x_ref, Q, R, Qf=None, act=None, u_ref=None, n_
             idx = np.flatnonzero(active)
             if stale[idx].any():
                 jacobians(idx[stale[idx]])
-            K, k, dV, status = backward(idx)
+            K, k, dV, status = backward(idx)[:4]
             go = []
             for i, l in enumerate(idx):
                 if status[i]:
@@ -273,17 +293,21 @@ def ilqr(model, qpos, qvel, ctrl, x_ref, Q, R, Qf=None, act=None, u_ref=None, n_
         if stale.any():
             jacobians(idx[stale])
         K = np.zeros((L, T, nu, nx))
+        clamped = np.zeros((L, T, nu), np.int32)
         todo = idx
         while len(todo):
-            Kt, _, _, status = backward(todo)
-            done = status == 0
-            K[todo[done]] = Kt[done]
+            out = backward(todo)
+            done = out[3] == 0
+            K[todo[done]] = out[0][done]
+            if box:
+                clamped[todo[done]] = out[4][done]
             todo = np.array([l for l in todo[~done] if raise_mu(l)], np.int64)
         clock.lap('host')
     finally:
         sim.close()
     n = int(iters.max()) + 1
-    return ILQR(xbar[..., :nq], xbar[..., nq:nq + nv], xbar[..., nq + nv:], ubar, K, hist[:, :n], iters, converged)
+    res = ILQR(xbar[..., :nq], xbar[..., nq:nq + nv], xbar[..., nq + nv:], ubar, K, hist[:, :n], iters, converged)
+    return BoxILQR(*res, clamped) if box else res
 
 
 SamplePlan = namedtuple('SamplePlan', ['qpos', 'qvel', 'act', 'ctrl', 'cost', 'status'])

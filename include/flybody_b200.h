@@ -724,6 +724,28 @@ int fb_rollout_sensor_read(FbHandle h, float* sensordata, float* sensor_mean, in
 int fb_lqr(FbHandle h, int L, int T, const float* A, const float* B, const double* q, const double* r, const double* Q, const double* R,
            const double* Qf, const double* mu, int is_device);
 int fb_lqr_read(FbHandle h, double* K, double* k, double* dV, int32_t* status, int is_device);
+/* Control-limited DDP (box-DDP; Tassa, Mansard & Todorov 2014): fb_lqr with bounds lower [L][T][nu] <= du_t <= upper [L][T][nu] on the
+ * control change du = u - ubar of every problem step (fp64, +-inf allowed).  At each step k_t solves the box-constrained QP
+ *   min 1/2 x'Quu x + Qu'x  subject to  lower_t <= x <= upper_t
+ * by the projected Newton method of Tassa's boxQP, one warp per problem: from x = clamp(0), at most 100 iterations of
+ *   g = Qu + Quu x; control i is clamped when x_i = lower_i and g_i > 0, or x_i = upper_i and g_i < 0; stop when every control is
+ *   clamped; (re)factor the free block Quu_ff (Cholesky; on the first iteration and whenever the clamped set changed); stop when
+ *   |g_free|_2 < 1e-8; dx_f = -Quu_ff^-1 g_f, dx_c = 0; a projected Armijo search from step 1: accept x_try = clamp(x + step dx) when
+ *   (f(x_try) - f(x)) / (step dx'g) >= 0.1, else step *= 0.6, giving up below 1e-22; stop when the step lowers f by less than 1e-8 |f|.
+ * Then the clamped set is taken again at the final x and its free block refactored if it changed.  K_t = -Quu_ff^-1 Qux_f on the free
+ * rows and exactly 0 on the clamped ones; s, P and dV follow fb_lqr's formulas, which hold for any K and k.  A free block whose pivot is
+ * not positive and finite sets status = t + 1, as fb_lqr's Cholesky.  Launches per step: fb_lqr's with the Cholesky and the solve
+ * replaced by the QP and a masked solve; no host synchronisation inside the pass; fixed-order sums and no atomics, so a problem's bits
+ * depend on neither its index nor L.  A problem's workspace grows by 8 4 nu + 4 nu bytes, a problem step's by 8 2 nu + 4 (nu + 2)
+ * bytes (bounds, clamped set, QP record).  Errors: fb_lqr's, NULL bounds, and for host bounds a NaN, lower > upper, lower = +inf or
+ * upper = -inf.  fb_lqr_read reads its K, k, dV and status.
+ * fb_lqr_box_read (synchronises; any pointer may be NULL; is_device: device pointers): clamped [L][T][nu] (-1 at lower, +1 at upper,
+ * 0 free, at the returned k) and qp [L][T][2] (accepted Newton steps, stop reason: -1 a free block that is not positive definite,
+ * 0 no descent direction, 1 100 iterations, 2 the line search gave up, 4 a small improvement, 5 a small free gradient, 6 every control
+ * clamped) (int32); an error before any pass and after a pass of fb_lqr.                                                            */
+int fb_lqr_box(FbHandle h, int L, int T, const float* A, const float* B, const double* q, const double* r, const double* Q,
+               const double* R, const double* Qf, const double* mu, const double* lower, const double* upper, int is_device);
+int fb_lqr_box_read(FbHandle h, int32_t* clamped, int32_t* qp, int is_device);
 /* Sampling-based MPC: MPPI (Williams et al. 2017, the information-theoretic update without the control cross term, R pricing the
  * controls) and predictive sampling (Howell et al. 2022, MuJoCo MPC), batched over L tracking problems of K = n_samples samples each
  * (nx = 2 nv + na, nr = nq + nv + na).  Problem l starts from state-bank row slots[l] with the nominal control sequence mean[l] [T][nu].
